@@ -1,7 +1,8 @@
 """bench.py -- images/sec of end-to-end ``Pipeline.recognize`` (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W                # this repository (B200 kernels)
+    python bench.py --gpus N --steps K --warmup W                # this repository (H100 kernels)
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU path
+    python bench.py ... --dump-outputs DIR                           # also write the last timed step's results
 
 One step = one ``recognize`` pass over a batch of 32 synthetic pages (768x768 RGB, 32 rendered
 words each, ``Pipeline(scale=2)`` -> 32x1536x1536 detector input, BASELINE.json configs[3]); with
@@ -13,8 +14,14 @@ Timed region: K steps bracketed by barrier + cuda synchronize, CUDA events, max 
 ``value``  : sources resident in HBM when the step starts (resize/pad ... CTC decode + result D2H).
 ``e2e``    : the same through the public API with HOST numpy images: pinned H2D copy of the step's
              inputs and D2H of the results inside the timed region.
-``roofline``: the dominant kernel (tcgen05 conv) -- algorithmic FLOPs of its launches in one step
-             / their CUDA-event time, against the measured bf16 peak (MEASURED_PEAKS.json).
+``roofline``: the dominant kernel (wgmma conv) -- algorithmic FLOPs of its launches in one step
+             / their CUDA-event time, against the dense fp16 peak (MEASURED_PEAKS.json if present, else
+             the H100 SXM data sheet's 989 TFLOP/s).
+``--dump-outputs DIR``: after the timed steps, what the last step of the device-resident timed leg returned
+             (with N GPUs: every rank's pages, gathered on rank 0 in global order) as DIR/<name>.npy:
+             boxes (words, 4, 2) float32, the words' characters as code points (words, MAX_TEXT) float32
+             padded with -1, and words per page float64.  The inputs are seeded, so two builds can be
+             compared output for output.
 ``cpu_baseline``: the oracle port of the reference path on the host cores, bounded sample.
 """
 import argparse
@@ -48,7 +55,7 @@ def workload_config(n_gpus):
         "detector_input": "1536x1536", "scale": SCALE, "parallelism": f"dp{n_gpus}",
         "weights": "no pretrained files offline: CRAFT seeded synthetic with textlike routing; CRNN = the reference architecture "
                    "trained on rendered Hershey-font words (oracle/train_crnn_full.py) -- the words found are the rendered words",
-        "l2": "per-step activations (>40 GB) exceed the 126 MB L2; no explicit flush needed",
+        "l2": "per-step activations (tens of GB) exceed the 50 MB L2; no explicit flush needed",
     }
 
 
@@ -84,11 +91,11 @@ def measured_peaks():
         with open(path) as f:
             p = json.load(f)
         return float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 1400.0))), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
-    return 1400.0, "fallback (B200_PROFILING.md sustained 1.4 PFLOP/s)"
+    return 989.0, "NVIDIA H100 SXM data sheet, dense fp16 (700 W); not a measured rate"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -199,6 +206,20 @@ def run_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
+def dump_outputs(result, out_dir):
+    """The arrays Pipeline.recognize returned for the step, as float32 / float64 .npy files (a few MB at most)."""
+    os.makedirs(out_dir, exist_ok=True)
+    words = [(text, np.asarray(box, np.float32)) for group in result for text, box in group]
+    boxes = np.stack([b for _, b in words]) if words else np.zeros((0, 4, 2), np.float32)
+    width = max([len(t) for t, _ in words] + [1])
+    text = np.full((len(words), width), -1.0, np.float32)
+    for k, (t, _) in enumerate(words):
+        text[k, :len(t)] = [ord(ch) for ch in t]
+    np.save(os.path.join(out_dir, "boxes.npy"), boxes.astype(np.float32))
+    np.save(os.path.join(out_dir, "text_codepoints.npy"), text)
+    np.save(os.path.join(out_dir, "words_per_page.npy"), np.array([len(g) for g in result], np.float64))
+
+
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -228,7 +249,7 @@ def run_b200(args):
     pages_pinned = torch.from_numpy(pages).pin_memory()
     pages = pages_pinned.numpy()
     max_boxes = 128
-    stats = {"words": 0}
+    stats = {"words": 0, "result": None}
 
     def step(inputs):
         if world == 1:
@@ -240,6 +261,7 @@ def run_b200(args):
             result = D.recognize_sharded(pipe, inputs, max_boxes=max_boxes, presharded=True)
         if result is not None:
             stats["words"] = sum(len(g) for g in result)
+            stats["result"] = result
         return result
 
     def barrier():
@@ -248,9 +270,8 @@ def run_b200(args):
         torch.cuda.synchronize()
 
     # N > 1: the K steps run as a stream, rank 0 decoding step k-1's gathered words while every GPU already works on step k
-    # (distributed.ShardedStream); all K results are produced inside the timed region (the last one by flush()).  Measured on
-    # 2 GPUs (profiles/r2d_bench_2gpu_*.json): 972.9 img/s against 969.2 with the per-step gather + decode
-    # (B2O_BENCH_STREAM=0 selects that).
+    # (distributed.ShardedStream); all K results are produced inside the timed region (the last one by flush()).
+    # B2O_BENCH_STREAM=0 selects the per-step gather + decode instead.
     stream = D.ShardedStream(pipe, max_boxes=max_boxes) if world > 1 and os.environ.get("B2O_BENCH_STREAM", "1") != "0" else None
 
     def timed(inputs, steps):
@@ -263,6 +284,7 @@ def run_b200(args):
             result = stream.flush()
             if result is not None:
                 stats["words"] = sum(len(g) for g in result)
+                stats["result"] = result
         else:
             for _ in range(steps):
                 step(inputs)
@@ -285,7 +307,9 @@ def run_b200(args):
         sampler.start()
     launches0 = det.ctx.launch_count() + rec.ctx.launch_count()
     D.stats["decode_ms"], D.stats["decodes"] = 0.0, 0
+    stats["result"] = None
     ms_dev = timed(pages_dev, args.steps)
+    last_result = stats["result"]                        # the last timed step's results (N GPUs: all ranks' pages, on rank 0)
     per_rank_dev = stats.get("per_rank_ms")
     decode_ms = D.stats["decode_ms"] / max(D.stats["decodes"], 1)
     launches = det.ctx.launch_count() + rec.ctx.launch_count() - launches0
@@ -318,11 +342,6 @@ def run_b200(args):
     peak, peak_src = measured_peaks()
     tc_ms, tc_flop, tc_n = ms_d + ms_r, fl_d + fl_r, n_d + n_r
     achieved = tc_flop / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else 0.0
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        with open(tpath) as f:
-            traffic = json.load(f).get("conv_tc_dram_bytes_per_launch")
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_dev / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -332,15 +351,18 @@ def run_b200(args):
                 "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": int(launches),
         "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": "conv_tc_kernel (tcgen05 implicit-GEMM conv/dense)",
+        "roofline": {"bound": "tensor", "kernel": "conv_tc_kernel (wgmma implicit-GEMM conv/dense)",
                      "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                      "peak_source": peak_src, "launches_per_step": int(tc_n),
                      "flop_per_step": tc_flop, "kernel_ms_per_step": tc_ms,
-                     "kernel_share_of_step": tc_ms / step_ms_plain if step_ms_plain > 0 else None,
-                     "traffic": traffic},
+                     "kernel_share_of_step": tc_ms / step_ms_plain if step_ms_plain > 0 else None},
         "words_per_step": stats["words"],
         "words_read_correctly": {"rank0_pages": PAGES_PER_RANK, "rendered": rendered, "read": hit},
     }
+    if args.dump_outputs:
+        if last_result is None:
+            raise RuntimeError("--dump-outputs: the timed steps returned no result on rank 0")
+        dump_outputs(last_result, args.dump_outputs)
     if hit < 0.9 * rendered:                                # reported, never fatal: the line above is the measurement
         sys.stderr.write(f"bench.py: only {hit} of {rendered} rendered words were read correctly\n")
     if world > 1:
@@ -362,6 +384,8 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results to DIR/<name>.npy (GPU arm, rank 0)")
     args = ap.parse_args()
     sys.exit(run_reference(args) if args.impl == "reference" else run_b200(args))
 

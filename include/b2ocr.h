@@ -1,5 +1,5 @@
 /*
- * b2ocr.h -- C-ABI of the B200-native drop-in for keras_ocr.pipeline.Pipeline.recognize().
+ * b2ocr.h -- C-ABI of the H100-native drop-in for keras_ocr.pipeline.Pipeline.recognize().
  *
  * The reference (faustomorales/keras-ocr @ 9661d6f) is pure Python and has no FFI of its own:
  * its "device boundary" is two keras.Model.predict() calls (detection.py:779, recognition.py:535)
@@ -52,9 +52,9 @@ typedef struct {
   int64_t shape[4];
 } b2o_tensor;
 
-/* Which convolution engine to use: B2O_CONV_AUTO = tcgen05 wherever the shape allows (the product
- * path), B2O_CONV_SIMT = CUDA-core debug engine used to cross-check the tcgen05 kernels.      */
-enum { B2O_CONV_AUTO = 0, B2O_CONV_SIMT = 1, B2O_CONV_TC_GENERIC = 2 /* tcgen05 without halo tiles / fused pool */ };
+/* Which convolution engine to use: B2O_CONV_AUTO = tensor cores (wgmma) wherever the shape allows (the product
+ * path), B2O_CONV_SIMT = CUDA-core debug engine used to cross-check the tensor-core kernels. */
+enum { B2O_CONV_AUTO = 0, B2O_CONV_SIMT = 1, B2O_CONV_TC_GENERIC = 2 /* tensor cores without halo tiles / fused pool */ };
 
 int b2o_version(void);
 int b2o_create(int device, b2o_ctx** out);

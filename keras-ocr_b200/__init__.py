@@ -1,8 +1,8 @@
-"""keras-ocr_b200: a B200-native drop-in for ``keras_ocr.pipeline.Pipeline.recognize``.
+"""keras-ocr_b200: an H100-native drop-in for ``keras_ocr.pipeline.Pipeline.recognize``.
 
 Public surface mirrors the reference (keras_ocr/pipeline.py:7-75, detection.py:661-785,
 recognition.py:353-537): ``Pipeline``, ``Detector``, ``Recognizer``.  Every stage runs as a
-hand-written sm_100a CUDA kernel behind the C-ABI in ``include/b2ocr.h``; there is no CPU
+hand-written sm_90a CUDA kernel behind the C-ABI in ``include/b2ocr.h``; there is no CPU
 fallback -- importing the compute classes without the built library raises.
 """
 __version__ = "0.1.0"

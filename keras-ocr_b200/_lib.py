@@ -1,7 +1,7 @@
 """ctypes binding of ``libb2ocr.so`` (C-ABI in include/b2ocr.h).
 
-There is deliberately no fallback: if the shared library is missing or the device is not a
-B200-class GPU, importing/creating fails loudly.  PyTorch is used by the callers only to own
+There is deliberately no fallback: if the shared library is missing or the device is not an
+H100-class (sm_90) GPU, importing/creating fails loudly.  PyTorch is used by the callers only to own
 device memory and streams; only raw pointers cross this boundary.
 """
 import ctypes
@@ -111,7 +111,7 @@ class Context:
         handle = _vp()
         rc = self.lib.b2o_create(int(device), ctypes.byref(handle))
         if rc != 0 or not handle:
-            raise B2OError(f"b2o_create(device={device}) failed with status {rc}: an sm_100 (B200) GPU is "
+            raise B2OError(f"b2o_create(device={device}) failed with status {rc}: an sm_90 (H100) GPU is "
                            "required and there is no CPU fallback")
         self.handle = handle
         self.device = device

@@ -1,9 +1,9 @@
-"""Build ``libb2ocr.so`` (the C-ABI of include/b2ocr.h) in-tree with nvcc for sm_100a.
+"""Build ``libb2ocr.so`` (the C-ABI of include/b2ocr.h) in-tree with nvcc for sm_90a (H100).
 
     python keras-ocr_b200/build.py [--force]
 
-The shared object lands next to this file so that it travels with the repository snapshot
-to the GPU box; it is git-ignored.  Compilation needs no GPU (nvcc cross-compiles).
+The shared object lands next to this file, so the package imports from the repository tree;
+it is git-ignored.  Compilation needs no GPU (nvcc cross-compiles).
 """
 import concurrent.futures
 import os
@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb2ocr.so")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "boxes.cu", "image.cu", "crnn_tail.cu", "jpeg.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -32,23 +32,6 @@ def _compile(src):
     r = subprocess.run([NVCC] + FLAGS + ["-c", os.path.join(CSRC, src), "-o", obj],
                        capture_output=True, text=True)
     return src, r.returncode, r.stdout + r.stderr
-
-
-def build_debug():
-    """Development build with the MMA-warp wait counters compiled in (-DB2O_TC_DEBUG; scripts/dev_tc_debug.py reads
-    them): ``libb2ocr_dbg.so`` next to the product library, picked up with B2O_LIB=<path>.  Never loaded by default."""
-    out = os.path.join(HERE, "libb2ocr_dbg.so")
-    objs = []
-    for src in SOURCES:
-        obj = os.path.join(CSRC, src.replace(".cu", ".dbg.o"))
-        r = subprocess.run([NVCC] + FLAGS + ["-DB2O_TC_DEBUG", "-c", os.path.join(CSRC, src), "-o", obj], capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(f"nvcc failed on {src}:\n{r.stdout}{r.stderr}")
-        objs.append(obj)
-    r = subprocess.run([NVCC, "-shared", "-o", out] + objs + ["-lcudart", "-ldl"], capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("link failed:\n" + r.stdout + r.stderr)
-    return out
 
 
 def build(force=False, verbose=False):
@@ -73,4 +56,4 @@ def build(force=False, verbose=False):
 
 
 if __name__ == "__main__":
-    print(build_debug() if "--debug-tc" in sys.argv else build(force="--force" in sys.argv, verbose="-v" in sys.argv))
+    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

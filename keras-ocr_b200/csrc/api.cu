@@ -236,21 +236,18 @@ extern "C" int b2o_create(int device, b2o_ctx** out) {
   DeviceGuard guard(device);                  // the caller's current device is restored on return
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return B2O_ERR_CUDA;
-  if (prop.major != 10) {
-    fprintf(stderr, "b2ocr: device %d is sm_%d%d; this library is built for sm_100a only\n", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    fprintf(stderr, "b2ocr: device %d is sm_%d%d; this library is built for sm_90a only\n", device, prop.major, prop.minor);
     return B2O_ERR_CUDA;
   }
   b2o_ctx* ctx = new b2o_ctx();
   ctx->device = device;
   ctx->sm_count = prop.multiProcessorCount;
-  if (const char* e = getenv("B2O_TC_ISSUERS")) ctx->tc_issuers = (atoi(e) == 2) ? 2 : (atoi(e) == 1 ? 1 : 0);
-  if (const char* e = getenv("B2O_TC_BOX16")) { const int v = atoi(e); ctx->tc_box16 = v == 0 ? 0 : (v == 10 ? 10 : 16); ctx->tc_box_forced = v != 0; }
-  if (const char* e = getenv("B2O_TC_BOX_ALL")) ctx->tc_box_all = atoi(e) != 0;
   if (const char* e = getenv("B2O_UPCONV_COMMUTE")) ctx->no_commute = atoi(e) == 0;      // 1: commuted decoder upsampling (opt-in, see common.cuh)
   if (const char* e = getenv("B2O_TC_AFF")) ctx->tc_aff_const = std::string(e) != "smem";
   if (const char* e = getenv("B2O_GLUE")) ctx->glue_v1 = std::string(e) == "v1";
   if (const char* e = getenv("B2O_FUSED_TAIL")) ctx->no_fused_tail = atoi(e) == 0;      // 0: separate head_tail_kernel (A/B, tests)
-  if (const char* e = getenv("B2O_TC_PAIR")) {        // default 1; 0 = single-CTA tiles (A/B runs); 2 = generic tiles too
+  if (const char* e = getenv("B2O_TC_PAIR")) {        // default 0 = single-CTA tiles; 1 = pairs on halo tiles; 2 = generic tiles too
     ctx->tc_pair = atoi(e) != 0;
     ctx->tc_pair_generic = atoi(e) == 2;
   }
@@ -560,7 +557,7 @@ extern "C" int b2o_craft_forward(b2o_ctx* ctx, const uint8_t* img, int n, int h,
   // UpsampleLike + Concatenate + 1x1 conv (380-390).  Opt-in (B2O_UPCONV_COMMUTE=1): where the skip tensor is exactly
   // twice the decoder tensor the upsampling is commuted behind the convolution -- the decoder half of the 1x1 conv runs
   // at LOW resolution and the full-resolution half adds its bilinear upsampling in the epilogue, so no upsampled tensor
-  // is written or read back.  Correct (tests) but slower than the explicit UpsampleLike on B200, hence not the default.
+  // is written or read back.  Correct (tests) but not the default: the explicit UpsampleLike is what the reference graph runs.
   auto level = [&](const char* name, const TensorView& y, const TensorView& cat_y, const TensorView& cat, const TensorView& skip,
                    size_t off_z, const TensorView& out) -> int {
     const std::string base(name);

@@ -485,7 +485,7 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
     // Close A under "8-neighbour inside B" with ONE warp sweeping the rows, alternately downwards and upwards, lane =
     // word of the row: a sweep carries the fill through every row it passes, so a blob takes about three sweeps
     // (down, up, one that changes nothing) where the all-words-at-once iteration took one round per row of the blob
-    // -- 64 rounds over ~480 words on the bench pages, half of this kernel's instructions (profiles/r2o_quads_source.txt).
+    // -- dozens of rounds on the bench pages' blobs.
     // The result is the same set: the smallest one that contains the seed and is closed under that neighbourhood.
     if (threadIdx.x < 32) {
       const int lane = threadIdx.x;
@@ -634,8 +634,7 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
 }
 
 // Pass 1, one block of 128 threads per (box slot, image) with SMALL planes: eight blocks per SM instead of the two
-// that 96 KB planes allow (the work is a chain of short latency-bound phases, profiles/r2n_glue_full.csv: 17 % of
-// the warp slots active with the large planes).  Components that do not fit are queued for pass 2.
+// that 96 KB planes allow (the work is a chain of short latency-bound phases, which wants many resident blocks).  Components that do not fit are queued for pass 2.
 __global__ void __launch_bounds__(256)
 quads_kernel(const uint8_t* __restrict__ mask, const int* __restrict__ label, int hs, int ws,
              const Component* __restrict__ comps, const int* __restrict__ counts, int max_boxes,

@@ -1,4 +1,4 @@
-// Shared declarations for the b2ocr CUDA library (sm_100a only).
+// Shared declarations for the b2ocr CUDA library (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -62,18 +62,18 @@ struct DeviceGuard {
 struct ConvLayer {
   std::string name;
   int cin = 0, cout = 0, ksize = 1, dil = 1, relu = 0;
-  __half* w_kmajor = nullptr;  // [cout][taps*cin] fp16, K index = tap*cin + c   (tcgen05 B operand)
+  __half* w_kmajor = nullptr;  // [cout][taps*cin] fp16, K index = tap*cin + c   (wgmma B operand)
   float* w_simt = nullptr;     // [taps][cin][cout] fp32 holding the fp16-rounded values (SIMT engine)
   float* w_f32 = nullptr;      // [taps][cin][cout] fp32 (only for the 3-channel / 1-channel stems)
   float *s1 = nullptr, *t1 = nullptr, *s2 = nullptr, *t2 = nullptr;
   std::vector<float> h_w_f32;                  // host copy of w_f32 (the 1- / 3-channel CRNN stem: kernel-parameter filter bank)
   std::vector<float> h_w_simt;                 // host copy of w_simt for layers of <= 1024 weights (fused into other kernels' parameters)
   std::vector<float> h_s1, h_t1, h_s2, h_t2;   // host copies: passed to the tensor-core kernel as a kernel parameter (constant bank)
-  CUtensorMap wmap;            // TMA map over w_kmajor (box 64 x block_n)
-  CUtensorMap wmap_pair;       // the same with box 64 x block_n/2: one CTA's half of a B tile (cta_group::2)
+  CUtensorMap wmap;            // TMA map over w_kmajor (box kch x block_n)
+  CUtensorMap wmap_pair;       // the same with box kch x block_n/2: the half of a B tile one CTA of a pair fetches
   bool pair_ok = false;        // wmap_pair is valid (64-channel chunks, block_n >= 64)
-  int block_n = 0;             // tcgen05 N tile; 0 = layer not eligible for the tensor-core engine
-  int kch = 0;                 // tcgen05 K chunk (channels per stage): 64 / 32 / 16
+  int block_n = 0;             // tensor-core N tile; 0 = layer not eligible for the tensor-core engine
+  int kch = 0;                 // tensor-core K chunk (channels per stage): 64 / 32 / 16
   // channels of the layer the reference defines, where the tensor-core form pads them (3 -> 16 input channels of the
   // CRAFT stem, 400 -> 512 columns of the STN GEMM): what the roofline's algorithmic FLOP count uses.  0 = cin / cout.
   int alg_cin = 0, alg_cout = 0;
@@ -87,19 +87,16 @@ struct TensorView {            // NHWC fp16 activation living inside a (possibly
 
 struct b2o_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int conv_engine = B2O_CONV_AUTO;
-  int tc_issuers = 0;          // MMA-issuing warps of conv_tc_kernel: 0 = auto (2 for N <= 128 tiles), 1, 2
-  bool tc_pair = true;         // CTA pairs (tcgen05 cta_group::2) for the halo-tile layers; B2O_TC_PAIR=0 turns them off
-  int tc_box16 = 16;           // width of the single A box per K chunk in MODE 3 layers (B2O_TC_BOX16=0: three 8 x 18 boxes; 10: tile + halo only)
-  bool tc_box_forced = false;  // B2O_TC_BOX16 was given: use that width everywhere instead of the per-layer rule
-  bool tc_box_all = false;     // B2O_TC_BOX_ALL=1: single-box tiles for every grouped layer (default: N <= 64 with 64-/32-channel chunks)
-  bool tc_pair_generic = false;   // B2O_TC_PAIR=2: also pair the generic tiles (1x1 / dilated layers): bit-identical, no gain measured (profiles/r2a_ab_pair2.log)
+  // CTA pairs (2-CTA clusters sharing B tiles by TMA multicast), opt-in with B2O_TC_PAIR=1 (halo-tile layers) or 2 (all
+  // eligible layers): bit-identical, but measured slower on H100 (bench: 141 against 202 img/s, 700 W H100 80GB HBM3)
+  bool tc_pair = false;
+  bool tc_pair_generic = false;   // B2O_TC_PAIR=2: also pair the generic tiles (1x1 / dilated layers)
   // Decoder glue: B2O_UPCONV_COMMUTE=1 commutes the 2x upsampling behind the decoder half of upconvN.conv.0 (low-res GEMM +
-  // upsample-add in the full-resolution layer's epilogue).  Numerically validated, but measured SLOWER on B200
-  // (profiles/r2e_layers.csv: upconv4.0 1.39 + upsample 0.85 ms -> 0.21 + 2.32 ms): the epilogue's per-pixel 16-byte
-  // gathers of the four taps are LSU-wavefront-bound.  Default: explicit UpsampleLike kernels.
-  bool tc_aff_const = true;    // epilogue constants as a kernel parameter (constant cache); B2O_TC_AFF=smem: round-1 staging in shared memory / global loads
+  // upsample-add in the full-resolution layer's epilogue).  Numerically validated; opt-in.  Default: explicit UpsampleLike
+  // kernels, as the reference graph has them.
+  bool tc_aff_const = true;    // epilogue constants as a kernel parameter (constant cache); B2O_TC_AFF=smem: staging in shared memory / global loads
   bool no_commute = true;
   bool glue_v1 = false;        // B2O_GLUE=v1: the round-1 upsample2x kernel (64-bit index chain, unshared blends) for A/B runs and the bit-identity test
   bool no_fused_tail = false;  // B2O_FUSED_TAIL=0: conv_cls.6/.8 as the separate head_tail_kernel instead of conv_cls.4's epilogue

@@ -177,10 +177,10 @@ __global__ void normalize16_kernel(const uint8_t* __restrict__ img, long long to
 
 // CRNN conv_1: x (B,200,31[,CIN]) fp16 -> (B,200,31,64) fp16, 3x3 same, bias + ReLU.  CIN = 1 (gray, the default) or 3
 // (build_model(color=True), recognition.py:214).  Weights [tap][cin][64].
-// (The 576 filter taps stay in shared memory: read as a kernel parameter through the constant cache -- 576 scalar LDC per
-// thread -- the kernel took 1.57 ms instead of 0.36, gpurun call r2k; the constant bank only pays for a few dozen reads.)
-// Each thread computes PIX consecutive pixels, so one shared-memory read of a filter tap feeds PIX FMAs (the kernel is
-// bound by the L1TEX data pipe: 97 % with one pixel per thread).
+// (The 576 filter taps stay in shared memory: read as a kernel parameter through the constant cache they would be 576
+// scalar constant loads per thread; the constant bank only pays for a few dozen reads.)
+// Each thread computes PIX consecutive pixels, so one shared-memory read of a filter tap feeds PIX FMAs (with one pixel
+// per thread the kernel is bound by shared-memory reads).
 template <int CIN, int PIX>
 __global__ void __launch_bounds__(128)
 stem_crnn_kernel(const __half* __restrict__ x, int B, int H, int W, const float* __restrict__ wgt /*[9*CIN][64]*/,
@@ -236,10 +236,9 @@ stem_crnn_kernel(const __half* __restrict__ x, int B, int H, int W, const float*
         const __half2 h = __floats2half2_rn(fmaxf(acc[q][2 * j], 0.f), fmaxf(acc[q][2 * j + 1], 0.f));
         pk[j] = *reinterpret_cast<const uint32_t*>(&h);
       }
-      __half* o = out + static_cast<size_t>(pix0 + q) * out_ld;
-      asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(o + cb), "r"(pk[0]), "r"(pk[1]),
-                   "r"(pk[2]), "r"(pk[3]), "r"(pk[4]), "r"(pk[5]), "r"(pk[6]), "r"(pk[7])
-                   : "memory");
+      uint4* o = reinterpret_cast<uint4*>(out + static_cast<size_t>(pix0 + q) * out_ld + cb);
+      o[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+      o[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
     }
   }
 }
@@ -396,8 +395,8 @@ __global__ void upsample2x_v1_kernel(const __half* __restrict__ in, int in_ld, i
   }
 }
 
-// The same quads with a third of the instructions (the v1 kernel issues 650 per thread and is issue-bound at 3.5 TB/s,
-// profiles/r2n_glue_full.csv): blockIdx.y walks the images so the decomposition of the index is 32-bit, and the two
+// The same quads with a third of the instructions (the v1 kernel is bound by instruction issue, not by memory):
+// blockIdx.y walks the images so the decomposition of the index is 32-bit, and the two
 // horizontal blends of a quad column (rows ya and yb) are formed once and shared by its two output rows.  Every
 // product and sum is the one v1 forms (same operands, same association), so the bits are v1's (B2O_GLUE=v1 A/B test).
 __global__ void __launch_bounds__(256, 4)

@@ -1,4 +1,4 @@
-// conv_tc.cu -- implicit-GEMM convolution / dense layer on the 5th-gen tensor cores (sm_100a).
+// conv_tc.cu -- implicit-GEMM convolution / dense layer on the Hopper tensor cores (sm_90a: wgmma, TMA, mbarrier).
 //
 // Replaces the TensorFlow Conv2D / Dense kernels behind keras.Model.predict for CRAFT
 // (reference detection.py:65-103, 365-410) and the CRNN (recognition.py:217-290, 292-327).
@@ -15,39 +15,24 @@
 //   filter bank fits in shared memory (small layers) it is loaded once per CTA and stays resident.
 // * K chunk KCH = 64 / 32 / 16 channels (128B / 64B / 32B swizzle) so 32- and 16-channel layers
 //   (CRAFT conv_cls.*, STN) also run on the tensor cores.
-// * one elected thread issues tcgen05.mma.kind::f16 (N=BLOCK_N, K=16); fp32 accumulators live in TMEM (2-8
-//   stages): the epilogue of tile i overlaps the main loop of tile i+1.  3x3 layers with 64-channel chunks and
-//   N >= 64 run as CTA PAIRS (clusters of two CTAs on one TPC, cta_group::2, M=256: each CTA stages its own A
-//   tile and half of the B tile, the leader issues for both); the rest use cta_group::1 with M=128.
-// * warp roles: warp0 = TMA producer (A ring + B ring), warp1 = TMEM allocator + MMA issuer,
-//   warps 3..18 = epilogue: tcgen05.ld -> scale/shift/ReLU/affine -> fp16|fp32 NHWC stores (possibly
-//   into a channel slice of a concat buffer) and, optionally, the fused 2x2 max-pool output.
+// * warp roles: thread 0 of warpgroup 0 = TMA producer (one ring of stages; a stage is the A box of one (tap group,
+//   channel chunk) plus, unless the filter bank is resident, its B boxes, all on one mbarrier); warpgroups 1 and 2 =
+//   consumers, one per 64-pixel half of the tile: wgmma.mma_async m64 x BLOCK_N x k16 with fp32 accumulators in
+//   registers, then the epilogue straight from those registers: scale/shift/ReLU/affine -> fp16|fp32 NHWC stores
+//   (possibly into a channel slice of a concat buffer) and, optionally, the fused 2x2 max-pool output or CRAFT tail.
 // * persistent: grid = min(#tiles, #SMs); n-tiles of one pixel tile run back to back.
 #include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
 
-// Development counters of the MMA warp (cycles): [cta][0]=total, [1]=wait tmem_empty, [2]=wait a_full,
-// [3]=wait b_full, [4]=tiles.  Read back with b2o_debug_read_tc().
-__device__ unsigned long long g_tc_debug[160 * 8];
-
 namespace {
 
-constexpr int BLOCK_M = 128;
-constexpr int UMMA_K = 16;
-// MMA-issuing warps: one, except in MODE 3 (one A slot per tile) with N <= 128, where two warps take alternate
-// TILES -- the scalar code of one warp (barrier waits, descriptor arithmetic) hides behind the other warp's
-// MMAs.  Every accumulator is fed by exactly one warp in program order, so the fp32 accumulation order is
-// fixed (two warps on alternate A stages of the SAME tile were tried first: faster too, but not
-// bit-reproducible run to run).  The A ring and the TMEM ring then have an even number of slots, so each slot
-// has ONE consumer: an mbarrier parity wait is only sound when the waiter is at most one phase behind, which
-// a warp skipping the other warp's stages in a shared ring is not (that variant dead-locked).
-// B2O_TC_ISSUERS=1 in the environment forces a single issuer.
-constexpr int MAX_ISSUERS = 2;            // warps 1..2 are issuer slots; p.issuers of them are active
-constexpr int NUM_THREADS = 32 * (1 + MAX_ISSUERS + 16);   // warp0 TMA, issuer slots, 16 epilogue warps (4 per TMEM quadrant)
-constexpr int EPI_THREADS = 512;
-constexpr int SMEM_TOTAL = 227 * 1024;     // dynamic shared memory per CTA (the sm_100 maximum, 232448 B)
+constexpr int WG_M = 64;                  // rows of one wgmma = pixels of the tile one consumer warpgroup owns
+constexpr int MMA_K = 16;
+constexpr int NUM_THREADS = 384;          // warpgroup 0: producer; warpgroups 1, 2: MMA + epilogue
+constexpr int CONSUMER_WARPS = 8;
+constexpr int SMEM_TOTAL = 227 * 1024;    // dynamic shared memory per CTA (the sm_90 maximum, 232448 B)
 constexpr int MAX_RING = 8;
 
 struct TcParams {
@@ -58,29 +43,25 @@ struct TcParams {
   int n_tiles;                            // cout / BLOCK_N
   int total_tiles;
   int halo, resident;
-  int na, nb;                             // ring depths
-  int a_stride, a_bytes;                  // bytes between A stages / bytes one A box delivers
-  int off_b, off_bar;                     // shared-memory offsets
+  int ns;                                 // ring depth (stages)
+  int a_bytes, a_stride;                  // bytes one A box delivers / offset of a stage's B boxes
+  int stage_bytes, stage_tx;              // bytes between stages / bytes a stage's barrier expects
+  int off_res, off_bar;                   // shared-memory offsets: resident filter bank, barriers
   int aff_smem;                           // epilogue constants staged in shared memory behind the barriers (B2O_TC_AFF=smem)
   int aff_const;                          // epilogue constants read from the AffConst kernel parameter (default)
-  int group;                              // MODE 3: A stages per tile (p.na then counts groups)
-  int issuers;                            // active MMA-issuing warps (2 = alternate tiles)
   const float *s1, *t1, *s2, *t2;
   int relu;
   void* out;
   int out_ld, out_f32, write_full;
-  int wide;                 // output rows are 32-byte aligned: one 256-bit store per 16 fp16 channels (full sector)
   __half* pool_out;                       // fused 2x2/2 max-pool output (or null)
   int pool_ld, PH, PW;
-  int box16;                              // MODE 3 with ONE 16 x 18 A box per K chunk (dx taps through the descriptor)
-  int debug_nostore;                      // development builds (-DB2O_TC_DEBUG, B2O_DEBUG_NOSTORE=1): epilogue computes but does not store
-  // fused CRAFT tail (16-channel layers only): conv_cls.6 (1x1 16->16 ReLU) + conv_cls.8 (1x1 16->2) applied to the
-  // epilogue's 16 channels in registers, fp32 (text, link) scores out -- detection.py:404-410
   // decoder glue (UPADD instances): the accumulator gets the exact-2x bilinear upsampling (half-pixel centres, clamped
   // borders -- UpsampleLike, detection.py:290-309) of a low-resolution fp16 tensor (N, H/2, W/2, cout) added BEFORE
   // the affine/ReLU: relu(bn(W_y.up(y) + W_s.skip)) = relu(bn(up(W_y.y) + W_s.skip)), detection.py:380-390
   const __half* up_src;
   int up_ld, UH, UW;
+  // fused CRAFT tail (16-channel layers only): conv_cls.6 (1x1 16->16 ReLU) + conv_cls.8 (1x1 16->2) applied to the
+  // epilogue's 16 channels in registers, fp32 (text, link) scores out -- detection.py:404-410
   const float *tail_w6, *tail_b6, *tail_w8, *tail_b8;   // [16][16], [16], [16][2], [2]
   float* tail_out;                        // (N,H,W,2) fp32, or null
 };
@@ -111,25 +92,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a broken pipeline traps (surfacing as a CUDA error) instead of hanging the GPU.
+// Bounded wait: a broken pipeline traps (surfacing as a CUDA error) instead of hanging the GPU.  No printf here: a
+// function call in the consumer loop makes ptxas serialize every wgmma.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("b2ocr conv_tc: mbarrier timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();
   }
 }
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -149,133 +122,88 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// ---- CTA pairs (cta_group::2).  The two CTAs of a cluster sit on the two SMs of a TPC; in the shared::cluster
-// window the CTA rank is bit 24 of a shared-memory address, so clearing it turns the address of a local
-// barrier into the address of the same barrier in the pair's leader (even) CTA.
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;
+// ---- CTA pairs: clusters of two CTAs share every B tile.  Each CTA loads half of the tile's rows and multicasts them
+// into the same shared-memory offset of both CTAs, signalling both CTAs' barriers at that offset.
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
 __device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.arrive.release;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
 }
-// TMA loads of a CTA pair: the data lands in THIS CTA's shared memory, the transaction bytes are counted on the
-// LEADER's barrier (which expects both CTAs' bytes).
-__device__ __forceinline__ void tma_load_4d_pair(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1,
-                                                 int c2, int c3) {
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(static_cast<uint16_t>(3))
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_pair(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
+// one arrival on the barrier at the same offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1)
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)), "r"(cta)
       : "memory");
 }
-// one arrival on the leader CTA's copy of `bar` (accumulator stage drained, from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_BIT_MASK) : "memory");
-}
-// K-major swizzled shared-memory matrix descriptor: rows of KCH*2 bytes, 8-row atoms SBO bytes apart.
-template <int KCH, int SBO_BYTES = 16 * KCH>
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  constexpr uint64_t SBO = SBO_BYTES;                      // 8 rows x (KCH*2) bytes unless the rows are strided apart
-  constexpr uint64_t LAYOUT = KCH == 64 ? 2 : (KCH == 32 ? 4 : 6);   // SWIZZLE_128B / 64B / 32B
+// K-major swizzled shared-memory matrix descriptor (wgmma): rows of KCH*2 bytes, 8-row atoms 16*KCH bytes apart.
+// Every start address used is a whole number of 8-row atoms from a 1 KB-aligned stage, plus the 32-byte k-step
+// inside a row, so the base-offset field stays 0.
+template <int KCH>
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
+  constexpr uint64_t SBO = 16 * KCH;                       // 8 rows x (KCH*2) bytes
+  constexpr uint64_t LAYOUT = KCH == 64 ? 1 : (KCH == 32 ? 2 : 3);   // SWIZZLE_128B / 64B / 32B
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);    // start address      bits [0,14)
   d |= static_cast<uint64_t>(1) << 16;                     // leading byte off.  bits [16,30) (unused: swizzled K-major)
   d |= (SBO >> 4) << 32;                                   // stride byte offset bits [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                     // descriptor version bits [46,48)
-  d |= LAYOUT << 61;                                       // swizzle mode       bits [61,64)
+  d |= LAYOUT << 62;                                       // swizzle mode       bits [62,64)
   return d;
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// CTA pair: M = 256 (128 rows from each CTA's A tile), B = BLOCK_N/2 rows from each CTA, accumulators in both
-// CTAs' TMEM at the same columns.  Issued by the leader CTA only.
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ... and its commit arrives on the barrier at the same offset in BOTH CTAs (mask 0b11)
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  const uint16_t mask = 3;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-template <bool PAIR>
-__device__ __forceinline__ void umma_issue(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  if (PAIR) umma_f16_pair(tmem_d, adesc, bdesc, idesc, accumulate);
-  else umma_f16(tmem_d, adesc, bdesc, idesc, accumulate);
-}
-template <bool PAIR>
-__device__ __forceinline__ void umma_done(uint64_t* bar) {
-  if (PAIR) umma_commit_pair(bar);
-  else umma_commit(bar);
-}
-template <int CH>
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, uint32_t* v);
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// D[64 x N] (+)= A[64 x 16] * B[16 x N]^T, f16 inputs K-major in shared memory, f32 accumulators in registers
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
 template <>
-__device__ __forceinline__ void tmem_ld<32>(uint32_t taddr, uint32_t* v) {
+__device__ __forceinline__ void wgmma_f16<16>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 template <>
-__device__ __forceinline__ void tmem_ld<16>(uint32_t taddr, uint32_t* v) {
+__device__ __forceinline__ void wgmma_f16<32>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// 256-bit global store (sm_100: STG.E.256).  A lane's 16 fp16 channels are one whole 32-byte sector; two
-// 128-bit stores touch the same sector twice (ncu: 32 sectors per request, half of each written per pass).
-__device__ __forceinline__ void st_global_256(void* ptr, const uint32_t* r) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
-               "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
+template <>
+__device__ __forceinline__ void wgmma_f16<64>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
+template <>
+__device__ __forceinline__ void wgmma_f16<128>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
 // Walks this CTA's tiles (cta, cta + ncta, ...) keeping the mixed-radix coordinate
@@ -285,12 +213,10 @@ struct TileIter {
   int d0, d1, d2, d3;        // gridDim.x in the same radix
   int r0, r1, r2;            // radices: n_tiles, tiles_w, tiles_h
   int tile, step, total;
-  // the CTA's tiles are blockIdx.x + i * gridDim.x; this iterator visits i = first, first + mult, ...
-  // cta / ncta: this CTA's (or CTA pair's) index and their number -- blockIdx.x / gridDim.x, halved for pairs
-  __device__ __forceinline__ TileIter(const TcParams& p, int cta, int ncta, int first = 0, int mult = 1) {
+  __device__ __forceinline__ TileIter(const TcParams& p, int cta, int ncta) {
     r0 = p.n_tiles; r1 = p.tiles_w; r2 = p.tiles_h;
-    total = p.total_tiles; step = ncta * mult;
-    tile = cta + first * ncta;
+    total = p.total_tiles; step = ncta;
+    tile = cta;
     int t = tile;
     c0 = t % r0; t /= r0; c1 = t % r1; t /= r1; c2 = t % r2; c3 = t / r2;
     t = step;
@@ -306,129 +232,40 @@ struct TileIter {
   }
 };
 
-// Per-channel epilogue constants as a KERNEL PARAMETER (constant bank): an epilogue warp reads them with a warp-uniform
-// index, which the constant cache serves without touching the L1TEX data pipe.  Staged in shared memory (round 1) the
-// same reads were 392 M LDS wavefronts per stem launch and 592 M per conv2 launch -- l1tex__data_pipe_lsu_wavefronts at
-// 98 % / 90 % of peak, on the very pipe the tensor core fetches its shared-memory operands through
-// (profiles/r2final_conv_full.csv).  16 KB of parameters need CUDA >= 12.1 (large kernel parameters).
+// Per-channel epilogue constants as a KERNEL PARAMETER (constant bank) for layers of <= AFF_MAX output channels.
+// 16 KB of parameters need CUDA >= 12.1 (large kernel parameters).
 constexpr int AFF_MAX = 1024;
 struct AffConst {
   float s1[AFF_MAX], t1[AFF_MAX], s2[AFF_MAX], t2[AFF_MAX];
   float tail[320];          // fused CRAFT tail: [w6 transposed [out j][in c] 256 | b6 16 | w8 [j][2] 32 | b8 2]
 };
 
-__device__ __forceinline__ void epi_affine_c(const TcParams& p, const AffConst& ac, const uint32_t* v, int c0, float* y) {
-#pragma unroll
-  for (int j = 0; j < 16; ++j) y[j] = fmaf(__uint_as_float(v[j]), ac.s1[c0 + j], ac.t1[c0 + j]);
-  if (p.relu) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) y[j] = fmaxf(y[j], 0.0f);
-  }
-  if (p.s2 != nullptr) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) y[j] = fmaf(y[j], ac.s2[c0 + j], ac.t2[c0 + j]);
-  }
-}
-
 // ------------------------------------------------------------------------------------------ kernel
-// Epilogue arithmetic of one 16-column accumulator chunk: y = relu?(acc * s1 + t1) [* s2 + t2].
-__device__ __forceinline__ void epi_affine(const TcParams& p, const float* s1, const float* t1, const float* s2,
-                                           const float* t2, const uint32_t* v, int c0, float* y) {
-#pragma unroll
-  for (int j = 0; j < 16; j += 4) {
-    const float4 a = *reinterpret_cast<const float4*>(s1 + c0 + j);
-    const float4 b = *reinterpret_cast<const float4*>(t1 + c0 + j);
-    y[j + 0] = fmaf(__uint_as_float(v[j + 0]), a.x, b.x);
-    y[j + 1] = fmaf(__uint_as_float(v[j + 1]), a.y, b.y);
-    y[j + 2] = fmaf(__uint_as_float(v[j + 2]), a.z, b.z);
-    y[j + 3] = fmaf(__uint_as_float(v[j + 3]), a.w, b.w);
-  }
-  if (p.relu) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) y[j] = fmaxf(y[j], 0.0f);
-  }
-  if (p.s2 != nullptr) {
-#pragma unroll
-    for (int j = 0; j < 16; j += 4) {
-      const float4 a = *reinterpret_cast<const float4*>(s2 + c0 + j);
-      const float4 b = *reinterpret_cast<const float4*>(t2 + c0 + j);
-      y[j + 0] = fmaf(y[j + 0], a.x, b.x);
-      y[j + 1] = fmaf(y[j + 1], a.y, b.y);
-      y[j + 2] = fmaf(y[j + 2], a.z, b.z);
-      y[j + 3] = fmaf(y[j + 3], a.w, b.w);
-    }
-  }
-}
-
-// 2x2/2 max pool of packed fp16 pairs across the halo tile's lanes (lane^1 = w neighbour, lane^8 = h neighbour).
-__device__ __forceinline__ void epi_pool8(uint32_t* pk) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    __half2 m = *reinterpret_cast<__half2*>(&pk[j]);
-    uint32_t o1 = __shfl_xor_sync(0xffffffffu, pk[j], 1);
-    m = __hmax2(m, *reinterpret_cast<__half2*>(&o1));
-    uint32_t mm = *reinterpret_cast<uint32_t*>(&m);
-    uint32_t o2 = __shfl_xor_sync(0xffffffffu, mm, 8);
-    m = __hmax2(m, *reinterpret_cast<__half2*>(&o2));
-    pk[j] = *reinterpret_cast<uint32_t*>(&m);
-  }
-}
-
-// MODE: 0 = generic tiles, 1 = halo tiles (3x3, dilation 1), 2 = halo tiles + resident filter bank,
-//       3 = as 2 with all A stages of a tile on ONE mbarrier (one wait + one issue region per tile)
-// PAIR: clusters of two CTAs (one TPC) run tcgen05.mma.cta_group::2 with M = 256: the CTAs take horizontally
-//       adjacent 8 x 16 pixel tiles (rank = which), each stages its own A boxes and HALF of the B tile
-//       (BLOCK_N / 2 filter rows), the leader CTA issues every MMA for both, each CTA's epilogue drains its own
-//       TMEM.  Per MMA a CTA's shared memory then supplies 4 KB of A + 16*BLOCK_N B of B instead of 32*BLOCK_N,
-//       and the filter bank is fetched from L2 once per 256 pixels instead of once per 128.  Validated and on by
-//       default for the halo modes; generic tiles (MODE 0: 1x1 and dilated layers) pair the same way but are opt-in
-//       (B2O_TC_PAIR=2) until they have run on a GPU.
-// BOX16 (MODE 3 only; the default there, B2O_TC_BOX16=0 turns it off; scripts/probes/dx_shift_probe.cu tests the
-//       descriptor semantics it relies on): ONE 16 x 18-pixel A box per K chunk serves all nine taps.  The dy taps
-//       move the A descriptor by whole image rows (2 KB = the stride between 8-row groups), the dx taps by single
-//       pixel rows (KCH * 2 bytes) inside a swizzle atom, descriptor base offset 0.  2.25x instead of
-//       3.375x of the tile's input crosses L2->SM, in one TMA instruction instead of three and 36 KB instead of 55 KB.
-//       The MMAs are issued in the same (dx, chunk, dy, k) order as without it.
-template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool BOX16 = false, bool UPADD = false>
+// MODE: 0 = generic tiles, 1 = halo tiles (3x3, dilation 1), 2 = halo tiles + resident filter bank
+// PAIR: clusters of two CTAs on horizontally adjacent pixel tiles of the same n-tile (rank = which).  Each CTA fetches
+//       HALF of every B tile from L2 and multicasts it to both, so the filter bank crosses L2 -> SM once per 256 pixels
+//       instead of once per 128; A boxes stay per CTA.  A stage may only be refilled when the consumers of BOTH CTAs have
+//       released it, so every consumer warp arrives on the empty barriers of both CTAs.  The MMAs and their order are
+//       those of the single-CTA tiles: results are bit-identical.
+template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
                const TcParams p, const __grid_constant__ AffConst ac) {
-  static_assert(!BOX16 || MODE == 3, "the single-box tile is implemented for grouped tiles (whole tile on one barrier)");
-  constexpr int B_ROWS = PAIR ? BLOCK_N / 2 : BLOCK_N;     // filter rows staged by one CTA
-  constexpr int B_BYTES = B_ROWS * KCH * 2;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;     // 0 = leader
+  constexpr bool HALO = MODE >= 1, RESIDENT = MODE == 2;
+  constexpr int TAPS_PER_A = HALO ? 3 : 1;                 // dy taps served by one A stage
+  constexpr int B_BYTES = BLOCK_N * KCH * 2;
+  constexpr int B_HALF = B_BYTES / 2;                      // pair: the B rows one CTA fetches and multicasts
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
   const int cta = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
   const int ncta = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
   const int pair_shift = PAIR ? 1 : 0;                     // tile column = (pair column << 1) + rank
-  // bytes between the tile's image rows in an A stage (= the descriptor's stride between 8-row groups): 8 pixels with three
-  // boxes per K chunk; with the single box its width p.box16 (10 = just the tile + halo, or 16 = whole 1 KB swizzle atoms
-  // per row).  Rows need not start on an atom boundary: the swizzle is a function of the absolute address (probe).
-  const int TAP_SHIFT = BOX16 ? p.box16 * 2 * KCH : 16 * KCH;
-  constexpr int KSTEPS = KCH / UMMA_K;
-  // TMEM accumulator stages: as many as fit in the 512 columns (max 8).  With only two, a short-K tile is
-  // bound by the *latency* of the epilogue hand-off (tmem_full -> LDTM -> stores -> tmem_empty), not by its
-  // throughput; with 4-8 the MMA warp runs several tiles ahead of the epilogue warps.
-  constexpr int ACC_STAGES = (512 / BLOCK_N) > 8 ? 8 : (512 / BLOCK_N);
-  constexpr int TMEM_COLS = (ACC_STAGES * BLOCK_N) < 32 ? 32 : (ACC_STAGES * BLOCK_N);
-  // Epilogue work split.  N = 256 (2 accumulator stages): the four warps of a TMEM quadrant share every tile,
-  // each taking every 4th 16-column chunk.  N <= 128 (>= 4 stages): each of the four warps takes every 4th
-  // TILE whole -- the per-tile fixed cost (barrier wake-up, coordinates, scale/shift loads) is then paid once
-  // per four tiles per warp, which is what bounds short-K layers.
-  constexpr bool TILE_PAR = ACC_STAGES >= 4;
-  constexpr int CH = 16;                                   // accumulator columns per tcgen05.ld (per epilogue warp visit)
+  constexpr int KSTEPS = KCH / MMA_K;
+  constexpr int NACC = BLOCK_N / 2;                        // fp32 accumulators per consumer thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + p.off_b;
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + p.off_bar);
-  uint64_t* a_empty = a_full + MAX_RING;
-  uint64_t* b_full = a_empty + MAX_RING;
-  uint64_t* b_empty = b_full + MAX_RING;
-  uint64_t* tmem_full = b_empty + MAX_RING;
-  uint64_t* tmem_empty = tmem_full + MAX_RING;
-  uint64_t* order_bar = tmem_empty + MAX_RING;
-  uint64_t* res_full = order_bar + MAX_RING;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_full + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bar);
+  uint64_t* empty = full + MAX_RING;
+  uint64_t* res_full = empty + MAX_RING;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -441,482 +278,281 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
       if (p.s2 != nullptr) { aff[2 * p.cout + i] = p.s2[i]; aff[3 * p.cout + i] = p.t2[i]; }
     }
   }
-  // fused tail constants behind the affine ones: [w6 | b6 | w8 | b8]
+  // fused tail constants behind the affine ones: [w6 transposed ([out j][in c]) | b6 | w8 | b8]
   float* const tail_s = aff + 4 * p.cout;
-  if (BLOCK_N == 16 && p.tail_out != nullptr) {
+  if (BLOCK_N == 16 && p.tail_out != nullptr && !p.aff_const) {
     for (int i = threadIdx.x; i < TAIL_FLOATS; i += NUM_THREADS)
-      // w6 is staged TRANSPOSED ([out j][in c]): a thread's 16 weights of one output are contiguous -> four LDS.128
       tail_s[i] = i < 256 ? p.tail_w6[(i & 15) * 16 + (i >> 4)] : (i < 272 ? p.tail_b6[i - 256] : (i < 304 ? p.tail_w8[i - 272] : p.tail_b8[i - 304]));
   }
-  const float* const e_s1 = p.aff_smem ? aff : p.s1;
-  const float* const e_t1 = p.aff_smem ? aff + p.cout : p.t1;
-  const float* const e_s2 = p.aff_smem ? aff + 2 * p.cout : p.s2;
-  const float* const e_t2 = p.aff_smem ? aff + 3 * p.cout : p.t2;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&amap);
-    tma_prefetch_desc(&bmap);
+  if (threadIdx.x == 0) {
     for (int s = 0; s < MAX_RING; ++s) {
-      mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
-      mbar_init(&b_full[s], 1);
-      mbar_init(&b_empty[s], 1);
-    }
-    for (int s = 0; s < ACC_STAGES; ++s) {
-      mbar_init(&tmem_full[s], 1);                          // the commit of the warp that issued the tile
-      mbar_init(&tmem_empty[s], (PAIR ? 2 : 1) * (TILE_PAR ? 4 : EPI_THREADS / 32));   // one arrival per epilogue warp on the tile (both CTAs of a pair arrive on the leader's)
-      mbar_init(&order_bar[s], 1);
+      mbar_init(&full[s], 1);                              // the producer's expect_tx arrival + the TMA bytes
+      mbar_init(&empty[s], (PAIR ? 2 : 1) * CONSUMER_WARPS);   // one arrival per consumer warp (of both CTAs of a pair) once its MMAs read the stage
     }
     mbar_init(res_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if (PAIR) {                                            // the same warp of both CTAs, collectively
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                   "r"(TMEM_COLS)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                   "r"(TMEM_COLS)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tcgen05_before_sync();
   if (PAIR) cluster_sync_all();                            // the peer's barriers exist before anything signals them
   else __syncthreads();
-  tcgen05_after_sync();
-  // Every launch requests > 114 KB of shared memory, so this CTA owns the SM and its TMEM allocation
-  // starts at column 0.  Using the literal 0 keeps the accumulator address in a uniform register:
-  // a per-thread value would make ptxas wrap every UTCHMMA in an ELECT / R2UR.BROADCAST loop, which
-  // costs ~120 cycles per MMA (measured with scripts/probes/mma_probe.cu).
-  if (*tmem_slot != 0u) {
-    if (threadIdx.x == 0) printf("b2ocr conv_tc: unexpected TMEM base %u\n", *tmem_slot);
-    __trap();
-  }
-  constexpr uint32_t tmem_base = 0u;
 
-  constexpr bool HALO = MODE >= 1, RESIDENT = MODE >= 2, GROUPED = MODE == 3;
-  constexpr int TAPS_PER_A = HALO ? 3 : 1;                 // dy taps served by one A stage
   const int taps = p.ksize * p.ksize;
   const int kchunks = p.cin / KCH;
-  const int half_k = p.ksize >> 1;
+  const int groups = HALO ? 3 : taps;                      // dx positions (halo) or filter taps (generic)
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
     // ===================================================================== TMA producer
-    if (lane == 0) {
-      const int b_row0 = static_cast<int>(rank) * B_ROWS;  // pair: this CTA's half of the filter rows of an n-tile
-      if (RESIDENT) {                                      // whole filter bank (pair: this CTA's half), once per CTA
-        if (rank == 0) mbar_expect_tx(res_full, static_cast<uint32_t>((PAIR ? 2 : 1) * taps * kchunks * B_BYTES));
+    if (threadIdx.x == 0) {
+      tma_prefetch_desc(&amap);
+      tma_prefetch_desc(&bmap);
+      const int half_k = p.ksize >> 1;
+      if (RESIDENT) {                                      // whole filter bank, once per CTA (pair: half of it from each CTA)
+        mbar_expect_tx(res_full, static_cast<uint32_t>(taps * kchunks * B_BYTES));
         for (int tap = 0; tap < taps; ++tap)
           for (int kc = 0; kc < kchunks; ++kc) {
-            if (PAIR) tma_load_2d_pair(&bmap, res_full, smem_b + (tap * kchunks + kc) * B_BYTES, tap * p.cin + kc * KCH, b_row0);
-            else tma_load_2d(&bmap, res_full, smem_b + (tap * kchunks + kc) * B_BYTES, tap * p.cin + kc * KCH, 0);
+            uint8_t* const dst = smem + p.off_res + (tap * kchunks + kc) * B_BYTES;
+            if (PAIR) tma_load_2d_multicast(&bmap, res_full, dst + rank * B_HALF, tap * p.cin + kc * KCH, static_cast<int>(rank) * (BLOCK_N / 2));
+            else tma_load_2d(&bmap, res_full, dst, tap * p.cin + kc * KCH, 0);
           }
       }
-      int sa = 0, sb = 0;
-      uint32_t pa = 0, pb = 0;
-      const int groups = HALO ? 3 : taps;                  // dx positions (halo) or filter taps (generic)
-      // pair: the leader's full barriers expect both CTAs' bytes; the peer only issues its loads (onto the
-      // leader's barriers).  The empty barriers are local: the leader's commits arrive on both CTAs' copies.
-      constexpr uint32_t TX_MULT = PAIR ? 2u : 1u;
+      int s = 0;
+      uint32_t ph = 0;
       for (TileIter ti(p, cta, ncta); ti.valid(); ti.next()) {
-        const int tw0 = ((ti.c1 << pair_shift) + static_cast<int>(rank)) << p.bw_log2, th0 = ti.c2 << p.bh_log2,
-                  tn0 = ti.c3 << p.bn_log2, t_ntile = ti.c0;
-        if (GROUPED) {                                     // every A box of the tile lands on one barrier
-          mbar_wait(&a_empty[sa], pa ^ 1);
-          if (rank == 0) mbar_expect_tx(&a_full[sa], TX_MULT * static_cast<uint32_t>(p.group * p.a_bytes));
-          uint8_t* dst = smem_a + sa * p.group * p.a_stride;
-          for (int g = 0; g < (BOX16 ? 1 : 3); ++g)        // BOX16: one 16-pixel-wide box holds all three dx positions
-            for (int kc = 0; kc < kchunks; ++kc) {
-              if (PAIR) tma_load_4d_pair(&amap, &a_full[sa], dst, kc * KCH, tw0 + g - 1, th0 - 1, tn0);
-              else tma_load_4d(&amap, &a_full[sa], dst, kc * KCH, tw0 + g - 1, th0 - 1, tn0);
-              dst += p.a_stride;
-            }
-          if (++sa == p.na) { sa = 0; pa ^= 1; }
-          continue;
-        }
+        const int tw0 = ((ti.c1 << pair_shift) + static_cast<int>(rank)) << p.bw_log2, th0 = ti.c2 << p.bh_log2, tn0 = ti.c3 << p.bn_log2;
         int ky = 0, kx = 0;
         for (int g = 0; g < groups; ++g) {
           const int ax = HALO ? (tw0 + g - 1) : (tw0 + (kx - half_k) * p.dil);
           const int ay = HALO ? (th0 - 1) : (th0 + (ky - half_k) * p.dil);
           for (int kc = 0; kc < kchunks; ++kc) {
-            mbar_wait(&a_empty[sa], pa ^ 1);
-            if (rank == 0) mbar_expect_tx(&a_full[sa], TX_MULT * static_cast<uint32_t>(p.a_bytes));
-            if (PAIR) tma_load_4d_pair(&amap, &a_full[sa], smem_a + sa * p.a_stride, kc * KCH, ax, ay, tn0);
-            else tma_load_4d(&amap, &a_full[sa], smem_a + sa * p.a_stride, kc * KCH, ax, ay, tn0);
-            if (++sa == p.na) { sa = 0; pa ^= 1; }
+            mbar_wait(&empty[s], ph ^ 1);
+            uint8_t* const st = smem + s * p.stage_bytes;
+            mbar_expect_tx(&full[s], static_cast<uint32_t>(p.stage_tx));
+            tma_load_4d(&amap, &full[s], st, kc * KCH, ax, ay, tn0);
             if (!RESIDENT) {
 #pragma unroll
               for (int t = 0; t < TAPS_PER_A; ++t) {
                 const int tap = HALO ? (t * 3 + g) : g;
-                mbar_wait(&b_empty[sb], pb ^ 1);
-                if (rank == 0) mbar_expect_tx(&b_full[sb], TX_MULT * B_BYTES);
-                if (PAIR) tma_load_2d_pair(&bmap, &b_full[sb], smem_b + sb * B_BYTES, tap * p.cin + kc * KCH, t_ntile * BLOCK_N + b_row0);
-                else tma_load_2d(&bmap, &b_full[sb], smem_b + sb * B_BYTES, tap * p.cin + kc * KCH, t_ntile * BLOCK_N);
-                if (++sb == p.nb) { sb = 0; pb ^= 1; }
+                uint8_t* const dst = st + p.a_stride + t * B_BYTES;
+                if (PAIR)
+                  tma_load_2d_multicast(&bmap, &full[s], dst + rank * B_HALF, tap * p.cin + kc * KCH,
+                                        ti.c0 * BLOCK_N + static_cast<int>(rank) * (BLOCK_N / 2));
+                else
+                  tma_load_2d(&bmap, &full[s], dst, tap * p.cin + kc * KCH, ti.c0 * BLOCK_N);
               }
             }
+            if (++s == p.ns) { s = 0; ph ^= 1; }
           }
           if (++kx == p.ksize) { kx = 0; ++ky; }
         }
       }
     }
-  } else if (warp >= 1 && warp <= MAX_ISSUERS) {
-    if (warp <= p.issuers && rank == 0) {                  // pair: the leader issues for both CTAs
-    // ===================================================================== MMA issuer
-    // The tensor pipe accepts MMAs with (almost) no queue, so every scalar instruction between two
-    // UTCHMMAs is exposed.  The issuing warp therefore runs warp-converged (descriptors, stage indices
-    // and the TMEM address stay in uniform registers; only the tcgen05 instructions are predicated on
-    // one elected lane) and issues all MMAs of an A stage from ONE elected region where it can.
-    // (The code is written for NUM_ISSUERS warps taking alternate A stages; see the note at NUM_ISSUERS.)
-    constexpr uint32_t idesc = (1u << 4) | (static_cast<uint32_t>(BLOCK_N >> 3) << 17) |
-                               (static_cast<uint32_t>((PAIR ? 2 * BLOCK_M : BLOCK_M) >> 4) << 24);   // D=f32, A=B=f16 K-major, N, M=128 (256 per pair)
-    const uint32_t TAP_DESC = static_cast<uint32_t>(TAP_SHIFT) >> 4;          // in 16-byte descriptor units
-    constexpr uint32_t B_DESC = B_BYTES >> 4;
-    const int me = warp - 1;
-    // (stride field bits [32,46) re-written for the run-time row pitch of the single-box tiles)
-    const uint64_t a_desc0 = (umma_desc<KCH, 16 * KCH>(smem_u32(smem_a)) & ~(static_cast<uint64_t>(0x3FFF) << 32)) |
-                             (static_cast<uint64_t>(static_cast<uint32_t>(TAP_SHIFT) >> 4) << 32);
-    const uint64_t b_desc0 = umma_desc<KCH>(smem_u32(smem_b));
-    const uint32_t a_step = static_cast<uint32_t>(p.a_stride) >> 4;
-    if (RESIDENT) { mbar_wait(res_full, 0); tcgen05_after_sync(); }
-    int sa = 0, sb = 0, acc = 0;
-    uint32_t pa = 0, pb = 0, acc_phase = 0;
-    const int groups = HALO ? 3 : taps;
-    // With two issuing warps the warps take alternate TILES: every accumulator is fed by one warp in program
-    // order (bit-reproducible), and while one warp runs its per-stage scalar code (barrier wait, descriptor
-    // arithmetic: ~500 cycles per stage, which the queue-less tensor pipe would otherwise sit idle through)
-    // the other warp's MMAs keep the pipe busy.  A skipped tile only advances the ring positions.
-    const bool alternate = GROUPED && ACC_STAGES >= 4 && p.issuers == 2;
-    const int a_per_tile = GROUPED ? 1 : groups * kchunks;
-    const int b_per_tile = RESIDENT ? 0 : a_per_tile * TAPS_PER_A;
-    int tile_seq = 0;
-#ifdef B2O_TC_DEBUG
-    long long dbg_t = 0, dbg_a = 0, dbg_b = 0, dbg_tiles = 0;
-    const long long dbg_start = clock64();
-#define B2O_TIMED_WAIT(counter, stmt) { const long long c0_ = clock64(); stmt; counter += clock64() - c0_; }
-#else
-#define B2O_TIMED_WAIT(counter, stmt) { stmt; }
-#endif
-    for (int tile = cta; tile < p.total_tiles; tile += ncta, ++tile_seq) {
-      if (alternate && (tile_seq & 1) != me) {             // the other warp's tile
-        sa += a_per_tile;
-        while (sa >= p.na) { sa -= p.na; pa ^= 1; }
-        if (!RESIDENT) {
-          sb += b_per_tile;
-          while (sb >= p.nb) { sb -= p.nb; pb ^= 1; }
-        }
-        if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-        continue;
-      }
-      B2O_TIMED_WAIT(dbg_t, mbar_wait(&tmem_empty[acc], acc_phase ^ 1))
-#ifdef B2O_TC_DEBUG
-      ++dbg_tiles;
-#endif
-      const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BLOCK_N);
-      if (GROUPED) {
-        // one wait and one elected region per tile: nothing but descriptor adds between the UTCHMMAs
-        B2O_TIMED_WAIT(dbg_a, mbar_wait(&a_full[sa], pa))
-        tcgen05_after_sync();
-        if (elect_one()) {
-          uint64_t adesc = a_desc0 + static_cast<uint64_t>(static_cast<uint32_t>(sa * p.group) * a_step);
-          uint32_t accumulate = 0;
-          // BOX16: dx = one 128-byte pixel row further into the same stages.  The descriptor's base-offset field stays 0:
-          // the swizzle pattern is a function of the absolute shared-memory address bits, so a start address that is not
-          // 1 KB-aligned needs no correction (scripts/probes/dx_shift_probe.cu on B200: offset 0 right for all nine taps,
-          // offset = dx wrong for dx = 1, 2 -- profiles/r2_dx_shift_probe.log)
-          constexpr uint64_t DX_STEP = static_cast<uint64_t>((KCH * 2) >> 4);
-          const uint64_t adesc_tile = adesc;
-          for (int g = 0; g < 3; ++g) {
-            if (BOX16) adesc = adesc_tile + static_cast<uint64_t>(g) * DX_STEP;
-            for (int kc = 0; kc < kchunks; ++kc) {
-#pragma unroll
-              for (int t = 0; t < 3; ++t) {
-                const uint64_t bdesc = b_desc0 + static_cast<uint64_t>(static_cast<uint32_t>((t * 3 + g) * kchunks + kc) * B_DESC);
-#pragma unroll
-                for (int k = 0; k < KSTEPS; ++k) {
-                  umma_issue<PAIR>(d_tmem, adesc + static_cast<uint64_t>(t * TAP_DESC + 2 * k), bdesc + static_cast<uint64_t>(2 * k), idesc,
-                           accumulate);
-                  accumulate = 1;
-                }
-              }
-              adesc += a_step;
-            }
-          }
-          umma_done<PAIR>(&a_empty[sa]);
-          umma_done<PAIR>(&tmem_full[acc]);
-        }
-        __syncwarp();
-        if (++sa == p.na) { sa = 0; pa ^= 1; }
-        if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-        continue;
-      }
-      tcgen05_after_sync();
+  } else {
+    // ===================================================================== consumers (warpgroups 1, 2)
+    const int wg = (threadIdx.x >> 7) - 1;                   // rows wg*64 .. wg*64+63 of the tile
+    const int q = lane & 3;
+    // accumulator layout of wgmma m64: this thread holds rows r0 and r0 + 8, columns 8i + 2q, 8i + 2q + 1
+    const int r0 = wg * WG_M + (warp & 3) * 16 + (lane >> 2);
+    constexpr uint32_t TAP_BYTES = 8 * KCH * 2;              // halo: one dy tap = 8 pixel rows further into the stage
+    const uint64_t desc_a0 = gmma_desc<KCH>(smem_u32(smem) + static_cast<uint32_t>(wg * WG_M * KCH * 2));
+    const uint64_t desc_b0 = gmma_desc<KCH>(smem_u32(smem) + static_cast<uint32_t>(RESIDENT ? p.off_res : p.a_stride));
+    const float* const e_s1 = p.aff_const ? ac.s1 : (p.aff_smem ? aff : p.s1);
+    const float* const e_t1 = p.aff_const ? ac.t1 : (p.aff_smem ? aff + p.cout : p.t1);
+    const float* const e_s2 = p.aff_const ? ac.s2 : (p.aff_smem ? aff + 2 * p.cout : p.s2);
+    const float* const e_t2 = p.aff_const ? ac.t2 : (p.aff_smem ? aff + 3 * p.cout : p.t2);
+    const float* const tail_c = p.aff_const ? ac.tail : tail_s;
+    if (RESIDENT) mbar_wait(res_full, 0);
+    const int bw_mask = (1 << p.bw_log2) - 1, bh_mask = (1 << p.bh_log2) - 1;
+    // a stage is free once the consumers of this CTA (and of the peer, whose B halves it also holds) are done with it
+    auto release = [&](int stage) {
+      if (PAIR) { mbar_arrive_cluster(&empty[stage], 0u); mbar_arrive_cluster(&empty[stage], 1u); }
+      else mbar_arrive(&empty[stage]);
+    };
+
+    int s = 0;
+    uint32_t ph = 0;
+    float acc[NACC];
+  #pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.0f;
+    for (TileIter ti(p, cta, ncta); ti.valid(); ti.next()) {
+      // ---- main loop: every stage of the tile, MMAs in (dx | tap, chunk, dy, k) order
+      int prev = -1;
+      uint32_t accumulate = 0;
       for (int g = 0; g < groups; ++g) {
         for (int kc = 0; kc < kchunks; ++kc) {
-          B2O_TIMED_WAIT(dbg_a, mbar_wait(&a_full[sa], pa))
-          const uint64_t adesc = a_desc0 + static_cast<uint64_t>(static_cast<uint32_t>(sa) * a_step);
-          const bool zeroing = g == 0 && kc == 0;          // this stage holds the tile's accumulator-zeroing MMA
-          if (RESIDENT || TAPS_PER_A == 1) {
-            // ONE elected region per stage: all taps' MMAs back to back, then the commits
-            uint64_t bdesc[TAPS_PER_A];
-#pragma unroll
-            for (int t = 0; t < TAPS_PER_A; ++t)
-              bdesc[t] = b_desc0 + static_cast<uint64_t>(
-                             static_cast<uint32_t>(RESIDENT ? ((t * 3 + g) * kchunks + kc) : sb) * B_DESC);
-            if (!RESIDENT) B2O_TIMED_WAIT(dbg_b, mbar_wait(&b_full[sb], pb))
-            tcgen05_after_sync();
-            if (elect_one()) {
-#pragma unroll
-              for (int t = 0; t < TAPS_PER_A; ++t) {
-#pragma unroll
-                for (int k = 0; k < KSTEPS; ++k)
-                  // dy tap t = the stage shifted by t rows of 8 pixels; k-step = +32 B inside the swizzle atom
-                  umma_issue<PAIR>(d_tmem, adesc + static_cast<uint64_t>(t * TAP_DESC + 2 * k), bdesc[t] + static_cast<uint64_t>(2 * k),
-                           idesc, (t == 0 && k == 0 && zeroing) ? 0u : 1u);
-              }
-              if (!RESIDENT) umma_done<PAIR>(&b_empty[sb]);
-              umma_done<PAIR>(&a_empty[sa]);                   // frees the A slot when these MMAs retire
+          mbar_wait(&full[s], ph);
+          const uint64_t adesc = desc_a0 + static_cast<uint64_t>(static_cast<uint32_t>(s * p.stage_bytes) >> 4);
+  #pragma unroll
+          for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
+          wgmma_fence();
+  #pragma unroll
+          for (int t = 0; t < TAPS_PER_A; ++t) {
+            const uint32_t boff = RESIDENT ? static_cast<uint32_t>(((t * 3 + g) * kchunks + kc) * B_BYTES)
+                                           : static_cast<uint32_t>(s * p.stage_bytes + t * B_BYTES);
+            const uint64_t bdesc = desc_b0 + static_cast<uint64_t>(boff >> 4);
+  #pragma unroll
+            for (int k = 0; k < KSTEPS; ++k) {
+              wgmma_f16<BLOCK_N>(acc, adesc + static_cast<uint64_t>((t * TAP_BYTES + k * 32) >> 4),
+                                 bdesc + static_cast<uint64_t>((k * 32) >> 4), accumulate);
+              accumulate = 1;
             }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();                                   // the previous stage's MMAs are done: release it
+          if (prev >= 0) {
             __syncwarp();
-            if (!RESIDENT) { if (++sb == p.nb) { sb = 0; pb ^= 1; } }
-          } else {
-            // halo tiles with a streamed filter bank: one B slot per dy tap, waited for tap by tap
-            tcgen05_after_sync();
-#pragma unroll
-            for (int t = 0; t < TAPS_PER_A; ++t) {
-              B2O_TIMED_WAIT(dbg_b, mbar_wait(&b_full[sb], pb))
-              tcgen05_after_sync();
-              const uint64_t bdesc = b_desc0 + static_cast<uint64_t>(static_cast<uint32_t>(sb) * B_DESC);
-              if (elect_one()) {
-#pragma unroll
-                for (int k = 0; k < KSTEPS; ++k)
-                  umma_issue<PAIR>(d_tmem, adesc + static_cast<uint64_t>(t * TAP_DESC + 2 * k), bdesc + static_cast<uint64_t>(2 * k),
-                           idesc, (t == 0 && k == 0 && zeroing) ? 0u : 1u);
-                umma_done<PAIR>(&b_empty[sb]);
-                if (t == TAPS_PER_A - 1) umma_done<PAIR>(&a_empty[sa]);
-              }
-              __syncwarp();
-              if (++sb == p.nb) { sb = 0; pb ^= 1; }
-            }
+            if (lane == 0) release(prev);
           }
-          if (++sa == p.na) { sa = 0; pa ^= 1; }
+          prev = s;
+          if (++s == p.ns) { s = 0; ph ^= 1; }
         }
       }
-      if (elect_one()) umma_done<PAIR>(&tmem_full[acc]);
+      wgmma_wait<0>();
+  #pragma unroll
+      for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
       __syncwarp();
-      if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-    }
-#ifdef B2O_TC_DEBUG
-    if (lane == 0 && cta < 160 && me == 0) {
-      unsigned long long* d = g_tc_debug + cta * 8;
-      d[0] = static_cast<unsigned long long>(clock64() - dbg_start);
-      d[1] = dbg_t; d[2] = dbg_a; d[3] = dbg_b; d[4] = dbg_tiles;
-    }
-#endif
-#undef B2O_TIMED_WAIT
-    }
-  } else {
-    // ===================================================================== epilogue (warps 3..18)
-    const int quad = warp & 3;                            // TMEM lane quadrant this warp may touch
-    const int sub = (warp - 1 - MAX_ISSUERS) >> 2;                      // the four warps of a quadrant split the column chunks
-    const int row = quad * 32 + lane;                     // accumulator row = pixel inside the tile
-    const int bw_mask = (1 << p.bw_log2) - 1, bh_mask = (1 << p.bh_log2) - 1;
-    const int wi = row & bw_mask;
-    const int hi = (row >> p.bw_log2) & bh_mask;
-    const int ni = row >> (p.bw_log2 + p.bh_log2);
-    // TILE_PAR: this warp owns tiles sub, sub + 4, ... of the CTA (and their accumulator stages)
-    constexpr int ACC_STEP = TILE_PAR ? 4 : 1;
-    int acc = TILE_PAR ? (sub % ACC_STAGES) : 0;
-    uint32_t acc_phase = 0;
-    for (TileIter ti(p, cta, ncta, TILE_PAR ? sub : 0, ACC_STEP); ti.valid(); ti.next()) {
-      const int w = (((ti.c1 << pair_shift) + static_cast<int>(rank)) << p.bw_log2) + wi, h = (ti.c2 << p.bh_log2) + hi,
-                n = (ti.c3 << p.bn_log2) + ni;
-      const bool valid = (w < p.W) && (h < p.H) && (n < p.N);
-      const size_t pix = (static_cast<size_t>(n) * p.H + h) * p.W + w;
+      if (lane == 0) release(prev);
+
+      // ---- epilogue from the registers
       const int c_base = ti.c0 * BLOCK_N;
-      // fused 2x2/2 max pool (halo tiles: lane^1 = w neighbour, lane^8 = h neighbour)
-      const bool pool_writer = p.pool_out != nullptr && !(w & 1) && !(h & 1) && (w >> 1) < p.PW && (h >> 1) < p.PH &&
-                               n < p.N;
-      const size_t ppix = (static_cast<size_t>(n) * p.PH + (h >> 1)) * p.PW + (w >> 1);
-
-      // UPADD: this pixel's four low-resolution taps (same rule and weights as upsample2x_kernel)
-      size_t up_a = 0, up_b = 0, up_c = 0, up_d = 0;
-      float up_ly = 0.f, up_lx = 0.f;
+      bool valid[2];
+      size_t pix[2];
+      int px_w[2], px_h[2], px_n[2];
+  #pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = r0 + 8 * hh;
+        px_w[hh] = (((ti.c1 << pair_shift) + static_cast<int>(rank)) << p.bw_log2) + (row & bw_mask);
+        px_h[hh] = (ti.c2 << p.bh_log2) + ((row >> p.bw_log2) & bh_mask);
+        px_n[hh] = (ti.c3 << p.bn_log2) + (row >> (p.bw_log2 + p.bh_log2));
+        valid[hh] = (px_w[hh] < p.W) && (px_h[hh] < p.H) && (px_n[hh] < p.N);
+        pix[hh] = (static_cast<size_t>(px_n[hh]) * p.H + px_h[hh]) * p.W + px_w[hh];
+      }
       if (UPADD) {
-        const int qy = (h + 1) >> 1, qx = (w + 1) >> 1;
-        const int ya = max(qy - 1, 0), yb = min(qy, p.UH - 1), xa = max(qx - 1, 0), xb = min(qx, p.UW - 1);
-        up_ly = ((h + 1) & 1) ? ((qy == 0) ? 0.0f : 0.75f) : 0.25f;      // ry = (h + 1) & 1
-        up_lx = ((w + 1) & 1) ? ((qx == 0) ? 0.0f : 0.75f) : 0.25f;
-        const size_t nb = static_cast<size_t>(min(n, p.N - 1)) * p.UH;
-        up_a = ((nb + ya) * p.UW + xa) * p.up_ld; up_b = ((nb + ya) * p.UW + xb) * p.up_ld;
-        up_c = ((nb + yb) * p.UW + xa) * p.up_ld; up_d = ((nb + yb) * p.UW + xb) * p.up_ld;
-      }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tcgen05_after_sync();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + static_cast<uint32_t>(acc * BLOCK_N);
-      // one 16-column chunk: affine/ReLU -> stores (+ fused pool)
-      auto chunk = [&](uint32_t* v, const int ch) {
-        const int c0 = c_base + ch * CH;
-        if (UPADD && valid) {
-          // acc += hy * (hx * A + lx * B) + ly * (hx * C + lx * D), the expression of upsample2x_kernel, in fp32
-          const float hy = 1.0f - up_ly, hx = 1.0f - up_lx;
-#pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            const uint4 ra = __ldg(reinterpret_cast<const uint4*>(p.up_src + up_a + c0 + 8 * half));
-            const uint4 rb = __ldg(reinterpret_cast<const uint4*>(p.up_src + up_b + c0 + 8 * half));
-            const uint4 rc = __ldg(reinterpret_cast<const uint4*>(p.up_src + up_c + c0 + 8 * half));
-            const uint4 rd = __ldg(reinterpret_cast<const uint4*>(p.up_src + up_d + c0 + 8 * half));
-            const __half2* pa = reinterpret_cast<const __half2*>(&ra);
-            const __half2* pb = reinterpret_cast<const __half2*>(&rb);
-            const __half2* pc = reinterpret_cast<const __half2*>(&rc);
-            const __half2* pd = reinterpret_cast<const __half2*>(&rd);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 fa = __half22float2(pa[i]), fb = __half22float2(pb[i]);
-              const float2 fc = __half22float2(pc[i]), fd = __half22float2(pd[i]);
-              const int j = 8 * half + 2 * i;
-              v[j] = __float_as_uint(__uint_as_float(v[j]) + (hy * (hx * fa.x + up_lx * fb.x) + up_ly * (hx * fc.x + up_lx * fd.x)));
-              v[j + 1] = __float_as_uint(__uint_as_float(v[j + 1]) + (hy * (hx * fa.y + up_lx * fb.y) + up_ly * (hx * fc.y + up_lx * fd.y)));
-            }
+        // acc += hy * (hx * A + lx * B) + ly * (hx * C + lx * D), the expression of upsample2x_kernel, in fp32
+  #pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          if (!valid[hh]) continue;
+          const int h = px_h[hh], w = px_w[hh];
+          const int qy = (h + 1) >> 1, qx = (w + 1) >> 1;
+          const int ya = max(qy - 1, 0), yb = min(qy, p.UH - 1), xa = max(qx - 1, 0), xb = min(qx, p.UW - 1);
+          const float ly = ((h + 1) & 1) ? ((qy == 0) ? 0.0f : 0.75f) : 0.25f;
+          const float lx = ((w + 1) & 1) ? ((qx == 0) ? 0.0f : 0.75f) : 0.25f;
+          const float hy = 1.0f - ly, hx = 1.0f - lx;
+          const size_t nb = static_cast<size_t>(px_n[hh]) * p.UH;
+          const __half* const ua = p.up_src + ((nb + ya) * p.UW + xa) * p.up_ld + c_base + 2 * q;
+          const __half* const ub = p.up_src + ((nb + ya) * p.UW + xb) * p.up_ld + c_base + 2 * q;
+          const __half* const uc = p.up_src + ((nb + yb) * p.UW + xa) * p.up_ld + c_base + 2 * q;
+          const __half* const ud = p.up_src + ((nb + yb) * p.UW + xb) * p.up_ld + c_base + 2 * q;
+  #pragma unroll
+          for (int i = 0; i < BLOCK_N / 8; ++i) {
+            const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(ua + 8 * i));
+            const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(ub + 8 * i));
+            const float2 fc = __half22float2(*reinterpret_cast<const __half2*>(uc + 8 * i));
+            const float2 fd = __half22float2(*reinterpret_cast<const __half2*>(ud + 8 * i));
+            acc[4 * i + 2 * hh] += hy * (hx * fa.x + lx * fb.x) + ly * (hx * fc.x + lx * fd.x);
+            acc[4 * i + 2 * hh + 1] += hy * (hx * fa.y + lx * fb.y) + ly * (hx * fc.y + lx * fd.y);
           }
-        }
-        float y[CH];
-        if (p.aff_const) epi_affine_c(p, ac, v, c0, y);     // warp-uniform
-        else epi_affine(p, e_s1, e_t1, e_s2, e_t2, v, c0, y);
-        if (BLOCK_N == 16 && p.tail_out != nullptr) {        // warp-uniform; only the 16-channel instances carry it
-          // The unfused path stores these 16 channels as fp16 and head_tail_kernel reads them back: round the same way
-          // and run the same fmaf chains, so the scores are bit-identical to conv_cls.4 -> head_tail_kernel.
-          float x[CH];
-#pragma unroll
-          for (int j = 0; j < CH; ++j) x[j] = __half2float(__float2half_rn(y[j]));
-          float o0, o1;
-          if (p.aff_const) {                                   // weights from the constant bank (no shared-memory pipe traffic)
-            o0 = ac.tail[304]; o1 = ac.tail[305];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float a = ac.tail[256 + j];
-#pragma unroll
-              for (int c = 0; c < 16; ++c) a = fmaf(x[c], ac.tail[j * 16 + c], a);
-              a = fmaxf(a, 0.0f);
-              o0 = fmaf(a, ac.tail[272 + j * 2 + 0], o0);
-              o1 = fmaf(a, ac.tail[272 + j * 2 + 1], o1);
-            }
-          } else {
-            o0 = tail_s[304]; o1 = tail_s[305];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float a = tail_s[256 + j];
-#pragma unroll
-              for (int c4 = 0; c4 < 16; c4 += 4) {
-                const float4 wv = *reinterpret_cast<const float4*>(tail_s + j * 16 + c4);
-                a = fmaf(x[c4], wv.x, a); a = fmaf(x[c4 + 1], wv.y, a); a = fmaf(x[c4 + 2], wv.z, a); a = fmaf(x[c4 + 3], wv.w, a);
-              }
-              a = fmaxf(a, 0.0f);
-              o0 = fmaf(a, tail_s[272 + j * 2 + 0], o0);
-              o1 = fmaf(a, tail_s[272 + j * 2 + 1], o1);
-            }
-          }
-          if (valid) reinterpret_cast<float2*>(p.tail_out)[pix] = make_float2(o0, o1);
-          return;
-        }
-        if (p.out_f32) {
-          if (valid) {
-            float* o = reinterpret_cast<float*>(p.out) + pix * p.out_ld + c0;
-            if (p.wide) {
-#pragma unroll
-              for (int j = 0; j < CH; j += 8) st_global_256(o + j, reinterpret_cast<const uint32_t*>(y + j));
-            } else {
-#pragma unroll
-              for (int j = 0; j < CH; j += 4)
-                *reinterpret_cast<float4*>(o + j) = make_float4(y[j], y[j + 1], y[j + 2], y[j + 3]);
-            }
-          }
-        } else {
-          uint32_t pk[CH / 2];
-#pragma unroll
-          for (int j = 0; j < CH; j += 2) {
-            __half2 hv = __floats2half2_rn(y[j], y[j + 1]);
-            pk[j / 2] = *reinterpret_cast<uint32_t*>(&hv);
-          }
-#ifdef B2O_TC_DEBUG
-          if (valid && p.write_full && !(p.debug_nostore && pk[0] != 0x12345678u)) {
-#else
-          if (valid && p.write_full) {
-#endif
-            __half* o = reinterpret_cast<__half*>(p.out) + pix * p.out_ld + c0;
-            if (p.wide) {
-              st_global_256(o, pk);
-            } else {
-#pragma unroll
-              for (int j = 0; j < CH / 2; j += 4)
-                *reinterpret_cast<uint4*>(o + 2 * j) = make_uint4(pk[j], pk[j + 1], pk[j + 2], pk[j + 3]);
-            }
-          }
-          if (p.pool_out != nullptr) {                    // warp-uniform branch
-            epi_pool8(pk);
-            if (pool_writer) {
-              __half* o = p.pool_out + ppix * p.pool_ld + c0;
-              if (p.wide) {
-                st_global_256(o, pk);
-              } else {
-#pragma unroll
-                for (int j = 0; j < CH / 2; j += 4)
-                  *reinterpret_cast<uint4*>(o + 2 * j) = make_uint4(pk[j], pk[j + 1], pk[j + 2], pk[j + 3]);
-              }
-            }
-          }
-        }
-      };
-      // chunks two at a time: both TMEM loads are in flight before the single wait
-      constexpr int CH_FIRST_STEP = TILE_PAR ? 1 : 4;
-      constexpr int PER_WARP = TILE_PAR ? BLOCK_N / CH : BLOCK_N / CH / 4;
-      const int ch_first = TILE_PAR ? 0 : sub;
-      if (PER_WARP >= 2 && !UPADD) {
-#pragma unroll 1
-        for (int i = 0; i < PER_WARP; i += 2) {
-          const int cha = ch_first + i * CH_FIRST_STEP, chb = cha + CH_FIRST_STEP;
-          uint32_t va[CH], vb[CH];
-          tmem_ld<CH>(taddr + static_cast<uint32_t>(cha * CH), va);
-          tmem_ld<CH>(taddr + static_cast<uint32_t>(chb * CH), vb);
-          tmem_ld_wait();
-          chunk(va, cha);
-          chunk(vb, chb);
-        }
-      } else {
-        // one chunk at a time (single-chunk tiles, and the UPADD instances, whose tap loads need the registers)
-#pragma unroll 1
-        for (int i = 0; i < PER_WARP; ++i) {
-          const int cha = ch_first + i * CH_FIRST_STEP;
-          uint32_t va[CH];
-          tmem_ld<CH>(taddr + static_cast<uint32_t>(cha * CH), va);
-          tmem_ld_wait();
-          chunk(va, cha);
         }
       }
-      tcgen05_before_sync();
-      __syncwarp();
-      if (lane == 0) {                                     // TMEM stage drained (one arrival per warp)
-        if (PAIR) mbar_arrive_leader(&tmem_empty[acc]);    // the issuer of both CTAs' MMAs lives in the leader
-        else mbar_arrive(&tmem_empty[acc]);
+      // y = relu?(acc * s1 + t1) [* s2 + t2], in place
+  #pragma unroll
+      for (int i = 0; i < BLOCK_N / 8; ++i) {
+        const int c = c_base + 8 * i + 2 * q;
+        const float2 a1 = *reinterpret_cast<const float2*>(e_s1 + c);
+        const float2 b1 = *reinterpret_cast<const float2*>(e_t1 + c);
+  #pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          float& y0 = acc[4 * i + 2 * hh];
+          float& y1 = acc[4 * i + 2 * hh + 1];
+          y0 = fmaf(y0, a1.x, b1.x);
+          y1 = fmaf(y1, a1.y, b1.y);
+          if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
+        }
+        if (p.s2 != nullptr) {
+          const float2 a2 = *reinterpret_cast<const float2*>(e_s2 + c);
+          const float2 b2 = *reinterpret_cast<const float2*>(e_t2 + c);
+  #pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            acc[4 * i + 2 * hh] = fmaf(acc[4 * i + 2 * hh], a2.x, b2.x);
+            acc[4 * i + 2 * hh + 1] = fmaf(acc[4 * i + 2 * hh + 1], a2.y, b2.y);
+          }
+        }
       }
-      acc += ACC_STEP;
-      if (acc >= ACC_STAGES) { acc -= ACC_STAGES; acc_phase ^= 1; }
+      if (BLOCK_N == 16 && p.tail_out != nullptr) {          // block-uniform; only the 16-channel instances carry it
+        // The unfused path stores these 16 channels as fp16 and head_tail_kernel reads them back: round the same way
+        // and run the same fmaf chains, so the scores are bit-identical to conv_cls.4 -> head_tail_kernel.
+        // The quad's four lanes hold a pixel's 16 channels between them: gather them, lane q & 1 takes pixel row
+        // r0 + 8 * (q & 1) (lanes 2, 3 compute the same pixels again and do not store).
+        uint32_t hv[2][2];                                   // [column group i][row hh]
+  #pragma unroll
+        for (int i = 0; i < 2; ++i)
+  #pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const __half2 h2 = __floats2half2_rn(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
+            hv[i][hh] = *reinterpret_cast<const uint32_t*>(&h2);
+          }
+        const int mine = q & 1;
+        float x[16];
+  #pragma unroll
+        for (int src = 0; src < 4; ++src)
+  #pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const uint32_t v0 = __shfl_sync(0xffffffffu, hv[i][0], (lane & ~3) | src);
+            const uint32_t v1 = __shfl_sync(0xffffffffu, hv[i][1], (lane & ~3) | src);
+            const uint32_t v = mine ? v1 : v0;
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&v));
+            x[8 * i + 2 * src] = f.x;
+            x[8 * i + 2 * src + 1] = f.y;
+          }
+        float o0 = tail_c[304], o1 = tail_c[305];
+  #pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          float a = tail_c[256 + j];
+  #pragma unroll
+          for (int c = 0; c < 16; ++c) a = fmaf(x[c], tail_c[j * 16 + c], a);
+          a = fmaxf(a, 0.0f);
+          o0 = fmaf(a, tail_c[272 + j * 2 + 0], o0);
+          o1 = fmaf(a, tail_c[272 + j * 2 + 1], o1);
+        }
+        if (q < 2 && valid[mine]) reinterpret_cast<float2*>(p.tail_out)[pix[mine]] = make_float2(o0, o1);
+        continue;
+      }
+      if (p.out_f32) {
+  #pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          if (!valid[hh]) continue;
+          float* const o = reinterpret_cast<float*>(p.out) + pix[hh] * p.out_ld + c_base + 2 * q;
+  #pragma unroll
+          for (int i = 0; i < BLOCK_N / 8; ++i)
+            *reinterpret_cast<float2*>(o + 8 * i) = make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
+        }
+        continue;
+      }
+      // fp16 out; fused 2x2/2 max pool on halo tiles: rows r0 / r0 + 8 are vertical neighbours (h even, h + 1), the w
+      // neighbour is lane ^ 4
+      const bool pool_writer = p.pool_out != nullptr && !(px_w[0] & 1) && !(px_h[0] & 1) && (px_w[0] >> 1) < p.PW &&
+                               (px_h[0] >> 1) < p.PH && px_n[0] < p.N;
+      const size_t ppix = (static_cast<size_t>(px_n[0]) * p.PH + (px_h[0] >> 1)) * p.PW + (px_w[0] >> 1);
+      __half* const o0 = reinterpret_cast<__half*>(p.out) + pix[0] * p.out_ld + c_base + 2 * q;
+      __half* const o1 = reinterpret_cast<__half*>(p.out) + pix[1] * p.out_ld + c_base + 2 * q;
+  #pragma unroll
+      for (int i = 0; i < BLOCK_N / 8; ++i) {
+        const __half2 h0 = __floats2half2_rn(acc[4 * i], acc[4 * i + 1]);
+        const __half2 h1 = __floats2half2_rn(acc[4 * i + 2], acc[4 * i + 3]);
+        if (p.write_full) {
+          if (valid[0]) *reinterpret_cast<__half2*>(o0 + 8 * i) = h0;
+          if (valid[1]) *reinterpret_cast<__half2*>(o1 + 8 * i) = h1;
+        }
+        if (p.pool_out != nullptr) {                         // block-uniform branch
+          __half2 m = __hmax2(h0, h1);
+          const uint32_t mu = *reinterpret_cast<const uint32_t*>(&m);
+          const uint32_t ou = __shfl_xor_sync(0xffffffffu, mu, 4);
+          m = __hmax2(m, *reinterpret_cast<const __half2*>(&ou));
+          if (pool_writer) *reinterpret_cast<__half2*>(p.pool_out + ppix * p.pool_ld + c_base + 8 * i + 2 * q) = m;
+        }
+      }
     }
   }
-
-  tcgen05_before_sync();
-  if (PAIR) cluster_sync_all();                            // neither CTA leaves while the other may still signal it
-  else __syncthreads();
-  if (warp == 1) {
-    tcgen05_after_sync();
-    if (PAIR)
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    else
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
+  // neither CTA of a pair leaves while the other may still signal its barriers
+  if (PAIR) cluster_sync_all();
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -959,11 +595,9 @@ double pick_box(int N, int H, int W, int* bw_l, int* bh_l, int* bn_l) {
   return best_cover;
 }
 
-constexpr int kRetrySingle = 1;            // launch(): the pair launch was refused, plan the layer again without pairs
-
 thread_local const float* g_tail_host = nullptr;     // the fused tail's constants in AffConst::tail order (set by conv_tc_run)
 
-template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool BOX16 = false, bool UPADD = false>
+template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD = false>
 int launch(b2o_ctx* ctx, const CUtensorMap& amap, const ConvLayer& L, const TcParams& p, int smem_bytes,
            cudaStream_t st) {
   static thread_local AffConst ac;                         // 16 KB: filled per launch from the layer's host copies
@@ -974,13 +608,13 @@ int launch(b2o_ctx* ctx, const CUtensorMap& amap, const ConvLayer& L, const TcPa
     if (!L.h_s2.empty()) { memcpy(ac.s2, L.h_s2.data(), nb); memcpy(ac.t2, L.h_t2.data(), nb); }
     if (p.tail_out != nullptr && g_tail_host != nullptr) memcpy(ac.tail, g_tail_host, TAIL_FLOATS * sizeof(float));
   }
-  const void* fn = reinterpret_cast<const void*>(&conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, BOX16, UPADD>);
+  const void* fn = reinterpret_cast<const void*>(&conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD>);
   if (!ctx->configured.count(fn)) {                        // a per-device attribute: remembered per context
-    B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, BOX16, UPADD>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, 232448));
+    B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
     ctx->configured.insert(fn);
   }
-  // persistent: one CTA per SM; pairs: one cluster of two CTAs per TPC
+  // persistent: one CTA per SM; pairs: one cluster of two CTAs per two SMs
   const int units = PAIR ? ctx->sm_count / 2 : ctx->sm_count;
   const int grid = (p.total_tiles < units ? p.total_tiles : units) * (PAIR ? 2 : 1);
   cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -1001,18 +635,9 @@ int launch(b2o_ctx* ctx, const CUtensorMap& amap, const ConvLayer& L, const TcPa
     attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    const cudaError_t le = cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, BOX16, UPADD>, amap, L.wmap_pair, p, ac);
-    if (le != cudaSuccess) {
-      // a device / partition that cannot co-schedule two such CTAs on a TPC: fall back, once and for good, to the
-      // single-CTA tiles of the same kernel (bit-identical results)
-      cudaGetLastError();
-      if (e0) { cudaEventDestroy(e0); cudaEventDestroy(e1); }
-      fprintf(stderr, "b2ocr: CTA-pair launch failed (%s); using single-CTA convolution tiles\n", cudaGetErrorString(le));
-      ctx->tc_pair = false;
-      return kRetrySingle;
-    }
+    B2O_CUDA_CHECK(ctx, cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD>, amap, L.wmap_pair, p, ac));
   } else {
-    conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, BOX16, UPADD><<<grid, NUM_THREADS, smem_bytes, st>>>(amap, L.wmap, p, ac);
+    conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD><<<grid, NUM_THREADS, smem_bytes, st>>>(amap, L.wmap, p, ac);
   }
   B2O_LAUNCH_CHECK(ctx);
   if (ctx->profile) {
@@ -1033,7 +658,8 @@ int conv_tc_prepare(b2o_ctx* ctx, ConvLayer& L) {
   L.block_n = 0;
   L.kch = L.cin % 64 == 0 ? 64 : (L.cin % 32 == 0 ? 32 : (L.cin % 16 == 0 ? 16 : 0));
   if (L.kch == 0 || L.cout % 16 != 0) return B2O_OK;      // handled by the SIMT engine
-  int bn = 256;
+  // N tile <= 128: a consumer thread holds BLOCK_N / 2 fp32 accumulators in registers
+  int bn = 128;
   while (bn > 16 && (L.cout % bn != 0)) bn >>= 1;
   if (L.cout % bn != 0) return B2O_OK;
   if (L.kch == 32 && bn > 32) return B2O_OK;               // instantiated combinations only
@@ -1053,7 +679,7 @@ int conv_tc_prepare(b2o_ctx* ctx, ConvLayer& L) {
     return B2O_ERR_CUDA;
   }
   L.block_n = bn;
-  // CTA pairs: each CTA stages bn / 2 filter rows of an n-tile (instantiated for 64-channel chunks, bn >= 64)
+  // CTA pairs: each CTA fetches bn / 2 filter rows of an n-tile (instantiated for 64-channel chunks, bn >= 64)
   L.pair_ok = false;
   if (L.kch == 64 && bn >= 64) {
     cuuint32_t half_box[2] = {static_cast<cuuint32_t>(L.kch), static_cast<cuuint32_t>(bn / 2)};
@@ -1095,7 +721,7 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   if (!enc) { ctx->set_error("cuTensorMapEncodeTiled entry point not available"); return B2O_ERR_CUDA; }
   const int kch = L.kch, bn = L.block_n;
   const int taps = L.ksize * L.ksize, kchunks = L.cin / kch;
-  int b_bytes = bn * kch * 2;
+  const int b_bytes = bn * kch * 2;
 
   TcParams p;
   memset(&p, 0, sizeof(p));
@@ -1114,12 +740,10 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
             (halo_cover <= 1.15 * generic_cover || want_pool)) ? 1 : 0;
   if (want_pool && !p.halo) { ctx->set_error("conv_tc_run: fused pool needs the halo tile (" + L.name + ")"); return B2O_ERR_ARG; }
   if (p.halo) { p.bw_log2 = 3; p.bh_log2 = 4; p.bn_log2 = 0; }
-  // CTA pairs (B2O_TC_PAIR=0 turns them off): halo tiles only; a pair covers two horizontally adjacent tiles, each
-  // CTA stages half of the B tile.  The accumulation order per output is the same as without pairs, so the results
-  // are bit-identical (tests/test_gpu_parity.py::test_cta_pairs_give_bit_identical_results).
+  // CTA pairs (opt-in): halo tiles with B2O_TC_PAIR=1, generic tiles too with B2O_TC_PAIR=2; a pair covers
+  // two horizontally adjacent tiles.  Same MMAs in the same order per output: bit-identical results.
   const bool pair = ctx->tc_pair && (p.halo || ctx->tc_pair_generic) && L.pair_ok && ctx->conv_engine == B2O_CONV_AUTO &&
                     up_add == nullptr;
-  if (pair) b_bytes /= 2;
   p.tiles_w = (in.w + (1 << p.bw_log2) - 1) >> p.bw_log2;
   if (pair) p.tiles_w = (p.tiles_w + 1) / 2;                // pair columns
   p.tiles_h = (in.h + (1 << p.bh_log2) - 1) >> p.bh_log2;
@@ -1129,13 +753,7 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   if (total > 0x7fffffffLL) { ctx->set_error("conv_tc_run: too many tiles"); return B2O_ERR_ARG; }
   p.total_tiles = static_cast<int>(total);
 
-  // shared-memory plan: [A ring][B ring | resident filter bank][barriers]
-  p.issuers = 1;
-  // layers with few output channels keep their epilogue constants (s1,t1,s2,t2) in shared memory: their
-  // epilogue is latency-bound and the per-chunk __ldg's of the constants were its top stall (ncu source view)
-  // measured per layer (profiles/r2l_epilogue_constants_ab.txt): wins wherever the constants used to be staged in shared
-  // memory (cout <= 256: stem 3.15 -> 2.88 ms, slice1.7 2.08 -> 1.92, conv_cls.4 + tail 0.90 -> 0.64), loses 1-2 % against
-  // the plain global loads of the wider layers -- those keep them
+  // shared-memory plan: [ring of stages: A box | B boxes][resident filter bank][barriers][epilogue constants]
   p.aff_const = (ctx->tc_aff_const && L.cout <= 256 && static_cast<int>(L.h_s1.size()) == L.cout) ? 1 : 0;
   p.aff_smem = (!p.aff_const && L.cout <= 256) ? 1 : 0;
   const int aff_bytes = (p.aff_smem ? 4 * L.cout * 4 : 0) + (tail ? TAIL_FLOATS * 4 : 0);
@@ -1143,61 +761,21 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   p.a_bytes = p.halo ? 18 * 8 * kch * 2 : 128 * kch * 2;
   p.a_stride = (p.a_bytes + 1023) / 1024 * 1024;
   const long long res_bytes = static_cast<long long>(taps) * kchunks * b_bytes;
-  // (the leader's barrier counts both CTAs' halves of a pair: the mbarrier tx-count holds 2^20 - 1 bytes)
-  p.resident = (p.halo && p.n_tiles == 1 && res_bytes + 2LL * p.a_stride <= budget &&
-                res_bytes * (pair ? 2 : 1) <= (1 << 20) - 1) ? 1 : 0;
-  // single-box tiles (default; B2O_TC_BOX16=0 restores three 8-pixel-wide boxes per K chunk): one 16-pixel-wide box per
-  // K chunk, where the layer then still runs as whole tiles per barrier (MODE 3).  Same MMA order, bit-identical results.
-  // Measured per layer on B200 (profiles/r2b_layers.csv vs r2a): N <= 64 tiles with 64- / 32-channel chunks gain
-  // (conv2 64->64 4.66 -> 4.31 ms, upconv4.3 1.12 -> 0.86, conv_cls.0/.2 0.64 -> 0.57), N = 128 tiles lose 3-5 % (fewer,
-  // larger ring slots) and the 16-channel stem loses 14 % (32-byte pixel rows: the dx-shifted operand reads straddle
-  // the 256-byte swizzle atoms) -- so only the former use it.
-  if (ctx->tc_box16 && p.resident && (ctx->tc_box_all || (bn <= 64 && kch >= 32)) && bn <= 128 && ctx->conv_engine == B2O_CONV_AUTO) {
-    // box width in pixels: 10 (just the tile + halo) for 64-channel chunks, 16 (image rows on whole swizzle atoms) for
-    // 32-channel chunks -- measured (profiles/r2g_box_width.txt): width 10 cuts conv2's DRAM re-reads (11.9 -> 10.4 GB) and
-    // gains on conv2 / upconv4.3, but loses 19-25 % on the 64-byte-row conv_cls layers; B2O_TC_BOX16=10|16 forces one
-    const int bw = ctx->tc_box_forced ? ctx->tc_box16 : (kch == 64 ? 10 : 16);
-    const int a1 = 18 * bw * kch * 2, a1s = (a1 + 1023) / 1024 * 1024;
-    if ((budget - res_bytes) / a1s >= 2 * kchunks) { p.box16 = bw; p.a_bytes = a1; p.a_stride = a1s; }
-  }
-  if (p.resident) {
-    p.na = static_cast<int>((budget - res_bytes) / p.a_stride);
-    const int n_a = (p.box16 ? 1 : 3) * kchunks;           // A stages per tile
-    if (p.na >= 2 * n_a) {                                 // MODE 3: whole tiles per barrier
-      p.group = n_a;
-      p.na = p.na / n_a;
-      if (p.na > MAX_RING) p.na = MAX_RING;
-      if (bn <= 128 && ctx->tc_issuers != 1) {             // two issuers on alternate tiles: even rings (see top)
-        p.na &= ~1;
-        p.issuers = 2;
-      }
-      p.off_b = p.na * n_a * p.a_stride;
-    } else {
-      if (p.na > MAX_RING) p.na = MAX_RING;
-      p.off_b = p.na * p.a_stride;
-    }
-    p.nb = 1;
-    p.off_bar = p.off_b + static_cast<int>((res_bytes + 1023) / 1024 * 1024);
-  } else if (p.halo) {
-    p.na = b_bytes <= 16384 ? 4 : 3;
-    p.nb = (budget - p.na * p.a_stride) / b_bytes;
-    if (p.nb > MAX_RING) p.nb = MAX_RING;
-    p.off_b = p.na * p.a_stride;
-    p.off_bar = p.off_b + (p.nb * b_bytes + 1023) / 1024 * 1024;
-  } else {
-    int s = budget / (p.a_stride + b_bytes);
-    if (s > MAX_RING) s = MAX_RING;
-    p.na = p.nb = s;
-    p.off_b = p.na * p.a_stride;
-    p.off_bar = p.off_b + (p.nb * b_bytes + 1023) / 1024 * 1024;
-  }
-  if (p.na < 2 || p.nb < 1) { ctx->set_error("conv_tc_run: shared-memory plan failed for " + L.name); return B2O_ERR_ARG; }
+  // (the mbarrier tx-count holds 2^20 - 1 bytes)
+  p.resident = (p.halo && p.n_tiles == 1 && res_bytes + 2LL * p.a_stride <= budget && res_bytes <= (1 << 20) - 1) ? 1 : 0;
+  const int b_per_stage = p.resident ? 0 : (p.halo ? 3 : 1);
+  p.stage_bytes = p.a_stride + b_per_stage * b_bytes;
+  p.stage_tx = p.a_bytes + b_per_stage * b_bytes;
+  p.ns = static_cast<int>((budget - (p.resident ? res_bytes : 0)) / p.stage_bytes);
+  if (p.ns > MAX_RING) p.ns = MAX_RING;
+  if (p.ns < 2) { ctx->set_error("conv_tc_run: shared-memory plan failed for " + L.name); return B2O_ERR_ARG; }
+  p.off_res = p.ns * p.stage_bytes;
+  p.off_bar = p.off_res + (p.resident ? static_cast<int>((res_bytes + 1023) / 1024 * 1024) : 0);
   int smem_bytes = p.off_bar + 512 + aff_bytes + 1024;
-  if (smem_bytes < 120 * 1024) smem_bytes = 120 * 1024;    // one CTA per SM (TMEM base 0, see kernel)
+  // the grid is one persistent CTA per SM: a request above half of the SM's 228 KB keeps a second CTA of a small layer
+  // from landing on an SM that already runs one while other SMs sit idle
+  if (smem_bytes < 116 * 1024) smem_bytes = 116 * 1024;
 
-#ifdef B2O_TC_DEBUG
-  if (const char* e = getenv("B2O_DEBUG_NOSTORE")) p.debug_nostore = atoi(e);
-#endif
   p.s1 = L.s1; p.t1 = L.t1; p.s2 = L.s2; p.t2 = L.t2; p.relu = L.relu;
   if (up_add) { p.up_src = up_add->ptr; p.up_ld = up_add->ld; p.UH = up_add->h; p.UW = up_add->w; }
   float tail_host[TAIL_FLOATS];
@@ -1219,11 +797,6 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
     }
     p.pool_out = pool_out->ptr; p.pool_ld = pool_out->ld; p.PH = pool_out->h; p.PW = pool_out->w;
   }
-  {
-    const size_t esz = out_f32 ? 4 : 2;
-    p.wide = reinterpret_cast<uintptr_t>(out.ptr) % 32 == 0 && (out.ld * esz) % 32 == 0;
-    if (want_pool) p.wide = p.wide && reinterpret_cast<uintptr_t>(pool_out->ptr) % 32 == 0 && (pool_out->ld * 2) % 32 == 0;
-  }
 
   CUtensorMap amap;
   cuuint64_t dims[4] = {static_cast<cuuint64_t>(in.c), static_cast<cuuint64_t>(in.w), static_cast<cuuint64_t>(in.h),
@@ -1231,7 +804,7 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   cuuint64_t strides[3] = {static_cast<cuuint64_t>(in.ld) * 2, static_cast<cuuint64_t>(in.ld) * 2 * in.w,
                            static_cast<cuuint64_t>(in.ld) * 2 * in.w * in.h};
   cuuint32_t box[4] = {static_cast<cuuint32_t>(kch), 1u << p.bw_log2, 1u << p.bh_log2, 1u << p.bn_log2};
-  if (p.halo) { box[1] = p.box16 ? p.box16 : 8; box[2] = 18; box[3] = 1; }
+  if (p.halo) { box[1] = 8; box[2] = 18; box[3] = 1; }
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(&amap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, in.ptr, dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(kch), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1241,51 +814,28 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
                    std::to_string(static_cast<int>(r)));
     return B2O_ERR_CUDA;
   }
-  if (up_add != nullptr) {                                 // generic 1x1 tiles, single CTAs
-    if (bn == 64) return launch<64, 64, 0, false, false, true>(ctx, amap, L, p, smem_bytes, st);
-    if (bn == 128) return launch<128, 64, 0, false, false, true>(ctx, amap, L, p, smem_bytes, st);
-    if (bn == 256) return launch<256, 64, 0, false, false, true>(ctx, amap, L, p, smem_bytes, st);
+  if (up_add != nullptr) {                                 // generic 1x1 tiles
+    if (bn == 64) return launch<64, 64, 0, false, true>(ctx, amap, L, p, smem_bytes, st);
+    if (bn == 128) return launch<128, 64, 0, false, true>(ctx, amap, L, p, smem_bytes, st);
   }
-#define B2O_TC_BOX16_PAIR_CASE(BN)                                                                     \
-  if (p.box16 && p.group && pair && bn == BN) {                                                       \
-    const int rc = launch<BN, 64, 3, true, true>(ctx, amap, L, p, smem_bytes, st);                    \
-    return rc == kRetrySingle ? conv_tc_run(ctx, L, in, out, out_f32, st, pool_out, write_full, tail, up_add) : rc; \
+#define B2O_TC_PAIR_CASE(BN)                                                           \
+  if (pair && bn == BN) {                                                              \
+    if (p.resident) return launch<BN, 64, 2, true>(ctx, amap, L, p, smem_bytes, st);   \
+    if (p.halo) return launch<BN, 64, 1, true>(ctx, amap, L, p, smem_bytes, st);       \
+    return launch<BN, 64, 0, true>(ctx, amap, L, p, smem_bytes, st);                   \
   }
-  B2O_TC_BOX16_PAIR_CASE(64); B2O_TC_BOX16_PAIR_CASE(128);
-#undef B2O_TC_BOX16_PAIR_CASE
-#define B2O_TC_BOX16_CASE(BN, KC)                                                                      \
-  if (p.box16 && p.group && !pair && bn == BN && kch == KC) return launch<BN, KC, 3, false, true>(ctx, amap, L, p, smem_bytes, st);
-  B2O_TC_BOX16_CASE(16, 64); B2O_TC_BOX16_CASE(32, 64); B2O_TC_BOX16_CASE(64, 64); B2O_TC_BOX16_CASE(128, 64);
-  B2O_TC_BOX16_CASE(16, 32); B2O_TC_BOX16_CASE(32, 32); B2O_TC_BOX16_CASE(32, 16); B2O_TC_BOX16_CASE(64, 16);
-#undef B2O_TC_BOX16_CASE
-  if (p.box16 && p.group) { ctx->set_error("conv_tc_run: no single-box kernel instance for " + L.name); return B2O_ERR_ARG; }
-#define B2O_TC_PAIR_CASE(BN)                                                                  \
-  if (pair && bn == BN) {                                                                     \
-    const int rc = (p.resident && p.group) ? launch<BN, 64, 3, true>(ctx, amap, L, p, smem_bytes, st) \
-                   : p.resident            ? launch<BN, 64, 2, true>(ctx, amap, L, p, smem_bytes, st) \
-                   : p.halo                ? launch<BN, 64, 1, true>(ctx, amap, L, p, smem_bytes, st) \
-                                           : launch<BN, 64, 0, true>(ctx, amap, L, p, smem_bytes, st); \
-    return rc == kRetrySingle ? conv_tc_run(ctx, L, in, out, out_f32, st, pool_out, write_full, tail, up_add) : rc; \
-  }
-  B2O_TC_PAIR_CASE(64); B2O_TC_PAIR_CASE(128); B2O_TC_PAIR_CASE(256);
+  B2O_TC_PAIR_CASE(64); B2O_TC_PAIR_CASE(128);
 #undef B2O_TC_PAIR_CASE
 #define B2O_TC_CASE(BN, KC)                                                            \
   if (bn == BN && kch == KC) {                                                         \
-    if (p.resident && p.group) return launch<BN, KC, 3, false>(ctx, amap, L, p, smem_bytes, st); \
     if (p.resident) return launch<BN, KC, 2, false>(ctx, amap, L, p, smem_bytes, st);  \
     if (p.halo) return launch<BN, KC, 1, false>(ctx, amap, L, p, smem_bytes, st);      \
     return launch<BN, KC, 0, false>(ctx, amap, L, p, smem_bytes, st);                  \
   }
-  B2O_TC_CASE(16, 64); B2O_TC_CASE(32, 64); B2O_TC_CASE(64, 64); B2O_TC_CASE(128, 64); B2O_TC_CASE(256, 64);
+  B2O_TC_CASE(16, 64); B2O_TC_CASE(32, 64); B2O_TC_CASE(64, 64); B2O_TC_CASE(128, 64);
   B2O_TC_CASE(16, 32); B2O_TC_CASE(32, 32);
   B2O_TC_CASE(32, 16); B2O_TC_CASE(64, 16);
 #undef B2O_TC_CASE
   ctx->set_error("conv_tc_run: no kernel instance for " + L.name);
   return B2O_ERR_ARG;
-}
-
-extern "C" int b2o_debug_read_tc(unsigned long long* out_host, int n) {
-  if (!out_host || n <= 0 || n > 160 * 8) return B2O_ERR_ARG;
-  return cudaMemcpyFromSymbol(out_host, g_tc_debug, static_cast<size_t>(n) * sizeof(unsigned long long)) == cudaSuccess
-             ? B2O_OK : B2O_ERR_CUDA;
 }

@@ -142,9 +142,9 @@ __device__ __forceinline__ void mma_m16n8k16(float* d, const uint32_t* a, uint32
 // shape with the crops as N: warp w owns units 8w..8w+7 and keeps its two 16-row slices of U^T
 // ({i,f} gates and {c,o} gates of those units, all 128 k) in registers for the whole sequence; the D fragment
 // then hands every thread all four gates of one unit for two crops, so the gate arithmetic needs no exchange
-// and the only shared data is the fp16 h vector (double-buffered, one __syncthreads per step).  tcgen05 does
-// not apply: M = 128 rows would be 94 % padding and its issue -> commit -> tcgen05.ld round trip is longer
-// than this whole step.  h is rounded to fp16 between steps -- the same value that is written to `out`.
+// and the only shared data is the fp16 h vector (double-buffered, one __syncthreads per step).  wgmma does
+// not apply: M = 64 rows would be mostly padding and its issue -> commit -> wait round trip is longer than this
+// whole step.  h is rounded to fp16 between steps -- the same value that is written to `out`.
 // xw  : (B*T, xw_ld) fp32 input projections x@W + b; this direction's 512 gate columns start at xw_off
 // u   : (128, 512) fp16 recurrent kernel (row k = previous-h unit, column g = gate; Keras order i,f,c,o)
 // out : (B, T, out_ld) fp16, written at channel offset out_off, indexed by PROCESSING step

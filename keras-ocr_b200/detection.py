@@ -33,7 +33,7 @@ def _as_device_images(images, device):
 
 
 class Detector:
-    """A text detector using the CRAFT architecture, running as sm_100a CUDA kernels.
+    """A text detector using the CRAFT architecture, running as sm_90a CUDA kernels.
 
     Args:
         weights: ``"clovaai_general"`` (reads ``craft_mlt_25k.pth`` from the keras-ocr cache dir),
@@ -49,7 +49,7 @@ class Detector:
         if backbone_name != "vgg":
             raise NotImplementedError
         if not torch.cuda.is_available():
-            raise _lib.B2OError("keras-ocr_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.B2OError("keras-ocr_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device_index = torch.cuda.current_device() if device is None else int(device)
         self.device = torch.device("cuda", self.device_index)
         if isinstance(weights, dict):

@@ -205,8 +205,7 @@ def _decode_blocks_impl(blocks, max_boxes, alphabet, recognition):
 
 class ShardedStream:
     """``recognize_sharded`` for a STREAM of batches, software-pipelined one batch deep: while every rank's GPU works
-    on batch k, rank 0 decodes the gathered words of batch k-1 (the only serial host work of the multi-GPU path:
-    ~3 ms for 8 x 1028 words).  Every rank passes its own, equally long, slice of each batch.
+    on batch k, rank 0 decodes the gathered words of batch k-1 (the only serial host work of the multi-GPU path).  Every rank passes its own, equally long, slice of each batch.
 
         stream = ShardedStream(pipeline)
         for batch in batches:
@@ -269,9 +268,9 @@ class ShardedStream:
 
     def _gather_on_side_stream(self, local, max_boxes):
         """The gather and rank 0's copy to the host run on a SIDE stream that waits for this batch's records; the compute
-        stream is never made to wait for another rank (with the collective on the compute stream, rank 0's next batch queued
-        behind a gather that completes only when the slowest rank has sent: measured on 8 GPUs, rank 0 66.0 ms per step against
-        62.4-65.0 for the others, profiles/r2scale8_bench_8gpu.json)."""
+        stream is never made to wait for another rank (with the collective on the compute stream, rank 0's next batch would
+        queue behind a gather that completes only when the slowest rank has sent, so rank 0 would run at the pace of the
+        slowest rank plus its own decode)."""
         main = torch.cuda.current_stream(local.device)
         if self._side is None:
             self._side = torch.cuda.Stream(device=local.device)

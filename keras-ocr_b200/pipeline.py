@@ -33,8 +33,8 @@ class Pipeline:
         # software-pipelined on one stream: while the host waits for the box counts of one sub-batch (the path's
         # one data-dependent synchronisation) or decodes its labels, the GPU already runs the next one.  Results
         # are identical to the unsplit batch (images are independent; the padding is that of the whole batch).
-        # Measured on the 32-page bench: ~2 % faster device-resident, but the half-size recurrent / box kernels
-        # lose what the overlap gains and the end-to-end number does not move, hence the default of 1.
+        # The half-size sub-batches run the recurrent / box kernels less efficiently, which eats what the overlap gains,
+        # hence the default of 1.
         self.inflight = inflight
         # gpu_decode: JPEG files / buffers in ``images`` are decoded by nvJPEG into device memory (tools.read_device)
         # instead of cv2 on the host (reference tools.py:19-38); pixels may differ from libjpeg's by a few levels, which is

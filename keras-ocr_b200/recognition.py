@@ -35,7 +35,7 @@ def labels_to_text(rows, alphabet=DEFAULT_ALPHABET):
 
 
 class Recognizer:
-    """A text recognizer using the CRNN architecture, running as sm_100a CUDA kernels.
+    """A text recognizer using the CRNN architecture, running as sm_90a CUDA kernels.
 
     Args:
         alphabet: the characters the model recognises (default ``0-9a-z``; up to 1023 characters).  The
@@ -63,7 +63,7 @@ class Recognizer:
             changed = sorted(k for k in params if params[k] != DEFAULT_BUILD_PARAMS.get(k))
             raise NotImplementedError(f"build_params other than the defaults are not supported by the CUDA recognizer: {changed}")
         if not torch.cuda.is_available():
-            raise _lib.B2OError("keras-ocr_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.B2OError("keras-ocr_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.alphabet = alphabet or DEFAULT_ALPHABET              # recognition.py:369-375
         if len(self.alphabet) + 1 > _lib.MAX_CLASSES:
             raise ValueError(f"alphabet too long: at most {_lib.MAX_CLASSES - 1} characters")

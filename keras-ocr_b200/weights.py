@@ -153,8 +153,8 @@ def synthetic_crnn_weights(seed=1, alphabet=ALPHABET, decisive=False, stn=True, 
     ``stn=False``: no spatial-transformer tensors (the ``build_model(stn=False)`` variant, recognition.py:196, 243).
     ``decisive=True`` (default alphabet, gray, with STN; ``seed`` is ignored): every tensor comes from
     ``data/crnn_hershey.npz`` -- the reference architecture TRAINED with CTC loss on words rendered in cv2's Hershey font
-    and cut out as the oracle pipeline cuts them (``oracle/train_crnn_full.py``; 3.5 minutes on one B200; no pretrained file
-    involved).  It reads the synthetic pages (99.7 % of unseen synthetic crops, 100 % of the crops of pages it never saw), its
+    and cut out as the oracle pipeline cuts them (``oracle/train_crnn_full.py``; a few minutes on one GPU; no pretrained file
+    involved).  It reads the synthetic pages (the bench reads 1020 of its 1024 rendered words), its
     per-step argmax is decided by a wide margin and its strings do not change when a box moves by a pixel, so decoded
     strings can be compared for identity (BASELINE.json north_star) instead of up to the near-ties random weights leave."""
     if decisive:

@@ -5,7 +5,7 @@ package (``keras-ocr_b200/``).  Only ``tests/``, ``__graft_entry__.smoke()`` and
 ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs may import it, and
 only as the checker / the CPU baseline.
 
-Every function restates one piece of the reference (``/root/reference``,
+Every function restates one piece of the reference (keras-ocr,
 faustomorales/keras-ocr @ 9661d6f) and cites the file:line it follows.  The
 restatement is validated in the authoring container against the reference's own
 code by ``oracle/validate_against_reference.py`` (which AST-lifts the reference

@@ -1,5 +1,5 @@
 """Train the whole CRNN recognizer on rendered words -- TEST INFRASTRUCTURE, meant to run where torch has a GPU
-(``gpurun -- python -m oracle.train_crnn_full``; a few minutes on one B200, PyTorch/cuDNN doing the training arithmetic).
+(``python -m oracle.train_crnn_full`` on a CUDA machine; a few minutes on one GPU, PyTorch/cuDNN doing the training arithmetic).
 
 (An earlier fixture fitted only the head on frozen random features: it memorised its pages and its strings changed when a
 box moved by a pixel.)  This script trains every layer of the reference architecture (``build_model``,

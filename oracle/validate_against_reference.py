@@ -102,8 +102,9 @@ def check_craft(det, out):
 def check_craft_c2(det, out):
     """BASELINE.json configs[1] at its own size: CRAFT on 8 x 768 x 768 (seeded uint8 noise, weights seed 3) through
     the reference's own PyTorch CRAFT (``build_torch_model``, detection.py:472-644).  The fp32 score maps (8,384,384,2)
-    are committed as float16 (4.7 MB; quantisation 5e-4 of the range, the GPU comparison allows 2e-2); the input is
-    regenerated from its seed by the test.  The oracle restatement is checked on the first two images."""
+    are committed as float16 at a fixed seeded sample of C2_PIXELS pixel positions per image (the same positions in every
+    image, both channels; quantisation 5e-4 of the range, the GPU comparison allows 2e-2); the input is regenerated from
+    its seed by the test, which runs the whole batch and compares it at those positions.  The oracle restatement is checked on the first two images."""
     torch.manual_seed(0)
     model = det.build_torch_model(None)
     wts = W.synthetic_craft_weights(seed=3)
@@ -124,9 +125,20 @@ def check_craft_c2(det, out):
                 assert err < 1e-4, err
     scores = np.concatenate(scores)
     print(f"  CRAFT C2: scores {scores.shape}, range [{scores.min():.3f}, {scores.max():.3f}]")
+    pixels = c2_pixels(seed, scores.shape[1] * scores.shape[2])
+    sample = scores.reshape(scores.shape[0], -1, scores.shape[3])[:, pixels]
     out["craft_c2_seed"] = np.array(seed)
-    out["craft_c2_scores_f16"] = scores.astype(np.float16)
-    out["craft_c2_checksum"] = np.array([float(scores.astype(np.float64).sum()), float(np.abs(scores).astype(np.float64).sum())])
+    out["craft_c2_pixels"] = pixels
+    out["craft_c2_scores_f16"] = sample.astype(np.float16)
+    out["craft_c2_checksum"] = np.array([float(sample.astype(np.float64).sum()), float(np.abs(sample).astype(np.float64).sum())])
+
+
+C2_PIXELS = 16384
+
+
+def c2_pixels(seed, n):
+    """The sampled pixel positions (flat h * w index, sorted) of the C2 fixture."""
+    return np.sort(np.random.default_rng(seed + 1).choice(n, C2_PIXELS, replace=False)).astype(np.int32)
 
 
 def check_boxes(det, out):
@@ -179,7 +191,7 @@ def check_warp(tools, out):
 
 def check_inputs(tools, out):
     rng = np.random.default_rng(31)
-    for tag, (h, w, scale, max_size) in {"x2": (120, 160, 2, 2048), "capped": (300, 500, 2, 800), "x3": (77, 93, 3, 2048)}.items():
+    for tag, (h, w, scale, max_size) in {"x2": (120, 160, 2, 2048), "capped": (150, 250, 2, 400), "x3": (77, 93, 3, 2048)}.items():
         img = cv2.GaussianBlur(rng.integers(0, 256, (h, w, 3)).astype(np.float32), (0, 0), 1.2).clip(0, 255).astype(np.uint8)
         ref, s_ref = tools.resize_image(img, max_scale=scale, max_size=max_size)
         mine, s_mine = o_img.resize_image(img, scale, max_size)

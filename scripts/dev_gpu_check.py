@@ -31,7 +31,7 @@ def main():
     det = Detector(weights=W.synthetic_craft_weights(3))
     rng = np.random.default_rng(0)
     img = torch.from_numpy(rng.integers(0, 256, (n, h, w, 3), dtype=np.uint8)).cuda()
-    for name, eng in (("tcgen05", _lib.CONV_AUTO),) + ((("simt", _lib.CONV_SIMT),) if os.environ.get("SIMT") else ()):
+    for name, eng in (("tc", _lib.CONV_AUTO),) + ((("simt", _lib.CONV_SIMT),) if os.environ.get("SIMT") else ()):
         det.ctx.set_conv_engine(eng)
         try:
             ms = timeit(lambda: det.predict_device(img), 2, iters)

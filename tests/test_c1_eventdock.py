@@ -5,7 +5,7 @@ prediction, ``"eventdock"``; a blank image -> no prediction.
 Neither weight file exists offline (no network, SURVEY.md 8(c)), so the test SKIPS unless they are present in the
 keras-ocr cache directory (``~/.keras-ocr`` or ``$KERAS_OCR_CACHE_DIR``, reference tools.py:495-498) with the reference's
 sha256 digests (detection.py:647-658, recognition.py:27-44), and unless the reference's test image can be found
-(``$KERAS_OCR_TEST_IMAGE``, or the reference checkout).  Everything between the files and the assertion is the product
+(``$KERAS_OCR_TEST_IMAGE``, or the copy in ``tests/golden/test_image.jpg``).  Everything between the files and the assertion is the product
 path: ``weights.load_craft_pth`` (torch.load), ``hdf5.read_datasets`` (own HDF5 reader), the CUDA pipeline."""
 import os
 
@@ -21,8 +21,7 @@ CRNN = ("crnn_kurapan.h5", "a7d8086ac8f5c3d6a0a828f7d6fbabcaf815415dd125c3253301
 
 
 def _test_image():
-    for path in (os.environ.get("KERAS_OCR_TEST_IMAGE"), "/root/reference/tests/test_image.jpg",
-                 os.path.join(os.path.dirname(__file__), "golden", "test_image.jpg")):
+    for path in (os.environ.get("KERAS_OCR_TEST_IMAGE"), os.path.join(os.path.dirname(__file__), "golden", "test_image.jpg")):
         if path and os.path.isfile(path):
             return path
     return None

@@ -1,5 +1,5 @@
 """GPU parity tests: every CUDA stage, called through the C-ABI, against the CPU oracle and the
-golden vectors generated from the reference.  Run on the B200 box: ``pytest tests -m gpu``.
+golden vectors generated from the reference.  Run on an H100: ``pytest tests -m gpu``.
 
 Tolerances (stated per test): integer/byte/index work is bit-exact; fp16 tensor-core stages are
 compared with the fp32 oracle at the tolerances proposed in SURVEY.md 8(c).
@@ -51,16 +51,18 @@ CONV_CASES = [
     (2, 50, 7, 512, 512, 3, 1, 1, 1),       # CRNN conv_7: ReLU then BN affine
     (1, 1, 300, 3584, 128, 1, 1, 1, 0),     # fc_9 as a 1x1 conv over rows
     (1, 8, 8, 1536, 512, 1, 1, 1, 0),       # upconv1.conv.0
-    (1, 96, 96, 64, 64, 3, 1, 1, 0),        # many tiles per CTA (persistent loop, both TMEM stages)
+    (1, 96, 96, 64, 64, 3, 1, 1, 0),        # many tiles per CTA (persistent loop, the stage ring wraps)
     (2, 40, 48, 32, 32, 3, 1, 1, 0),        # conv_cls.0: 32-channel K chunk (64B swizzle), resident filters
     (1, 33, 29, 32, 16, 3, 1, 1, 0),        # conv_cls.4, ragged halo tiles
     (2, 50, 7, 16, 32, 5, 1, 1, 0),         # STN conv_b: 16-channel K chunk (32B swizzle), 5x5
     (1, 48, 40, 128, 128, 3, 1, 1, 0),      # halo tiles with a streamed (non-resident) filter bank
-    (1, 32, 24, 256, 512, 3, 1, 1, 0),      # halo tiles, two n-tiles of 256
+    (1, 32, 24, 256, 512, 3, 1, 1, 0),      # halo tiles, four n-tiles of 128
     (2, 40, 56, 16, 64, 3, 1, 1, 0),        # tensor-core stem shape: 16-channel chunk, resident filters
 ]
 
 ENGINES = [_lib.CONV_SIMT, _lib.CONV_TC_GENERIC, _lib.CONV_AUTO]
+# ids kept from the first tensor-core engine (tcgen05) so that test ids stay stable: "tcgen05_generic" = the tensor-core
+# engine without halo tiles (B2O_CONV_TC_GENERIC), "tcgen05" = the product path (B2O_CONV_AUTO, wgmma on sm_90a)
 ENGINE_IDS = ["simt", "tcgen05_generic", "tcgen05"]
 
 
@@ -811,8 +813,8 @@ def test_crnn_batch256_labels_do_not_depend_on_the_batch(recognizer):
 
 
 def test_cta_pairs_give_bit_identical_results(cuda_device, monkeypatch):
-    """The CTA-pair convolution path (tcgen05 cta_group::2, the default) and the single-CTA path (B2O_TC_PAIR=0, read at
-    context creation) add every output's terms in the same order: score maps and CRNN logits are bit-identical, for
+    """The CTA-pair convolution path (2-CTA clusters sharing B tiles by TMA multicast, B2O_TC_PAIR=1) and the single-CTA
+    path (B2O_TC_PAIR=0, the default; read at context creation) add every output's terms in the same order: score maps and CRNN logits are bit-identical, for
     even and odd numbers of tile columns (the odd one leaves the second CTA of the last pair on a dummy tile)."""
     from keras_ocr_b200.detection import Detector
     from keras_ocr_b200.recognition import Recognizer
@@ -865,16 +867,11 @@ def test_decoder_commute_matches_explicit_upsample(cuda_device, monkeypatch, gol
         assert err <= 2e-2, err
 
 
-@pytest.mark.parametrize("switch", [("B2O_TC_BOX16", "0"), ("B2O_TC_BOX16", "10"), ("B2O_TC_BOX16", "16"), ("B2O_TC_BOX_ALL", "1"), ("B2O_TC_PAIR", "2"),
-                                    ("B2O_FUSED_TAIL", "0"), ("B2O_TC_AFF", "smem"), ("B2O_GLUE", "v1")],
-                         ids=["three_boxes_vs_single_box", "box_width_10", "box_width_16", "single_box_everywhere", "generic_pairs", "separate_head_tail",
-                              "epilogue_constants_in_smem", "round1_upsample2x"])
+@pytest.mark.parametrize("switch", [("B2O_TC_PAIR", "2"), ("B2O_FUSED_TAIL", "0"), ("B2O_TC_AFF", "smem"), ("B2O_GLUE", "v1")],
+                         ids=["generic_pairs", "separate_head_tail", "epilogue_constants_in_smem", "round1_upsample2x"])
 def test_conv_variants_are_bit_identical(cuda_device, monkeypatch, switch):
     """Kernel variants that keep the MMA / fmaf order of the default path must not change a bit of the CRAFT score
-    maps or the CRNN logits:  B2O_TC_BOX16=0 -- three 8 x 18 A boxes per K chunk instead of the default single
-    box (dx taps through the descriptor start address), =10 / =16 -- the width of that box (image rows then start inside
-    a swizzle atom), B2O_TC_BOX_ALL=1 -- single boxes in every grouped layer;  B2O_TC_PAIR=2 -- CTA pairs on the generic tiles too;
-    B2O_FUSED_TAIL=0 -- conv_cls.6 / conv_cls.8 as the separate head_tail_kernel instead of conv_cls.4's epilogue;
+    maps or the CRNN logits:  B2O_TC_PAIR=2 -- CTA pairs on the generic tiles too;  B2O_FUSED_TAIL=0 -- conv_cls.6 / conv_cls.8 as the separate head_tail_kernel instead of conv_cls.4's epilogue;
     B2O_TC_AFF=smem -- the per-channel epilogue constants staged in shared memory / read from global memory (round 1)
     instead of the kernel-parameter constant bank;  B2O_GLUE=v1 -- the round-1 2x upsampling kernel (64-bit index chain, each output
     pixel blending its four taps on its own) instead of the one that shares a quad column's two horizontal blends.
