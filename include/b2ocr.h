@@ -180,6 +180,38 @@ int b2o_conv2d_test(b2o_ctx* ctx, const void* x_dev, int n, int h, int w, int ci
                     const float* s2_host, const float* t2_host, void* out_dev, int engine,
                     void* stream);
 
+/* One convolution with every epilogue feature the networks use (test hook, not on the product path).  Every "_dev"
+ * pointer addresses channel 0 of a channel slice of a wider NHWC buffer whose channel stride is the matching "_ld".
+ *   x      (n,h,w,cin) fp16, x_ld >= cin.  wgt (cout,k,k,cin) fp32 host; y = relu?(acc*s1+t1)*s2+t2 (s2/t2 may be NULL).
+ *   out    (n,h,w,cout), fp32 when out_f32 else fp16, out_ld >= cout; write_full = 0 skips it where the pool is fused.
+ *   pool   optional (n,h/2,w/2,cout) fp16 2x2/2 max pool of the output (floor for odd sizes), pool_ld >= cout.
+ *   up     optional (n,h/2,w/2,cout) fp16 whose exact-2x bilinear upsampling is added to the accumulator before the
+ *          epilogue (the commuted decoder upsampling; tensor-core engines only).
+ *   tail   optional CRAFT head tail (16-channel layers): w6 (16 in,16 out), b6 (16), w8 (16 in,2 out), b8 (2) fp32 host;
+ *          scores (n,h,w,2) fp32.  B2O_CONV_AUTO fuses it into the conv epilogue when the layer allows, as
+ *          b2o_craft_forward does; other engines run the separate head_tail kernel on `out`.
+ * Plain and pooled layers are routed as b2o_craft_forward / b2o_crnn_forward route them for the given engine.
+ * Synchronises the stream before returning.                                                              */
+typedef struct {
+  const void* x_dev;
+  int n, h, w, cin, x_ld;
+  const float* wgt_host;
+  int cout, ksize, dilation;
+  const float *s1_host, *t1_host;
+  int relu;
+  const float *s2_host, *t2_host;
+  void* out_dev;
+  int out_ld, out_f32, write_full;
+  void* pool_dev;
+  int pool_ld;
+  const void* up_dev;
+  int up_ld;
+  const float *w6_host, *b6_host, *w8_host, *b8_host;
+  float* scores_dev;
+  int engine;
+} b2o_conv_test_desc;
+int b2o_conv_test(b2o_ctx* ctx, const b2o_conv_test_desc* desc, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

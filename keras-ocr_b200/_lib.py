@@ -27,6 +27,18 @@ class _Tensor(ctypes.Structure):
 
 _c = ctypes
 _vp, _i, _f, _sz = _c.c_void_p, _c.c_int, _c.c_float, _c.c_size_t
+_fp = _c.POINTER(_c.c_float)
+
+
+class _ConvTestDesc(ctypes.Structure):
+    """b2o_conv_test_desc (include/b2ocr.h), field for field."""
+    _fields_ = [("x_dev", _vp), ("n", _i), ("h", _i), ("w", _i), ("cin", _i), ("x_ld", _i),
+                ("wgt_host", _fp), ("cout", _i), ("ksize", _i), ("dilation", _i),
+                ("s1_host", _fp), ("t1_host", _fp), ("relu", _i), ("s2_host", _fp), ("t2_host", _fp),
+                ("out_dev", _vp), ("out_ld", _i), ("out_f32", _i), ("write_full", _i),
+                ("pool_dev", _vp), ("pool_ld", _i), ("up_dev", _vp), ("up_ld", _i),
+                ("w6_host", _fp), ("b6_host", _fp), ("w8_host", _fp), ("b8_host", _fp), ("scores_dev", _vp),
+                ("engine", _i)]
 
 # name -> (restype, argtypes); mirrors include/b2ocr.h one to one
 SIGNATURES = {
@@ -63,6 +75,7 @@ SIGNATURES = {
     "b2o_conv2d_test": (_i, [_vp, _vp, _i, _i, _i, _i, _c.POINTER(_c.c_float), _i, _i, _i,
                              _c.POINTER(_c.c_float), _c.POINTER(_c.c_float), _i,
                              _c.POINTER(_c.c_float), _c.POINTER(_c.c_float), _vp, _i, _vp]),
+    "b2o_conv_test": (_i, [_vp, _c.POINTER(_ConvTestDesc), _vp]),
 }
 
 _lib = None
@@ -229,6 +242,17 @@ class Context:
         self._check(self.lib.b2o_conv2d_test(self.handle, x, n, h, w, cin, _fptr(wgt), cout, ksize, dilation, _fptr(s1),
                                              _fptr(t1), int(relu), _fptr(s2), _fptr(t2), out, engine, stream),
                     "b2o_conv2d_test")
+
+    def conv_test(self, x, n, h, w, cin, x_ld, wgt, cout, ksize, dilation, s1, t1, relu, s2, t2, out, out_ld, engine,
+                  stream, out_f32=False, write_full=True, pool=None, pool_ld=0, up=None, up_ld=0, tail=None, scores=None):
+        """b2o_conv_test: device pointers are ints (channel 0 of their slice); ``tail`` = (w6 (16,16), b6, w8 (16,2), b8)
+        host arrays, ``scores`` the device pointer of the (n,h,w,2) fp32 output."""
+        keep = [np.ascontiguousarray(a, np.float32) if a is not None else None for a in (wgt, s1, t1, s2, t2)]
+        tail = [np.ascontiguousarray(a, np.float32) for a in tail] if tail is not None else [None] * 4
+        d = _ConvTestDesc(x, n, h, w, cin, x_ld, _fptr(keep[0]), cout, ksize, dilation, _fptr(keep[1]), _fptr(keep[2]),
+                          int(relu), _fptr(keep[3]), _fptr(keep[4]), out, out_ld, int(out_f32), int(write_full),
+                          pool, pool_ld, up, up_ld, *[_fptr(a) for a in tail], scores, engine)
+        self._check(self.lib.b2o_conv_test(self.handle, ctypes.byref(d), stream), "b2o_conv_test")
 
 
 _contexts = {}

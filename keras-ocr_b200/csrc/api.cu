@@ -727,3 +727,96 @@ extern "C" int b2o_conv2d_test(b2o_ctx* ctx, const void* x, int n, int h, int w,
   while (ctx->owned.size() > owned_before) { cudaFree(ctx->owned.back()); ctx->owned.pop_back(); }
   return rc;
 }
+
+namespace {
+
+// The body of b2o_conv_test: builds the layer(s) like b2o_load_craft / b2o_load_crnn do and routes the launch like
+// b2o_craft_forward / b2o_crnn_forward.  The caller frees what build_layer allocated.
+int conv_test_run(b2o_ctx* ctx, const b2o_conv_test_desc& d, cudaStream_t st) {
+  const int cin = d.cin, k = d.ksize;
+  if (!d.x_dev || !d.wgt_host || !d.s1_host || !d.t1_host || !d.out_dev || d.n <= 0 || d.h <= 0 || d.w <= 0 ||
+      cin <= 0 || d.cout <= 0 || k <= 0 || d.dilation <= 0 || d.x_ld < cin || d.out_ld < d.cout ||
+      (d.pool_dev && d.pool_ld < d.cout) || (d.up_dev && d.up_ld < d.cout) || (!d.s2_host) != (!d.t2_host)) {
+    ctx->set_error("b2o_conv_test: bad argument");
+    return B2O_ERR_ARG;
+  }
+  // the vector loads and stores of every engine (and of maxpool2_kernel) need 16-byte aligned pixels
+  auto misaligned = [](const void* p, int ld, int elems) { return (reinterpret_cast<uintptr_t>(p) & 15) || (ld % elems); };
+  if (cin % 8 || misaligned(d.x_dev, d.x_ld, 8) || misaligned(d.out_dev, d.out_ld, d.out_f32 ? 4 : 8) ||
+      (d.pool_dev && (d.cout % 8 || d.out_f32 || misaligned(d.pool_dev, d.pool_ld, 8)))) {
+    ctx->set_error("b2o_conv_test: misaligned view");
+    return B2O_ERR_ARG;
+  }
+  const bool tail = d.scores_dev != nullptr;
+  if (tail && (!d.w6_host || !d.b6_host || !d.w8_host || !d.b8_host || d.cout != 16 || d.pool_dev || d.out_f32)) {
+    ctx->set_error("b2o_conv_test: the tail needs a 16-channel fp16 layer without pool");
+    return B2O_ERR_ARG;
+  }
+  if (d.up_dev && d.engine == B2O_CONV_SIMT) {
+    ctx->set_error("b2o_conv_test: upsample-add runs on the tensor-core engine only");
+    return B2O_ERR_ARG;
+  }
+  ConvLayer L;
+  const float* wgt = d.wgt_host;
+  auto wget = [wgt, cin, k](int o, int c, int ky, int kx) {
+    return wgt[((static_cast<size_t>(o) * k + ky) * k + kx) * cin + c];
+  };
+  std::vector<float> s1(d.s1_host, d.s1_host + d.cout), t1(d.t1_host, d.t1_host + d.cout), s2, t2;
+  if (d.s2_host) { s2.assign(d.s2_host, d.s2_host + d.cout); t2.assign(d.t2_host, d.t2_host + d.cout); }
+  B2O_RETURN_IF(build_layer(ctx, L, "test", cin, d.cout, k, d.dilation, d.relu, wget, s1, t1, d.s2_host ? &s2 : nullptr,
+                            d.s2_host ? &t2 : nullptr, false));
+  const TensorView in = make_view(const_cast<void*>(d.x_dev), d.n, d.h, d.w, cin, d.x_ld);
+  TensorView out = make_view(d.out_dev, d.n, d.h, d.w, d.cout, d.out_ld);
+  ctx->conv_engine = d.engine;
+  if (d.up_dev) {                         // conv_tc_run checks the layer and the views (tail / pool / fp32 are refused)
+    const TensorView up = make_view(const_cast<void*>(d.up_dev), d.n, d.h / 2, d.w / 2, d.cout, d.up_ld);
+    const TensorView pool = d.pool_dev ? make_view(d.pool_dev, d.n, d.h / 2, d.w / 2, d.cout, d.pool_ld) : TensorView();
+    ConvTail none = {nullptr, nullptr, nullptr, nullptr, d.scores_dev};
+    return conv_tc_run(ctx, L, in, out, d.out_f32, st, d.pool_dev ? &pool : nullptr, 1, tail ? &none : nullptr, &up);
+  }
+  if (tail) {
+    // conv_cls.6 (16 -> 16, ReLU) and conv_cls.8 (16 -> 2) built as b2o_load_craft builds them; w6 / w8 are (in, out)
+    ConvLayer L6, L8;
+    const float *w6 = d.w6_host, *w8 = d.w8_host;
+    auto g6 = [w6](int o, int c, int, int) { return w6[c * 16 + o]; };
+    auto g8 = [w8](int o, int c, int, int) { return w8[c * 2 + o]; };
+    B2O_RETURN_IF(build_layer(ctx, L6, "test.6", 16, 16, 1, 1, 1, g6, ones(16), std::vector<float>(d.b6_host, d.b6_host + 16),
+                              nullptr, nullptr, false));
+    B2O_RETURN_IF(build_layer(ctx, L8, "test.8", 16, 2, 1, 1, 0, g8, ones(2), std::vector<float>(d.b8_host, d.b8_host + 2),
+                              nullptr, nullptr, false));
+    if (ctx->conv_engine == B2O_CONV_AUTO && L.block_n == 16 && !ctx->no_fused_tail) {      // as b2o_craft_forward
+      ConvTail ct = {L6.w_simt, L6.t1, L8.w_simt, L8.t1, d.scores_dev};
+      if (L6.h_w_simt.size() == 256 && L8.h_w_simt.size() == 32) {
+        ct.h_w6 = L6.h_w_simt.data(); ct.h_b6 = L6.h_t1.data(); ct.h_w8 = L8.h_w_simt.data(); ct.h_b8 = L8.h_t1.data();
+      }
+      return conv_tc_run(ctx, L, in, out, 0, st, nullptr, 1, &ct);
+    }
+    B2O_RETURN_IF(conv_run(ctx, L, in, out, 0, st));
+    return head_tail_run(ctx, L6, L8, out, d.scores_dev, st);
+  }
+  if (d.pool_dev) {
+    const TensorView pool = make_view(d.pool_dev, d.n, d.h / 2, d.w / 2, d.cout, d.pool_ld);
+    return conv_run(ctx, L, in, out, d.out_f32, st, &pool, d.write_full);
+  }
+  return conv_run(ctx, L, in, out, d.out_f32, st);
+}
+
+}  // namespace
+
+extern "C" int b2o_conv_test(b2o_ctx* ctx, const b2o_conv_test_desc* desc, void* stream) {
+  if (!ctx || !desc) return B2O_ERR_ARG;
+  if (desc->engine != B2O_CONV_AUTO && desc->engine != B2O_CONV_SIMT && desc->engine != B2O_CONV_TC_GENERIC) {
+    ctx->set_error("b2o_conv_test: unknown engine");
+    return B2O_ERR_ARG;
+  }
+  DeviceGuard guard(ctx->device);
+  const size_t owned_before = ctx->owned.size();
+  const int saved = ctx->conv_engine;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int rc = conv_test_run(ctx, *desc, st);
+  ctx->conv_engine = saved;
+  cudaError_t e = cudaStreamSynchronize(st);
+  if (rc == B2O_OK && e != cudaSuccess) { ctx->set_error(std::string("b2o_conv_test: ") + cudaGetErrorString(e)); rc = B2O_ERR_CUDA; }
+  while (ctx->owned.size() > owned_before) { cudaFree(ctx->owned.back()); ctx->owned.pop_back(); }
+  return rc;
+}
