@@ -117,6 +117,14 @@ int b2o_get_boxes(b2o_ctx* ctx, const float* scores_dev, int n, int hs, int ws,
                   float detection_threshold, float text_threshold, float link_threshold,
                   int size_threshold, float* boxes_dev, int32_t* counts_dev, int max_boxes,
                   void* ws_dev, size_t ws_bytes, void* stream);
+/* The same, and box_scores_dev (n, max_boxes) float32 receives each stored box's detection score, in box order: the
+ * largest text-channel value (channel 0 of scores) over the box's connected component -- the value compared with
+ * detection_threshold (detection.py:240-241), so every kept box scores >= detection_threshold.  It is a max over the
+ * map's own floats, hence exact.  box_scores_dev == NULL behaves as b2o_get_boxes.                            */
+int b2o_get_boxes_scored(b2o_ctx* ctx, const float* scores_dev, int n, int hs, int ws,
+                         float detection_threshold, float text_threshold, float link_threshold,
+                         int size_threshold, float* boxes_dev, int32_t* counts_dev, float* box_scores_dev,
+                         int max_boxes, void* ws_dev, size_t ws_bytes, void* stream);
 
 /* The box bookkeeping of recognize_from_boxes (recognition.py:511-521: crops are appended image after
  * image, start_end = running offsets) on the device: the (n,max_boxes,4,2) table of b2o_get_boxes becomes
@@ -150,6 +158,14 @@ int b2o_crops_to_input(b2o_ctx* ctx, const uint8_t* crops_dev, int b, void* crnn
 int b2o_crops_to_input_color(b2o_ctx* ctx, const uint8_t* crops_dev, int b, void* crnn_in_dev, void* stream);
 int b2o_crnn_forward(b2o_ctx* ctx, const void* crnn_in_dev, int b, int32_t* labels_dev,
                      void* ws_dev, size_t ws_bytes, void* stream);
+/* The same labels, and logp_dev (b) float32 receives each crop's greedy-path log-probability
+ * S = sum over the 48 kept steps t of log(max_c p[t,c] + 1e-7), p = softmax of fc_12 (recognition.py:322-328).
+ * exp(S) in (0, 1] is the word's confidence; per TensorFlow's documentation S is minus the second output of
+ * keras.backend.ctc_decode(greedy=True), which CTCDecoder drops (recognition.py:175) -- that link is not pinned
+ * against TensorFlow.  S of a crop is bit-reproducible and does not depend on the batch it runs in.  logp_dev == NULL
+ * behaves as b2o_crnn_forward.                                                                                */
+int b2o_crnn_forward_scored(b2o_ctx* ctx, const void* crnn_in_dev, int b, int32_t* labels_dev, float* logp_dev,
+                            void* ws_dev, size_t ws_bytes, void* stream);
 
 /* Result records of Pipeline.recognize for the multi-GPU gather (pipeline.py:66-75; SURVEY.md 8(e)): one
  * fixed-size float32 row per image = [count][rec_boxes x (4,2) boxes * inv_scale[i] (tools.adjust_boxes,
@@ -161,6 +177,14 @@ size_t b2o_record_floats(int rec_boxes);
 int b2o_pack_records(b2o_ctx* ctx, const float* boxes_dev, const int32_t* counts_dev, const int32_t* labels_dev,
                      const float* inv_scale_dev, int n, int max_boxes, int rows, int rec_boxes,
                      float* records_dev, void* stream);
+/* Scored records: the unscored record above, unchanged, followed by [rec_boxes detection scores][rec_boxes path
+ * log-probabilities S], b2o_record_floats_scored(rec_boxes) = b2o_record_floats(rec_boxes) + 2 * rec_boxes floats.
+ * box_scores (n, max_boxes) as written by b2o_get_boxes_scored; logp (sum counts) as written by
+ * b2o_crnn_forward_scored (NULL when no image has a box).  Slots past an image's words hold 0.                */
+size_t b2o_record_floats_scored(int rec_boxes);
+int b2o_pack_records_scored(b2o_ctx* ctx, const float* boxes_dev, const int32_t* counts_dev, const int32_t* labels_dev,
+                            const float* box_scores_dev, const float* logp_dev, const float* inv_scale_dev, int n,
+                            int max_boxes, int rows, int rec_boxes, float* records_dev, void* stream);
 
 /* Debug / test taps (not on the product path): b2o_set_debug_taps(ctx, 1) makes b2o_crnn_forward also write the
  * fp32 fc_12 outputs ("logits") to its workspace; by default (0) the fused Dense + CTC kernel keeps them in

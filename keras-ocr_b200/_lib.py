@@ -61,15 +61,19 @@ SIGNATURES = {
     "b2o_craft_forward": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "b2o_boxes_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "b2o_get_boxes": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _i, _vp, _sz, _vp]),
+    "b2o_get_boxes_scored": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp, _i, _vp, _sz, _vp]),
     "b2o_compact_boxes": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "b2o_record_floats": (_sz, [_i]),
+    "b2o_record_floats_scored": (_sz, [_i]),
     "b2o_pack_records": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "b2o_pack_records_scored": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "b2o_warp_boxes": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "b2o_warp_boxes_color": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "b2o_crops_to_input_color": (_i, [_vp, _vp, _i, _vp, _vp]),
     "b2o_crnn_workspace_bytes": (_sz, [_i]),
     "b2o_crops_to_input": (_i, [_vp, _vp, _i, _vp, _vp]),
     "b2o_crnn_forward": (_i, [_vp, _vp, _i, _vp, _vp, _sz, _vp]),
+    "b2o_crnn_forward_scored": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_set_debug_taps": (_i, [_vp, _i]),
     "b2o_crnn_tap": (_i, [_vp, _c.c_char_p, _vp, _i, _vp, _sz, _vp]),
     "b2o_conv2d_test": (_i, [_vp, _vp, _i, _i, _i, _i, _c.POINTER(_c.c_float), _i, _i, _i,
@@ -202,6 +206,11 @@ class Context:
         self._check(self.lib.b2o_get_boxes(self.handle, scores, n, hs, ws, det, text, link, size, boxes, counts,
                                            max_boxes, wsp, ws_bytes, stream), "b2o_get_boxes")
 
+    def get_boxes_scored(self, scores, n, hs, ws, det, text, link, size, boxes, counts, box_scores, max_boxes, wsp,
+                         ws_bytes, stream):
+        self._check(self.lib.b2o_get_boxes_scored(self.handle, scores, n, hs, ws, det, text, link, size, boxes, counts,
+                                                  box_scores, max_boxes, wsp, ws_bytes, stream), "b2o_get_boxes_scored")
+
     def compact_boxes(self, boxes, counts, n, max_boxes, flat, image_index, stream):
         self._check(self.lib.b2o_compact_boxes(self.handle, boxes, counts, n, max_boxes, flat, image_index, stream),
                     "b2o_compact_boxes")
@@ -212,6 +221,15 @@ class Context:
     def pack_records(self, boxes, counts, labels, inv_scale, n, max_boxes, rows, rec_boxes, records, stream):
         self._check(self.lib.b2o_pack_records(self.handle, boxes, counts, labels, inv_scale, n, max_boxes, rows,
                                               rec_boxes, records, stream), "b2o_pack_records")
+
+    def record_floats_scored(self, rec_boxes):
+        return int(self.lib.b2o_record_floats_scored(rec_boxes))
+
+    def pack_records_scored(self, boxes, counts, labels, box_scores, logp, inv_scale, n, max_boxes, rows, rec_boxes,
+                            records, stream):
+        self._check(self.lib.b2o_pack_records_scored(self.handle, boxes, counts, labels, box_scores, logp, inv_scale, n,
+                                                     max_boxes, rows, rec_boxes, records, stream),
+                    "b2o_pack_records_scored")
 
     def warp_boxes(self, gray, n, h, w, boxes, image_index, n_boxes, crops, crnn_in, stream, color=False):
         fn = self.lib.b2o_warp_boxes_color if color else self.lib.b2o_warp_boxes
@@ -226,6 +244,10 @@ class Context:
 
     def crnn_forward(self, crnn_in, b, labels, ws, ws_bytes, stream):
         self._check(self.lib.b2o_crnn_forward(self.handle, crnn_in, b, labels, ws, ws_bytes, stream), "b2o_crnn_forward")
+
+    def crnn_forward_scored(self, crnn_in, b, labels, logp, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_crnn_forward_scored(self.handle, crnn_in, b, labels, logp, ws, ws_bytes, stream),
+                    "b2o_crnn_forward_scored")
 
     def set_debug_taps(self, on):
         self._check(self.lib.b2o_set_debug_taps(self.handle, int(on)), "b2o_set_debug_taps")

@@ -14,7 +14,7 @@ int stn_sample_run(b2o_ctx* ctx, const __half* feat, const float* theta, int B, 
 int lstm_run(b2o_ctx* ctx, const float* xw, int xw_ld, int xw_off, const __half* u, int B, int backwards, __half* out,
              int out_ld, int out_off, cudaStream_t st);
 int add_run(b2o_ctx* ctx, const __half* a, const __half* b, __half* o, long long n, cudaStream_t st);
-int fc_ctc_run(b2o_ctx* ctx, const __half* l2, int B, float* logits, int* labels, cudaStream_t st);
+int fc_ctc_run(b2o_ctx* ctx, const __half* l2, int B, float* logits, int* labels, float* logp, cudaStream_t st);
 
 namespace {
 
@@ -601,6 +601,11 @@ extern "C" size_t b2o_crnn_workspace_bytes(int b) { return b > 0 ? plan_crnn(b).
 
 extern "C" int b2o_crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, void* ws, size_t ws_bytes,
                                 void* stream) {
+  return b2o_crnn_forward_scored(ctx, crnn_in, b, labels, nullptr, ws, ws_bytes, stream);
+}
+
+extern "C" int b2o_crnn_forward_scored(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, float* logp, void* ws,
+                                       size_t ws_bytes, void* stream) {
   if (!ctx) return B2O_ERR_ARG;
   if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_forward: CRNN weights not loaded"); return B2O_ERR_STATE; }
   DeviceGuard guard(ctx->device);
@@ -664,7 +669,8 @@ extern "C" int b2o_crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_
   B2O_RETURN_IF(lstm_run(ctx, xw2f, 1024, 0, ctx->lstm_u[2], b, 0, l2, 256, 0, st));
   B2O_RETURN_IF(lstm_run(ctx, xw2f, 1024, 512, ctx->lstm_u[3], b, 1, l2, 256, 128, st));
   // fc_12 + discard + greedy CTC (321-333)
-  B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, ctx->debug_taps ? reinterpret_cast<float*>(base + p.off_logits) : nullptr, labels, st));
+  B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, ctx->debug_taps ? reinterpret_cast<float*>(base + p.off_logits) : nullptr, labels,
+                           logp, st));
   return B2O_OK;
 }
 

@@ -22,6 +22,7 @@ constexpr int kMaxHullRows = 2048;      // score maps are at most 1024 rows (max
 
 struct Component {                       // one kept connected component
   int root, x, y, w, h, area;
+  int maxtext;                           // float_key of its largest text score (np.max(textmap[labels == k]))
 };
 
 // cv2.threshold x2 + union mask + label init.  A pixel's initial label is the start of its horizontal run
@@ -107,6 +108,7 @@ __device__ __forceinline__ int float_key(float f) {
   const int b = __float_as_int(f);
   return b >= 0 ? b : b ^ 0x7fffffff;
 }
+__device__ __forceinline__ float key_float(int k) { return __int_as_float(k >= 0 ? k : k ^ 0x7fffffff); }
 
 struct Stats {        // indexed by root pixel
   int* area; int* minx; int* maxx; int* miny; int* maxy; int* maxtext;
@@ -143,9 +145,10 @@ __global__ void stats_kernel(const float* __restrict__ scores, const int* __rest
 // (detection.py:233-241) and compact them -- the slot order is the reference's label order.
 // Each thread looks at 4 consecutive pixels per round; rounds without any kept root (almost all of them:
 // a page has tens of components in 590k pixels) cost one __syncthreads_or.
+// box_scores (optional, (n, max_boxes)): the detection score of each stored box, in box order.
 __global__ void __launch_bounds__(1024)
 select_kernel(const int* __restrict__ label, int hw, Stats st, int size_thr, float det_thr, Component* __restrict__ comps,
-              int max_boxes, int* __restrict__ counts) {
+              int max_boxes, int* __restrict__ counts, float* __restrict__ box_scores) {
   __shared__ int warp_sums[32];
   __shared__ int carry;
   const int img = blockIdx.x;
@@ -206,7 +209,9 @@ select_kernel(const int* __restrict__ label, int hw, Stats st, int size_thr, flo
           c.w = st.maxx[base + q] - c.x + 1;
           c.h = st.maxy[base + q] - c.y + 1;
           c.area = st.area[base + q];
+          c.maxtext = st.maxtext[base + q];
           comps[static_cast<size_t>(img) * max_boxes + slot] = c;
+          if (box_scores) box_scores[static_cast<size_t>(img) * max_boxes + slot] = key_float(c.maxtext);
         }
         ++slot;
       }
@@ -714,6 +719,14 @@ extern "C" size_t b2o_boxes_workspace_bytes(int n, int hs, int ws, int max_boxes
 extern "C" int b2o_get_boxes(b2o_ctx* ctx, const float* scores, int n, int hs, int ws, float detection_threshold,
                              float text_threshold, float link_threshold, int size_threshold, float* boxes,
                              int32_t* counts, int max_boxes, void* ws_dev, size_t ws_bytes, void* stream) {
+  return b2o_get_boxes_scored(ctx, scores, n, hs, ws, detection_threshold, text_threshold, link_threshold,
+                              size_threshold, boxes, counts, nullptr, max_boxes, ws_dev, ws_bytes, stream);
+}
+
+extern "C" int b2o_get_boxes_scored(b2o_ctx* ctx, const float* scores, int n, int hs, int ws,
+                                    float detection_threshold, float text_threshold, float link_threshold,
+                                    int size_threshold, float* boxes, int32_t* counts, float* box_scores,
+                                    int max_boxes, void* ws_dev, size_t ws_bytes, void* stream) {
   if (!ctx) return B2O_ERR_ARG;
   DeviceGuard guard(ctx->device);
   if (!scores || !boxes || !counts || !ws_dev || n <= 0 || hs <= 0 || ws <= 0 || max_boxes <= 0) {
@@ -747,7 +760,7 @@ extern "C" int b2o_get_boxes(b2o_ctx* ctx, const float* scores, int n, int hs, i
   stats_kernel<<<nblocks(total, 256), 256, 0, st>>>(scores, w.label, total, hs * ws, ws, w.st);
   B2O_LAUNCH_CHECK(ctx);
   select_kernel<<<n, 1024, 0, st>>>(w.label, hs * ws, w.st, size_threshold, detection_threshold, w.comps, max_boxes,
-                                    counts);
+                                    counts, box_scores);
   B2O_LAUNCH_CHECK(ctx);
   const int dyn = 2 * kQuadSmemPlaneWords * 4, dyn_small = 2 * kQuadSmallPlaneWords * 4;
   if (!ctx->quads_configured) {        // a per-device attribute, hence per context (one context per device)
@@ -804,12 +817,16 @@ compact_boxes_kernel(const float* __restrict__ boxes, const int32_t* __restrict_
 
 constexpr int kSteps = 48;                         // label steps per word (recognition.py:20: 50 - 2 discarded)
 
+// SCORES: the record goes on with rec_boxes detection scores (box_scores, (n, max_boxes) as b2o_get_boxes_scored writes
+// them) and rec_boxes path log-probabilities (logp, (sum counts) as b2o_crnn_forward_scored writes them), 0 past c.
+template <bool SCORES>
 __global__ void __launch_bounds__(128)
 pack_records_kernel(const float* __restrict__ boxes, const int32_t* __restrict__ counts,
-                    const int32_t* __restrict__ labels, const float* __restrict__ inv_scale, int n, int max_boxes,
+                    const int32_t* __restrict__ labels, const float* __restrict__ box_scores,
+                    const float* __restrict__ logp, const float* __restrict__ inv_scale, int n, int max_boxes,
                     int rec_boxes, float* __restrict__ rec) {
   const int row = blockIdx.x;
-  const int rec_len = 1 + rec_boxes * 8 + rec_boxes * (kSteps / 4);
+  const int rec_len = 1 + rec_boxes * 8 + rec_boxes * (kSteps / 4) + (SCORES ? 2 * rec_boxes : 0);
   float* r = rec + static_cast<size_t>(row) * rec_len;
   int8_t* lab = reinterpret_cast<int8_t*>(r + 1 + rec_boxes * 8);
   int c = 0, off = 0, held = 0;
@@ -830,6 +847,14 @@ pack_records_kernel(const float* __restrict__ boxes, const int32_t* __restrict__
     const int k = t / kSteps;
     lab[t] = (k < c && labels) ? static_cast<int8_t>(labels[static_cast<size_t>(off + k) * kSteps + (t - k * kSteps)])
                    : static_cast<int8_t>(-1);
+  }
+  if constexpr (SCORES) {
+    float* sc = r + 1 + rec_boxes * 8 + rec_boxes * (kSteps / 4);
+    const float* ssrc = box_scores + static_cast<size_t>(min(row, n - 1)) * max_boxes;
+    for (int t = threadIdx.x; t < rec_boxes; t += blockDim.x) {
+      sc[t] = t < c ? ssrc[t] : 0.f;
+      sc[rec_boxes + t] = (t < c && logp) ? logp[off + t] : 0.f;
+    }
   }
 }
 
@@ -853,17 +878,46 @@ extern "C" size_t b2o_record_floats(int rec_boxes) {
   return rec_boxes > 0 ? 1 + static_cast<size_t>(rec_boxes) * 8 + static_cast<size_t>(rec_boxes) * (kSteps / 4) : 0;
 }
 
+extern "C" size_t b2o_record_floats_scored(int rec_boxes) {
+  return rec_boxes > 0 ? b2o_record_floats(rec_boxes) + 2 * static_cast<size_t>(rec_boxes) : 0;
+}
+
+namespace {
+
+// scored == false: the layout of b2o_pack_records; true: that of b2o_pack_records_scored
+int pack_records(b2o_ctx* ctx, bool scored, const float* boxes, const int32_t* counts, const int32_t* labels,
+                 const float* box_scores, const float* logp, const float* inv_scale, int n, int max_boxes, int rows,
+                 int rec_boxes, float* records, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!boxes || !counts || !inv_scale || !records || n <= 0 || rows < n || max_boxes <= 0 || rec_boxes <= 0 ||
+      (scored && !box_scores)) {
+    ctx->set_error("b2o_pack_records: bad argument");      // labels / logp may be NULL when no image has a box
+    return B2O_ERR_ARG;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (scored)
+    pack_records_kernel<true><<<rows, 128, 0, st>>>(boxes, counts, labels, box_scores, logp, inv_scale, n, max_boxes,
+                                                    rec_boxes, records);
+  else
+    pack_records_kernel<false><<<rows, 128, 0, st>>>(boxes, counts, labels, nullptr, nullptr, inv_scale, n, max_boxes,
+                                                     rec_boxes, records);
+  B2O_LAUNCH_CHECK(ctx);
+  return B2O_OK;
+}
+
+}  // namespace
+
 extern "C" int b2o_pack_records(b2o_ctx* ctx, const float* boxes, const int32_t* counts, const int32_t* labels,
                                 const float* inv_scale, int n, int max_boxes, int rows, int rec_boxes, float* records,
                                 void* stream) {
-  if (!ctx) return B2O_ERR_ARG;
-  DeviceGuard guard(ctx->device);
-  if (!boxes || !counts || !inv_scale || !records || n <= 0 || rows < n || max_boxes <= 0 || rec_boxes <= 0) {
-    ctx->set_error("b2o_pack_records: bad argument");      // labels may be NULL when no image has a box
-    return B2O_ERR_ARG;
-  }
-  pack_records_kernel<<<rows, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(boxes, counts, labels, inv_scale, n,
-                                                                              max_boxes, rec_boxes, records);
-  B2O_LAUNCH_CHECK(ctx);
-  return B2O_OK;
+  return pack_records(ctx, false, boxes, counts, labels, nullptr, nullptr, inv_scale, n, max_boxes, rows, rec_boxes,
+                      records, stream);
+}
+
+extern "C" int b2o_pack_records_scored(b2o_ctx* ctx, const float* boxes, const int32_t* counts, const int32_t* labels,
+                                       const float* box_scores, const float* logp, const float* inv_scale, int n,
+                                       int max_boxes, int rows, int rec_boxes, float* records, void* stream) {
+  return pack_records(ctx, true, boxes, counts, labels, box_scores, logp, inv_scale, n, max_boxes, rows, rec_boxes,
+                      records, stream);
 }

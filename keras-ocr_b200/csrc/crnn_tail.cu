@@ -6,7 +6,8 @@
 //                      outputs kept in processing order; recurrent matrix column-resident in registers
 //   add_kernel         keras.layers.Add (305)
 //   fc_ctc_kernel      Dense(256->37) (322-327; softmax skipped: argmax-invariant), [:, 2:] (328),
-//                      greedy CTC with repeat merge + blank removal, -1 padding (169-184)
+//                      greedy CTC with repeat merge + blank removal, -1 padding (169-184); optionally the greedy
+//                      path's log-probability (ctc_decode's second output, which CTCDecoder drops, 175)
 #include <math.h>
 
 #include "common.cuh"
@@ -233,11 +234,17 @@ constexpr int kKeep = 48, kDiscard = 2, kFeat = 256, kFcWarps = 8, kStepsPerWarp
 // run-time value: recognition.py:376-381 sizes the Dense layer from the alphabet).  Every logit is the same
 // serial fmaf chain over the 256 features in ascending order whatever K is; the argmax keeps the first maximum
 // (np.argmax / tf.argmax tie rule) and the collapse drops blanks (index K-1) and repeats.
+// SCORES: also logp[b] = sum_t log(max_c softmax(l_t)_c + 1e-7), the log-probability of the greedy path, with
+// max_c softmax = 1 / sum_c exp(l_c - l_max): every lane keeps an online sum-exp next to its running maximum, the lanes
+// merge in the butterfly of the argmax and thread 0 adds the 48 step terms in step order -- a function of the crop's
+// logits alone, so it does not depend on the batch.  The false instantiation is the labels-only kernel.
+template <bool SCORES>
 __global__ void __launch_bounds__(32 * kFcWarps)
 fc_ctc_kernel(const __half* __restrict__ l2 /*[B][50][256]*/, const float* __restrict__ w /*[256][K]*/,
               const float* __restrict__ bias, int B, int K, float* __restrict__ logits /*[B][48][K] or null*/,
-              int* __restrict__ labels /*[B][48]*/) {
+              int* __restrict__ labels /*[B][48]*/, float* __restrict__ logp /*[B], SCORES only*/) {
   __shared__ int best[kKeep];
+  __shared__ float term[SCORES ? kKeep : 1];
   __shared__ __half xs[kKeep][kFeat];
   const int b = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -250,8 +257,9 @@ fc_ctc_kernel(const __half* __restrict__ l2 /*[B][50][256]*/, const float* __res
   const int t0 = warp * kStepsPerWarp;
   float mx[kStepsPerWarp];
   int arg[kStepsPerWarp];
+  float se[kStepsPerWarp];                                            // SCORES: sum_c exp(l_c - mx) of this lane
 #pragma unroll
-  for (int j = 0; j < kStepsPerWarp; ++j) { mx[j] = -INFINITY; arg[j] = 0x7fffffff; }
+  for (int j = 0; j < kStepsPerWarp; ++j) { mx[j] = -INFINITY; arg[j] = 0x7fffffff; se[j] = 0.f; }
   for (int k = lane; k < K; k += 32) {
     float acc[kStepsPerWarp];
     const float bk = bias[k];
@@ -265,6 +273,10 @@ fc_ctc_kernel(const __half* __restrict__ l2 /*[B][50][256]*/, const float* __res
     }
 #pragma unroll
     for (int j = 0; j < kStepsPerWarp; ++j) {
+      if constexpr (SCORES) {                                          // online sum-exp against the running maximum
+        if (acc[j] > mx[j]) se[j] = __fadd_rn(__fmul_rn(se[j], expf(mx[j] - acc[j])), 1.f);
+        else se[j] = __fadd_rn(se[j], expf(acc[j] - mx[j]));
+      }
       if (acc[j] > mx[j]) { mx[j] = acc[j]; arg[j] = k; }            // ascending k: first maximum wins
       if (logits) logits[(static_cast<size_t>(b) * kKeep + t0 + j) * K + k] = acc[j];
     }
@@ -275,11 +287,29 @@ fc_ctc_kernel(const __half* __restrict__ l2 /*[B][50][256]*/, const float* __res
     for (int off = 16; off > 0; off >>= 1) {
       const float om = __shfl_xor_sync(0xffffffffu, mx[j], off);
       const int oa = __shfl_xor_sync(0xffffffffu, arg[j], off);
+      if constexpr (SCORES) {
+        // a lane without classes (K < 32) holds (-inf, 0) and contributes nothing
+        const float os = __shfl_xor_sync(0xffffffffu, se[j], off);
+        const float m = fmaxf(mx[j], om);
+        const float mine = mx[j] == -INFINITY ? 0.f : __fmul_rn(se[j], expf(mx[j] - m));
+        const float other = om == -INFINITY ? 0.f : __fmul_rn(os, expf(om - m));
+        se[j] = __fadd_rn(mine, other);
+      }
       if (om > mx[j] || (om == mx[j] && oa < arg[j])) { mx[j] = om; arg[j] = oa; }
     }
     if (lane == 0) best[t0 + j] = arg[j] == 0x7fffffff ? 0 : arg[j];  // all-NaN row: argmax returns 0
+    if constexpr (SCORES) {
+      if (lane == 0) term[t0 + j] = logf(__fadd_rn(__frcp_rn(se[j]), 1e-7f));
+    }
   }
   __syncthreads();
+  if constexpr (SCORES) {
+    if (threadIdx.x == 32) {                                           // next to thread 0's collapse
+      float s = 0.f;
+      for (int t = 0; t < kKeep; ++t) s = __fadd_rn(s, term[t]);
+      logp[b] = s;
+    }
+  }
   if (threadIdx.x == 0) {
     int* o = labels + static_cast<size_t>(b) * kKeep;
     int n = 0, prev = -1;
@@ -331,8 +361,12 @@ int add_run(b2o_ctx* ctx, const __half* a, const __half* b, __half* o, long long
   return B2O_OK;
 }
 
-int fc_ctc_run(b2o_ctx* ctx, const __half* l2, int B, float* logits, int* labels, cudaStream_t st) {
-  fc_ctc_kernel<<<B, 32 * kFcWarps, 0, st>>>(l2, ctx->fc12_w, ctx->fc12_b, B, ctx->n_classes, logits, labels);
+int fc_ctc_run(b2o_ctx* ctx, const __half* l2, int B, float* logits, int* labels, float* logp, cudaStream_t st) {
+  if (logp)
+    fc_ctc_kernel<true><<<B, 32 * kFcWarps, 0, st>>>(l2, ctx->fc12_w, ctx->fc12_b, B, ctx->n_classes, logits, labels, logp);
+  else
+    fc_ctc_kernel<false><<<B, 32 * kFcWarps, 0, st>>>(l2, ctx->fc12_w, ctx->fc12_b, B, ctx->n_classes, logits, labels,
+                                                      nullptr);
   B2O_LAUNCH_CHECK(ctx);
   return B2O_OK;
 }

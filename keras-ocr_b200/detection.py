@@ -85,10 +85,11 @@ class Detector:
         return scores
 
     def boxes_enqueue(self, scores, detection_threshold=0.7, text_threshold=0.4, link_threshold=0.4,
-                      size_threshold=10):
+                      size_threshold=10, with_scores=False):
         """getBoxes on the device, asynchronously: launches the kernels and the copy of the per-image counts into
         pinned memory, records an event and returns at once (``boxes_finish`` waits for that event only, so work
-        enqueued afterwards keeps the GPU busy while the host reads the counts)."""
+        enqueued afterwards keeps the GPU busy while the host reads the counts).  ``with_scores``: the state also
+        holds ``box_scores`` (N,M) float32 CUDA, each box's detection score (``b2o_get_boxes_scored``)."""
         n, hs, ws_, _ = scores.shape
         stream = torch.cuda.current_stream(self.device)
         scores = scores.contiguous()
@@ -101,8 +102,14 @@ class Detector:
             self._box_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         wsp = self._box_ws
         thr = (float(detection_threshold), float(text_threshold), float(link_threshold), int(size_threshold))
-        self.ctx.get_boxes(scores.data_ptr(), n, hs, ws_, *thr, boxes.data_ptr(), counts.data_ptr(), m,
-                           wsp.data_ptr(), nbytes, stream.cuda_stream)
+        box_scores = None
+        if with_scores:
+            box_scores = torch.empty((n, m), dtype=torch.float32, device=self.device)
+            self.ctx.get_boxes_scored(scores.data_ptr(), n, hs, ws_, *thr, boxes.data_ptr(), counts.data_ptr(),
+                                      box_scores.data_ptr(), m, wsp.data_ptr(), nbytes, stream.cuda_stream)
+        else:
+            self.ctx.get_boxes(scores.data_ptr(), n, hs, ws_, *thr, boxes.data_ptr(), counts.data_ptr(), m,
+                               wsp.data_ptr(), nbytes, stream.cuda_stream)
         counts_pin = torch.empty((n,), dtype=torch.int32, pin_memory=True)
         counts_pin.copy_(counts, non_blocking=True)
         event = torch.cuda.Event()
@@ -114,17 +121,18 @@ class Detector:
         self.ctx.compact_boxes(boxes.data_ptr(), counts.data_ptr(), n, m, flat.data_ptr(), image_index.data_ptr(),
                                stream.cuda_stream)
         return {"scores": scores, "boxes": boxes, "counts": counts, "counts_pin": counts_pin, "event": event, "m": m,
-                "thr": thr, "flat": flat, "image_index": image_index}
+                "thr": thr, "flat": flat, "image_index": image_index, "box_scores": box_scores}
 
     def boxes_finish(self, state):
         """Wait for ``boxes_enqueue``.  Returns (boxes (N,M,4,2) float32 CUDA, counts ndarray (N,)); re-runs
-        getBoxes with a larger box table in the (rare) case an image had more boxes than the table holds."""
+        getBoxes with a larger box table in the (rare) case an image had more boxes than the table holds (the state's
+        ``box_scores``, when asked for, then come from that run too)."""
         state["event"].synchronize()                     # the one synchronisation of the detector half
         counts_host = state["counts_pin"].numpy().copy()
         while counts_host.size and int(counts_host.max()) > state["boxes"].shape[1]:
             self.max_boxes = int(2 ** np.ceil(np.log2(int(counts_host.max()))))
             d, t, l, s = state["thr"]
-            again = self.boxes_enqueue(state["scores"], d, t, l, s)
+            again = self.boxes_enqueue(state["scores"], d, t, l, s, with_scores=state["box_scores"] is not None)
             again["event"].synchronize()
             state.update(again)
             counts_host = state["counts_pin"].numpy().copy()
@@ -141,13 +149,21 @@ class Detector:
 
     # ------------------------------------------------------------------ reference API
     def detect(self, images: typing.List[typing.Union[np.ndarray, str]], detection_threshold=0.7,
-               text_threshold=0.4, link_threshold=0.4, size_threshold=10, **kwargs):
+               text_threshold=0.4, link_threshold=0.4, size_threshold=10, return_scores=False, **kwargs):
         """Same contract as reference detection.py:745-785: a list with one array of boxes
         ``(n_i, 4, 2)`` float32 per image (``np.array([])`` when there is none).  ``kwargs`` are the
-        keras ``predict`` arguments of the reference (batch_size, verbose, ...) and are ignored."""
+        keras ``predict`` arguments of the reference (batch_size, verbose, ...) and are ignored.
+
+        ``return_scores=True``: one ``(boxes, scores)`` pair per image instead, ``scores`` (n_i,) float32 the
+        detection score of each box -- the largest text score over its connected component, the value compared
+        with ``detection_threshold`` (so every score is >= it)."""
         images_t = _as_device_images(images, self.device)
-        boxes, counts = self.detect_device(images_t, detection_threshold=detection_threshold,
-                                           text_threshold=text_threshold, link_threshold=link_threshold,
-                                           size_threshold=size_threshold)
+        state = self.boxes_enqueue(self.predict_device(images_t), detection_threshold, text_threshold, link_threshold,
+                                   size_threshold, with_scores=return_scores)
+        boxes, counts = self.boxes_finish(state)
         boxes_host = boxes.cpu().numpy()
-        return [boxes_host[i, :c].copy() if c else np.array([]) for i, c in enumerate(counts)]
+        groups = [boxes_host[i, :c].copy() if c else np.array([]) for i, c in enumerate(counts)]
+        if not return_scores:
+            return groups
+        scores_host = state["box_scores"].cpu().numpy()
+        return [(g, scores_host[i, :c].copy()) for i, (g, c) in enumerate(zip(groups, counts))]

@@ -20,15 +20,24 @@ def shard_bounds(n_items, world_size, rank):
     return lo, lo + base + (1 if rank < extra else 0)
 
 
-def pack_records(counts, boxes, labels, per_rank, max_boxes):
+def record_floats(max_boxes, scores=False):
+    """Floats per record: b2o_record_floats (b2o_record_floats_scored with ``scores``) of include/b2ocr.h."""
+    return 1 + max_boxes * 8 + max_boxes * (STEPS // 4) + (2 * max_boxes if scores else 0)
+
+
+def pack_records(counts, boxes, labels, per_rank, max_boxes, box_scores=None, logp=None):
     """Fixed-size record block for one rank: float32 tensor (per_rank, 1 + max_boxes*8 + max_boxes*12).
 
     labels (int8, 48 per word) are bit-packed 4 per float32 slot so that a single dtype travels.
     counts (n,), boxes (n,M,4,2) float32, labels (sum(counts),48) int -> one contiguous CPU tensor.
+    ``box_scores`` (n,M) and ``logp`` (sum(counts),) float32: the scored layout (as ``b2o_pack_records_scored``), the
+    record above followed by max_boxes detection scores and max_boxes path log-probabilities.
     """
     n = len(counts)
-    rec = np.zeros((per_rank, 1 + max_boxes * 8 + max_boxes * (STEPS // 4)), dtype=np.float32)
+    scored = box_scores is not None
+    rec = np.zeros((per_rank, record_floats(max_boxes, scored)), dtype=np.float32)
     lab8 = np.full((per_rank, max_boxes, STEPS), -1, dtype=np.int8)
+    s0 = record_floats(max_boxes)
     start = 0
     for i in range(n):
         c = min(int(counts[i]), max_boxes)
@@ -36,8 +45,11 @@ def pack_records(counts, boxes, labels, per_rank, max_boxes):
         rec[i, 1:1 + c * 8] = np.asarray(boxes[i][:c], dtype=np.float32).reshape(-1)
         if c:
             lab8[i, :c] = np.asarray(labels[start:start + c], dtype=np.int8)
+            if scored:
+                rec[i, s0:s0 + c] = np.asarray(box_scores[i][:c], dtype=np.float32)
+                rec[i, s0 + max_boxes:s0 + max_boxes + c] = np.asarray(logp[start:start + c], dtype=np.float32)
         start += int(counts[i])
-    rec[:, 1 + max_boxes * 8:] = lab8.reshape(per_rank, -1).view(np.float32)
+    rec[:, 1 + max_boxes * 8:s0] = lab8.reshape(per_rank, -1).view(np.float32)
     rec[n:, 0] = -1                                    # padding rows of a short last shard
     return torch.from_numpy(rec)
 
@@ -53,17 +65,19 @@ class RecordOverflow(ValueError):
     """An image has more words than a fixed-size record holds (``max_boxes``)."""
 
 
-def unpack_blocks(blocks, max_boxes, strict=True):
+def unpack_blocks(blocks, max_boxes, strict=True, scores=False):
     """All gathered blocks at once (rank order = global image order): returns (counts (n_images,), boxes (total,4,2)
     float32, labels (total,48) int8) with the words of image i at [sum(counts[:i]), +counts[i]).  Only the used
     prefix of every record is touched (two concatenations of per-image views), not the 75 % padding.
+    ``scores=True`` reads the scored layout and also returns (box_scores (total,), logp (total,)) float32.
 
     A record's count field is the number of words its image HAS; a record holds ``max_boxes`` of them.  The
     single-GPU ``Pipeline.recognize`` grows its box table on demand (as the reference returns every box), so a
     count above ``max_boxes`` raises ``RecordOverflow`` rather than dropping words (``strict=False``: keep the
     first ``max_boxes``, for callers that asked for a cap)."""
-    box_parts, lab_parts, counts = [], [], []
+    box_parts, lab_parts, counts, score_parts, logp_parts = [], [], [], [], []
     lab0 = (1 + max_boxes * 8) * 4                     # byte offset of the label area inside a record
+    s0 = record_floats(max_boxes)                      # float offset of the score area (scored layout)
     for r, block in enumerate(blocks):
         rec = np.ascontiguousarray(np.asarray(block.cpu() if isinstance(block, torch.Tensor) else block))
         rec8 = rec.view(np.int8)
@@ -79,8 +93,14 @@ def unpack_blocks(blocks, max_boxes, strict=True):
             if c:
                 box_parts.append(rec[i, 1:1 + c * 8])
                 lab_parts.append(rec8[i, lab0:lab0 + c * STEPS])
+                if scores:
+                    score_parts.append(rec[i, s0:s0 + c])
+                    logp_parts.append(rec[i, s0 + max_boxes:s0 + max_boxes + c])
     boxes = np.concatenate(box_parts).reshape(-1, 4, 2) if box_parts else np.zeros((0, 4, 2), np.float32)
     labels = np.concatenate(lab_parts).reshape(-1, STEPS) if lab_parts else np.zeros((0, STEPS), np.int8)
+    if scores:
+        cat = lambda parts: np.concatenate(parts) if parts else np.zeros((0,), np.float32)      # noqa: E731
+        return np.asarray(counts, dtype=np.int64), boxes, labels, cat(score_parts), cat(logp_parts)
     return np.asarray(counts, dtype=np.int64), boxes, labels
 
 
@@ -109,7 +129,7 @@ def _host_records(pipeline, local, per_rank, max_boxes):
     return pack_records(counts, boxes, labels, per_rank, max_boxes)
 
 
-def recognize_sharded(pipeline, images, max_boxes=128, presharded=False):
+def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_scores=False):
     """Run ``pipeline.recognize`` on this rank's shard of ``images`` and gather to rank 0.
 
     ``images`` is the global batch (every rank passes the same list and takes its contiguous slice) or, with
@@ -120,7 +140,9 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False):
     ``pack_records``.
 
     Returns, on rank 0, the same list-of-lists as ``Pipeline.recognize`` for ALL images (global
-    order); ``None`` on the other ranks.  Boxes are in source-image pixels.
+    order); ``None`` on the other ranks.  Boxes are in source-image pixels.  ``return_scores=True``: the words are
+    (text, box, detection_score, confidence) as ``Pipeline.recognize(return_scores=True)`` returns them, carried in
+    the scored record layout (device records only).
     """
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
@@ -134,15 +156,18 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False):
     if per_rank == 0:
         return [] if rank == 0 else None
     native = getattr(pipeline, "recognize_records", None) is not None and getattr(pipeline, "_native", lambda: True)()
+    if return_scores and not native:
+        raise NotImplementedError("return_scores=True needs this package's Pipeline with its own Detector and Recognizer")
+    sk = {"scores": True} if return_scores else {}      # pipelines without the flag keep working unscored
     if native:
         if getattr(pipeline, "records_counts", None) is not None:
-            state = pipeline.records_begin(mine, rows=per_rank, rec_boxes=16 if max_boxes == "auto" else max_boxes)
+            state = pipeline.records_begin(mine, rows=per_rank, rec_boxes=16 if max_boxes == "auto" else max_boxes, **sk)
             if max_boxes == "auto":
                 max_boxes = agree_max_boxes(pipeline.records_counts(state), _collective_device(pipeline))
             local = pipeline.records_end(state, rec_boxes=max_boxes)
         else:                                           # a pipeline that only offers the one-call form
             assert max_boxes != "auto", "max_boxes='auto' needs records_begin / records_counts / records_end"
-            local = pipeline.recognize_records(mine, rows=per_rank, rec_boxes=max_boxes)
+            local = pipeline.recognize_records(mine, rows=per_rank, rec_boxes=max_boxes, **sk)
         device = None                                   # already where the backend wants it
     else:
         result = pipeline.recognize(mine) if len(mine) else []
@@ -153,7 +178,7 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False):
     blocks = gather_records(local, world, rank, device)
     if rank != 0:
         return None
-    return _decode_blocks(blocks, max_boxes, alphabet)
+    return _decode_blocks(blocks, max_boxes, alphabet, return_scores)
 
 
 def _collective_device(pipeline):
@@ -180,25 +205,33 @@ def agree_max_boxes(counts, device=None, floor=16):
 stats = {"decode_ms": 0.0, "decodes": 0}      # rank 0's serial host work (bench.py reports it per step)
 
 
-def _decode_blocks(blocks, max_boxes, alphabet):
+def _decode_blocks(blocks, max_boxes, alphabet, scores=False):
     import time
 
     from . import recognition
 
     t0 = time.perf_counter()
     try:
-        return _decode_blocks_impl(blocks, max_boxes, alphabet, recognition)
+        return _decode_blocks_impl(blocks, max_boxes, alphabet, recognition, scores)
     finally:
         stats["decode_ms"] += (time.perf_counter() - t0) * 1e3
         stats["decodes"] += 1
 
 
-def _decode_blocks_impl(blocks, max_boxes, alphabet, recognition):
-    counts, boxes, labels = unpack_blocks(blocks, max_boxes)
+def _decode_blocks_impl(blocks, max_boxes, alphabet, recognition, scores=False):
+    if scores:
+        counts, boxes, labels, box_scores, logp = unpack_blocks(blocks, max_boxes, scores=True)
+        conf = recognition.confidences(logp)
+    else:
+        counts, boxes, labels = unpack_blocks(blocks, max_boxes)
     texts = recognition.labels_to_text(labels, alphabet)
     quads, out, start = list(boxes), [], 0             # one (4,2) view per word, made once
     for c in counts.tolist():
-        out.append(list(zip(texts[start:start + c], quads[start:start + c])))
+        if scores:
+            out.append(list(zip(texts[start:start + c], quads[start:start + c], box_scores[start:start + c],
+                                conf[start:start + c])))
+        else:
+            out.append(list(zip(texts[start:start + c], quads[start:start + c])))
         start += c
     return out
 
@@ -215,9 +248,10 @@ class ShardedStream:
     With this package's ``Pipeline`` the records stay on the device until the gather and reach the host through ONE
     asynchronous copy into pinned memory; any other pipeline (``recognize`` only) is served too, without the overlap.
     ``max_boxes``: words a record holds (an image with more raises ``RecordOverflow`` on rank 0 when its batch is
-    decoded) or ``"auto"`` (sized per batch by ``agree_max_boxes``)."""
+    decoded) or ``"auto"`` (sized per batch by ``agree_max_boxes``).  ``return_scores=True``: words as
+    ``recognize_sharded(return_scores=True)`` returns them (device records only)."""
 
-    def __init__(self, pipeline, max_boxes=128):
+    def __init__(self, pipeline, max_boxes=128, return_scores=False):
         self.pipeline, self.max_boxes = pipeline, max_boxes
         self.world = dist.get_world_size() if dist.is_initialized() else 1
         self.rank = dist.get_rank() if dist.is_initialized() else 0
@@ -225,6 +259,11 @@ class ShardedStream:
         assert len(self.alphabet) + 1 <= 127, "record labels travel as int8: alphabets up to 126 characters"
         self._native = (getattr(pipeline, "records_begin", None) is not None
                         and getattr(pipeline, "_native", lambda: True)())
+        if return_scores and not self._native:
+            raise NotImplementedError("return_scores=True needs this package's Pipeline with its own Detector and "
+                                      "Recognizer")
+        self.return_scores = return_scores
+        self._sk = {"scores": True} if return_scores else {}
         self._pending = None                             # (host blocks, event or None) of the batch in flight
         self._side = None                                # communication stream (CUDA tensors only)
         self._keep = None
@@ -237,7 +276,7 @@ class ShardedStream:
         self._pending = None
         if event is not None:
             event.synchronize()
-        return _decode_blocks(list(host), max_boxes, self.alphabet)
+        return _decode_blocks(list(host), max_boxes, self.alphabet, self.return_scores)
 
     def submit(self, images):
         rows = len(images)
@@ -245,7 +284,8 @@ class ShardedStream:
             return self._take_pending()
         max_boxes = self.max_boxes
         if self._native:
-            state = self.pipeline.records_begin(images, rows=rows, rec_boxes=16 if max_boxes == "auto" else max_boxes)   # GPU busy from here on
+            state = self.pipeline.records_begin(images, rows=rows, rec_boxes=16 if max_boxes == "auto" else max_boxes,
+                                                **self._sk)                      # GPU busy from here on
             previous = self._take_pending()              # ... while the host decodes the batch before
             if max_boxes == "auto":
                 max_boxes = agree_max_boxes(self.pipeline.records_counts(state), _collective_device(self.pipeline))

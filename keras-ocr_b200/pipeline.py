@@ -115,25 +115,34 @@ class Pipeline:
         return (batch, scales, gray) if want_gray else (batch, scales)
 
     # ---------------------------------------------------------------- the three stages of one sub-batch
-    def _stage_detect(self, images, pad_to, thresholds):
+    def _stage_detect(self, images, pad_to, thresholds, with_scores=False):
         batch, scales, gray = self.prepare_device(images, pad_to, want_gray=True)
         scores = self.detector.predict_device(batch)
         return {"batch": batch, "scales": scales, "gray": gray,
-                "boxes_state": self.detector.boxes_enqueue(scores, **thresholds)}
+                "boxes_state": self.detector.boxes_enqueue(scores, **thresholds, with_scores=with_scores)}
+
+    @staticmethod
+    def _to_host(st, key, t):
+        st[key] = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
+        st[key].copy_(t, non_blocking=True)
 
     def _stage_recognize(self, st):
         det, rec = self.detector, self.recognizer
         bst = st.pop("boxes_state")
         boxes, counts = det.boxes_finish(bst)
+        box_scores, logp = bst["box_scores"], None
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
-                                                 image_index=bst["image_index"])
+                                                 image_index=bst["image_index"], with_scores=box_scores is not None)
+        if box_scores is not None:
+            labels, logp = labels
+            self._to_host(st, "box_scores_host", box_scores)
         st["counts"] = counts
-        st["boxes_host"] = torch.empty(boxes.shape, dtype=boxes.dtype, pin_memory=True)
-        st["boxes_host"].copy_(boxes, non_blocking=True)
+        self._to_host(st, "boxes_host", boxes)
         if labels is not None:
-            st["labels_host"] = torch.empty(labels.shape, dtype=labels.dtype, pin_memory=True)
-            st["labels_host"].copy_(labels, non_blocking=True)
-        st["keep"] = (boxes, labels)                     # alive until the copies have run
+            self._to_host(st, "labels_host", labels)
+        if logp is not None:
+            self._to_host(st, "logp_host", logp)
+        st["keep"] = (boxes, labels, box_scores, logp)   # alive until the copies have run
         st["done"] = torch.cuda.Event()
         st["done"].record(torch.cuda.current_stream(det.device))
 
@@ -147,6 +156,11 @@ class Pipeline:
             texts = recognition.labels_to_text(labels_host, self.recognizer.alphabet)
         else:
             texts = []
+        scored = "box_scores_host" in st
+        if scored:
+            box_scores = st["box_scores_host"].numpy()
+            conf = recognition.confidences(st["logp_host"].numpy()) if "logp_host" in st else np.zeros(0, np.float32)
+            d2h += box_scores.nbytes + conf.nbytes
         self.last_stats["d2h_bytes"] += int(d2h)
         out, start = [], 0
         for i, (c, scale) in enumerate(zip(counts, st["scales"])):
@@ -154,15 +168,20 @@ class Pipeline:
             group = boxes_host[i, :c].copy()
             if scale != 1:
                 group = tools.adjust_boxes(boxes=group, boxes_format="boxes", scale=1 / scale)
-            out.append(list(zip(texts[start:start + c], group)))
+            if scored:
+                out.append(list(zip(texts[start:start + c], group, box_scores[i, :c], conf[start:start + c])))
+            else:
+                out.append(list(zip(texts[start:start + c], group)))
             start += c
         return out
 
-    def recognize(self, images, detection_kwargs=None, recognition_kwargs=None):
+    def recognize(self, images, detection_kwargs=None, recognition_kwargs=None, return_scores=False):
         """Run the pipeline on one or multiple images (reference pipeline.py:28-75).
 
         Returns a list (one entry per image) of lists of (text, box) tuples, boxes (4,2) float32 in
-        the coordinates of the *input* image.
+        the coordinates of the *input* image.  ``return_scores=True``: (text, box, detection_score, confidence)
+        tuples instead -- the box's detection score (``Detector.detect(return_scores=True)``) and the word's
+        confidence exp(S) in (0, 1] (``recognition.confidences``); texts and boxes are those of the default call.
         """
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
@@ -174,6 +193,9 @@ class Pipeline:
         if recognition_kwargs is None:
             recognition_kwargs = {}
         if not self._native():
+            if return_scores:
+                raise NotImplementedError("return_scores=True needs this package's Detector and Recognizer; injected "
+                                          "detectors / recognizers do not report scores")
             return self._recognize_generic(images, detection_kwargs, recognition_kwargs)
         thresholds = {k: detection_kwargs[k] for k in ("detection_threshold", "text_threshold", "link_threshold",
                                                         "size_threshold") if k in detection_kwargs}
@@ -188,7 +210,8 @@ class Pipeline:
         states, out = [], []
         for step in range(k + 2):                        # detect(i) | recognize(i-1) | finish(i-2)
             if step < k:
-                states.append(self._stage_detect(images[bounds[step]:bounds[step + 1]], pad_to, thresholds))
+                states.append(self._stage_detect(images[bounds[step]:bounds[step + 1]], pad_to, thresholds,
+                                                 with_scores=return_scores))
             if 1 <= step <= k:
                 self._stage_recognize(states[step - 1])
             if step >= 2:
@@ -196,15 +219,17 @@ class Pipeline:
                 states[step - 2] = None
         return out
 
-    def recognize_records(self, images, rows=None, rec_boxes=128, detection_kwargs=None):
+    def recognize_records(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False):
         """``recognize`` without the trip to the host: returns the results as a CUDA float32 tensor of fixed-size
         per-image records, ``(rows, b2o_record_floats(rec_boxes))`` = [count | rec_boxes x (4,2) boxes in source
         pixels | rec_boxes x 48 int8 labels] (``distributed.unpack_blocks`` decodes it; rows beyond ``len(images)``
         carry count -1).  This is the payload of the multi-GPU gather (SURVEY.md 8(e)): only the per-image box
-        counts ever reach the host on this rank."""
-        return self.records_end(self.records_begin(images, rows, rec_boxes, detection_kwargs))
+        counts ever reach the host on this rank.  ``scores=True``: the scored layout,
+        ``(rows, b2o_record_floats_scored(rec_boxes))``, which appends [rec_boxes detection scores | rec_boxes
+        path log-probabilities] to that record."""
+        return self.records_end(self.records_begin(images, rows, rec_boxes, detection_kwargs, scores))
 
-    def records_begin(self, images, rows=None, rec_boxes=128, detection_kwargs=None):
+    def records_begin(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False):
         """First half of ``recognize_records``: queues resize/pad, CRAFT and getBoxes and returns at once (no
         synchronisation), so the caller can use the host while the GPU works (``distributed.ShardedStream`` decodes the
         previous batch's words here).  Pass the returned state to ``records_end``."""
@@ -221,10 +246,11 @@ class Pipeline:
         rows = n if rows is None else int(rows)
         assert rows >= n and rows > 0
         self.last_stats = {"h2d_bytes": 0, "d2h_bytes": 0}
-        state = {"n": n, "rows": rows, "rec_boxes": rec_boxes}
+        state = {"n": n, "rows": rows, "rec_boxes": rec_boxes, "scores": bool(scores)}
         if n:
             plans = self._plans(images)
-            state["st"] = self._stage_detect(images, (max(p[1] for p in plans), max(p[2] for p in plans)), thresholds)
+            state["st"] = self._stage_detect(images, (max(p[1] for p in plans), max(p[2] for p in plans)), thresholds,
+                                             with_scores=bool(scores))
         return state
 
     def records_counts(self, state):
@@ -246,7 +272,9 @@ class Pipeline:
         det, rec = self.detector, self.recognizer
         n, rows = state["n"], state["rows"]
         rec_boxes = state["rec_boxes"] if rec_boxes is None else int(rec_boxes)
-        records = torch.empty((rows, det.ctx.record_floats(rec_boxes)), dtype=torch.float32, device=det.device)
+        scored = state.get("scores", False)
+        floats = det.ctx.record_floats_scored(rec_boxes) if scored else det.ctx.record_floats(rec_boxes)
+        records = torch.empty((rows, floats), dtype=torch.float32, device=det.device)
         if n == 0:
             records.zero_()
             records[:, 0] = -1
@@ -256,11 +284,18 @@ class Pipeline:
         bst = st.pop("boxes_state")
         boxes = state["boxes"]
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
-                                                 image_index=bst["image_index"])
+                                                 image_index=bst["image_index"], with_scores=scored)
         inv = torch.tensor([1.0 / s for s in st["scales"]], dtype=torch.float32).to(det.device, non_blocking=True)
-        det.ctx.pack_records(boxes.data_ptr(), bst["counts"].data_ptr(), labels.data_ptr() if labels is not None else None,
-                             inv.data_ptr(), n, boxes.shape[1], rows, rec_boxes, records.data_ptr(),
-                             torch.cuda.current_stream(det.device).cuda_stream)
+        stream = torch.cuda.current_stream(det.device).cuda_stream
+        ptr = lambda t: t.data_ptr() if t is not None else None      # noqa: E731
+        if scored:
+            labels, logp = labels
+            det.ctx.pack_records_scored(boxes.data_ptr(), bst["counts"].data_ptr(), ptr(labels), bst["box_scores"].data_ptr(),
+                                        ptr(logp), inv.data_ptr(), n, boxes.shape[1], rows, rec_boxes, records.data_ptr(),
+                                        stream)
+        else:
+            det.ctx.pack_records(boxes.data_ptr(), bst["counts"].data_ptr(), ptr(labels), inv.data_ptr(), n,
+                                 boxes.shape[1], rows, rec_boxes, records.data_ptr(), stream)
         self.last_stats["d2h_bytes"] = int(counts.nbytes)
         return records
 

@@ -34,6 +34,13 @@ def labels_to_text(rows, alphabet=DEFAULT_ALPHABET):
     return ["".join(alphabet[idx] for idx in row if idx not in (blank, -1)) for row in rows]
 
 
+def confidences(logp):
+    """Word confidences exp(S) in (0, 1] (float32) from the greedy-path log-probabilities
+    S = sum_t log(max_c p[t,c] + 1e-7) that ``b2o_crnn_forward_scored`` writes.  The 1e-7 floor lets S of a
+    certain word reach 48 * log(1 + 1e-7) ~ 5e-6 > 0, hence the clip at 1."""
+    return np.minimum(np.exp(np.asarray(logp, dtype=np.float32)), np.float32(1.0))
+
+
 class Recognizer:
     """A text recognizer using the CRNN architecture, running as sm_90a CUDA kernels.
 
@@ -144,8 +151,9 @@ class Recognizer:
                             torch.cuda.current_stream(self.device).cuda_stream, color=color)
         return crnn_in, crops
 
-    def predict_device(self, crnn_in):
-        """CRNN + greedy CTC.  crnn_in: (B,200,31) fp16 -> labels (B,48) int32 (-1 padded)."""
+    def predict_device(self, crnn_in, with_scores=False):
+        """CRNN + greedy CTC.  crnn_in: (B,200,31) fp16 -> labels (B,48) int32 (-1 padded).  ``with_scores``: returns
+        (labels, logp) with logp (B,) float32 the greedy path's log-probability (``b2o_crnn_forward_scored``)."""
         b = crnn_in.shape[0]
         labels = torch.empty((b, STEPS), dtype=torch.int32, device=self.device)
         nbytes = self.ctx.crnn_workspace_bytes(b)
@@ -153,10 +161,16 @@ class Recognizer:
             self._ws = None
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         ws = self._ws
-        self.ctx.crnn_forward(crnn_in.data_ptr(), b, labels.data_ptr(), ws.data_ptr(), nbytes,
-                              torch.cuda.current_stream(self.device).cuda_stream)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        logp = None
+        if with_scores:
+            logp = torch.empty((b,), dtype=torch.float32, device=self.device)
+            self.ctx.crnn_forward_scored(crnn_in.data_ptr(), b, labels.data_ptr(), logp.data_ptr(), ws.data_ptr(), nbytes,
+                                         stream)
+        else:
+            self.ctx.crnn_forward(crnn_in.data_ptr(), b, labels.data_ptr(), ws.data_ptr(), nbytes, stream)
         self._last_ws = (ws, b) if self.keep_workspace else None
-        return labels
+        return (labels, logp) if with_scores else labels
 
     def tap(self, name, shape, dtype):
         """Debug: copy an intermediate of the last predict_device call (needs keep_workspace=True)."""
@@ -166,8 +180,9 @@ class Recognizer:
                           torch.cuda.current_stream(self.device).cuda_stream)
         return out
 
-    def recognize_crops(self, crops):
-        """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str]."""
+    def recognize_crops(self, crops, return_scores=False):
+        """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str].
+        ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``."""
         t = crops if isinstance(crops, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(crops))
         t = t.to(self.device).contiguous()
         b = t.shape[0]
@@ -177,7 +192,10 @@ class Recognizer:
         crnn_in = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + ((3,) if self.color else ()), dtype=torch.float16, device=self.device)
         self.ctx.crops_to_input(t.data_ptr(), b, crnn_in.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream,
                                 color=self.color)
-        return labels_to_text(self.predict_device(crnn_in).cpu().numpy(), self.alphabet)
+        if not return_scores:
+            return labels_to_text(self.predict_device(crnn_in).cpu().numpy(), self.alphabet)
+        labels, logp = self.predict_device(crnn_in, with_scores=True)
+        return list(zip(labels_to_text(labels.cpu().numpy(), self.alphabet), confidences(logp.cpu().numpy())))
 
     def recognize(self, image):
         """Recognize text from a single pre-cropped image (reference recognition.py:467-489): fit to
@@ -189,8 +207,10 @@ class Recognizer:
             image = cv2.cvtColor(image, code=cv2.COLOR_RGB2GRAY)
         return self.recognize_crops(np.ascontiguousarray(image.reshape((1, TARGET_HEIGHT, TARGET_WIDTH) + ((3,) if self.color else ()))))[0]
 
-    def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None):
-        """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA.
+    def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
+                                    with_scores=False):
+        """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
+        (``with_scores``: (labels, logp (B,) f32 CUDA), see ``predict_device``).
 
         Optional device-side by-products of the earlier stages, so that nothing but the kernel launches is
         left to do once the host knows the counts: ``gray`` (N,H,W) u8 from ``b2o_resize_pad_batch``;
@@ -199,7 +219,7 @@ class Recognizer:
         m = boxes.shape[1]
         total = int(np.minimum(counts, m).sum())
         if total == 0:
-            return None
+            return (None, None) if with_scores else None
         if self.color:
             gray = images_t                                       # color recognizer: crops come straight from the RGB batch
         elif gray is None:
@@ -212,11 +232,12 @@ class Recognizer:
             self.ctx.compact_boxes(boxes.data_ptr(), counts_dev.data_ptr(), n, m, flat.data_ptr(),
                                    image_index.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
-        return self.predict_device(crnn_in)
+        return self.predict_device(crnn_in, with_scores=with_scores)
 
     # ------------------------------------------------------------------ reference API
-    def recognize_from_boxes(self, images, box_groups, **kwargs) -> typing.List[typing.List[str]]:
-        """Same contract as reference recognition.py:491-537."""
+    def recognize_from_boxes(self, images, box_groups, return_scores=False, **kwargs) -> typing.List[typing.List[str]]:
+        """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
+        (text, confidence) pair instead, see ``confidences``."""
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
 
@@ -232,6 +253,10 @@ class Recognizer:
         flat_t = torch.from_numpy(np.ascontiguousarray(flat)).to(self.device)
         idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
         crnn_in, _ = self.warp_device(images_t if self.color else self.gray_device(images_t), flat_t, idx)
-        predictions = labels_to_text(self.predict_device(crnn_in).cpu().numpy(), self.alphabet)
+        if return_scores:
+            labels, logp = self.predict_device(crnn_in, with_scores=True)
+            predictions = list(zip(labels_to_text(labels.cpu().numpy(), self.alphabet), confidences(logp.cpu().numpy())))
+        else:
+            predictions = labels_to_text(self.predict_device(crnn_in).cpu().numpy(), self.alphabet)
         ends = np.cumsum(counts)
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]
