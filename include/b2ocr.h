@@ -148,7 +148,8 @@ int b2o_warp_boxes_color(b2o_ctx* ctx, const uint8_t* rgb_dev, int n, int h, int
                          const float* boxes_dev, const int32_t* image_index_dev, int n_boxes,
                          uint8_t* crops_dev, void* crnn_in_dev, void* stream);
 
-/* prediction_model.predict (recognition.py:535; graph 214-333): CRNN + STN + BiLSTM + greedy CTC.
+/* prediction_model.predict (recognition.py:535; graph 214-333): CRNN + STN + BiLSTM + greedy CTC (beam search:
+ * b2o_crnn_forward_beam below).
  * crnn_in: (b,200,31) fp16 from b2o_warp_boxes (or b2o_crops_to_input).  labels: (b,48) int32,
  * merged + blank-free, padded with -1 -- the tensor recognize_from_boxes iterates (527-534).  */
 size_t b2o_crnn_workspace_bytes(int b);
@@ -166,6 +167,25 @@ int b2o_crnn_forward(b2o_ctx* ctx, const void* crnn_in_dev, int b, int32_t* labe
  * behaves as b2o_crnn_forward.                                                                                */
 int b2o_crnn_forward_scored(b2o_ctx* ctx, const void* crnn_in_dev, int b, int32_t* labels_dev, float* logp_dev,
                             void* ws_dev, size_t ws_bytes, void* stream);
+
+/* CTC prefix beam search, the greedy=False form of keras.backend.ctc_decode (which CTCDecoder does not use,
+ * recognition.py:169-184).  Per kept step t and class c the input is lp[t,c] = log(softmax(logits_t)_c + 1e-7), blank =
+ * k-1; a beam is a label prefix with the log-probabilities of ending in blank and in a label, scored by their logaddexp;
+ * each step every beam continues via blank, via its last label and by every label (a repeated label only after a
+ * blank), equal prefixes merge and the beam_width best survive.  Equal scores rank by label sequence, ascending, a
+ * prefix before its extensions.  Repeated letters are kept as the prefix search yields them (no merge_repeated pass).
+ * 1 <= beam_width <= B2O_MAX_BEAM_WIDTH, 1 <= top_paths <= beam_width, otherwise B2O_ERR_ARG.
+ * labels_dev (b, top_paths, 48) int32, best first, -1 padded; logp_dev (b, top_paths) float32, the beam scores,
+ * non-increasing (NULL: not written).  Paths beyond the number of distinct prefixes (tiny k) are all -1 with logp -inf.
+ * A crop's result is bit-identical in any batch and on every run.  A (b, 1, 48) result has the (b, 48) layout that
+ * b2o_pack_records(_scored) takes.
+ * b2o_ctc_beam_decode: the search alone on caller-supplied (b, 48, k) float32 logits, 2 <= k <= B2O_MAX_CLASSES.
+ * b2o_crnn_forward_beam: the CRNN of b2o_crnn_forward, its fc_12 logits into the workspace, then the search.       */
+#define B2O_MAX_BEAM_WIDTH 128
+int b2o_ctc_beam_decode(b2o_ctx* ctx, const float* logits_dev, int b, int k, int beam_width, int top_paths,
+                        int32_t* labels_dev, float* logp_dev, void* stream);
+int b2o_crnn_forward_beam(b2o_ctx* ctx, const void* crnn_in_dev, int b, int beam_width, int top_paths,
+                          int32_t* labels_dev, float* logp_dev, void* ws_dev, size_t ws_bytes, void* stream);
 
 /* Result records of Pipeline.recognize for the multi-GPU gather (pipeline.py:66-75; SURVEY.md 8(e)): one
  * fixed-size float32 row per image = [count][rec_boxes x (4,2) boxes * inv_scale[i] (tools.adjust_boxes,

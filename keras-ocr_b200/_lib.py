@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get("B2O_LIB") or os.path.join(_HERE, "libb2ocr.so")      
 
 CONV_AUTO, CONV_SIMT, CONV_TC_GENERIC = 0, 1, 2
 MAX_CLASSES = 1024            # B2O_MAX_CLASSES in include/b2ocr.h
+MAX_BEAM_WIDTH = 128          # B2O_MAX_BEAM_WIDTH in include/b2ocr.h
 
 
 class B2OError(RuntimeError):
@@ -74,6 +75,8 @@ SIGNATURES = {
     "b2o_crops_to_input": (_i, [_vp, _vp, _i, _vp, _vp]),
     "b2o_crnn_forward": (_i, [_vp, _vp, _i, _vp, _vp, _sz, _vp]),
     "b2o_crnn_forward_scored": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_ctc_beam_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "b2o_crnn_forward_beam": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_set_debug_taps": (_i, [_vp, _i]),
     "b2o_crnn_tap": (_i, [_vp, _c.c_char_p, _vp, _i, _vp, _sz, _vp]),
     "b2o_conv2d_test": (_i, [_vp, _vp, _i, _i, _i, _i, _c.POINTER(_c.c_float), _i, _i, _i,
@@ -248,6 +251,14 @@ class Context:
     def crnn_forward_scored(self, crnn_in, b, labels, logp, ws, ws_bytes, stream):
         self._check(self.lib.b2o_crnn_forward_scored(self.handle, crnn_in, b, labels, logp, ws, ws_bytes, stream),
                     "b2o_crnn_forward_scored")
+
+    def ctc_beam_decode(self, logits, b, k, beam_width, top_paths, labels, logp, stream):
+        self._check(self.lib.b2o_ctc_beam_decode(self.handle, logits, b, k, beam_width, top_paths, labels, logp, stream),
+                    "b2o_ctc_beam_decode")
+
+    def crnn_forward_beam(self, crnn_in, b, beam_width, top_paths, labels, logp, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_crnn_forward_beam(self.handle, crnn_in, b, beam_width, top_paths, labels, logp, ws,
+                                                   ws_bytes, stream), "b2o_crnn_forward_beam")
 
     def set_debug_taps(self, on):
         self._check(self.lib.b2o_set_debug_taps(self.handle, int(on)), "b2o_set_debug_taps")

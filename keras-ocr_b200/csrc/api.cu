@@ -15,6 +15,8 @@ int lstm_run(b2o_ctx* ctx, const float* xw, int xw_ld, int xw_off, const __half*
              int out_ld, int out_off, cudaStream_t st);
 int add_run(b2o_ctx* ctx, const __half* a, const __half* b, __half* o, long long n, cudaStream_t st);
 int fc_ctc_run(b2o_ctx* ctx, const __half* l2, int B, float* logits, int* labels, float* logp, cudaStream_t st);
+int ctc_beam_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths, int* labels, float* logp,
+                 cudaStream_t st);
 
 namespace {
 
@@ -604,8 +606,12 @@ extern "C" int b2o_crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_
   return b2o_crnn_forward_scored(ctx, crnn_in, b, labels, nullptr, ws, ws_bytes, stream);
 }
 
-extern "C" int b2o_crnn_forward_scored(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, float* logp, void* ws,
-                                       size_t ws_bytes, void* stream) {
+namespace {
+
+// The CRNN through fc_12 + greedy CTC.  keep_logits: the fp32 logits always go to the workspace's logits slot (the beam
+// search reads them there); otherwise only with the debug taps on.
+int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, float* logp, bool keep_logits, void* ws,
+                 size_t ws_bytes, void* stream) {
   if (!ctx) return B2O_ERR_ARG;
   if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_forward: CRNN weights not loaded"); return B2O_ERR_STATE; }
   DeviceGuard guard(ctx->device);
@@ -669,9 +675,52 @@ extern "C" int b2o_crnn_forward_scored(b2o_ctx* ctx, const void* crnn_in, int b,
   B2O_RETURN_IF(lstm_run(ctx, xw2f, 1024, 0, ctx->lstm_u[2], b, 0, l2, 256, 0, st));
   B2O_RETURN_IF(lstm_run(ctx, xw2f, 1024, 512, ctx->lstm_u[3], b, 1, l2, 256, 128, st));
   // fc_12 + discard + greedy CTC (321-333)
-  B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, ctx->debug_taps ? reinterpret_cast<float*>(base + p.off_logits) : nullptr, labels,
-                           logp, st));
+  B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, keep_logits || ctx->debug_taps ? reinterpret_cast<float*>(base + p.off_logits) : nullptr,
+                           labels, logp, st));
   return B2O_OK;
+}
+
+bool beam_args_ok(b2o_ctx* ctx, const char* fn, int k, int beam_width, int top_paths) {
+  if (k < 2 || k > B2O_MAX_CLASSES) { ctx->set_error(std::string(fn) + ": k must be in [2, 1024]"); return false; }
+  if (beam_width < 1 || beam_width > B2O_MAX_BEAM_WIDTH) {
+    ctx->set_error(std::string(fn) + ": beam_width must be in [1, 128]");
+    return false;
+  }
+  if (top_paths < 1 || top_paths > beam_width) {
+    ctx->set_error(std::string(fn) + ": top_paths must be in [1, beam_width]");
+    return false;
+  }
+  return true;
+}
+
+}  // namespace
+
+extern "C" int b2o_crnn_forward_scored(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, float* logp, void* ws,
+                                       size_t ws_bytes, void* stream) {
+  return crnn_forward(ctx, crnn_in, b, labels, logp, false, ws, ws_bytes, stream);
+}
+
+extern "C" int b2o_crnn_forward_beam(b2o_ctx* ctx, const void* crnn_in, int b, int beam_width, int top_paths,
+                                     int32_t* labels, float* logp, void* ws, size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_forward_beam: CRNN weights not loaded"); return B2O_ERR_STATE; }
+  if (!beam_args_ok(ctx, "b2o_crnn_forward_beam", ctx->n_classes, beam_width, top_paths)) return B2O_ERR_ARG;
+  if (b == 0) return B2O_OK;
+  // the greedy labels of fc_ctc_kernel go to the first b * 48 entries of `labels`, which the beam search then overwrites
+  B2O_RETURN_IF(crnn_forward(ctx, crnn_in, b, labels, nullptr, true, ws, ws_bytes, stream));
+  DeviceGuard guard(ctx->device);
+  const float* logits = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(ws) + plan_crnn(b).off_logits);
+  return ctc_beam_run(ctx, logits, b, ctx->n_classes, beam_width, top_paths, labels, logp,
+                      reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2o_ctc_beam_decode(b2o_ctx* ctx, const float* logits, int b, int k, int beam_width, int top_paths,
+                                   int32_t* labels, float* logp, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!beam_args_ok(ctx, "b2o_ctc_beam_decode", k, beam_width, top_paths)) return B2O_ERR_ARG;
+  if (b < 0 || (b > 0 && (!logits || !labels))) { ctx->set_error("b2o_ctc_beam_decode: bad argument"); return B2O_ERR_ARG; }
+  DeviceGuard guard(ctx->device);
+  return ctc_beam_run(ctx, logits, b, k, beam_width, top_paths, labels, logp, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b2o_set_debug_taps(b2o_ctx* ctx, int on) {

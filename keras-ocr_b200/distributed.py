@@ -129,7 +129,8 @@ def _host_records(pipeline, local, per_rank, max_boxes):
     return pack_records(counts, boxes, labels, per_rank, max_boxes)
 
 
-def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_scores=False):
+def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_scores=False, beam_width=None,
+                      top_paths=1):
     """Run ``pipeline.recognize`` on this rank's shard of ``images`` and gather to rank 0.
 
     ``images`` is the global batch (every rank passes the same list and takes its contiguous slice) or, with
@@ -142,8 +143,11 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
     Returns, on rank 0, the same list-of-lists as ``Pipeline.recognize`` for ALL images (global
     order); ``None`` on the other ranks.  Boxes are in source-image pixels.  ``return_scores=True``: the words are
     (text, box, detection_score, confidence) as ``Pipeline.recognize(return_scores=True)`` returns them, carried in
-    the scored record layout (device records only).
+    the scored record layout (device records only).  ``beam_width``: beam-search decoding
+    (``recognition.check_beam``); records carry the best path only, so ``top_paths`` > 1 raises ``ValueError``.
     """
+    from .pipeline import check_records_beam
+    check_records_beam(beam_width, top_paths)
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
     if presharded:
@@ -159,6 +163,8 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
     if return_scores and not native:
         raise NotImplementedError("return_scores=True needs this package's Pipeline with its own Detector and Recognizer")
     sk = {"scores": True} if return_scores else {}      # pipelines without the flag keep working unscored
+    if beam_width is not None:
+        sk["beam_width"] = beam_width
     if native:
         if getattr(pipeline, "records_counts", None) is not None:
             state = pipeline.records_begin(mine, rows=per_rank, rec_boxes=16 if max_boxes == "auto" else max_boxes, **sk)
@@ -170,7 +176,8 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
             local = pipeline.recognize_records(mine, rows=per_rank, rec_boxes=max_boxes, **sk)
         device = None                                   # already where the backend wants it
     else:
-        result = pipeline.recognize(mine) if len(mine) else []
+        rk = {} if beam_width is None else {"recognition_kwargs": {"beam_width": beam_width}}
+        result = pipeline.recognize(mine, **rk) if len(mine) else []
         if max_boxes == "auto":
             max_boxes = agree_max_boxes([len(g) for g in result], _collective_device(pipeline))
         local = _host_records(pipeline, result, per_rank, max_boxes)
@@ -249,9 +256,12 @@ class ShardedStream:
     asynchronous copy into pinned memory; any other pipeline (``recognize`` only) is served too, without the overlap.
     ``max_boxes``: words a record holds (an image with more raises ``RecordOverflow`` on rank 0 when its batch is
     decoded) or ``"auto"`` (sized per batch by ``agree_max_boxes``).  ``return_scores=True``: words as
-    ``recognize_sharded(return_scores=True)`` returns them (device records only)."""
+    ``recognize_sharded(return_scores=True)`` returns them (device records only).  ``beam_width``: as
+    ``recognize_sharded``."""
 
-    def __init__(self, pipeline, max_boxes=128, return_scores=False):
+    def __init__(self, pipeline, max_boxes=128, return_scores=False, beam_width=None, top_paths=1):
+        from .pipeline import check_records_beam
+        check_records_beam(beam_width, top_paths)
         self.pipeline, self.max_boxes = pipeline, max_boxes
         self.world = dist.get_world_size() if dist.is_initialized() else 1
         self.rank = dist.get_rank() if dist.is_initialized() else 0
@@ -264,6 +274,10 @@ class ShardedStream:
                                       "Recognizer")
         self.return_scores = return_scores
         self._sk = {"scores": True} if return_scores else {}
+        self._rk = {}
+        if beam_width is not None:
+            self._sk["beam_width"] = beam_width
+            self._rk = {"recognition_kwargs": {"beam_width": beam_width}}
         self._pending = None                             # (host blocks, event or None) of the batch in flight
         self._side = None                                # communication stream (CUDA tensors only)
         self._keep = None
@@ -293,7 +307,7 @@ class ShardedStream:
             device = None
         else:
             previous = self._take_pending()
-            result = self.pipeline.recognize(images)
+            result = self.pipeline.recognize(images, **self._rk)
             if max_boxes == "auto":
                 max_boxes = agree_max_boxes([len(g) for g in result], _collective_device(self.pipeline))
             local = _host_records(self.pipeline, result, rows, max_boxes)

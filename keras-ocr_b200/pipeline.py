@@ -5,6 +5,13 @@ import torch
 from . import detection, recognition, tools
 
 
+def check_records_beam(beam_width=None, top_paths=1):
+    """``recognition.check_beam`` for the records path, whose fixed-size records carry one reading per word."""
+    recognition.check_beam(beam_width, top_paths)
+    if top_paths != 1:
+        raise ValueError("records carry the best path only: top_paths must be 1")
+
+
 class Pipeline:
     """A wrapper for a combination of detector and recognizer.
 
@@ -126,13 +133,14 @@ class Pipeline:
         st[key] = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
         st[key].copy_(t, non_blocking=True)
 
-    def _stage_recognize(self, st):
+    def _stage_recognize(self, st, beam):
         det, rec = self.detector, self.recognizer
         bst = st.pop("boxes_state")
         boxes, counts = det.boxes_finish(bst)
         box_scores, logp = bst["box_scores"], None
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
-                                                 image_index=bst["image_index"], with_scores=box_scores is not None)
+                                                 image_index=bst["image_index"], with_scores=box_scores is not None,
+                                                 **beam)
         if box_scores is not None:
             labels, logp = labels
             self._to_host(st, "box_scores_host", box_scores)
@@ -150,17 +158,19 @@ class Pipeline:
         st["done"].synchronize()
         boxes_host, counts = st["boxes_host"].numpy(), st["counts"]
         d2h = boxes_host.nbytes + counts.nbytes
+        texts, conf = [], np.zeros(0, np.float32)
         if "labels_host" in st:
             labels_host = st["labels_host"].numpy()
             d2h += labels_host.nbytes
-            texts = recognition.labels_to_text(labels_host, self.recognizer.alphabet)
-        else:
-            texts = []
+            logp_host = st["logp_host"].numpy() if "logp_host" in st else None
+            texts, c = recognition.decode_paths(labels_host, self.recognizer.alphabet, logp_host)
+            if logp_host is not None:
+                conf = c
+                d2h += logp_host.nbytes
         scored = "box_scores_host" in st
         if scored:
             box_scores = st["box_scores_host"].numpy()
-            conf = recognition.confidences(st["logp_host"].numpy()) if "logp_host" in st else np.zeros(0, np.float32)
-            d2h += box_scores.nbytes + conf.nbytes
+            d2h += box_scores.nbytes
         self.last_stats["d2h_bytes"] += int(d2h)
         out, start = [], 0
         for i, (c, scale) in enumerate(zip(counts, st["scales"])):
@@ -182,6 +192,10 @@ class Pipeline:
         the coordinates of the *input* image.  ``return_scores=True``: (text, box, detection_score, confidence)
         tuples instead -- the box's detection score (``Detector.detect(return_scores=True)``) and the word's
         confidence exp(S) in (0, 1] (``recognition.confidences``); texts and boxes are those of the default call.
+        ``recognition_kwargs`` may hold ``beam_width`` / ``top_paths`` (``recognition.check_beam``): CTC beam search
+        instead of greedy decoding, boxes unchanged; with ``top_paths = P > 1`` the text of every word is a list of P
+        readings and its confidence a list of P floats, best first.  Injected recognizers get ``recognition_kwargs``
+        as they are.
         """
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
@@ -192,6 +206,9 @@ class Pipeline:
             detection_kwargs = {}
         if recognition_kwargs is None:
             recognition_kwargs = {}
+        if self._native():
+            beam = {k: recognition_kwargs[k] for k in ("beam_width", "top_paths") if k in recognition_kwargs}
+            recognition.check_beam(**beam)
         if not self._native():
             if return_scores:
                 raise NotImplementedError("return_scores=True needs this package's Detector and Recognizer; injected "
@@ -213,26 +230,31 @@ class Pipeline:
                 states.append(self._stage_detect(images[bounds[step]:bounds[step + 1]], pad_to, thresholds,
                                                  with_scores=return_scores))
             if 1 <= step <= k:
-                self._stage_recognize(states[step - 1])
+                self._stage_recognize(states[step - 1], beam)
             if step >= 2:
                 out.extend(self._stage_finish(states[step - 2]))
                 states[step - 2] = None
         return out
 
-    def recognize_records(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False):
+    def recognize_records(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
+                          top_paths=1):
         """``recognize`` without the trip to the host: returns the results as a CUDA float32 tensor of fixed-size
         per-image records, ``(rows, b2o_record_floats(rec_boxes))`` = [count | rec_boxes x (4,2) boxes in source
         pixels | rec_boxes x 48 int8 labels] (``distributed.unpack_blocks`` decodes it; rows beyond ``len(images)``
         carry count -1).  This is the payload of the multi-GPU gather (SURVEY.md 8(e)): only the per-image box
         counts ever reach the host on this rank.  ``scores=True``: the scored layout,
         ``(rows, b2o_record_floats_scored(rec_boxes))``, which appends [rec_boxes detection scores | rec_boxes
-        path log-probabilities] to that record."""
-        return self.records_end(self.records_begin(images, rows, rec_boxes, detection_kwargs, scores))
+        path log-probabilities] to that record.  ``beam_width``: the words are beam-search decoded
+        (``recognition.check_beam``); a record carries the best path only, so ``top_paths`` > 1 raises ``ValueError``."""
+        return self.records_end(self.records_begin(images, rows, rec_boxes, detection_kwargs, scores, beam_width,
+                                                   top_paths))
 
-    def records_begin(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False):
+    def records_begin(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
+                      top_paths=1):
         """First half of ``recognize_records``: queues resize/pad, CRAFT and getBoxes and returns at once (no
         synchronisation), so the caller can use the host while the GPU works (``distributed.ShardedStream`` decodes the
         previous batch's words here).  Pass the returned state to ``records_end``."""
+        check_records_beam(beam_width, top_paths)
         assert self._native(), "recognize_records needs this package's Detector and Recognizer"
         assert len(self.recognizer.alphabet) + 1 <= 127, "record labels travel as int8: alphabets up to 126 characters"
         if not isinstance(images, (np.ndarray, torch.Tensor)):
@@ -246,7 +268,7 @@ class Pipeline:
         rows = n if rows is None else int(rows)
         assert rows >= n and rows > 0
         self.last_stats = {"h2d_bytes": 0, "d2h_bytes": 0}
-        state = {"n": n, "rows": rows, "rec_boxes": rec_boxes, "scores": bool(scores)}
+        state = {"n": n, "rows": rows, "rec_boxes": rec_boxes, "scores": bool(scores), "beam_width": beam_width}
         if n:
             plans = self._plans(images)
             state["st"] = self._stage_detect(images, (max(p[1] for p in plans), max(p[2] for p in plans)), thresholds,
@@ -284,7 +306,8 @@ class Pipeline:
         bst = st.pop("boxes_state")
         boxes = state["boxes"]
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
-                                                 image_index=bst["image_index"], with_scores=scored)
+                                                 image_index=bst["image_index"], with_scores=scored,
+                                                 beam_width=state.get("beam_width"))
         inv = torch.tensor([1.0 / s for s in st["scales"]], dtype=torch.float32).to(det.device, non_blocking=True)
         stream = torch.cuda.current_stream(det.device).cuda_stream
         ptr = lambda t: t.data_ptr() if t is not None else None      # noqa: E731

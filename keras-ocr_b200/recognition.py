@@ -41,6 +41,37 @@ def confidences(logp):
     return np.minimum(np.exp(np.asarray(logp, dtype=np.float32)), np.float32(1.0))
 
 
+def check_beam(beam_width=None, top_paths=1):
+    """Validates a decoder choice before anything is launched (``ValueError`` otherwise): ``beam_width=None`` is greedy
+    CTC (the default, and then ``top_paths`` must be 1); an int 1 <= ``beam_width`` <= 128 is CTC prefix beam search
+    (``b2o_crnn_forward_beam``) returning the ``top_paths`` best readings, 1 <= ``top_paths`` <= ``beam_width``."""
+    def is_int(v):
+        return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+    if not is_int(top_paths) or top_paths < 1:
+        raise ValueError(f"top_paths must be an int >= 1, got {top_paths!r}")
+    if beam_width is None:
+        if top_paths != 1:
+            raise ValueError("top_paths > 1 needs beam search: pass beam_width")
+        return
+    if not is_int(beam_width) or not 1 <= beam_width <= _lib.MAX_BEAM_WIDTH:
+        raise ValueError(f"beam_width must be None or an int in [1, {_lib.MAX_BEAM_WIDTH}], got {beam_width!r}")
+    if top_paths > beam_width:
+        raise ValueError(f"top_paths ({top_paths}) must not exceed beam_width ({beam_width})")
+
+
+def decode_paths(labels, alphabet=DEFAULT_ALPHABET, logp=None):
+    """Host labels -> texts, and logp -> confidences (None without logp).  (B,48) labels / (B,) logp give B strings and
+    a float32 array, as the greedy decoder returns them; (B,P,48) / (B,P) -- ``top_paths = P > 1`` -- give B lists of P
+    strings and B lists of P confidences, best first."""
+    labels = np.asarray(labels)
+    if labels.ndim == 2:
+        return labels_to_text(labels, alphabet), (None if logp is None else confidences(logp))
+    b, p = labels.shape[:2]
+    flat = labels_to_text(labels.reshape(b * p, STEPS), alphabet)
+    texts = [flat[i * p:(i + 1) * p] for i in range(b)]
+    return texts, (None if logp is None else [list(row) for row in confidences(logp)])
+
+
 class Recognizer:
     """A text recognizer using the CRNN architecture, running as sm_90a CUDA kernels.
 
@@ -151,9 +182,12 @@ class Recognizer:
                             torch.cuda.current_stream(self.device).cuda_stream, color=color)
         return crnn_in, crops
 
-    def predict_device(self, crnn_in, with_scores=False):
+    def predict_device(self, crnn_in, with_scores=False, beam_width=None, top_paths=1):
         """CRNN + greedy CTC.  crnn_in: (B,200,31) fp16 -> labels (B,48) int32 (-1 padded).  ``with_scores``: returns
-        (labels, logp) with logp (B,) float32 the greedy path's log-probability (``b2o_crnn_forward_scored``)."""
+        (labels, logp) with logp (B,) float32 the greedy path's log-probability (``b2o_crnn_forward_scored``).
+        ``beam_width``: CTC prefix beam search instead (``b2o_crnn_forward_beam``, see ``check_beam``), logp = the beam
+        scores; ``top_paths > 1`` gives labels (B,P,48) and logp (B,P), best first."""
+        check_beam(beam_width, top_paths)
         b = crnn_in.shape[0]
         labels = torch.empty((b, STEPS), dtype=torch.int32, device=self.device)
         nbytes = self.ctx.crnn_workspace_bytes(b)
@@ -163,7 +197,13 @@ class Recognizer:
         ws = self._ws
         stream = torch.cuda.current_stream(self.device).cuda_stream
         logp = None
-        if with_scores:
+        if beam_width is not None:
+            lead = (b,) if top_paths == 1 else (b, top_paths)
+            labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
+            logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
+            self.ctx.crnn_forward_beam(crnn_in.data_ptr(), b, int(beam_width), int(top_paths), labels.data_ptr(),
+                                       logp.data_ptr() if with_scores else None, ws.data_ptr(), nbytes, stream)
+        elif with_scores:
             logp = torch.empty((b,), dtype=torch.float32, device=self.device)
             self.ctx.crnn_forward_scored(crnn_in.data_ptr(), b, labels.data_ptr(), logp.data_ptr(), ws.data_ptr(), nbytes,
                                          stream)
@@ -180,9 +220,12 @@ class Recognizer:
                           torch.cuda.current_stream(self.device).cuda_stream)
         return out
 
-    def recognize_crops(self, crops, return_scores=False):
+    def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1):
         """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str].
-        ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``."""
+        ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``.  ``beam_width``: beam search
+        decoding (``check_beam``); with ``top_paths = P > 1`` each text is a list of P strings and each confidence a
+        list of P floats, best first (``decode_paths``)."""
+        check_beam(beam_width, top_paths)
         t = crops if isinstance(crops, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(crops))
         t = t.to(self.device).contiguous()
         b = t.shape[0]
@@ -192,29 +235,34 @@ class Recognizer:
         crnn_in = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + ((3,) if self.color else ()), dtype=torch.float16, device=self.device)
         self.ctx.crops_to_input(t.data_ptr(), b, crnn_in.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream,
                                 color=self.color)
+        beam = {"beam_width": beam_width, "top_paths": top_paths}
         if not return_scores:
-            return labels_to_text(self.predict_device(crnn_in).cpu().numpy(), self.alphabet)
-        labels, logp = self.predict_device(crnn_in, with_scores=True)
-        return list(zip(labels_to_text(labels.cpu().numpy(), self.alphabet), confidences(logp.cpu().numpy())))
+            return decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
+        labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
+        return list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
 
-    def recognize(self, image):
+    def recognize(self, image, beam_width=None, top_paths=1):
         """Recognize text from a single pre-cropped image (reference recognition.py:467-489): fit to
-        200x31 with zero fill (host, as upstream), gray conversion, then the CUDA CRNN."""
+        200x31 with zero fill (host, as upstream), gray conversion, then the CUDA CRNN.  ``beam_width`` / ``top_paths``:
+        as ``recognize_crops``."""
         import cv2
 
+        check_beam(beam_width, top_paths)
         image = tools.read_and_fit(filepath_or_array=image, width=TARGET_WIDTH, height=TARGET_HEIGHT, cval=0)
         if not self.color and image.ndim == 3 and image.shape[-1] == 3:      # recognition.py:481-483
             image = cv2.cvtColor(image, code=cv2.COLOR_RGB2GRAY)
-        return self.recognize_crops(np.ascontiguousarray(image.reshape((1, TARGET_HEIGHT, TARGET_WIDTH) + ((3,) if self.color else ()))))[0]
+        return self.recognize_crops(np.ascontiguousarray(image.reshape((1, TARGET_HEIGHT, TARGET_WIDTH) + ((3,) if self.color else ()))),
+                                    beam_width=beam_width, top_paths=top_paths)[0]
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
-                                    with_scores=False):
+                                    with_scores=False, beam_width=None, top_paths=1):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
-        (``with_scores``: (labels, logp (B,) f32 CUDA), see ``predict_device``).
+        (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths``: see ``predict_device``).
 
         Optional device-side by-products of the earlier stages, so that nothing but the kernel launches is
         left to do once the host knows the counts: ``gray`` (N,H,W) u8 from ``b2o_resize_pad_batch``;
         ``flat`` (>=B,4,2) / ``image_index`` (>=B,) from ``b2o_compact_boxes``."""
+        check_beam(beam_width, top_paths)
         counts = np.asarray(counts)
         m = boxes.shape[1]
         total = int(np.minimum(counts, m).sum())
@@ -232,12 +280,14 @@ class Recognizer:
             self.ctx.compact_boxes(boxes.data_ptr(), counts_dev.data_ptr(), n, m, flat.data_ptr(),
                                    image_index.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
-        return self.predict_device(crnn_in, with_scores=with_scores)
+        return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths)
 
     # ------------------------------------------------------------------ reference API
-    def recognize_from_boxes(self, images, box_groups, return_scores=False, **kwargs) -> typing.List[typing.List[str]]:
+    def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1,
+                             **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
-        (text, confidence) pair instead, see ``confidences``."""
+        (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths``: as ``recognize_crops``."""
+        check_beam(beam_width, top_paths)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
 
@@ -253,10 +303,11 @@ class Recognizer:
         flat_t = torch.from_numpy(np.ascontiguousarray(flat)).to(self.device)
         idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
         crnn_in, _ = self.warp_device(images_t if self.color else self.gray_device(images_t), flat_t, idx)
+        beam = {"beam_width": beam_width, "top_paths": top_paths}
         if return_scores:
-            labels, logp = self.predict_device(crnn_in, with_scores=True)
-            predictions = list(zip(labels_to_text(labels.cpu().numpy(), self.alphabet), confidences(logp.cpu().numpy())))
+            labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
+            predictions = list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
         else:
-            predictions = labels_to_text(self.predict_device(crnn_in).cpu().numpy(), self.alphabet)
+            predictions = decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
         ends = np.cumsum(counts)
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]

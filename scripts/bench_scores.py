@@ -1,11 +1,13 @@
-"""bench_scores.py -- what detection scores and word confidences cost: ``Pipeline.recognize`` with and without
-``return_scores=True`` on the workload of bench.py (32 pages 768x768, scale 2 -> 1536x1536, sources resident in HBM).
+"""bench_scores.py -- what detection scores, word confidences and beam-search decoding cost: ``Pipeline.recognize``
+with and without ``return_scores=True``, and with ``recognition_kwargs={"beam_width": W}`` for every W given, on the
+workload of bench.py (32 pages 768x768, scale 2 -> 1536x1536, sources resident in HBM).
 
-    python scripts/bench_scores.py [--steps K] [--warmup W] [--rounds R]
+    python scripts/bench_scores.py [--steps K] [--warmup W] [--rounds R] [--beam-width W [W ...]]
 
-The two calls are timed alternately, R rounds of K steps each (CUDA events around K steps bracketed by a device
-synchronise), so that drifting clocks and other work on the host hit both alike; prints one JSON line with the medians,
-the spread over the rounds and the card's name and power limit.  Writes nothing.
+The calls are timed alternately, R rounds of K steps each (CUDA events around K steps bracketed by a device
+synchronise), so that drifting clocks and other work on the host hit all alike; prints one JSON line with the medians,
+the spread over the rounds, the rendered words each call reads correctly (``bench.words_read``) and the card's name
+and power limit.  Writes nothing.
 """
 import argparse
 import json
@@ -34,6 +36,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--beam-width", type=int, nargs="+", default=[])
     args = ap.parse_args()
 
     import torch
@@ -49,8 +52,11 @@ def main():
     det = Detector(weights=W.synthetic_craft_weights(3, textlike=True), device=0)
     rec = Recognizer(weights=W.synthetic_crnn_weights(2, decisive=True), device=0)
     pipe = Pipeline(detector=det, recognizer=rec, scale=bench.SCALE, max_size=2048)
-    pages = torch.from_numpy(bench.make_pages(0)).to(device)
+    pages_host, page_words, page_rects = bench.make_pages(0, with_layout=True)
+    pages = torch.from_numpy(pages_host).to(device)
     calls = {"default": lambda: pipe.recognize(pages), "scored": lambda: pipe.recognize(pages, return_scores=True)}
+    for w in args.beam_width:
+        calls[f"beam{w}"] = lambda w=w: pipe.recognize(pages, recognition_kwargs={"beam_width": w})
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -77,6 +83,19 @@ def main():
         "default_ms_spread": [min(ms["default"]), max(ms["default"])],
         "scored_ms_spread": [min(ms["scored"]), max(ms["scored"])],
         "overhead": statistics.median(ms["scored"]) / statistics.median(ms["default"]) - 1.0})
+    default_words = [t for g in calls["default"]() for t, _ in g]
+    for k, fn in calls.items():
+        if k == "scored":
+            continue
+        result = fn()
+        hit, rendered = bench.words_read(result, page_words, page_rects)
+        line[f"{k}_words_read"] = [hit, rendered]
+        if k != "default":
+            line[f"{k}_ms_per_step"] = statistics.median(ms[k])
+            line[f"{k}_ms_spread"] = [min(ms[k]), max(ms[k])]
+            line[f"{k}_overhead"] = statistics.median(ms[k]) / statistics.median(ms["default"]) - 1.0
+            line[f"{k}_words_differing_from_default"] = sum(a != b for a, b in zip([t for g in result for t, _ in g],
+                                                                                  default_words))
     print(json.dumps(line))
 
 
