@@ -256,6 +256,17 @@ typedef struct {
 } b2o_conv_test_desc;
 int b2o_conv_test(b2o_ctx* ctx, const b2o_conv_test_desc* desc, void* stream);
 
+/* The plan b2o_warp_boxes derives from each box (test hook, not on the product path): get_rotated_box ordering,
+ * get_rotated_width_height, the fp64 cv2.getPerspectiveTransform solve and the closed-form 3x3 inverse.  boxes: (n,4,2)
+ * float32; plans: n records of 88 bytes.  m = inverse homography (destination -> source, row major), dw, dh = dsize of
+ * warpPerspective; valid = 0 where warpBox raises ZeroDivisionError (m, dw and dh are then 0) or the fp64 system is
+ * singular, and b2o_warp_boxes writes an all-zero crop for such a box.                                           */
+typedef struct {
+  double m[9];
+  int32_t dw, dh, valid;
+} b2o_warp_plan;
+int b2o_warp_plan_test(b2o_ctx* ctx, const float* boxes_dev, int n, b2o_warp_plan* plans_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -83,7 +83,11 @@ SIGNATURES = {
                              _c.POINTER(_c.c_float), _c.POINTER(_c.c_float), _i,
                              _c.POINTER(_c.c_float), _c.POINTER(_c.c_float), _vp, _i, _vp]),
     "b2o_conv_test": (_i, [_vp, _c.POINTER(_ConvTestDesc), _vp]),
+    "b2o_warp_plan_test": (_i, [_vp, _vp, _i, _vp, _vp]),
 }
+
+# b2o_warp_plan (include/b2ocr.h), field for field: 9 float64, 3 int32, padded to 88 bytes
+WARP_PLAN_DTYPE = np.dtype([("m", "<f8", (9,)), ("dw", "<i4"), ("dh", "<i4"), ("valid", "<i4")], align=True)
 
 _lib = None
 
@@ -286,6 +290,10 @@ class Context:
                           int(relu), _fptr(keep[3]), _fptr(keep[4]), out, out_ld, int(out_f32), int(write_full),
                           pool, pool_ld, up, up_ld, *[_fptr(a) for a in tail], scores, engine)
         self._check(self.lib.b2o_conv_test(self.handle, ctypes.byref(d), stream), "b2o_conv_test")
+
+    def warp_plan_test(self, boxes, n, plans, stream):
+        """b2o_warp_plan_test: ``plans`` addresses n records of WARP_PLAN_DTYPE on the device."""
+        self._check(self.lib.b2o_warp_plan_test(self.handle, boxes, n, plans, stream), "b2o_warp_plan_test")
 
 
 _contexts = {}

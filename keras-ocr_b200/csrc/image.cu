@@ -1,6 +1,7 @@
 // image.cu -- the OpenCV image stages of Pipeline.recognize as CUDA kernels, bit-compatible with
 // OpenCV 4.x fixed-point arithmetic (models of the arithmetic are pinned against cv2 in
-// tests/test_cv_models.py):
+// tests/test_cv_models.py and tests/test_image_refs.py; these kernels against the models, plan included, in
+// tests/test_gpu_image_stages.py):
 //   resize_pad_kernel : cv2.resize INTER_LINEAR on uint8 (tools.py:394-396) + tools.pad(255) (356-375)
 //   gray_kernel       : cv2.cvtColor(RGB2GRAY) (recognition.py:510)
 //   warp_kernel       : tools.warpBox (tools.py:61-117): get_rotated_box ordering (533-581, rectangle
@@ -37,15 +38,16 @@ __global__ void resize_pad_kernel(const uint8_t* __restrict__ src, int hs, int w
     return;
   }
   // OpenCV: scale = 1 / (dsize / ssize), source coordinate at pixel centres, float fractions,
-  // 11-bit coefficients (INTER_RESIZE_COEF_BITS), horizontal pass first.
-  float fx = static_cast<float>((x + 0.5) * scale_x - 0.5);
+  // 11-bit coefficients (INTER_RESIZE_COEF_BITS), horizontal pass first.  (x + 0.5) * scale - 0.5 rounds the
+  // product and the difference separately, as OpenCV does: a contracted DFMA would round once.
+  float fx = static_cast<float>(__dadd_rn(__dmul_rn(x + 0.5, scale_x), -0.5));
   int sx = static_cast<int>(floorf(fx));
   fx -= sx;
   if (sx < 0) { fx = 0.f; sx = 0; }
   if (sx >= ws - 1) { fx = 0.f; sx = ws - 1; }
   const int sx1 = min(sx + 1, ws - 1);
   const int a0 = __float2int_rn((1.f - fx) * 2048.f), a1 = __float2int_rn(fx * 2048.f);
-  float fy = static_cast<float>((y + 0.5) * scale_y - 0.5);
+  float fy = static_cast<float>(__dadd_rn(__dmul_rn(y + 0.5, scale_y), -0.5));
   const int sy = static_cast<int>(floorf(fy));
   fy -= sy;
   const int b0 = __float2int_rn((1.f - fy) * 2048.f), b1 = __float2int_rn(fy * 2048.f);
@@ -73,11 +75,9 @@ __global__ void gray_kernel(const uint8_t* __restrict__ img, long long total, ui
 }
 
 // ------------------------------------------------------------------------------------ warpBox
-struct WarpPlan {
-  double m[9];     // inverse homography (destination -> source), fp64 like cv2
-  int dw, dh;      // dsize of warpPerspective
-  int valid;
-};
+// b2o_warp_plan (include/b2ocr.h): m[9] = inverse homography (destination -> source), fp64 like cv2; dw, dh = dsize
+// of warpPerspective; valid = 0 where warpBox raises ZeroDivisionError (or the system is singular).
+using WarpPlan = b2o_warp_plan;
 
 __device__ double dist2(const float* a, const float* b) {
   const double dx = static_cast<double>(a[0]) - static_cast<double>(b[0]);
@@ -89,7 +89,7 @@ __device__ void plan_warp(const float* q /*4x2*/, int target_w, int target_h, Wa
   plan->valid = 0;
   // --- get_rotated_box on a rectangle: stable sort by x, split, order by y / by distance ---------
   int idx[4] = {0, 1, 2, 3};
-  for (int i = 1; i < 4; ++i) {              // insertion sort == numpy's small-array argsort (stable)
+  for (int i = 1; i < 4; ++i) {              // insertion sort == numpy's argsort(kind="stable")
     const int v = idx[i];
     int j = i - 1;
     while (j >= 0 && q[2 * idx[j]] > q[2 * v]) { idx[j + 1] = idx[j]; --j; }
@@ -244,6 +244,15 @@ warp_kernel(const uint8_t* __restrict__ gray, int n, int H, int W, const float* 
   }
 }
 
+// b2o_warp_plan_test: plan_warp alone, one thread per box.  A degenerate box leaves m, dw and dh zero.
+__global__ void warp_plan_kernel(const float* __restrict__ boxes, int n, WarpPlan* __restrict__ plans) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  WarpPlan p = {};
+  plan_warp(boxes + static_cast<size_t>(k) * 8, kCropW, kCropH, &p);
+  plans[k] = p;
+}
+
 // crops (k,31,200[,ch]) u8 -> CRNN input (k,200,31[,ch]) fp16 = crop / 255 after Permute((2,1,3)) and the axis flip
 __global__ void crops_to_input_kernel(const uint8_t* __restrict__ crops, long long total, int ch, __half* __restrict__ out) {
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -323,6 +332,16 @@ extern "C" int b2o_warp_boxes(b2o_ctx* ctx, const uint8_t* gray, int n, int h, i
 extern "C" int b2o_warp_boxes_color(b2o_ctx* ctx, const uint8_t* rgb, int n, int h, int w, const float* boxes,
                                     const int32_t* image_index, int n_boxes, uint8_t* crops, void* crnn_in, void* stream) {
   return warp_boxes_impl(ctx, rgb, 3, n, h, w, boxes, image_index, n_boxes, crops, crnn_in, stream);
+}
+
+extern "C" int b2o_warp_plan_test(b2o_ctx* ctx, const float* boxes, int n, b2o_warp_plan* plans, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  DeviceGuard guard(ctx->device);
+  if (n == 0) return B2O_OK;
+  if (!boxes || !plans || n < 0) { ctx->set_error("b2o_warp_plan_test: bad argument"); return B2O_ERR_ARG; }
+  warp_plan_kernel<<<(n + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(boxes, n, plans);
+  B2O_LAUNCH_CHECK(ctx);
+  return B2O_OK;
 }
 
 static int crops_to_input_impl(b2o_ctx* ctx, const uint8_t* crops, int ch, int b, void* crnn_in, void* stream) {

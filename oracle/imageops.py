@@ -161,13 +161,15 @@ def order_corners(points):
         near = np.abs(rect[:, None, :] - pts[None, :, :].astype(np.float64)).max(-1).min(-1)
         if near.max() > 1e-3:
             pts = rect
-    by_x = pts[np.argsort(pts[:, 0]), :]
+    # kind="stable": upstream's default argsort breaks ties (a square at 45 degrees ties in x) by whatever the host's
+    # NumPy sort does -- with AVX-512 it is not stable on 4 elements.  The stable order is the one the kernel follows.
+    by_x = pts[np.argsort(pts[:, 0], kind="stable"), :]
     left, right = by_x[:2], by_x[2:]
-    left = left[np.argsort(left[:, 1]), :]
+    left = left[np.argsort(left[:, 1], kind="stable"), :]
     tl, bl = left
     delta = right.astype(np.float64) - tl.astype(np.float64)[np.newaxis]   # cdist works in float64
     dist = np.sqrt((delta ** 2).sum(axis=1))
-    br, tr = right[np.argsort(dist)[::-1], :]
+    br, tr = right[np.argsort(dist, kind="stable")[::-1], :]
     return np.array([tl, tr, br, bl], dtype="float32")
 
 
