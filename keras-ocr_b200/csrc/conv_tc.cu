@@ -17,9 +17,11 @@
 //   (CRAFT conv_cls.*, STN) also run on the tensor cores.
 // * warp roles: thread 0 of warpgroup 0 = TMA producer (one ring of stages; a stage is the A box of one (tap group,
 //   channel chunk) plus, unless the filter bank is resident, its B boxes, all on one mbarrier); warpgroups 1 and 2 =
-//   consumers, one per 64-pixel half of the tile: wgmma.mma_async m64 x BLOCK_N x k16 with fp32 accumulators in
-//   registers, then the epilogue straight from those registers: scale/shift/ReLU/affine -> fp16|fp32 NHWC stores
-//   (possibly into a channel slice of a concat buffer) and, optionally, the fused 2x2 max-pool output or CRAFT tail.
+//   ping-pong consumers, each owning whole tiles (the CTA's even / odd ones): two wgmma.mma_async m64 x BLOCK_N x k16
+//   per k step (tile rows 0-63 and 64-127) with fp32 accumulators in registers, then the epilogue straight from those
+//   registers: scale/shift/ReLU/affine -> fp16|fp32 NHWC stores (possibly into a channel slice of a concat buffer) and,
+//   optionally, the fused 2x2 max-pool output or CRAFT tail.  The two warpgroups take turns on the main loop, so one
+//   runs its epilogue while the other keeps the tensor cores busy.
 // * persistent: grid = min(#tiles, #SMs); n-tiles of one pixel tile run back to back.
 #include <stdlib.h>
 #include <string.h>
@@ -28,10 +30,12 @@
 
 namespace {
 
-constexpr int WG_M = 64;                  // rows of one wgmma = pixels of the tile one consumer warpgroup owns
+constexpr int WG_M = 64;                  // rows of one wgmma: half of a 128-pixel tile
 constexpr int MMA_K = 16;
 constexpr int NUM_THREADS = 384;          // warpgroup 0: producer; warpgroups 1, 2: MMA + epilogue
-constexpr int CONSUMER_WARPS = 8;
+constexpr int TILE_WARPS = 4;             // the warps of the one consumer warpgroup that reads a stage
+// setmaxnreg split of the 64K registers: the producer needs few, a consumer thread holds 2 x BLOCK_N / 2 accumulators
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 constexpr int SMEM_TOTAL = 227 * 1024;    // dynamic shared memory per CTA (the sm_90 maximum, 232448 B)
 constexpr int MAX_RING = 8;
 
@@ -162,6 +166,17 @@ __device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
   d |= LAYOUT << 62;                                       // swizzle mode       bits [62,64)
   return d;
 }
+// named barriers between the two consumer warpgroups (id 0 is __syncthreads')
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -206,28 +221,28 @@ __device__ __forceinline__ void wgmma_f16<128>(float* d, uint64_t adesc, uint64_
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
-// Walks this CTA's tiles (cta, cta + ncta, ...) keeping the mixed-radix coordinate
-// (n_tile, tile_w, tile_h, tile_n) incrementally: no integer divisions in the per-tile path.
+// Walks the tiles first, first + step, ... keeping the mixed-radix coordinate (n_tile, tile_w, tile_h, tile_n)
+// incrementally: no integer divisions in the per-tile path.  The radices are read from the kernel parameters rather
+// than held in registers (the consumers need every register they can get for accumulators).
 struct TileIter {
   int c0, c1, c2, c3;        // n_tile, tile_w, tile_h, tile_n
-  int d0, d1, d2, d3;        // gridDim.x in the same radix
-  int r0, r1, r2;            // radices: n_tiles, tiles_w, tiles_h
-  int tile, step, total;
-  __device__ __forceinline__ TileIter(const TcParams& p, int cta, int ncta) {
-    r0 = p.n_tiles; r1 = p.tiles_w; r2 = p.tiles_h;
-    total = p.total_tiles; step = ncta;
-    tile = cta;
-    int t = tile;
+  int d0, d1, d2, d3;        // step in the same radix
+  int tile, step;
+  __device__ __forceinline__ TileIter(const TcParams& p, int first, int step_) {
+    const int r0 = p.n_tiles, r1 = p.tiles_w, r2 = p.tiles_h;
+    tile = first;
+    step = step_;
+    int t = first;
     c0 = t % r0; t /= r0; c1 = t % r1; t /= r1; c2 = t % r2; c3 = t / r2;
     t = step;
     d0 = t % r0; t /= r0; d1 = t % r1; t /= r1; d2 = t % r2; d3 = t / r2;
   }
-  __device__ __forceinline__ bool valid() const { return tile < total; }
-  __device__ __forceinline__ void next() {
+  __device__ __forceinline__ bool valid(const TcParams& p) const { return tile < p.total_tiles; }
+  __device__ __forceinline__ void next(const TcParams& p) {
     tile += step;
-    c0 += d0; if (c0 >= r0) { c0 -= r0; ++c1; }
-    c1 += d1; if (c1 >= r1) { c1 -= r1; ++c2; }
-    c2 += d2; if (c2 >= r2) { c2 -= r2; ++c3; }
+    c0 += d0; if (c0 >= p.n_tiles) { c0 -= p.n_tiles; ++c1; }
+    c1 += d1; if (c1 >= p.tiles_w) { c1 -= p.tiles_w; ++c2; }
+    c2 += d2; if (c2 >= p.tiles_h) { c2 -= p.tiles_h; ++c3; }
     c3 += d3;
   }
 };
@@ -260,7 +275,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
   const int ncta = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
   const int pair_shift = PAIR ? 1 : 0;                     // tile column = (pair column << 1) + rank
   constexpr int KSTEPS = KCH / MMA_K;
-  constexpr int NACC = BLOCK_N / 2;                        // fp32 accumulators per consumer thread
+  constexpr int NACC = BLOCK_N / 2;                        // fp32 accumulators per consumer thread and 64-row half
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bar);
@@ -287,7 +302,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int s = 0; s < MAX_RING; ++s) {
       mbar_init(&full[s], 1);                              // the producer's expect_tx arrival + the TMA bytes
-      mbar_init(&empty[s], (PAIR ? 2 : 1) * CONSUMER_WARPS);   // one arrival per consumer warp (of both CTAs of a pair) once its MMAs read the stage
+      mbar_init(&empty[s], (PAIR ? 2 : 1) * TILE_WARPS);   // one arrival per warp of the stage's consumer warpgroup (of both CTAs of a pair) once its MMAs read it
     }
     mbar_init(res_full, 1);
     fence_barrier_init();
@@ -301,6 +316,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
 
   if (threadIdx.x < 128) {
     // ===================================================================== TMA producer
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       tma_prefetch_desc(&amap);
       tma_prefetch_desc(&bmap);
@@ -316,7 +332,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
       }
       int s = 0;
       uint32_t ph = 0;
-      for (TileIter ti(p, cta, ncta); ti.valid(); ti.next()) {
+      for (TileIter ti(p, cta, ncta); ti.valid(p); ti.next(p)) {
         const int tw0 = ((ti.c1 << pair_shift) + static_cast<int>(rank)) << p.bw_log2, th0 = ti.c2 << p.bh_log2, tn0 = ti.c3 << p.bn_log2;
         int ky = 0, kx = 0;
         for (int g = 0; g < groups; ++g) {
@@ -347,19 +363,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
     }
   } else {
     // ===================================================================== consumers (warpgroups 1, 2)
-    const int wg = (threadIdx.x >> 7) - 1;                   // rows wg*64 .. wg*64+63 of the tile
+    // Ping-pong: warpgroup 1 takes the CTA's tiles 0, 2, 4, ... (TileIter order), warpgroup 2 tiles 1, 3, 5, ...  Both
+    // CTAs of a pair give a tile to the same warpgroup, so the multicast B halves line up.  Every tile takes the same
+    // number of ring stages, so a warpgroup steps over the other's tile by arithmetic on (s, ph).  The main loops take
+    // turns: a warpgroup starts a tile only after the other has issued all MMAs of the tile before (named barrier 1 +
+    // wg), which also keeps it from waiting on a stage more than one ring lap ahead of the one the producer fills.
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = (threadIdx.x >> 7) - 1;
     const int q = lane & 3;
-    // accumulator layout of wgmma m64: this thread holds rows r0 and r0 + 8, columns 8i + 2q, 8i + 2q + 1
-    const int r0 = wg * WG_M + (warp & 3) * 16 + (lane >> 2);
+    // accumulator layout of wgmma m64: this thread holds rows r0 and r0 + 8 of each 64-row half, columns 8i + 2q, 8i + 2q + 1
+    const int r0 = (warp & 3) * 16 + (lane >> 2);
     constexpr uint32_t TAP_BYTES = 8 * KCH * 2;              // halo: one dy tap = 8 pixel rows further into the stage
-    const uint64_t desc_a0 = gmma_desc<KCH>(smem_u32(smem) + static_cast<uint32_t>(wg * WG_M * KCH * 2));
+    constexpr uint32_t HALF_BYTES = WG_M * KCH * 2;          // tile rows 64-127: 64 rows (whole 8-row atoms) further
+    const uint64_t desc_a0 = gmma_desc<KCH>(smem_u32(smem));
     const uint64_t desc_b0 = gmma_desc<KCH>(smem_u32(smem) + static_cast<uint32_t>(RESIDENT ? p.off_res : p.a_stride));
     const float* const e_s1 = p.aff_const ? ac.s1 : (p.aff_smem ? aff : p.s1);
     const float* const e_t1 = p.aff_const ? ac.t1 : (p.aff_smem ? aff + p.cout : p.t1);
     const float* const e_s2 = p.aff_const ? ac.s2 : (p.aff_smem ? aff + 2 * p.cout : p.s2);
     const float* const e_t2 = p.aff_const ? ac.t2 : (p.aff_smem ? aff + 3 * p.cout : p.t2);
     const float* const tail_c = p.aff_const ? ac.tail : tail_s;
-    if (RESIDENT) mbar_wait(res_full, 0);
     const int bw_mask = (1 << p.bw_log2) - 1, bh_mask = (1 << p.bh_log2) - 1;
     // a stage is free once the consumers of this CTA (and of the peer, whose B halves it also holds) are done with it
     auto release = [&](int stage) {
@@ -369,11 +391,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
 
     int s = 0;
     uint32_t ph = 0;
-    float acc[NACC];
+    const int tile_stages = groups * kchunks;
+    auto skip_tile = [&]() {                                 // the other warpgroup's tile
+      s += tile_stages;
+      const int laps = s / p.ns;
+      s -= laps * p.ns;
+      ph ^= static_cast<uint32_t>(laps & 1);
+    };
+    TileIter ti(p, cta + wg * ncta, 2 * ncta);              // the CTA's tiles wg, wg + 2, ...
+    if (wg == 1) skip_tile();
+    if (RESIDENT && ti.valid(p)) mbar_wait(res_full, 0);
+    float acc[2 * NACC];                                     // [rows 0-63 | rows 64-127]
   #pragma unroll
-    for (int i = 0; i < NACC; ++i) acc[i] = 0.0f;
-    for (TileIter ti(p, cta, ncta); ti.valid(); ti.next()) {
-      // ---- main loop: every stage of the tile, MMAs in (dx | tap, chunk, dy, k) order
+    for (int i = 0; i < 2 * NACC; ++i) acc[i] = 0.0f;
+    for (bool after_other = wg == 1; ti.valid(p); ti.next(p), after_other = true) {
+      if (after_other) named_bar_sync(1 + wg, 2 * 128);      // the other warpgroup has issued the previous tile
+      // ---- main loop: every stage of the tile, MMAs in (dx | tap, chunk, dy, k) order, both halves per k step
       int prev = -1;
       uint32_t accumulate = 0;
       for (int g = 0; g < groups; ++g) {
@@ -381,7 +414,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
           mbar_wait(&full[s], ph);
           const uint64_t adesc = desc_a0 + static_cast<uint64_t>(static_cast<uint32_t>(s * p.stage_bytes) >> 4);
   #pragma unroll
-          for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
+          for (int i = 0; i < 2 * NACC; ++i) reg_fence(acc[i]);
           wgmma_fence();
   #pragma unroll
           for (int t = 0; t < TAPS_PER_A; ++t) {
@@ -390,8 +423,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
             const uint64_t bdesc = desc_b0 + static_cast<uint64_t>(boff >> 4);
   #pragma unroll
             for (int k = 0; k < KSTEPS; ++k) {
-              wgmma_f16<BLOCK_N>(acc, adesc + static_cast<uint64_t>((t * TAP_BYTES + k * 32) >> 4),
-                                 bdesc + static_cast<uint64_t>((k * 32) >> 4), accumulate);
+  #pragma unroll
+              for (int mh = 0; mh < 2; ++mh)
+                wgmma_f16<BLOCK_N>(acc + mh * NACC, adesc + static_cast<uint64_t>((mh * HALF_BYTES + t * TAP_BYTES + k * 32) >> 4),
+                                   bdesc + static_cast<uint64_t>((k * 32) >> 4), accumulate);
               accumulate = 1;
             }
           }
@@ -405,148 +440,154 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
           if (++s == p.ns) { s = 0; ph ^= 1; }
         }
       }
+      if (ti.tile + ncta < p.total_tiles) named_bar_arrive(1 + (wg ^ 1), 2 * 128);   // the CTA's next tile may start
+      skip_tile();
       wgmma_wait<0>();
   #pragma unroll
-      for (int i = 0; i < NACC; ++i) reg_fence(acc[i]);
+      for (int i = 0; i < 2 * NACC; ++i) reg_fence(acc[i]);
       __syncwarp();
       if (lane == 0) release(prev);
 
-      // ---- epilogue from the registers
+      // ---- epilogue from the registers, one 64-row half after the other
       const int c_base = ti.c0 * BLOCK_N;
-      bool valid[2];
-      size_t pix[2];
-      int px_w[2], px_h[2], px_n[2];
   #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int row = r0 + 8 * hh;
-        px_w[hh] = (((ti.c1 << pair_shift) + static_cast<int>(rank)) << p.bw_log2) + (row & bw_mask);
-        px_h[hh] = (ti.c2 << p.bh_log2) + ((row >> p.bw_log2) & bh_mask);
-        px_n[hh] = (ti.c3 << p.bn_log2) + (row >> (p.bw_log2 + p.bh_log2));
-        valid[hh] = (px_w[hh] < p.W) && (px_h[hh] < p.H) && (px_n[hh] < p.N);
-        pix[hh] = (static_cast<size_t>(px_n[hh]) * p.H + px_h[hh]) * p.W + px_w[hh];
-      }
-      if (UPADD) {
-        // acc += hy * (hx * A + lx * B) + ly * (hx * C + lx * D), the expression of upsample2x_kernel, in fp32
+      for (int mh = 0; mh < 2; ++mh) {
+        float* const acc_h = acc + mh * NACC;
+        bool valid[2];
+        size_t pix[2];
+        int px_w[2], px_h[2], px_n[2];
   #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
-          if (!valid[hh]) continue;
-          const int h = px_h[hh], w = px_w[hh];
-          const int qy = (h + 1) >> 1, qx = (w + 1) >> 1;
-          const int ya = max(qy - 1, 0), yb = min(qy, p.UH - 1), xa = max(qx - 1, 0), xb = min(qx, p.UW - 1);
-          const float ly = ((h + 1) & 1) ? ((qy == 0) ? 0.0f : 0.75f) : 0.25f;
-          const float lx = ((w + 1) & 1) ? ((qx == 0) ? 0.0f : 0.75f) : 0.25f;
-          const float hy = 1.0f - ly, hx = 1.0f - lx;
-          const size_t nb = static_cast<size_t>(px_n[hh]) * p.UH;
-          const __half* const ua = p.up_src + ((nb + ya) * p.UW + xa) * p.up_ld + c_base + 2 * q;
-          const __half* const ub = p.up_src + ((nb + ya) * p.UW + xb) * p.up_ld + c_base + 2 * q;
-          const __half* const uc = p.up_src + ((nb + yb) * p.UW + xa) * p.up_ld + c_base + 2 * q;
-          const __half* const ud = p.up_src + ((nb + yb) * p.UW + xb) * p.up_ld + c_base + 2 * q;
-  #pragma unroll
-          for (int i = 0; i < BLOCK_N / 8; ++i) {
-            const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(ua + 8 * i));
-            const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(ub + 8 * i));
-            const float2 fc = __half22float2(*reinterpret_cast<const __half2*>(uc + 8 * i));
-            const float2 fd = __half22float2(*reinterpret_cast<const __half2*>(ud + 8 * i));
-            acc[4 * i + 2 * hh] += hy * (hx * fa.x + lx * fb.x) + ly * (hx * fc.x + lx * fd.x);
-            acc[4 * i + 2 * hh + 1] += hy * (hx * fa.y + lx * fb.y) + ly * (hx * fc.y + lx * fd.y);
-          }
+          const int row = mh * WG_M + r0 + 8 * hh;
+          px_w[hh] = (((ti.c1 << pair_shift) + static_cast<int>(rank)) << p.bw_log2) + (row & bw_mask);
+          px_h[hh] = (ti.c2 << p.bh_log2) + ((row >> p.bw_log2) & bh_mask);
+          px_n[hh] = (ti.c3 << p.bn_log2) + (row >> (p.bw_log2 + p.bh_log2));
+          valid[hh] = (px_w[hh] < p.W) && (px_h[hh] < p.H) && (px_n[hh] < p.N);
+          pix[hh] = (static_cast<size_t>(px_n[hh]) * p.H + px_h[hh]) * p.W + px_w[hh];
         }
-      }
-      // y = relu?(acc * s1 + t1) [* s2 + t2], in place
-  #pragma unroll
-      for (int i = 0; i < BLOCK_N / 8; ++i) {
-        const int c = c_base + 8 * i + 2 * q;
-        const float2 a1 = *reinterpret_cast<const float2*>(e_s1 + c);
-        const float2 b1 = *reinterpret_cast<const float2*>(e_t1 + c);
-  #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          float& y0 = acc[4 * i + 2 * hh];
-          float& y1 = acc[4 * i + 2 * hh + 1];
-          y0 = fmaf(y0, a1.x, b1.x);
-          y1 = fmaf(y1, a1.y, b1.y);
-          if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
-        }
-        if (p.s2 != nullptr) {
-          const float2 a2 = *reinterpret_cast<const float2*>(e_s2 + c);
-          const float2 b2 = *reinterpret_cast<const float2*>(e_t2 + c);
+        if (UPADD) {
+          // acc += hy * (hx * A + lx * B) + ly * (hx * C + lx * D), the expression of upsample2x_kernel, in fp32
   #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
-            acc[4 * i + 2 * hh] = fmaf(acc[4 * i + 2 * hh], a2.x, b2.x);
-            acc[4 * i + 2 * hh + 1] = fmaf(acc[4 * i + 2 * hh + 1], a2.y, b2.y);
+            if (!valid[hh]) continue;
+            const int h = px_h[hh], w = px_w[hh];
+            const int qy = (h + 1) >> 1, qx = (w + 1) >> 1;
+            const int ya = max(qy - 1, 0), yb = min(qy, p.UH - 1), xa = max(qx - 1, 0), xb = min(qx, p.UW - 1);
+            const float ly = ((h + 1) & 1) ? ((qy == 0) ? 0.0f : 0.75f) : 0.25f;
+            const float lx = ((w + 1) & 1) ? ((qx == 0) ? 0.0f : 0.75f) : 0.25f;
+            const float hy = 1.0f - ly, hx = 1.0f - lx;
+            const size_t nb = static_cast<size_t>(px_n[hh]) * p.UH;
+            const __half* const ua = p.up_src + ((nb + ya) * p.UW + xa) * p.up_ld + c_base + 2 * q;
+            const __half* const ub = p.up_src + ((nb + ya) * p.UW + xb) * p.up_ld + c_base + 2 * q;
+            const __half* const uc = p.up_src + ((nb + yb) * p.UW + xa) * p.up_ld + c_base + 2 * q;
+            const __half* const ud = p.up_src + ((nb + yb) * p.UW + xb) * p.up_ld + c_base + 2 * q;
+  #pragma unroll
+            for (int i = 0; i < BLOCK_N / 8; ++i) {
+              const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(ua + 8 * i));
+              const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(ub + 8 * i));
+              const float2 fc = __half22float2(*reinterpret_cast<const __half2*>(uc + 8 * i));
+              const float2 fd = __half22float2(*reinterpret_cast<const __half2*>(ud + 8 * i));
+              acc_h[4 * i + 2 * hh] += hy * (hx * fa.x + lx * fb.x) + ly * (hx * fc.x + lx * fd.x);
+              acc_h[4 * i + 2 * hh + 1] += hy * (hx * fa.y + lx * fb.y) + ly * (hx * fc.y + lx * fd.y);
+            }
           }
         }
-      }
-      if (BLOCK_N == 16 && p.tail_out != nullptr) {          // block-uniform; only the 16-channel instances carry it
-        // The unfused path stores these 16 channels as fp16 and head_tail_kernel reads them back: round the same way
-        // and run the same fmaf chains, so the scores are bit-identical to conv_cls.4 -> head_tail_kernel.
-        // The quad's four lanes hold a pixel's 16 channels between them: gather them, lane q & 1 takes pixel row
-        // r0 + 8 * (q & 1) (lanes 2, 3 compute the same pixels again and do not store).
-        uint32_t hv[2][2];                                   // [column group i][row hh]
+        // y = relu?(acc * s1 + t1) [* s2 + t2], in place
   #pragma unroll
-        for (int i = 0; i < 2; ++i)
+        for (int i = 0; i < BLOCK_N / 8; ++i) {
+          const int c = c_base + 8 * i + 2 * q;
+          const float2 a1 = *reinterpret_cast<const float2*>(e_s1 + c);
+          const float2 b1 = *reinterpret_cast<const float2*>(e_t1 + c);
   #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
-            const __half2 h2 = __floats2half2_rn(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
-            hv[i][hh] = *reinterpret_cast<const uint32_t*>(&h2);
+            float& y0 = acc_h[4 * i + 2 * hh];
+            float& y1 = acc_h[4 * i + 2 * hh + 1];
+            y0 = fmaf(y0, a1.x, b1.x);
+            y1 = fmaf(y1, a1.y, b1.y);
+            if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
           }
-        const int mine = q & 1;
-        float x[16];
+          if (p.s2 != nullptr) {
+            const float2 a2 = *reinterpret_cast<const float2*>(e_s2 + c);
+            const float2 b2 = *reinterpret_cast<const float2*>(e_t2 + c);
   #pragma unroll
-        for (int src = 0; src < 4; ++src)
-  #pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const uint32_t v0 = __shfl_sync(0xffffffffu, hv[i][0], (lane & ~3) | src);
-            const uint32_t v1 = __shfl_sync(0xffffffffu, hv[i][1], (lane & ~3) | src);
-            const uint32_t v = mine ? v1 : v0;
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&v));
-            x[8 * i + 2 * src] = f.x;
-            x[8 * i + 2 * src + 1] = f.y;
+            for (int hh = 0; hh < 2; ++hh) {
+              acc_h[4 * i + 2 * hh] = fmaf(acc_h[4 * i + 2 * hh], a2.x, b2.x);
+              acc_h[4 * i + 2 * hh + 1] = fmaf(acc_h[4 * i + 2 * hh + 1], a2.y, b2.y);
+            }
           }
-        float o0 = tail_c[304], o1 = tail_c[305];
-  #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          float a = tail_c[256 + j];
-  #pragma unroll
-          for (int c = 0; c < 16; ++c) a = fmaf(x[c], tail_c[j * 16 + c], a);
-          a = fmaxf(a, 0.0f);
-          o0 = fmaf(a, tail_c[272 + j * 2 + 0], o0);
-          o1 = fmaf(a, tail_c[272 + j * 2 + 1], o1);
         }
-        if (q < 2 && valid[mine]) reinterpret_cast<float2*>(p.tail_out)[pix[mine]] = make_float2(o0, o1);
-        continue;
-      }
-      if (p.out_f32) {
+        if (BLOCK_N == 16 && p.tail_out != nullptr) {          // block-uniform; only the 16-channel instances carry it
+          // The unfused path stores these 16 channels as fp16 and head_tail_kernel reads them back: round the same way
+          // and run the same fmaf chains, so the scores are bit-identical to conv_cls.4 -> head_tail_kernel.
+          // The quad's four lanes hold a pixel's 16 channels between them: gather them, lane q & 1 takes pixel row
+          // r0 + 8 * (q & 1) (lanes 2, 3 compute the same pixels again and do not store).
+          uint32_t hv[2][2];                                   // [column group i][row hh]
   #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          if (!valid[hh]) continue;
-          float* const o = reinterpret_cast<float*>(p.out) + pix[hh] * p.out_ld + c_base + 2 * q;
+          for (int i = 0; i < 2; ++i)
   #pragma unroll
-          for (int i = 0; i < BLOCK_N / 8; ++i)
-            *reinterpret_cast<float2*>(o + 8 * i) = make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
+            for (int hh = 0; hh < 2; ++hh) {
+              const __half2 h2 = __floats2half2_rn(acc_h[4 * i + 2 * hh], acc_h[4 * i + 2 * hh + 1]);
+              hv[i][hh] = *reinterpret_cast<const uint32_t*>(&h2);
+            }
+          const int mine = q & 1;
+          float x[16];
+  #pragma unroll
+          for (int src = 0; src < 4; ++src)
+  #pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const uint32_t v0 = __shfl_sync(0xffffffffu, hv[i][0], (lane & ~3) | src);
+              const uint32_t v1 = __shfl_sync(0xffffffffu, hv[i][1], (lane & ~3) | src);
+              const uint32_t v = mine ? v1 : v0;
+              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&v));
+              x[8 * i + 2 * src] = f.x;
+              x[8 * i + 2 * src + 1] = f.y;
+            }
+          float o0 = tail_c[304], o1 = tail_c[305];
+  #pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            float a = tail_c[256 + j];
+  #pragma unroll
+            for (int c = 0; c < 16; ++c) a = fmaf(x[c], tail_c[j * 16 + c], a);
+            a = fmaxf(a, 0.0f);
+            o0 = fmaf(a, tail_c[272 + j * 2 + 0], o0);
+            o1 = fmaf(a, tail_c[272 + j * 2 + 1], o1);
+          }
+          if (q < 2 && valid[mine]) reinterpret_cast<float2*>(p.tail_out)[pix[mine]] = make_float2(o0, o1);
+          continue;
         }
-        continue;
-      }
-      // fp16 out; fused 2x2/2 max pool on halo tiles: rows r0 / r0 + 8 are vertical neighbours (h even, h + 1), the w
-      // neighbour is lane ^ 4
-      const bool pool_writer = p.pool_out != nullptr && !(px_w[0] & 1) && !(px_h[0] & 1) && (px_w[0] >> 1) < p.PW &&
-                               (px_h[0] >> 1) < p.PH && px_n[0] < p.N;
-      const size_t ppix = (static_cast<size_t>(px_n[0]) * p.PH + (px_h[0] >> 1)) * p.PW + (px_w[0] >> 1);
-      __half* const o0 = reinterpret_cast<__half*>(p.out) + pix[0] * p.out_ld + c_base + 2 * q;
-      __half* const o1 = reinterpret_cast<__half*>(p.out) + pix[1] * p.out_ld + c_base + 2 * q;
+        if (p.out_f32) {
   #pragma unroll
-      for (int i = 0; i < BLOCK_N / 8; ++i) {
-        const __half2 h0 = __floats2half2_rn(acc[4 * i], acc[4 * i + 1]);
-        const __half2 h1 = __floats2half2_rn(acc[4 * i + 2], acc[4 * i + 3]);
-        if (p.write_full) {
-          if (valid[0]) *reinterpret_cast<__half2*>(o0 + 8 * i) = h0;
-          if (valid[1]) *reinterpret_cast<__half2*>(o1 + 8 * i) = h1;
+          for (int hh = 0; hh < 2; ++hh) {
+            if (!valid[hh]) continue;
+            float* const o = reinterpret_cast<float*>(p.out) + pix[hh] * p.out_ld + c_base + 2 * q;
+  #pragma unroll
+            for (int i = 0; i < BLOCK_N / 8; ++i)
+              *reinterpret_cast<float2*>(o + 8 * i) = make_float2(acc_h[4 * i + 2 * hh], acc_h[4 * i + 2 * hh + 1]);
+          }
+          continue;
         }
-        if (p.pool_out != nullptr) {                         // block-uniform branch
-          __half2 m = __hmax2(h0, h1);
-          const uint32_t mu = *reinterpret_cast<const uint32_t*>(&m);
-          const uint32_t ou = __shfl_xor_sync(0xffffffffu, mu, 4);
-          m = __hmax2(m, *reinterpret_cast<const __half2*>(&ou));
-          if (pool_writer) *reinterpret_cast<__half2*>(p.pool_out + ppix * p.pool_ld + c_base + 8 * i + 2 * q) = m;
+        // fp16 out; fused 2x2/2 max pool on halo tiles: rows r0 / r0 + 8 are vertical neighbours (h even, h + 1), the w
+        // neighbour is lane ^ 4
+        const bool pool_writer = p.pool_out != nullptr && !(px_w[0] & 1) && !(px_h[0] & 1) && (px_w[0] >> 1) < p.PW &&
+                                 (px_h[0] >> 1) < p.PH && px_n[0] < p.N;
+        const size_t ppix = (static_cast<size_t>(px_n[0]) * p.PH + (px_h[0] >> 1)) * p.PW + (px_w[0] >> 1);
+        __half* const o0 = reinterpret_cast<__half*>(p.out) + pix[0] * p.out_ld + c_base + 2 * q;
+        __half* const o1 = reinterpret_cast<__half*>(p.out) + pix[1] * p.out_ld + c_base + 2 * q;
+  #pragma unroll
+        for (int i = 0; i < BLOCK_N / 8; ++i) {
+          const __half2 h0 = __floats2half2_rn(acc_h[4 * i], acc_h[4 * i + 1]);
+          const __half2 h1 = __floats2half2_rn(acc_h[4 * i + 2], acc_h[4 * i + 3]);
+          if (p.write_full) {
+            if (valid[0]) *reinterpret_cast<__half2*>(o0 + 8 * i) = h0;
+            if (valid[1]) *reinterpret_cast<__half2*>(o1 + 8 * i) = h1;
+          }
+          if (p.pool_out != nullptr) {                         // block-uniform branch
+            __half2 m = __hmax2(h0, h1);
+            const uint32_t mu = *reinterpret_cast<const uint32_t*>(&m);
+            const uint32_t ou = __shfl_xor_sync(0xffffffffu, mu, 4);
+            m = __hmax2(m, *reinterpret_cast<const __half2*>(&ou));
+            if (pool_writer) *reinterpret_cast<__half2*>(p.pool_out + ppix * p.pool_ld + c_base + 8 * i + 2 * q) = m;
+          }
         }
       }
     }
