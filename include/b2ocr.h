@@ -149,7 +149,7 @@ int b2o_warp_boxes_color(b2o_ctx* ctx, const uint8_t* rgb_dev, int n, int h, int
                          uint8_t* crops_dev, void* crnn_in_dev, void* stream);
 
 /* prediction_model.predict (recognition.py:535; graph 214-333): CRNN + STN + BiLSTM + greedy CTC (beam search:
- * b2o_crnn_forward_beam below).
+ * b2o_crnn_forward_beam below; a caller's word list: b2o_crnn_forward_lexicon).
  * crnn_in: (b,200,31) fp16 from b2o_warp_boxes (or b2o_crops_to_input).  labels: (b,48) int32,
  * merged + blank-free, padded with -1 -- the tensor recognize_from_boxes iterates (527-534).  */
 size_t b2o_crnn_workspace_bytes(int b);
@@ -186,6 +186,39 @@ int b2o_ctc_beam_decode(b2o_ctx* ctx, const float* logits_dev, int b, int k, int
                         int32_t* labels_dev, float* logp_dev, void* stream);
 int b2o_crnn_forward_beam(b2o_ctx* ctx, const void* crnn_in_dev, int b, int beam_width, int top_paths,
                           int32_t* labels_dev, float* logp_dev, void* ws_dev, size_t ws_bytes, void* stream);
+
+/* Lexicon-constrained CTC decoding: the top_paths most probable entries of a caller's word list, per crop.
+ * Inputs: the beam decoder's lp[t,c] = log(softmax(logits_t)_c + 1e-7) over the 48 kept steps, blank = k-1.
+ * Lexicon: n_words entries in CSR form, offsets_dev (n_words + 1) int32 and the concatenated labels_dev int16; entry i
+ * is labels[offsets[i] .. offsets[i+1]).  An entry's score is its CTC forward log-probability: the log of the sum,
+ * over every 48-step alignment that collapses (merge repeats, drop blanks) to the entry, of exp(sum_t lp[t, pi_t]).
+ * A doubled letter needs a blank between its copies, so an entry of L labels with R adjacent repeats that has
+ * L + R > 48 cannot be aligned and scores -inf; so does an entry that is empty, longer than 48, has a label outside
+ * [0, k-2] or labels beyond index 2^24 (never read out of bounds).  Every other entry's score is finite, however
+ * improbable (down to about 48 log(1e-7) ~ -774): the recursion runs in the linear domain with exact power-of-two
+ * rescaling, and the score is rounded to float32 once.
+ * Result: per crop the top_paths best entries, score descending, equal float32 scores by entry index ascending.
+ * labels_out_dev (b, top_paths, 48) int32: entry p's labels, -1 padded; logp_dev (b, top_paths) float32 its score
+ * (NULL: not written).  Slots beyond the number of finite-score entries are all -1 with logp -inf.  A (b, 1, 48)
+ * result has the (b, 48) layout that b2o_pack_records(_scored) takes.
+ * A crop's result is a function of its logits and the lexicon alone: bit-identical alone, in any batch and on every
+ * run; an entry's score does not depend on its position in the lexicon or on the other entries.
+ * 1 <= n_words <= B2O_MAX_LEXICON_WORDS, 1 <= top_paths <= B2O_MAX_LEXICON_TOP_PATHS, 2 <= k <= B2O_MAX_CLASSES,
+ * otherwise B2O_ERR_ARG.  The caller owns the scratch: b2o_lexicon_workspace_bytes(b, n_words, top_paths) bytes.
+ * b2o_ctc_lexicon_decode: the decoder alone on caller-supplied (b, 48, k) float32 logits; ws_dev is that scratch.
+ * b2o_crnn_forward_lexicon: the CRNN of b2o_crnn_forward, its fc_12 logits into the workspace's logits slot, then the
+ * decoder; ws_bytes >= b2o_crnn_workspace_bytes(b) + b2o_lexicon_workspace_bytes(b, n_words, top_paths) (the
+ * decoder's scratch follows the CRNN's).                                                                        */
+#define B2O_MAX_LEXICON_WORDS (1 << 20)
+#define B2O_MAX_LEXICON_LABELS (1 << 24)
+#define B2O_MAX_LEXICON_TOP_PATHS 128
+size_t b2o_lexicon_workspace_bytes(int b, int n_words, int top_paths);
+int b2o_ctc_lexicon_decode(b2o_ctx* ctx, const float* logits_dev, int b, int k, const int32_t* offsets_dev,
+                           const int16_t* labels_dev, int n_words, int top_paths, int32_t* labels_out_dev,
+                           float* logp_dev, void* ws_dev, size_t ws_bytes, void* stream);
+int b2o_crnn_forward_lexicon(b2o_ctx* ctx, const void* crnn_in_dev, int b, const int32_t* offsets_dev,
+                             const int16_t* labels_dev, int n_words, int top_paths, int32_t* labels_out_dev,
+                             float* logp_dev, void* ws_dev, size_t ws_bytes, void* stream);
 
 /* Result records of Pipeline.recognize for the multi-GPU gather (pipeline.py:66-75; SURVEY.md 8(e)): one
  * fixed-size float32 row per image = [count][rec_boxes x (4,2) boxes * inv_scale[i] (tools.adjust_boxes,

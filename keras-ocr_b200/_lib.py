@@ -15,6 +15,9 @@ LIB_PATH = os.environ.get("B2O_LIB") or os.path.join(_HERE, "libb2ocr.so")      
 CONV_AUTO, CONV_SIMT, CONV_TC_GENERIC = 0, 1, 2
 MAX_CLASSES = 1024            # B2O_MAX_CLASSES in include/b2ocr.h
 MAX_BEAM_WIDTH = 128          # B2O_MAX_BEAM_WIDTH in include/b2ocr.h
+MAX_LEXICON_WORDS = 1 << 20   # B2O_MAX_LEXICON_WORDS
+MAX_LEXICON_LABELS = 1 << 24  # B2O_MAX_LEXICON_LABELS
+MAX_LEXICON_TOP_PATHS = 128   # B2O_MAX_LEXICON_TOP_PATHS
 
 
 class B2OError(RuntimeError):
@@ -77,6 +80,9 @@ SIGNATURES = {
     "b2o_crnn_forward_scored": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_ctc_beam_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "b2o_crnn_forward_beam": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_lexicon_workspace_bytes": (_sz, [_i, _i, _i]),
+    "b2o_ctc_lexicon_decode": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_crnn_forward_lexicon": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_set_debug_taps": (_i, [_vp, _i]),
     "b2o_crnn_tap": (_i, [_vp, _c.c_char_p, _vp, _i, _vp, _sz, _vp]),
     "b2o_conv2d_test": (_i, [_vp, _vp, _i, _i, _i, _i, _c.POINTER(_c.c_float), _i, _i, _i,
@@ -264,6 +270,19 @@ class Context:
     def crnn_forward_beam(self, crnn_in, b, beam_width, top_paths, labels, logp, ws, ws_bytes, stream):
         self._check(self.lib.b2o_crnn_forward_beam(self.handle, crnn_in, b, beam_width, top_paths, labels, logp, ws,
                                                    ws_bytes, stream), "b2o_crnn_forward_beam")
+
+    def lexicon_workspace_bytes(self, b, n_words, top_paths):
+        return int(self.lib.b2o_lexicon_workspace_bytes(b, n_words, top_paths))
+
+    def ctc_lexicon_decode(self, logits, b, k, offsets, labels, n_words, top_paths, labels_out, logp, ws, ws_bytes,
+                           stream):
+        self._check(self.lib.b2o_ctc_lexicon_decode(self.handle, logits, b, k, offsets, labels, n_words, top_paths,
+                                                    labels_out, logp, ws, ws_bytes, stream), "b2o_ctc_lexicon_decode")
+
+    def crnn_forward_lexicon(self, crnn_in, b, offsets, labels, n_words, top_paths, labels_out, logp, ws, ws_bytes,
+                             stream):
+        self._check(self.lib.b2o_crnn_forward_lexicon(self.handle, crnn_in, b, offsets, labels, n_words, top_paths,
+                                                      labels_out, logp, ws, ws_bytes, stream), "b2o_crnn_forward_lexicon")
 
     def set_debug_taps(self, on):
         self._check(self.lib.b2o_set_debug_taps(self.handle, int(on)), "b2o_set_debug_taps")

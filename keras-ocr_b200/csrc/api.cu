@@ -17,6 +17,9 @@ int add_run(b2o_ctx* ctx, const __half* a, const __half* b, __half* o, long long
 int fc_ctc_run(b2o_ctx* ctx, const __half* l2, int B, float* logits, int* labels, float* logp, cudaStream_t st);
 int ctc_beam_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths, int* labels, float* logp,
                  cudaStream_t st);
+size_t ctc_lexicon_workspace_bytes(int B, int n_words);
+int ctc_lexicon_run(b2o_ctx* ctx, const float* logits, int B, int K, const int* offsets, const short* labels,
+                    int n_words, int top_paths, int* labels_out, float* logp, void* ws, cudaStream_t st);
 
 namespace {
 
@@ -721,6 +724,74 @@ extern "C" int b2o_ctc_beam_decode(b2o_ctx* ctx, const float* logits, int b, int
   if (b < 0 || (b > 0 && (!logits || !labels))) { ctx->set_error("b2o_ctc_beam_decode: bad argument"); return B2O_ERR_ARG; }
   DeviceGuard guard(ctx->device);
   return ctc_beam_run(ctx, logits, b, k, beam_width, top_paths, labels, logp, reinterpret_cast<cudaStream_t>(stream));
+}
+
+namespace {
+
+bool lexicon_args_ok(b2o_ctx* ctx, const char* fn, int k, int n_words, int top_paths) {
+  if (k < 2 || k > B2O_MAX_CLASSES) { ctx->set_error(std::string(fn) + ": k must be in [2, 1024]"); return false; }
+  if (n_words < 1 || n_words > B2O_MAX_LEXICON_WORDS) {
+    ctx->set_error(std::string(fn) + ": n_words must be in [1, 2^20]");
+    return false;
+  }
+  if (top_paths < 1 || top_paths > B2O_MAX_LEXICON_TOP_PATHS) {
+    ctx->set_error(std::string(fn) + ": top_paths must be in [1, 128]");
+    return false;
+  }
+  return true;
+}
+
+size_t crnn_lexicon_scratch_offset(int b) { return (plan_crnn(b).bytes + 255) / 256 * 256; }
+
+}  // namespace
+
+extern "C" size_t b2o_lexicon_workspace_bytes(int b, int n_words, int top_paths) {
+  if (b <= 0 || n_words < 1 || n_words > B2O_MAX_LEXICON_WORDS || top_paths < 1) return 0;
+  return ctc_lexicon_workspace_bytes(b, n_words);
+}
+
+extern "C" int b2o_ctc_lexicon_decode(b2o_ctx* ctx, const float* logits, int b, int k, const int32_t* offsets,
+                                      const int16_t* labels, int n_words, int top_paths, int32_t* labels_out,
+                                      float* logp, void* ws, size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!lexicon_args_ok(ctx, "b2o_ctc_lexicon_decode", k, n_words, top_paths)) return B2O_ERR_ARG;
+  if (b < 0 || (b > 0 && (!logits || !offsets || !labels || !labels_out || !ws))) {
+    ctx->set_error("b2o_ctc_lexicon_decode: bad argument");
+    return B2O_ERR_ARG;
+  }
+  if (b == 0) return B2O_OK;
+  if (ws_bytes < ctc_lexicon_workspace_bytes(b, n_words)) {
+    ctx->set_error("b2o_ctc_lexicon_decode: workspace too small");
+    return B2O_ERR_WORKSPACE;
+  }
+  DeviceGuard guard(ctx->device);
+  return ctc_lexicon_run(ctx, logits, b, k, offsets, labels, n_words, top_paths, labels_out, logp, ws,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2o_crnn_forward_lexicon(b2o_ctx* ctx, const void* crnn_in, int b, const int32_t* offsets,
+                                        const int16_t* labels, int n_words, int top_paths, int32_t* labels_out,
+                                        float* logp, void* ws, size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_forward_lexicon: CRNN weights not loaded"); return B2O_ERR_STATE; }
+  if (!lexicon_args_ok(ctx, "b2o_crnn_forward_lexicon", ctx->n_classes, n_words, top_paths)) return B2O_ERR_ARG;
+  if (b < 0 || (b > 0 && (!crnn_in || !offsets || !labels || !labels_out || !ws))) {
+    ctx->set_error("b2o_crnn_forward_lexicon: bad argument");
+    return B2O_ERR_ARG;
+  }
+  if (b == 0) return B2O_OK;
+  const size_t scratch = crnn_lexicon_scratch_offset(b);
+  if (ws_bytes < scratch + ctc_lexicon_workspace_bytes(b, n_words)) {
+    ctx->set_error("b2o_crnn_forward_lexicon: workspace too small");
+    return B2O_ERR_WORKSPACE;
+  }
+  // the greedy labels of fc_ctc_kernel go to the first b * 48 entries of `labels_out`, which the decoder then overwrites
+  B2O_RETURN_IF(crnn_forward(ctx, crnn_in, b, labels_out, nullptr, true, ws, ws_bytes, stream));
+  DeviceGuard guard(ctx->device);
+  uint8_t* base = reinterpret_cast<uint8_t*>(ws);
+  const float* logits = reinterpret_cast<const float*>(base + plan_crnn(b).off_logits);
+  return ctc_lexicon_run(ctx, logits, b, ctx->n_classes, offsets, labels, n_words, top_paths, labels_out, logp,
+                         base + scratch, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b2o_set_debug_taps(b2o_ctx* ctx, int on) {

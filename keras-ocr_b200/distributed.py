@@ -130,7 +130,7 @@ def _host_records(pipeline, local, per_rank, max_boxes):
 
 
 def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_scores=False, beam_width=None,
-                      top_paths=1):
+                      top_paths=1, lexicon=None):
     """Run ``pipeline.recognize`` on this rank's shard of ``images`` and gather to rank 0.
 
     ``images`` is the global batch (every rank passes the same list and takes its contiguous slice) or, with
@@ -145,9 +145,12 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
     (text, box, detection_score, confidence) as ``Pipeline.recognize(return_scores=True)`` returns them, carried in
     the scored record layout (device records only).  ``beam_width``: beam-search decoding
     (``recognition.check_beam``); records carry the best path only, so ``top_paths`` > 1 raises ``ValueError``.
+    ``lexicon``: every word reads as the most probable entry of that word list (``recognition.check_decoder``); a
+    ``recognition.Lexicon`` is compiled once and uploaded once per device, a plain list is compiled here.
     """
-    from .pipeline import check_records_beam
-    check_records_beam(beam_width, top_paths)
+    from .pipeline import check_records_decoder
+    lexicon = check_records_decoder(beam_width, top_paths, lexicon,
+                                    None if lexicon is None else pipeline.recognizer.alphabet)
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
     if presharded:
@@ -165,6 +168,8 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
     sk = {"scores": True} if return_scores else {}      # pipelines without the flag keep working unscored
     if beam_width is not None:
         sk["beam_width"] = beam_width
+    if lexicon is not None:
+        sk["lexicon"] = lexicon
     if native:
         if getattr(pipeline, "records_counts", None) is not None:
             state = pipeline.records_begin(mine, rows=per_rank, rec_boxes=16 if max_boxes == "auto" else max_boxes, **sk)
@@ -176,7 +181,8 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
             local = pipeline.recognize_records(mine, rows=per_rank, rec_boxes=max_boxes, **sk)
         device = None                                   # already where the backend wants it
     else:
-        rk = {} if beam_width is None else {"recognition_kwargs": {"beam_width": beam_width}}
+        rk = {k: v for k, v in (("beam_width", beam_width), ("lexicon", lexicon)) if v is not None}
+        rk = {"recognition_kwargs": rk} if rk else {}
         result = pipeline.recognize(mine, **rk) if len(mine) else []
         if max_boxes == "auto":
             max_boxes = agree_max_boxes([len(g) for g in result], _collective_device(pipeline))
@@ -256,12 +262,13 @@ class ShardedStream:
     asynchronous copy into pinned memory; any other pipeline (``recognize`` only) is served too, without the overlap.
     ``max_boxes``: words a record holds (an image with more raises ``RecordOverflow`` on rank 0 when its batch is
     decoded) or ``"auto"`` (sized per batch by ``agree_max_boxes``).  ``return_scores=True``: words as
-    ``recognize_sharded(return_scores=True)`` returns them (device records only).  ``beam_width``: as
+    ``recognize_sharded(return_scores=True)`` returns them (device records only).  ``beam_width`` / ``lexicon``: as
     ``recognize_sharded``."""
 
-    def __init__(self, pipeline, max_boxes=128, return_scores=False, beam_width=None, top_paths=1):
-        from .pipeline import check_records_beam
-        check_records_beam(beam_width, top_paths)
+    def __init__(self, pipeline, max_boxes=128, return_scores=False, beam_width=None, top_paths=1, lexicon=None):
+        from .pipeline import check_records_decoder
+        lexicon = check_records_decoder(beam_width, top_paths, lexicon,
+                                        None if lexicon is None else pipeline.recognizer.alphabet)
         self.pipeline, self.max_boxes = pipeline, max_boxes
         self.world = dist.get_world_size() if dist.is_initialized() else 1
         self.rank = dist.get_rank() if dist.is_initialized() else 0
@@ -275,9 +282,10 @@ class ShardedStream:
         self.return_scores = return_scores
         self._sk = {"scores": True} if return_scores else {}
         self._rk = {}
-        if beam_width is not None:
-            self._sk["beam_width"] = beam_width
-            self._rk = {"recognition_kwargs": {"beam_width": beam_width}}
+        for k, v in (("beam_width", beam_width), ("lexicon", lexicon)):
+            if v is not None:
+                self._sk[k] = v
+                self._rk.setdefault("recognition_kwargs", {})[k] = v
         self._pending = None                             # (host blocks, event or None) of the batch in flight
         self._side = None                                # communication stream (CUDA tensors only)
         self._keep = None

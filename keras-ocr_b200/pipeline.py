@@ -5,11 +5,13 @@ import torch
 from . import detection, recognition, tools
 
 
-def check_records_beam(beam_width=None, top_paths=1):
-    """``recognition.check_beam`` for the records path, whose fixed-size records carry one reading per word."""
-    recognition.check_beam(beam_width, top_paths)
+def check_records_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=recognition.DEFAULT_ALPHABET):
+    """``recognition.check_decoder`` for the records path, whose fixed-size records carry one reading per word; returns
+    the compiled lexicon or None."""
+    lexicon = recognition.check_decoder(beam_width, top_paths, lexicon, alphabet)
     if top_paths != 1:
         raise ValueError("records carry the best path only: top_paths must be 1")
+    return lexicon
 
 
 class Pipeline:
@@ -194,8 +196,9 @@ class Pipeline:
         confidence exp(S) in (0, 1] (``recognition.confidences``); texts and boxes are those of the default call.
         ``recognition_kwargs`` may hold ``beam_width`` / ``top_paths`` (``recognition.check_beam``): CTC beam search
         instead of greedy decoding, boxes unchanged; with ``top_paths = P > 1`` the text of every word is a list of P
-        readings and its confidence a list of P floats, best first.  Injected recognizers get ``recognition_kwargs``
-        as they are.
+        readings and its confidence a list of P floats, best first.  Or ``lexicon`` (a ``recognition.Lexicon`` or a
+        list of strings) / ``top_paths``: every word reads as the most probable entries of that list, in the same
+        shapes (``recognition.check_decoder``).  Injected recognizers get ``recognition_kwargs`` as they are.
         """
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
@@ -207,8 +210,10 @@ class Pipeline:
         if recognition_kwargs is None:
             recognition_kwargs = {}
         if self._native():
-            beam = {k: recognition_kwargs[k] for k in ("beam_width", "top_paths") if k in recognition_kwargs}
-            recognition.check_beam(**beam)
+            beam = {k: recognition_kwargs[k] for k in ("beam_width", "top_paths", "lexicon") if k in recognition_kwargs}
+            lexicon = self.recognizer._decoder(beam.get("beam_width"), beam.get("top_paths", 1), beam.get("lexicon"))
+            if lexicon is not None:
+                beam["lexicon"] = lexicon                 # compiled once for every sub-batch
         if not self._native():
             if return_scores:
                 raise NotImplementedError("return_scores=True needs this package's Detector and Recognizer; injected "
@@ -237,7 +242,7 @@ class Pipeline:
         return out
 
     def recognize_records(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
-                          top_paths=1):
+                          top_paths=1, lexicon=None):
         """``recognize`` without the trip to the host: returns the results as a CUDA float32 tensor of fixed-size
         per-image records, ``(rows, b2o_record_floats(rec_boxes))`` = [count | rec_boxes x (4,2) boxes in source
         pixels | rec_boxes x 48 int8 labels] (``distributed.unpack_blocks`` decodes it; rows beyond ``len(images)``
@@ -245,16 +250,19 @@ class Pipeline:
         counts ever reach the host on this rank.  ``scores=True``: the scored layout,
         ``(rows, b2o_record_floats_scored(rec_boxes))``, which appends [rec_boxes detection scores | rec_boxes
         path log-probabilities] to that record.  ``beam_width``: the words are beam-search decoded
-        (``recognition.check_beam``); a record carries the best path only, so ``top_paths`` > 1 raises ``ValueError``."""
+        (``recognition.check_beam``); a record carries the best path only, so ``top_paths`` > 1 raises ``ValueError``.
+        ``lexicon``: every word reads as the most probable entry of that word list (``recognition.check_decoder``), its
+        log-probability in the scored layout."""
         return self.records_end(self.records_begin(images, rows, rec_boxes, detection_kwargs, scores, beam_width,
-                                                   top_paths))
+                                                   top_paths, lexicon))
 
     def records_begin(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
-                      top_paths=1):
+                      top_paths=1, lexicon=None):
         """First half of ``recognize_records``: queues resize/pad, CRAFT and getBoxes and returns at once (no
         synchronisation), so the caller can use the host while the GPU works (``distributed.ShardedStream`` decodes the
         previous batch's words here).  Pass the returned state to ``records_end``."""
-        check_records_beam(beam_width, top_paths)
+        lexicon = check_records_decoder(beam_width, top_paths, lexicon,
+                                        recognition.DEFAULT_ALPHABET if lexicon is None else self.recognizer.alphabet)
         assert self._native(), "recognize_records needs this package's Detector and Recognizer"
         assert len(self.recognizer.alphabet) + 1 <= 127, "record labels travel as int8: alphabets up to 126 characters"
         if not isinstance(images, (np.ndarray, torch.Tensor)):
@@ -268,7 +276,8 @@ class Pipeline:
         rows = n if rows is None else int(rows)
         assert rows >= n and rows > 0
         self.last_stats = {"h2d_bytes": 0, "d2h_bytes": 0}
-        state = {"n": n, "rows": rows, "rec_boxes": rec_boxes, "scores": bool(scores), "beam_width": beam_width}
+        state = {"n": n, "rows": rows, "rec_boxes": rec_boxes, "scores": bool(scores), "beam_width": beam_width,
+                 "lexicon": lexicon}
         if n:
             plans = self._plans(images)
             state["st"] = self._stage_detect(images, (max(p[1] for p in plans), max(p[2] for p in plans)), thresholds,
@@ -307,7 +316,7 @@ class Pipeline:
         boxes = state["boxes"]
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
                                                  image_index=bst["image_index"], with_scores=scored,
-                                                 beam_width=state.get("beam_width"))
+                                                 beam_width=state.get("beam_width"), lexicon=state.get("lexicon"))
         inv = torch.tensor([1.0 / s for s in st["scales"]], dtype=torch.float32).to(det.device, non_blocking=True)
         stream = torch.cuda.current_stream(det.device).cuda_stream
         ptr = lambda t: t.data_ptr() if t is not None else None      # noqa: E731

@@ -59,6 +59,78 @@ def check_beam(beam_width=None, top_paths=1):
         raise ValueError(f"top_paths ({top_paths}) must not exceed beam_width ({beam_width})")
 
 
+class Lexicon:
+    """A word list for lexicon-constrained decoding (``b2o_crnn_forward_lexicon``): every crop reads as the entry with the
+    highest CTC forward log-probability -- the sum over every 48-step alignment that collapses to the entry -- and
+    ``top_paths`` gives the P best entries.  Entries are non-empty strings over ``alphabet`` of at most 48 characters,
+    distinct, at most 2^20 of them; anything else raises ``ValueError`` naming the first offending entry.  An entry whose
+    doubled letters make it longer than 48 steps (length + adjacent repeats > 48) is valid but scores -inf.
+
+    The lexicon is compiled once on the host (CSR: ``offsets`` (n+1) int32, ``labels`` int16) and uploaded lazily, once
+    per CUDA device, so one object serves every rank of a sharded run.  A plain list or tuple of strings is accepted
+    wherever a ``Lexicon`` is and is compiled for that call."""
+
+    def __init__(self, words, alphabet=DEFAULT_ALPHABET):
+        if isinstance(words, str) or not isinstance(words, (list, tuple)):
+            raise ValueError("a lexicon is a list or tuple of strings")
+        if not words:
+            raise ValueError("the lexicon is empty")
+        if len(words) > _lib.MAX_LEXICON_WORDS:
+            raise ValueError(f"the lexicon has {len(words)} entries; at most {_lib.MAX_LEXICON_WORDS} are supported")
+        index = {ch: i for i, ch in enumerate(alphabet)}
+        seen = set()
+        for i, w in enumerate(words):
+            if not isinstance(w, str) or not w:
+                raise ValueError(f"lexicon entry {i} ({w!r}) is not a non-empty string")
+            if len(w) > STEPS:
+                raise ValueError(f"lexicon entry {i} ({w!r}) is longer than {STEPS} characters")
+            bad = next((ch for ch in w if ch not in index), None)
+            if bad is not None:
+                raise ValueError(f"lexicon entry {i} ({w!r}) has {bad!r}, which is not in the alphabet")
+            if w in seen:
+                raise ValueError(f"lexicon entry {i} ({w!r}) is a duplicate")
+            seen.add(w)
+        self.words, self.alphabet = tuple(words), alphabet
+        lengths = np.fromiter((len(w) for w in words), dtype=np.int64, count=len(words))
+        if lengths.sum() > _lib.MAX_LEXICON_LABELS:
+            i = int(np.argmax(np.cumsum(lengths) > _lib.MAX_LEXICON_LABELS))
+            raise ValueError(f"lexicon entry {i} ({words[i]!r}) takes the lexicon past {_lib.MAX_LEXICON_LABELS} "
+                             "characters in all")
+        self.offsets = np.zeros(len(words) + 1, np.int32)
+        self.offsets[1:] = np.cumsum(lengths)
+        self.labels = np.fromiter((index[ch] for w in words for ch in w), dtype=np.int16, count=int(lengths.sum()))
+        self._device = {}
+
+    def __len__(self):
+        return len(self.words)
+
+    def device_arrays(self, device):
+        """(offsets, labels) CUDA tensors on ``device``, uploaded on first use."""
+        device = torch.device(device)
+        if device not in self._device:
+            self._device[device] = (torch.from_numpy(self.offsets).to(device), torch.from_numpy(self.labels).to(device))
+        return self._device[device]
+
+
+def check_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET):
+    """Validates a decoder choice before anything is launched (``ValueError`` otherwise) and returns the ``Lexicon`` to
+    decode with, or None.  Without a lexicon this is ``check_beam``.  With one (a ``Lexicon`` over ``alphabet``, or a
+    list / tuple of strings, compiled here): ``beam_width`` must be None and 1 <= ``top_paths`` <= 128."""
+    if lexicon is None:
+        check_beam(beam_width, top_paths)
+        return None
+    if beam_width is not None:
+        raise ValueError("lexicon and beam_width are mutually exclusive")
+    if (not isinstance(top_paths, (int, np.integer)) or isinstance(top_paths, (bool, np.bool_))
+            or not 1 <= top_paths <= _lib.MAX_LEXICON_TOP_PATHS):
+        raise ValueError(f"with a lexicon, top_paths must be an int in [1, {_lib.MAX_LEXICON_TOP_PATHS}], got {top_paths!r}")
+    if not isinstance(lexicon, Lexicon):
+        lexicon = Lexicon(lexicon, alphabet)
+    elif lexicon.alphabet != alphabet:
+        raise ValueError("the lexicon was compiled for another alphabet than the recognizer's")
+    return lexicon
+
+
 def decode_paths(labels, alphabet=DEFAULT_ALPHABET, logp=None):
     """Host labels -> texts, and logp -> confidences (None without logp).  (B,48) labels / (B,) logp give B strings and
     a float32 array, as the greedy decoder returns them; (B,P,48) / (B,P) -- ``top_paths = P > 1`` -- give B lists of P
@@ -182,22 +254,38 @@ class Recognizer:
                             torch.cuda.current_stream(self.device).cuda_stream, color=color)
         return crnn_in, crops
 
-    def predict_device(self, crnn_in, with_scores=False, beam_width=None, top_paths=1):
+    def _decoder(self, beam_width, top_paths, lexicon):
+        """``check_decoder`` for this recognizer's alphabet."""
+        return check_decoder(beam_width, top_paths, lexicon, DEFAULT_ALPHABET if lexicon is None else self.alphabet)
+
+    def predict_device(self, crnn_in, with_scores=False, beam_width=None, top_paths=1, lexicon=None):
         """CRNN + greedy CTC.  crnn_in: (B,200,31) fp16 -> labels (B,48) int32 (-1 padded).  ``with_scores``: returns
         (labels, logp) with logp (B,) float32 the greedy path's log-probability (``b2o_crnn_forward_scored``).
         ``beam_width``: CTC prefix beam search instead (``b2o_crnn_forward_beam``, see ``check_beam``), logp = the beam
-        scores; ``top_paths > 1`` gives labels (B,P,48) and logp (B,P), best first."""
-        check_beam(beam_width, top_paths)
+        scores; ``top_paths > 1`` gives labels (B,P,48) and logp (B,P), best first.  ``lexicon`` (a ``Lexicon`` or a
+        list of strings, see ``check_decoder``): the ``top_paths`` most probable entries instead
+        (``b2o_crnn_forward_lexicon``), logp = their CTC forward log-probabilities, in the same shapes."""
+        lexicon = self._decoder(beam_width, top_paths, lexicon)
         b = crnn_in.shape[0]
         labels = torch.empty((b, STEPS), dtype=torch.int32, device=self.device)
         nbytes = self.ctx.crnn_workspace_bytes(b)
+        if lexicon is not None:
+            nbytes = (nbytes + 255) // 256 * 256 + self.ctx.lexicon_workspace_bytes(b, len(lexicon), int(top_paths))
         if self._ws is None or self._ws.numel() < nbytes:
             self._ws = None
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         ws = self._ws
         stream = torch.cuda.current_stream(self.device).cuda_stream
         logp = None
-        if beam_width is not None:
+        if lexicon is not None:
+            offsets, lex_labels = lexicon.device_arrays(self.device)
+            lead = (b,) if top_paths == 1 else (b, top_paths)
+            labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
+            logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
+            self.ctx.crnn_forward_lexicon(crnn_in.data_ptr(), b, offsets.data_ptr(), lex_labels.data_ptr(), len(lexicon),
+                                          int(top_paths), labels.data_ptr(), logp.data_ptr() if with_scores else None,
+                                          ws.data_ptr(), nbytes, stream)
+        elif beam_width is not None:
             lead = (b,) if top_paths == 1 else (b, top_paths)
             labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
             logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
@@ -220,12 +308,13 @@ class Recognizer:
                           torch.cuda.current_stream(self.device).cuda_stream)
         return out
 
-    def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1):
+    def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1, lexicon=None):
         """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str].
         ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``.  ``beam_width``: beam search
         decoding (``check_beam``); with ``top_paths = P > 1`` each text is a list of P strings and each confidence a
-        list of P floats, best first (``decode_paths``)."""
-        check_beam(beam_width, top_paths)
+        list of P floats, best first (``decode_paths``).  ``lexicon``: the most probable entries of a word list instead
+        (``check_decoder``), in the same shapes; a confidence is exp(the entry's CTC log-probability), clipped to 1."""
+        lexicon = self._decoder(beam_width, top_paths, lexicon)
         t = crops if isinstance(crops, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(crops))
         t = t.to(self.device).contiguous()
         b = t.shape[0]
@@ -235,34 +324,35 @@ class Recognizer:
         crnn_in = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + ((3,) if self.color else ()), dtype=torch.float16, device=self.device)
         self.ctx.crops_to_input(t.data_ptr(), b, crnn_in.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream,
                                 color=self.color)
-        beam = {"beam_width": beam_width, "top_paths": top_paths}
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
         if not return_scores:
             return decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
         labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
         return list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
 
-    def recognize(self, image, beam_width=None, top_paths=1):
+    def recognize(self, image, beam_width=None, top_paths=1, lexicon=None):
         """Recognize text from a single pre-cropped image (reference recognition.py:467-489): fit to
-        200x31 with zero fill (host, as upstream), gray conversion, then the CUDA CRNN.  ``beam_width`` / ``top_paths``:
-        as ``recognize_crops``."""
+        200x31 with zero fill (host, as upstream), gray conversion, then the CUDA CRNN.  ``beam_width`` / ``top_paths`` /
+        ``lexicon``: as ``recognize_crops``."""
         import cv2
 
-        check_beam(beam_width, top_paths)
+        lexicon = self._decoder(beam_width, top_paths, lexicon)
         image = tools.read_and_fit(filepath_or_array=image, width=TARGET_WIDTH, height=TARGET_HEIGHT, cval=0)
         if not self.color and image.ndim == 3 and image.shape[-1] == 3:      # recognition.py:481-483
             image = cv2.cvtColor(image, code=cv2.COLOR_RGB2GRAY)
         return self.recognize_crops(np.ascontiguousarray(image.reshape((1, TARGET_HEIGHT, TARGET_WIDTH) + ((3,) if self.color else ()))),
-                                    beam_width=beam_width, top_paths=top_paths)[0]
+                                    beam_width=beam_width, top_paths=top_paths, lexicon=lexicon)[0]
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
-                                    with_scores=False, beam_width=None, top_paths=1):
+                                    with_scores=False, beam_width=None, top_paths=1, lexicon=None):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
-        (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths``: see ``predict_device``).
+        (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon``: see
+        ``predict_device``).
 
         Optional device-side by-products of the earlier stages, so that nothing but the kernel launches is
         left to do once the host knows the counts: ``gray`` (N,H,W) u8 from ``b2o_resize_pad_batch``;
         ``flat`` (>=B,4,2) / ``image_index`` (>=B,) from ``b2o_compact_boxes``."""
-        check_beam(beam_width, top_paths)
+        lexicon = self._decoder(beam_width, top_paths, lexicon)
         counts = np.asarray(counts)
         m = boxes.shape[1]
         total = int(np.minimum(counts, m).sum())
@@ -280,14 +370,16 @@ class Recognizer:
             self.ctx.compact_boxes(boxes.data_ptr(), counts_dev.data_ptr(), n, m, flat.data_ptr(),
                                    image_index.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
-        return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths)
+        return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
+                                   lexicon=lexicon)
 
     # ------------------------------------------------------------------ reference API
-    def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1,
+    def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
                              **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
-        (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths``: as ``recognize_crops``."""
-        check_beam(beam_width, top_paths)
+        (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon``: as
+        ``recognize_crops``."""
+        lexicon = self._decoder(beam_width, top_paths, lexicon)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
 
@@ -303,7 +395,7 @@ class Recognizer:
         flat_t = torch.from_numpy(np.ascontiguousarray(flat)).to(self.device)
         idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
         crnn_in, _ = self.warp_device(images_t if self.color else self.gray_device(images_t), flat_t, idx)
-        beam = {"beam_width": beam_width, "top_paths": top_paths}
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
         if return_scores:
             labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
             predictions = list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))

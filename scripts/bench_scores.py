@@ -1,8 +1,14 @@
-"""bench_scores.py -- what detection scores, word confidences and beam-search decoding cost: ``Pipeline.recognize``
-with and without ``return_scores=True``, and with ``recognition_kwargs={"beam_width": W}`` for every W given, on the
-workload of bench.py (32 pages 768x768, scale 2 -> 1536x1536, sources resident in HBM).
+"""bench_scores.py -- what detection scores, word confidences, beam-search and lexicon decoding cost:
+``Pipeline.recognize`` with and without ``return_scores=True``, with ``recognition_kwargs={"beam_width": W}`` for every
+W given and with ``recognition_kwargs={"lexicon": L}`` for every lexicon size N given, on the workload of bench.py
+(32 pages 768x768, scale 2 -> 1536x1536, sources resident in HBM).  A size-N lexicon is the bench pages' rendered words
+plus seeded distractors (``oracle.synth.random_word``) up to N entries.
 
     python scripts/bench_scores.py [--steps K] [--warmup W] [--rounds R] [--beam-width W [W ...]]
+                                   [--lexicon-size N [N ...]] [--decoder-lexicon-size N [N ...]] [--decoder-calls C]
+
+``--decoder-lexicon-size``: the lexicon decoder alone (``b2o_ctc_lexicon_decode``, top_paths 1) on the fc_12 logits
+of one bench step's crops, C launches between CUDA events after a warm-up, in ms per call.
 
 The calls are timed alternately, R rounds of K steps each (CUDA events around K steps bracketed by a device
 synchronise), so that drifting clocks and other work on the host hit all alike; prints one JSON line with the medians,
@@ -37,15 +43,20 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--beam-width", type=int, nargs="+", default=[])
+    ap.add_argument("--lexicon-size", type=int, nargs="+", default=[])
+    ap.add_argument("--decoder-lexicon-size", type=int, nargs="+", default=[])
+    ap.add_argument("--decoder-calls", type=int, default=20)
     args = ap.parse_args()
 
+    import numpy as np
     import torch
 
     import bench
     from keras_ocr_b200 import weights as W
     from keras_ocr_b200.detection import Detector
     from keras_ocr_b200.pipeline import Pipeline
-    from keras_ocr_b200.recognition import Recognizer
+    from keras_ocr_b200.recognition import Lexicon, Recognizer
+    from oracle import synth
 
     assert torch.cuda.is_available(), "bench_scores.py needs a CUDA device; there is no CPU fallback"
     device = torch.device("cuda", 0)
@@ -57,6 +68,20 @@ def main():
     calls = {"default": lambda: pipe.recognize(pages), "scored": lambda: pipe.recognize(pages, return_scores=True)}
     for w in args.beam_width:
         calls[f"beam{w}"] = lambda w=w: pipe.recognize(pages, recognition_kwargs={"beam_width": w})
+
+    def lexicon(n):
+        words = list(dict.fromkeys(w for page in page_words for w in page))[:n]
+        seen, rng = set(words), np.random.default_rng(n)
+        while len(words) < n:
+            w = synth.random_word(rng)
+            if w not in seen:
+                seen.add(w)
+                words.append(w)
+        return Lexicon(words, rec.alphabet)
+
+    lexicons = {n: lexicon(n) for n in sorted(set(args.lexicon_size) | set(args.decoder_lexicon_size))}
+    for n in args.lexicon_size:
+        calls[f"lexicon{n}"] = lambda n=n: pipe.recognize(pages, recognition_kwargs={"lexicon": lexicons[n]})
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -96,6 +121,33 @@ def main():
             line[f"{k}_overhead"] = statistics.median(ms[k]) / statistics.median(ms["default"]) - 1.0
             line[f"{k}_words_differing_from_default"] = sum(a != b for a, b in zip([t for g in result for t, _ in g],
                                                                                   default_words))
+    if args.decoder_lexicon_size:
+        rec.keep_workspace = True
+        n_crops = sum(len(g) for g in pipe.recognize(pages))
+        logits = rec.tap("logits", (n_crops, 48, len(rec.alphabet) + 1), torch.float32)
+        rec.keep_workspace = False
+        line["decoder_crops"] = n_crops
+        for n in args.decoder_lexicon_size:
+            off, lab = lexicons[n].device_arrays(device)
+            out = torch.empty((n_crops, 1, 48), dtype=torch.int32, device=device)
+            logp = torch.empty((n_crops, 1), dtype=torch.float32, device=device)
+            nbytes = rec.ctx.lexicon_workspace_bytes(n_crops, n, 1)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+            stream = torch.cuda.current_stream(device).cuda_stream
+
+            def call():
+                rec.ctx.ctc_lexicon_decode(logits.data_ptr(), n_crops, logits.shape[2], off.data_ptr(), lab.data_ptr(), n,
+                                           1, out.data_ptr(), logp.data_ptr(), ws.data_ptr(), nbytes, stream)
+            for _ in range(3):
+                call()
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(args.decoder_calls):
+                call()
+            e1.record()
+            torch.cuda.synchronize()
+            line[f"decoder_lexicon{n}_ms_per_call"] = e0.elapsed_time(e1) / args.decoder_calls
     print(json.dumps(line))
 
 
