@@ -148,6 +148,39 @@ int b2o_warp_boxes_color(b2o_ctx* ctx, const uint8_t* rgb_dev, int n, int h, int
                          const float* boxes_dev, const int32_t* image_index_dev, int n_boxes,
                          uint8_t* crops_dev, void* crnn_in_dev, void* stream);
 
+/* The crops of b2o_warp_boxes (channels = 1) or b2o_warp_boxes_color (channels = 3) cut in quarter turn `turn` (0..3).
+ * With c = (tl, tr, br, bl) the corner order warpBox cuts with (get_rotated_box, tools.py:533-581), the crop in turn r is
+ * warpBox(image, np.roll(c, -r, axis=0), 31, 200, skip_rotate=True): its top-left is c[r], and width and height are
+ * measured after the roll, so odd turns swap them.  A word on a page turned by np.rot90(page, k) reads upright in turn
+ * (4 - k) % 4.  Turn 0 is bit-identical to b2o_warp_boxes / b2o_warp_boxes_color; the kernel is the same one.        */
+int b2o_warp_boxes_turned(b2o_ctx* ctx, const uint8_t* img_dev, int channels, int n, int h, int w,
+                          const float* boxes_dev, const int32_t* image_index_dev, int n_boxes, int turn,
+                          uint8_t* crops_dev, void* crnn_in_dev, void* stream);
+
+/* Choosing between the readings of several quarter turns.  Inputs: the results of n_turns runs of
+ * b2o_warp_boxes_turned + a decoder (b2o_crnn_forward_scored, _beam or _lexicon), stacked in the order of turns_host
+ * (host, n_turns distinct values in 0..3, 1 <= n_turns <= 4): labels_dev (n_turns, b, top_paths, 48) int32 and
+ * logp_dev (n_turns, b, top_paths) float32, best reading first.  image_index_dev (b) int32 is non-decreasing with values
+ * in [0, n_images), as b2o_compact_boxes writes it.
+ * The vote compares each turn's best reading, logp[j, k, 0]:
+ *   B2O_ROTATION_VOTE_WORD: every word keeps the turn with the largest score;
+ *   B2O_ROTATION_VOTE_PAGE: every image keeps one turn for all its words, the one with the largest float32 sum of its
+ *                           words' scores, added in word order by one thread (the sum does not depend on the batch).
+ * Ties, and words or images whose scores are all -inf, keep the turn listed first.
+ * Outputs: labels_out_dev (b, top_paths, 48) and logp_out_dev (b, top_paths), the chosen turn's readings (a (b, 1, 48)
+ * result has the (b, 48) layout b2o_pack_records(_scored) takes), and turn_out_dev (b) int32 the chosen turn r.
+ * boxes_dev (b,4,2) float32, when not NULL, is rewritten in place as np.roll(c, -r, axis=0): box[0] is then the corner the
+ * crop started at, the text's own top-left, still clockwise.  table_dev (n_images, max_boxes, 4, 2), when not NULL, is
+ * the b2o_get_boxes table that b2o_compact_boxes made boxes_dev from, and receives the same rolled boxes (word k of
+ * image i at slot k - (first word of i)), so the host copy and b2o_pack_records(_scored) read them unchanged.
+ * The corner order is the one b2o_warp_boxes_turned uses.  A word's result is bit-identical in any batch.          */
+#define B2O_ROTATION_VOTE_WORD 0
+#define B2O_ROTATION_VOTE_PAGE 1
+int b2o_select_rotation(b2o_ctx* ctx, const int32_t* labels_dev, const float* logp_dev, const int32_t* image_index_dev,
+                        int n_images, int b, int top_paths, const int32_t* turns_host, int n_turns, int vote,
+                        int32_t* labels_out_dev, float* logp_out_dev, int32_t* turn_out_dev, float* boxes_dev,
+                        float* table_dev, int max_boxes, void* stream);
+
 /* prediction_model.predict (recognition.py:535; graph 214-333): CRNN + STN + BiLSTM + greedy CTC (beam search:
  * b2o_crnn_forward_beam below; a caller's word list: b2o_crnn_forward_lexicon).
  * crnn_in: (b,200,31) fp16 from b2o_warp_boxes (or b2o_crops_to_input).  labels: (b,48) int32,

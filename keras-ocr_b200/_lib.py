@@ -18,6 +18,7 @@ MAX_BEAM_WIDTH = 128          # B2O_MAX_BEAM_WIDTH in include/b2ocr.h
 MAX_LEXICON_WORDS = 1 << 20   # B2O_MAX_LEXICON_WORDS
 MAX_LEXICON_LABELS = 1 << 24  # B2O_MAX_LEXICON_LABELS
 MAX_LEXICON_TOP_PATHS = 128   # B2O_MAX_LEXICON_TOP_PATHS
+ROTATION_VOTE_WORD, ROTATION_VOTE_PAGE = 0, 1   # B2O_ROTATION_VOTE_WORD / _PAGE
 
 
 class B2OError(RuntimeError):
@@ -73,6 +74,9 @@ SIGNATURES = {
     "b2o_pack_records_scored": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "b2o_warp_boxes": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
     "b2o_warp_boxes_color": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "b2o_warp_boxes_turned": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "b2o_select_rotation": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _c.POINTER(_c.c_int32), _i, _i, _vp, _vp, _vp, _vp,
+                                 _vp, _i, _vp]),
     "b2o_crops_to_input_color": (_i, [_vp, _vp, _i, _vp, _vp]),
     "b2o_crnn_workspace_bytes": (_sz, [_i]),
     "b2o_crops_to_input": (_i, [_vp, _vp, _i, _vp, _vp]),
@@ -248,6 +252,18 @@ class Context:
     def warp_boxes(self, gray, n, h, w, boxes, image_index, n_boxes, crops, crnn_in, stream, color=False):
         fn = self.lib.b2o_warp_boxes_color if color else self.lib.b2o_warp_boxes
         self._check(fn(self.handle, gray, n, h, w, boxes, image_index, n_boxes, crops, crnn_in, stream), "b2o_warp_boxes")
+
+    def warp_boxes_turned(self, img, channels, n, h, w, boxes, image_index, n_boxes, turn, crops, crnn_in, stream):
+        self._check(self.lib.b2o_warp_boxes_turned(self.handle, img, channels, n, h, w, boxes, image_index, n_boxes,
+                                                   turn, crops, crnn_in, stream), "b2o_warp_boxes_turned")
+
+    def select_rotation(self, labels, logp, image_index, n_images, b, top_paths, turns, vote, labels_out, logp_out,
+                        turn_out, boxes, table, max_boxes, stream):
+        """b2o_select_rotation: ``turns`` a host sequence of ints, ``vote`` ROTATION_VOTE_WORD / ROTATION_VOTE_PAGE."""
+        t = (ctypes.c_int32 * len(turns))(*[int(r) for r in turns])
+        self._check(self.lib.b2o_select_rotation(self.handle, labels, logp, image_index, n_images, b, top_paths, t,
+                                                 len(turns), vote, labels_out, logp_out, turn_out, boxes, table,
+                                                 max_boxes, stream), "b2o_select_rotation")
 
     def crnn_workspace_bytes(self, b):
         return int(self.lib.b2o_crnn_workspace_bytes(b))

@@ -157,6 +157,34 @@ int upsample_run(b2o_ctx* ctx, const TensorView& in, const TensorView& out, cuda
 int head_tail_run(b2o_ctx* ctx, const ConvLayer& L6, const ConvLayer& L8, const TensorView& in,
                   float* scores, cudaStream_t st);
 
+// ---- box corner order (image.cu's warp, rotation.cu's box roll) ---------------------------------
+// fp64 Euclidean distance of two float32 points, as scipy's cdist computes it (tools.py:41-57)
+static __device__ inline double corner_dist(const float* a, const float* b) {
+  const double dx = static_cast<double>(a[0]) - static_cast<double>(b[0]);
+  const double dy = static_cast<double>(a[1]) - static_cast<double>(b[1]);
+  return sqrt(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
+}
+
+// get_rotated_box on a rectangle (tools.py:533-581): ord = the indices of q (4x2) in the order tl, tr, br, bl -- stable
+// sort by x, the two left corners split by y, the right ones by distance from tl.
+static __device__ inline void order_corners(const float* q, int ord[4]) {
+  int idx[4] = {0, 1, 2, 3};
+  for (int i = 1; i < 4; ++i) {              // insertion sort == numpy's argsort(kind="stable")
+    const int v = idx[i];
+    int j = i - 1;
+    while (j >= 0 && q[2 * idx[j]] > q[2 * v]) { idx[j + 1] = idx[j]; --j; }
+    idx[j + 1] = v;
+  }
+  int l0 = idx[0], l1 = idx[1];
+  if (q[2 * l0 + 1] > q[2 * l1 + 1]) { const int t = l0; l0 = l1; l1 = t; }
+  const int r0 = idx[2], r1 = idx[3];
+  const double d0 = corner_dist(q + 2 * l0, q + 2 * r0), d1 = corner_dist(q + 2 * l0, q + 2 * r1);
+  ord[0] = l0;                               // tl
+  ord[3] = l1;                               // bl
+  // (br, tr) = rightMost[argsort(D)[::-1]]
+  if (d0 <= d1) { ord[2] = r1; ord[1] = r0; } else { ord[2] = r0; ord[1] = r1; }
+}
+
 static inline TensorView make_view(void* base, int n, int h, int w, int c, int ld = 0, int coff = 0) {
   TensorView v;
   v.ptr = reinterpret_cast<__half*>(base) + coff;

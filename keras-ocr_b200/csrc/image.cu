@@ -6,7 +6,8 @@
 //   gray_kernel       : cv2.cvtColor(RGB2GRAY) (recognition.py:510)
 //   warp_kernel       : tools.warpBox (tools.py:61-117): get_rotated_box ordering (533-581, rectangle
 //                       branch), get_rotated_width_height (41-57), cv2.getPerspectiveTransform (8x8 LU,
-//                       fp64), cv2.warpPerspective INTER_LINEAR (1/32-pixel coordinates, 15-bit weights)
+//                       fp64), cv2.warpPerspective INTER_LINEAR (1/32-pixel coordinates, 15-bit weights); in quarter
+//                       turn r the ordered box is rolled by r first (warpBox(skip_rotate=True), b2o_warp_boxes_turned)
 #include <math.h>
 
 #include "common.cuh"
@@ -79,33 +80,21 @@ __global__ void gray_kernel(const uint8_t* __restrict__ img, long long total, ui
 // of warpPerspective; valid = 0 where warpBox raises ZeroDivisionError (or the system is singular).
 using WarpPlan = b2o_warp_plan;
 
-__device__ double dist2(const float* a, const float* b) {
-  const double dx = static_cast<double>(a[0]) - static_cast<double>(b[0]);
-  const double dy = static_cast<double>(a[1]) - static_cast<double>(b[1]);
-  return sqrt(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
-}
-
-__device__ void plan_warp(const float* q /*4x2*/, int target_w, int target_h, WarpPlan* plan) {
+// turn r (0..3): warpBox(skip_rotate=True) of the ordered box rolled by r, np.roll(c, -r, axis=0) -- the crop starts at
+// corner c[r] and odd turns swap width and height.  Turn 0 is tools.warpBox itself.
+__device__ void plan_warp(const float* q /*4x2*/, int turn, int target_w, int target_h, WarpPlan* plan) {
   plan->valid = 0;
-  // --- get_rotated_box on a rectangle: stable sort by x, split, order by y / by distance ---------
-  int idx[4] = {0, 1, 2, 3};
-  for (int i = 1; i < 4; ++i) {              // insertion sort == numpy's argsort(kind="stable")
-    const int v = idx[i];
-    int j = i - 1;
-    while (j >= 0 && q[2 * idx[j]] > q[2 * v]) { idx[j + 1] = idx[j]; --j; }
-    idx[j + 1] = v;
+  // --- get_rotated_box on a rectangle, then the roll -----------------------------------------------
+  int ord[4];
+  order_corners(q, ord);
+  float box[8];
+  for (int i = 0; i < 4; ++i) {
+    box[2 * i] = q[2 * ord[(i + turn) & 3]];
+    box[2 * i + 1] = q[2 * ord[(i + turn) & 3] + 1];
   }
-  int l0 = idx[0], l1 = idx[1], r0 = idx[2], r1 = idx[3];
-  if (q[2 * l0 + 1] > q[2 * l1 + 1]) { const int t = l0; l0 = l1; l1 = t; }
-  const int tl = l0, bl = l1;
-  const double d0 = dist2(q + 2 * tl, q + 2 * r0), d1 = dist2(q + 2 * tl, q + 2 * r1);
-  // (br, tr) = rightMost[argsort(D)[::-1]]
-  int br, tr;
-  if (d0 <= d1) { br = r1; tr = r0; } else { br = r0; tr = r1; }
-  float box[8] = {q[2 * tl], q[2 * tl + 1], q[2 * tr], q[2 * tr + 1], q[2 * br], q[2 * br + 1], q[2 * bl], q[2 * bl + 1]};
   // --- get_rotated_width_height --------------------------------------------------------------------
-  const int w = static_cast<int>((dist2(box + 0, box + 2) + dist2(box + 4, box + 6)) / 2);
-  const int h = static_cast<int>((dist2(box + 0, box + 6) + dist2(box + 2, box + 4)) / 2);
+  const int w = static_cast<int>((corner_dist(box + 0, box + 2) + corner_dist(box + 4, box + 6)) / 2);
+  const int h = static_cast<int>((corner_dist(box + 0, box + 6) + corner_dist(box + 2, box + 4)) / 2);
   if (w <= 0 || h <= 0) return;              // the reference raises ZeroDivisionError here
   const double sa = static_cast<double>(target_w) / w, sb = static_cast<double>(target_h) / h;
   const double scale = sa < sb ? sa : sb;
@@ -182,11 +171,11 @@ constexpr int kCropH = 31, kCropW = 200;
 template <int CH>
 __global__ void __launch_bounds__(256)
 warp_kernel(const uint8_t* __restrict__ gray, int n, int H, int W, const float* __restrict__ boxes,
-            const int* __restrict__ image_index, uint8_t* __restrict__ crops, __half* __restrict__ crnn_in) {
+            const int* __restrict__ image_index, int turn, uint8_t* __restrict__ crops, __half* __restrict__ crnn_in) {
   __shared__ WarpPlan plan;
   __shared__ uint8_t tile[kCropH * kCropW * CH];
   const int k = blockIdx.x;
-  if (threadIdx.x == 0) plan_warp(boxes + static_cast<size_t>(k) * 8, kCropW, kCropH, &plan);
+  if (threadIdx.x == 0) plan_warp(boxes + static_cast<size_t>(k) * 8, turn, kCropW, kCropH, &plan);
   __syncthreads();
   int img = image_index[k];
   img = min(max(img, 0), n - 1);
@@ -249,7 +238,7 @@ __global__ void warp_plan_kernel(const float* __restrict__ boxes, int n, WarpPla
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
   WarpPlan p = {};
-  plan_warp(boxes + static_cast<size_t>(k) * 8, kCropW, kCropH, &p);
+  plan_warp(boxes + static_cast<size_t>(k) * 8, 0, kCropW, kCropH, &p);
   plans[k] = p;
 }
 
@@ -309,29 +298,38 @@ extern "C" int b2o_rgb_to_gray(b2o_ctx* ctx, const uint8_t* img, int n, int h, i
 }
 
 static int warp_boxes_impl(b2o_ctx* ctx, const uint8_t* img, int ch, int n, int h, int w, const float* boxes,
-                           const int32_t* image_index, int n_boxes, uint8_t* crops, void* crnn_in, void* stream) {
+                           const int32_t* image_index, int n_boxes, int turn, uint8_t* crops, void* crnn_in,
+                           void* stream) {
   if (!ctx) return B2O_ERR_ARG;
   DeviceGuard guard(ctx->device);
+  if (ch != 1 && ch != 3) { ctx->set_error("b2o_warp_boxes: channels must be 1 or 3"); return B2O_ERR_ARG; }
+  if (turn < 0 || turn > 3) { ctx->set_error("b2o_warp_boxes_turned: turn must be 0, 1, 2 or 3"); return B2O_ERR_ARG; }
   if (n_boxes == 0) return B2O_OK;
   if (!img || !boxes || !image_index || n <= 0 || h <= 0 || w <= 0 || n_boxes < 0 || (!crops && !crnn_in)) {
     ctx->set_error("b2o_warp_boxes: bad argument");
     return B2O_ERR_ARG;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (ch == 3) warp_kernel<3><<<n_boxes, 256, 0, st>>>(img, n, h, w, boxes, image_index, crops, reinterpret_cast<__half*>(crnn_in));
-  else warp_kernel<1><<<n_boxes, 256, 0, st>>>(img, n, h, w, boxes, image_index, crops, reinterpret_cast<__half*>(crnn_in));
+  if (ch == 3) warp_kernel<3><<<n_boxes, 256, 0, st>>>(img, n, h, w, boxes, image_index, turn, crops, reinterpret_cast<__half*>(crnn_in));
+  else warp_kernel<1><<<n_boxes, 256, 0, st>>>(img, n, h, w, boxes, image_index, turn, crops, reinterpret_cast<__half*>(crnn_in));
   B2O_LAUNCH_CHECK(ctx);
   return B2O_OK;
 }
 
 extern "C" int b2o_warp_boxes(b2o_ctx* ctx, const uint8_t* gray, int n, int h, int w, const float* boxes,
                               const int32_t* image_index, int n_boxes, uint8_t* crops, void* crnn_in, void* stream) {
-  return warp_boxes_impl(ctx, gray, 1, n, h, w, boxes, image_index, n_boxes, crops, crnn_in, stream);
+  return warp_boxes_impl(ctx, gray, 1, n, h, w, boxes, image_index, n_boxes, 0, crops, crnn_in, stream);
 }
 
 extern "C" int b2o_warp_boxes_color(b2o_ctx* ctx, const uint8_t* rgb, int n, int h, int w, const float* boxes,
                                     const int32_t* image_index, int n_boxes, uint8_t* crops, void* crnn_in, void* stream) {
-  return warp_boxes_impl(ctx, rgb, 3, n, h, w, boxes, image_index, n_boxes, crops, crnn_in, stream);
+  return warp_boxes_impl(ctx, rgb, 3, n, h, w, boxes, image_index, n_boxes, 0, crops, crnn_in, stream);
+}
+
+extern "C" int b2o_warp_boxes_turned(b2o_ctx* ctx, const uint8_t* img, int channels, int n, int h, int w,
+                                     const float* boxes, const int32_t* image_index, int n_boxes, int turn,
+                                     uint8_t* crops, void* crnn_in, void* stream) {
+  return warp_boxes_impl(ctx, img, channels, n, h, w, boxes, image_index, n_boxes, turn, crops, crnn_in, stream);
 }
 
 extern "C" int b2o_warp_plan_test(b2o_ctx* ctx, const float* boxes, int n, b2o_warp_plan* plans, void* stream) {

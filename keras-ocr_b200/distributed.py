@@ -130,7 +130,7 @@ def _host_records(pipeline, local, per_rank, max_boxes):
 
 
 def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_scores=False, beam_width=None,
-                      top_paths=1, lexicon=None):
+                      top_paths=1, lexicon=None, rotations=None, rotation_vote="word"):
     """Run ``pipeline.recognize`` on this rank's shard of ``images`` and gather to rank 0.
 
     ``images`` is the global batch (every rank passes the same list and takes its contiguous slice) or, with
@@ -147,10 +147,14 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
     (``recognition.check_beam``); records carry the best path only, so ``top_paths`` > 1 raises ``ValueError``.
     ``lexicon``: every word reads as the most probable entry of that word list (``recognition.check_decoder``); a
     ``recognition.Lexicon`` is compiled once and uploaded once per device, a plain list is compiled here.
+    ``rotations`` / ``rotation_vote``: every word is read in each listed quarter turn and the most probable reading kept
+    (``recognition.check_rotations``); boxes start at the chosen turn's corner, as ``Pipeline.recognize`` returns them.
     """
     from .pipeline import check_records_decoder
+    from .recognition import check_rotations
     lexicon = check_records_decoder(beam_width, top_paths, lexicon,
                                     None if lexicon is None else pipeline.recognizer.alphabet)
+    rotations = check_rotations(rotations, rotation_vote)
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
     if presharded:
@@ -170,6 +174,8 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
         sk["beam_width"] = beam_width
     if lexicon is not None:
         sk["lexicon"] = lexicon
+    if rotations is not None:
+        sk["rotations"], sk["rotation_vote"] = rotations, rotation_vote
     if native:
         if getattr(pipeline, "records_counts", None) is not None:
             state = pipeline.records_begin(mine, rows=per_rank, rec_boxes=16 if max_boxes == "auto" else max_boxes, **sk)
@@ -181,7 +187,7 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
             local = pipeline.recognize_records(mine, rows=per_rank, rec_boxes=max_boxes, **sk)
         device = None                                   # already where the backend wants it
     else:
-        rk = {k: v for k, v in (("beam_width", beam_width), ("lexicon", lexicon)) if v is not None}
+        rk = {k: v for k, v in sk.items() if k != "scores"}
         rk = {"recognition_kwargs": rk} if rk else {}
         result = pipeline.recognize(mine, **rk) if len(mine) else []
         if max_boxes == "auto":
@@ -262,13 +268,16 @@ class ShardedStream:
     asynchronous copy into pinned memory; any other pipeline (``recognize`` only) is served too, without the overlap.
     ``max_boxes``: words a record holds (an image with more raises ``RecordOverflow`` on rank 0 when its batch is
     decoded) or ``"auto"`` (sized per batch by ``agree_max_boxes``).  ``return_scores=True``: words as
-    ``recognize_sharded(return_scores=True)`` returns them (device records only).  ``beam_width`` / ``lexicon``: as
-    ``recognize_sharded``."""
+    ``recognize_sharded(return_scores=True)`` returns them (device records only).  ``beam_width`` / ``lexicon`` /
+    ``rotations`` / ``rotation_vote``: as ``recognize_sharded``."""
 
-    def __init__(self, pipeline, max_boxes=128, return_scores=False, beam_width=None, top_paths=1, lexicon=None):
+    def __init__(self, pipeline, max_boxes=128, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
+                 rotations=None, rotation_vote="word"):
         from .pipeline import check_records_decoder
+        from .recognition import check_rotations
         lexicon = check_records_decoder(beam_width, top_paths, lexicon,
                                         None if lexicon is None else pipeline.recognizer.alphabet)
+        rotations = check_rotations(rotations, rotation_vote)
         self.pipeline, self.max_boxes = pipeline, max_boxes
         self.world = dist.get_world_size() if dist.is_initialized() else 1
         self.rank = dist.get_rank() if dist.is_initialized() else 0
@@ -282,7 +291,8 @@ class ShardedStream:
         self.return_scores = return_scores
         self._sk = {"scores": True} if return_scores else {}
         self._rk = {}
-        for k, v in (("beam_width", beam_width), ("lexicon", lexicon)):
+        rot = (("rotations", rotations), ("rotation_vote", rotation_vote)) if rotations is not None else ()
+        for k, v in (("beam_width", beam_width), ("lexicon", lexicon)) + rot:
             if v is not None:
                 self._sk[k] = v
                 self._rk.setdefault("recognition_kwargs", {})[k] = v

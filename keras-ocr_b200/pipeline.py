@@ -143,6 +143,8 @@ class Pipeline:
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
                                                  image_index=bst["image_index"], with_scores=box_scores is not None,
                                                  **beam)
+        if beam.get("rotations") is not None:            # drop the chosen turns: the rolled boxes carry them
+            labels = labels[:-1] if box_scores is not None else labels[0]
         if box_scores is not None:
             labels, logp = labels
             self._to_host(st, "box_scores_host", box_scores)
@@ -198,7 +200,11 @@ class Pipeline:
         instead of greedy decoding, boxes unchanged; with ``top_paths = P > 1`` the text of every word is a list of P
         readings and its confidence a list of P floats, best first.  Or ``lexicon`` (a ``recognition.Lexicon`` or a
         list of strings) / ``top_paths``: every word reads as the most probable entries of that list, in the same
-        shapes (``recognition.check_decoder``).  Injected recognizers get ``recognition_kwargs`` as they are.
+        shapes (``recognition.check_decoder``).  With any of these decoders, ``rotations`` / ``rotation_vote``
+        (``recognition.check_rotations``) read every word in each listed quarter turn and keep the most probable
+        reading, per word or per image; every returned box then starts at the chosen turn's corner, so box[0] is the
+        text's own top-left corner (the same corners, still clockwise).  Injected recognizers get
+        ``recognition_kwargs`` as they are.
         """
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
@@ -214,6 +220,10 @@ class Pipeline:
             lexicon = self.recognizer._decoder(beam.get("beam_width"), beam.get("top_paths", 1), beam.get("lexicon"))
             if lexicon is not None:
                 beam["lexicon"] = lexicon                 # compiled once for every sub-batch
+            vote = recognition_kwargs.get("rotation_vote", "word")
+            turns = recognition.check_rotations(recognition_kwargs.get("rotations"), vote)
+            if turns is not None:
+                beam["rotations"], beam["rotation_vote"] = turns, vote
         if not self._native():
             if return_scores:
                 raise NotImplementedError("return_scores=True needs this package's Detector and Recognizer; injected "
@@ -242,7 +252,7 @@ class Pipeline:
         return out
 
     def recognize_records(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
-                          top_paths=1, lexicon=None):
+                          top_paths=1, lexicon=None, rotations=None, rotation_vote="word"):
         """``recognize`` without the trip to the host: returns the results as a CUDA float32 tensor of fixed-size
         per-image records, ``(rows, b2o_record_floats(rec_boxes))`` = [count | rec_boxes x (4,2) boxes in source
         pixels | rec_boxes x 48 int8 labels] (``distributed.unpack_blocks`` decodes it; rows beyond ``len(images)``
@@ -252,17 +262,20 @@ class Pipeline:
         path log-probabilities] to that record.  ``beam_width``: the words are beam-search decoded
         (``recognition.check_beam``); a record carries the best path only, so ``top_paths`` > 1 raises ``ValueError``.
         ``lexicon``: every word reads as the most probable entry of that word list (``recognition.check_decoder``), its
-        log-probability in the scored layout."""
+        log-probability in the scored layout.  ``rotations`` / ``rotation_vote``: every word is read in each listed
+        quarter turn and the most probable reading kept (``recognition.check_rotations``); the records' boxes start at
+        the chosen turn's corner, as ``recognize`` returns them."""
         return self.records_end(self.records_begin(images, rows, rec_boxes, detection_kwargs, scores, beam_width,
-                                                   top_paths, lexicon))
+                                                   top_paths, lexicon, rotations, rotation_vote))
 
     def records_begin(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
-                      top_paths=1, lexicon=None):
+                      top_paths=1, lexicon=None, rotations=None, rotation_vote="word"):
         """First half of ``recognize_records``: queues resize/pad, CRAFT and getBoxes and returns at once (no
         synchronisation), so the caller can use the host while the GPU works (``distributed.ShardedStream`` decodes the
         previous batch's words here).  Pass the returned state to ``records_end``."""
         lexicon = check_records_decoder(beam_width, top_paths, lexicon,
                                         recognition.DEFAULT_ALPHABET if lexicon is None else self.recognizer.alphabet)
+        turns = recognition.check_rotations(rotations, rotation_vote)
         assert self._native(), "recognize_records needs this package's Detector and Recognizer"
         assert len(self.recognizer.alphabet) + 1 <= 127, "record labels travel as int8: alphabets up to 126 characters"
         if not isinstance(images, (np.ndarray, torch.Tensor)):
@@ -277,7 +290,7 @@ class Pipeline:
         assert rows >= n and rows > 0
         self.last_stats = {"h2d_bytes": 0, "d2h_bytes": 0}
         state = {"n": n, "rows": rows, "rec_boxes": rec_boxes, "scores": bool(scores), "beam_width": beam_width,
-                 "lexicon": lexicon}
+                 "lexicon": lexicon, "rotations": turns, "rotation_vote": rotation_vote}
         if n:
             plans = self._plans(images)
             state["st"] = self._stage_detect(images, (max(p[1] for p in plans), max(p[2] for p in plans)), thresholds,
@@ -316,7 +329,11 @@ class Pipeline:
         boxes = state["boxes"]
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
                                                  image_index=bst["image_index"], with_scores=scored,
-                                                 beam_width=state.get("beam_width"), lexicon=state.get("lexicon"))
+                                                 beam_width=state.get("beam_width"), lexicon=state.get("lexicon"),
+                                                 rotations=state.get("rotations"),
+                                                 rotation_vote=state.get("rotation_vote", "word"))
+        if state.get("rotations") is not None:           # the turns are in the rolled boxes the records carry
+            labels = labels[:-1] if scored else labels[0]
         inv = torch.tensor([1.0 / s for s in st["scales"]], dtype=torch.float32).to(det.device, non_blocking=True)
         stream = torch.cuda.current_stream(det.device).cuda_stream
         ptr = lambda t: t.data_ptr() if t is not None else None      # noqa: E731

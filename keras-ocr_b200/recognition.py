@@ -131,6 +131,32 @@ def check_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_A
     return lexicon
 
 
+ROTATION_VOTES = {"word": _lib.ROTATION_VOTE_WORD, "page": _lib.ROTATION_VOTE_PAGE}
+
+
+def check_rotations(rotations=None, rotation_vote="word"):
+    """Validates a choice of quarter turns before anything is launched (``ValueError`` otherwise) and returns the turns
+    as a tuple of ints, or None.  ``rotations=None`` (the default) reads every crop as it is cut.  Otherwise a non-empty
+    tuple or list of distinct ints from {0, 1, 2, 3}: every box is cut and decoded once per listed turn -- turn r starts
+    the crop at corner r of the ordered box (tl, tr, br, bl), so a word on a page turned by ``np.rot90(page, k)`` reads
+    upright in turn (4 - k) % 4 -- and ``rotation_vote`` picks one reading: ``"word"`` keeps, per word, the turn whose
+    best reading has the largest log-probability; ``"page"`` keeps one turn per image, the one with the largest sum over
+    the image's words.  Ties, and all -inf scores, go to the turn listed first."""
+    if not isinstance(rotation_vote, str) or rotation_vote not in ROTATION_VOTES:
+        raise ValueError(f"rotation_vote must be 'word' or 'page', got {rotation_vote!r}")
+    if rotations is None:
+        return None
+    if not isinstance(rotations, (tuple, list)) or not rotations:
+        raise ValueError(f"rotations must be None or a non-empty tuple or list of quarter turns, got {rotations!r}")
+    for r in rotations:
+        if not isinstance(r, (int, np.integer)) or isinstance(r, (bool, np.bool_)) or not 0 <= r <= 3:
+            raise ValueError(f"rotations holds quarter turns 0, 1, 2 or 3, got {r!r}")
+    turns = tuple(int(r) for r in rotations)
+    if len(set(turns)) != len(turns):
+        raise ValueError(f"rotations must be distinct, got {rotations!r}")
+    return turns
+
+
 def decode_paths(labels, alphabet=DEFAULT_ALPHABET, logp=None):
     """Host labels -> texts, and logp -> confidences (None without logp).  (B,48) labels / (B,) logp give B strings and
     a float32 array, as the greedy decoder returns them; (B,P,48) / (B,P) -- ``top_paths = P > 1`` -- give B lists of P
@@ -239,8 +265,9 @@ class Recognizer:
         self.ctx.rgb_to_gray(images_t.data_ptr(), n, h, w, gray.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
         return gray
 
-    def warp_device(self, gray, boxes_flat, image_index, want_crops=False):
+    def warp_device(self, gray, boxes_flat, image_index, want_crops=False, turn=None):
         """tools.warpBox for every box.  ``gray``: (N,H,W) u8 -- or the RGB batch (N,H,W,3) for a color recognizer.
+        ``turn`` (0..3): the crops in that quarter turn (``b2o_warp_boxes_turned``, see ``check_rotations``).
         Returns (crnn_in (B,200,31[,3]) fp16, crops (B,31,200[,3]) u8 or None)."""
         n, h, w = gray.shape[:3]
         color = gray.dim() == 4
@@ -249,9 +276,14 @@ class Recognizer:
         b = boxes_flat.shape[0]
         crnn_in = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + tail, dtype=torch.float16, device=self.device)
         crops = torch.empty((b, TARGET_HEIGHT, TARGET_WIDTH) + tail, dtype=torch.uint8, device=self.device) if want_crops else None
-        self.ctx.warp_boxes(gray.data_ptr(), n, h, w, boxes_flat.data_ptr(), image_index.data_ptr(), b,
-                            crops.data_ptr() if want_crops else None, crnn_in.data_ptr(),
-                            torch.cuda.current_stream(self.device).cuda_stream, color=color)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        if turn is None:
+            self.ctx.warp_boxes(gray.data_ptr(), n, h, w, boxes_flat.data_ptr(), image_index.data_ptr(), b,
+                                crops.data_ptr() if want_crops else None, crnn_in.data_ptr(), stream, color=color)
+        else:
+            self.ctx.warp_boxes_turned(gray.data_ptr(), 3 if color else 1, n, h, w, boxes_flat.data_ptr(),
+                                       image_index.data_ptr(), b, int(turn), crops.data_ptr() if want_crops else None,
+                                       crnn_in.data_ptr(), stream)
         return crnn_in, crops
 
     def _decoder(self, beam_width, top_paths, lexicon):
@@ -267,7 +299,16 @@ class Recognizer:
         (``b2o_crnn_forward_lexicon``), logp = their CTC forward log-probabilities, in the same shapes."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
         b = crnn_in.shape[0]
-        labels = torch.empty((b, STEPS), dtype=torch.int32, device=self.device)
+        lead = (b,) if top_paths == 1 else (b, top_paths)
+        labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
+        logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
+        self._forward(crnn_in, labels, logp, beam_width, top_paths, lexicon)
+        return (labels, logp) if with_scores else labels
+
+    def _forward(self, crnn_in, labels, logp, beam_width, top_paths, lexicon):
+        """The CRNN and the decoder of ``predict_device`` into caller-allocated ``labels`` / ``logp`` (None: greedy
+        without scores, or scores not written); ``lexicon`` is already compiled."""
+        b = crnn_in.shape[0]
         nbytes = self.ctx.crnn_workspace_bytes(b)
         if lexicon is not None:
             nbytes = (nbytes + 255) // 256 * 256 + self.ctx.lexicon_workspace_bytes(b, len(lexicon), int(top_paths))
@@ -276,29 +317,20 @@ class Recognizer:
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         ws = self._ws
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        logp = None
+        logp_ptr = logp.data_ptr() if logp is not None else None
         if lexicon is not None:
             offsets, lex_labels = lexicon.device_arrays(self.device)
-            lead = (b,) if top_paths == 1 else (b, top_paths)
-            labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
-            logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
             self.ctx.crnn_forward_lexicon(crnn_in.data_ptr(), b, offsets.data_ptr(), lex_labels.data_ptr(), len(lexicon),
-                                          int(top_paths), labels.data_ptr(), logp.data_ptr() if with_scores else None,
-                                          ws.data_ptr(), nbytes, stream)
+                                          int(top_paths), labels.data_ptr(), logp_ptr, ws.data_ptr(), nbytes, stream)
         elif beam_width is not None:
-            lead = (b,) if top_paths == 1 else (b, top_paths)
-            labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
-            logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
             self.ctx.crnn_forward_beam(crnn_in.data_ptr(), b, int(beam_width), int(top_paths), labels.data_ptr(),
-                                       logp.data_ptr() if with_scores else None, ws.data_ptr(), nbytes, stream)
-        elif with_scores:
-            logp = torch.empty((b,), dtype=torch.float32, device=self.device)
-            self.ctx.crnn_forward_scored(crnn_in.data_ptr(), b, labels.data_ptr(), logp.data_ptr(), ws.data_ptr(), nbytes,
+                                       logp_ptr, ws.data_ptr(), nbytes, stream)
+        elif logp is not None:
+            self.ctx.crnn_forward_scored(crnn_in.data_ptr(), b, labels.data_ptr(), logp_ptr, ws.data_ptr(), nbytes,
                                          stream)
         else:
             self.ctx.crnn_forward(crnn_in.data_ptr(), b, labels.data_ptr(), ws.data_ptr(), nbytes, stream)
         self._last_ws = (ws, b) if self.keep_workspace else None
-        return (labels, logp) if with_scores else labels
 
     def tap(self, name, shape, dtype):
         """Debug: copy an intermediate of the last predict_device call (needs keep_workspace=True)."""
@@ -344,20 +376,29 @@ class Recognizer:
                                     beam_width=beam_width, top_paths=top_paths, lexicon=lexicon)[0]
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
-                                    with_scores=False, beam_width=None, top_paths=1, lexicon=None):
+                                    with_scores=False, beam_width=None, top_paths=1, lexicon=None, rotations=None,
+                                    rotation_vote="word"):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
         (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon``: see
         ``predict_device``).
+
+        ``rotations`` / ``rotation_vote`` (``check_rotations``): every box is cut and decoded once per listed turn, one
+        turn after another (the CRNN workspace stays that of B crops), and ``b2o_select_rotation`` keeps one reading per
+        word.  The result then ends with the chosen turns (B,) int32 CUDA: (labels, turns) or (labels, logp, turns), in
+        the shapes of the call without rotations.  ``boxes`` and ``flat`` are rolled in place to start at the chosen
+        turn's corner: box[0] is the text's own top-left corner.
 
         Optional device-side by-products of the earlier stages, so that nothing but the kernel launches is
         left to do once the host knows the counts: ``gray`` (N,H,W) u8 from ``b2o_resize_pad_batch``;
         ``flat`` (>=B,4,2) / ``image_index`` (>=B,) from ``b2o_compact_boxes``."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
+        turns = check_rotations(rotations, rotation_vote)
         counts = np.asarray(counts)
         m = boxes.shape[1]
         total = int(np.minimum(counts, m).sum())
         if total == 0:
-            return (None, None) if with_scores else None
+            parts = 1 + bool(with_scores) + (turns is not None)
+            return None if parts == 1 else (None,) * parts
         if self.color:
             gray = images_t                                       # color recognizer: crops come straight from the RGB batch
         elif gray is None:
@@ -369,17 +410,43 @@ class Recognizer:
             counts_dev = torch.from_numpy(counts.astype(np.int32)).to(self.device)
             self.ctx.compact_boxes(boxes.data_ptr(), counts_dev.data_ptr(), n, m, flat.data_ptr(),
                                    image_index.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
+        if turns is not None:
+            return self._recognize_turns(gray, flat[:total], image_index[:total], len(counts), boxes, turns,
+                                         rotation_vote, with_scores, beam_width, top_paths, lexicon)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
         return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
                                    lexicon=lexicon)
 
+    def _recognize_turns(self, gray, flat, image_index, n_images, table, turns, vote, with_scores, beam_width,
+                         top_paths, lexicon):
+        """Warp + CRNN + decoder for each turn into its slot of one (R,B,P,48) / (R,B,P) stack, then
+        ``b2o_select_rotation``, which also rolls ``flat`` and ``table`` (None: no table) in place."""
+        b, p, r = flat.shape[0], int(top_paths), len(turns)
+        labels_all = torch.empty((r, b, p, STEPS), dtype=torch.int32, device=self.device)
+        logp_all = torch.empty((r, b, p), dtype=torch.float32, device=self.device)
+        for j, turn in enumerate(turns):
+            crnn_in, _ = self.warp_device(gray, flat, image_index, turn=turn)
+            self._forward(crnn_in, labels_all[j], logp_all[j], beam_width, p, lexicon)
+        labels = torch.empty((b, p, STEPS), dtype=torch.int32, device=self.device)
+        logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
+        chosen = torch.empty((b,), dtype=torch.int32, device=self.device)
+        self.ctx.select_rotation(labels_all.data_ptr(), logp_all.data_ptr(), image_index.data_ptr(), n_images, b, p,
+                                 turns, ROTATION_VOTES[vote], labels.data_ptr(), logp.data_ptr(), chosen.data_ptr(),
+                                 flat.data_ptr(), None if table is None else table.data_ptr(),
+                                 0 if table is None else table.shape[1], torch.cuda.current_stream(self.device).cuda_stream)
+        if p == 1:
+            labels, logp = labels.view(b, STEPS), logp.view(b)
+        return (labels, logp, chosen) if with_scores else (labels, chosen)
+
     # ------------------------------------------------------------------ reference API
     def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                             **kwargs) -> typing.List[typing.List[str]]:
+                             rotations=None, rotation_vote="word", **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
         (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon``: as
-        ``recognize_crops``."""
+        ``recognize_crops``.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
+        most probable reading kept, per word or per image (one box group), see ``check_rotations``."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
+        turns = check_rotations(rotations, rotation_vote)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
 
@@ -394,12 +461,19 @@ class Recognizer:
         flat = tools.rectify_boxes(flat)
         flat_t = torch.from_numpy(np.ascontiguousarray(flat)).to(self.device)
         idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
-        crnn_in, _ = self.warp_device(images_t if self.color else self.gray_device(images_t), flat_t, idx)
+        gray = images_t if self.color else self.gray_device(images_t)
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
-        if return_scores:
+        if turns is not None:
+            labels, logp, _ = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns, rotation_vote, True,
+                                                    **beam)
+            texts, conf = decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())
+            predictions = list(zip(texts, conf)) if return_scores else texts
+        elif return_scores:
+            crnn_in, _ = self.warp_device(gray, flat_t, idx)
             labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
             predictions = list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
         else:
+            crnn_in, _ = self.warp_device(gray, flat_t, idx)
             predictions = decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
         ends = np.cumsum(counts)
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]

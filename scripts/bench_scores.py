@@ -1,11 +1,17 @@
-"""bench_scores.py -- what detection scores, word confidences, beam-search and lexicon decoding cost:
-``Pipeline.recognize`` with and without ``return_scores=True``, with ``recognition_kwargs={"beam_width": W}`` for every
-W given and with ``recognition_kwargs={"lexicon": L}`` for every lexicon size N given, on the workload of bench.py
-(32 pages 768x768, scale 2 -> 1536x1536, sources resident in HBM).  A size-N lexicon is the bench pages' rendered words
-plus seeded distractors (``oracle.synth.random_word``) up to N entries.
+"""bench_scores.py -- what detection scores, word confidences, beam-search, lexicon decoding and quarter-turn reading
+cost: ``Pipeline.recognize`` with and without ``return_scores=True``, with ``recognition_kwargs={"beam_width": W}`` for
+every W given, with ``recognition_kwargs={"lexicon": L}`` for every lexicon size N given and with
+``recognition_kwargs={"rotations": T, "rotation_vote": V}`` for every turn list T and vote V given, on the workload of
+bench.py (32 pages 768x768, scale 2 -> 1536x1536, sources resident in HBM).  A size-N lexicon is the bench pages'
+rendered words plus seeded distractors (``oracle.synth.random_word``) up to N entries.
 
     python scripts/bench_scores.py [--steps K] [--warmup W] [--rounds R] [--beam-width W [W ...]]
                                    [--lexicon-size N [N ...]] [--decoder-lexicon-size N [N ...]] [--decoder-calls C]
+                                   [--rotations 02 0123 ...] [--rotation-vote word page] [--rotation-beam-width W ...]
+
+``--rotations``: turn lists as digit strings (``02`` = (0, 2)), each timed with every ``--rotation-vote`` (default
+page), greedy and with every ``--rotation-beam-width``.  Besides the words read on the upright pages, the line then reports ``words_read`` of the default call and of
+every rotation leg on the pages turned by np.rot90(page, k), k = 1, 2, 3 (outside the timed region).
 
 ``--decoder-lexicon-size``: the lexicon decoder alone (``b2o_ctc_lexicon_decode``, top_paths 1) on the fc_12 logits
 of one bench step's crops, C launches between CUDA events after a warm-up, in ms per call.
@@ -37,6 +43,15 @@ def card_info(device_index):
         return {"gpu": None, "power_limit_w": None}
 
 
+def rot90_rect(rect, k, h, w):
+    """(x0, y0, x1, y1) of an (h, w) page on np.rot90(page, k): (x, y) -> (y, w - 1 - x), applied k times."""
+    x0, y0, x1, y1 = rect
+    for _ in range(k):
+        x0, y0, x1, y1 = y0, w - 1 - x1, y1, w - 1 - x0
+        h, w = w, h
+    return x0, y0, x1, y1
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
@@ -46,6 +61,10 @@ def main():
     ap.add_argument("--lexicon-size", type=int, nargs="+", default=[])
     ap.add_argument("--decoder-lexicon-size", type=int, nargs="+", default=[])
     ap.add_argument("--decoder-calls", type=int, default=20)
+    ap.add_argument("--rotations", nargs="+", default=[], help="turn lists as digit strings, e.g. 02 0123")
+    ap.add_argument("--rotation-vote", nargs="+", default=["page"], choices=["word", "page"])
+    ap.add_argument("--rotation-beam-width", type=int, nargs="+", default=[],
+                    help="also time every rotation leg with beam search of these widths")
     args = ap.parse_args()
 
     import numpy as np
@@ -82,6 +101,14 @@ def main():
     lexicons = {n: lexicon(n) for n in sorted(set(args.lexicon_size) | set(args.decoder_lexicon_size))}
     for n in args.lexicon_size:
         calls[f"lexicon{n}"] = lambda n=n: pipe.recognize(pages, recognition_kwargs={"lexicon": lexicons[n]})
+    rotation_kwargs = {}
+    for spec in args.rotations:
+        for vote in args.rotation_vote:
+            rotation_kwargs[f"rot{spec}_{vote}"] = {"rotations": tuple(int(c) for c in spec), "rotation_vote": vote}
+            for w in args.rotation_beam_width:
+                rotation_kwargs[f"rot{spec}_{vote}_beam{w}"] = dict(rotation_kwargs[f"rot{spec}_{vote}"], beam_width=w)
+    for name, kw in rotation_kwargs.items():
+        calls[name] = lambda kw=kw, imgs=pages: pipe.recognize(imgs, recognition_kwargs=kw)
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -121,6 +148,14 @@ def main():
             line[f"{k}_overhead"] = statistics.median(ms[k]) / statistics.median(ms["default"]) - 1.0
             line[f"{k}_words_differing_from_default"] = sum(a != b for a, b in zip([t for g in result for t, _ in g],
                                                                                   default_words))
+    if rotation_kwargs:                                  # accuracy on the pages turned by np.rot90(page, k), untimed
+        for k in (1, 2, 3):
+            turned = torch.from_numpy(np.ascontiguousarray(np.rot90(pages_host, k, axes=(1, 2)))).to(device)
+            rects = [[rot90_rect(r, k, bench.PAGE_H, bench.PAGE_W) for r in page] for page in page_rects]
+            legs = {"default": {}, **rotation_kwargs}
+            for name, kw in legs.items():
+                hit, rendered = bench.words_read(pipe.recognize(turned, recognition_kwargs=kw), page_words, rects)
+                line[f"{name}_words_read_rot90_k{k}"] = [hit, rendered]
     if args.decoder_lexicon_size:
         rec.keep_workspace = True
         n_crops = sum(len(g) for g in pipe.recognize(pages))
