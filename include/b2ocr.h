@@ -253,6 +253,47 @@ int b2o_crnn_forward_lexicon(b2o_ctx* ctx, const void* crnn_in_dev, int b, const
                              const int16_t* labels_dev, int n_words, int top_paths, int32_t* labels_out_dev,
                              float* logp_dev, void* ws_dev, size_t ws_bytes, void* stream);
 
+/* Character positions: where each character of a reading lies (DESIGN.md section 1).
+ * b2o_ctc_align: the best single CTC alignment of each reading over the 48 kept steps, on lp[t,c] = log(softmax(l_t)_c +
+ * 1e-7) (blank = k-1), by a Viterbi pass over the 2n + 1 states (blank, l_0, blank, ..., l_{n-1}, blank) of an n-label
+ * reading: a path starts in the first blank or l_0 and ends in l_{n-1} or the trailing blank, a doubled letter needs a
+ * blank between its copies.  Ties among the predecessors of a state go to staying, then to advancing by one, then to
+ * skipping a blank; the trailing blank ends the path only when it scores strictly more than l_{n-1}.
+ * Inputs: logits_dev (b, 48, k) float32 and labels_dev (b, top_paths, 48) int32, each reading's labels followed by -1
+ * (what the decoders write).  Outputs: spans_dev (b, top_paths, 48, 2) int32, (f_j, l_j) = the first and last step (0..47)
+ * at which character j's state is occupied, -1 past the last character; logp_dev (b, top_paths) float32 (NULL: not
+ * written), the alignment's log-probability.  A reading with no finite alignment (too many doubled letters, a label
+ * outside [0, k-2]) gets spans -1 and logp -inf; an empty reading gets its all-blank score.  A crop's result is a
+ * function of its logits and labels alone: bit-identical alone, in any batch and on every run.
+ * 2 <= k <= B2O_MAX_CLASSES, 1 <= top_paths <= B2O_MAX_ALIGN_PATHS, otherwise B2O_ERR_ARG.
+ *
+ * b2o_char_cells: the characters tile the word box along its reading direction.  The cut between characters j-1 and j
+ * is grid row r = (l_{j-1} + f_j) / 2 + 2 (2 discarded steps); with the STN's theta (b, 6) it is crop column
+ * x = 4u + 1.5, u = 0.5 (theta[4] gy + theta[5] + 1) 50, gy = -1 + 2r/49 (the STN's time coordinate on the grid's centre
+ * column); without (theta_dev NULL, build_model(stn=False)) u = r.  Cuts are clamped to [0, sw] -- sw x sh the crop's
+ * content, the float32 corners warpBox maps the box onto -- and made non-decreasing by a running max (a theta may flip
+ * time).  Cell j is (a,0), (b,0), (b,sh), (a,sh) between its cuts, mapped to detector-input pixels by the inverse
+ * homography of the word's warp in the turn it was read in (turns_dev (b) int32, NULL: turn 0; boxes_dev (b,4,2) the
+ * boxes as they were cut, before b2o_select_rotation rolls them) in fp64 with the projective divide, rounded once to
+ * float32.  The leading edge of the first cell and the trailing edge of the last are the rolled box's own corners, bit
+ * for bit; corner 0 of a cell is its top-left in reading order, clockwise.  boxes_dev NULL: cells in the 200 x 31 crop
+ * frame (outer edges x = 0 and 200, height 31).  cells_dev (b, top_paths, 48, 4, 2) float32, NaN past the last character,
+ * for readings without spans and for boxes whose warp plan is invalid.
+ *
+ * The product path: b2o_crnn_forward_logits is b2o_crnn_forward_scored that also keeps the fc_12 logits in the
+ * workspace's logits slot (logp_dev may be NULL), as b2o_crnn_forward_beam and _lexicon always do; b2o_crnn_align then
+ * aligns labels_dev on the logits of the preceding forward in ws_dev and copies its theta (b, 6) to theta_dev (NULL, or
+ * a recognizer without STN: not written).  Workspace sizes are those of the forward.                               */
+#define B2O_MAX_ALIGN_PATHS 128
+int b2o_ctc_align(b2o_ctx* ctx, const float* logits_dev, int b, int k, const int32_t* labels_dev, int top_paths,
+                  int32_t* spans_dev, float* logp_dev, void* stream);
+int b2o_char_cells(b2o_ctx* ctx, const int32_t* spans_dev, int b, int top_paths, const float* theta_dev,
+                   const float* boxes_dev, const int32_t* turns_dev, float* cells_dev, void* stream);
+int b2o_crnn_forward_logits(b2o_ctx* ctx, const void* crnn_in_dev, int b, int32_t* labels_dev, float* logp_dev,
+                            void* ws_dev, size_t ws_bytes, void* stream);
+int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths, int32_t* spans_dev, float* logp_dev,
+                   float* theta_dev, const void* ws_dev, size_t ws_bytes, void* stream);
+
 /* Result records of Pipeline.recognize for the multi-GPU gather (pipeline.py:66-75; SURVEY.md 8(e)): one
  * fixed-size float32 row per image = [count][rec_boxes x (4,2) boxes * inv_scale[i] (tools.adjust_boxes,
  * tools.py:232-260)][rec_boxes x 48 labels as int8, -1 padded], b2o_record_floats(rec_boxes) floats long.

@@ -19,6 +19,7 @@ MAX_LEXICON_WORDS = 1 << 20   # B2O_MAX_LEXICON_WORDS
 MAX_LEXICON_LABELS = 1 << 24  # B2O_MAX_LEXICON_LABELS
 MAX_LEXICON_TOP_PATHS = 128   # B2O_MAX_LEXICON_TOP_PATHS
 ROTATION_VOTE_WORD, ROTATION_VOTE_PAGE = 0, 1   # B2O_ROTATION_VOTE_WORD / _PAGE
+MAX_ALIGN_PATHS = 128         # B2O_MAX_ALIGN_PATHS
 
 
 class B2OError(RuntimeError):
@@ -87,6 +88,10 @@ SIGNATURES = {
     "b2o_lexicon_workspace_bytes": (_sz, [_i, _i, _i]),
     "b2o_ctc_lexicon_decode": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_crnn_forward_lexicon": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_ctc_align": (_i, [_vp, _vp, _i, _i, _vp, _i, _vp, _vp, _vp]),
+    "b2o_char_cells": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "b2o_crnn_forward_logits": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_crnn_align": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2o_set_debug_taps": (_i, [_vp, _i]),
     "b2o_crnn_tap": (_i, [_vp, _c.c_char_p, _vp, _i, _vp, _sz, _vp]),
     "b2o_conv2d_test": (_i, [_vp, _vp, _i, _i, _i, _i, _c.POINTER(_c.c_float), _i, _i, _i,
@@ -299,6 +304,22 @@ class Context:
                              stream):
         self._check(self.lib.b2o_crnn_forward_lexicon(self.handle, crnn_in, b, offsets, labels, n_words, top_paths,
                                                       labels_out, logp, ws, ws_bytes, stream), "b2o_crnn_forward_lexicon")
+
+    def ctc_align(self, logits, b, k, labels, top_paths, spans, logp, stream):
+        self._check(self.lib.b2o_ctc_align(self.handle, logits, b, k, labels, top_paths, spans, logp, stream),
+                    "b2o_ctc_align")
+
+    def char_cells(self, spans, b, top_paths, theta, boxes, turns, cells, stream):
+        self._check(self.lib.b2o_char_cells(self.handle, spans, b, top_paths, theta, boxes, turns, cells, stream),
+                    "b2o_char_cells")
+
+    def crnn_forward_logits(self, crnn_in, b, labels, logp, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_crnn_forward_logits(self.handle, crnn_in, b, labels, logp, ws, ws_bytes, stream),
+                    "b2o_crnn_forward_logits")
+
+    def crnn_align(self, b, labels, top_paths, spans, logp, theta, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_crnn_align(self.handle, b, labels, top_paths, spans, logp, theta, ws, ws_bytes, stream),
+                    "b2o_crnn_align")
 
     def set_debug_taps(self, on):
         self._check(self.lib.b2o_set_debug_taps(self.handle, int(on)), "b2o_set_debug_taps")

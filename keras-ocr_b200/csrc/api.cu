@@ -20,6 +20,8 @@ int ctc_beam_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width
 size_t ctc_lexicon_workspace_bytes(int B, int n_words);
 int ctc_lexicon_run(b2o_ctx* ctx, const float* logits, int B, int K, const int* offsets, const short* labels,
                     int n_words, int top_paths, int* labels_out, float* logp, void* ws, cudaStream_t st);
+int ctc_align_run(b2o_ctx* ctx, const float* logits, int B, int K, const int32_t* labels, int P, int32_t* spans,
+                  float* logp, cudaStream_t st);
 
 namespace {
 
@@ -792,6 +794,32 @@ extern "C" int b2o_crnn_forward_lexicon(b2o_ctx* ctx, const void* crnn_in, int b
   const float* logits = reinterpret_cast<const float*>(base + plan_crnn(b).off_logits);
   return ctc_lexicon_run(ctx, logits, b, ctx->n_classes, offsets, labels, n_words, top_paths, labels_out, logp,
                          base + scratch, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2o_crnn_forward_logits(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, float* logp, void* ws,
+                                       size_t ws_bytes, void* stream) {
+  return crnn_forward(ctx, crnn_in, b, labels, logp, true, ws, ws_bytes, stream);
+}
+
+extern "C" int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths, int32_t* spans_dev,
+                              float* logp_dev, float* theta_dev, const void* ws, size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_align: CRNN weights not loaded"); return B2O_ERR_STATE; }
+  if (top_paths < 1 || top_paths > B2O_MAX_ALIGN_PATHS || b < 0 || (b > 0 && (!labels_dev || !spans_dev || !ws))) {
+    ctx->set_error("b2o_crnn_align: bad argument");
+    return B2O_ERR_ARG;
+  }
+  if (b == 0) return B2O_OK;
+  const CrnnPlan p = plan_crnn(b);
+  if (ws_bytes < p.bytes) { ctx->set_error("b2o_crnn_align: workspace too small"); return B2O_ERR_WORKSPACE; }
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const uint8_t* base = reinterpret_cast<const uint8_t*>(ws);
+  if (theta_dev && ctx->crnn_stn)
+    B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(theta_dev, base + p.off_theta, static_cast<size_t>(b) * 6 * sizeof(float),
+                                        cudaMemcpyDeviceToDevice, st));
+  return ctc_align_run(ctx, reinterpret_cast<const float*>(base + p.off_logits), b, ctx->n_classes, labels_dev, top_paths,
+                       spans_dev, logp_dev, st);
 }
 
 extern "C" int b2o_set_debug_taps(b2o_ctx* ctx, int on) {

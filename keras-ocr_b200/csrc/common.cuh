@@ -157,7 +157,7 @@ int upsample_run(b2o_ctx* ctx, const TensorView& in, const TensorView& out, cuda
 int head_tail_run(b2o_ctx* ctx, const ConvLayer& L6, const ConvLayer& L8, const TensorView& in,
                   float* scores, cudaStream_t st);
 
-// ---- box corner order (image.cu's warp, rotation.cu's box roll) ---------------------------------
+// ---- box corner order (image.cu's warp, rotation.cu's box roll, ctc_align.cu's cells) ------------
 // fp64 Euclidean distance of two float32 points, as scipy's cdist computes it (tools.py:41-57)
 static __device__ inline double corner_dist(const float* a, const float* b) {
   const double dx = static_cast<double>(a[0]) - static_cast<double>(b[0]);
@@ -183,6 +183,103 @@ static __device__ inline void order_corners(const float* q, int ord[4]) {
   ord[3] = l1;                               // bl
   // (br, tr) = rightMost[argsort(D)[::-1]]
   if (d0 <= d1) { ord[2] = r1; ord[1] = r0; } else { ord[2] = r0; ord[1] = r1; }
+}
+
+// ---- warpBox geometry (image.cu's warp, ctc_align.cu's character cells) ------------------------------
+// turn r (0..3): warpBox(skip_rotate=True) of the ordered box rolled by r, np.roll(c, -r, axis=0) -- the crop starts at
+// corner c[r] and odd turns swap width and height.  Turn 0 is tools.warpBox itself.
+// warp_extent: the rolled box (get_rotated_box on a rectangle, then the roll), get_rotated_width_height and the scaled
+// content size sw x sh of the crop in fp64; the homography maps the box onto (0,0), (sw,0), (sw,sh), (0,sh) rounded to
+// float32.  False where the reference raises ZeroDivisionError (w or h is 0).
+static __device__ inline bool warp_extent(const float* q /*4x2*/, int turn, int target_w, int target_h, float box[8],
+                                          double* sw, double* sh) {
+  // --- get_rotated_box on a rectangle, then the roll -----------------------------------------------
+  int ord[4];
+  order_corners(q, ord);
+  for (int i = 0; i < 4; ++i) {
+    box[2 * i] = q[2 * ord[(i + turn) & 3]];
+    box[2 * i + 1] = q[2 * ord[(i + turn) & 3] + 1];
+  }
+  // --- get_rotated_width_height --------------------------------------------------------------------
+  const int w = static_cast<int>((corner_dist(box + 0, box + 2) + corner_dist(box + 4, box + 6)) / 2);
+  const int h = static_cast<int>((corner_dist(box + 0, box + 6) + corner_dist(box + 2, box + 4)) / 2);
+  if (w <= 0 || h <= 0) return false;        // the reference raises ZeroDivisionError here
+  const double sa = static_cast<double>(target_w) / w, sb = static_cast<double>(target_h) / h;
+  const double scale = sa < sb ? sa : sb;
+  *sw = scale * w;
+  *sh = scale * h;
+  return true;
+}
+
+// b2o_warp_plan (include/b2ocr.h): m[9] = inverse homography (destination -> source), fp64 like cv2; dw, dh = dsize
+// of warpPerspective; valid = 0 where warpBox raises ZeroDivisionError (or the system is singular).
+static __device__ inline void plan_warp(const float* q /*4x2*/, int turn, int target_w, int target_h, b2o_warp_plan* plan) {
+  plan->valid = 0;
+  float box[8];
+  double sw, sh;
+  if (!warp_extent(q, turn, target_w, target_h, box, &sw, &sh)) return;
+  const float dst[8] = {0.f, 0.f, static_cast<float>(sw), 0.f, static_cast<float>(sw), static_cast<float>(sh),
+                        0.f, static_cast<float>(sh)};
+  plan->dw = static_cast<int>(sw);
+  plan->dh = static_cast<int>(sh);
+  // --- cv2.getPerspectiveTransform: 8x8 system, LU with partial pivoting in fp64 -----------------
+  double A[8][8], b[8];
+  for (int i = 0; i < 4; ++i) {
+    const double sxx = box[2 * i], syy = box[2 * i + 1], dx = dst[2 * i], dy = dst[2 * i + 1];
+    for (int k = 0; k < 8; ++k) { A[i][k] = 0.0; A[i + 4][k] = 0.0; }
+    A[i][0] = A[i + 4][3] = sxx;
+    A[i][1] = A[i + 4][4] = syy;
+    A[i][2] = A[i + 4][5] = 1.0;
+    A[i][6] = __dmul_rn(-sxx, dx);
+    A[i][7] = __dmul_rn(-syy, dx);
+    A[i + 4][6] = __dmul_rn(-sxx, dy);
+    A[i + 4][7] = __dmul_rn(-syy, dy);
+    b[i] = dx;
+    b[i + 4] = dy;
+  }
+  for (int i = 0; i < 8; ++i) {
+    int k = i;
+    for (int j = i + 1; j < 8; ++j)
+      if (fabs(A[j][i]) > fabs(A[k][i])) k = j;
+    if (fabs(A[k][i]) < 2.220446049250313e-14) return;     // DBL_EPSILON*100: singular
+    if (k != i) {
+      for (int j = i; j < 8; ++j) { const double t = A[i][j]; A[i][j] = A[k][j]; A[k][j] = t; }
+      const double t = b[i]; b[i] = b[k]; b[k] = t;
+    }
+    const double d = -1.0 / A[i][i];
+    for (int j = i + 1; j < 8; ++j) {
+      const double alpha = __dmul_rn(A[j][i], d);
+      for (int kk = i + 1; kk < 8; ++kk) A[j][kk] = __dadd_rn(A[j][kk], __dmul_rn(alpha, A[i][kk]));
+      b[j] = __dadd_rn(b[j], __dmul_rn(alpha, b[i]));
+    }
+  }
+  for (int i = 7; i >= 0; --i) {
+    double s = b[i];
+    for (int kk = i + 1; kk < 8; ++kk) s = __dsub_rn(s, __dmul_rn(A[i][kk], b[kk]));
+    b[i] = s / A[i][i];
+  }
+  const double M[9] = {b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7], 1.0};
+  // --- cv::invert of a 3x3 (closed form) -----------------------------------------------------------
+#define MM(r, c) M[(r) * 3 + (c)]
+#define DET2(a, b, c, d) __dsub_rn(__dmul_rn(a, b), __dmul_rn(c, d))
+  const double det = __dadd_rn(
+      __dsub_rn(__dmul_rn(MM(0, 0), DET2(MM(1, 1), MM(2, 2), MM(1, 2), MM(2, 1))),
+                __dmul_rn(MM(0, 1), DET2(MM(1, 0), MM(2, 2), MM(1, 2), MM(2, 0)))),
+      __dmul_rn(MM(0, 2), DET2(MM(1, 0), MM(2, 1), MM(1, 1), MM(2, 0))));
+  if (det == 0.0) return;
+  const double id = 1.0 / det;
+  plan->m[0] = __dmul_rn(DET2(MM(1, 1), MM(2, 2), MM(1, 2), MM(2, 1)), id);
+  plan->m[1] = __dmul_rn(DET2(MM(0, 2), MM(2, 1), MM(0, 1), MM(2, 2)), id);
+  plan->m[2] = __dmul_rn(DET2(MM(0, 1), MM(1, 2), MM(0, 2), MM(1, 1)), id);
+  plan->m[3] = __dmul_rn(DET2(MM(1, 2), MM(2, 0), MM(1, 0), MM(2, 2)), id);
+  plan->m[4] = __dmul_rn(DET2(MM(0, 0), MM(2, 2), MM(0, 2), MM(2, 0)), id);
+  plan->m[5] = __dmul_rn(DET2(MM(0, 2), MM(1, 0), MM(0, 0), MM(1, 2)), id);
+  plan->m[6] = __dmul_rn(DET2(MM(1, 0), MM(2, 1), MM(1, 1), MM(2, 0)), id);
+  plan->m[7] = __dmul_rn(DET2(MM(0, 1), MM(2, 0), MM(0, 0), MM(2, 1)), id);
+  plan->m[8] = __dmul_rn(DET2(MM(0, 0), MM(1, 1), MM(0, 1), MM(1, 0)), id);
+#undef MM
+#undef DET2
+  plan->valid = 1;
 }
 
 static inline TensorView make_view(void* base, int n, int h, int w, int c, int ld = 0, int coff = 0) {

@@ -76,92 +76,8 @@ __global__ void gray_kernel(const uint8_t* __restrict__ img, long long total, ui
 }
 
 // ------------------------------------------------------------------------------------ warpBox
-// b2o_warp_plan (include/b2ocr.h): m[9] = inverse homography (destination -> source), fp64 like cv2; dw, dh = dsize
-// of warpPerspective; valid = 0 where warpBox raises ZeroDivisionError (or the system is singular).
+// plan_warp / warp_extent (common.cuh): the WarpPlan of a box in quarter turn r.
 using WarpPlan = b2o_warp_plan;
-
-// turn r (0..3): warpBox(skip_rotate=True) of the ordered box rolled by r, np.roll(c, -r, axis=0) -- the crop starts at
-// corner c[r] and odd turns swap width and height.  Turn 0 is tools.warpBox itself.
-__device__ void plan_warp(const float* q /*4x2*/, int turn, int target_w, int target_h, WarpPlan* plan) {
-  plan->valid = 0;
-  // --- get_rotated_box on a rectangle, then the roll -----------------------------------------------
-  int ord[4];
-  order_corners(q, ord);
-  float box[8];
-  for (int i = 0; i < 4; ++i) {
-    box[2 * i] = q[2 * ord[(i + turn) & 3]];
-    box[2 * i + 1] = q[2 * ord[(i + turn) & 3] + 1];
-  }
-  // --- get_rotated_width_height --------------------------------------------------------------------
-  const int w = static_cast<int>((corner_dist(box + 0, box + 2) + corner_dist(box + 4, box + 6)) / 2);
-  const int h = static_cast<int>((corner_dist(box + 0, box + 6) + corner_dist(box + 2, box + 4)) / 2);
-  if (w <= 0 || h <= 0) return;              // the reference raises ZeroDivisionError here
-  const double sa = static_cast<double>(target_w) / w, sb = static_cast<double>(target_h) / h;
-  const double scale = sa < sb ? sa : sb;
-  const double sw = scale * w, sh = scale * h;
-  const float dst[8] = {0.f, 0.f, static_cast<float>(sw), 0.f, static_cast<float>(sw), static_cast<float>(sh),
-                        0.f, static_cast<float>(sh)};
-  plan->dw = static_cast<int>(sw);
-  plan->dh = static_cast<int>(sh);
-  // --- cv2.getPerspectiveTransform: 8x8 system, LU with partial pivoting in fp64 -----------------
-  double A[8][8], b[8];
-  for (int i = 0; i < 4; ++i) {
-    const double sxx = box[2 * i], syy = box[2 * i + 1], dx = dst[2 * i], dy = dst[2 * i + 1];
-    for (int k = 0; k < 8; ++k) { A[i][k] = 0.0; A[i + 4][k] = 0.0; }
-    A[i][0] = A[i + 4][3] = sxx;
-    A[i][1] = A[i + 4][4] = syy;
-    A[i][2] = A[i + 4][5] = 1.0;
-    A[i][6] = __dmul_rn(-sxx, dx);
-    A[i][7] = __dmul_rn(-syy, dx);
-    A[i + 4][6] = __dmul_rn(-sxx, dy);
-    A[i + 4][7] = __dmul_rn(-syy, dy);
-    b[i] = dx;
-    b[i + 4] = dy;
-  }
-  for (int i = 0; i < 8; ++i) {
-    int k = i;
-    for (int j = i + 1; j < 8; ++j)
-      if (fabs(A[j][i]) > fabs(A[k][i])) k = j;
-    if (fabs(A[k][i]) < 2.220446049250313e-14) return;     // DBL_EPSILON*100: singular
-    if (k != i) {
-      for (int j = i; j < 8; ++j) { const double t = A[i][j]; A[i][j] = A[k][j]; A[k][j] = t; }
-      const double t = b[i]; b[i] = b[k]; b[k] = t;
-    }
-    const double d = -1.0 / A[i][i];
-    for (int j = i + 1; j < 8; ++j) {
-      const double alpha = __dmul_rn(A[j][i], d);
-      for (int kk = i + 1; kk < 8; ++kk) A[j][kk] = __dadd_rn(A[j][kk], __dmul_rn(alpha, A[i][kk]));
-      b[j] = __dadd_rn(b[j], __dmul_rn(alpha, b[i]));
-    }
-  }
-  for (int i = 7; i >= 0; --i) {
-    double s = b[i];
-    for (int kk = i + 1; kk < 8; ++kk) s = __dsub_rn(s, __dmul_rn(A[i][kk], b[kk]));
-    b[i] = s / A[i][i];
-  }
-  const double M[9] = {b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7], 1.0};
-  // --- cv::invert of a 3x3 (closed form) -----------------------------------------------------------
-#define MM(r, c) M[(r) * 3 + (c)]
-#define DET2(a, b, c, d) __dsub_rn(__dmul_rn(a, b), __dmul_rn(c, d))
-  const double det = __dadd_rn(
-      __dsub_rn(__dmul_rn(MM(0, 0), DET2(MM(1, 1), MM(2, 2), MM(1, 2), MM(2, 1))),
-                __dmul_rn(MM(0, 1), DET2(MM(1, 0), MM(2, 2), MM(1, 2), MM(2, 0)))),
-      __dmul_rn(MM(0, 2), DET2(MM(1, 0), MM(2, 1), MM(1, 1), MM(2, 0))));
-  if (det == 0.0) return;
-  const double id = 1.0 / det;
-  plan->m[0] = __dmul_rn(DET2(MM(1, 1), MM(2, 2), MM(1, 2), MM(2, 1)), id);
-  plan->m[1] = __dmul_rn(DET2(MM(0, 2), MM(2, 1), MM(0, 1), MM(2, 2)), id);
-  plan->m[2] = __dmul_rn(DET2(MM(0, 1), MM(1, 2), MM(0, 2), MM(1, 1)), id);
-  plan->m[3] = __dmul_rn(DET2(MM(1, 2), MM(2, 0), MM(1, 0), MM(2, 2)), id);
-  plan->m[4] = __dmul_rn(DET2(MM(0, 0), MM(2, 2), MM(0, 2), MM(2, 0)), id);
-  plan->m[5] = __dmul_rn(DET2(MM(0, 2), MM(1, 0), MM(0, 0), MM(1, 2)), id);
-  plan->m[6] = __dmul_rn(DET2(MM(1, 0), MM(2, 1), MM(1, 1), MM(2, 0)), id);
-  plan->m[7] = __dmul_rn(DET2(MM(0, 1), MM(2, 0), MM(0, 0), MM(2, 1)), id);
-  plan->m[8] = __dmul_rn(DET2(MM(0, 0), MM(1, 1), MM(0, 1), MM(1, 0)), id);
-#undef MM
-#undef DET2
-  plan->valid = 1;
-}
 
 constexpr int kCropH = 31, kCropW = 200;
 

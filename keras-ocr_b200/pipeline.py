@@ -135,14 +135,17 @@ class Pipeline:
         st[key] = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
         st[key].copy_(t, non_blocking=True)
 
-    def _stage_recognize(self, st, beam):
+    def _stage_recognize(self, st, beam, char_boxes=False):
         det, rec = self.detector, self.recognizer
         bst = st.pop("boxes_state")
         boxes, counts = det.boxes_finish(bst)
-        box_scores, logp = bst["box_scores"], None
+        box_scores, logp, cells = bst["box_scores"], None, None
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
                                                  image_index=bst["image_index"], with_scores=box_scores is not None,
-                                                 **beam)
+                                                 **beam, **({"char_boxes": True} if char_boxes else {}))
+        if char_boxes:                                   # (..., spans, cells): keep the cells
+            cells, labels = labels[-1], labels[:-2]
+            labels = labels if len(labels) > 1 else labels[0]
         if beam.get("rotations") is not None:            # drop the chosen turns: the rolled boxes carry them
             labels = labels[:-1] if box_scores is not None else labels[0]
         if box_scores is not None:
@@ -154,7 +157,11 @@ class Pipeline:
             self._to_host(st, "labels_host", labels)
         if logp is not None:
             self._to_host(st, "logp_host", logp)
-        st["keep"] = (boxes, labels, box_scores, logp)   # alive until the copies have run
+        if char_boxes:
+            st["char_boxes"] = True
+            if cells is not None:
+                self._to_host(st, "cells_host", cells)
+        st["keep"] = (boxes, labels, box_scores, logp, cells)   # alive until the copies have run
         st["done"] = torch.cuda.Event()
         st["done"].record(torch.cuda.current_stream(det.device))
 
@@ -175,6 +182,11 @@ class Pipeline:
         if scored:
             box_scores = st["box_scores_host"].numpy()
             d2h += box_scores.nbytes
+        cells = None
+        if "cells_host" in st:
+            cells_host = st["cells_host"].numpy()
+            d2h += cells_host.nbytes
+            cells = recognition.char_boxes_host(cells_host, texts)
         self.last_stats["d2h_bytes"] += int(d2h)
         out, start = [], 0
         for i, (c, scale) in enumerate(zip(counts, st["scales"])):
@@ -183,13 +195,19 @@ class Pipeline:
             if scale != 1:
                 group = tools.adjust_boxes(boxes=group, boxes_format="boxes", scale=1 / scale)
             if scored:
-                out.append(list(zip(texts[start:start + c], group, box_scores[i, :c], conf[start:start + c])))
+                words = list(zip(texts[start:start + c], group, box_scores[i, :c], conf[start:start + c]))
             else:
-                out.append(list(zip(texts[start:start + c], group)))
+                words = list(zip(texts[start:start + c], group))
+            if st.get("char_boxes") and c:               # the cells, scaled as the word boxes are
+                adjust = lambda q: tools.adjust_boxes(boxes=q, boxes_format="boxes", scale=1 / scale)  # noqa: E731
+                words = [w + ((adjust(q) if not isinstance(q, list) else [adjust(a) for a in q]),)
+                         for w, q in zip(words, cells[start:start + c])]
+            out.append(words)
             start += c
         return out
 
-    def recognize(self, images, detection_kwargs=None, recognition_kwargs=None, return_scores=False):
+    def recognize(self, images, detection_kwargs=None, recognition_kwargs=None, return_scores=False,
+                  return_char_boxes=False):
         """Run the pipeline on one or multiple images (reference pipeline.py:28-75).
 
         Returns a list (one entry per image) of lists of (text, box) tuples, boxes (4,2) float32 in
@@ -205,6 +223,10 @@ class Pipeline:
         reading, per word or per image; every returned box then starts at the chosen turn's corner, so box[0] is the
         text's own top-left corner (the same corners, still clockwise).  Injected recognizers get
         ``recognition_kwargs`` as they are.
+        ``return_char_boxes=True``: every word's tuple ends with its character cells, an (n,4,2) float32 array of quads
+        in the input image's pixels for a text of n characters (a list of P arrays with ``top_paths = P > 1``), cell
+        corner 0 the character's top-left in reading order, clockwise (``Recognizer.recognize_from_boxes_device``):
+        (text, box, cells), or (text, box, detection_score, confidence, cells) with ``return_scores``.
         """
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
@@ -228,6 +250,9 @@ class Pipeline:
             if return_scores:
                 raise NotImplementedError("return_scores=True needs this package's Detector and Recognizer; injected "
                                           "detectors / recognizers do not report scores")
+            if return_char_boxes:
+                raise NotImplementedError("return_char_boxes=True needs this package's Detector and Recognizer; "
+                                          "injected detectors / recognizers do not report character positions")
             return self._recognize_generic(images, detection_kwargs, recognition_kwargs)
         thresholds = {k: detection_kwargs[k] for k in ("detection_threshold", "text_threshold", "link_threshold",
                                                         "size_threshold") if k in detection_kwargs}
@@ -245,7 +270,7 @@ class Pipeline:
                 states.append(self._stage_detect(images[bounds[step]:bounds[step + 1]], pad_to, thresholds,
                                                  with_scores=return_scores))
             if 1 <= step <= k:
-                self._stage_recognize(states[step - 1], beam)
+                self._stage_recognize(states[step - 1], beam, char_boxes=return_char_boxes)
             if step >= 2:
                 out.extend(self._stage_finish(states[step - 2]))
                 states[step - 2] = None

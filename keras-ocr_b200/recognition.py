@@ -170,6 +170,15 @@ def decode_paths(labels, alphabet=DEFAULT_ALPHABET, logp=None):
     return texts, (None if logp is None else [list(row) for row in confidences(logp)])
 
 
+def char_boxes_host(cells, texts):
+    """Host cells (B,48,4,2) or (B,P,48,4,2) float32 (``b2o_char_cells``) -> one (n,4,2) float32 array per word, n =
+    len(text); with ``top_paths = P > 1`` (texts are lists of P strings) a list of P arrays per word."""
+    cells = np.asarray(cells)
+    if cells.ndim == 4:
+        return [cells[i, :len(t)] for i, t in enumerate(texts)]
+    return [[cells[i, j, :len(t)] for j, t in enumerate(row)] for i, row in enumerate(texts)]
+
+
 class Recognizer:
     """A text recognizer using the CRNN architecture, running as sm_90a CUDA kernels.
 
@@ -305,9 +314,11 @@ class Recognizer:
         self._forward(crnn_in, labels, logp, beam_width, top_paths, lexicon)
         return (labels, logp) if with_scores else labels
 
-    def _forward(self, crnn_in, labels, logp, beam_width, top_paths, lexicon):
+    def _forward(self, crnn_in, labels, logp, beam_width, top_paths, lexicon, spans=None, theta=None):
         """The CRNN and the decoder of ``predict_device`` into caller-allocated ``labels`` / ``logp`` (None: greedy
-        without scores, or scores not written); ``lexicon`` is already compiled."""
+        without scores, or scores not written); ``lexicon`` is already compiled.  ``spans`` (B,P,48,2) int32: also the
+        characters' emission spans of every reading (``b2o_crnn_align``) and, with an STN, its ``theta`` (B,6) float32;
+        the greedy forward then keeps its logits (``b2o_crnn_forward_logits``)."""
         b = crnn_in.shape[0]
         nbytes = self.ctx.crnn_workspace_bytes(b)
         if lexicon is not None:
@@ -325,12 +336,39 @@ class Recognizer:
         elif beam_width is not None:
             self.ctx.crnn_forward_beam(crnn_in.data_ptr(), b, int(beam_width), int(top_paths), labels.data_ptr(),
                                        logp_ptr, ws.data_ptr(), nbytes, stream)
+        elif spans is not None:
+            self.ctx.crnn_forward_logits(crnn_in.data_ptr(), b, labels.data_ptr(), logp_ptr, ws.data_ptr(), nbytes,
+                                         stream)
         elif logp is not None:
             self.ctx.crnn_forward_scored(crnn_in.data_ptr(), b, labels.data_ptr(), logp_ptr, ws.data_ptr(), nbytes,
                                          stream)
         else:
             self.ctx.crnn_forward(crnn_in.data_ptr(), b, labels.data_ptr(), ws.data_ptr(), nbytes, stream)
+        if spans is not None:
+            self.ctx.crnn_align(b, labels.data_ptr(), int(top_paths), spans.data_ptr(), None,
+                                theta.data_ptr() if theta is not None else None, ws.data_ptr(), nbytes, stream)
         self._last_ws = (ws, b) if self.keep_workspace else None
+
+    def _predict_aligned(self, crnn_in, beam_width, top_paths, lexicon):
+        """``predict_device(with_scores=True)`` plus every reading's spans: (labels (B,P,48), logp (B,P), spans
+        (B,P,48,2) int32, theta (B,6) float32 or None without an STN)."""
+        b, p = crnn_in.shape[0], int(top_paths)
+        labels = torch.empty((b, p, STEPS), dtype=torch.int32, device=self.device)
+        logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
+        spans = torch.empty((b, p, STEPS, 2), dtype=torch.int32, device=self.device)
+        theta = torch.empty((b, 6), dtype=torch.float32, device=self.device) if self.stn else None
+        self._forward(crnn_in, labels, logp, beam_width, p, lexicon, spans, theta)
+        return labels, logp, spans, theta
+
+    def char_cells_device(self, spans, theta, boxes=None, turns=None):
+        """``b2o_char_cells``: spans (B,P,48,2) int32, theta (B,6) or None, boxes (B,4,2) float32 as they were cut (None:
+        the 200 x 31 crop frame), turns (B,) int32 or None -> cells (B,P,48,4,2) float32 CUDA."""
+        b, p = spans.shape[:2]
+        cells = torch.empty((b, p, STEPS, 4, 2), dtype=torch.float32, device=self.device)
+        ptr = lambda t: t.data_ptr() if t is not None else None      # noqa: E731
+        self.ctx.char_cells(spans.data_ptr(), b, p, ptr(theta), ptr(boxes), ptr(turns), cells.data_ptr(),
+                            torch.cuda.current_stream(self.device).cuda_stream)
+        return cells
 
     def tap(self, name, shape, dtype):
         """Debug: copy an intermediate of the last predict_device call (needs keep_workspace=True)."""
@@ -340,12 +378,16 @@ class Recognizer:
                           torch.cuda.current_stream(self.device).cuda_stream)
         return out
 
-    def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1, lexicon=None):
+    def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
+                        return_char_boxes=False):
         """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str].
         ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``.  ``beam_width``: beam search
         decoding (``check_beam``); with ``top_paths = P > 1`` each text is a list of P strings and each confidence a
         list of P floats, best first (``decode_paths``).  ``lexicon``: the most probable entries of a word list instead
-        (``check_decoder``), in the same shapes; a confidence is exp(the entry's CTC log-probability), clipped to 1."""
+        (``check_decoder``), in the same shapes; a confidence is exp(the entry's CTC log-probability), clipped to 1.
+        ``return_char_boxes=True``: every word is a tuple that ends with its character cells (``b2o_char_cells``), an
+        (n,4,2) float32 array for a text of n characters (a list of P arrays with ``top_paths = P > 1``), in the crop's
+        200 x 31 frame: (text, cells) or (text, confidence, cells)."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
         t = crops if isinstance(crops, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(crops))
         t = t.to(self.device).contiguous()
@@ -357,10 +399,21 @@ class Recognizer:
         self.ctx.crops_to_input(t.data_ptr(), b, crnn_in.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream,
                                 color=self.color)
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
+        if return_char_boxes:
+            labels, logp, spans, theta = self._predict_aligned(crnn_in, **beam)
+            return self._with_cells(labels, logp, self.char_cells_device(spans, theta), top_paths, return_scores)
         if not return_scores:
             return decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
         labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
         return list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
+
+    def _with_cells(self, labels, logp, cells, top_paths, return_scores):
+        """Host words of ``recognize_crops`` / ``recognize_from_boxes`` with cells: (text[, confidence], cells)."""
+        if top_paths == 1:
+            labels, logp, cells = labels[:, 0], logp[:, 0], cells[:, 0]
+        texts, conf = decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())
+        boxes = char_boxes_host(cells.cpu().numpy(), texts)
+        return list(zip(texts, conf, boxes)) if return_scores else list(zip(texts, boxes))
 
     def recognize(self, image, beam_width=None, top_paths=1, lexicon=None):
         """Recognize text from a single pre-cropped image (reference recognition.py:467-489): fit to
@@ -377,7 +430,7 @@ class Recognizer:
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
                                     with_scores=False, beam_width=None, top_paths=1, lexicon=None, rotations=None,
-                                    rotation_vote="word"):
+                                    rotation_vote="word", char_boxes=False):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
         (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon``: see
         ``predict_device``).
@@ -388,6 +441,11 @@ class Recognizer:
         the shapes of the call without rotations.  ``boxes`` and ``flat`` are rolled in place to start at the chosen
         turn's corner: box[0] is the text's own top-left corner.
 
+        ``char_boxes=True``: the result also ends with every reading's characters, spans (B,48,2) int32 -- each
+        character's first and last emitting step (``b2o_ctc_align``), -1 past the last -- and cells (B,48,4,2) float32,
+        its quad in detector-input pixels (``b2o_char_cells``), NaN past the last character; (B,P,48,2) / (B,P,48,4,2)
+        with ``top_paths = P > 1``.
+
         Optional device-side by-products of the earlier stages, so that nothing but the kernel launches is
         left to do once the host knows the counts: ``gray`` (N,H,W) u8 from ``b2o_resize_pad_batch``;
         ``flat`` (>=B,4,2) / ``image_index`` (>=B,) from ``b2o_compact_boxes``."""
@@ -397,7 +455,7 @@ class Recognizer:
         m = boxes.shape[1]
         total = int(np.minimum(counts, m).sum())
         if total == 0:
-            parts = 1 + bool(with_scores) + (turns is not None)
+            parts = 1 + bool(with_scores) + (turns is not None) + 2 * bool(char_boxes)
             return None if parts == 1 else (None,) * parts
         if self.color:
             gray = images_t                                       # color recognizer: crops come straight from the RGB batch
@@ -412,21 +470,42 @@ class Recognizer:
                                    image_index.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
         if turns is not None:
             return self._recognize_turns(gray, flat[:total], image_index[:total], len(counts), boxes, turns,
-                                         rotation_vote, with_scores, beam_width, top_paths, lexicon)
+                                         rotation_vote, with_scores, beam_width, top_paths, lexicon, char_boxes)
+        if char_boxes:
+            labels, logp, spans, cells = self._read_cells(gray, flat[:total], image_index[:total], beam_width,
+                                                          top_paths, lexicon)
+            return (labels, logp, spans, cells) if with_scores else (labels, spans, cells)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
         return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
                                    lexicon=lexicon)
 
+    def _read_cells(self, gray, flat, image_index, beam_width, top_paths, lexicon):
+        """Warp + CRNN + decoder + alignment + cells of one pass: (labels, logp, spans, cells) in the shapes of
+        ``recognize_from_boxes_device``."""
+        crnn_in, _ = self.warp_device(gray, flat, image_index)
+        labels, logp, spans, theta = self._predict_aligned(crnn_in, beam_width, top_paths, lexicon)
+        cells = self.char_cells_device(spans, theta, flat)
+        if top_paths == 1:
+            labels, logp, spans, cells = labels[:, 0], logp[:, 0], spans[:, 0], cells[:, 0]
+        return labels, logp, spans, cells
+
     def _recognize_turns(self, gray, flat, image_index, n_images, table, turns, vote, with_scores, beam_width,
-                         top_paths, lexicon):
+                         top_paths, lexicon, char_boxes=False):
         """Warp + CRNN + decoder for each turn into its slot of one (R,B,P,48) / (R,B,P) stack, then
-        ``b2o_select_rotation``, which also rolls ``flat`` and ``table`` (None: no table) in place."""
+        ``b2o_select_rotation``, which also rolls ``flat`` and ``table`` (None: no table) in place.  ``char_boxes``: each
+        turn's spans and theta are stacked alike, and the chosen turn's cells are built from the boxes as they were cut."""
         b, p, r = flat.shape[0], int(top_paths), len(turns)
         labels_all = torch.empty((r, b, p, STEPS), dtype=torch.int32, device=self.device)
         logp_all = torch.empty((r, b, p), dtype=torch.float32, device=self.device)
+        spans_all = theta_all = cut = None
+        if char_boxes:
+            spans_all = torch.empty((r, b, p, STEPS, 2), dtype=torch.int32, device=self.device)
+            theta_all = torch.empty((r, b, 6), dtype=torch.float32, device=self.device) if self.stn else None
+            cut = flat.clone()                           # b2o_select_rotation rolls flat in place
         for j, turn in enumerate(turns):
             crnn_in, _ = self.warp_device(gray, flat, image_index, turn=turn)
-            self._forward(crnn_in, labels_all[j], logp_all[j], beam_width, p, lexicon)
+            self._forward(crnn_in, labels_all[j], logp_all[j], beam_width, p, lexicon,
+                          None if spans_all is None else spans_all[j], None if theta_all is None else theta_all[j])
         labels = torch.empty((b, p, STEPS), dtype=torch.int32, device=self.device)
         logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
         chosen = torch.empty((b,), dtype=torch.int32, device=self.device)
@@ -434,17 +513,29 @@ class Recognizer:
                                  turns, ROTATION_VOTES[vote], labels.data_ptr(), logp.data_ptr(), chosen.data_ptr(),
                                  flat.data_ptr(), None if table is None else table.data_ptr(),
                                  0 if table is None else table.shape[1], torch.cuda.current_stream(self.device).cuda_stream)
+        extra = ()
+        if char_boxes:
+            slot = torch.zeros(4, dtype=torch.int64, device=self.device)
+            slot[list(turns)] = torch.arange(r, device=self.device)
+            pick, rows = slot[chosen.long()], torch.arange(b, device=self.device)
+            spans = spans_all[pick, rows]
+            cells = self.char_cells_device(spans, None if theta_all is None else theta_all[pick, rows], cut, chosen)
+            extra = (spans[:, 0], cells[:, 0]) if p == 1 else (spans, cells)
         if p == 1:
             labels, logp = labels.view(b, STEPS), logp.view(b)
-        return (labels, logp, chosen) if with_scores else (labels, chosen)
+        return ((labels, logp, chosen) if with_scores else (labels, chosen)) + extra
 
     # ------------------------------------------------------------------ reference API
     def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                             rotations=None, rotation_vote="word", **kwargs) -> typing.List[typing.List[str]]:
+                             rotations=None, rotation_vote="word", return_char_boxes=False,
+                             **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
         (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon``: as
         ``recognize_crops``.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
-        most probable reading kept, per word or per image (one box group), see ``check_rotations``."""
+        most probable reading kept, per word or per image (one box group), see ``check_rotations``.
+        ``return_char_boxes=True``: every word is a tuple that ends with its character cells, an (n,4,2) float32 array
+        of quads in the image's pixels for a text of n characters (a list of P arrays with ``top_paths = P > 1``):
+        (text, cells) or (text, confidence, cells); see ``recognize_from_boxes_device``."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
         turns = check_rotations(rotations, rotation_vote)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
@@ -463,7 +554,16 @@ class Recognizer:
         idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
         gray = images_t if self.color else self.gray_device(images_t)
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
-        if turns is not None:
+        if return_char_boxes:
+            if turns is not None:
+                labels, logp, _, _, cells = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns,
+                                                                  rotation_vote, True, char_boxes=True, **beam)
+            else:
+                labels, logp, _, cells = self._read_cells(gray, flat_t, idx, **beam)
+            texts, conf = decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())
+            cells = char_boxes_host(cells.cpu().numpy(), texts)
+            predictions = list(zip(texts, conf, cells)) if return_scores else list(zip(texts, cells))
+        elif turns is not None:
             labels, logp, _ = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns, rotation_vote, True,
                                                     **beam)
             texts, conf = decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())

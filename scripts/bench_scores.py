@@ -13,6 +13,9 @@ rendered words plus seeded distractors (``oracle.synth.random_word``) up to N en
 page), greedy and with every ``--rotation-beam-width``.  Besides the words read on the upright pages, the line then reports ``words_read`` of the default call and of
 every rotation leg on the pages turned by np.rot90(page, k), k = 1, 2, 3 (outside the timed region).
 
+``--char-boxes``: also ``recognize(return_char_boxes=True)`` (leg ``char_boxes``) and every rotation leg with it
+(``<leg>_char_boxes``): the cost of locating every character (alignment, cells, and the greedy forward's logits).
+
 ``--decoder-lexicon-size``: the lexicon decoder alone (``b2o_ctc_lexicon_decode``, top_paths 1) on the fc_12 logits
 of one bench step's crops, C launches between CUDA events after a warm-up, in ms per call.
 
@@ -65,6 +68,7 @@ def main():
     ap.add_argument("--rotation-vote", nargs="+", default=["page"], choices=["word", "page"])
     ap.add_argument("--rotation-beam-width", type=int, nargs="+", default=[],
                     help="also time every rotation leg with beam search of these widths")
+    ap.add_argument("--char-boxes", action="store_true", help="also time return_char_boxes=True")
     args = ap.parse_args()
 
     import numpy as np
@@ -109,6 +113,13 @@ def main():
                 rotation_kwargs[f"rot{spec}_{vote}_beam{w}"] = dict(rotation_kwargs[f"rot{spec}_{vote}"], beam_width=w)
     for name, kw in rotation_kwargs.items():
         calls[name] = lambda kw=kw, imgs=pages: pipe.recognize(imgs, recognition_kwargs=kw)
+    with_cells = set()
+    if args.char_boxes:
+        calls["char_boxes"] = lambda: pipe.recognize(pages, return_char_boxes=True)
+        with_cells.add("char_boxes")
+        for name, kw in rotation_kwargs.items():
+            calls[f"{name}_char_boxes"] = lambda kw=kw: pipe.recognize(pages, recognition_kwargs=kw, return_char_boxes=True)
+            with_cells.add(f"{name}_char_boxes")
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -140,6 +151,8 @@ def main():
         if k == "scored":
             continue
         result = fn()
+        if k in with_cells:                              # (text, box, cells) -> (text, box)
+            result = [[w[:2] for w in g] for g in result]
         hit, rendered = bench.words_read(result, page_words, page_rects)
         line[f"{k}_words_read"] = [hit, rendered]
         if k != "default":
