@@ -108,6 +108,29 @@ size_t b2o_craft_workspace_bytes(int n, int h, int w);
 int b2o_craft_forward(b2o_ctx* ctx, const uint8_t* img_dev, int n, int h, int w, float* scores_dev,
                       void* ws_dev, size_t ws_bytes, void* stream);
 
+/* Test hooks into the CRAFT forward (not on the product path).  The forward is a chain of steps, 0 normalize16,
+ * 1 stem, 2 slice1.3, ..., 12 slice4.37, 13 maxpool3, 14 slice5.1, 15 slice5.2, 16 upconv1.0, 17 upconv1.3,
+ * 18 / 21 / 24 the decoder upsampling (or the low-resolution half of upconvN.conv.0 when it is commuted),
+ * 19 / 22 / 25 upconv2/3/4.conv.0, 20 / 23 / 26 upconv2/3/4.conv.3, 27 conv_cls.0, 28 conv_cls.2, 29 conv_cls.4 (with
+ * the fused tail when it runs), 30 the separate head tail; a step with nothing to launch on the selected path is empty.
+ * b2o_craft_forward_until runs steps 0..last_step (0 <= last_step <= B2O_CRAFT_LAST_STEP) and returns; b2o_craft_forward
+ * is b2o_craft_forward_until(B2O_CRAFT_LAST_STEP).
+ * b2o_craft_tap copies one workspace buffer of the most recent forward of this context (n, h, w and ws_dev as passed to
+ * it), NHWC fp16 in its full channel stride: "x16" (h,w,16), "a", "b" (h,w,64), "p1" (h/2,w/2,64), "c" (128),
+ * "cat4" (192 = [upsampled | s1]), "p2" (h/4,w/4,128), "d" (256), "cat3" (384), "e" (256), "p3" (h/8,w/8,256),
+ * "f" (512), "cat2" (768), "g" (512), "p4" (h/16,w/16,512), "hh" (512), "cat1" (1536 = [s5 | s4]), "mp" (512),
+ * "s5a" (1024), "u1a" (512), "u1b" (256), "u2a" (h/8: 256), "u2b" (128), "u3a" (h/4: 128), "u3b" (64),
+ * "u4a" (h/2: 64), "u4b" (32), "h1", "h2" (32), "h3" (16), "z2" (h/16: 256), "z3" (h/8: 128), "z4" (h/4: 64)
+ * (sizes floor-halved per level).  Buffers whose lifetimes do not overlap share memory, so a buffer is only readable
+ * while its lifetime includes the forward's last step: otherwise B2O_ERR_STATE, as for ws_dev, n, h, w other than those
+ * of the context's last successful forward.  Unknown name or out_bytes smaller than n * h_buf * w_buf * c_buf * 2:
+ * B2O_ERR_ARG.                                                                                                 */
+#define B2O_CRAFT_LAST_STEP 30
+int b2o_craft_forward_until(b2o_ctx* ctx, const uint8_t* img_dev, int n, int h, int w, float* scores_dev,
+                            void* ws_dev, size_t ws_bytes, int last_step, void* stream);
+int b2o_craft_tap(b2o_ctx* ctx, const char* name, const void* ws_dev, int n, int h, int w, void* out_dev,
+                  size_t out_bytes, void* stream);
+
 /* getBoxes (detection.py:207-287).  scores: (n,hs,ws,2) float32.  Writes, per image i,
  * counts[i] = number of boxes found (may exceed max_boxes: then only the first max_boxes are
  * stored and the caller retries with a larger buffer) and boxes[i][k][4][2] float32 in
@@ -317,7 +340,10 @@ int b2o_pack_records_scored(b2o_ctx* ctx, const float* boxes_dev, const int32_t*
  * fp32 fc_12 outputs ("logits") to its workspace; by default (0) the fused Dense + CTC kernel keeps them in
  * registers and only the labels reach memory.  b2o_crnn_tap copies an intermediate of the last forward pass.
  * b2o_crnn_tap names: "features" (b,50,7,512 f16), "theta" (b,6 f32), "warped" (b,50,7,512 f16),
- * "fc_9" (b,50,128 f16), "l1" (b,50,128 f16), "l2" (b,50,256 f16), "logits" (b,48,K f32).      */
+ * "fc_9" (b,50,128 f16), "l1" (b,50,128 f16), "l2" (b,50,256 f16), "logits" (b,48,K f32); the conv backbone
+ * "x1" (b,200,31,64 f16, conv_1), "x2" (128, conv_2), "x3" (256, conv_3), "p3" (b,100,15,256, its pool),
+ * "x4" (256, conv_4), "x5" (512, conv_5), "p5" (b,50,7,512, its pool), "x6" (512, conv_6).  "x3" and "x5" are only
+ * written by engines that do not fuse the pool into the convolution (SIMT, TC_GENERIC).                     */
 int b2o_set_debug_taps(b2o_ctx* ctx, int on);
 int b2o_crnn_tap(b2o_ctx* ctx, const char* name, const void* ws_dev, int b, void* out_dev,
                  size_t out_bytes, void* stream);

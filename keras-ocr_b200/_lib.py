@@ -20,6 +20,7 @@ MAX_LEXICON_LABELS = 1 << 24  # B2O_MAX_LEXICON_LABELS
 MAX_LEXICON_TOP_PATHS = 128   # B2O_MAX_LEXICON_TOP_PATHS
 ROTATION_VOTE_WORD, ROTATION_VOTE_PAGE = 0, 1   # B2O_ROTATION_VOTE_WORD / _PAGE
 MAX_ALIGN_PATHS = 128         # B2O_MAX_ALIGN_PATHS
+CRAFT_LAST_STEP = 30          # B2O_CRAFT_LAST_STEP
 
 
 class B2OError(RuntimeError):
@@ -65,6 +66,8 @@ SIGNATURES = {
     "b2o_rgb_to_gray": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "b2o_craft_workspace_bytes": (_sz, [_i, _i, _i]),
     "b2o_craft_forward": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "b2o_craft_forward_until": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _i, _vp]),
+    "b2o_craft_tap": (_i, [_vp, _c.c_char_p, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "b2o_boxes_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "b2o_get_boxes": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _i, _vp, _sz, _vp]),
     "b2o_get_boxes_scored": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp, _i, _vp, _sz, _vp]),
@@ -221,6 +224,16 @@ class Context:
 
     def craft_forward(self, img, n, h, w, scores, ws, ws_bytes, stream):
         self._check(self.lib.b2o_craft_forward(self.handle, img, n, h, w, scores, ws, ws_bytes, stream), "b2o_craft_forward")
+
+    def craft_forward_until(self, img, n, h, w, scores, ws, ws_bytes, last_step, stream):
+        self._check(self.lib.b2o_craft_forward_until(self.handle, img, n, h, w, scores, ws, ws_bytes, last_step, stream),
+                    "b2o_craft_forward_until")
+
+    def craft_tap(self, name, ws, n, h, w, out, out_bytes, stream):
+        """b2o_craft_tap: raises B2OError; its status (B2O_ERR_STATE = -5 for a buffer that is not live) is in the
+        message."""
+        self._check(self.lib.b2o_craft_tap(self.handle, name.encode(), ws, n, h, w, out, out_bytes, stream),
+                    "b2o_craft_tap")
 
     def boxes_workspace_bytes(self, n, hs, ws, max_boxes):
         return int(self.lib.b2o_boxes_workspace_bytes(n, hs, ws, max_boxes))

@@ -119,12 +119,16 @@ const CraftSpec kCraft[] = {
     {"conv_cls.8", 16, 2, 1, 1, nullptr, 0},
 };
 
+// One buffer of the plan: its name (b2o_craft_tap), placement, NHWC shape and lifetime in forward steps.
+struct CraftBuf { const char* name; size_t off, bytes; int h, w, c, first, last; };
+
 // Buffer plan of the CRAFT forward pass (all NHWC fp16 unless noted), carved from one workspace.
 struct CraftPlan {
   int n, h1, w1, h2, w2, h4, w4, h8, w8, h16, w16;
   size_t off_a, off_b, off_p1, off_c, off_cat4, off_p2, off_d, off_cat3, off_e, off_p3, off_f, off_cat2, off_g, off_p4,
       off_hh, off_cat1, off_mp, off_s5a, off_u1a, off_u1b, off_u2a, off_u2b, off_u3a, off_u3b, off_u4a, off_u4b, off_h1,
       off_h2, off_h3, off_x16, off_z2, off_z3, off_z4, bytes;
+  std::vector<CraftBuf> bufs;
 };
 
 // Liveness-based packing: every buffer lives from the launch that first writes it to the launch that last reads it
@@ -137,48 +141,48 @@ CraftPlan plan_craft(int n, int h, int w) {
   p.n = n; p.h1 = h; p.w1 = w;
   p.h2 = h / 2; p.w2 = w / 2; p.h4 = p.h2 / 2; p.w4 = p.w2 / 2;
   p.h8 = p.h4 / 2; p.w8 = p.w4 / 2; p.h16 = p.h8 / 2; p.w16 = p.w8 / 2;
-  struct Buf { size_t* off; size_t bytes; int first, last; };
+  struct Buf { const char* name; size_t* off; size_t bytes; int first, last, hh, ww, c; };
   std::vector<Buf> bufs;
-  auto take = [&](size_t* off, int hh, int ww, int c, int first, int last) {
-    bufs.push_back({off, (static_cast<size_t>(n) * hh * ww * c * 2 + 255) / 256 * 256, first, last});
+  auto take = [&](const char* name, size_t* off, int hh, int ww, int c, int first, int last) {
+    bufs.push_back({name, off, (static_cast<size_t>(n) * hh * ww * c * 2 + 255) / 256 * 256, first, last, hh, ww, c});
   };
   // step: 0 normalize16, 1 stem, 2 slice1.3, 3 slice1.7, 4 slice1.10, 5 slice2.14, 6 slice2.17, 7 slice3.20, 8 slice3.24,
   // 9 slice3.27, 10 slice4.30, 11 slice4.34, 12 slice4.37, 13 maxpool3, 14 slice5.1, 15 slice5.2, 16 upconv1.0,
   // 17 upconv1.3, 18 upsample, 19 upconv2.0, 20 upconv2.3, 21 upsample, 22 upconv3.0, 23 upconv3.3, 24 upsample,
   // 25 upconv4.0, 26 upconv4.3, 27 conv_cls.0, 28 conv_cls.2, 29 conv_cls.4 (+ fused tail), 30 head_tail
-  take(&p.off_x16, p.h1, p.w1, 16, 0, 1);          // normalised input, 3 -> 16 channels, for the tensor-core stem
-  take(&p.off_a, p.h1, p.w1, 64, 1, 2);
-  take(&p.off_b, p.h1, p.w1, 64, 2, 2);            // full-resolution conv output: only written when the pool is not fused
-  take(&p.off_p1, p.h2, p.w2, 64, 2, 3);
-  take(&p.off_c, p.h2, p.w2, 128, 3, 4);
-  take(&p.off_cat4, p.h2, p.w2, 192, 4, 25);       // [upsampled decoder | tap s1]: written at 4 and 24, read at 25
-  take(&p.off_p2, p.h4, p.w4, 128, 4, 5);
-  take(&p.off_d, p.h4, p.w4, 256, 5, 6);
-  take(&p.off_cat3, p.h4, p.w4, 384, 6, 22);
-  take(&p.off_e, p.h4, p.w4, 256, 7, 7);
-  take(&p.off_p3, p.h8, p.w8, 256, 7, 8);
-  take(&p.off_f, p.h8, p.w8, 512, 8, 9);
-  take(&p.off_cat2, p.h8, p.w8, 768, 9, 19);
-  take(&p.off_g, p.h8, p.w8, 512, 10, 10);
-  take(&p.off_p4, p.h16, p.w16, 512, 10, 11);
-  take(&p.off_hh, p.h16, p.w16, 512, 11, 12);
-  take(&p.off_cat1, p.h16, p.w16, 1536, 12, 16);
-  take(&p.off_mp, p.h16, p.w16, 512, 13, 14);
-  take(&p.off_s5a, p.h16, p.w16, 1024, 14, 15);
-  take(&p.off_u1a, p.h16, p.w16, 512, 16, 17);
-  take(&p.off_u1b, p.h16, p.w16, 256, 17, 18);
-  take(&p.off_u2a, p.h8, p.w8, 256, 19, 20);
-  take(&p.off_u2b, p.h8, p.w8, 128, 20, 21);
-  take(&p.off_u3a, p.h4, p.w4, 128, 22, 23);
-  take(&p.off_u3b, p.h4, p.w4, 64, 23, 24);
-  take(&p.off_u4a, p.h2, p.w2, 64, 25, 26);
-  take(&p.off_u4b, p.h2, p.w2, 32, 26, 27);
-  take(&p.off_h1, p.h2, p.w2, 32, 27, 28);
-  take(&p.off_h2, p.h2, p.w2, 32, 28, 29);
-  take(&p.off_h3, p.h2, p.w2, 16, 29, 30);
-  take(&p.off_z2, p.h16, p.w16, 256, 18, 19);      // low-resolution halves of upconv2/3/4.conv.0 (commuted upsampling)
-  take(&p.off_z3, p.h8, p.w8, 128, 21, 22);
-  take(&p.off_z4, p.h4, p.w4, 64, 24, 25);
+  take("x16", &p.off_x16, p.h1, p.w1, 16, 0, 1);          // normalised input, 3 -> 16 channels, for the tensor-core stem
+  take("a", &p.off_a, p.h1, p.w1, 64, 1, 2);
+  take("b", &p.off_b, p.h1, p.w1, 64, 2, 2);            // full-resolution conv output: only written when the pool is not fused
+  take("p1", &p.off_p1, p.h2, p.w2, 64, 2, 3);
+  take("c", &p.off_c, p.h2, p.w2, 128, 3, 4);
+  take("cat4", &p.off_cat4, p.h2, p.w2, 192, 4, 25);       // [upsampled decoder | tap s1]: written at 4 and 24, read at 25
+  take("p2", &p.off_p2, p.h4, p.w4, 128, 4, 5);
+  take("d", &p.off_d, p.h4, p.w4, 256, 5, 6);
+  take("cat3", &p.off_cat3, p.h4, p.w4, 384, 6, 22);
+  take("e", &p.off_e, p.h4, p.w4, 256, 7, 7);
+  take("p3", &p.off_p3, p.h8, p.w8, 256, 7, 8);
+  take("f", &p.off_f, p.h8, p.w8, 512, 8, 9);
+  take("cat2", &p.off_cat2, p.h8, p.w8, 768, 9, 19);
+  take("g", &p.off_g, p.h8, p.w8, 512, 10, 10);
+  take("p4", &p.off_p4, p.h16, p.w16, 512, 10, 11);
+  take("hh", &p.off_hh, p.h16, p.w16, 512, 11, 12);
+  take("cat1", &p.off_cat1, p.h16, p.w16, 1536, 12, 16);
+  take("mp", &p.off_mp, p.h16, p.w16, 512, 13, 14);
+  take("s5a", &p.off_s5a, p.h16, p.w16, 1024, 14, 15);
+  take("u1a", &p.off_u1a, p.h16, p.w16, 512, 16, 17);
+  take("u1b", &p.off_u1b, p.h16, p.w16, 256, 17, 18);
+  take("u2a", &p.off_u2a, p.h8, p.w8, 256, 19, 20);
+  take("u2b", &p.off_u2b, p.h8, p.w8, 128, 20, 21);
+  take("u3a", &p.off_u3a, p.h4, p.w4, 128, 22, 23);
+  take("u3b", &p.off_u3b, p.h4, p.w4, 64, 23, 24);
+  take("u4a", &p.off_u4a, p.h2, p.w2, 64, 25, 26);
+  take("u4b", &p.off_u4b, p.h2, p.w2, 32, 26, 27);
+  take("h1", &p.off_h1, p.h2, p.w2, 32, 27, 28);
+  take("h2", &p.off_h2, p.h2, p.w2, 32, 28, 29);
+  take("h3", &p.off_h3, p.h2, p.w2, 16, 29, 30);
+  take("z2", &p.off_z2, p.h16, p.w16, 256, 18, 19);      // low-resolution halves of upconv2/3/4.conv.0 (commuted upsampling)
+  take("z3", &p.off_z3, p.h8, p.w8, 128, 21, 22);
+  take("z4", &p.off_z4, p.h4, p.w4, 64, 24, 25);
   std::vector<int> order(bufs.size());
   for (size_t i = 0; i < order.size(); ++i) order[i] = static_cast<int>(i);
   std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return bufs[a].bytes > bufs[b].bytes; });
@@ -200,6 +204,7 @@ CraftPlan plan_craft(int n, int h, int w) {
     if (at + bufs[i].bytes > total) total = at + bufs[i].bytes;
   }
   p.bytes = total;
+  for (const Buf& b : bufs) p.bufs.push_back({b.name, *b.off, b.bytes, b.hh, b.ww, b.c, b.first, b.last});
   return p;
 }
 
@@ -502,14 +507,28 @@ extern "C" size_t b2o_craft_workspace_bytes(int n, int h, int w) {
   return plan_craft(n, h, w).bytes;
 }
 
-extern "C" int b2o_craft_forward(b2o_ctx* ctx, const uint8_t* img, int n, int h, int w, float* scores, void* ws,
-                                 size_t ws_bytes, void* stream) {
+extern "C" int b2o_craft_forward_until(b2o_ctx* ctx, const uint8_t* img, int n, int h, int w, float* scores, void* ws,
+                                       size_t ws_bytes, int last_step, void* stream) {
   if (!ctx) return B2O_ERR_ARG;
   if (!ctx->craft_loaded) { ctx->set_error("b2o_craft_forward: CRAFT weights not loaded"); return B2O_ERR_STATE; }
   DeviceGuard guard(ctx->device);
-  if (!img || !scores || !ws || n <= 0 || h < 32 || w < 32) { ctx->set_error("b2o_craft_forward: bad argument"); return B2O_ERR_ARG; }
+  if (!img || !scores || !ws || n <= 0 || h < 32 || w < 32 || last_step < 0 || last_step > B2O_CRAFT_LAST_STEP) {
+    ctx->set_error("b2o_craft_forward: bad argument");
+    return B2O_ERR_ARG;
+  }
   const CraftPlan p = plan_craft(n, h, w);
   if (ws_bytes < p.bytes) { ctx->set_error("b2o_craft_forward: workspace too small"); return B2O_ERR_WORKSPACE; }
+  ctx->craft_step = -1;
+  // the step numbers are those of plan_craft's lifetimes; after step last_step the forward stops (host side, between
+  // launches) and records the step for b2o_craft_tap
+  auto stop_after = [&](int step) {
+    if (step < last_step) return false;
+    ctx->craft_step = last_step;
+    ctx->craft_ws = ws; ctx->craft_n = n; ctx->craft_h = h; ctx->craft_w = w;
+    return true;
+  };
+#define B2O_STOP_AFTER(step) \
+  if (stop_after(step)) return B2O_OK
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   uint8_t* base = reinterpret_cast<uint8_t*>(ws);
   auto V = [&](size_t off, int hh, int ww, int c, int ld = 0, int coff = 0) { return make_view(base + off, n, hh, ww, c, ld, coff); };
@@ -537,56 +556,94 @@ extern "C" int b2o_craft_forward(b2o_ctx* ctx, const uint8_t* img, int n, int h,
 
   // encoder (detection.py:312-324); taps s1..s4 are written straight into the concat buffers
   if (ctx->conv_engine == B2O_CONV_SIMT || L("stem16").block_n == 0) {
+    B2O_STOP_AFTER(0);
     B2O_RETURN_IF(stem_rgb_run(ctx, L("basenet.slice1.0"), img, n, h, w, a, st));          // fp32 CUDA-core stem
   } else {
     const TensorView x16 = V(p.off_x16, p.h1, p.w1, 16);
     B2O_RETURN_IF(normalize16_run(ctx, img, n, h, w, x16.ptr, st));
+    B2O_STOP_AFTER(0);
     B2O_RETURN_IF(conv_run(ctx, L("stem16"), x16, a, 0, st));
   }
+  B2O_STOP_AFTER(1);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice1.3"), a, b, 0, st, &p1, 0));     // conv + fused 2x2 max pool
+  B2O_STOP_AFTER(2);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice1.7"), p1, c, 0, st));
+  B2O_STOP_AFTER(3);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice1.10"), c, s1, 0, st, &p2, 1));   // tap s1 (full) + pooled
+  B2O_STOP_AFTER(4);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice2.14"), p2, d, 0, st));
+  B2O_STOP_AFTER(5);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice2.17"), d, s2, 0, st));
+  B2O_STOP_AFTER(6);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice3.20"), s2, e, 0, st, &p3, 0));
+  B2O_STOP_AFTER(7);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice3.24"), p3, f, 0, st));
+  B2O_STOP_AFTER(8);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice3.27"), f, s3, 0, st));
+  B2O_STOP_AFTER(9);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice4.30"), s3, g, 0, st, &p4, 0));
+  B2O_STOP_AFTER(10);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice4.34"), p4, hh, 0, st));
+  B2O_STOP_AFTER(11);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice4.37"), hh, s4, 0, st));          // BN only, no ReLU (333)
+  B2O_STOP_AFTER(12);
   // slice5 (365-378)
   B2O_RETURN_IF(maxpool3s1_run(ctx, s4, mp, st));
+  B2O_STOP_AFTER(13);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice5.1"), mp, s5a, 0, st));
+  B2O_STOP_AFTER(14);
   B2O_RETURN_IF(conv_run(ctx, L("basenet.slice5.2"), s5a, s5, 0, st));
+  B2O_STOP_AFTER(15);
   // decoder (380-390)
   B2O_RETURN_IF(conv_run(ctx, L("upconv1.conv.0"), cat1, u1a, 0, st));
+  B2O_STOP_AFTER(16);
   B2O_RETURN_IF(conv_run(ctx, L("upconv1.conv.3"), u1a, u1b, 0, st));
+  B2O_STOP_AFTER(17);
   // UpsampleLike + Concatenate + 1x1 conv (380-390).  Opt-in (B2O_UPCONV_COMMUTE=1): where the skip tensor is exactly
   // twice the decoder tensor the upsampling is commuted behind the convolution -- the decoder half of the 1x1 conv runs
   // at LOW resolution and the full-resolution half adds its bilinear upsampling in the epilogue, so no upsampled tensor
   // is written or read back.  Correct (tests) but not the default: the explicit UpsampleLike is what the reference graph runs.
-  auto level = [&](const char* name, const TensorView& y, const TensorView& cat_y, const TensorView& cat, const TensorView& skip,
-                   size_t off_z, const TensorView& out) -> int {
+  // Each level is two steps: the upsampling (or, commuted, the low-resolution decoder half z), then the 1x1 conv.
+  auto commuted = [&](const std::string& base, const TensorView& y, const TensorView& skip) {
+    return ctx->conv_engine == B2O_CONV_AUTO && !ctx->no_commute && skip.h == 2 * y.h && skip.w == 2 * y.w &&
+           ctx->craft[base + ".y"].block_n != 0 && ctx->craft[base + ".s"].kch == 64 && ctx->craft[base + ".s"].block_n >= 64;
+  };
+  auto level_up = [&](const char* name, const TensorView& y, const TensorView& cat_y, const TensorView& skip, size_t off_z,
+                      const TensorView& out) -> int {
     const std::string base(name);
-    const bool commute = ctx->conv_engine == B2O_CONV_AUTO && !ctx->no_commute && skip.h == 2 * y.h && skip.w == 2 * y.w &&
-                         ctx->craft[base + ".y"].block_n != 0 && ctx->craft[base + ".s"].kch == 64 && ctx->craft[base + ".s"].block_n >= 64;
-    if (!commute) {
-      B2O_RETURN_IF(upsample_run(ctx, y, cat_y, st));
-      return conv_run(ctx, ctx->craft[base], cat, out, 0, st);
-    }
+    if (!commuted(base, y, skip)) return upsample_run(ctx, y, cat_y, st);
+    return conv_run(ctx, ctx->craft[base + ".y"], y, V(off_z, y.h, y.w, out.c), 0, st);
+  };
+  auto level_conv = [&](const char* name, const TensorView& y, const TensorView& cat, const TensorView& skip, size_t off_z,
+                        const TensorView& out) -> int {
+    const std::string base(name);
+    if (!commuted(base, y, skip)) return conv_run(ctx, ctx->craft[base], cat, out, 0, st);
     const TensorView z = V(off_z, y.h, y.w, out.c);
-    B2O_RETURN_IF(conv_run(ctx, ctx->craft[base + ".y"], y, z, 0, st));
     return conv_tc_run(ctx, ctx->craft[base + ".s"], skip, out, 0, st, nullptr, 1, nullptr, &z);
   };
-  B2O_RETURN_IF(level("upconv2.conv.0", u1b, cat2_y, cat2, s3, p.off_z2, u2a));
+  B2O_RETURN_IF(level_up("upconv2.conv.0", u1b, cat2_y, s3, p.off_z2, u2a));
+  B2O_STOP_AFTER(18);
+  B2O_RETURN_IF(level_conv("upconv2.conv.0", u1b, cat2, s3, p.off_z2, u2a));
+  B2O_STOP_AFTER(19);
   B2O_RETURN_IF(conv_run(ctx, L("upconv2.conv.3"), u2a, u2b, 0, st));
-  B2O_RETURN_IF(level("upconv3.conv.0", u2b, cat3_y, cat3, s2, p.off_z3, u3a));
+  B2O_STOP_AFTER(20);
+  B2O_RETURN_IF(level_up("upconv3.conv.0", u2b, cat3_y, s2, p.off_z3, u3a));
+  B2O_STOP_AFTER(21);
+  B2O_RETURN_IF(level_conv("upconv3.conv.0", u2b, cat3, s2, p.off_z3, u3a));
+  B2O_STOP_AFTER(22);
   B2O_RETURN_IF(conv_run(ctx, L("upconv3.conv.3"), u3a, u3b, 0, st));
-  B2O_RETURN_IF(level("upconv4.conv.0", u3b, cat4_y, cat4, s1, p.off_z4, u4a));
+  B2O_STOP_AFTER(23);
+  B2O_RETURN_IF(level_up("upconv4.conv.0", u3b, cat4_y, s1, p.off_z4, u4a));
+  B2O_STOP_AFTER(24);
+  B2O_RETURN_IF(level_conv("upconv4.conv.0", u3b, cat4, s1, p.off_z4, u4a));
+  B2O_STOP_AFTER(25);
   B2O_RETURN_IF(conv_run(ctx, L("upconv4.conv.3"), u4a, u4b, 0, st));
+  B2O_STOP_AFTER(26);
   // head (392-410)
   B2O_RETURN_IF(conv_run(ctx, L("conv_cls.0"), u4b, h1, 0, st));
+  B2O_STOP_AFTER(27);
   B2O_RETURN_IF(conv_run(ctx, L("conv_cls.2"), h1, h2, 0, st));
+  B2O_STOP_AFTER(28);
   if (ctx->conv_engine == B2O_CONV_AUTO && L("conv_cls.4").block_n == 16 && !ctx->no_fused_tail) {
     // conv_cls.6 + conv_cls.8 ride in conv_cls.4's epilogue (same arithmetic as head_tail_kernel, bit for bit):
     // one launch and the 16-channel map's round trip through HBM less
@@ -596,11 +653,47 @@ extern "C" int b2o_craft_forward(b2o_ctx* ctx, const uint8_t* img, int n, int h,
       tail.h_w6 = L6.h_w_simt.data(); tail.h_b6 = L6.h_t1.data(); tail.h_w8 = L8.h_w_simt.data(); tail.h_b8 = L8.h_t1.data();
     }
     B2O_RETURN_IF(conv_tc_run(ctx, L("conv_cls.4"), h2, h3, 0, st, nullptr, 1, &tail));
+    B2O_STOP_AFTER(29);
   } else {
     B2O_RETURN_IF(conv_run(ctx, L("conv_cls.4"), h2, h3, 0, st));
+    B2O_STOP_AFTER(29);
     B2O_RETURN_IF(head_tail_run(ctx, L("conv_cls.6"), L("conv_cls.8"), h3, scores, st));
   }
+  B2O_STOP_AFTER(30);
+#undef B2O_STOP_AFTER
   return B2O_OK;
+}
+
+extern "C" int b2o_craft_forward(b2o_ctx* ctx, const uint8_t* img, int n, int h, int w, float* scores, void* ws,
+                                 size_t ws_bytes, void* stream) {
+  return b2o_craft_forward_until(ctx, img, n, h, w, scores, ws, ws_bytes, B2O_CRAFT_LAST_STEP, stream);
+}
+
+extern "C" int b2o_craft_tap(b2o_ctx* ctx, const char* name, const void* ws, int n, int h, int w, void* out,
+                             size_t out_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!name || !ws || !out || n <= 0 || h < 32 || w < 32) { ctx->set_error("b2o_craft_tap: bad argument"); return B2O_ERR_ARG; }
+  // the plan's offsets are only those of the workspace the last forward wrote if the shape and workspace are its own
+  if (ctx->craft_step < 0 || ws != ctx->craft_ws || n != ctx->craft_n || h != ctx->craft_h || w != ctx->craft_w) {
+    ctx->set_error("b2o_craft_tap: ws, n, h, w are not those of the last successful forward of this context");
+    return B2O_ERR_STATE;
+  }
+  DeviceGuard guard(ctx->device);
+  const CraftPlan p = plan_craft(n, h, w);
+  for (const CraftBuf& b : p.bufs) {
+    if (std::string(name) != b.name) continue;
+    const size_t bytes = static_cast<size_t>(n) * b.h * b.w * b.c * 2;
+    if (out_bytes < bytes) { ctx->set_error("b2o_craft_tap: output too small"); return B2O_ERR_ARG; }
+    if (ctx->craft_step < b.first || ctx->craft_step > b.last) {
+      ctx->set_error(std::string("b2o_craft_tap: ") + name + " is not live after the last forward's step");
+      return B2O_ERR_STATE;
+    }
+    B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(out, reinterpret_cast<const uint8_t*>(ws) + b.off, bytes, cudaMemcpyDeviceToDevice,
+                                        reinterpret_cast<cudaStream_t>(stream)));
+    return B2O_OK;
+  }
+  ctx->set_error(std::string("b2o_craft_tap: unknown buffer ") + name);
+  return B2O_ERR_ARG;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -836,6 +929,14 @@ extern "C" int b2o_crnn_tap(b2o_ctx* ctx, const char* name, const void* ws, int 
   size_t off = 0, bytes = 0;
   const std::string s(name);
   if (s == "features") { off = p.off_x7; bytes = B * 50 * 7 * 512 * 2; }
+  else if (s == "x1") { off = p.off_x1; bytes = B * 200 * 31 * 64 * 2; }
+  else if (s == "x2") { off = p.off_x2; bytes = B * 200 * 31 * 128 * 2; }
+  else if (s == "x3") { off = p.off_x3; bytes = B * 200 * 31 * 256 * 2; }
+  else if (s == "p3") { off = p.off_p3; bytes = B * 100 * 15 * 256 * 2; }
+  else if (s == "x4") { off = p.off_x4; bytes = B * 100 * 15 * 256 * 2; }
+  else if (s == "x5") { off = p.off_x5; bytes = B * 100 * 15 * 512 * 2; }
+  else if (s == "p5") { off = p.off_p5; bytes = B * 50 * 7 * 512 * 2; }
+  else if (s == "x6") { off = p.off_x6; bytes = B * 50 * 7 * 512 * 2; }
   else if ((s == "theta" || s == "warped") && !ctx->crnn_stn) { ctx->set_error("b2o_crnn_tap: this recognizer has no spatial transformer"); return B2O_ERR_STATE; }
   else if (s == "theta") { off = p.off_theta; bytes = B * 6 * 4; }
   else if (s == "warped") { off = p.off_warp; bytes = B * 50 * 7 * 512 * 2; }

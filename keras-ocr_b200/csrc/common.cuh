@@ -116,6 +116,9 @@ struct b2o_ctx {
   std::vector<void*> owned;    // device allocations freed in b2o_destroy
   // optional per-launch timing of the tensor-core conv kernel (bench.py's roofline leg)
   bool debug_taps = false;     // b2o_set_debug_taps: the CRNN forward also writes its fp32 logits (tests only)
+  int craft_step = -1;         // last step of the most recent successful CRAFT forward (b2o_craft_tap), -1: none
+  const void* craft_ws = nullptr;   // ... and its workspace and input shape, which b2o_craft_tap must be given again
+  int craft_n = 0, craft_h = 0, craft_w = 0;
   bool profile = false;
   std::vector<cudaEvent_t> prof_events;   // (start, stop) pairs
   double prof_flop = 0.0;

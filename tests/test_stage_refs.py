@@ -118,3 +118,78 @@ def _nchw_pool(a):
 def test_ulp16():
     assert R.ulp16(1.0) == 2.0 ** -10 and R.ulp16(0.75) == 2.0 ** -11 and R.ulp16(0.0) == 2.0 ** -24
     assert R.ulp16(65504.0) == 32.0
+
+
+# ------------------------------------------------------------------------------------------------ CRAFT / CRNN stage tables
+def test_craft_stage_chain_is_the_oracle_forward():
+    """Chaining CRAFT_STEPS in fp64 (the graph tests/test_gpu_craft_stages.py checks stage by stage, BN folded from the
+    raw weights) reproduces oracle.craft.craft_forward, at a size where every decoder level takes the general
+    upsampling (33 x 47) and at a multiple of 32."""
+    from keras_ocr_b200 import weights as W
+    from oracle import craft
+    w = W.synthetic_craft_weights(3)
+    rng = np.random.default_rng(4)
+    for n, h, wd in [(2, 33, 47), (1, 32, 64)]:
+        img = rng.integers(0, 256, (n, h, wd, 3), dtype=np.uint8)
+        got = R.craft_chain(w, img)
+        x = torch.from_numpy(R.compute_input_f32(img)).permute(0, 3, 1, 2)
+        want = craft.craft_forward(w, x).numpy()
+        assert got.shape == want.shape == (n, h // 2, wd // 2, 2)
+        assert np.abs(got - want).max() <= 1e-4 * np.abs(want).max(), np.abs(got - want).max()
+
+
+def test_crnn_backbone_chain_is_the_oracle_features():
+    from keras_ocr_b200 import weights as W
+    from oracle import crnn
+    rng = np.random.default_rng(5)
+    for color in (False, True):
+        w = W.synthetic_crnn_weights(seed=2, color=color)
+        crops = rng.integers(0, 256, (2, 31, 200) + ((3,) if color else ()), dtype=np.uint8)
+        c = crops.astype(np.float64)[..., None] if not color else crops.astype(np.float64)
+        x = np.flip(np.transpose(c, (0, 2, 1, 3)), 2) / 255.0                     # crnn_in: (b, 200, 31, ch)
+        taps = {"in": x}
+        for layer, src, dst, pool in R.CRNN_STEPS:
+            taps[dst] = R.crnn_layer_ref(w, layer, taps[src], round_w=False)[0]
+            if pool:
+                taps[pool] = R.pool_ref(taps[dst], taps[dst])[0]
+        want = crnn.crnn_features(w, crops.astype(np.float32) / 255.0).permute(0, 2, 3, 1).numpy()
+        assert np.abs(taps["features"] - want).max() <= 1e-4 * np.abs(want).max()
+
+
+# decoder size pairs (n_out <- n_in) of the CRAFT sizes tests/test_gpu_craft_stages.py runs that are not exactly 2x, i.e.
+# the ones upsample_kernel (not upsample2x_kernel) computes, plus exact 2x pairs
+UPSAMPLE_PAIRS = [(25, 12), (23, 11), (11, 5), (5, 2), (9, 4), (18, 9), (16, 8), (36, 18), (1024, 512), (2, 1), (3, 1)]
+
+
+def _torch_weights(n_out, n_in):
+    """torch's float32 bilinear weights along one axis, read off F.interpolate of one-hot rows: [source, output]."""
+    eye = torch.eye(n_in, dtype=torch.float32).reshape(n_in, 1, n_in, 1)
+    return F.interpolate(eye, size=(n_out, 1), mode="bilinear", align_corners=False)[:, 0, :, 0].numpy()
+
+
+def test_upsample_coordinates_are_torch_float_coordinates():
+    for n_out, n_in in UPSAMPLE_PAIRS:
+        i0, i1, lam, hi = R.upsample_coords_f32(n_out, n_in)
+        mine = np.zeros((n_in, n_out), np.float32)
+        o = np.arange(n_out)
+        np.add.at(mine, (i0, o), hi)
+        np.add.at(mine, (i1, o), lam)
+        assert np.array_equal(mine, _torch_weights(n_out, n_in)), (n_out, n_in)
+        assert (i0 <= i1).all() and (i1 < n_in).all() and ((lam >= 0) & (lam < 1)).all()
+
+
+def test_upsample_reference_is_interpolate():
+    """upsample_ref with float32 coordinates is F.interpolate (fp64 coordinates) up to the coordinates' float32
+    rounding, and its bound covers the same blend done in float32 and rounded to fp16."""
+    rng = np.random.default_rng(6)
+    for n_out, n_in in [(25, 12), (11, 5), (16, 8)]:
+        x = R.f16(rng.standard_normal((2, n_in, n_in + 3, 8)))
+        val, bound = R.upsample_ref(x, np.arange(n_in), n_in, np.arange(n_out), n_out, 2 * n_in + 1)
+        want = R._nhwc(R.upsample_like(R._nchw(x), n_out, 2 * n_in + 1))
+        assert np.abs(val - want).max() <= 1e-5 * np.abs(x).max()
+        y32 = torch.from_numpy(x).float().permute(0, 3, 1, 2)
+        got = F.interpolate(y32, size=(n_out, 2 * n_in + 1), mode="bilinear", align_corners=False)
+        got = R.f16(got.permute(0, 2, 3, 1).double()).numpy()
+        assert (np.abs(got - val) <= bound).all()
+        part = R.upsample_ref(x[:, :3], np.array([0, 1, 2]), n_in, np.arange(n_out), n_out, 2 * n_in + 1)[0]
+        assert np.isnan(part[:, -1]).all() and np.array_equal(part[:, 0], val[:, 0])    # rows past the band: NaN
