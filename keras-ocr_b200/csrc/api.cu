@@ -119,117 +119,194 @@ const CraftSpec kCraft[] = {
     {"conv_cls.8", 16, 2, 1, 1, nullptr, 0},
 };
 
-// One buffer of the plan: its name (b2o_craft_tap), placement, NHWC shape and lifetime in forward steps.
-struct CraftBuf { const char* name; size_t off, bytes; int h, w, c, first, last; };
-
-// Buffer plan of the CRAFT forward pass (all NHWC fp16 unless noted), carved from one workspace.
-struct CraftPlan {
-  int n, h1, w1, h2, w2, h4, w4, h8, w8, h16, w16;
-  size_t off_a, off_b, off_p1, off_c, off_cat4, off_p2, off_d, off_cat3, off_e, off_p3, off_f, off_cat2, off_g, off_p4,
-      off_hh, off_cat1, off_mp, off_s5a, off_u1a, off_u1b, off_u2a, off_u2b, off_u3a, off_u3b, off_u4a, off_u4b, off_h1,
-      off_h2, off_h3, off_x16, off_z2, off_z3, off_z4, bytes;
-  std::vector<CraftBuf> bufs;
+// The CRAFT forward's buffers (NHWC fp16), named as b2o_craft_tap names them.  The packer's stable sort breaks ties
+// between equal sizes in this order, so reordering the table moves buffers in the workspace.
+namespace cb {
+enum Id : int8_t { x16, a, b, p1, c, cat4, p2, d, cat3, e, p3, f, cat2, g, p4, hh, cat1, mp, s5a, u1a, u1b, u2a, u2b, u3a,
+                   u3b, u4a, u4b, h1, h2, h3, z2, z3, z4, count, none = -1 };
+}
+struct CraftBufSpec { const char* name; int level, c; };      // level: resolution divisor (1, 2, 4, 8, 16)
+constexpr CraftBufSpec kCraftBufs[cb::count] = {
+    {"x16", 1, 16},                                          // normalised input, 3 -> 16 channels, for the tensor-core stem
+    {"a", 1, 64},     {"b", 1, 64},     {"p1", 2, 64},     {"c", 2, 128},     {"cat4", 2, 192},  {"p2", 4, 128},
+    {"d", 4, 256},    {"cat3", 4, 384}, {"e", 4, 256},     {"p3", 8, 256},    {"f", 8, 512},     {"cat2", 8, 768},
+    {"g", 8, 512},    {"p4", 16, 512},  {"hh", 16, 512},   {"cat1", 16, 1536}, {"mp", 16, 512},  {"s5a", 16, 1024},
+    {"u1a", 16, 512}, {"u1b", 16, 256}, {"u2a", 8, 256},   {"u2b", 8, 128},   {"u3a", 4, 128},   {"u3b", 4, 64},
+    {"u4a", 2, 64},   {"u4b", 2, 32},   {"h1", 2, 32},     {"h2", 2, 32},     {"h3", 2, 16},
+    {"z2", 16, 256},  {"z3", 8, 128},   {"z4", 4, 64},       // low-resolution halves of upconv2/3/4.conv.0 (commuted)
 };
 
-// Liveness-based packing: every buffer lives from the launch that first writes it to the launch that last reads it
-// (the forward pass is one stream-ordered chain of launches, see b2o_craft_forward: the step numbers below are its
-// launch order); buffers whose lifetimes do not overlap share memory.  Greedy by size: largest first, each at the
-// lowest offset that is free for its whole lifetime.  32 x 1536 x 1536: 21.8 GB instead of 41 GB with every buffer
-// live (the peak is the two full-resolution 64-channel maps around slice1.3), and 73 -> 39 GB at max_size 2048.
+// Channels [c0, c1) of a buffer; S(buf) is all of it.
+struct Slice { cb::Id buf = cb::none; int c0 = 0, c1 = 0; };
+constexpr Slice S(cb::Id buf, int c0 = 0, int c1 = -1) { return {buf, c0, c1 < 0 ? kCraftBufs[buf].c : c1}; }
+
+// level_up / level_conv: the two steps of a decoder level, UpsampleLike(y) into the concat's decoder half and
+// upconvN.conv.0 over the concat -- or, commuted, the decoder half z of that 1x1 conv at y's resolution and the skip half
+// at full resolution adding z's upsampling in its epilogue.
+enum class StepKind : int8_t { normalize, stem, conv, maxpool3, level_up, level_conv, tail };
+
+// One launch of the forward (or none, where the engine folds the step into another).  Every slice any engine or switch
+// setting may touch is listed: buffer lifetimes are derived from them.  A level step's y is src at level_up; at
+// level_conv only z and skip (read by the commuted path) stand for it -- y is not read there.
+struct CraftStep {
+  StepKind kind;
+  const char* layer;
+  Slice src, out, pool, z, skip;
+  int write_full = 1;         // a pooled conv stores its full-resolution output too (conv_run)
+};
+constexpr CraftStep kCraftSteps[] = {
+    // encoder (detection.py:312-324); taps s1..s4 are written straight into the concat buffers
+    {StepKind::normalize, nullptr, {}, S(cb::x16)},
+    {StepKind::stem, "basenet.slice1.0", S(cb::x16), S(cb::a)},
+    {StepKind::conv, "basenet.slice1.3", S(cb::a), S(cb::b), S(cb::p1), {}, {}, 0},
+    {StepKind::conv, "basenet.slice1.7", S(cb::p1), S(cb::c)},
+    {StepKind::conv, "basenet.slice1.10", S(cb::c), S(cb::cat4, 64, 192), S(cb::p2)},
+    {StepKind::conv, "basenet.slice2.14", S(cb::p2), S(cb::d)},
+    {StepKind::conv, "basenet.slice2.17", S(cb::d), S(cb::cat3, 128, 384)},
+    {StepKind::conv, "basenet.slice3.20", S(cb::cat3, 128, 384), S(cb::e), S(cb::p3), {}, {}, 0},
+    {StepKind::conv, "basenet.slice3.24", S(cb::p3), S(cb::f)},
+    {StepKind::conv, "basenet.slice3.27", S(cb::f), S(cb::cat2, 256, 768)},
+    {StepKind::conv, "basenet.slice4.30", S(cb::cat2, 256, 768), S(cb::g), S(cb::p4), {}, {}, 0},
+    {StepKind::conv, "basenet.slice4.34", S(cb::p4), S(cb::hh)},
+    {StepKind::conv, "basenet.slice4.37", S(cb::hh), S(cb::cat1, 1024, 1536)},      // BN only, no ReLU (333)
+    // slice5 (365-378)
+    {StepKind::maxpool3, nullptr, S(cb::cat1, 1024, 1536), S(cb::mp)},
+    {StepKind::conv, "basenet.slice5.1", S(cb::mp), S(cb::s5a)},
+    {StepKind::conv, "basenet.slice5.2", S(cb::s5a), S(cb::cat1, 0, 1024)},
+    // decoder (380-390)
+    {StepKind::conv, "upconv1.conv.0", S(cb::cat1), S(cb::u1a)},
+    {StepKind::conv, "upconv1.conv.3", S(cb::u1a), S(cb::u1b)},
+    {StepKind::level_up, "upconv2.conv.0", S(cb::u1b), S(cb::cat2, 0, 256), {}, S(cb::z2)},
+    {StepKind::level_conv, "upconv2.conv.0", S(cb::cat2), S(cb::u2a), {}, S(cb::z2), S(cb::cat2, 256, 768)},
+    {StepKind::conv, "upconv2.conv.3", S(cb::u2a), S(cb::u2b)},
+    {StepKind::level_up, "upconv3.conv.0", S(cb::u2b), S(cb::cat3, 0, 128), {}, S(cb::z3)},
+    {StepKind::level_conv, "upconv3.conv.0", S(cb::cat3), S(cb::u3a), {}, S(cb::z3), S(cb::cat3, 128, 384)},
+    {StepKind::conv, "upconv3.conv.3", S(cb::u3a), S(cb::u3b)},
+    {StepKind::level_up, "upconv4.conv.0", S(cb::u3b), S(cb::cat4, 0, 64), {}, S(cb::z4)},
+    {StepKind::level_conv, "upconv4.conv.0", S(cb::cat4), S(cb::u4a), {}, S(cb::z4), S(cb::cat4, 64, 192)},
+    {StepKind::conv, "upconv4.conv.3", S(cb::u4a), S(cb::u4b)},
+    // head (392-410)
+    {StepKind::conv, "conv_cls.0", S(cb::u4b), S(cb::h1)},
+    {StepKind::conv, "conv_cls.2", S(cb::h1), S(cb::h2)},
+    {StepKind::conv, "conv_cls.4", S(cb::h2), S(cb::h3)},          // the tail rides in its epilogue where tail_fused
+    {StepKind::tail, nullptr, S(cb::h3)},                           // conv_cls.6 + conv_cls.8
+};
+static_assert(sizeof(kCraftSteps) / sizeof(kCraftSteps[0]) == B2O_CRAFT_LAST_STEP + 1, "one row per forward step");
+static_assert(kCraftSteps[B2O_CRAFT_LAST_STEP].kind == StepKind::tail && kCraftSteps[B2O_CRAFT_LAST_STEP - 1].kind ==
+              StepKind::conv, "the forward ends with conv_cls.4 and its tail");
+
+// One buffer of the plan: placement, NHWC shape and lifetime in forward steps.
+struct CraftBuf { size_t off, bytes; int h, w, first, last; };
+
+// Buffer plan of the CRAFT forward pass, carved from one workspace.
+struct CraftPlan {
+  int n;
+  size_t bytes;
+  CraftBuf bufs[cb::count];
+  TensorView view(void* ws, const Slice& s) const {
+    if (s.buf == cb::none) return TensorView();
+    const CraftBuf& b = bufs[s.buf];
+    return make_view(reinterpret_cast<uint8_t*>(ws) + b.off, n, b.h, b.w, s.c1 - s.c0, kCraftBufs[s.buf].c, s.c0);
+  }
+};
+
+// Liveness-based packing: every buffer lives from the first step that touches it (the one that writes it) to the last
+// step that touches it (the forward pass is one stream-ordered chain of launches in kCraftSteps' order); buffers whose
+// lifetimes do not overlap share memory.  Greedy by size: largest first, each at the lowest offset that is free for its
+// whole lifetime.  32 x 1536 x 1536: 21.8 GB instead of 41 GB with every buffer live (the peak is the two
+// full-resolution 64-channel maps around slice1.3), and 73 -> 39 GB at max_size 2048.
 CraftPlan plan_craft(int n, int h, int w) {
   CraftPlan p;
-  p.n = n; p.h1 = h; p.w1 = w;
-  p.h2 = h / 2; p.w2 = w / 2; p.h4 = p.h2 / 2; p.w4 = p.w2 / 2;
-  p.h8 = p.h4 / 2; p.w8 = p.w4 / 2; p.h16 = p.h8 / 2; p.w16 = p.w8 / 2;
-  struct Buf { const char* name; size_t* off; size_t bytes; int first, last, hh, ww, c; };
-  std::vector<Buf> bufs;
-  auto take = [&](const char* name, size_t* off, int hh, int ww, int c, int first, int last) {
-    bufs.push_back({name, off, (static_cast<size_t>(n) * hh * ww * c * 2 + 255) / 256 * 256, first, last, hh, ww, c});
-  };
-  // step: 0 normalize16, 1 stem, 2 slice1.3, 3 slice1.7, 4 slice1.10, 5 slice2.14, 6 slice2.17, 7 slice3.20, 8 slice3.24,
-  // 9 slice3.27, 10 slice4.30, 11 slice4.34, 12 slice4.37, 13 maxpool3, 14 slice5.1, 15 slice5.2, 16 upconv1.0,
-  // 17 upconv1.3, 18 upsample, 19 upconv2.0, 20 upconv2.3, 21 upsample, 22 upconv3.0, 23 upconv3.3, 24 upsample,
-  // 25 upconv4.0, 26 upconv4.3, 27 conv_cls.0, 28 conv_cls.2, 29 conv_cls.4 (+ fused tail), 30 head_tail
-  take("x16", &p.off_x16, p.h1, p.w1, 16, 0, 1);          // normalised input, 3 -> 16 channels, for the tensor-core stem
-  take("a", &p.off_a, p.h1, p.w1, 64, 1, 2);
-  take("b", &p.off_b, p.h1, p.w1, 64, 2, 2);            // full-resolution conv output: only written when the pool is not fused
-  take("p1", &p.off_p1, p.h2, p.w2, 64, 2, 3);
-  take("c", &p.off_c, p.h2, p.w2, 128, 3, 4);
-  take("cat4", &p.off_cat4, p.h2, p.w2, 192, 4, 25);       // [upsampled decoder | tap s1]: written at 4 and 24, read at 25
-  take("p2", &p.off_p2, p.h4, p.w4, 128, 4, 5);
-  take("d", &p.off_d, p.h4, p.w4, 256, 5, 6);
-  take("cat3", &p.off_cat3, p.h4, p.w4, 384, 6, 22);
-  take("e", &p.off_e, p.h4, p.w4, 256, 7, 7);
-  take("p3", &p.off_p3, p.h8, p.w8, 256, 7, 8);
-  take("f", &p.off_f, p.h8, p.w8, 512, 8, 9);
-  take("cat2", &p.off_cat2, p.h8, p.w8, 768, 9, 19);
-  take("g", &p.off_g, p.h8, p.w8, 512, 10, 10);
-  take("p4", &p.off_p4, p.h16, p.w16, 512, 10, 11);
-  take("hh", &p.off_hh, p.h16, p.w16, 512, 11, 12);
-  take("cat1", &p.off_cat1, p.h16, p.w16, 1536, 12, 16);
-  take("mp", &p.off_mp, p.h16, p.w16, 512, 13, 14);
-  take("s5a", &p.off_s5a, p.h16, p.w16, 1024, 14, 15);
-  take("u1a", &p.off_u1a, p.h16, p.w16, 512, 16, 17);
-  take("u1b", &p.off_u1b, p.h16, p.w16, 256, 17, 18);
-  take("u2a", &p.off_u2a, p.h8, p.w8, 256, 19, 20);
-  take("u2b", &p.off_u2b, p.h8, p.w8, 128, 20, 21);
-  take("u3a", &p.off_u3a, p.h4, p.w4, 128, 22, 23);
-  take("u3b", &p.off_u3b, p.h4, p.w4, 64, 23, 24);
-  take("u4a", &p.off_u4a, p.h2, p.w2, 64, 25, 26);
-  take("u4b", &p.off_u4b, p.h2, p.w2, 32, 26, 27);
-  take("h1", &p.off_h1, p.h2, p.w2, 32, 27, 28);
-  take("h2", &p.off_h2, p.h2, p.w2, 32, 28, 29);
-  take("h3", &p.off_h3, p.h2, p.w2, 16, 29, 30);
-  take("z2", &p.off_z2, p.h16, p.w16, 256, 18, 19);      // low-resolution halves of upconv2/3/4.conv.0 (commuted upsampling)
-  take("z3", &p.off_z3, p.h8, p.w8, 128, 21, 22);
-  take("z4", &p.off_z4, p.h4, p.w4, 64, 24, 25);
-  std::vector<int> order(bufs.size());
-  for (size_t i = 0; i < order.size(); ++i) order[i] = static_cast<int>(i);
-  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return bufs[a].bytes > bufs[b].bytes; });
+  p.n = n;
+  for (int i = 0; i < cb::count; ++i) {
+    const CraftBufSpec& s = kCraftBufs[i];
+    const int hh = h / s.level, ww = w / s.level;
+    p.bufs[i] = {0, (static_cast<size_t>(n) * hh * ww * s.c * 2 + 255) / 256 * 256, hh, ww, B2O_CRAFT_LAST_STEP + 1, -1};
+  }
+  for (int k = 0; k <= B2O_CRAFT_LAST_STEP; ++k) {
+    const CraftStep& s = kCraftSteps[k];
+    for (const Slice* sl : {&s.src, &s.out, &s.pool, &s.z, &s.skip}) {
+      if (sl->buf == cb::none) continue;
+      CraftBuf& b = p.bufs[sl->buf];
+      b.first = std::min(b.first, k);
+      b.last = std::max(b.last, k);
+    }
+  }
+  int order[cb::count];
+  for (int i = 0; i < cb::count; ++i) order[i] = i;
+  std::stable_sort(order, order + cb::count, [&](int a, int b) { return p.bufs[a].bytes > p.bufs[b].bytes; });
   std::vector<int> placed;
   size_t total = 0;
   for (int i : order) {
+    CraftBuf& bi = p.bufs[i];
     // candidate offsets: 0 and the end of every placed buffer that is live at the same time
     std::vector<std::pair<size_t, size_t>> busy;      // [begin, end) of time-overlapping placed buffers
-    for (int j : placed)
-      if (bufs[j].first <= bufs[i].last && bufs[i].first <= bufs[j].last) busy.push_back({*bufs[j].off, *bufs[j].off + bufs[j].bytes});
+    for (int j : placed) {
+      const CraftBuf& bj = p.bufs[j];
+      if (bj.first <= bi.last && bi.first <= bj.last) busy.push_back({bj.off, bj.off + bj.bytes});
+    }
     std::sort(busy.begin(), busy.end());
     size_t at = 0;
     for (const auto& b : busy) {
-      if (at + bufs[i].bytes <= b.first) break;
+      if (at + bi.bytes <= b.first) break;
       if (b.second > at) at = b.second;
     }
-    *bufs[i].off = at;
+    bi.off = at;
     placed.push_back(i);
-    if (at + bufs[i].bytes > total) total = at + bufs[i].bytes;
+    if (at + bi.bytes > total) total = at + bi.bytes;
   }
   p.bytes = total;
-  for (const Buf& b : bufs) p.bufs.push_back({b.name, *b.off, b.bytes, b.hh, b.ww, b.c, b.first, b.last});
   return p;
 }
 
+// The CRNN's buffers, laid out one after the other (not liveness-packed: every tap stays readable after the forward).
+// tap: b2o_crnn_tap reads the buffer under its name.
+namespace rb {
+enum Id : int8_t { x1, x2, x3, p3, x4, x5, p5, x6, features, sa, sb, d1, theta, warped, fc_9, xw1, hf, hb, l1, xw2, l2,
+                   logits, count };
+}
+struct CrnnBufSpec { const char* name; size_t bytes; bool tap; };     // bytes per crop
+constexpr CrnnBufSpec kCrnnBufs[rb::count] = {
+    {"x1", 200 * 31 * 64 * 2, true},     {"x2", 200 * 31 * 128 * 2, true},  {"x3", 200 * 31 * 256 * 2, true},
+    {"p3", 100 * 15 * 256 * 2, true},    {"x4", 100 * 15 * 256 * 2, true},  {"x5", 100 * 15 * 512 * 2, true},
+    {"p5", 50 * 7 * 512 * 2, true},      {"x6", 50 * 7 * 512 * 2, true},    {"features", 50 * 7 * 512 * 2, true},
+    {"sa", 50 * 7 * 16 * 2, false},      {"sb", 50 * 7 * 32 * 2, false},    {"d1", 64 * 2, false},
+    {"theta", 6 * 4, true},              {"warped", 50 * 7 * 512 * 2, true}, {"fc_9", 50 * 128 * 2, true},
+    {"xw1", 50 * 1024 * 4, false},       {"hf", 50 * 128 * 2, false},       {"hb", 50 * 128 * 2, false},
+    {"l1", 50 * 128 * 2, true},          {"xw2", 50 * 1024 * 4, false},     {"l2", 50 * 256 * 2, true},
+    {"logits", 48 * B2O_MAX_CLASSES * 4, true},   // sized for the largest alphabet so the plan is context-free
+};
+
 struct CrnnPlan {
-  int b;
-  size_t off_x1, off_x2, off_x3, off_p3, off_x4, off_x5, off_p5, off_x6, off_x7, off_sa, off_sb, off_d1, off_theta,
-      off_warp, off_fc9, off_xw1, off_hf, off_hb, off_l1, off_xw2, off_l2, off_logits, bytes;
+  size_t off[rb::count], bytes;      // bytes: a multiple of 256
 };
 
 CrnnPlan plan_crnn(int b) {
   CrnnPlan p;
-  p.b = b;
   size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t r = off; off += (bytes + 255) / 256 * 256; return r; };
-  const size_t B = static_cast<size_t>(b);
-  p.off_x1 = take(B * 200 * 31 * 64 * 2); p.off_x2 = take(B * 200 * 31 * 128 * 2); p.off_x3 = take(B * 200 * 31 * 256 * 2);
-  p.off_p3 = take(B * 100 * 15 * 256 * 2); p.off_x4 = take(B * 100 * 15 * 256 * 2); p.off_x5 = take(B * 100 * 15 * 512 * 2);
-  p.off_p5 = take(B * 50 * 7 * 512 * 2); p.off_x6 = take(B * 50 * 7 * 512 * 2); p.off_x7 = take(B * 50 * 7 * 512 * 2);
-  p.off_sa = take(B * 50 * 7 * 16 * 2); p.off_sb = take(B * 50 * 7 * 32 * 2); p.off_d1 = take(B * 64 * 2);
-  p.off_theta = take(B * 6 * 4); p.off_warp = take(B * 50 * 7 * 512 * 2); p.off_fc9 = take(B * 50 * 128 * 2);
-  p.off_xw1 = take(B * 50 * 1024 * 4); p.off_hf = take(B * 50 * 128 * 2); p.off_hb = take(B * 50 * 128 * 2);
-  p.off_l1 = take(B * 50 * 128 * 2); p.off_xw2 = take(B * 50 * 1024 * 4); p.off_l2 = take(B * 50 * 256 * 2);
-  p.off_logits = take(B * 48 * B2O_MAX_CLASSES * 4);   // sized for the largest alphabet so the plan is context-free
+  for (int i = 0; i < rb::count; ++i) {
+    p.off[i] = off;
+    off += (static_cast<size_t>(b) * kCrnnBufs[i].bytes + 255) / 256 * 256;
+  }
   p.bytes = off;
   return p;
+}
+
+// conv_cls.6 + conv_cls.8 (the tail) ride in conv_cls.4's epilogue on the auto engine's 16-column tile (same arithmetic
+// as head_tail_kernel, bit for bit): one launch and the 16-channel map's round trip through HBM less.
+bool tail_fused(const b2o_ctx* ctx, const ConvLayer& L4) {
+  return ctx->conv_engine == B2O_CONV_AUTO && L4.block_n == 16 && !ctx->no_fused_tail;
+}
+
+// conv_cls.4 (L4: in -> out), with the tail (L6, L8) into scores where tail_fused; otherwise head_tail_run follows it.
+int head_conv_run(b2o_ctx* ctx, const ConvLayer& L4, const ConvLayer& L6, const ConvLayer& L8, const TensorView& in,
+                  const TensorView& out, float* scores, cudaStream_t st) {
+  if (!tail_fused(ctx, L4)) return conv_run(ctx, L4, in, out, 0, st);
+  ConvTail tail = {L6.w_simt, L6.t1, L8.w_simt, L8.t1, scores};
+  if (L6.h_w_simt.size() == 256 && L8.h_w_simt.size() == 32) {
+    tail.h_w6 = L6.h_w_simt.data(); tail.h_b6 = L6.h_t1.data(); tail.h_w8 = L8.h_w_simt.data(); tail.h_b8 = L8.h_t1.data();
+  }
+  return conv_tc_run(ctx, L4, in, out, 0, st, nullptr, 1, &tail);
 }
 
 std::vector<float> ones(int n) { return std::vector<float>(static_cast<size_t>(n), 1.0f); }
@@ -519,148 +596,64 @@ extern "C" int b2o_craft_forward_until(b2o_ctx* ctx, const uint8_t* img, int n, 
   const CraftPlan p = plan_craft(n, h, w);
   if (ws_bytes < p.bytes) { ctx->set_error("b2o_craft_forward: workspace too small"); return B2O_ERR_WORKSPACE; }
   ctx->craft_step = -1;
-  // the step numbers are those of plan_craft's lifetimes; after step last_step the forward stops (host side, between
-  // launches) and records the step for b2o_craft_tap
-  auto stop_after = [&](int step) {
-    if (step < last_step) return false;
-    ctx->craft_step = last_step;
-    ctx->craft_ws = ws; ctx->craft_n = n; ctx->craft_h = h; ctx->craft_w = w;
-    return true;
-  };
-#define B2O_STOP_AFTER(step) \
-  if (stop_after(step)) return B2O_OK
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  uint8_t* base = reinterpret_cast<uint8_t*>(ws);
-  auto V = [&](size_t off, int hh, int ww, int c, int ld = 0, int coff = 0) { return make_view(base + off, n, hh, ww, c, ld, coff); };
-  auto L = [&](const char* name) -> const ConvLayer& { return ctx->craft[name]; };
-
-  const TensorView a = V(p.off_a, p.h1, p.w1, 64), b = V(p.off_b, p.h1, p.w1, 64), p1 = V(p.off_p1, p.h2, p.w2, 64);
-  const TensorView c = V(p.off_c, p.h2, p.w2, 128);
-  const TensorView cat4 = V(p.off_cat4, p.h2, p.w2, 192), cat4_y = V(p.off_cat4, p.h2, p.w2, 64, 192, 0),
-                   s1 = V(p.off_cat4, p.h2, p.w2, 128, 192, 64);
-  const TensorView p2 = V(p.off_p2, p.h4, p.w4, 128), d = V(p.off_d, p.h4, p.w4, 256);
-  const TensorView cat3 = V(p.off_cat3, p.h4, p.w4, 384), cat3_y = V(p.off_cat3, p.h4, p.w4, 128, 384, 0),
-                   s2 = V(p.off_cat3, p.h4, p.w4, 256, 384, 128);
-  const TensorView e = V(p.off_e, p.h4, p.w4, 256), p3 = V(p.off_p3, p.h8, p.w8, 256), f = V(p.off_f, p.h8, p.w8, 512);
-  const TensorView cat2 = V(p.off_cat2, p.h8, p.w8, 768), cat2_y = V(p.off_cat2, p.h8, p.w8, 256, 768, 0),
-                   s3 = V(p.off_cat2, p.h8, p.w8, 512, 768, 256);
-  const TensorView g = V(p.off_g, p.h8, p.w8, 512), p4 = V(p.off_p4, p.h16, p.w16, 512), hh = V(p.off_hh, p.h16, p.w16, 512);
-  const TensorView cat1 = V(p.off_cat1, p.h16, p.w16, 1536), s5 = V(p.off_cat1, p.h16, p.w16, 1024, 1536, 0),
-                   s4 = V(p.off_cat1, p.h16, p.w16, 512, 1536, 1024);
-  const TensorView mp = V(p.off_mp, p.h16, p.w16, 512), s5a = V(p.off_s5a, p.h16, p.w16, 1024);
-  const TensorView u1a = V(p.off_u1a, p.h16, p.w16, 512), u1b = V(p.off_u1b, p.h16, p.w16, 256);
-  const TensorView u2a = V(p.off_u2a, p.h8, p.w8, 256), u2b = V(p.off_u2b, p.h8, p.w8, 128);
-  const TensorView u3a = V(p.off_u3a, p.h4, p.w4, 128), u3b = V(p.off_u3b, p.h4, p.w4, 64);
-  const TensorView u4a = V(p.off_u4a, p.h2, p.w2, 64), u4b = V(p.off_u4b, p.h2, p.w2, 32);
-  const TensorView h1 = V(p.off_h1, p.h2, p.w2, 32), h2 = V(p.off_h2, p.h2, p.w2, 32), h3 = V(p.off_h3, p.h2, p.w2, 16);
-
-  // encoder (detection.py:312-324); taps s1..s4 are written straight into the concat buffers
-  if (ctx->conv_engine == B2O_CONV_SIMT || L("stem16").block_n == 0) {
-    B2O_STOP_AFTER(0);
-    B2O_RETURN_IF(stem_rgb_run(ctx, L("basenet.slice1.0"), img, n, h, w, a, st));          // fp32 CUDA-core stem
-  } else {
-    const TensorView x16 = V(p.off_x16, p.h1, p.w1, 16);
-    B2O_RETURN_IF(normalize16_run(ctx, img, n, h, w, x16.ptr, st));
-    B2O_STOP_AFTER(0);
-    B2O_RETURN_IF(conv_run(ctx, L("stem16"), x16, a, 0, st));
-  }
-  B2O_STOP_AFTER(1);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice1.3"), a, b, 0, st, &p1, 0));     // conv + fused 2x2 max pool
-  B2O_STOP_AFTER(2);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice1.7"), p1, c, 0, st));
-  B2O_STOP_AFTER(3);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice1.10"), c, s1, 0, st, &p2, 1));   // tap s1 (full) + pooled
-  B2O_STOP_AFTER(4);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice2.14"), p2, d, 0, st));
-  B2O_STOP_AFTER(5);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice2.17"), d, s2, 0, st));
-  B2O_STOP_AFTER(6);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice3.20"), s2, e, 0, st, &p3, 0));
-  B2O_STOP_AFTER(7);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice3.24"), p3, f, 0, st));
-  B2O_STOP_AFTER(8);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice3.27"), f, s3, 0, st));
-  B2O_STOP_AFTER(9);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice4.30"), s3, g, 0, st, &p4, 0));
-  B2O_STOP_AFTER(10);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice4.34"), p4, hh, 0, st));
-  B2O_STOP_AFTER(11);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice4.37"), hh, s4, 0, st));          // BN only, no ReLU (333)
-  B2O_STOP_AFTER(12);
-  // slice5 (365-378)
-  B2O_RETURN_IF(maxpool3s1_run(ctx, s4, mp, st));
-  B2O_STOP_AFTER(13);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice5.1"), mp, s5a, 0, st));
-  B2O_STOP_AFTER(14);
-  B2O_RETURN_IF(conv_run(ctx, L("basenet.slice5.2"), s5a, s5, 0, st));
-  B2O_STOP_AFTER(15);
-  // decoder (380-390)
-  B2O_RETURN_IF(conv_run(ctx, L("upconv1.conv.0"), cat1, u1a, 0, st));
-  B2O_STOP_AFTER(16);
-  B2O_RETURN_IF(conv_run(ctx, L("upconv1.conv.3"), u1a, u1b, 0, st));
-  B2O_STOP_AFTER(17);
+  auto V = [&](const Slice& s) { return p.view(ws, s); };
+  auto L = [&](const std::string& name) -> const ConvLayer& { return ctx->craft[name]; };
+  const bool rgb_stem = ctx->conv_engine == B2O_CONV_SIMT || L("stem16").block_n == 0;     // fp32 CUDA-core stem
   // UpsampleLike + Concatenate + 1x1 conv (380-390).  Opt-in (B2O_UPCONV_COMMUTE=1): where the skip tensor is exactly
   // twice the decoder tensor the upsampling is commuted behind the convolution -- the decoder half of the 1x1 conv runs
   // at LOW resolution and the full-resolution half adds its bilinear upsampling in the epilogue, so no upsampled tensor
   // is written or read back.  Correct (tests) but not the default: the explicit UpsampleLike is what the reference graph runs.
-  // Each level is two steps: the upsampling (or, commuted, the low-resolution decoder half z), then the 1x1 conv.
-  auto commuted = [&](const std::string& base, const TensorView& y, const TensorView& skip) {
+  // z has the decoder tensor's resolution, `full` (a slice of the concat) the skip tensor's.
+  auto commuted = [&](const CraftStep& s, const Slice& full) {
+    const CraftBuf &y = p.bufs[s.z.buf], &skip = p.bufs[full.buf];
+    const std::string base(s.layer);
     return ctx->conv_engine == B2O_CONV_AUTO && !ctx->no_commute && skip.h == 2 * y.h && skip.w == 2 * y.w &&
-           ctx->craft[base + ".y"].block_n != 0 && ctx->craft[base + ".s"].kch == 64 && ctx->craft[base + ".s"].block_n >= 64;
+           L(base + ".y").block_n != 0 && L(base + ".s").kch == 64 && L(base + ".s").block_n >= 64;
   };
-  auto level_up = [&](const char* name, const TensorView& y, const TensorView& cat_y, const TensorView& skip, size_t off_z,
-                      const TensorView& out) -> int {
-    const std::string base(name);
-    if (!commuted(base, y, skip)) return upsample_run(ctx, y, cat_y, st);
-    return conv_run(ctx, ctx->craft[base + ".y"], y, V(off_z, y.h, y.w, out.c), 0, st);
-  };
-  auto level_conv = [&](const char* name, const TensorView& y, const TensorView& cat, const TensorView& skip, size_t off_z,
-                        const TensorView& out) -> int {
-    const std::string base(name);
-    if (!commuted(base, y, skip)) return conv_run(ctx, ctx->craft[base], cat, out, 0, st);
-    const TensorView z = V(off_z, y.h, y.w, out.c);
-    return conv_tc_run(ctx, ctx->craft[base + ".s"], skip, out, 0, st, nullptr, 1, nullptr, &z);
-  };
-  B2O_RETURN_IF(level_up("upconv2.conv.0", u1b, cat2_y, s3, p.off_z2, u2a));
-  B2O_STOP_AFTER(18);
-  B2O_RETURN_IF(level_conv("upconv2.conv.0", u1b, cat2, s3, p.off_z2, u2a));
-  B2O_STOP_AFTER(19);
-  B2O_RETURN_IF(conv_run(ctx, L("upconv2.conv.3"), u2a, u2b, 0, st));
-  B2O_STOP_AFTER(20);
-  B2O_RETURN_IF(level_up("upconv3.conv.0", u2b, cat3_y, s2, p.off_z3, u3a));
-  B2O_STOP_AFTER(21);
-  B2O_RETURN_IF(level_conv("upconv3.conv.0", u2b, cat3, s2, p.off_z3, u3a));
-  B2O_STOP_AFTER(22);
-  B2O_RETURN_IF(conv_run(ctx, L("upconv3.conv.3"), u3a, u3b, 0, st));
-  B2O_STOP_AFTER(23);
-  B2O_RETURN_IF(level_up("upconv4.conv.0", u3b, cat4_y, s1, p.off_z4, u4a));
-  B2O_STOP_AFTER(24);
-  B2O_RETURN_IF(level_conv("upconv4.conv.0", u3b, cat4, s1, p.off_z4, u4a));
-  B2O_STOP_AFTER(25);
-  B2O_RETURN_IF(conv_run(ctx, L("upconv4.conv.3"), u4a, u4b, 0, st));
-  B2O_STOP_AFTER(26);
-  // head (392-410)
-  B2O_RETURN_IF(conv_run(ctx, L("conv_cls.0"), u4b, h1, 0, st));
-  B2O_STOP_AFTER(27);
-  B2O_RETURN_IF(conv_run(ctx, L("conv_cls.2"), h1, h2, 0, st));
-  B2O_STOP_AFTER(28);
-  if (ctx->conv_engine == B2O_CONV_AUTO && L("conv_cls.4").block_n == 16 && !ctx->no_fused_tail) {
-    // conv_cls.6 + conv_cls.8 ride in conv_cls.4's epilogue (same arithmetic as head_tail_kernel, bit for bit):
-    // one launch and the 16-channel map's round trip through HBM less
-    const ConvLayer &L6 = L("conv_cls.6"), &L8 = L("conv_cls.8");
-    ConvTail tail = {L6.w_simt, L6.t1, L8.w_simt, L8.t1, scores};
-    if (L6.h_w_simt.size() == 256 && L8.h_w_simt.size() == 32) {
-      tail.h_w6 = L6.h_w_simt.data(); tail.h_b6 = L6.h_t1.data(); tail.h_w8 = L8.h_w_simt.data(); tail.h_b8 = L8.h_t1.data();
+  for (int k = 0; k <= last_step; ++k) {
+    const CraftStep& s = kCraftSteps[k];
+    const TensorView src = V(s.src), out = V(s.out);
+    switch (s.kind) {
+      case StepKind::normalize:
+        if (!rgb_stem) B2O_RETURN_IF(normalize16_run(ctx, img, n, h, w, out.ptr, st));
+        break;
+      case StepKind::stem:
+        B2O_RETURN_IF(rgb_stem ? stem_rgb_run(ctx, L(s.layer), img, n, h, w, out, st)
+                               : conv_run(ctx, L("stem16"), src, out, 0, st));
+        break;
+      case StepKind::conv:
+        if (kCraftSteps[k + 1].kind == StepKind::tail) {
+          B2O_RETURN_IF(head_conv_run(ctx, L(s.layer), L("conv_cls.6"), L("conv_cls.8"), src, out, scores, st));
+        } else {
+          const TensorView pool = V(s.pool);      // conv + fused 2x2 max pool
+          B2O_RETURN_IF(conv_run(ctx, L(s.layer), src, out, 0, st, s.pool.buf == cb::none ? nullptr : &pool, s.write_full));
+        }
+        break;
+      case StepKind::maxpool3:
+        B2O_RETURN_IF(maxpool3s1_run(ctx, src, out, st));
+        break;
+      case StepKind::level_up:
+        B2O_RETURN_IF(commuted(s, s.out) ? conv_run(ctx, L(std::string(s.layer) + ".y"), src, V(s.z), 0, st)
+                                         : upsample_run(ctx, src, out, st));
+        break;
+      case StepKind::level_conv:
+        if (commuted(s, s.skip)) {
+          const TensorView z = V(s.z);
+          B2O_RETURN_IF(conv_tc_run(ctx, L(std::string(s.layer) + ".s"), V(s.skip), out, 0, st, nullptr, 1, nullptr, &z));
+        } else {
+          B2O_RETURN_IF(conv_run(ctx, L(s.layer), src, out, 0, st));
+        }
+        break;
+      case StepKind::tail:
+        if (!tail_fused(ctx, L(kCraftSteps[k - 1].layer)))
+          B2O_RETURN_IF(head_tail_run(ctx, L("conv_cls.6"), L("conv_cls.8"), src, scores, st));
+        break;
     }
-    B2O_RETURN_IF(conv_tc_run(ctx, L("conv_cls.4"), h2, h3, 0, st, nullptr, 1, &tail));
-    B2O_STOP_AFTER(29);
-  } else {
-    B2O_RETURN_IF(conv_run(ctx, L("conv_cls.4"), h2, h3, 0, st));
-    B2O_STOP_AFTER(29);
-    B2O_RETURN_IF(head_tail_run(ctx, L("conv_cls.6"), L("conv_cls.8"), h3, scores, st));
   }
-  B2O_STOP_AFTER(30);
-#undef B2O_STOP_AFTER
+  // the forward stops after step last_step (host side, between launches) and records it for b2o_craft_tap
+  ctx->craft_step = last_step;
+  ctx->craft_ws = ws; ctx->craft_n = n; ctx->craft_h = h; ctx->craft_w = w;
   return B2O_OK;
 }
 
@@ -680,9 +673,10 @@ extern "C" int b2o_craft_tap(b2o_ctx* ctx, const char* name, const void* ws, int
   }
   DeviceGuard guard(ctx->device);
   const CraftPlan p = plan_craft(n, h, w);
-  for (const CraftBuf& b : p.bufs) {
-    if (std::string(name) != b.name) continue;
-    const size_t bytes = static_cast<size_t>(n) * b.h * b.w * b.c * 2;
+  for (int i = 0; i < cb::count; ++i) {
+    if (std::string(name) != kCraftBufs[i].name) continue;
+    const CraftBuf& b = p.bufs[i];
+    const size_t bytes = static_cast<size_t>(n) * b.h * b.w * kCraftBufs[i].c * 2;
     if (out_bytes < bytes) { ctx->set_error("b2o_craft_tap: output too small"); return B2O_ERR_ARG; }
     if (ctx->craft_step < b.first || ctx->craft_step > b.last) {
       ctx->set_error(std::string("b2o_craft_tap: ") + name + " is not live after the last forward's step");
@@ -719,12 +713,13 @@ int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, floa
   if (ws_bytes < p.bytes) { ctx->set_error("b2o_crnn_forward: workspace too small"); return B2O_ERR_WORKSPACE; }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   uint8_t* base = reinterpret_cast<uint8_t*>(ws);
-  auto V = [&](size_t off, int nn, int hh, int ww, int c) { return make_view(base + off, nn, hh, ww, c); };
+  auto at = [&](rb::Id i) { return base + p.off[i]; };
+  auto V = [&](rb::Id i, int nn, int hh, int ww, int c) { return make_view(at(i), nn, hh, ww, c); };
   auto L = [&](const char* name) -> const ConvLayer& { return ctx->crnn[name]; };
-  const TensorView x1 = V(p.off_x1, b, 200, 31, 64), x2 = V(p.off_x2, b, 200, 31, 128), x3 = V(p.off_x3, b, 200, 31, 256);
-  const TensorView p3 = V(p.off_p3, b, 100, 15, 256), x4 = V(p.off_x4, b, 100, 15, 256), x5 = V(p.off_x5, b, 100, 15, 512);
-  const TensorView p5 = V(p.off_p5, b, 50, 7, 512), x6 = V(p.off_x6, b, 50, 7, 512), x7 = V(p.off_x7, b, 50, 7, 512);
-  const TensorView sa = V(p.off_sa, b, 50, 7, 16), sb = V(p.off_sb, b, 50, 7, 32);
+  const TensorView x1 = V(rb::x1, b, 200, 31, 64), x2 = V(rb::x2, b, 200, 31, 128), x3 = V(rb::x3, b, 200, 31, 256);
+  const TensorView p3 = V(rb::p3, b, 100, 15, 256), x4 = V(rb::x4, b, 100, 15, 256), x5 = V(rb::x5, b, 100, 15, 512);
+  const TensorView p5 = V(rb::p5, b, 50, 7, 512), x6 = V(rb::x6, b, 50, 7, 512), x7 = V(rb::features, b, 50, 7, 512);
+  const TensorView sa = V(rb::sa, b, 50, 7, 16), sb = V(rb::sb, b, 50, 7, 32);
   // conv stack (recognition.py:217-242)
   B2O_RETURN_IF(stem_crnn_run(ctx, L("conv_1"), reinterpret_cast<const __half*>(crnn_in), b, x1, st));
   B2O_RETURN_IF(conv_run(ctx, L("conv_2"), x1, x2, 0, st));
@@ -733,47 +728,47 @@ int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, floa
   B2O_RETURN_IF(conv_run(ctx, L("conv_5"), x4, x5, 0, st, &p5, 0));
   B2O_RETURN_IF(conv_run(ctx, L("conv_6"), p5, x6, 0, st));
   B2O_RETURN_IF(conv_run(ctx, L("conv_7"), x6, x7, 0, st));
-  __half* warped = reinterpret_cast<__half*>(base + p.off_warp);
+  __half* warped = reinterpret_cast<__half*>(at(rb::warped));
   if (!ctx->crnn_stn) {
     warped = x7.ptr;                                      // stn=False: Reshape consumes bn_7's output directly (282)
   } else {
   // spatial transformer (263-281)
   if (ctx->conv_engine == B2O_CONV_AUTO && L("stn.conv_a_gemm").block_n != 0) {
-    const TensorView y = V(p.off_warp, b, 50, 7, 512);   // the warp buffer is free until stn_sample
+    const TensorView y = V(rb::warped, b, 50, 7, 512);   // the warp buffer is free until stn_sample
     B2O_RETURN_IF(conv_run(ctx, L("stn.conv_a_gemm"), x7, y, 0, st));
     B2O_RETURN_IF(stn_col2im_run(ctx, y.ptr, L("stn.conv_a").t1, b, sa.ptr, st));
   } else {
     B2O_RETURN_IF(conv_run(ctx, L("stn.conv_a"), x7, sa, 0, st));
   }
   B2O_RETURN_IF(conv_run(ctx, L("stn.conv_b"), sa, sb, 0, st));
-  const TensorView sb_flat = make_view(base + p.off_sb, 1, 1, b, 11200), d1 = make_view(base + p.off_d1, 1, 1, b, 64);
+  const TensorView sb_flat = V(rb::sb, 1, 1, b, 11200), d1 = V(rb::d1, 1, 1, b, 64);
   B2O_RETURN_IF(conv_run(ctx, L("stn.dense_a"), sb_flat, d1, 0, st));
-  float* theta = reinterpret_cast<float*>(base + p.off_theta);
+  float* theta = reinterpret_cast<float*>(at(rb::theta));
   B2O_RETURN_IF(stn_theta_run(ctx, d1.ptr, b, theta, st));
   B2O_RETURN_IF(stn_sample_run(ctx, x7.ptr, theta, b, warped, st));
   }
   // reshape + fc_9 (282-290)
-  const TensorView seq_in = make_view(warped, 1, 1, b * 50, 3584), fc9 = make_view(base + p.off_fc9, 1, 1, b * 50, 128);
+  const TensorView seq_in = make_view(warped, 1, 1, b * 50, 3584), fc9 = V(rb::fc_9, 1, 1, b * 50, 128);
   B2O_RETURN_IF(conv_run(ctx, L("fc_9"), seq_in, fc9, 0, st));
   // BiLSTM (292-319)
-  const TensorView xw1 = make_view(base + p.off_xw1, 1, 1, b * 50, 1024);
+  const TensorView xw1 = V(rb::xw1, 1, 1, b * 50, 1024);
   TensorView xw1v = xw1;      // fp32 output: the view's pointer arithmetic is done by the engine in floats
   B2O_RETURN_IF(conv_run(ctx, L("lstm_in_1"), fc9, xw1v, 1, st));
-  __half* hf = reinterpret_cast<__half*>(base + p.off_hf);
-  __half* hb = reinterpret_cast<__half*>(base + p.off_hb);
-  __half* l1 = reinterpret_cast<__half*>(base + p.off_l1);
-  const float* xw1f = reinterpret_cast<const float*>(base + p.off_xw1);
+  __half* hf = reinterpret_cast<__half*>(at(rb::hf));
+  __half* hb = reinterpret_cast<__half*>(at(rb::hb));
+  __half* l1 = reinterpret_cast<__half*>(at(rb::l1));
+  const float* xw1f = reinterpret_cast<const float*>(at(rb::xw1));
   B2O_RETURN_IF(lstm_run(ctx, xw1f, 1024, 0, ctx->lstm_u[0], b, 0, hf, 128, 0, st));
   B2O_RETURN_IF(lstm_run(ctx, xw1f, 1024, 512, ctx->lstm_u[1], b, 1, hb, 128, 0, st));
   B2O_RETURN_IF(add_run(ctx, hf, hb, l1, static_cast<long long>(b) * 50 * 128, st));
-  const TensorView l1v = make_view(l1, 1, 1, b * 50, 128), xw2 = make_view(base + p.off_xw2, 1, 1, b * 50, 1024);
+  const TensorView l1v = make_view(l1, 1, 1, b * 50, 128), xw2 = V(rb::xw2, 1, 1, b * 50, 1024);
   B2O_RETURN_IF(conv_run(ctx, L("lstm_in_2"), l1v, xw2, 1, st));
-  const float* xw2f = reinterpret_cast<const float*>(base + p.off_xw2);
-  __half* l2 = reinterpret_cast<__half*>(base + p.off_l2);
+  const float* xw2f = reinterpret_cast<const float*>(at(rb::xw2));
+  __half* l2 = reinterpret_cast<__half*>(at(rb::l2));
   B2O_RETURN_IF(lstm_run(ctx, xw2f, 1024, 0, ctx->lstm_u[2], b, 0, l2, 256, 0, st));
   B2O_RETURN_IF(lstm_run(ctx, xw2f, 1024, 512, ctx->lstm_u[3], b, 1, l2, 256, 128, st));
   // fc_12 + discard + greedy CTC (321-333)
-  B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, keep_logits || ctx->debug_taps ? reinterpret_cast<float*>(base + p.off_logits) : nullptr,
+  B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, keep_logits || ctx->debug_taps ? reinterpret_cast<float*>(at(rb::logits)) : nullptr,
                            labels, logp, st));
   return B2O_OK;
 }
@@ -807,7 +802,7 @@ extern "C" int b2o_crnn_forward_beam(b2o_ctx* ctx, const void* crnn_in, int b, i
   // the greedy labels of fc_ctc_kernel go to the first b * 48 entries of `labels`, which the beam search then overwrites
   B2O_RETURN_IF(crnn_forward(ctx, crnn_in, b, labels, nullptr, true, ws, ws_bytes, stream));
   DeviceGuard guard(ctx->device);
-  const float* logits = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(ws) + plan_crnn(b).off_logits);
+  const float* logits = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(ws) + plan_crnn(b).off[rb::logits]);
   return ctc_beam_run(ctx, logits, b, ctx->n_classes, beam_width, top_paths, labels, logp,
                       reinterpret_cast<cudaStream_t>(stream));
 }
@@ -835,8 +830,6 @@ bool lexicon_args_ok(b2o_ctx* ctx, const char* fn, int k, int n_words, int top_p
   }
   return true;
 }
-
-size_t crnn_lexicon_scratch_offset(int b) { return (plan_crnn(b).bytes + 255) / 256 * 256; }
 
 }  // namespace
 
@@ -875,7 +868,8 @@ extern "C" int b2o_crnn_forward_lexicon(b2o_ctx* ctx, const void* crnn_in, int b
     return B2O_ERR_ARG;
   }
   if (b == 0) return B2O_OK;
-  const size_t scratch = crnn_lexicon_scratch_offset(b);
+  const CrnnPlan p = plan_crnn(b);
+  const size_t scratch = p.bytes;           // the decoder's scratch follows the CRNN's buffers, 256-byte aligned
   if (ws_bytes < scratch + ctc_lexicon_workspace_bytes(b, n_words)) {
     ctx->set_error("b2o_crnn_forward_lexicon: workspace too small");
     return B2O_ERR_WORKSPACE;
@@ -884,7 +878,7 @@ extern "C" int b2o_crnn_forward_lexicon(b2o_ctx* ctx, const void* crnn_in, int b
   B2O_RETURN_IF(crnn_forward(ctx, crnn_in, b, labels_out, nullptr, true, ws, ws_bytes, stream));
   DeviceGuard guard(ctx->device);
   uint8_t* base = reinterpret_cast<uint8_t*>(ws);
-  const float* logits = reinterpret_cast<const float*>(base + plan_crnn(b).off_logits);
+  const float* logits = reinterpret_cast<const float*>(base + p.off[rb::logits]);
   return ctc_lexicon_run(ctx, logits, b, ctx->n_classes, offsets, labels, n_words, top_paths, labels_out, logp,
                          base + scratch, reinterpret_cast<cudaStream_t>(stream));
 }
@@ -909,9 +903,9 @@ extern "C" int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, in
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const uint8_t* base = reinterpret_cast<const uint8_t*>(ws);
   if (theta_dev && ctx->crnn_stn)
-    B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(theta_dev, base + p.off_theta, static_cast<size_t>(b) * 6 * sizeof(float),
+    B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(theta_dev, base + p.off[rb::theta], static_cast<size_t>(b) * 6 * sizeof(float),
                                         cudaMemcpyDeviceToDevice, st));
-  return ctc_align_run(ctx, reinterpret_cast<const float*>(base + p.off_logits), b, ctx->n_classes, labels_dev, top_paths,
+  return ctc_align_run(ctx, reinterpret_cast<const float*>(base + p.off[rb::logits]), b, ctx->n_classes, labels_dev, top_paths,
                        spans_dev, logp_dev, st);
 }
 
@@ -924,33 +918,23 @@ extern "C" int b2o_set_debug_taps(b2o_ctx* ctx, int on) {
 extern "C" int b2o_crnn_tap(b2o_ctx* ctx, const char* name, const void* ws, int b, void* out, size_t out_bytes, void* stream) {
   if (!ctx || !name || !ws || !out || b <= 0) return B2O_ERR_ARG;
   DeviceGuard guard(ctx->device);
-  const CrnnPlan p = plan_crnn(b);
-  const size_t B = static_cast<size_t>(b);
-  size_t off = 0, bytes = 0;
   const std::string s(name);
-  if (s == "features") { off = p.off_x7; bytes = B * 50 * 7 * 512 * 2; }
-  else if (s == "x1") { off = p.off_x1; bytes = B * 200 * 31 * 64 * 2; }
-  else if (s == "x2") { off = p.off_x2; bytes = B * 200 * 31 * 128 * 2; }
-  else if (s == "x3") { off = p.off_x3; bytes = B * 200 * 31 * 256 * 2; }
-  else if (s == "p3") { off = p.off_p3; bytes = B * 100 * 15 * 256 * 2; }
-  else if (s == "x4") { off = p.off_x4; bytes = B * 100 * 15 * 256 * 2; }
-  else if (s == "x5") { off = p.off_x5; bytes = B * 100 * 15 * 512 * 2; }
-  else if (s == "p5") { off = p.off_p5; bytes = B * 50 * 7 * 512 * 2; }
-  else if (s == "x6") { off = p.off_x6; bytes = B * 50 * 7 * 512 * 2; }
-  else if ((s == "theta" || s == "warped") && !ctx->crnn_stn) { ctx->set_error("b2o_crnn_tap: this recognizer has no spatial transformer"); return B2O_ERR_STATE; }
-  else if (s == "theta") { off = p.off_theta; bytes = B * 6 * 4; }
-  else if (s == "warped") { off = p.off_warp; bytes = B * 50 * 7 * 512 * 2; }
-  else if (s == "fc_9") { off = p.off_fc9; bytes = B * 50 * 128 * 2; }
-  else if (s == "l1") { off = p.off_l1; bytes = B * 50 * 128 * 2; }
-  else if (s == "l2") { off = p.off_l2; bytes = B * 50 * 256 * 2; }
-  else if (s == "logits") {
-    if (!ctx->debug_taps) { ctx->set_error("b2o_crnn_tap: logits are only kept after b2o_set_debug_taps(ctx, 1)"); return B2O_ERR_STATE; }
-    off = p.off_logits; bytes = B * 48 * ctx->n_classes * 4;
+  int i = 0;
+  while (i < rb::count && !(kCrnnBufs[i].tap && s == kCrnnBufs[i].name)) ++i;
+  if (i == rb::count) { ctx->set_error("b2o_crnn_tap: unknown tap " + s); return B2O_ERR_ARG; }
+  if ((i == rb::theta || i == rb::warped) && !ctx->crnn_stn) {
+    ctx->set_error("b2o_crnn_tap: this recognizer has no spatial transformer");
+    return B2O_ERR_STATE;
   }
-  else { ctx->set_error("b2o_crnn_tap: unknown tap " + s); return B2O_ERR_ARG; }
+  if (i == rb::logits && !ctx->debug_taps) {
+    ctx->set_error("b2o_crnn_tap: logits are only kept after b2o_set_debug_taps(ctx, 1)");
+    return B2O_ERR_STATE;
+  }
+  // the logits slot is sized for B2O_MAX_CLASSES; the tap copies the context's classes
+  const size_t bytes = static_cast<size_t>(b) * (i == rb::logits ? 48 * ctx->n_classes * 4 : kCrnnBufs[i].bytes);
   if (out_bytes < bytes) { ctx->set_error("b2o_crnn_tap: output too small"); return B2O_ERR_ARG; }
-  B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(out, reinterpret_cast<const uint8_t*>(ws) + off, bytes, cudaMemcpyDeviceToDevice,
-                                      reinterpret_cast<cudaStream_t>(stream)));
+  B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(out, reinterpret_cast<const uint8_t*>(ws) + plan_crnn(b).off[i], bytes,
+                                      cudaMemcpyDeviceToDevice, reinterpret_cast<cudaStream_t>(stream)));
   return B2O_OK;
 }
 
@@ -1039,15 +1023,8 @@ int conv_test_run(b2o_ctx* ctx, const b2o_conv_test_desc& d, cudaStream_t st) {
                               nullptr, nullptr, false));
     B2O_RETURN_IF(build_layer(ctx, L8, "test.8", 16, 2, 1, 1, 0, g8, ones(2), std::vector<float>(d.b8_host, d.b8_host + 2),
                               nullptr, nullptr, false));
-    if (ctx->conv_engine == B2O_CONV_AUTO && L.block_n == 16 && !ctx->no_fused_tail) {      // as b2o_craft_forward
-      ConvTail ct = {L6.w_simt, L6.t1, L8.w_simt, L8.t1, d.scores_dev};
-      if (L6.h_w_simt.size() == 256 && L8.h_w_simt.size() == 32) {
-        ct.h_w6 = L6.h_w_simt.data(); ct.h_b6 = L6.h_t1.data(); ct.h_w8 = L8.h_w_simt.data(); ct.h_b8 = L8.h_t1.data();
-      }
-      return conv_tc_run(ctx, L, in, out, 0, st, nullptr, 1, &ct);
-    }
-    B2O_RETURN_IF(conv_run(ctx, L, in, out, 0, st));
-    return head_tail_run(ctx, L6, L8, out, d.scores_dev, st);
+    B2O_RETURN_IF(head_conv_run(ctx, L, L6, L8, in, out, d.scores_dev, st));
+    return tail_fused(ctx, L) ? B2O_OK : head_tail_run(ctx, L6, L8, out, d.scores_dev, st);
   }
   if (d.pool_dev) {
     const TensorView pool = make_view(d.pool_dev, d.n, d.h / 2, d.w / 2, d.cout, d.pool_ld);

@@ -304,7 +304,8 @@ def upsample_ref(x, rows_in, ih, rows_out, oh, ow):
     return val, bound
 
 
-# plan_craft's buffers (keras-ocr_b200/csrc/api.cu): name -> (level = resolution divisor, channels, first step, last step)
+# The CRAFT workspace's buffers (kCraftBufs in keras-ocr_b200/csrc/api.cu, with the lifetimes plan_craft derives from
+# kCraftSteps): name -> (level = resolution divisor, channels, first step, last step)
 CRAFT_BUFS = {
     "x16": (1, 16, 0, 1), "a": (1, 64, 1, 2), "b": (1, 64, 2, 2), "p1": (2, 64, 2, 3), "c": (2, 128, 3, 4),
     "cat4": (2, 192, 4, 25), "p2": (4, 128, 4, 5), "d": (4, 256, 5, 6), "cat3": (4, 384, 6, 22), "e": (4, 256, 7, 7),
