@@ -317,6 +317,45 @@ int b2o_crnn_forward_logits(b2o_ctx* ctx, const void* crnn_in_dev, int b, int32_
 int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths, int32_t* spans_dev, float* logp_dev,
                    float* theta_dev, const void* ws_dev, size_t ws_bytes, void* stream);
 
+/* Training the output layer for a custom alphabet: Recognizer.compile() + training_model with ctc_batch_cost
+ * (recognition.py:321-349, 539-545; docs/examples/fine_tuning_recognizer.rst) restricted to fc_12 (Dense 256 -> k plus
+ * bias), the rest of the CRNN frozen.
+ * b2o_crnn_features: the forward of b2o_crnn_forward up to the BiLSTM output l2, whose 48 kept steps (2..49,
+ * rnn_steps_to_discard, recognition.py:328) go to features_dev (b, 48, 256) fp16; fc_12 and the decoder do not run.
+ * Workspace: b2o_crnn_workspace_bytes(b).
+ * b2o_ctc_loss_grad: per crop i the Keras ctc_batch_cost loss on the softmax output over the 48 kept steps,
+ *   L_i = -log sum over the alignments of the text of prod_t q[t, path_t],  q = softmax(x_t w + bias) + 1e-7, blank = k-1,
+ * i.e. minus the b2o_ctc_lexicon_decode score of the text.  x_t is row index_dev[i] of features_dev (n_rows, 48, 256)
+ * fp16 (16-byte aligned; index_dev NULL: row i), after Dropout(dropout) (recognition.py:321): feature c of step t of row r
+ * is kept iff splitmix64(key0 ^ (r * 12288 + t * 256 + c)) >> 40 >= floor(dropout * 2^24), key0 =
+ * splitmix64(splitmix64(seed) ^ step), and kept features are multiplied by the fp32 1 / (1 - dropout); dropout = 0 uses the
+ * features unchanged.  The logits are fc_ctc_kernel's (the serial fmaf chain over the features in ascending order), so
+ * with dropout 0 they are bit for bit those inference decodes; logits_dev (b, 48, k) float32, when not NULL, receives them.
+ * w_dev (256, k) and bias_dev (k) float32 are the caller's.  Texts: CSR as for the lexicon, offsets_dev (b + 1) int32,
+ * labels_dev int16.  loss_dev (b) float32: L_i, a function of the crop's features, text, the weights and (with dropout)
+ * seed, step and its row only -- bit-identical in any batch and on every run.  A text that is empty, longer than 48, has
+ * a label outside [0, k-2] or cannot be aligned in 48 steps (L + adjacent repeats > 48) gets +inf, a row index outside
+ * [0, n_rows) NaN; such crops add nothing to the gradient.
+ * grad_w_dev (256, k) and grad_b_dev (k) float32: (1/b) sum over crops and steps of x_t^T dL_i/dlogits_t and of
+ * dL_i/dlogits_t, summed in a fixed order (bit-identical run to run; the order of the crops in the batch matters in the
+ * last bits).  Both NULL: the loss only, and ws_dev may be NULL.  Otherwise ws_bytes >= b2o_ctc_train_workspace_bytes(b, k).
+ * 2 <= k <= B2O_MAX_CLASSES, 0 <= dropout < 1, otherwise B2O_ERR_ARG.
+ * b2o_rmsprop_step: Keras RMSprop with momentum 0 (the default optimizer of Recognizer.compile, recognition.py:539-545)
+ * on n float32 elements: acc = rho acc + (1 - rho) g^2; param -= lr g / (sqrt(acc) + eps), in fp32, in that order.  acc
+ * starts at 0; Keras' defaults are lr 1e-3, rho 0.9, eps 1e-7.
+ * b2o_crnn_set_top: copies (256, k) w_dev and (k) bias_dev into the context's fc_12; every forward enqueued after it uses
+ * them.  k must equal the loaded class count (B2O_ERR_ARG otherwise).                                              */
+int b2o_crnn_features(b2o_ctx* ctx, const void* crnn_in_dev, int b, void* features_dev, void* ws_dev, size_t ws_bytes,
+                      void* stream);
+size_t b2o_ctc_train_workspace_bytes(int b, int k);
+int b2o_ctc_loss_grad(b2o_ctx* ctx, const void* features_dev, int n_rows, const int32_t* index_dev, int b, int k,
+                      const float* w_dev, const float* bias_dev, const int32_t* offsets_dev, const int16_t* labels_dev,
+                      float dropout, uint64_t seed, uint64_t step, float* loss_dev, float* grad_w_dev,
+                      float* grad_b_dev, float* logits_dev, void* ws_dev, size_t ws_bytes, void* stream);
+int b2o_rmsprop_step(b2o_ctx* ctx, float* param_dev, const float* grad_dev, float* acc_dev, int64_t n, float lr,
+                     float rho, float eps, void* stream);
+int b2o_crnn_set_top(b2o_ctx* ctx, const float* w_dev, const float* bias_dev, int k, void* stream);
+
 /* Result records of Pipeline.recognize for the multi-GPU gather (pipeline.py:66-75; SURVEY.md 8(e)): one
  * fixed-size float32 row per image = [count][rec_boxes x (4,2) boxes * inv_scale[i] (tools.adjust_boxes,
  * tools.py:232-260)][rec_boxes x 48 labels as int8, -1 padded], b2o_record_floats(rec_boxes) floats long.

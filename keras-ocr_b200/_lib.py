@@ -95,6 +95,12 @@ SIGNATURES = {
     "b2o_char_cells": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "b2o_crnn_forward_logits": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_crnn_align": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_crnn_features": (_i, [_vp, _vp, _i, _vp, _vp, _sz, _vp]),
+    "b2o_ctc_train_workspace_bytes": (_sz, [_i, _i]),
+    "b2o_ctc_loss_grad": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _c.c_uint64, _c.c_uint64, _vp, _vp,
+                               _vp, _vp, _vp, _sz, _vp]),
+    "b2o_rmsprop_step": (_i, [_vp, _vp, _vp, _vp, _c.c_int64, _f, _f, _f, _vp]),
+    "b2o_crnn_set_top": (_i, [_vp, _vp, _vp, _i, _vp]),
     "b2o_set_debug_taps": (_i, [_vp, _i]),
     "b2o_crnn_tap": (_i, [_vp, _c.c_char_p, _vp, _i, _vp, _sz, _vp]),
     "b2o_conv2d_test": (_i, [_vp, _vp, _i, _i, _i, _i, _c.POINTER(_c.c_float), _i, _i, _i,
@@ -333,6 +339,25 @@ class Context:
     def crnn_align(self, b, labels, top_paths, spans, logp, theta, ws, ws_bytes, stream):
         self._check(self.lib.b2o_crnn_align(self.handle, b, labels, top_paths, spans, logp, theta, ws, ws_bytes, stream),
                     "b2o_crnn_align")
+
+    def crnn_features(self, crnn_in, b, features, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_crnn_features(self.handle, crnn_in, b, features, ws, ws_bytes, stream),
+                    "b2o_crnn_features")
+
+    def ctc_train_workspace_bytes(self, b, k):
+        return int(self.lib.b2o_ctc_train_workspace_bytes(b, k))
+
+    def ctc_loss_grad(self, features, n_rows, index, b, k, w, bias, offsets, labels, dropout, seed, step, loss, grad_w,
+                      grad_b, logits, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_ctc_loss_grad(self.handle, features, n_rows, index, b, k, w, bias, offsets, labels,
+                                               float(dropout), int(seed), int(step), loss, grad_w, grad_b, logits, ws,
+                                               ws_bytes, stream), "b2o_ctc_loss_grad")
+
+    def rmsprop_step(self, param, grad, acc, n, lr, rho, eps, stream):
+        self._check(self.lib.b2o_rmsprop_step(self.handle, param, grad, acc, n, lr, rho, eps, stream), "b2o_rmsprop_step")
+
+    def crnn_set_top(self, w, bias, k, stream):
+        self._check(self.lib.b2o_crnn_set_top(self.handle, w, bias, k, stream), "b2o_crnn_set_top")
 
     def set_debug_taps(self, on):
         self._check(self.lib.b2o_set_debug_taps(self.handle, int(on)), "b2o_set_debug_taps")

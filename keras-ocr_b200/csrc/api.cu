@@ -22,6 +22,13 @@ int ctc_lexicon_run(b2o_ctx* ctx, const float* logits, int B, int K, const int* 
                     int n_words, int top_paths, int* labels_out, float* logp, void* ws, cudaStream_t st);
 int ctc_align_run(b2o_ctx* ctx, const float* logits, int B, int K, const int32_t* labels, int P, int32_t* spans,
                   float* logp, cudaStream_t st);
+size_t ctc_train_workspace_bytes(int B, int K);
+int ctc_loss_grad_run(b2o_ctx* ctx, const __half* features, int n_rows, const int* index, int B, int K, const float* w,
+                      const float* bias, const int* offsets, const short* labels, float rate, uint64_t seed,
+                      uint64_t step, float* loss, float* grad_w, float* grad_b, float* logits, void* ws,
+                      cudaStream_t st);
+int rmsprop_run(b2o_ctx* ctx, float* param, const float* grad, float* acc, long long n, float lr, float rho, float eps,
+                cudaStream_t st);
 
 namespace {
 
@@ -701,14 +708,15 @@ extern "C" int b2o_crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_
 namespace {
 
 // The CRNN through fc_12 + greedy CTC.  keep_logits: the fp32 logits always go to the workspace's logits slot (the beam
-// search reads them there); otherwise only with the debug taps on.
+// search reads them there); otherwise only with the debug taps on.  features (b2o_crnn_features): the forward stops
+// after the BiLSTM and copies its 48 kept steps (b, 48, 256) fp16 there instead of running fc_12 + CTC (labels unused).
 int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, float* logp, bool keep_logits, void* ws,
-                 size_t ws_bytes, void* stream) {
+                 size_t ws_bytes, void* stream, __half* features = nullptr) {
   if (!ctx) return B2O_ERR_ARG;
   if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_forward: CRNN weights not loaded"); return B2O_ERR_STATE; }
   DeviceGuard guard(ctx->device);
   if (b == 0) return B2O_OK;
-  if (!crnn_in || !labels || !ws || b < 0) { ctx->set_error("b2o_crnn_forward: bad argument"); return B2O_ERR_ARG; }
+  if (!crnn_in || (!labels && !features) || !ws || b < 0) { ctx->set_error("b2o_crnn_forward: bad argument"); return B2O_ERR_ARG; }
   const CrnnPlan p = plan_crnn(b);
   if (ws_bytes < p.bytes) { ctx->set_error("b2o_crnn_forward: workspace too small"); return B2O_ERR_WORKSPACE; }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -767,6 +775,11 @@ int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, floa
   __half* l2 = reinterpret_cast<__half*>(at(rb::l2));
   B2O_RETURN_IF(lstm_run(ctx, xw2f, 1024, 0, ctx->lstm_u[2], b, 0, l2, 256, 0, st));
   B2O_RETURN_IF(lstm_run(ctx, xw2f, 1024, 512, ctx->lstm_u[3], b, 1, l2, 256, 128, st));
+  if (features) {            // rnn_steps_to_discard = 2 (recognition.py:328): steps 2..49 of every crop
+    B2O_CUDA_CHECK(ctx, cudaMemcpy2DAsync(features, 48 * 256 * sizeof(__half), l2 + 2 * 256, 50 * 256 * sizeof(__half),
+                                          48 * 256 * sizeof(__half), b, cudaMemcpyDeviceToDevice, st));
+    return B2O_OK;
+  }
   // fc_12 + discard + greedy CTC (321-333)
   B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, keep_logits || ctx->debug_taps ? reinterpret_cast<float*>(at(rb::logits)) : nullptr,
                            labels, logp, st));
@@ -886,6 +899,66 @@ extern "C" int b2o_crnn_forward_lexicon(b2o_ctx* ctx, const void* crnn_in, int b
 extern "C" int b2o_crnn_forward_logits(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, float* logp, void* ws,
                                        size_t ws_bytes, void* stream) {
   return crnn_forward(ctx, crnn_in, b, labels, logp, true, ws, ws_bytes, stream);
+}
+
+extern "C" int b2o_crnn_features(b2o_ctx* ctx, const void* crnn_in, int b, void* features, void* ws, size_t ws_bytes,
+                                 void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (b > 0 && !features) { ctx->set_error("b2o_crnn_features: bad argument"); return B2O_ERR_ARG; }
+  return crnn_forward(ctx, crnn_in, b, nullptr, nullptr, false, ws, ws_bytes, stream, reinterpret_cast<__half*>(features));
+}
+
+extern "C" size_t b2o_ctc_train_workspace_bytes(int b, int k) {
+  if (b <= 0 || k < 2 || k > B2O_MAX_CLASSES) return 0;
+  return ctc_train_workspace_bytes(b, k);
+}
+
+extern "C" int b2o_ctc_loss_grad(b2o_ctx* ctx, const void* features, int n_rows, const int32_t* index, int b, int k,
+                                 const float* w, const float* bias, const int32_t* offsets, const int16_t* labels,
+                                 float dropout, uint64_t seed, uint64_t step, float* loss, float* grad_w, float* grad_b,
+                                 float* logits, void* ws, size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  const char* fn = "b2o_ctc_loss_grad";
+  if (k < 2 || k > B2O_MAX_CLASSES) { ctx->set_error(std::string(fn) + ": k must be in [2, 1024]"); return B2O_ERR_ARG; }
+  if (!(dropout >= 0.f && dropout < 1.f)) { ctx->set_error(std::string(fn) + ": dropout must be in [0, 1)"); return B2O_ERR_ARG; }
+  if (b < 0 || (b > 0 && (!features || n_rows <= 0 || !w || !bias || !offsets || !labels || !loss)) ||
+      (!grad_w) != (!grad_b) || (reinterpret_cast<uintptr_t>(features) & 15)) {
+    ctx->set_error(std::string(fn) + ": bad argument");
+    return B2O_ERR_ARG;
+  }
+  if (b == 0) return B2O_OK;
+  if (grad_w && (!ws || ws_bytes < ctc_train_workspace_bytes(b, k))) {
+    ctx->set_error(std::string(fn) + ": workspace too small");
+    return B2O_ERR_WORKSPACE;
+  }
+  DeviceGuard guard(ctx->device);
+  return ctc_loss_grad_run(ctx, reinterpret_cast<const __half*>(features), n_rows, index, b, k, w, bias, offsets, labels,
+                           dropout, seed, step, loss, grad_w, grad_b, logits, ws, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2o_rmsprop_step(b2o_ctx* ctx, float* param, const float* grad, float* acc, int64_t n, float lr, float rho,
+                                float eps, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (n < 0 || (n > 0 && (!param || !grad || !acc)) || !(lr >= 0.f) || !(rho >= 0.f && rho <= 1.f) || !(eps >= 0.f)) {
+    ctx->set_error("b2o_rmsprop_step: bad argument");
+    return B2O_ERR_ARG;
+  }
+  DeviceGuard guard(ctx->device);
+  return rmsprop_run(ctx, param, grad, acc, n, lr, rho, eps, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2o_crnn_set_top(b2o_ctx* ctx, const float* w, const float* bias, int k, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_set_top: CRNN weights not loaded"); return B2O_ERR_STATE; }
+  if (!w || !bias || k != ctx->n_classes) {
+    ctx->set_error("b2o_crnn_set_top: w, bias must be given and k must equal the loaded class count");
+    return B2O_ERR_ARG;
+  }
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->fc12_w, w, static_cast<size_t>(256) * k * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->fc12_b, bias, static_cast<size_t>(k) * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return B2O_OK;
 }
 
 extern "C" int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths, int32_t* spans_dev,

@@ -28,10 +28,12 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "ctc_q.cuh"
 
 namespace {
 
-constexpr int kT = 48, kThreads = 128, kChunk = 1024, kSelThreads = 256;
+using ctcq::kT;
+constexpr int kThreads = 128, kChunk = 1024, kSelThreads = 256;
 constexpr int kMaxLabelEnd = 1 << 24;            // entries whose labels end beyond 2^24 score -inf (B2O_MAX_LEXICON_LABELS)
 
 __device__ __forceinline__ unsigned okey(float f) {           // order-preserving uint32 of a float
@@ -47,59 +49,22 @@ __device__ __forceinline__ int entry_len(const int* __restrict__ offsets, int i,
   return (o0 >= 0 && o1 <= kMaxLabelEnd && o1 - o0 >= 1 && o1 - o0 <= kT) ? o1 - o0 : 0;
 }
 
-// q of one crop's 48 steps into s (row stride K+1, column K = 0): one warp per step, fixed-order reductions.
+// q of one crop's 48 steps into s (row stride K+1, column K = 0): one warp per step, fixed-order reductions
+// (ctc_q.cuh, shared with the training loss).
 __device__ void stage_probs(const float* __restrict__ logits, int K, float* s) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int t = warp; t < kT; t += kThreads / 32) {
     const float* row = logits + t * K;
     float* out = s + t * (K + 1);
-    float m = -INFINITY;
-    for (int c = lane; c < K; c += 32) m = fmaxf(m, row[c]);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    float se = 0.f;
-    for (int c = lane; c < K; c += 32) se = __fadd_rn(se, expf(__fsub_rn(row[c], m)));
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) se = __fadd_rn(se, __shfl_xor_sync(0xffffffffu, se, o));
-    for (int c = lane; c < K; c += 32) out[c] = __fadd_rn(__fdiv_rn(expf(__fsub_rn(row[c], m)), se), 1e-7f);
+    float m, se;
+    ctcq::ctc_step_norm(row, K, lane, &m, &se);
+    for (int c = lane; c < K; c += 32) out[c] = ctcq::ctc_q(row[c], m, se);
     if (lane == 0) out[K] = 0.f;
   }
 }
 
-template <int NS>
-__device__ __forceinline__ void rescale(float (&a)[NS], int& e_sum) {
-  float m = a[0];
-#pragma unroll
-  for (int s = 1; s < NS; ++s) m = fmaxf(m, a[s]);
-  if (m > 0.f && (m < 0x1p32f || m >= 0x1p100f)) {
-    int sh = 99 - ((__float_as_int(m) >> 23) - 127);            // the largest state into [2^99, 2^100)
-    sh = max(-126, min(126, sh));
-    const float f = __int_as_float((127 + sh) << 23);
-#pragma unroll
-    for (int s = 0; s < NS; ++s) a[s] = __fmul_rn(a[s], f);
-    e_sum += sh;
-  }
-}
-
-// Steps an alignment needs from state s to a final state (S-2 or S-1): one per label still to come, one per blank a
-// repeated label among them needs, one more from a blank state.
-__device__ __forceinline__ int need_steps(int s, int L, unsigned long long rep) {
-  if (s >= 2 * L - 1) return 0;
-  const int i = s >> 1;
-  return (L - 1 - i) + __popcll(rep >> (i + 1)) + ((s & 1) ? 0 : 1);
-}
-
-// Zeroes the states that can no longer reach a final state in the `left` steps that remain.  They are a prefix
-// (need_steps does not increase with s), [0, live), and never flow into a state that can: s -> s' in one step means
-// need(s) <= need(s') + 1.  So zeroing them changes no score, and the rescaling follows the largest state that counts
-// -- without it, a state that stays on blank would hold the scale while the only path to the end underflows.
-template <int NS>
-__device__ __forceinline__ void prune(float (&a)[NS], int& live, int left, int L, unsigned long long rep) {
-  while (live < 2 * L - 1 && need_steps(live, L, rep) > left) ++live;
-#pragma unroll
-  for (int s = 0; s < NS; ++s)
-    if (s < live) a[s] = 0.f;
-}
+using ctcq::ctc_prune;
+using ctcq::ctc_rescale;
 
 // okey of the entry's CTC forward log-probability over q (row stride K+1), 0 for -inf.
 template <int NL>
@@ -129,8 +94,8 @@ __device__ unsigned entry_key(const float* q, int K, const short* __restrict__ l
   a[0] = q[K - 1];
   a[1] = q[col[0]];
   int e_sum = 0, live = 0;
-  prune(a, live, kT - 1, L, rep);
-  rescale(a, e_sum);
+  ctc_prune(a, live, kT - 1, L, rep);
+  ctc_rescale(a, e_sum);
   for (int t = 1; t < kT; ++t) {
     const float* r = q + t * (K + 1);
     const float qb = r[K - 1];
@@ -147,8 +112,8 @@ __device__ unsigned entry_key(const float* q, int K, const short* __restrict__ l
       a[s] = v;
     }
     a[0] = __fmul_rn(a[0], qb);
-    prune(a, live, kT - 1 - t, L, rep);
-    rescale(a, e_sum);
+    ctc_prune(a, live, kT - 1 - t, L, rep);
+    ctc_rescale(a, e_sum);
   }
   const int S = 2 * L + 1;
   float x2 = 0.f, x1 = 0.f;

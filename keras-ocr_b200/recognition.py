@@ -59,6 +59,51 @@ def check_beam(beam_width=None, top_paths=1):
         raise ValueError(f"top_paths ({top_paths}) must not exceed beam_width ({beam_width})")
 
 
+def _check_word(i, w, index, what):
+    """The rules a lexicon entry and a training text share: a non-empty string of at most 48 characters of the
+    alphabet (``index``: character -> label); ``ValueError`` naming entry ``i`` otherwise."""
+    if not isinstance(w, str) or not w:
+        raise ValueError(f"{what} {i} ({w!r}) is not a non-empty string")
+    if len(w) > STEPS:
+        raise ValueError(f"{what} {i} ({w!r}) is longer than {STEPS} characters")
+    bad = next((ch for ch in w if ch not in index), None)
+    if bad is not None:
+        raise ValueError(f"{what} {i} ({w!r}) has {bad!r}, which is not in the alphabet")
+
+
+def encode_csr(words, index):
+    """Checked words -> CSR: (offsets (n+1) int32, labels int16), word i is labels[offsets[i]:offsets[i+1]]."""
+    lengths = np.fromiter((len(w) for w in words), dtype=np.int64, count=len(words))
+    offsets = np.zeros(len(words) + 1, np.int32)
+    offsets[1:] = np.cumsum(lengths)
+    labels = np.fromiter((index[ch] for w in words for ch in w), dtype=np.int16, count=int(lengths.sum()))
+    return offsets, labels
+
+
+def check_texts(texts, alphabet=DEFAULT_ALPHABET):
+    """Validates the target texts of ``Recognizer.fit_top`` on the host, before anything is launched, and returns their
+    CSR encoding (``encode_csr``).  The rules are the reference's training rules (``get_batch_generator``,
+    recognition.py:440-449): every text is a non-empty string of at most 48 characters, all in ``alphabet``, without two
+    spaces in a row; and it must be alignable in the 48 steps, i.e. its length plus its adjacent repeated characters
+    (each needs a blank between its copies) is at most 48 -- Keras would give such a text an infinite loss and NaN
+    gradients.  Texts may repeat.  ``ValueError`` names the first offending text."""
+    if isinstance(texts, str) or not isinstance(texts, (list, tuple, np.ndarray)):
+        raise ValueError("texts must be a list or tuple of strings")
+    texts = list(texts)
+    if not texts:
+        raise ValueError("there are no texts")
+    index = {ch: i for i, ch in enumerate(alphabet)}
+    for i, w in enumerate(texts):
+        _check_word(i, w, index, "text")
+        if "  " in w:
+            raise ValueError(f"text {i} ({w!r}) has two spaces in a row, which the reference does not train on")
+        repeats = sum(a == b for a, b in zip(w, w[1:]))
+        if len(w) + repeats > STEPS:
+            raise ValueError(f"text {i} ({w!r}) cannot be aligned in {STEPS} steps: {len(w)} characters and {repeats} "
+                             "doubled letters, each of which needs a blank")
+    return encode_csr(texts, index)
+
+
 class Lexicon:
     """A word list for lexicon-constrained decoding (``b2o_crnn_forward_lexicon``): every crop reads as the entry with the
     highest CTC forward log-probability -- the sum over every 48-step alignment that collapses to the entry -- and
@@ -80,13 +125,7 @@ class Lexicon:
         index = {ch: i for i, ch in enumerate(alphabet)}
         seen = set()
         for i, w in enumerate(words):
-            if not isinstance(w, str) or not w:
-                raise ValueError(f"lexicon entry {i} ({w!r}) is not a non-empty string")
-            if len(w) > STEPS:
-                raise ValueError(f"lexicon entry {i} ({w!r}) is longer than {STEPS} characters")
-            bad = next((ch for ch in w if ch not in index), None)
-            if bad is not None:
-                raise ValueError(f"lexicon entry {i} ({w!r}) has {bad!r}, which is not in the alphabet")
+            _check_word(i, w, index, "lexicon entry")
             if w in seen:
                 raise ValueError(f"lexicon entry {i} ({w!r}) is a duplicate")
             seen.add(w)
@@ -96,9 +135,7 @@ class Lexicon:
             i = int(np.argmax(np.cumsum(lengths) > _lib.MAX_LEXICON_LABELS))
             raise ValueError(f"lexicon entry {i} ({words[i]!r}) takes the lexicon past {_lib.MAX_LEXICON_LABELS} "
                              "characters in all")
-        self.offsets = np.zeros(len(words) + 1, np.int32)
-        self.offsets[1:] = np.cumsum(lengths)
-        self.labels = np.fromiter((index[ch] for w in words for ch in w), dtype=np.int16, count=int(lengths.sum()))
+        self.offsets, self.labels = encode_csr(words, index)
         self._device = {}
 
     def __len__(self):
@@ -186,7 +223,8 @@ class Recognizer:
         alphabet: the characters the model recognises (default ``0-9a-z``; up to 1023 characters).  The
             checkpoint's ``fc_12`` must have ``len(alphabet) + 1`` classes; if it does not, the reference's
             "backbone weights only" behaviour applies (recognition.py:399-411): the top layer is
-            re-initialised (Glorot uniform, zero bias) and has to be trained before it is useful.
+            re-initialised (Glorot uniform, zero bias) and has to be trained before it is useful: ``fit_top`` trains it
+            on the GPU from labelled word crops, and ``save_weights`` keeps the result.
         weights: ``None`` builds an untrained model for ``alphabet`` (as the reference does); ``"kurapan"`` looks for ``crnn_kurapan.npz`` (exported) or the reference's ``crnn_kurapan.h5``
             (read with h5py where installed) in the cache dir; otherwise a ``.npz`` / ``.h5`` path or a dict
             keyed like ``weights.py``.
@@ -252,6 +290,7 @@ class Recognizer:
             tensors["fc_12.bias"] = np.zeros(n_classes, np.float32)
         self.ctx = _lib.Context(self.device_index)
         self.ctx.load_crnn(tensors)
+        self._tensors = tensors          # host weights as loaded (save_weights; fit_top replaces the top)
         self._keep_workspace = False     # tests set keep_workspace to read intermediate taps
         self._last_ws = None
         self._ws = None                  # reusable CRNN workspace (grown on demand)
@@ -577,3 +616,141 @@ class Recognizer:
             predictions = decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
         ends = np.cumsum(counts)
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]
+
+    # ------------------------------------------------------------------ training the top layer
+    def _input_crops(self, crops, what):
+        """(N,31,200[,3]) uint8 crops -> the CRNN input (N,200,31[,3]) fp16 on the device."""
+        tail = (3,) if self.color else ()
+        shape = tuple(crops.shape) if hasattr(crops, "shape") else None
+        dtype_ok = (crops.dtype == torch.uint8) if isinstance(crops, torch.Tensor) else (np.asarray(crops).dtype == np.uint8)
+        if shape is None or shape[1:] != (TARGET_HEIGHT, TARGET_WIDTH) + tail or not dtype_ok:
+            raise ValueError(f"{what} must be a uint8 array of shape (N, {TARGET_HEIGHT}, {TARGET_WIDTH}"
+                             f"{', 3' if self.color else ''}), got {shape}")
+        return crops
+
+    def _features(self, crops, chunk=512):
+        """``b2o_crnn_features`` of every crop, in chunks that bound the CRNN workspace: (N,48,256) fp16 CUDA."""
+        n = int(crops.shape[0])
+        feats = torch.empty((n, STEPS, 256), dtype=torch.float16, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        nbytes = self.ctx.crnn_workspace_bytes(min(chunk, n))
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        tail = (3,) if self.color else ()
+        for i in range(0, n, chunk):
+            part = crops[i:i + chunk]
+            t = part if isinstance(part, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(part))
+            t = t.to(self.device).contiguous()
+            b = t.shape[0]
+            x = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + tail, dtype=torch.float16, device=self.device)
+            self.ctx.crops_to_input(t.data_ptr(), b, x.data_ptr(), stream, color=self.color)
+            self.ctx.crnn_features(x.data_ptr(), b, feats[i:i + b].data_ptr(), ws.data_ptr(), nbytes, stream)
+        return feats
+
+    def _batch_targets(self, offsets, labels, idx):
+        """The CSR targets of rows ``idx`` of a CSR set, on the device."""
+        lengths = np.diff(offsets)[idx]
+        off = np.zeros(len(idx) + 1, np.int32)
+        off[1:] = np.cumsum(lengths)
+        lab = np.concatenate([labels[offsets[j]:offsets[j + 1]] for j in idx]).astype(np.int16)
+        return torch.from_numpy(off).to(self.device), torch.from_numpy(lab).to(self.device)
+
+    def _mean_loss(self, feats, offsets, labels, w, bias, chunk=1024):
+        """Mean of L_b over a feature set, without dropout (``b2o_ctc_loss_grad``, loss only), in fp64 on the host."""
+        n, k = feats.shape[0], w.shape[1]
+        loss = torch.empty(n, dtype=torch.float32, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        for i in range(0, n, chunk):
+            idx = np.arange(i, min(n, i + chunk), dtype=np.int32)
+            off, lab = self._batch_targets(offsets, labels, idx)
+            index = torch.from_numpy(idx).to(self.device)
+            self.ctx.ctc_loss_grad(feats.data_ptr(), n, index.data_ptr(), len(idx), k, w.data_ptr(), bias.data_ptr(),
+                                   off.data_ptr(), lab.data_ptr(), 0.0, 0, 0, loss[i:].data_ptr(), None, None, None,
+                                   None, 0, stream)
+        return float(loss.cpu().numpy().astype(np.float64).mean())
+
+    def fit_top(self, crops, texts, epochs=1, batch_size=64, learning_rate=1e-3, dropout=0.25, seed=0, validation=None):
+        """Train the output layer (``fc_12``, Dense 256 -> len(alphabet) + 1 with bias) on labelled word crops, the rest
+        of the CRNN frozen -- the reference's fine-tuning workflow (``compile()`` + ``training_model``,
+        recognition.py:334-349, 539-545) restricted to the top.  ``crops``: (N,31,200) uint8 -- (N,31,200,3) for a color
+        recognizer -- as ``recognize_crops`` takes them; ``texts``: N strings over the alphabet (``check_texts``).
+        ``validation``: an optional (crops, texts) pair.
+
+        The BiLSTM features of every crop are computed once (``b2o_crnn_features``) and kept on the device, 24.6 kB per
+        crop.  Each epoch shuffles them with ``np.random.default_rng(seed)`` and runs, per batch, the Keras
+        ``ctc_batch_cost`` loss and its gradient (``b2o_ctc_loss_grad``; Dropout(``dropout``) before the layer, as in
+        the reference's graph) and one RMSprop step (``b2o_rmsprop_step``, Keras' defaults rho 0.9, eps 1e-7).  Training
+        starts from the current top: the re-initialised one for a new alphabet, the checkpoint's otherwise.  At the end
+        the new top is installed (``b2o_crnn_set_top``), so every recognition path uses it.  Same seed and inputs give
+        bit-identical weights.
+
+        Returns {"loss": [...], "val_loss": [...]}: per epoch the mean L_b over the training crops (as they were seen,
+        with dropout) and over the validation crops (without dropout, after the epoch; empty without ``validation``)."""
+        def is_int(v):
+            return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+        offsets, labels = check_texts(texts, self.alphabet)
+        n = len(offsets) - 1
+        crops = self._input_crops(crops, "crops")
+        if crops.shape[0] != n:
+            raise ValueError(f"{crops.shape[0]} crops but {n} texts")
+        if not is_int(epochs) or epochs < 1:
+            raise ValueError(f"epochs must be an int >= 1, got {epochs!r}")
+        if not is_int(batch_size) or batch_size < 1:
+            raise ValueError(f"batch_size must be an int >= 1, got {batch_size!r}")
+        if not is_int(seed) or seed < 0:
+            raise ValueError(f"seed must be an int >= 0, got {seed!r}")
+        if not (isinstance(learning_rate, (int, float)) and learning_rate > 0):
+            raise ValueError(f"learning_rate must be a positive number, got {learning_rate!r}")
+        if not (isinstance(dropout, (int, float)) and 0 <= dropout < 1):
+            raise ValueError(f"dropout must be in [0, 1), got {dropout!r}")
+        val = None
+        if validation is not None:
+            if not isinstance(validation, (tuple, list)) or len(validation) != 2:
+                raise ValueError("validation must be a (crops, texts) pair")
+            v_off, v_lab = check_texts(validation[1], self.alphabet)
+            v_crops = self._input_crops(validation[0], "validation crops")
+            if v_crops.shape[0] != len(v_off) - 1:
+                raise ValueError(f"{v_crops.shape[0]} validation crops but {len(v_off) - 1} texts")
+            val = (v_crops, v_off, v_lab)
+        k = len(self.alphabet) + 1
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        feats = self._features(crops)
+        v_feats = self._features(val[0]) if val is not None else None
+        w = torch.from_numpy(np.ascontiguousarray(self._tensors["fc_12.kernel"], np.float32)).to(self.device)
+        bias = torch.from_numpy(np.ascontiguousarray(self._tensors["fc_12.bias"], np.float32)).to(self.device)
+        acc_w, acc_b = torch.zeros_like(w), torch.zeros_like(bias)
+        grad_w, grad_b = torch.empty_like(w), torch.empty_like(bias)
+        bs = min(int(batch_size), n)
+        nbytes = self.ctx.ctc_train_workspace_bytes(bs, k)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        loss = torch.empty(n, dtype=torch.float32, device=self.device)
+        rng = np.random.default_rng(seed)
+        history = {"loss": [], "val_loss": []}
+        step = 0
+        for _ in range(epochs):
+            perm = rng.permutation(n).astype(np.int32)
+            for i in range(0, n, bs):
+                idx = perm[i:i + bs]
+                off, lab = self._batch_targets(offsets, labels, idx)
+                index = torch.from_numpy(idx).to(self.device)
+                self.ctx.ctc_loss_grad(feats.data_ptr(), n, index.data_ptr(), len(idx), k, w.data_ptr(),
+                                       bias.data_ptr(), off.data_ptr(), lab.data_ptr(), dropout, seed, step,
+                                       loss[i:].data_ptr(), grad_w.data_ptr(), grad_b.data_ptr(), None, ws.data_ptr(),
+                                       nbytes, stream)
+                self.ctx.rmsprop_step(w.data_ptr(), grad_w.data_ptr(), acc_w.data_ptr(), w.numel(), learning_rate, 0.9,
+                                      1e-7, stream)
+                self.ctx.rmsprop_step(bias.data_ptr(), grad_b.data_ptr(), acc_b.data_ptr(), bias.numel(),
+                                      learning_rate, 0.9, 1e-7, stream)
+                step += 1
+            history["loss"].append(float(loss.cpu().numpy().astype(np.float64).mean()))
+            if val is not None:
+                history["val_loss"].append(self._mean_loss(v_feats, val[1], val[2], w, bias))
+        self.ctx.crnn_set_top(w.data_ptr(), bias.data_ptr(), k, stream)
+        self._tensors = dict(self._tensors)
+        self._tensors["fc_12.kernel"] = w.cpu().numpy()
+        self._tensors["fc_12.bias"] = bias.cpu().numpy()
+        return history
+
+    def save_weights(self, path):
+        """Every CRNN tensor of this recognizer -- with the top ``fit_top`` trained -- as a flat ``.npz`` keyed like
+        ``weights.py``, which ``Recognizer(alphabet, weights=path)`` loads unchanged."""
+        np.savez(path, **{name: np.asarray(v, dtype=np.float32) for name, v in self._tensors.items()})
