@@ -134,7 +134,9 @@ int b2o_craft_tap(b2o_ctx* ctx, const char* name, const void* ws_dev, int n, int
 /* getBoxes (detection.py:207-287).  scores: (n,hs,ws,2) float32.  Writes, per image i,
  * counts[i] = number of boxes found (may exceed max_boxes: then only the first max_boxes are
  * stored and the caller retries with a larger buffer) and boxes[i][k][4][2] float32 in
- * detector-input pixels, in connected-component label order (= reference order).              */
+ * detector-input pixels, in connected-component label order (= reference order).  Slots k >= min(counts[i], max_boxes)
+ * of boxes (and of box_scores below) are left as they were.  Every byte of the workspace the result depends on is
+ * written by the call itself: the result does not depend on what the workspace held.                          */
 size_t b2o_boxes_workspace_bytes(int n, int hs, int ws, int max_boxes);
 int b2o_get_boxes(b2o_ctx* ctx, const float* scores_dev, int n, int hs, int ws,
                   float detection_threshold, float text_threshold, float link_threshold,
@@ -306,7 +308,10 @@ int b2o_crnn_forward_lexicon(b2o_ctx* ctx, const void* crnn_in_dev, int b, const
  * The product path: b2o_crnn_forward_logits is b2o_crnn_forward_scored that also keeps the fc_12 logits in the
  * workspace's logits slot (logp_dev may be NULL), as b2o_crnn_forward_beam and _lexicon always do; b2o_crnn_align then
  * aligns labels_dev on the logits of the preceding forward in ws_dev and copies its theta (b, 6) to theta_dev (NULL, or
- * a recognizer without STN: not written).  Workspace sizes are those of the forward.                               */
+ * a recognizer without STN: not written).  Workspace sizes are those of the forward.  The logits must be those of the
+ * context's last successful CRNN forward, with the same ws_dev and b, and that forward must have kept them (_logits,
+ * _beam, _lexicon, or any greedy forward with the debug taps on; b2o_crnn_features never does): otherwise
+ * B2O_ERR_STATE and nothing is written.                                                                            */
 #define B2O_MAX_ALIGN_PATHS 128
 int b2o_ctc_align(b2o_ctx* ctx, const float* logits_dev, int b, int k, const int32_t* labels_dev, int top_paths,
                   int32_t* spans_dev, float* logp_dev, void* stream);
@@ -335,7 +340,7 @@ int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths
  * labels_dev int16.  loss_dev (b) float32: L_i, a function of the crop's features, text, the weights and (with dropout)
  * seed, step and its row only -- bit-identical in any batch and on every run.  A text that is empty, longer than 48, has
  * a label outside [0, k-2] or cannot be aligned in 48 steps (L + adjacent repeats > 48) gets +inf, a row index outside
- * [0, n_rows) NaN; such crops add nothing to the gradient.
+ * [0, n_rows) NaN; such crops add nothing to the gradient, and their logits_dev rows are all NaN.
  * grad_w_dev (256, k) and grad_b_dev (k) float32: (1/b) sum over crops and steps of x_t^T dL_i/dlogits_t and of
  * dL_i/dlogits_t, summed in a fixed order (bit-identical run to run; the order of the crops in the batch matters in the
  * last bits).  Both NULL: the loss only, and ws_dev may be NULL.  Otherwise ws_bytes >= b2o_ctc_train_workspace_bytes(b, k).
@@ -382,7 +387,13 @@ int b2o_pack_records_scored(b2o_ctx* ctx, const float* boxes_dev, const int32_t*
  * "fc_9" (b,50,128 f16), "l1" (b,50,128 f16), "l2" (b,50,256 f16), "logits" (b,48,K f32); the conv backbone
  * "x1" (b,200,31,64 f16, conv_1), "x2" (128, conv_2), "x3" (256, conv_3), "p3" (b,100,15,256, its pool),
  * "x4" (256, conv_4), "x5" (512, conv_5), "p5" (b,50,7,512, its pool), "x6" (512, conv_6).  "x3" and "x5" are only
- * written by engines that do not fuse the pool into the convolution (SIMT, TC_GENERIC).                     */
+ * written by engines that do not fuse the pool into the convolution (SIMT, TC_GENERIC).
+ * As for b2o_craft_tap, a tap reads the context's last successful CRNN forward (any b2o_crnn_forward*, or
+ * b2o_crnn_features, which stops after "l2"), given the same ws_dev and b, and only a buffer that forward wrote: "x3"
+ * and "x5" per its engine, "theta" and "warped" with a spatial transformer, "logits" when it kept them (the debug taps
+ * on at the forward, or _logits, _beam, _lexicon).  Otherwise B2O_ERR_STATE, also before any forward, after a forward
+ * that failed once it had begun enqueueing work, and after b2o_load_crnn (a call rejected by its argument or workspace
+ * checks changes nothing).  Unknown name or out_bytes too small: B2O_ERR_ARG.                                  */
 int b2o_set_debug_taps(b2o_ctx* ctx, int on);
 int b2o_crnn_tap(b2o_ctx* ctx, const char* name, const void* ws_dev, int b, void* out_dev,
                  size_t out_bytes, void* stream);
@@ -444,7 +455,7 @@ int b2o_warp_plan_test(b2o_ctx* ctx, const float* boxes_dev, int n, b2o_warp_pla
  * image of the component's first pixel in raster order; -1 for background.  comps_dev (n,max_boxes,7) int32: the kept
  * components in box order, (root, left, top, width, height, area, maxtext) with maxtext the order-preserving int key
  * of the largest text score (the float's bits if >= 0, else bits ^ 0x7fffffff); entries past min(count, max_boxes)
- * are left as they were.                                                                                       */
+ * are left as they were.  labels_dev or comps_dev NULL: B2O_ERR_ARG before anything is enqueued.               */
 int b2o_get_boxes_test(b2o_ctx* ctx, const float* scores_dev, int n, int hs, int ws,
                        float detection_threshold, float text_threshold, float link_threshold,
                        int size_threshold, float* boxes_dev, int32_t* counts_dev, float* box_scores_dev,

@@ -299,6 +299,13 @@ CrnnPlan plan_crnn(int b) {
   return p;
 }
 
+// slot i of ws holds values of the context's last successful CRNN forward: plan_crnn(b) places the slots, so ws and b must
+// be that forward's, and it must have written the slot
+static_assert(rb::count <= 32, "b2o_ctx::crnn_written has one bit per slot");
+bool crnn_wrote(const b2o_ctx* ctx, rb::Id i, const void* ws, int b) {
+  return ws == ctx->crnn_ws && b == ctx->crnn_b && ((ctx->crnn_written >> i) & 1u);
+}
+
 // conv_cls.6 + conv_cls.8 (the tail) ride in conv_cls.4's epilogue on the auto engine's 16-column tile (same arithmetic
 // as head_tail_kernel, bit for bit): one launch and the 16-channel map's round trip through HBM less.
 bool tail_fused(const b2o_ctx* ctx, const ConvLayer& L4) {
@@ -460,6 +467,7 @@ extern "C" int b2o_load_crnn(b2o_ctx* ctx, const b2o_tensor* tensors, int n) {
   DeviceGuard guard(ctx->device);
   TensorMap m;
   for (int i = 0; i < n; ++i) m[tensors[i].name] = &tensors[i];
+  ctx->crnn_written = 0;      // a workspace written with other weights (other classes, no STN) has nothing to tap
   struct Spec { const char* name; int cin, cout, k; const char* bn; };
   const Spec convs[] = {{"conv_1", 1, 64, 3, nullptr},    {"conv_2", 64, 128, 3, nullptr}, {"conv_3", 128, 256, 3, "bn_3"},
                         {"conv_4", 256, 256, 3, nullptr}, {"conv_5", 256, 512, 3, "bn_5"}, {"conv_6", 512, 512, 3, nullptr},
@@ -719,11 +727,23 @@ int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, floa
   if (!crnn_in || (!labels && !features) || !ws || b < 0) { ctx->set_error("b2o_crnn_forward: bad argument"); return B2O_ERR_ARG; }
   const CrnnPlan p = plan_crnn(b);
   if (ws_bytes < p.bytes) { ctx->set_error("b2o_crnn_forward: workspace too small"); return B2O_ERR_WORKSPACE; }
+  ctx->crnn_written = 0;      // from here on the slots hold neither the last forward's values nor this one's
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   uint8_t* base = reinterpret_cast<uint8_t*>(ws);
   auto at = [&](rb::Id i) { return base + p.off[i]; };
   auto V = [&](rb::Id i, int nn, int hh, int ww, int c) { return make_view(at(i), nn, hh, ww, c); };
   auto L = [&](const char* name) -> const ConvLayer& { return ctx->crnn[name]; };
+  // the slots this forward writes, recorded on success for b2o_crnn_tap / b2o_crnn_align
+  auto bit = [](rb::Id i) { return 1u << i; };
+  const bool logits_kept = !features && (keep_logits || ctx->debug_taps);
+  const uint32_t wrote = bit(rb::x1) | bit(rb::x2) | (conv_pool_fused(ctx, L("conv_3")) ? 0u : bit(rb::x3)) | bit(rb::p3) |
+                         bit(rb::x4) | (conv_pool_fused(ctx, L("conv_5")) ? 0u : bit(rb::x5)) | bit(rb::p5) | bit(rb::x6) |
+                         bit(rb::features) | (ctx->crnn_stn ? bit(rb::theta) | bit(rb::warped) : 0u) | bit(rb::fc_9) |
+                         bit(rb::l1) | bit(rb::l2) | (logits_kept ? bit(rb::logits) : 0u);
+  auto record = [&]() {
+    ctx->crnn_ws = ws; ctx->crnn_b = b; ctx->crnn_written = wrote;
+    return B2O_OK;
+  };
   const TensorView x1 = V(rb::x1, b, 200, 31, 64), x2 = V(rb::x2, b, 200, 31, 128), x3 = V(rb::x3, b, 200, 31, 256);
   const TensorView p3 = V(rb::p3, b, 100, 15, 256), x4 = V(rb::x4, b, 100, 15, 256), x5 = V(rb::x5, b, 100, 15, 512);
   const TensorView p5 = V(rb::p5, b, 50, 7, 512), x6 = V(rb::x6, b, 50, 7, 512), x7 = V(rb::features, b, 50, 7, 512);
@@ -778,12 +798,11 @@ int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, floa
   if (features) {            // rnn_steps_to_discard = 2 (recognition.py:328): steps 2..49 of every crop
     B2O_CUDA_CHECK(ctx, cudaMemcpy2DAsync(features, 48 * 256 * sizeof(__half), l2 + 2 * 256, 50 * 256 * sizeof(__half),
                                           48 * 256 * sizeof(__half), b, cudaMemcpyDeviceToDevice, st));
-    return B2O_OK;
+    return record();
   }
   // fc_12 + discard + greedy CTC (321-333)
-  B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, keep_logits || ctx->debug_taps ? reinterpret_cast<float*>(at(rb::logits)) : nullptr,
-                           labels, logp, st));
-  return B2O_OK;
+  B2O_RETURN_IF(fc_ctc_run(ctx, l2, b, logits_kept ? reinterpret_cast<float*>(at(rb::logits)) : nullptr, labels, logp, st));
+  return record();
 }
 
 bool beam_args_ok(b2o_ctx* ctx, const char* fn, int k, int beam_width, int top_paths) {
@@ -972,6 +991,11 @@ extern "C" int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, in
   if (b == 0) return B2O_OK;
   const CrnnPlan p = plan_crnn(b);
   if (ws_bytes < p.bytes) { ctx->set_error("b2o_crnn_align: workspace too small"); return B2O_ERR_WORKSPACE; }
+  if (!crnn_wrote(ctx, rb::logits, ws, b)) {
+    ctx->set_error("b2o_crnn_align: the last successful CRNN forward of this context did not keep its logits in this ws "
+                   "with this b");
+    return B2O_ERR_STATE;
+  }
   DeviceGuard guard(ctx->device);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const uint8_t* base = reinterpret_cast<const uint8_t*>(ws);
@@ -995,12 +1019,10 @@ extern "C" int b2o_crnn_tap(b2o_ctx* ctx, const char* name, const void* ws, int 
   int i = 0;
   while (i < rb::count && !(kCrnnBufs[i].tap && s == kCrnnBufs[i].name)) ++i;
   if (i == rb::count) { ctx->set_error("b2o_crnn_tap: unknown tap " + s); return B2O_ERR_ARG; }
-  if ((i == rb::theta || i == rb::warped) && !ctx->crnn_stn) {
-    ctx->set_error("b2o_crnn_tap: this recognizer has no spatial transformer");
-    return B2O_ERR_STATE;
-  }
-  if (i == rb::logits && !ctx->debug_taps) {
-    ctx->set_error("b2o_crnn_tap: logits are only kept after b2o_set_debug_taps(ctx, 1)");
+  if (!crnn_wrote(ctx, static_cast<rb::Id>(i), ws, b)) {
+    ctx->set_error("b2o_crnn_tap: the last successful CRNN forward of this context did not write " + s +
+                   " in this ws with this b" + ((i == rb::theta || i == rb::warped) && !ctx->crnn_stn
+                                                    ? " (this recognizer has no spatial transformer)" : ""));
     return B2O_ERR_STATE;
   }
   // the logits slot is sized for B2O_MAX_CLASSES; the tap copies the context's classes

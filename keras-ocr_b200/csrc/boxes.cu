@@ -814,20 +814,38 @@ extern "C" int b2o_get_boxes_scored(b2o_ctx* ctx, const float* scores, int n, in
   return B2O_OK;
 }
 
+namespace {
+
+// comps of b2o_get_boxes_test: the min(count, max_boxes) kept components of each image; the slots past them, which select_kernel
+// did not write in this call, keep the caller's bytes
+__global__ void __launch_bounds__(128)
+copy_kept_comps_kernel(const Component* __restrict__ src, const int32_t* __restrict__ counts, int max_boxes,
+                       int32_t* __restrict__ comps) {
+  static_assert(sizeof(Component) == 7 * sizeof(int32_t), "b2o_get_boxes_test copies 7 int32 per component");
+  const int i = blockIdx.x;
+  const int c = min(max(counts[i], 0), max_boxes);
+  const int32_t* s = reinterpret_cast<const int32_t*>(src + static_cast<size_t>(i) * max_boxes);
+  int32_t* d = comps + static_cast<size_t>(i) * max_boxes * 7;
+  for (int t = threadIdx.x; t < 7 * c; t += blockDim.x) d[t] = s[t];
+}
+
+}  // namespace
+
 extern "C" int b2o_get_boxes_test(b2o_ctx* ctx, const float* scores, int n, int hs, int ws, float detection_threshold,
                                   float text_threshold, float link_threshold, int size_threshold, float* boxes,
                                   int32_t* counts, float* box_scores, int max_boxes, void* ws_dev, size_t ws_bytes,
                                   int32_t* labels, int32_t* comps, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!labels || !comps) { ctx->set_error("b2o_get_boxes_test: bad argument"); return B2O_ERR_ARG; }
   const int rc = b2o_get_boxes_scored(ctx, scores, n, hs, ws, detection_threshold, text_threshold, link_threshold,
                                       size_threshold, boxes, counts, box_scores, max_boxes, ws_dev, ws_bytes, stream);
   if (rc != B2O_OK) return rc;
-  if (!labels || !comps) { ctx->set_error("b2o_get_boxes_test: bad argument"); return B2O_ERR_ARG; }
+  DeviceGuard guard(ctx->device);
   const BoxWorkspace w = carve(ws_dev, n, hs, ws, max_boxes);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  static_assert(sizeof(Component) == 7 * sizeof(int32_t), "b2o_get_boxes_test copies 7 int32 per component");
   B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(labels, w.label, static_cast<size_t>(n) * hs * ws * 4, cudaMemcpyDeviceToDevice, st));
-  B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(comps, w.comps, static_cast<size_t>(n) * max_boxes * sizeof(Component),
-                                      cudaMemcpyDeviceToDevice, st));
+  copy_kept_comps_kernel<<<n, 128, 0, st>>>(w.comps, counts, max_boxes, comps);
+  B2O_LAUNCH_CHECK(ctx);
   return B2O_OK;
 }
 

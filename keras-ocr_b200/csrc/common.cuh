@@ -119,6 +119,11 @@ struct b2o_ctx {
   int craft_step = -1;         // last step of the most recent successful CRAFT forward (b2o_craft_tap), -1: none
   const void* craft_ws = nullptr;   // ... and its workspace and input shape, which b2o_craft_tap must be given again
   int craft_n = 0, craft_h = 0, craft_w = 0;
+  // the most recent successful CRNN forward (b2o_crnn_tap, b2o_crnn_align): its workspace and batch, and bit i set for
+  // every workspace slot rb::i (api.cu) it wrote; 0: none since creation, or the last forward failed after it started
+  const void* crnn_ws = nullptr;
+  int crnn_b = 0;
+  uint32_t crnn_written = 0;
   bool profile = false;
   std::vector<cudaEvent_t> prof_events;   // (start, stop) pairs
   double prof_flop = 0.0;
@@ -149,6 +154,8 @@ int conv_simt_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const 
                   int out_f32, cudaStream_t st);
 int conv_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const TensorView& out,
              int out_f32, cudaStream_t st, const TensorView* pool_out = nullptr, int write_full = 1);
+// conv_run of L with a pool_out fuses the pool into the convolution (then write_full = 0 leaves `out` unwritten)
+bool conv_pool_fused(const b2o_ctx* ctx, const ConvLayer& L);
 int stem_rgb_run(b2o_ctx* ctx, const ConvLayer& L, const uint8_t* img, int n, int h, int w,
                  const TensorView& out, cudaStream_t st);
 int normalize16_run(b2o_ctx* ctx, const uint8_t* img, int n, int h, int w, __half* out, cudaStream_t st);

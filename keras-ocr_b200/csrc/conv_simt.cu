@@ -518,10 +518,14 @@ int conv_simt_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const 
   return B2O_OK;
 }
 
+bool conv_pool_fused(const b2o_ctx* ctx, const ConvLayer& L) {
+  return ctx->conv_engine == B2O_CONV_AUTO && L.block_n != 0;      // generic tiles and SIMT pool in a kernel of its own
+}
+
 int conv_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const TensorView& out, int out_f32,
              cudaStream_t st, const TensorView* pool_out, int write_full) {
   if (ctx->conv_engine != B2O_CONV_SIMT && L.block_n != 0) {
-    if (pool_out != nullptr && (ctx->conv_engine == B2O_CONV_TC_GENERIC)) {      // generic tiles: unfused pool
+    if (pool_out != nullptr && !conv_pool_fused(ctx, L)) {      // generic tiles: unfused pool
       B2O_RETURN_IF(conv_tc_run(ctx, L, in, out, out_f32, st));
       return maxpool2_run(ctx, out, *pool_out, st);
     }

@@ -141,8 +141,10 @@ ctc_loss_kernel(const __half* __restrict__ features /*[n_rows][48][256]*/, int n
   const unsigned long long rep = s_rep;
   if (bad) {
     if (tid == 0) loss[b] = bad == 2 ? __int_as_float(0x7fc00000) : INFINITY;
-    if (g)
-      for (int i = tid; i < kT * K; i += kThreads) g[static_cast<size_t>(b) * kT * K + i] = 0.f;
+    for (int i = tid; i < kT * K; i += kThreads) {
+      if (g) g[static_cast<size_t>(b) * kT * K + i] = 0.f;
+      if (logits_out) logits_out[static_cast<size_t>(b) * kT * K + i] = __int_as_float(0x7fc00000);   // no logits: NaN
+    }
     return;
   }
   // ---- features (and the dropout mask) into shared memory
