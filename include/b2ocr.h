@@ -361,6 +361,38 @@ int b2o_rmsprop_step(b2o_ctx* ctx, float* param_dev, const float* grad_dev, floa
                      float rho, float eps, void* stream);
 int b2o_crnn_set_top(b2o_ctx* ctx, const float* w_dev, const float* bias_dev, int k, void* stream);
 
+/* Fine-tuning the recurrent head: Recognizer.compile() + training_model with ctc_batch_cost (recognition.py:292-349,
+ * 539-545; docs/examples/fine_tuning_recognizer.rst) restricted to lstm_10, lstm_10_back, lstm_11, lstm_11_back and fc_12;
+ * the convolutions, the STN and fc_9 stay frozen.
+ * b2o_crnn_sequence_features: the forward of b2o_crnn_forward up to fc_9 (recognition.py:282-290), whose output goes to
+ * out_dev (b, 50, 128) fp16, bit for bit the "fc_9" tap; the BiLSTM, fc_12 and the decoder do not run.  Workspace:
+ * b2o_crnn_workspace_bytes(b).  Afterwards b2o_crnn_tap reads every slot up to "fc_9", not "l1" / "l2" / "logits".
+ * b2o_rnn_loss_grad: per crop i the loss of b2o_ctc_loss_grad (same q, dropout mask, +inf / NaN rules) on the l2 that the
+ * BiLSTM computes from row index_dev[i] of x_dev (n_rows, 50, 128) fp16 (16-byte aligned; index_dev NULL: row i), the
+ * dropout mask keyed on that row, so loss_dev (b) float32 is a function of the crop's row, text, the weights, seed and
+ * step only.  params_dev is one float32 vector, per LSTM in the order lstm_10, lstm_10_back, lstm_11, lstm_11_back its
+ * kernel (128, 512), recurrent_kernel (128, 512) and bias (512) (131,584 floats each), then fc_12.kernel (256, k) and
+ * fc_12.bias (k): 526,336 + 257 k floats.  The forward is the inference arithmetic: kernels and recurrent kernels rounded
+ * to fp16 at every call as b2o_load_crnn packs them, fp32 accumulation, h rounded to fp16 between steps, go_backwards
+ * outputs kept in processing order (recognition.py:298-319), l1 = fp16(hf + hb), l2 = [h11f, h11b], steps 0 and 1
+ * discarded before fc_12.  grad_dev (same layout) receives the batch means of dW = x^T dz, dU = h_prev^T dz, db = sum dz
+ * of the four directions by backpropagation through time (fp16 roundings taken as the identity; the gradient of l1 at
+ * processing step s goes to step s of both lstm_10 and lstm_10_back, lstm_11_back's input gradient lands at time 49 - s)
+ * and fc_12's gradients as b2o_ctc_loss_grad forms them.  Fixed-order sums, no atomics: bit-identical run to run.
+ * grad_dev NULL: the loss only.  ws_bytes >= b2o_rnn_train_workspace_bytes(b, k) always.  The workspace holds, in this
+ * order, each slot rounded up to 256 bytes: W^T (4, 512, 128) fp16, U (4, 128, 512) fp16, xw then dz (4, b, 50, 512) f32
+ * (processing order), acts (4, b, 50, 5, 128) f32 = i, f, g = tanh(z_c), o, c per processing step, hf / hb (2, b, 50, 128)
+ * fp16, l1 (b, 50, 128) fp16, l2 (b, 50, 256) fp16, dL/dl2 (b, 50, 256) f32, dL/dl1 (b, 50, 128) f32, the split-K
+ * partials ((b + 15) / 16, 526336) f32, and b2o_ctc_train_workspace_bytes(b, k) for the CTC, which starts with dL/dlogits
+ * (b, 48, k) f32.  2 <= k <= B2O_MAX_CLASSES, 0 <= dropout < 1, otherwise B2O_ERR_ARG.                             */
+int b2o_crnn_sequence_features(b2o_ctx* ctx, const void* crnn_in_dev, int b, void* out_dev, void* ws_dev,
+                               size_t ws_bytes, void* stream);
+size_t b2o_rnn_train_workspace_bytes(int b, int k);
+int b2o_rnn_loss_grad(b2o_ctx* ctx, const void* x_dev, int n_rows, const int32_t* index_dev, int b, int k,
+                      const float* params_dev, const int32_t* offsets_dev, const int16_t* labels_dev, float dropout,
+                      uint64_t seed, uint64_t step, float* loss_dev, float* grad_dev, void* ws_dev, size_t ws_bytes,
+                      void* stream);
+
 /* Result records of Pipeline.recognize for the multi-GPU gather (pipeline.py:66-75; SURVEY.md 8(e)): one
  * fixed-size float32 row per image = [count][rec_boxes x (4,2) boxes * inv_scale[i] (tools.adjust_boxes,
  * tools.py:232-260)][rec_boxes x 48 labels as int8, -1 padded], b2o_record_floats(rec_boxes) floats long.

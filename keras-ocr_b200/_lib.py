@@ -101,6 +101,10 @@ SIGNATURES = {
                                _vp, _vp, _vp, _sz, _vp]),
     "b2o_rmsprop_step": (_i, [_vp, _vp, _vp, _vp, _c.c_int64, _f, _f, _f, _vp]),
     "b2o_crnn_set_top": (_i, [_vp, _vp, _vp, _i, _vp]),
+    "b2o_crnn_sequence_features": (_i, [_vp, _vp, _i, _vp, _vp, _sz, _vp]),
+    "b2o_rnn_train_workspace_bytes": (_sz, [_i, _i]),
+    "b2o_rnn_loss_grad": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _f, _c.c_uint64, _c.c_uint64, _vp, _vp, _vp,
+                               _sz, _vp]),
     "b2o_set_debug_taps": (_i, [_vp, _i]),
     "b2o_crnn_tap": (_i, [_vp, _c.c_char_p, _vp, _i, _vp, _sz, _vp]),
     "b2o_conv2d_test": (_i, [_vp, _vp, _i, _i, _i, _i, _c.POINTER(_c.c_float), _i, _i, _i,
@@ -358,6 +362,19 @@ class Context:
 
     def crnn_set_top(self, w, bias, k, stream):
         self._check(self.lib.b2o_crnn_set_top(self.handle, w, bias, k, stream), "b2o_crnn_set_top")
+
+    def crnn_sequence_features(self, crnn_in, b, out, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_crnn_sequence_features(self.handle, crnn_in, b, out, ws, ws_bytes, stream),
+                    "b2o_crnn_sequence_features")
+
+    def rnn_train_workspace_bytes(self, b, k):
+        return int(self.lib.b2o_rnn_train_workspace_bytes(b, k))
+
+    def rnn_loss_grad(self, x, n_rows, index, b, k, params, offsets, labels, dropout, seed, step, loss, grad, ws,
+                      ws_bytes, stream):
+        self._check(self.lib.b2o_rnn_loss_grad(self.handle, x, n_rows, index, b, k, params, offsets, labels,
+                                               float(dropout), int(seed), int(step), loss, grad, ws, ws_bytes, stream),
+                    "b2o_rnn_loss_grad")
 
     def set_debug_taps(self, on):
         self._check(self.lib.b2o_set_debug_taps(self.handle, int(on)), "b2o_set_debug_taps")

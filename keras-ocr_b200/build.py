@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb2ocr.so")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "boxes.cu", "image.cu", "crnn_tail.cu", "ctc_beam.cu", "ctc_lexicon.cu",
-           "jpeg.cu", "rotation.cu", "ctc_align.cu", "ctc_train.cu"]
+           "jpeg.cu", "rotation.cu", "ctc_align.cu", "ctc_train.cu", "rnn_train.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
@@ -27,6 +27,7 @@ def _newer(a, b):
 def _compile(src):
     obj = os.path.join(CSRC, src.replace(".cu", ".o"))
     deps = [os.path.join(CSRC, src), os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "ctc_q.cuh"),
+            os.path.join(CSRC, "ctc_dropout.cuh"),
             os.path.join(os.path.dirname(HERE), "include", "b2ocr.h")]
     if not any(_newer(d, obj) for d in deps):
         return src, 0, ""

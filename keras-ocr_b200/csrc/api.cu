@@ -23,10 +23,14 @@ int ctc_lexicon_run(b2o_ctx* ctx, const float* logits, int B, int K, const int* 
 int ctc_align_run(b2o_ctx* ctx, const float* logits, int B, int K, const int32_t* labels, int P, int32_t* spans,
                   float* logp, cudaStream_t st);
 size_t ctc_train_workspace_bytes(int B, int K);
-int ctc_loss_grad_run(b2o_ctx* ctx, const __half* features, int n_rows, const int* index, int B, int K, const float* w,
-                      const float* bias, const int* offsets, const short* labels, float rate, uint64_t seed,
-                      uint64_t step, float* loss, float* grad_w, float* grad_b, float* logits, void* ws,
-                      cudaStream_t st);
+int ctc_loss_grad_run(b2o_ctx* ctx, const __half* features, long long feat_stride, bool feat_by_batch, int n_rows,
+                      const int* index, int B, int K, const float* w, const float* bias, const int* offsets,
+                      const short* labels, float rate, uint64_t seed, uint64_t step, float* loss, float* grad_w,
+                      float* grad_b, float* logits, void* ws, cudaStream_t st);
+size_t rnn_train_workspace_bytes(int B, int K);
+int rnn_loss_grad_run(b2o_ctx* ctx, const __half* x, int n_rows, const int* index, int B, int K, const float* params,
+                      const int* offsets, const short* labels, float rate, uint64_t seed, uint64_t step, float* loss,
+                      float* grad, void* ws, cudaStream_t st);
 int rmsprop_run(b2o_ctx* ctx, float* param, const float* grad, float* acc, long long n, float lr, float rho, float eps,
                 cudaStream_t st);
 
@@ -718,13 +722,17 @@ namespace {
 // The CRNN through fc_12 + greedy CTC.  keep_logits: the fp32 logits always go to the workspace's logits slot (the beam
 // search reads them there); otherwise only with the debug taps on.  features (b2o_crnn_features): the forward stops
 // after the BiLSTM and copies its 48 kept steps (b, 48, 256) fp16 there instead of running fc_12 + CTC (labels unused).
+// seq (b2o_crnn_sequence_features): the forward stops after fc_9 and copies it, (b, 50, 128) fp16, there.
 int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, float* logp, bool keep_logits, void* ws,
-                 size_t ws_bytes, void* stream, __half* features = nullptr) {
+                 size_t ws_bytes, void* stream, __half* features = nullptr, __half* seq = nullptr) {
   if (!ctx) return B2O_ERR_ARG;
   if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_forward: CRNN weights not loaded"); return B2O_ERR_STATE; }
   DeviceGuard guard(ctx->device);
   if (b == 0) return B2O_OK;
-  if (!crnn_in || (!labels && !features) || !ws || b < 0) { ctx->set_error("b2o_crnn_forward: bad argument"); return B2O_ERR_ARG; }
+  if (!crnn_in || (!labels && !features && !seq) || !ws || b < 0) {
+    ctx->set_error("b2o_crnn_forward: bad argument");
+    return B2O_ERR_ARG;
+  }
   const CrnnPlan p = plan_crnn(b);
   if (ws_bytes < p.bytes) { ctx->set_error("b2o_crnn_forward: workspace too small"); return B2O_ERR_WORKSPACE; }
   ctx->crnn_written = 0;      // from here on the slots hold neither the last forward's values nor this one's
@@ -735,11 +743,11 @@ int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, floa
   auto L = [&](const char* name) -> const ConvLayer& { return ctx->crnn[name]; };
   // the slots this forward writes, recorded on success for b2o_crnn_tap / b2o_crnn_align
   auto bit = [](rb::Id i) { return 1u << i; };
-  const bool logits_kept = !features && (keep_logits || ctx->debug_taps);
+  const bool logits_kept = !features && !seq && (keep_logits || ctx->debug_taps);
   const uint32_t wrote = bit(rb::x1) | bit(rb::x2) | (conv_pool_fused(ctx, L("conv_3")) ? 0u : bit(rb::x3)) | bit(rb::p3) |
                          bit(rb::x4) | (conv_pool_fused(ctx, L("conv_5")) ? 0u : bit(rb::x5)) | bit(rb::p5) | bit(rb::x6) |
                          bit(rb::features) | (ctx->crnn_stn ? bit(rb::theta) | bit(rb::warped) : 0u) | bit(rb::fc_9) |
-                         bit(rb::l1) | bit(rb::l2) | (logits_kept ? bit(rb::logits) : 0u);
+                         (seq ? 0u : bit(rb::l1) | bit(rb::l2)) | (logits_kept ? bit(rb::logits) : 0u);
   auto record = [&]() {
     ctx->crnn_ws = ws; ctx->crnn_b = b; ctx->crnn_written = wrote;
     return B2O_OK;
@@ -778,6 +786,11 @@ int crnn_forward(b2o_ctx* ctx, const void* crnn_in, int b, int32_t* labels, floa
   // reshape + fc_9 (282-290)
   const TensorView seq_in = make_view(warped, 1, 1, b * 50, 3584), fc9 = V(rb::fc_9, 1, 1, b * 50, 128);
   B2O_RETURN_IF(conv_run(ctx, L("fc_9"), seq_in, fc9, 0, st));
+  if (seq) {
+    B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(seq, fc9.ptr, static_cast<size_t>(b) * 50 * 128 * sizeof(__half),
+                                        cudaMemcpyDeviceToDevice, st));
+    return record();
+  }
   // BiLSTM (292-319)
   const TensorView xw1 = V(rb::xw1, 1, 1, b * 50, 1024);
   TensorView xw1v = xw1;      // fp32 output: the view's pointer arithmetic is done by the engine in floats
@@ -951,8 +964,9 @@ extern "C" int b2o_ctc_loss_grad(b2o_ctx* ctx, const void* features, int n_rows,
     return B2O_ERR_WORKSPACE;
   }
   DeviceGuard guard(ctx->device);
-  return ctc_loss_grad_run(ctx, reinterpret_cast<const __half*>(features), n_rows, index, b, k, w, bias, offsets, labels,
-                           dropout, seed, step, loss, grad_w, grad_b, logits, ws, reinterpret_cast<cudaStream_t>(stream));
+  return ctc_loss_grad_run(ctx, reinterpret_cast<const __half*>(features), 48 * 256, false, n_rows, index, b, k, w, bias,
+                           offsets, labels, dropout, seed, step, loss, grad_w, grad_b, logits, ws,
+                           reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b2o_rmsprop_step(b2o_ctx* ctx, float* param, const float* grad, float* acc, int64_t n, float lr, float rho,
@@ -978,6 +992,42 @@ extern "C" int b2o_crnn_set_top(b2o_ctx* ctx, const float* w, const float* bias,
   B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->fc12_w, w, static_cast<size_t>(256) * k * sizeof(float), cudaMemcpyDeviceToDevice, st));
   B2O_CUDA_CHECK(ctx, cudaMemcpyAsync(ctx->fc12_b, bias, static_cast<size_t>(k) * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return B2O_OK;
+}
+
+extern "C" int b2o_crnn_sequence_features(b2o_ctx* ctx, const void* crnn_in, int b, void* out, void* ws, size_t ws_bytes,
+                                          void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (b > 0 && !out) { ctx->set_error("b2o_crnn_sequence_features: bad argument"); return B2O_ERR_ARG; }
+  return crnn_forward(ctx, crnn_in, b, nullptr, nullptr, false, ws, ws_bytes, stream, nullptr,
+                      reinterpret_cast<__half*>(out));
+}
+
+extern "C" size_t b2o_rnn_train_workspace_bytes(int b, int k) {
+  if (b <= 0 || k < 2 || k > B2O_MAX_CLASSES) return 0;
+  return rnn_train_workspace_bytes(b, k);
+}
+
+extern "C" int b2o_rnn_loss_grad(b2o_ctx* ctx, const void* x, int n_rows, const int32_t* index, int b, int k,
+                                 const float* params, const int32_t* offsets, const int16_t* labels, float dropout,
+                                 uint64_t seed, uint64_t step, float* loss, float* grad, void* ws, size_t ws_bytes,
+                                 void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  const char* fn = "b2o_rnn_loss_grad";
+  if (k < 2 || k > B2O_MAX_CLASSES) { ctx->set_error(std::string(fn) + ": k must be in [2, 1024]"); return B2O_ERR_ARG; }
+  if (!(dropout >= 0.f && dropout < 1.f)) { ctx->set_error(std::string(fn) + ": dropout must be in [0, 1)"); return B2O_ERR_ARG; }
+  if (b < 0 || (b > 0 && (!x || n_rows <= 0 || !params || !offsets || !labels || !loss)) ||
+      (reinterpret_cast<uintptr_t>(x) & 15)) {
+    ctx->set_error(std::string(fn) + ": bad argument");
+    return B2O_ERR_ARG;
+  }
+  if (b == 0) return B2O_OK;
+  if (!ws || ws_bytes < rnn_train_workspace_bytes(b, k)) {
+    ctx->set_error(std::string(fn) + ": workspace too small");
+    return B2O_ERR_WORKSPACE;
+  }
+  DeviceGuard guard(ctx->device);
+  return rnn_loss_grad_run(ctx, reinterpret_cast<const __half*>(x), n_rows, index, b, k, params, offsets, labels, dropout,
+                           seed, step, loss, grad, ws, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths, int32_t* spans_dev,

@@ -44,9 +44,12 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "ctc_dropout.cuh"
 #include "ctc_q.cuh"
 
 using ctcq::kT;
+using ctcdrop::Dropout;
+using ctcdrop::kept;
 
 namespace {
 
@@ -56,24 +59,16 @@ constexpr int kMaxLabelEnd = 1 << 24;
 constexpr int kChunkRows = 16 * kT;                // split-K chunk: 16 crops
 constexpr int kTile = 64, kSub = 32;               // grad_partial_kernel: 64 x 64 outputs, 32 rows per stage
 
-__host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
-struct Dropout {
-  uint64_t key0;
-  unsigned thr;       // keep iff hash >> 40 >= thr
-  float scale;
-  bool on;
+// Where crop b's 48 x 256 features start: at row index[b] of an (n_rows, 48, 256) cache (fit_top), or, by_batch, at
+// entry b of the batch's own rows `stride` halves apart (the recurrent training's l2, whose 48 kept steps lie inside a
+// 50-step row).  Either way the dropout mask stays keyed on the dataset row index[b].
+struct FeatRows {
+  long long stride;
+  bool by_batch;
+  __device__ __forceinline__ size_t of(int b, int row) const {
+    return static_cast<size_t>(by_batch ? b : row) * static_cast<size_t>(stride);
+  }
 };
-
-__device__ __forceinline__ bool kept(const Dropout& d, int row, int t, int c) {
-  const uint64_t k = static_cast<uint64_t>(row) * (kT * kFeat) + static_cast<uint64_t>(t * kFeat + c);
-  return static_cast<unsigned>(mix64(d.key0 ^ k) >> 40) >= d.thr;
-}
 
 // The feature value x' the logits and grad_W use.
 __device__ __forceinline__ float feat_value(const __half h, bool keep, const Dropout& d) {
@@ -94,7 +89,7 @@ struct LossSmem {
 
 template <bool DROP>
 __global__ void __launch_bounds__(kThreads)
-ctc_loss_kernel(const __half* __restrict__ features /*[n_rows][48][256]*/, int n_rows, const int* __restrict__ index,
+ctc_loss_kernel(const __half* __restrict__ features, FeatRows fr, int n_rows, const int* __restrict__ index,
                 int K, const float* __restrict__ w /*[256][K]*/, const float* __restrict__ bias,
                 const int* __restrict__ offsets, const short* __restrict__ labels, Dropout drop,
                 float* __restrict__ loss, float* __restrict__ g /*[B][48][K] or null*/,
@@ -149,7 +144,7 @@ ctc_loss_kernel(const __half* __restrict__ features /*[n_rows][48][256]*/, int n
   }
   // ---- features (and the dropout mask) into shared memory
   {
-    const uint4* src = reinterpret_cast<const uint4*>(features + static_cast<size_t>(row) * kT * kFeat);
+    const uint4* src = reinterpret_cast<const uint4*>(features + fr.of(b, row));
     uint4* dst = reinterpret_cast<uint4*>(xs);
     for (int i = tid; i < kT * kFeat / 8; i += kThreads) dst[i] = src[i];
     if (DROP) {
@@ -358,7 +353,7 @@ ctc_loss_kernel(const __half* __restrict__ features /*[n_rows][48][256]*/, int n
 // partial[chunk][c][k] = sum over the chunk's rows r (ascending) of x'[r][c] g[r][k], one 64 x 64 tile per CTA.
 template <bool DROP>
 __global__ void __launch_bounds__(256)
-grad_partial_kernel(const __half* __restrict__ features, int n_rows, const int* __restrict__ index, int B, int K,
+grad_partial_kernel(const __half* __restrict__ features, FeatRows fr, int n_rows, const int* __restrict__ index, int B, int K,
                     const float* __restrict__ g, Dropout drop, float* __restrict__ partial) {
   __shared__ float xs[kSub][kTile], gs[kSub][kTile];
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -379,7 +374,7 @@ grad_partial_kernel(const __half* __restrict__ features, int n_rows, const int* 
         if (row >= 0 && row < n_rows) {
           const int c = c0 + cc;
           const bool keep = DROP ? kept(drop, row, t, c) : true;
-          xv = feat_value(features[(static_cast<size_t>(row) * kT + t) * kFeat + c], keep, drop);
+          xv = feat_value(features[fr.of(bi, row) + static_cast<size_t>(t) * kFeat + c], keep, drop);
         }
         const int k = k0 + cc;
         if (k < K) gv = g[static_cast<size_t>(r) * K + k];
@@ -451,22 +446,19 @@ size_t ctc_train_workspace_bytes(int B, int K) {
 
 size_t ctc_train_smem_bytes(int K) { return LossSmem::bytes(K); }
 
-int ctc_loss_grad_run(b2o_ctx* ctx, const __half* features, int n_rows, const int* index, int B, int K, const float* w,
-                      const float* bias, const int* offsets, const short* labels, float rate, uint64_t seed,
-                      uint64_t step, float* loss, float* grad_w, float* grad_b, float* logits, void* ws,
-                      cudaStream_t st) {
-  Dropout d;
-  d.on = rate > 0.f;
-  d.key0 = mix64(mix64(seed) ^ step);
-  d.thr = static_cast<unsigned>(static_cast<double>(rate) * 16777216.0);
-  d.scale = 1.0f / (1.0f - rate);
+int ctc_loss_grad_run(b2o_ctx* ctx, const __half* features, long long feat_stride, bool feat_by_batch, int n_rows,
+                      const int* index, int B, int K, const float* w, const float* bias, const int* offsets,
+                      const short* labels, float rate, uint64_t seed, uint64_t step, float* loss, float* grad_w,
+                      float* grad_b, float* logits, void* ws, cudaStream_t st) {
+  const Dropout d = ctcdrop::make_dropout(rate, seed, step);
+  const FeatRows fr = {feat_stride, feat_by_batch};
   const bool grads = grad_w != nullptr;
   uint8_t* base = reinterpret_cast<uint8_t*>(ws);
   float* g = grads ? reinterpret_cast<float*>(base) : nullptr;
   const size_t smem = LossSmem::bytes(K);
   auto kern = d.on ? ctc_loss_kernel<true> : ctc_loss_kernel<false>;
   B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  kern<<<B, kThreads, smem, st>>>(features, n_rows, index, K, w, bias, offsets, labels, d, loss, g, logits);
+  kern<<<B, kThreads, smem, st>>>(features, fr, n_rows, index, K, w, bias, offsets, labels, d, loss, g, logits);
   B2O_LAUNCH_CHECK(ctx);
   if (!grads) return B2O_OK;
   const int nch = chunks_of(B);
@@ -474,8 +466,8 @@ int ctc_loss_grad_run(b2o_ctx* ctx, const __half* features, int n_rows, const in
   float* partial_b = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(partial) +
                                               align256(static_cast<size_t>(nch) * kFeat * K * 4));
   const dim3 grid((K + kTile - 1) / kTile, kFeat / kTile, nch);
-  if (d.on) grad_partial_kernel<true><<<grid, 256, 0, st>>>(features, n_rows, index, B, K, g, d, partial);
-  else grad_partial_kernel<false><<<grid, 256, 0, st>>>(features, n_rows, index, B, K, g, d, partial);
+  if (d.on) grad_partial_kernel<true><<<grid, 256, 0, st>>>(features, fr, n_rows, index, B, K, g, d, partial);
+  else grad_partial_kernel<false><<<grid, 256, 0, st>>>(features, fr, n_rows, index, B, K, g, d, partial);
   B2O_LAUNCH_CHECK(ctx);
   bias_partial_kernel<<<dim3((K + 127) / 128, nch), 128, 0, st>>>(g, B, K, partial_b);
   B2O_LAUNCH_CHECK(ctx);

@@ -628,10 +628,12 @@ class Recognizer:
                              f"{', 3' if self.color else ''}), got {shape}")
         return crops
 
-    def _features(self, crops, chunk=512):
-        """``b2o_crnn_features`` of every crop, in chunks that bound the CRNN workspace: (N,48,256) fp16 CUDA."""
+    def _features(self, crops, chunk=512, sequence=False):
+        """``b2o_crnn_features`` of every crop, in chunks that bound the CRNN workspace: (N,48,256) fp16 CUDA; with
+        ``sequence``, ``b2o_crnn_sequence_features`` (fc_9's output): (N,50,128)."""
         n = int(crops.shape[0])
-        feats = torch.empty((n, STEPS, 256), dtype=torch.float16, device=self.device)
+        feats = torch.empty((n,) + ((50, 128) if sequence else (STEPS, 256)), dtype=torch.float16, device=self.device)
+        run = self.ctx.crnn_sequence_features if sequence else self.ctx.crnn_features
         stream = torch.cuda.current_stream(self.device).cuda_stream
         nbytes = self.ctx.crnn_workspace_bytes(min(chunk, n))
         ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
@@ -643,7 +645,7 @@ class Recognizer:
             b = t.shape[0]
             x = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + tail, dtype=torch.float16, device=self.device)
             self.ctx.crops_to_input(t.data_ptr(), b, x.data_ptr(), stream, color=self.color)
-            self.ctx.crnn_features(x.data_ptr(), b, feats[i:i + b].data_ptr(), ws.data_ptr(), nbytes, stream)
+            run(x.data_ptr(), b, feats[i:i + b].data_ptr(), ws.data_ptr(), nbytes, stream)
         return feats
 
     def _batch_targets(self, offsets, labels, idx):
@@ -668,23 +670,9 @@ class Recognizer:
                                    None, 0, stream)
         return float(loss.cpu().numpy().astype(np.float64).mean())
 
-    def fit_top(self, crops, texts, epochs=1, batch_size=64, learning_rate=1e-3, dropout=0.25, seed=0, validation=None):
-        """Train the output layer (``fc_12``, Dense 256 -> len(alphabet) + 1 with bias) on labelled word crops, the rest
-        of the CRNN frozen -- the reference's fine-tuning workflow (``compile()`` + ``training_model``,
-        recognition.py:334-349, 539-545) restricted to the top.  ``crops``: (N,31,200) uint8 -- (N,31,200,3) for a color
-        recognizer -- as ``recognize_crops`` takes them; ``texts``: N strings over the alphabet (``check_texts``).
-        ``validation``: an optional (crops, texts) pair.
-
-        The BiLSTM features of every crop are computed once (``b2o_crnn_features``) and kept on the device, 24.6 kB per
-        crop.  Each epoch shuffles them with ``np.random.default_rng(seed)`` and runs, per batch, the Keras
-        ``ctc_batch_cost`` loss and its gradient (``b2o_ctc_loss_grad``; Dropout(``dropout``) before the layer, as in
-        the reference's graph) and one RMSprop step (``b2o_rmsprop_step``, Keras' defaults rho 0.9, eps 1e-7).  Training
-        starts from the current top: the re-initialised one for a new alphabet, the checkpoint's otherwise.  At the end
-        the new top is installed (``b2o_crnn_set_top``), so every recognition path uses it.  Same seed and inputs give
-        bit-identical weights.
-
-        Returns {"loss": [...], "val_loss": [...]}: per epoch the mean L_b over the training crops (as they were seen,
-        with dropout) and over the validation crops (without dropout, after the epoch; empty without ``validation``)."""
+    def _fit_args(self, crops, texts, epochs, batch_size, learning_rate, dropout, seed, validation):
+        """The argument checks of ``fit_top`` and ``fit_recurrent``, all made before anything runs on the device:
+        (CSR offsets, labels, N, crops, validation as (crops, offsets, labels) or None)."""
         def is_int(v):
             return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
         offsets, labels = check_texts(texts, self.alphabet)
@@ -711,6 +699,27 @@ class Recognizer:
             if v_crops.shape[0] != len(v_off) - 1:
                 raise ValueError(f"{v_crops.shape[0]} validation crops but {len(v_off) - 1} texts")
             val = (v_crops, v_off, v_lab)
+        return offsets, labels, n, crops, val
+
+    def fit_top(self, crops, texts, epochs=1, batch_size=64, learning_rate=1e-3, dropout=0.25, seed=0, validation=None):
+        """Train the output layer (``fc_12``, Dense 256 -> len(alphabet) + 1 with bias) on labelled word crops, the rest
+        of the CRNN frozen -- the reference's fine-tuning workflow (``compile()`` + ``training_model``,
+        recognition.py:334-349, 539-545) restricted to the top.  ``crops``: (N,31,200) uint8 -- (N,31,200,3) for a color
+        recognizer -- as ``recognize_crops`` takes them; ``texts``: N strings over the alphabet (``check_texts``).
+        ``validation``: an optional (crops, texts) pair.
+
+        The BiLSTM features of every crop are computed once (``b2o_crnn_features``) and kept on the device, 24.6 kB per
+        crop.  Each epoch shuffles them with ``np.random.default_rng(seed)`` and runs, per batch, the Keras
+        ``ctc_batch_cost`` loss and its gradient (``b2o_ctc_loss_grad``; Dropout(``dropout``) before the layer, as in
+        the reference's graph) and one RMSprop step (``b2o_rmsprop_step``, Keras' defaults rho 0.9, eps 1e-7).  Training
+        starts from the current top: the re-initialised one for a new alphabet, the checkpoint's otherwise.  At the end
+        the new top is installed (``b2o_crnn_set_top``), so every recognition path uses it.  Same seed and inputs give
+        bit-identical weights.
+
+        Returns {"loss": [...], "val_loss": [...]}: per epoch the mean L_b over the training crops (as they were seen,
+        with dropout) and over the validation crops (without dropout, after the epoch; empty without ``validation``)."""
+        offsets, labels, n, crops, val = self._fit_args(crops, texts, epochs, batch_size, learning_rate, dropout, seed,
+                                                        validation)
         k = len(self.alphabet) + 1
         stream = torch.cuda.current_stream(self.device).cuda_stream
         feats = self._features(crops)
@@ -748,6 +757,83 @@ class Recognizer:
         self._tensors = dict(self._tensors)
         self._tensors["fc_12.kernel"] = w.cpu().numpy()
         self._tensors["fc_12.bias"] = bias.cpu().numpy()
+        return history
+
+    # ------------------------------------------------------------------ fine-tuning the recurrent head
+    RNN_LAYERS = ("lstm_10", "lstm_10_back", "lstm_11", "lstm_11_back")
+    _RNN_PARTS = (("kernel", (128, 512)), ("recurrent_kernel", (128, 512)), ("bias", (512,)))
+
+    def _rnn_tensor_names(self):
+        """The 14 tensors ``fit_recurrent`` trains, in the order of ``b2o_rnn_loss_grad``'s parameter vector."""
+        k = len(self.alphabet) + 1
+        names = [(f"{layer}.{part}", shape) for layer in self.RNN_LAYERS for part, shape in self._RNN_PARTS]
+        return names + [("fc_12.kernel", (256, k)), ("fc_12.bias", (k,))]
+
+    def fit_recurrent(self, crops, texts, epochs=1, batch_size=64, learning_rate=1e-3, dropout=0.25, seed=0,
+                      validation=None):
+        """Fine-tune the BiLSTM (``lstm_10``, ``lstm_10_back``, ``lstm_11``, ``lstm_11_back``: kernel, recurrent kernel
+        and bias of each) together with the output layer ``fc_12`` -- the reference's fine-tuning workflow
+        (``compile()`` + ``training_model``, recognition.py:334-349, 539-545) with the convolutions, the STN and
+        ``fc_9`` frozen.  Arguments, checks and the returned history are those of ``fit_top``.
+
+        The ``fc_9`` output of every crop is computed once (``b2o_crnn_sequence_features``) and kept on the device,
+        12.8 kB per crop.  Each batch runs the BiLSTM forward with the inference arithmetic, the CTC loss and
+        backpropagation through time (``b2o_rnn_loss_grad``), then one Keras RMSprop step (momentum 0, rho 0.9,
+        eps 1e-7) on fp32 master weights of all 14 tensors (``b2o_rmsprop_step``).  At the end the trained tensors
+        replace this recognizer's and the CRNN is reloaded from them, so it equals ``Recognizer(alphabet,
+        weights=<save_weights file>)`` bit for bit.  Same seed and inputs give bit-identical weights."""
+        offsets, labels, n, crops, val = self._fit_args(crops, texts, epochs, batch_size, learning_rate, dropout, seed,
+                                                        validation)
+        k = len(self.alphabet) + 1
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        seq = self._features(crops, sequence=True)
+        v_seq = self._features(val[0], sequence=True) if val is not None else None
+        names = self._rnn_tensor_names()
+        params = torch.from_numpy(np.concatenate(
+            [np.ascontiguousarray(self._tensors[name], np.float32).reshape(-1) for name, _ in names])).to(self.device)
+        acc, grad = torch.zeros_like(params), torch.empty_like(params)
+        bs = min(int(batch_size), n)
+        nbytes = self.ctx.rnn_train_workspace_bytes(bs, k)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        loss = torch.empty(n, dtype=torch.float32, device=self.device)
+
+        def mean_loss(x, off, lab):
+            m = x.shape[0]
+            out = torch.empty(m, dtype=torch.float32, device=self.device)
+            for i in range(0, m, bs):
+                idx = np.arange(i, min(m, i + bs), dtype=np.int32)
+                o, lb = self._batch_targets(off, lab, idx)
+                index = torch.from_numpy(idx).to(self.device)
+                self.ctx.rnn_loss_grad(x.data_ptr(), m, index.data_ptr(), len(idx), k, params.data_ptr(), o.data_ptr(),
+                                       lb.data_ptr(), 0.0, 0, 0, out[i:].data_ptr(), None, ws.data_ptr(), nbytes, stream)
+            return float(out.cpu().numpy().astype(np.float64).mean())
+
+        rng = np.random.default_rng(seed)
+        history = {"loss": [], "val_loss": []}
+        step = 0
+        for _ in range(epochs):
+            perm = rng.permutation(n).astype(np.int32)
+            for i in range(0, n, bs):
+                idx = perm[i:i + bs]
+                off, lab = self._batch_targets(offsets, labels, idx)
+                index = torch.from_numpy(idx).to(self.device)
+                self.ctx.rnn_loss_grad(seq.data_ptr(), n, index.data_ptr(), len(idx), k, params.data_ptr(),
+                                       off.data_ptr(), lab.data_ptr(), dropout, seed, step, loss[i:].data_ptr(),
+                                       grad.data_ptr(), ws.data_ptr(), nbytes, stream)
+                self.ctx.rmsprop_step(params.data_ptr(), grad.data_ptr(), acc.data_ptr(), params.numel(), learning_rate,
+                                      0.9, 1e-7, stream)
+                step += 1
+            history["loss"].append(float(loss.cpu().numpy().astype(np.float64).mean()))
+            if val is not None:
+                history["val_loss"].append(mean_loss(v_seq, val[1], val[2]))
+        host = params.cpu().numpy()
+        tensors, at = dict(self._tensors), 0
+        for name, shape in names:
+            size = int(np.prod(shape))
+            tensors[name] = host[at:at + size].reshape(shape).copy()
+            at += size
+        self.ctx.load_crnn(tensors)
+        self._tensors = tensors
         return history
 
     def save_weights(self, path):
