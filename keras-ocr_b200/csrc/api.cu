@@ -354,6 +354,7 @@ extern "C" int b2o_create(int device, b2o_ctx** out) {
   if (const char* e = getenv("B2O_TC_AFF")) ctx->tc_aff_const = std::string(e) != "smem";
   if (const char* e = getenv("B2O_GLUE")) ctx->glue_v1 = std::string(e) == "v1";
   if (const char* e = getenv("B2O_FUSED_TAIL")) ctx->no_fused_tail = atoi(e) == 0;      // 0: separate head_tail_kernel (A/B, tests)
+  if (const char* e = getenv("B2O_TC_SWAP")) ctx->tc_swap = atoi(e) != 0;               // 0: 64-channel layers as pixels x channels (A/B, tests)
   if (const char* e = getenv("B2O_TC_PAIR")) {        // default 0 = single-CTA tiles; 1 = pairs on halo tiles; 2 = generic tiles too
     ctx->tc_pair = atoi(e) != 0;
     ctx->tc_pair_generic = atoi(e) == 2;

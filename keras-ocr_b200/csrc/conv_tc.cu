@@ -21,7 +21,8 @@
 //   per k step (tile rows 0-63 and 64-127) with fp32 accumulators in registers, then the epilogue straight from those
 //   registers: scale/shift/ReLU/affine -> fp16|fp32 NHWC stores (possibly into a channel slice of a concat buffer) and,
 //   optionally, the fused 2x2 max-pool output or CRAFT tail.  The two warpgroups take turns on the main loop, so one
-//   runs its epilogue while the other keeps the tensor cores busy.
+//   runs its epilogue while the other keeps the tensor cores busy.  64-channel fp16 layers run transposed (p.ct,
+//   see conv_tc_body): one m64 (channels) x n128 (pixels) x k16 wgmma per k step and TMA-stored outputs.
 // * persistent: grid = min(#tiles, #SMs); n-tiles of one pixel tile run back to back.
 #include <stdlib.h>
 #include <string.h>
@@ -51,6 +52,8 @@ struct TcParams {
   int a_bytes, a_stride;                  // bytes one A box delivers / offset of a stage's B boxes
   int stage_bytes, stage_tx;              // bytes between stages / bytes a stage's barrier expects
   int off_res, off_bar;                   // shared-memory offsets: resident filter bank, barriers
+  int ct;                                 // channels by pixels (64-channel fp16 layers, see conv_tc_body)
+  int off_out;                            // ct: the two warpgroups' output tiles (+ pooled tiles)
   int aff_smem;                           // epilogue constants staged in shared memory behind the barriers (B2O_TC_AFF=smem)
   int aff_const;                          // epilogue constants read from the AffConst kernel parameter (default)
   const float *s1, *t1, *s2, *t2;
@@ -125,6 +128,25 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
       " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
+}
+// ---- epilogue stores of the channels-by-pixels body: shared-memory tile -> global through TMA (bulk groups)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+          reinterpret_cast<uint64_t>(m)),
+      "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// four transposed 8x8 b16 matrices: register j of a lane holds row lane / 4, columns 2 (lane % 4) + {0, 1} of matrix j;
+// lanes 8j .. 8j + 7 give the addresses of the 8 stored rows (= the matrix's columns) of matrix j
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
 }
 // ---- CTA pairs: clusters of two CTAs share every B tile.  Each CTA loads half of the tile's rows and multicasts them
 // into the same shared-memory offset of both CTAs, signalling both CTAs' barriers at that offset.
@@ -262,10 +284,17 @@ struct AffConst {
 //       instead of once per 128; A boxes stay per CTA.  A stage may only be refilled when the consumers of BOTH CTAs have
 //       released it, so every consumer warp arrives on the empty barriers of both CTAs.  The MMAs and their order are
 //       those of the single-CTA tiles: results are bit-identical.
-template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD = false>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
-               const TcParams p, const __grid_constant__ AffConst ac) {
+// CT:   channels by pixels (p.ct), for 64-channel fp16 layers: D^T[cout, pixel] = W . X^T, the filter stage (K-major, 64 rows)
+//       as the wgmma A operand and the pixel stage (K-major, 128 rows) as B -- one m64 x n128 x k16 per k step instead
+//       of two m64 x n64 x k16 that both read the same B tile, so a k step reads 6 KB of shared memory instead of 8 KB.
+//       Every output sums the same products in the same order: results are bit-identical to the pixels-by-channels
+//       body.  A thread then holds 2 channels x 32 pixels, so the epilogue goes through a 16 KB shared-memory
+//       tile per warpgroup (stmatrix .trans) and TMA stores (omap, and pmap for the fused pool), which clip at the
+//       image edges.
+template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD, bool CT>
+__device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUtensorMap& bmap, const CUtensorMap& omap,
+                                             const CUtensorMap& pmap, const TcParams& p, const AffConst& ac) {
+  static_assert(!CT || (BLOCK_N == 64 && !PAIR && !UPADD), "channels by pixels: 64-channel single-CTA tiles");
   constexpr bool HALO = MODE >= 1, RESIDENT = MODE == 2;
   constexpr int TAPS_PER_A = HALO ? 3 : 1;                 // dy taps served by one A stage
   constexpr int B_BYTES = BLOCK_N * KCH * 2;
@@ -423,10 +452,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
             const uint64_t bdesc = desc_b0 + static_cast<uint64_t>(boff >> 4);
   #pragma unroll
             for (int k = 0; k < KSTEPS; ++k) {
+              if constexpr (CT) {
+                wgmma_f16<128>(acc, bdesc + static_cast<uint64_t>((k * 32) >> 4),
+                               adesc + static_cast<uint64_t>((t * TAP_BYTES + k * 32) >> 4), accumulate);
+              } else {
   #pragma unroll
-              for (int mh = 0; mh < 2; ++mh)
-                wgmma_f16<BLOCK_N>(acc + mh * NACC, adesc + static_cast<uint64_t>((mh * HALF_BYTES + t * TAP_BYTES + k * 32) >> 4),
-                                   bdesc + static_cast<uint64_t>((k * 32) >> 4), accumulate);
+                for (int mh = 0; mh < 2; ++mh)
+                  wgmma_f16<BLOCK_N>(acc + mh * NACC, adesc + static_cast<uint64_t>((mh * HALF_BYTES + t * TAP_BYTES + k * 32) >> 4),
+                                     bdesc + static_cast<uint64_t>((k * 32) >> 4), accumulate);
+              }
               accumulate = 1;
             }
           }
@@ -450,8 +484,72 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
 
       // ---- epilogue from the registers, one 64-row half after the other
       const int c_base = ti.c0 * BLOCK_N;
+      if constexpr (CT) {
+        // this thread holds channels r0, r0 + 8 (hh = 0, 1) x pixels 8i + 2q, 8i + 2q + 1 (i < 16) in acc[4i + 2hh + 0, 1]:
+        // the same per-element fmaf / ReLU / fmaf and fp16 rounding as below, with per-channel scalars
+        uint32_t hv[16][2];
   #pragma unroll
-      for (int mh = 0; mh < 2; ++mh) {
+        for (int hh = 0; hh < 2; ++hh) {
+          const int c = r0 + 8 * hh;
+          const float a1 = e_s1[c], b1 = e_t1[c];
+          const float a2 = p.s2 != nullptr ? e_s2[c] : 0.0f, b2 = p.s2 != nullptr ? e_t2[c] : 0.0f;
+  #pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            float y0 = fmaf(acc[4 * i + 2 * hh], a1, b1);
+            float y1 = fmaf(acc[4 * i + 2 * hh + 1], a1, b1);
+            if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
+            if (p.s2 != nullptr) { y0 = fmaf(y0, a2, b2); y1 = fmaf(y1, a2, b2); }
+            const __half2 h2 = __floats2half2_rn(y0, y1);
+            hv[i][hh] = *reinterpret_cast<const uint32_t*>(&h2);
+          }
+        }
+        // NHWC tile [128 pixel rows][64 channels] with the 128B swizzle of omap / pmap: 16-byte chunk j of row r sits at
+        // chunk j ^ (r & 7).  An 8x8 block (8 channels x 8 pixels) stored transposed = 8 pixel rows of one chunk.
+        constexpr int OUT_TILE = 128 * 64 * 2, POOL_TILE = 32 * 64 * 2;
+        uint8_t* const otile = smem + p.off_out + wg * OUT_TILE;
+        uint8_t* const ptile = smem + p.off_out + 2 * OUT_TILE + wg * POOL_TILE;
+        const int et = threadIdx.x & 127;
+        if (et == 0) bulk_wait_read_all();                   // the previous tile's stores have read the tile
+        named_bar_sync(3 + wg, 128);
+        {
+          const int m = lane >> 3, r = lane & 7;               // this lane addresses row r of matrix m = (i & 1, hh)
+          const uint32_t row = smem_u32(otile) + static_cast<uint32_t>(r * 128 + (((2 * (warp & 3) + (m & 1)) ^ r) << 4));
+  #pragma unroll
+          for (int i0 = 0; i0 < 16; i0 += 2)
+            stmatrix_x4_trans(row + static_cast<uint32_t>((8 * (i0 + (m >> 1))) * 128), hv[i0][0], hv[i0][1],
+                              hv[i0 + 1][0], hv[i0 + 1][1]);
+        }
+        fence_proxy_async_smem();
+        named_bar_sync(3 + wg, 128);
+        if (p.pool_out != nullptr) {                           // halo tile 8 x 16 -> pooled 4 x 8, max(max(v00, v10), max(v01, v11))
+  #pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const int item = et + 128 * j, pr = item >> 3, ch = item & 7;
+            const int r00 = 2 * (pr & 3) + 16 * (pr >> 2);   // (2 pw, 2 ph) in the 8-wide tile
+            auto ld = [&](int rr) { return *reinterpret_cast<const uint4*>(otile + rr * 128 + ((ch ^ (rr & 7)) << 4)); };
+            const uint4 v00 = ld(r00), v10 = ld(r00 + 8), v01 = ld(r00 + 1), v11 = ld(r00 + 9);
+            uint4 o;
+            const __half2* a = reinterpret_cast<const __half2*>(&v00);
+            const __half2* b = reinterpret_cast<const __half2*>(&v10);
+            const __half2* c = reinterpret_cast<const __half2*>(&v01);
+            const __half2* d = reinterpret_cast<const __half2*>(&v11);
+            __half2* op = reinterpret_cast<__half2*>(&o);
+  #pragma unroll
+            for (int e = 0; e < 4; ++e) op[e] = __hmax2(__hmax2(a[e], b[e]), __hmax2(c[e], d[e]));
+            *reinterpret_cast<uint4*>(ptile + pr * 128 + ((ch ^ (pr & 7)) << 4)) = o;
+          }
+          fence_proxy_async_smem();
+          named_bar_sync(3 + wg, 128);
+        }
+        if (et == 0) {
+          const int tw0 = ti.c1 << p.bw_log2, th0 = ti.c2 << p.bh_log2, tn0 = ti.c3 << p.bn_log2;
+          if (p.write_full) tma_store_4d(&omap, otile, 0, tw0, th0, tn0);
+          if (p.pool_out != nullptr) tma_store_4d(&pmap, ptile, 0, tw0 >> 1, th0 >> 1, tn0);
+          bulk_commit();
+        }
+      }
+  #pragma unroll
+      for (int mh = 0; mh < (CT ? 0 : 2); ++mh) {
         float* const acc_h = acc + mh * NACC;
         bool valid[2];
         size_t pix[2];
@@ -591,9 +689,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
         }
       }
     }
+    if (CT && (threadIdx.x & 127) == 0) bulk_wait_all();    // the output tiles stay until the last stores are done
   }
   // neither CTA of a pair leaves while the other may still signal its barriers
   if (PAIR) cluster_sync_all();
+}
+
+// The 64-channel single-CTA instances carry both bodies and take the channels-by-pixels one when p.ct is set.
+template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD = false>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
+               const __grid_constant__ CUtensorMap omap, const __grid_constant__ CUtensorMap pmap,
+               const TcParams p, const __grid_constant__ AffConst ac) {
+  if constexpr (BLOCK_N == 64 && !PAIR && !UPADD) {
+    if (p.ct) {
+      conv_tc_body<BLOCK_N, KCH, MODE, PAIR, UPADD, true>(amap, bmap, omap, pmap, p, ac);
+      return;
+    }
+  }
+  conv_tc_body<BLOCK_N, KCH, MODE, PAIR, UPADD, false>(amap, bmap, omap, pmap, p, ac);
 }
 
 // ------------------------------------------------------------------------------------------ host
@@ -639,8 +753,8 @@ double pick_box(int N, int H, int W, int* bw_l, int* bh_l, int* bn_l) {
 thread_local const float* g_tail_host = nullptr;     // the fused tail's constants in AffConst::tail order (set by conv_tc_run)
 
 template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD = false>
-int launch(b2o_ctx* ctx, const CUtensorMap& amap, const ConvLayer& L, const TcParams& p, int smem_bytes,
-           cudaStream_t st) {
+int launch(b2o_ctx* ctx, const CUtensorMap& amap, const CUtensorMap& omap, const CUtensorMap& pmap, const ConvLayer& L,
+           const TcParams& p, int smem_bytes, cudaStream_t st) {
   static thread_local AffConst ac;                         // 16 KB: filled per launch from the layer's host copies
   if (p.aff_const) {
     const size_t nb = static_cast<size_t>(L.cout) * sizeof(float);
@@ -676,9 +790,9 @@ int launch(b2o_ctx* ctx, const CUtensorMap& amap, const ConvLayer& L, const TcPa
     attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    B2O_CUDA_CHECK(ctx, cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD>, amap, L.wmap_pair, p, ac));
+    B2O_CUDA_CHECK(ctx, cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD>, amap, L.wmap_pair, omap, pmap, p, ac));
   } else {
-    conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD><<<grid, NUM_THREADS, smem_bytes, st>>>(amap, L.wmap, p, ac);
+    conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD><<<grid, NUM_THREADS, smem_bytes, st>>>(amap, L.wmap, omap, pmap, p, ac);
   }
   B2O_LAUNCH_CHECK(ctx);
   if (ctx->profile) {
@@ -793,12 +907,17 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   const long long total = static_cast<long long>(p.tiles_w) * p.tiles_h * p.tiles_n * p.n_tiles;
   if (total > 0x7fffffffLL) { ctx->set_error("conv_tc_run: too many tiles"); return B2O_ERR_ARG; }
   p.total_tiles = static_cast<int>(total);
+  // channels by pixels for the 64-channel fp16 layers; a pool whose output has no pixel keeps the old path
+  const bool ct = ctx->tc_swap && L.cout == 64 && bn == 64 && !out_f32 && up_add == nullptr && tail == nullptr && !pair &&
+                  (!want_pool || (in.h >= 2 && in.w >= 2));
+  p.ct = ct ? 1 : 0;
 
-  // shared-memory plan: [ring of stages: A box | B boxes][resident filter bank][barriers][epilogue constants]
+  // shared-memory plan: [ring of stages: A box | B boxes][resident filter bank][ct output tiles][barriers][epilogue constants]
   p.aff_const = (ctx->tc_aff_const && L.cout <= 256 && static_cast<int>(L.h_s1.size()) == L.cout) ? 1 : 0;
   p.aff_smem = (!p.aff_const && L.cout <= 256) ? 1 : 0;
   const int aff_bytes = (p.aff_smem ? 4 * L.cout * 4 : 0) + (tail ? TAIL_FLOATS * 4 : 0);
-  const int budget = SMEM_TOTAL - 1024 /*alignment slack*/ - 512 /*barriers*/ - aff_bytes;
+  const int out_tiles = ct ? 2 * 128 * 64 * 2 + (want_pool ? 2 * 32 * 64 * 2 : 0) : 0;   // per warpgroup: 16 KB (+ 4 KB pooled)
+  const int budget = SMEM_TOTAL - 1024 /*alignment slack*/ - 512 /*barriers*/ - aff_bytes - out_tiles;
   p.a_bytes = p.halo ? 18 * 8 * kch * 2 : 128 * kch * 2;
   p.a_stride = (p.a_bytes + 1023) / 1024 * 1024;
   const long long res_bytes = static_cast<long long>(taps) * kchunks * b_bytes;
@@ -811,7 +930,8 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   if (p.ns > MAX_RING) p.ns = MAX_RING;
   if (p.ns < 2) { ctx->set_error("conv_tc_run: shared-memory plan failed for " + L.name); return B2O_ERR_ARG; }
   p.off_res = p.ns * p.stage_bytes;
-  p.off_bar = p.off_res + (p.resident ? static_cast<int>((res_bytes + 1023) / 1024 * 1024) : 0);
+  p.off_out = p.off_res + (p.resident ? static_cast<int>((res_bytes + 1023) / 1024 * 1024) : 0);
+  p.off_bar = p.off_out + out_tiles;
   int smem_bytes = p.off_bar + 512 + aff_bytes + 1024;
   // the grid is one persistent CTA per SM: a request above half of the SM's 228 KB keeps a second CTA of a small layer
   // from landing on an SM that already runs one while other SMs sit idle
@@ -855,23 +975,46 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
                    std::to_string(static_cast<int>(r)));
     return B2O_ERR_CUDA;
   }
-  if (up_add != nullptr) {                                 // generic 1x1 tiles
-    if (bn == 64) return launch<64, 64, 0, false, true>(ctx, amap, L, p, smem_bytes, st);
-    if (bn == 128) return launch<128, 64, 0, false, true>(ctx, amap, L, p, smem_bytes, st);
+  // channels-by-pixels output maps: 4-D (c, w, h, n) over the 64-channel view (a channel slice: base pointer + ld), boxes of one tile
+  CUtensorMap omap, pmap;
+  memset(&omap, 0, sizeof(omap));
+  memset(&pmap, 0, sizeof(pmap));
+  auto encode_out = [&](CUtensorMap* m, void* ptr, int ld, int n, int h, int w, const cuuint32_t* obox) {
+    cuuint64_t odims[4] = {64, static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h), static_cast<cuuint64_t>(n)};
+    cuuint64_t ostr[3] = {static_cast<cuuint64_t>(ld) * 2, static_cast<cuuint64_t>(ld) * 2 * w,
+                          static_cast<cuuint64_t>(ld) * 2 * w * h};
+    return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, ptr, odims, ostr, obox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  };
+  if (ct && write_full) {
+    const cuuint32_t obox[4] = {64, 1u << p.bw_log2, 1u << p.bh_log2, 1u << p.bn_log2};
+    r = encode_out(&omap, out.ptr, out.ld, in.n, in.h, in.w, obox);
   }
-#define B2O_TC_PAIR_CASE(BN)                                                           \
-  if (pair && bn == BN) {                                                              \
-    if (p.resident) return launch<BN, 64, 2, true>(ctx, amap, L, p, smem_bytes, st);   \
-    if (p.halo) return launch<BN, 64, 1, true>(ctx, amap, L, p, smem_bytes, st);       \
-    return launch<BN, 64, 0, true>(ctx, amap, L, p, smem_bytes, st);                   \
+  if (ct && want_pool && r == CUDA_SUCCESS) {
+    const cuuint32_t pbox[4] = {64, 4, 8, 1};              // the 2x2 max of one 8 x 16 halo tile
+    r = encode_out(&pmap, pool_out->ptr, pool_out->ld, in.n, p.PH, p.PW, pbox);
+  }
+  if (r != CUDA_SUCCESS) {
+    ctx->set_error("cuTensorMapEncodeTiled(output of " + L.name + ") failed: " + std::to_string(static_cast<int>(r)));
+    return B2O_ERR_CUDA;
+  }
+  if (up_add != nullptr) {                                 // generic 1x1 tiles
+    if (bn == 64) return launch<64, 64, 0, false, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);
+    if (bn == 128) return launch<128, 64, 0, false, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);
+  }
+#define B2O_TC_PAIR_CASE(BN)                                                                                           \
+  if (pair && bn == BN) {                                                                                              \
+    if (p.resident) return launch<BN, 64, 2, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                       \
+    if (p.halo) return launch<BN, 64, 1, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                           \
+    return launch<BN, 64, 0, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                                       \
   }
   B2O_TC_PAIR_CASE(64); B2O_TC_PAIR_CASE(128);
 #undef B2O_TC_PAIR_CASE
-#define B2O_TC_CASE(BN, KC)                                                            \
-  if (bn == BN && kch == KC) {                                                         \
-    if (p.resident) return launch<BN, KC, 2, false>(ctx, amap, L, p, smem_bytes, st);  \
-    if (p.halo) return launch<BN, KC, 1, false>(ctx, amap, L, p, smem_bytes, st);      \
-    return launch<BN, KC, 0, false>(ctx, amap, L, p, smem_bytes, st);                  \
+#define B2O_TC_CASE(BN, KC)                                                                                            \
+  if (bn == BN && kch == KC) {                                                                                         \
+    if (p.resident) return launch<BN, KC, 2, false>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                      \
+    if (p.halo) return launch<BN, KC, 1, false>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                          \
+    return launch<BN, KC, 0, false>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                                      \
   }
   B2O_TC_CASE(16, 64); B2O_TC_CASE(32, 64); B2O_TC_CASE(64, 64); B2O_TC_CASE(128, 64);
   B2O_TC_CASE(16, 32); B2O_TC_CASE(32, 32);
