@@ -380,8 +380,9 @@ int b2o_crnn_set_top(b2o_ctx* ctx, const float* w_dev, const float* bias_dev, in
  * processing step s goes to step s of both lstm_10 and lstm_10_back, lstm_11_back's input gradient lands at time 49 - s)
  * and fc_12's gradients as b2o_ctc_loss_grad forms them.  Fixed-order sums, no atomics: bit-identical run to run.
  * grad_dev NULL: the loss only.  ws_bytes >= b2o_rnn_train_workspace_bytes(b, k) always.  The workspace holds, in this
- * order, each slot rounded up to 256 bytes: W^T (4, 512, 128) fp16, U (4, 128, 512) fp16, xw then dz (4, b, 50, 512) f32
- * (processing order), acts (4, b, 50, 5, 128) f32 = i, f, g = tanh(z_c), o, c per processing step, hf / hb (2, b, 50, 128)
+ * order, each slot rounded up to 256 bytes: W^T (4, 512, 128) fp16, U (4, 128, 512) fp16, xw = x W + b (4, b, 50, 512)
+ * f32 in input order (row b * 50 + t; after a loss-only call it holds all four directions), then dz over it in processing
+ * order, acts (4, b, 50, 5, 128) f32 = i, f, g = tanh(z_c), o, c per processing step, hf / hb (2, b, 50, 128)
  * fp16, l1 (b, 50, 128) fp16, l2 (b, 50, 256) fp16, dL/dl2 (b, 50, 256) f32, dL/dl1 (b, 50, 128) f32, the split-K
  * partials ((b + 15) / 16, 526336) f32, and b2o_ctc_train_workspace_bytes(b, k) for the CTC, which starts with dL/dlogits
  * (b, 48, k) f32.  2 <= k <= B2O_MAX_CLASSES, 0 <= dropout < 1, otherwise B2O_ERR_ARG.                             */

@@ -2,7 +2,8 @@
 
 * ``keep_mask``: the dropout mask of include/b2ocr.h, rebuilt bit for bit from the kernel's hash (splitmix64 of the seed,
   the step, the cached row, the step t and the feature c).
-* ``dropped``: the features after dropout, in the kernel's fp32 arithmetic (x * fp32(1 / (1 - rate)), or 0).
+* ``dropped`` / ``drop``: the features after dropout, in the kernel's fp32 arithmetic (x * fp32(1 / (1 - rate)), or 0),
+  from a cache and its rows or from features already gathered.
 * ``loss_grad``: the Keras ``ctc_batch_cost`` loss of one crop, L = -log sum over alignments of prod_t q[t, path_t] with
   q = softmax(l) + 1e-7 and blank = K-1, and its gradient dL/dl, by the forward-backward algorithm in the log domain,
   in fp64.  Also the pieces the GPU test's bound needs: p, q, the posteriors gamma and D_t = sum_c gamma_c p_c / q_c.
@@ -39,7 +40,12 @@ def keep_mask(rows, rate, seed, step):
 
 def dropped(features, rows, rate, seed, step):
     """float32 (B, 48, 256): the features of ``rows`` (of an (n, 48, 256) fp16 array) as the kernel uses them."""
-    x = np.asarray(features)[np.asarray(rows)].astype(np.float32)
+    return drop(np.asarray(features)[np.asarray(rows)], rows, rate, seed, step)
+
+
+def drop(x, rows, rate, seed, step):
+    """float32 (B, 48, 256): features x (B, 48, 256) of the dataset rows ``rows`` after the kernel's dropout."""
+    x = np.asarray(x).astype(np.float32)
     rate = np.float32(rate)
     if rate == 0:
         return x
@@ -108,7 +114,7 @@ def batch_grads(x, g):
     x = np.asarray(x, np.float64)
     g = np.asarray(g, np.float64)
     b = x.shape[0]
-    return np.einsum("btc,btk->ck", x, g) / b, g.sum((0, 1)) / b
+    return np.einsum("btc,btk->ck", x, g, optimize=True) / b, g.sum((0, 1)) / b
 
 
 def rmsprop(param, grad, acc, lr=1e-3, rho=0.9, eps=1e-7):

@@ -8,6 +8,10 @@
   processing order (recognition.py:298-319).
 * ``backward``: the same gradients by hand, from given activations (the device's own, read from its workspace), with a
   running first-order bound of the device's fp32 arithmetic next to every value (see tests/test_gpu_fit_recurrent.py).
+* ``forward_state``: the fp64 forward with every value the device saves for the backward (xw, the gate activations
+  and c, h), rounding emulated or not; ``forward_acts`` its unrounded activations.
+* ``state_ratios``: checks the device's saved forward state step by step, each step on the device's own previous
+  state, so that the ``backward`` above is known to run on the activations of the right step, gate and direction.
 """
 import numpy as np
 import torch
@@ -167,8 +171,9 @@ def _wsum(a, dz, ez):
     """sum over (b, s) of a^T dz, and the bound of the device's chunked fp32 sum divided by B."""
     n = a.shape[0] * a.shape[1]
     aa = np.abs(a)
-    val = np.einsum("bsm,bsn->mn", a, dz)
-    err = gamma(n + 1) * np.einsum("bsm,bsn->mn", aa, np.abs(dz)) + np.einsum("bsm,bsn->mn", aa, ez)
+    val = np.einsum("bsm,bsn->mn", a, dz, optimize=True)
+    err = (gamma(n + 1) * np.einsum("bsm,bsn->mn", aa, np.abs(dz), optimize=True)
+           + np.einsum("bsm,bsn->mn", aa, ez, optimize=True))
     return val, err
 
 
@@ -219,8 +224,8 @@ def backward(x, acts, h1, l1, l2, g, tensors, rows, dropout=0.0, seed=0, step=0,
             bounds[f"{n}.{part}"] = e / b + U32 * np.abs(v / b)
     xk = l2[:, DISCARD:] * ms
     n = b * 48
-    grads["fc_12.kernel"] = np.einsum("btc,btk->ck", xk, g) / b
-    bounds["fc_12.kernel"] = gamma(n + 1) * np.einsum("btc,btk->ck", np.abs(xk), np.abs(g)) / b + \
+    grads["fc_12.kernel"] = np.einsum("btc,btk->ck", xk, g, optimize=True) / b
+    bounds["fc_12.kernel"] = gamma(n + 1) * np.einsum("btc,btk->ck", np.abs(xk), np.abs(g), optimize=True) / b + \
         U32 * np.abs(grads["fc_12.kernel"])
     grads["fc_12.bias"] = g.sum((0, 1)) / b
     bounds["fc_12.bias"] = gamma(n + 1) * np.abs(g).sum((0, 1)) / b + U32 * np.abs(grads["fc_12.bias"])
@@ -230,30 +235,107 @@ def backward(x, acts, h1, l1, l2, g, tensors, rows, dropout=0.0, seed=0, step=0,
 def forward_acts(tensors, x):
     """fp64 forward without rounding that also returns what ``backward`` needs: (acts (4,B,50,5,128), h1 (2,B,50,128),
     l1 (B,50,128), l2 (B,50,256)), in processing order."""
+    st = forward_state(tensors, x, rounding=False)
+    return st["acts"], st["h1"], st["l1"], st["l2"]
+
+
+def _sig(v):
+    return 1 / (1 + np.exp(-v))
+
+
+def forward_state(tensors, x, rounding=True):
+    """The fp64 forward with every value ``b2o_rnn_loss_grad`` keeps in its workspace, as a dict: xw (4,B,50,512) =
+    x W + b per direction in input order (row b*50 + t), acts (4,B,50,5,128) = i, f, g, o, c, h1 (2,B,50,128) = hf, hb,
+    l1 (B,50,128), l2 (B,50,256), all but xw in processing order.  ``rounding``: W and U rounded to fp16, h and l1
+    rounded to fp16, as the device rounds them."""
     x = np.asarray(x, np.float64)
+    rnd = R.f16 if rounding else (lambda a: np.asarray(a, np.float64))
 
     def run(layer, inp, back):
-        w = np.asarray(tensors[layer + ".kernel"], np.float64)
-        u = np.asarray(tensors[layer + ".recurrent_kernel"], np.float64)
+        w = rnd(tensors[layer + ".kernel"])
+        u = rnd(tensors[layer + ".recurrent_kernel"])
         xw = inp @ w + np.asarray(tensors[layer + ".bias"], np.float64)
-        if back:
-            xw = xw[:, ::-1]
+        xs = xw[:, ::-1] if back else xw
         b = xw.shape[0]
         h = np.zeros((b, UNITS))
         c = np.zeros((b, UNITS))
         acts, hs = np.zeros((b, STEPS, 5, UNITS)), np.zeros((b, STEPS, UNITS))
-        sig = lambda v: 1 / (1 + np.exp(-v))                                         # noqa: E731
         for s in range(STEPS):
-            zi, zf, zc, zo = np.split(xw[:, s] + h @ u, 4, 1)
-            i, f, g, o = sig(zi), sig(zf), np.tanh(zc), sig(zo)
+            zi, zf, zc, zo = np.split(xs[:, s] + h @ u, 4, 1)
+            i, f, g, o = _sig(zi), _sig(zf), np.tanh(zc), _sig(zo)
             c = f * c + i * g
-            h = o * np.tanh(c)
+            h = rnd(o * np.tanh(c))
             acts[:, s] = np.stack([i, f, g, o, c], 1)
             hs[:, s] = h
-        return acts, hs
-    a0, hf = run("lstm_10", x, False)
-    a1, hb = run("lstm_10_back", x, True)
-    l1 = hf + hb
-    a2, h2f = run("lstm_11", l1, False)
-    a3, h2b = run("lstm_11_back", l1, True)
-    return np.stack([a0, a1, a2, a3]), np.stack([hf, hb]), l1, np.concatenate([h2f, h2b], -1)
+        return xw, acts, hs
+    w0, a0, hf = run("lstm_10", x, False)
+    w1, a1, hb = run("lstm_10_back", x, True)
+    l1 = rnd(hf + hb)
+    w2, a2, h2f = run("lstm_11", l1, False)
+    w3, a3, h2b = run("lstm_11_back", l1, True)
+    return {"xw": np.stack([w0, w1, w2, w3]), "acts": np.stack([a0, a1, a2, a3]), "h1": np.stack([hf, hb]), "l1": l1,
+            "l2": np.concatenate([h2f, h2b], -1)}
+
+
+# 1 / (1 + expf(-z)): expf's 2 ulp (4u relative) pass through the addition with weight e / (1 + e) < 1, then the
+# addition and the division round once each.  tanhf: 2 ulp.
+SIG_REL = 6 * U32
+TANH_REL = 4 * U32
+
+
+def _slope_bound(deriv, z, ez):
+    """max of a derivative that falls with |z| (sigmoid', tanh') over [z - ez, z + ez]."""
+    return deriv(np.maximum(np.abs(z) - ez, 0.0))
+
+
+def state_ratios(x, tensors, xw, acts, h1, l1, l2):
+    """Worst |device - fp64| / bound of the training forward's saved state, each value judged on the device's own
+    inputs of its step, so that no bound grows along the 50 steps.  x (B,50,128): the fc_9 rows the crops read (zeros
+    for a row outside the cache); xw, acts, h1, l1, l2: the workspace slots of ``b2o_rnn_loss_grad`` (layouts as in
+    ``forward_state``).  Returns {"xw", "i", "f", "g", "o", "c", "h"} -> worst ratio over the four directions.
+    * xw[d] = x W16 + b (x the fc_9 rows for layer 1, the device's own l1 for layer 2): the MMA's fp32 sum of exact
+      fp16 products within stage_refs.gamma(128) |x| |W16|, then the bias in one rounding, u |xw|.
+    * z at processing step s = xw[d][t(s)] + h_{s-1} U16 (t(s) = s, or 49 - s going backwards; h_{s-1} the device's
+      fp16 h, 0 at s = 0): the MMA sum that starts from xw, within ez = stage_refs.gamma(129) (|xw| + |h| |U16|).
+    * i, f, o = sigmoid(z), g = tanh(z): the largest slope over z +- ez times ez, plus SIG_REL / TANH_REL relative.
+    * c = f c' + i g with the device's c' (acts at s - 1): the gate errors times their weights plus 2u (|f c'| + |i g|).
+    * h: the stored fp16 h = fp16(o tanh(c)) of the device's own o and c: half an fp16 ulp plus 5u |o tanh c|.
+    Each bound is taken 1.01 times (second-order terms) plus 1e-30 absolute."""
+    x, xw, acts, h1, l1, l2 = (np.asarray(a, np.float64) for a in (x, xw, acts, h1, l1, l2))
+    out = dict.fromkeys(("xw", "i", "f", "g", "o", "c", "h"), 0.0)
+
+    def worst(name, dev, ref, bound):
+        out[name] = max(out[name], float((np.abs(dev - ref) / (1.01 * bound + 1e-30)).max()))
+    dsig = lambda v: _sig(v) * (1 - _sig(v))                                            # noqa: E731
+    dtanh = lambda v: 1 - np.tanh(v) ** 2                                               # noqa: E731
+    for d, layer in enumerate(LAYERS):
+        w16, u16 = R.f16(tensors[layer + ".kernel"]), R.f16(tensors[layer + ".recurrent_kernel"])
+        inp = x if d < 2 else l1
+        ref = inp @ w16 + np.asarray(tensors[layer + ".bias"], np.float64)
+        worst("xw", xw[d], ref, R.gamma(128) * (np.abs(inp) @ np.abs(w16)) + U32 * np.abs(ref))
+        h = h1[d] if d < 2 else l2[..., 128 * (d - 2):128 * (d - 1)]
+        hprev = np.concatenate([np.zeros_like(h[:, :1]), h[:, :-1]], 1)
+        xs = xw[d][:, ::-1] if d % 2 else xw[d]
+        z = xs + hprev @ u16
+        ez = R.gamma(129) * (np.abs(xs) + np.abs(hprev) @ np.abs(u16))
+        zi, zf, zg, zo = (z[..., 128 * j:128 * (j + 1)] for j in range(4))
+        ei, ef, eg, eo = (ez[..., 128 * j:128 * (j + 1)] for j in range(4))
+        a = acts[d]
+        gates = {}
+        for j, (name, zz, ee) in enumerate((("i", zi, ei), ("f", zf, ef), ("g", zg, eg), ("o", zo, eo))):
+            if name == "g":
+                val = np.tanh(zz)
+                err = _slope_bound(dtanh, zz, ee) * ee + TANH_REL * np.abs(val)
+            else:
+                val = _sig(zz)
+                err = _slope_bound(dsig, zz, ee) * ee + SIG_REL * val
+            gates[name] = (val, err)
+            worst(name, a[:, :, j], val, err)
+        (i, e_i), (f, e_f), (g, e_g) = gates["i"], gates["f"], gates["g"]
+        cp = np.concatenate([np.zeros_like(a[:, :1, 4]), a[:, :-1, 4]], 1)
+        c = f * cp + i * g
+        worst("c", a[:, :, 4], c, np.abs(cp) * e_f + np.abs(g) * e_i + np.abs(i) * e_g
+              + 2 * U32 * (np.abs(f * cp) + np.abs(i * g)))
+        p = a[:, :, 3] * np.tanh(a[:, :, 4])
+        worst("h", h, p, 0.5 * R.ulp16(h) + 5 * U32 * np.abs(p))
+    return out

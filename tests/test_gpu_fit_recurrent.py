@@ -2,7 +2,8 @@
 ``Recognizer.fit_recurrent``) against the fp64 references of tests/rnn_train_refs.py.
 
 Bounds.  u = 2^-24, gamma(n) = n u / (1 - n u).
-* Sequence features: bit for bit the "fc_9" tap of a full forward (the same kernels stop earlier).
+* Sequence features: bit for bit the "fc_9" tap of a full forward (the same kernels stop earlier), on the trained
+  recognizer and on the stn=False and color=True variants.
 * Training forward, dropout 0: l1 and l2 within LSTM_TIGHT = 2^-9 of the fp16-emulating fp64 LSTM fed x W + b with the
   fp16-rounded W (tests/test_gpu_crnn_stages.py derives it for the inference LSTM, whose arithmetic this is), and within
   LSTM_LOOSE = 2^-7 of ``oracle.crnn.lstm``.  Loss against fit_top's loss on the inference features of the same crops: the
@@ -17,8 +18,21 @@ Bounds.  u = 2^-24, gamma(n) = n u / (1 - n u).
   quarter chains plus two shuffle additions, K for dL/dl2, 1024 for dL/dl1, B * 50 + 1 for the chunked weight sums and
   their ordered second pass); tanhf 2 ulp = 4u |tanh c|; the errors of the inputs propagated with the absolute partial
   derivatives.  The test allows 1.01 times that bound (second-order terms) plus 1e-30 absolute.
+  They run at b = 11 (LSTM CTAs of 8 and 3 crops), 8 (one full CTA), 16 (one split-K chunk), 17 (a one-crop second
+  chunk), 64 and 256 (4 and 16 chunks: the batch sizes training runs at), each case asserting its chunk count as read off
+  the workspace size the library reports.
+* Saved forward state (what the teacher-forced check trusts): ``rnn_train_refs.state_ratios`` judges xw, the gates, c and
+  h of every direction and processing step on the device's own inputs of that step (its docstring derives the bounds),
+  at b = 1, 17 and 64 with a permuted index and a row outside the cache; acts, hf / hb, l1 and l2 are bit-identical over
+  loss-only and gradient calls, with and without dropout.
+* fc_12's gradient, the loss and g of b2o_rnn_loss_grad equal b2o_ctc_loss_grad's on the device's own l2 bit for bit.
+* The whole chain against autograd (``rnn_train_refs.head_losses`` with the roundings emulated, the fp64 forward rather
+  than the device's activations): no rigorous bound exists, because an fp16 rounding of h can fall the other way in
+  fp32; relative Frobenius error per tensor <= AUTOGRAD_TOL = 2^-6.
+* Dropout keys past 2^31 (rows 174,763 and 200,003 of a 200,004-row cache): dL/dl2 is 0 exactly where the mask drops.
 * One crop whose text cannot be aligned (25 copies of one letter need 49 steps) has loss +inf and adds nothing: the
   gradient times b equals the one of the other crops times b - 1 within the same kind of bound (checked to 1e-5 relative).
+* ``fit_recurrent`` is restated call by call through the C ABI and must match it bit for bit.
 The worst ratio of each check is printed.
 
 End to end, on the decisive Hershey recognizer with lstm_11 and lstm_11_back re-drawn as Keras initialises them (fc_12
@@ -26,7 +40,14 @@ kept), with fit_top's 4096 training and 1024 held-out crops, 8 epochs at learnin
 once on an H100 80GB HBM3 (700 W): exact reads 0.0000 before, 0.9932 after fit_recurrent (1.6 s), 0.8740 after fit_top
 from the same start with the same data, epochs and seed; the trained model reads 0.9941.  The test asks for at least the
 trained model's rate minus MARGIN = 0.01 and strictly more than fit_top.  One epoch of fit_recurrent on the trained model
-took it from 0.9941 to 0.9951.  Worst gradient ratios measured: 0.050 of the bound (K = 1024), the largest on fc_12.
+took it from 0.9941 to 0.9951.
+
+Measured on an H100 80GB HBM3 (700 W).  Worst teacher-forced gradient ratios, the largest on fc_12: 0.050 of the bound
+(b = 11, K = 1024), 0.017 (b = 17, K = 2), 0.0096 (b = 64, K = 1024), 0.00042 (b = 256, K = 38).  Saved state, worst
+over b = 1, 17, 64: xw 0.015, i 0.31, f 0.32, g 0.11, o 0.31, c 0.050 and h 0.99 of their bounds (h's bound is mostly
+the half fp16 ulp its rounding may take).  Against autograd: 1.1e-5 relative (fc_12.kernel), the losses 2.2e-6.  The
+batch-size, saved-state, fc_12, autograd, dropout-key, model-variant and fit-loop checks add about 13 s to the file's run
+time on that H100.
 """
 import numpy as np
 import pytest
@@ -34,6 +55,7 @@ import torch
 
 from keras_ocr_b200 import _lib, weights as W
 from keras_ocr_b200.recognition import Recognizer
+from tests import ctc_train_refs as TR
 from tests import rnn_train_refs as RR
 from tests import stage_refs as R
 
@@ -42,6 +64,7 @@ pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
 LSTM_TIGHT = 2.0 ** -9
 LSTM_LOOSE = 2.0 ** -7
+AUTOGRAD_TOL = 2.0 ** -6
 
 
 def _stream():
@@ -61,12 +84,14 @@ def _a256(x):
     return (x + 255) // 256 * 256
 
 
-def ws_slots(b, k, ctx):
-    """Byte offsets of the workspace slots documented in include/b2ocr.h (b2o_rnn_loss_grad)."""
+def ws_slots(b, k, ctx, chunks=None):
+    """Byte offsets of the workspace slots documented in include/b2ocr.h (b2o_rnn_loss_grad); ``chunks``: the number of
+    split-K partials, (b + 15) // 16 as documented."""
     rows = b * 50
+    chunks = (b + 15) // 16 if chunks is None else chunks
     sizes = [("w16t", 4 * 128 * 512 * 2), ("u16", 4 * 128 * 512 * 2), ("xz", 4 * rows * 512 * 4),
              ("acts", 4 * rows * 640 * 4), ("h1", 2 * rows * 128 * 2), ("l1", rows * 128 * 2), ("l2", rows * 256 * 2),
-             ("dl2", rows * 256 * 4), ("dl1", rows * 128 * 4), ("partial", (b + 15) // 16 * 526336 * 4),
+             ("dl2", rows * 256 * 4), ("dl1", rows * 128 * 4), ("partial", chunks * 526336 * 4),
              ("ctc", ctx.ctc_train_workspace_bytes(b, k))]
     out, at = {}, 0
     for name, n in sizes:
@@ -74,6 +99,25 @@ def ws_slots(b, k, ctx):
         at += _a256(n)
     out["end"] = at
     return out
+
+
+def device_chunks(ctx, b, k):
+    """The number of split-K chunks the LSTM weight gradients are summed over at batch b, read off the workspace size
+    the library reports."""
+    nbytes = ctx.rnn_train_workspace_bytes(b, k)
+    found = [n for n in range(1, b + 1) if ws_slots(b, k, ctx, n)["end"] == nbytes]
+    assert len(found) == 1, (b, k, nbytes)
+    return found[0]
+
+
+def state_of(ws, b, k, ctx):
+    """The forward state in the workspace after a call: xw (valid after a loss-only call), acts, h1, l1, l2."""
+    sl = ws_slots(b, k, ctx)
+    return {"xw": _view(ws, sl["xz"], (4, b, 50, 512), torch.float32),
+            "acts": _view(ws, sl["acts"], (4, b, 50, 5, 128), torch.float32),
+            "h1": _view(ws, sl["h1"], (2, b, 50, 128), torch.float16),
+            "l1": _view(ws, sl["l1"], (b, 50, 128), torch.float16),
+            "l2": _view(ws, sl["l2"], (b, 50, 256), torch.float16)}
 
 
 def _view(ws, off, shape, dtype):
@@ -148,17 +192,15 @@ def _synth(seeds):
 
 def _input(rec, crops):
     t = torch.from_numpy(np.ascontiguousarray(crops)).cuda()
-    x = torch.empty((len(crops), 200, 31), dtype=torch.float16, device="cuda")
-    rec.ctx.crops_to_input(t.data_ptr(), len(crops), x.data_ptr(), _stream())
+    x = torch.empty((len(crops), 200, 31) + ((3,) if rec.color else ()), dtype=torch.float16, device="cuda")
+    rec.ctx.crops_to_input(t.data_ptr(), len(crops), x.data_ptr(), _stream(), color=rec.color)
     return x
 
 
 # ------------------------------------------------------------------------------------------ 1. sequence features
-def test_sequence_features_are_the_fc9_tap():
-    hw = W.synthetic_crnn_weights(decisive=True)
-    rec = Recognizer(weights=hw)
+def _sequence_features_vs_tap(rec, crops, what):
+    """b2o_crnn_sequence_features of ``crops`` on ``rec`` against the "fc_9" tap of a full forward, bit for bit."""
     rec.keep_workspace = True
-    crops, _ = _synth(range(72_000_000, 72_000_019))
     b = len(crops)
     x = _input(rec, crops)
     rec.predict_device(x)
@@ -173,11 +215,29 @@ def test_sequence_features_are_the_fc9_tap():
     rec.ctx.crnn_sequence_features(x.data_ptr(), b, out.data_ptr(), ws.data_ptr(), nbytes, _stream())
     n2 = rec.ctx.launch_count()
     assert np.array_equal(out.cpu().numpy().view(np.int16), tap.view(np.int16))
-    print(f"sequence features: {n2 - n1} launches (b2o_crnn_features: {n1 - n0}), bit-identical to the fc_9 tap")
+    print(f"sequence features ({what}): {n2 - n1} launches (b2o_crnn_features: {n1 - n0}), bit-identical to the "
+          f"fc_9 tap")
     assert 0 < n2 - n1 < n1 - n0
     small = torch.empty(16, dtype=torch.uint8, device="cuda")
     with pytest.raises(_lib.B2OError):                    # the last forward stopped after fc_9: no l1 / l2 to tap
         rec.ctx.crnn_tap("l2", ws.data_ptr(), b, small.data_ptr(), 16, _stream())
+
+
+def test_sequence_features_are_the_fc9_tap():
+    crops, _ = _synth(range(72_000_000, 72_000_019))
+    _sequence_features_vs_tap(Recognizer(weights=W.synthetic_crnn_weights(decisive=True)), crops, "trained")
+
+
+@pytest.mark.parametrize("variant", ["stn_false", "color"])
+def test_sequence_features_are_the_fc9_tap_on_variants(variant):
+    """build_model(stn=False), whose fc_9 reads bn_7's output directly, and build_model(color=True), on RGB crops."""
+    crops, _ = _synth(range(72_000_000, 72_000_019))
+    if variant == "stn_false":
+        rec = Recognizer(weights=W.synthetic_crnn_weights(5, stn=False), build_params={"stn": False})
+    else:
+        rec = Recognizer(weights=W.synthetic_crnn_weights(6, color=True), build_params={"color": True})
+        crops = np.stack([crops, crops[:, ::-1], 255 - crops], -1)
+    _sequence_features_vs_tap(rec, crops, variant)
 
 
 # ------------------------------------------------------------------------------------------ 2. training forward
@@ -238,12 +298,20 @@ def test_training_forward(ctx):
 
 
 # ------------------------------------------------------------------------------------------ 3. gradients
-@pytest.mark.parametrize("k", [2, 38, 1024])
-def test_gradients_teacher_forced(ctx, k):
-    n_rows, b = 23, 11
-    rng = np.random.default_rng(k)
-    t = _tensors(k, k)
-    xs = _x(n_rows, k + 1)
+# (b, K, chunks): LSTM CTAs of 8 crops with a partial last one (11), one full CTA (8), one chunk of 16 crops, one crop
+# more (a one-crop chunk tail), and the batch sizes training runs at (64 by default, 256 in scripts/bench_fit_recurrent.py)
+GRAD_CASES = [(11, 2, 1), (11, 38, 1), (11, 1024, 1), (8, 38, 1), (16, 38, 1), (17, 2, 2), (64, 1024, 4),
+              (256, 38, 16)]
+
+
+@pytest.mark.parametrize("b,k,chunks", GRAD_CASES, ids=[str(k) if b == 11 else f"{k}-b{b}" for b, k, _ in GRAD_CASES])
+def test_gradients_teacher_forced(ctx, b, k, chunks):
+    n_rows = b + 12
+    assert device_chunks(ctx, b, k) == chunks
+    seed = k if b == 11 else 1000 * b + k
+    rng = np.random.default_rng(seed)
+    t = _tensors(k, seed)
+    xs = _x(n_rows, seed + 1)
     targets = _targets(rng, k, b)
     index = rng.permutation(n_rows)[:b]
     x_t = torch.from_numpy(xs).cuda()
@@ -271,7 +339,101 @@ def test_gradients_teacher_forced(ctx, k):
         if dropout == 0:
             only, none, _ = run(ctx, x_t, n_rows, index, k, params, off, lab, grads=False)
             assert none is None and np.array_equal(only.view(np.int32), loss.view(np.int32))
-    print(f"rnn_loss_grad K={k}: " + "; ".join(report))
+    print(f"rnn_loss_grad b={b} ({chunks} chunks) K={k}: " + "; ".join(report))
+
+
+def _problem(b, k, seed, out_of_range=True):
+    """(tensors, x cache, n_rows, permuted index with one row outside the cache when b > 1 and out_of_range, targets)."""
+    n_rows = b + 7
+    rng = np.random.default_rng(seed)
+    t = _tensors(k, seed)
+    xs = _x(n_rows, seed + 1)
+    index = rng.permutation(n_rows)[:b]
+    if b > 1 and out_of_range:
+        index[b // 2] = n_rows + 3
+    return t, xs, n_rows, index, _targets(rng, k, b)
+
+
+@pytest.mark.parametrize("b", [1, 17, 64])
+def test_forward_state_vs_fp64(ctx, b):
+    """The state the teacher-forced gradient test feeds to the reference backward, checked step by step by
+    ``rnn_train_refs.state_ratios`` (xw of all four directions in input order, the gates and c per processing step, h),
+    with a permuted index and one row outside the cache (its x reads as zeros: xw = the bias).  The forward does not
+    depend on dropout or on whether gradients are asked for: acts, h1, l1 and l2 are bit-identical over loss-only and
+    gradient calls with dropout 0 and 0.25, so the state checked here is the one the gradient test reads."""
+    k = 38
+    t, xs, n_rows, index, targets = _problem(b, k, 500 + b)
+    x_t = torch.from_numpy(xs).cuda()
+    params = torch.from_numpy(RR.flat(t, k)).cuda()
+    off, lab = _csr(targets)
+    states = []
+    for dropout, seed, step in ((0.0, 0, 0), (0.25, 7, 3)):
+        for grads in (False, True):
+            ws = run(ctx, x_t, n_rows, index, k, params, off, lab, dropout, seed, step, grads=grads)[2]
+            states.append(state_of(ws, b, k, ctx))
+    first = states[0]
+    for st in states[1:]:
+        for name in ("acts", "h1", "l1", "l2"):
+            assert np.array_equal(st[name].view(np.uint8), first[name].view(np.uint8)), name
+    assert np.array_equal(states[2]["xw"].view(np.uint8), first["xw"].view(np.uint8))     # gradient calls reuse xw for dz
+    x = np.where((index < n_rows)[:, None, None], xs[np.minimum(index, n_rows - 1)], 0)
+    ratios = RR.state_ratios(x, t, first["xw"], first["acts"], first["h1"], first["l1"], first["l2"])
+    print(f"forward state b={b}: worst " + ", ".join(f"{n} {v:.3g}" for n, v in ratios.items()) + " of their bounds")
+    assert max(ratios.values()) <= 1.0, ratios
+
+
+@pytest.mark.parametrize("b", [17, 64])
+def test_fc12_gradient_is_the_fit_top_kernel(ctx, b):
+    """fc_12's part of b2o_rnn_loss_grad is b2o_ctc_loss_grad on the device's own l2: with l2's kept steps placed at
+    the crops' rows of an (n_rows, 48, 256) cache, the fit_top entry point gives the same loss, g = dL/dlogits and fc_12
+    gradients in every bit, with and without dropout."""
+    k = 38
+    t, xs, n_rows, index, targets = _problem(b, k, 600 + b, out_of_range=False)
+    x_t = torch.from_numpy(xs).cuda()
+    params = torch.from_numpy(RR.flat(t, k)).cuda()
+    off, lab = _csr(targets)
+    idx = torch.from_numpy(index.astype(np.int32)).cuda()
+    n_lstm = sum(int(np.prod(shape)) for _, shape in RR.tensor_names(k)[:12])
+    fc_w, fc_b = params[n_lstm:n_lstm + 256 * k], params[n_lstm + 256 * k:]
+    for dropout, seed, step in ((0.0, 0, 0), (0.25, 7, 3)):
+        loss, grad, ws = run(ctx, x_t, n_rows, index, k, params, off, lab, dropout, seed, step)
+        sl = ws_slots(b, k, ctx)
+        l2 = ws[sl["l2"]:sl["l2"] + b * 50 * 256 * 2].view(torch.float16).view(b, 50, 256)
+        feats = torch.zeros((n_rows, 48, 256), dtype=torch.float16, device="cuda")
+        feats[idx.long()] = l2[:, 2:]
+        loss2 = torch.empty(b, dtype=torch.float32, device="cuda")
+        gw, gb = torch.empty(256 * k, dtype=torch.float32, device="cuda"), torch.empty(k, dtype=torch.float32,
+                                                                                       device="cuda")
+        nbytes = ctx.ctc_train_workspace_bytes(b, k)
+        ws2 = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+        ctx.ctc_loss_grad(feats.data_ptr(), n_rows, idx.data_ptr(), b, k, fc_w.data_ptr(), fc_b.data_ptr(),
+                          off.data_ptr(), lab.data_ptr(), dropout, seed, step, loss2.data_ptr(), gw.data_ptr(),
+                          gb.data_ptr(), None, ws2.data_ptr(), nbytes, _stream())
+        n_g = b * 48 * k * 4
+        assert np.isfinite(loss).all()
+        assert np.array_equal(loss2.cpu().numpy().view(np.int32), loss.view(np.int32))
+        assert torch.equal(ws2[:n_g], ws[sl["ctc"]:sl["ctc"] + n_g])
+        assert np.array_equal(gw.cpu().numpy().view(np.int32), grad[n_lstm:n_lstm + 256 * k].view(np.int32))
+        assert np.array_equal(gb.cpu().numpy().view(np.int32), grad[n_lstm + 256 * k:].view(np.int32))
+
+
+def test_gradients_vs_autograd(ctx):
+    """The whole chain against autograd through ``rnn_train_refs.head_losses`` with the device's roundings emulated
+    (the fp64 forward, not the device's activations), at a batch of two chunks with dropout.  There is no rigorous bound:
+    an fp16 rounding of h that falls the other way in fp32 than in fp64 moves everything after it.  Relative Frobenius
+    error per tensor <= AUTOGRAD_TOL."""
+    k, b = 38, 17
+    t, xs, n_rows, index, targets = _problem(b, k, 700, out_of_range=False)
+    x_t = torch.from_numpy(xs).cuda()
+    params = torch.from_numpy(RR.flat(t, k)).cuda()
+    loss, grad, _ = run(ctx, x_t, n_rows, index, k, params, *_csr(targets), 0.25, 7, 3)
+    ref_loss, ref = RR.head_losses(t, xs[index].astype(np.float64), targets, index, 0.25, 7, 3, rounding=True)
+    dev = RR.unflat(grad, k)
+    err = {n: float(np.linalg.norm(dev[n] - ref[n]) / np.linalg.norm(ref[n])) for n, _ in RR.tensor_names(k)}
+    name = max(err, key=err.get)
+    loss_err = float(np.abs(loss - ref_loss).max() / np.abs(ref_loss).max())
+    print(f"gradients vs autograd: worst relative Frobenius error {err[name]:.3g} ({name}), loss {loss_err:.3g}")
+    assert err[name] <= AUTOGRAD_TOL, err
 
 
 def test_unalignable_crop_adds_nothing(ctx):
@@ -289,6 +451,34 @@ def test_unalignable_crop_adds_nothing(ctx):
     assert np.abs(grad * 6 - grad2 * 5).max() <= 1e-5 * scale
     bad_row, _, _ = run(ctx, x_t, n_rows, [0, 99], k, params, *_csr(good[:2]), grads=False)
     assert np.isfinite(bad_row[0]) and np.isnan(bad_row[1])
+
+
+def test_dropout_keys_past_2_31(ctx):
+    """Crops at rows 174,763 and 200,003 of a 200,004-row fc_9 cache (2.6 GB, only the used rows written), whose dropout
+    keys row * 48 * 256 pass 2^31: on the kept steps dL/dl2 is 0 exactly where the mask rebuilt from 64-bit keys drops a
+    feature, wherever g w^T is certainly not 0 (|g w^T| above twice the gamma(K) bound of its fp32 sum)."""
+    rows, n_rows = np.array([0, 174_763, 200_003]), 200_004
+    assert int(rows[1]) * 48 * 256 >= 2 ** 31 > (int(rows[1]) - 1) * 48 * 256
+    k, dropout, seed, step = 38, 0.25, 7, 3
+    t = _tensors(k, 31)
+    params = torch.from_numpy(RR.flat(t, k)).cuda()
+    targets = _targets(np.random.default_rng(31), k, len(rows))
+    x_t = torch.empty((n_rows, 50, 128), dtype=torch.float16, device="cuda")
+    try:
+        x_t[torch.from_numpy(rows).cuda()] = torch.from_numpy(_x(len(rows), 32)).cuda()
+        loss, _, ws = run(ctx, x_t, n_rows, rows, k, params, *_csr(targets), dropout, seed, step)
+    finally:
+        del x_t
+        torch.cuda.empty_cache()
+    sl = ws_slots(len(rows), k, ctx)
+    dl2 = _view(ws, sl["dl2"], (len(rows), 50, 256), torch.float32)
+    g = _view(ws, sl["ctc"], (len(rows), 48, k), torch.float32).astype(np.float64)
+    w = t["fc_12.kernel"].astype(np.float64)
+    sure = np.abs(g @ w.T) > 2 * _gamma(k) * (np.abs(g) @ np.abs(w).T)
+    mask = TR.keep_mask(rows, dropout, seed, step)
+    print(f"dropout keys past 2^31: dL/dl2's zeros checked on {sure.mean():.4f} of the kept steps' features")
+    assert np.isfinite(loss).all() and sure.mean() > 0.9
+    assert not dl2[:, :2].any() and np.array_equal((dl2[:, 2:] != 0)[sure], mask[sure])
 
 
 # ------------------------------------------------------------------------------------------ 4. determinism
@@ -468,6 +658,65 @@ def test_fit_recurrent_does_no_harm(ctx, word_crops):
     after, _ = _rate(rec, hc, hwords)
     print(f"fine-tuning the trained BiLSTM: held-out exact reads {before:.4f} -> {after:.4f}")
     assert after >= before
+
+
+def _logits(rec, crops):
+    rec.keep_workspace = True
+    rec.predict_device(_input(rec, crops))
+    return rec.tap("logits", (len(crops), 48, len(rec.alphabet) + 1), torch.float32).cpu().numpy()
+
+
+def test_fit_recurrent_is_its_abi_calls(ctx, tmp_path):
+    """fit_recurrent, restated as the calls its docstring describes: per epoch a default_rng(seed) permutation, batches
+    of batch_size in its order with a short last one (70 = 32 + 32 + 6), dropout keyed on a step counter that runs on
+    across epochs, one RMSprop accumulator over the flat parameters carried over, the history as the means of the fp32
+    losses, the validation loss without dropout after each epoch.  The 14 tensors and the history bit for bit; the
+    reloaded CRNN reads like a recognizer loaded from save_weights."""
+    n, bs, epochs, lr, dropout, seed = 70, 32, 2, 1e-3, 0.25, 5
+    hw = W.synthetic_crnn_weights(decisive=True)
+    crops, words = _synth(range(76_000_000, 76_000_000 + n))
+    v_crops, v_words = _synth(range(76_100_000, 76_100_019))
+    rec = Recognizer(weights=hw)
+    hist = rec.fit_recurrent(crops, words, epochs=epochs, batch_size=bs, learning_rate=lr, dropout=dropout, seed=seed,
+                             validation=(v_crops, v_words))
+    k = len(rec.alphabet) + 1
+    ref = Recognizer(weights=hw)
+
+    def features(c):
+        x = _input(ref, c)
+        out = torch.empty((len(c), 50, 128), dtype=torch.float16, device="cuda")
+        ws = torch.empty(ref.ctx.crnn_workspace_bytes(len(c)), dtype=torch.uint8, device="cuda")
+        ref.ctx.crnn_sequence_features(x.data_ptr(), len(c), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream())
+        return out
+    seq, v_seq = features(crops), features(v_crops)
+    labels = [[rec.alphabet.index(c) for c in wd] for wd in words]
+    v_labels = [[rec.alphabet.index(c) for c in wd] for wd in v_words]
+    params = torch.from_numpy(RR.flat(hw, k)).cuda()
+    acc = torch.zeros_like(params)
+    rng = np.random.default_rng(seed)
+    want = {"loss": [], "val_loss": []}
+    step = 0
+    for _ in range(epochs):
+        perm = rng.permutation(n)
+        seen = np.empty(n, np.float32)
+        for i in range(0, n, bs):
+            idx = perm[i:i + bs]
+            loss, grad, _ = run(ctx, seq, n, idx, k, params, *_csr([labels[j] for j in idx]), dropout, seed, step)
+            seen[i:i + len(idx)] = loss
+            gt = torch.from_numpy(grad).cuda()
+            ctx.rmsprop_step(params.data_ptr(), gt.data_ptr(), acc.data_ptr(), params.numel(), lr, 0.9, 1e-7, _stream())
+            step += 1
+        want["loss"].append(float(seen.astype(np.float64).mean()))
+        v_loss = run(ctx, v_seq, len(v_crops), np.arange(len(v_crops)), k, params, *_csr(v_labels), grads=False)[0]
+        want["val_loss"].append(float(v_loss.astype(np.float64).mean()))
+    assert step == 6 and hist == want, (hist, want)
+    trained = RR.unflat(params.cpu().numpy(), k)
+    for name, _ in RR.tensor_names(k):
+        assert np.array_equal(rec._tensors[name].view(np.int32), trained[name].view(np.int32)), name
+    path = str(tmp_path / "recurrent.npz")
+    rec.save_weights(path)
+    assert np.array_equal(_logits(rec, v_crops).view(np.int32), _logits(Recognizer(weights=path), v_crops).view(np.int32))
+    print(f"fit_recurrent as its ABI calls: history {hist}")
 
 
 # ------------------------------------------------------------------------------------------ 7. argument checks

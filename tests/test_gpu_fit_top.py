@@ -22,6 +22,15 @@ Bounds.  u = 2^-24, gamma(n) = n u / (1 - n u).
 * RMSprop: acc = rho acc + (1 - rho) g^2 is four roundings of non-negative terms (the fp32 1 - rho one more): within 5u
   acc; the step lr g / (sqrt(acc) + eps) then within 10u relative; param within that plus u |param|.
 The worst ratio to each bound is printed.
+
+The loss and gradient check runs at b = 13 and 16 (one chunk of the split-K sums), 17 (a one-crop second chunk), 64 and
+256 (4 and 16 chunks: the batch sizes training runs at), each case asserting its chunk count as read off the workspace
+size the library reports; the bounds above hold for any chunking.  A final kernel that added only some chunks, used the
+wrong chunk stride or divided by the wrong B fails there (RMSprop, being scale-free, would still train).  Measured on an
+H100 80GB HBM3 (700 W), worst over all 12 cases and both dropout rates: logits 0.033, L_b 0.066, g 0.0043, grad_W
+0.00087, grad_bias 0.00073 of their bounds.  Dropout keys of rows past 174,762 (row * 12,288 >= 2^31) are checked on a
+200,004-row cache: logits 0.015, grad_W 0.043 of their bounds.  ``fit_top`` is restated call by call through the C ABI
+and must match it bit for bit.  These checks add about 9 s to the file's run time on that H100.
 """
 import numpy as np
 import pytest
@@ -112,11 +121,32 @@ def run_loss_grad(ctx, feats_t, n_rows, index, k, w_t, b_t, off, lab, dropout, s
     return loss.cpu().numpy(), host(gw), host(gb), logits.cpu().numpy(), g
 
 
+def _a256(x):
+    return (x + 255) // 256 * 256
+
+
+def device_chunks(ctx, b, k):
+    """The number of split-K chunks the kernels sum grad_W over at batch b, read off the workspace size the library
+    reports (g, then per chunk 256 x K and K partial sums, each slot 256-byte aligned)."""
+    nbytes = ctx.ctc_train_workspace_bytes(b, k)
+    found = [n for n in range(1, b + 1) if _a256(b * T * k * 4) + _a256(n * 256 * k * 4) + _a256(n * k * 4) == nbytes]
+    assert len(found) == 1, (b, k, nbytes)
+    return found[0]
+
+
+# (b, K, chunks): batches of one chunk of 16 crops, of one crop more (a one-crop tail), and the batch sizes training runs
+# at (64 by default, 256 in scripts/bench_fit_top.py); K = 37 is not a multiple of the 64-class tiles, 1024 the widest grid.
+LOSS_GRAD_CASES = [(13, 2, 1), (13, 37, 1), (13, 38, 1), (13, 1024, 1), (16, 37, 1), (16, 1024, 1), (17, 37, 2),
+                   (17, 1024, 2), (64, 37, 4), (64, 1024, 4), (256, 37, 16), (256, 1024, 16)]
+
+
 # ------------------------------------------------------------------------------------------ 1. loss and gradient
-@pytest.mark.parametrize("k", [2, 37, 38, 1024])
-def test_loss_grad_vs_fp64(ctx, k):
-    n_rows, b = 29, 13
-    rng, feats, w, bias = _problem(k, n_rows, seed=k)
+@pytest.mark.parametrize("b,k,chunks", LOSS_GRAD_CASES,
+                         ids=[str(k) if b == 13 else f"{k}-b{b}" for b, k, _ in LOSS_GRAD_CASES])
+def test_loss_grad_vs_fp64(ctx, b, k, chunks):
+    n_rows = b + 16
+    assert device_chunks(ctx, b, k) == chunks
+    rng, feats, w, bias = _problem(k, n_rows, seed=k if b == 13 else 1000 * b + k)
     targets = _targets(rng, k, b)
     off, lab = _csr(targets)
     index = rng.permutation(n_rows)[:b]
@@ -145,9 +175,10 @@ def test_loss_grad_vs_fp64(ctx, k):
         assert r_g.max() <= 1.0, (k, dropout, float(r_g.max()))
         n = b * T
         xd = x.astype(np.float64)
-        ref_w = np.einsum("btc,btk->ck", xd, g.astype(np.float64)) / b
-        tau_w = (np.einsum("btc,btk->ck", np.abs(xd), tau_g) + _gamma(n + 1) *
-                 np.einsum("btc,btk->ck", np.abs(xd), np.abs(g.astype(np.float64)))) / b + U * np.abs(ref_w) + 1e-30
+        ref_w = np.einsum("btc,btk->ck", xd, g.astype(np.float64), optimize=True) / b
+        tau_w = (np.einsum("btc,btk->ck", np.abs(xd), tau_g, optimize=True) + _gamma(n + 1) *
+                 np.einsum("btc,btk->ck", np.abs(xd), np.abs(g.astype(np.float64)), optimize=True)) / b + \
+            U * np.abs(ref_w) + 1e-30
         ref_gw, ref_gb = TR.batch_grads(x, ref_g)
         r_w = np.abs(gw - ref_gw) / tau_w
         tau_b = (tau_g.sum((0, 1)) + _gamma(n + 1) * np.abs(g).sum((0, 1))) / b + U * np.abs(ref_gb) + 1e-30
@@ -157,7 +188,7 @@ def test_loss_grad_vs_fp64(ctx, k):
         assert np.array_equal(loss_only.view(np.int32), loss.view(np.int32))
         report.append(f"dropout {dropout}: worst logits {r_lg.max():.3g}, L_b {r_l:.3g}, g {r_g.max():.3g}, "
                       f"grad_W {r_w.max():.3g}, grad_bias {r_b.max():.3g} of their bounds")
-    print(f"ctc_loss_grad K={k}: " + "; ".join(report))
+    print(f"ctc_loss_grad b={b} ({chunks} chunks) K={k}: " + "; ".join(report))
 
 
 def test_invalid_targets_and_rows(ctx):
@@ -173,6 +204,41 @@ def test_invalid_targets_and_rows(ctx):
     assert np.array_equal(ok.view(np.int32), loss[[0, 4]].view(np.int32))
     # the invalid crops add nothing: the sums are those of the two valid crops, divided by 6 instead of 2
     assert np.allclose(gw * 6, gw2 * 2, rtol=1e-5, atol=1e-7) and np.allclose(gb * 6, gb2 * 2, rtol=1e-5, atol=1e-7)
+
+
+# dataset rows whose dropout key row * 48 * 256 passes 2^31 (174,763 * 12,288 > 2^31): the key must be formed in 64 bits
+BIG_ROWS = np.array([0, 174_763, 200_003])
+BIG_N_ROWS = 200_004
+
+
+def test_dropout_keys_past_2_31(ctx):
+    """The logits of crops at rows 174,763 and 200,003 of a 200,004-row cache (4.9 GB of features, only the used rows
+    written) against fp64 on the mask rebuilt from 64-bit keys, within the gamma(257) bound of section 1."""
+    assert int(BIG_ROWS[1]) * T * 256 >= 2 ** 31 > (int(BIG_ROWS[1]) - 1) * T * 256
+    k, dropout, seed, step = 38, 0.25, 7, 3
+    rng, small, w, bias = _problem(k, len(BIG_ROWS), seed=31)
+    feats = torch.empty((BIG_N_ROWS, T, 256), dtype=torch.float16, device="cuda")
+    try:
+        feats[torch.from_numpy(BIG_ROWS).cuda()] = torch.from_numpy(small).cuda()
+        targets = _targets(rng, k, len(BIG_ROWS))
+        off, lab = _csr(targets)
+        wt, bt = torch.from_numpy(w).cuda(), torch.from_numpy(bias).cuda()
+        loss, gw, gb, logits, g = run_loss_grad(ctx, feats, BIG_N_ROWS, BIG_ROWS, k, wt, bt, off, lab, dropout, seed,
+                                                step)
+    finally:
+        del feats
+        torch.cuda.empty_cache()
+    x = TR.drop(small, BIG_ROWS, dropout, seed, step)
+    tau = _gamma(257) * (np.abs(x).astype(np.float64) @ np.abs(w).astype(np.float64) + np.abs(bias))
+    r = np.abs(logits - TR.logits(x, w, bias)) / tau
+    # grad_partial_kernel forms the mask again: grad_W on the device's own g, within section 1's chain bound
+    xd, gd = x.astype(np.float64), g.astype(np.float64)
+    ref_w = np.einsum("btc,btk->ck", xd, gd) / len(BIG_ROWS)
+    tau_w = _gamma(len(BIG_ROWS) * T + 1) * np.einsum("btc,btk->ck", np.abs(xd), np.abs(gd)) / len(BIG_ROWS) + \
+        U * np.abs(ref_w) + 1e-30
+    r_w = np.abs(gw - ref_w) / tau_w
+    print(f"dropout keys past 2^31: worst logits {r.max():.3g}, grad_W {r_w.max():.3g} of their bounds")
+    assert np.isfinite(loss).all() and r.max() <= 1.0 and r_w.max() <= 1.0
 
 
 # ------------------------------------------------------------------------------------------ 2.-3. through the CRNN
@@ -344,6 +410,68 @@ def test_fine_tuning_does_no_harm(ctx, word_crops):
     after, _ = _rate(rec, hc, hwords)
     print(f"fine-tuning the trained top: held-out exact reads {before:.4f} -> {after:.4f}")
     assert after >= before
+
+
+def _logits(rec, crops):
+    rec.keep_workspace = True
+    rec.predict_device(_input(rec, crops))
+    return rec.tap("logits", (len(crops), T, len(rec.alphabet) + 1), torch.float32).cpu().numpy()
+
+
+def test_fit_top_is_its_abi_calls(ctx, tmp_path):
+    """fit_top, restated as the calls its docstring describes: per epoch a default_rng(seed) permutation, batches of
+    batch_size in its order with a short last one (70 = 32 + 32 + 6), dropout keyed on a step counter that runs on
+    across epochs, two RMSprop accumulators carried over, the history as the means of the fp32 losses, the validation
+    loss without dropout after each epoch.  Tensors and history bit for bit; the installed top reads like a recognizer
+    loaded from save_weights."""
+    n, bs, epochs, lr, dropout, seed = 70, 32, 2, 3e-3, 0.25, 5
+    hw = W.synthetic_crnn_weights(decisive=True)
+    crops, words = _synth(range(75_000_000, 75_000_000 + n))
+    v_crops, v_words = _synth(range(75_100_000, 75_100_019))
+    rec = Recognizer(weights=hw)
+    hist = rec.fit_top(crops, words, epochs=epochs, batch_size=bs, learning_rate=lr, dropout=dropout, seed=seed,
+                       validation=(v_crops, v_words))
+    k = len(rec.alphabet) + 1
+    ref = Recognizer(weights=hw)
+
+    def features(c):
+        x = _input(ref, c)
+        out = torch.empty((len(c), T, 256), dtype=torch.float16, device="cuda")
+        ws = torch.empty(ref.ctx.crnn_workspace_bytes(len(c)), dtype=torch.uint8, device="cuda")
+        ref.ctx.crnn_features(x.data_ptr(), len(c), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream())
+        return out
+    feats, v_feats = features(crops), features(v_crops)
+    labels = [[rec.alphabet.index(c) for c in wd] for wd in words]
+    v_labels = [[rec.alphabet.index(c) for c in wd] for wd in v_words]
+    w = torch.from_numpy(hw["fc_12.kernel"].copy()).cuda()
+    bias = torch.from_numpy(hw["fc_12.bias"].copy()).cuda()
+    acc_w, acc_b = torch.zeros_like(w), torch.zeros_like(bias)
+    rng = np.random.default_rng(seed)
+    want = {"loss": [], "val_loss": []}
+    step = 0
+    for _ in range(epochs):
+        perm = rng.permutation(n)
+        seen = np.empty(n, np.float32)
+        for i in range(0, n, bs):
+            idx = perm[i:i + bs]
+            loss, gw, gb, _, _ = run_loss_grad(ctx, feats, n, idx, k, w, bias, *_csr([labels[j] for j in idx]),
+                                               dropout, seed, step)
+            seen[i:i + len(idx)] = loss
+            for p, g, a in ((w, gw, acc_w), (bias, gb, acc_b)):
+                gt = torch.from_numpy(g).cuda()
+                ctx.rmsprop_step(p.data_ptr(), gt.data_ptr(), a.data_ptr(), p.numel(), lr, 0.9, 1e-7, _stream())
+            step += 1
+        want["loss"].append(float(seen.astype(np.float64).mean()))
+        v_loss = run_loss_grad(ctx, v_feats, len(v_crops), np.arange(len(v_crops)), k, w, bias, *_csr(v_labels), 0.0,
+                               0, 0, grads=False)[0]
+        want["val_loss"].append(float(v_loss.astype(np.float64).mean()))
+    assert step == 6 and hist == want, (hist, want)
+    for name, t in (("fc_12.kernel", w), ("fc_12.bias", bias)):
+        assert np.array_equal(rec._tensors[name].view(np.int32), t.cpu().numpy().view(np.int32)), name
+    path = str(tmp_path / "top.npz")
+    rec.save_weights(path)
+    assert np.array_equal(_logits(rec, v_crops).view(np.int32), _logits(Recognizer(weights=path), v_crops).view(np.int32))
+    print(f"fit_top as its ABI calls: history {hist}")
 
 
 # ------------------------------------------------------------------------------------------ 8. argument checks

@@ -3,7 +3,9 @@
 * autograd's gradients of all 14 tensors equal central differences of the loss;
 * the hand-written backward (the one the GPU test runs on the device's activations) equals autograd, with and without
   dropout, and it follows the reference's go_backwards quirk: a model whose backward outputs are re-reversed into input
-  order has different gradients, which the backward does not match.
+  order has different gradients, which the backward does not match;
+* the per-step checker of the saved forward state accepts the rounding-emulating fp64 forward and rejects swapped gates,
+  a cell state one step late, a backward direction's activations in input order and xw without its bias.
 """
 import numpy as np
 import torch
@@ -116,6 +118,35 @@ def test_manual_backward_matches_autograd_and_the_quirk():
     for name in ("lstm_10_back.kernel", "lstm_11_back.recurrent_kernel", "lstm_10.kernel"):
         rel = np.abs(wrong[name] - auto[name]).max() / np.abs(auto[name]).max()
         assert rel > 1e-2, (name, rel)
+
+
+def _state_worst(x, t, st):
+    return max(RR.state_ratios(x, t, st["xw"], st["acts"], st["h1"], st["l1"], st["l2"]).values())
+
+
+def test_state_checker_accepts_the_emulation_and_rejects_mutations():
+    """The per-step check of the device's saved forward state (run on the GPU by tests/test_gpu_fit_recurrent.py) passes
+    the fp64 forward with the device's roundings, and fails each way a saving kernel could be wrong."""
+    k = 5
+    t = _tensors(k, 11)
+    x = _x(3, 12)
+    x[1] = 0                                                      # a crop whose row lies outside the cache
+    st = RR.forward_state(t, x, rounding=True)
+    assert np.array_equal(st["xw"][0, 1], np.broadcast_to(t["lstm_10.bias"].astype(np.float64), (50, 512)))
+    ok = RR.state_ratios(x, t, st["xw"], st["acts"], st["h1"], st["l1"], st["l2"])
+    assert max(ok.values()) <= 1.0, ok
+    swapped = st["acts"].copy()                                   # i and f in each other's slot
+    swapped[:, :, :, [0, 1]] = swapped[:, :, :, [1, 0]]
+    shifted = st["acts"].copy()                                   # c of the step before (the state before the update)
+    shifted[:, :, 1:, 4] = st["acts"][:, :, :-1, 4]
+    shifted[:, :, 0, 4] = 0
+    input_order = st["acts"].copy()                               # a backward direction's activations in input order
+    input_order[3] = st["acts"][3][:, ::-1]
+    no_bias = st["xw"].copy()
+    no_bias[2] -= t["lstm_11.bias"].astype(np.float64)
+    for name, mutated in (("i/f swapped", dict(st, acts=swapped)), ("c one step late", dict(st, acts=shifted)),
+                          ("acts in input order", dict(st, acts=input_order)), ("xw without bias", dict(st, xw=no_bias))):
+        assert _state_worst(x, t, mutated) > 1.0, name
 
 
 def test_flat_layout():
