@@ -151,6 +151,27 @@ int b2o_get_boxes_scored(b2o_ctx* ctx, const float* scores_dev, int n, int hs, i
                          int size_threshold, float* boxes_dev, int32_t* counts_dev, float* box_scores_dev,
                          int max_boxes, void* ws_dev, size_t ws_bytes, void* stream);
 
+/* Polygons for curved words (DESIGN.md section 1): b2o_get_boxes_scored, and per kept component a polygon that follows
+ * the word's centre line.  boxes, counts and box_scores (may be NULL) are bit-identical to b2o_get_boxes_scored's.
+ * polys_dev (n, max_boxes, 2 * (B2O_MAX_POLY_SEGMENTS + 1), 2) float32 and points_dev (n, max_boxes) int32: a word kept
+ * as its rectangle has 4 points, the box itself; a polygon of s segments has 2 (s + 1) points, the top edge t_0 .. t_s
+ * left to right, then the bottom edge b_s .. b_0, clockwise from the top-left (s = 1 would be the box).  Points past
+ * points[k] are NaN.  Slots k >= min(counts[i], max_boxes) are left as they were.  The polygon is a function of the
+ * component's filled blob and its box, computed in fp64 with order-independent reductions: bit-identical in any batch
+ * and on every run.  Workspace: b2o_boxes_workspace_bytes.                                                       */
+#define B2O_MAX_POLY_SEGMENTS 8
+int b2o_get_boxes_poly(b2o_ctx* ctx, const float* scores_dev, int n, int hs, int ws,
+                       float detection_threshold, float text_threshold, float link_threshold,
+                       int size_threshold, float* boxes_dev, int32_t* counts_dev, float* box_scores_dev,
+                       float* polys_dev, int32_t* points_dev, int max_boxes, void* ws_dev, size_t ws_bytes,
+                       void* stream);
+
+/* b2o_compact_boxes for the polygons of b2o_get_boxes_poly: flat_polys (sum_i min(counts[i], max_boxes),
+ * 2 * (B2O_MAX_POLY_SEGMENTS + 1), 2), flat_points and image_index, each sized for n * max_boxes entries.        */
+int b2o_compact_polys(b2o_ctx* ctx, const float* polys_dev, const int32_t* points_dev, const int32_t* counts_dev, int n,
+                      int max_boxes, float* flat_polys_dev, int32_t* flat_points_dev, int32_t* image_index_dev,
+                      void* stream);
+
 /* The box bookkeeping of recognize_from_boxes (recognition.py:511-521: crops are appended image after
  * image, start_end = running offsets) on the device: the (n,max_boxes,4,2) table of b2o_get_boxes becomes
  * the dense list flat (sum_i min(counts[i],max_boxes), 4, 2) with image_index[k] = image of box k, both
@@ -181,6 +202,20 @@ int b2o_warp_boxes_color(b2o_ctx* ctx, const uint8_t* rgb_dev, int n, int h, int
 int b2o_warp_boxes_turned(b2o_ctx* ctx, const uint8_t* img_dev, int channels, int n, int h, int w,
                           const float* boxes_dev, const int32_t* image_index_dev, int n_boxes, int turn,
                           uint8_t* crops_dev, void* crnn_in_dev, void* stream);
+
+/* warpBox along a polygon (the piecewise form of b2o_warp_boxes): polys (n_polys, 2 * (B2O_MAX_POLY_SEGMENTS + 1), 2)
+ * float32 laid out as b2o_get_boxes_poly writes them, points (n_polys) int32, image_index (n_polys) int32; channels 1
+ * (gray image (n,h,w)) or 3 (RGB (n,h,w,3)).  Crops and CRNN input as b2o_warp_boxes(_color) writes them.
+ * A 4-point entry is cut exactly as b2o_warp_boxes cuts it.  An entry of s >= 2 segments (t_i the top edge, b_i the
+ * bottom edge): w = int(sum_i (|t_i t_i+1| + |b_i b_i+1|) / 2), h = int(mean_j |t_j b_j|), scale = min(200 / w, 31 / h),
+ * dsize = (int(scale w), int(scale h)); segment i maps (t_i, t_i+1, b_i+1, b_i) onto x in [X_i, X_i+1], y in
+ * [0, scale h], X_i = float32(scale w * cum_i / cum_s) with cum_i the running sum of (|t t| + |b b|) / 2 (fp64
+ * cv2.getPerspectiveTransform), and crop column x takes the last segment with X_i <= x, sampled as
+ * cv2.warpPerspective samples it over the full dsize.  An entry whose w or h is 0, or whose point count is not 4
+ * or an even number in [6, 2 (B2O_MAX_POLY_SEGMENTS + 1)], gets an all-zero crop; a singular segment zero columns. */
+int b2o_warp_polys(b2o_ctx* ctx, const uint8_t* img_dev, int channels, int n, int h, int w, const float* polys_dev,
+                   const int32_t* points_dev, const int32_t* image_index_dev, int n_polys, uint8_t* crops_dev,
+                   void* crnn_in_dev, void* stream);
 
 /* Choosing between the readings of several quarter turns.  Inputs: the results of n_turns runs of
  * b2o_warp_boxes_turned + a decoder (b2o_crnn_forward_scored, _beam or _lexicon), stacked in the order of turns_host

@@ -21,6 +21,8 @@ MAX_LEXICON_TOP_PATHS = 128   # B2O_MAX_LEXICON_TOP_PATHS
 ROTATION_VOTE_WORD, ROTATION_VOTE_PAGE = 0, 1   # B2O_ROTATION_VOTE_WORD / _PAGE
 MAX_ALIGN_PATHS = 128         # B2O_MAX_ALIGN_PATHS
 CRAFT_LAST_STEP = 30          # B2O_CRAFT_LAST_STEP
+MAX_POLY_SEGMENTS = 8         # B2O_MAX_POLY_SEGMENTS
+POLY_POINTS = 2 * (MAX_POLY_SEGMENTS + 1)   # points per entry of a dense polygon table
 
 
 class B2OError(RuntimeError):
@@ -72,6 +74,9 @@ SIGNATURES = {
     "b2o_get_boxes": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _i, _vp, _sz, _vp]),
     "b2o_get_boxes_scored": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp, _i, _vp, _sz, _vp]),
     "b2o_compact_boxes": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "b2o_get_boxes_poly": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _sz, _vp]),
+    "b2o_compact_polys": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "b2o_warp_polys": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
     "b2o_record_floats": (_sz, [_i]),
     "b2o_record_floats_scored": (_sz, [_i]),
     "b2o_pack_records": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
@@ -260,6 +265,20 @@ class Context:
     def compact_boxes(self, boxes, counts, n, max_boxes, flat, image_index, stream):
         self._check(self.lib.b2o_compact_boxes(self.handle, boxes, counts, n, max_boxes, flat, image_index, stream),
                     "b2o_compact_boxes")
+
+    def get_boxes_poly(self, scores, n, hs, ws, det, text, link, size, boxes, counts, box_scores, polys, points,
+                       max_boxes, wsp, ws_bytes, stream):
+        self._check(self.lib.b2o_get_boxes_poly(self.handle, scores, n, hs, ws, det, text, link, size, boxes, counts,
+                                                box_scores, polys, points, max_boxes, wsp, ws_bytes, stream),
+                    "b2o_get_boxes_poly")
+
+    def compact_polys(self, polys, points, counts, n, max_boxes, flat_polys, flat_points, image_index, stream):
+        self._check(self.lib.b2o_compact_polys(self.handle, polys, points, counts, n, max_boxes, flat_polys, flat_points,
+                                               image_index, stream), "b2o_compact_polys")
+
+    def warp_polys(self, img, channels, n, h, w, polys, points, image_index, n_polys, crops, crnn_in, stream):
+        self._check(self.lib.b2o_warp_polys(self.handle, img, channels, n, h, w, polys, points, image_index, n_polys,
+                                            crops, crnn_in, stream), "b2o_warp_polys")
 
     def record_floats(self, rec_boxes):
         return int(self.lib.b2o_record_floats(rec_boxes))

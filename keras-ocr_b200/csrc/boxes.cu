@@ -437,14 +437,230 @@ __device__ __forceinline__ bool fits_words(const Roi& r, int words) {
   return r.plane_words <= words && 56 * r.rh + 64 <= 4 * words;
 }
 
-// One component -> one quad.  `dyn_smem` holds two planes of `smem_plane_words` words; a component whose planes
+// --------------------------------------------------------------------------- polygon stage (b2o_get_boxes_poly)
+// Per kept component, after its box: a polygon along the centre line of its filled blob B (DESIGN.md section 1).
+// Every per-pixel expression is fp64 with a fixed operation order and every reduction is an integer sum or a max, so
+// the result does not depend on which thread saw which pixel (tests/polygon_refs.py restates it on the CPU).
+constexpr int kMaxSeg = B2O_MAX_POLY_SEGMENTS;
+constexpr int kPolyPoints = 2 * (kMaxSeg + 1);
+constexpr double kStraightness = 0.25;   // max |v(c_j) - mean v| <= 0.25 t: straight, keep the rectangle
+
+struct PolyState {
+  double ox, oy, eux, euy, evx, evy, W, t;
+  int S;                                  // bands; 0 = keep the rectangle
+  unsigned long long cnt;                 // |B|
+  long long bx[kMaxSeg], by[kMaxSeg], bn[kMaxSeg];
+  unsigned long long ext[2];              // float bits of the (non-negative) end extensions
+  unsigned long long rho[kMaxSeg];        // float bits of each band's largest distance from its chord
+  double cu[kMaxSeg], cv[kMaxSeg];        // band centroids in the frame
+  double qu[kMaxSeg + 1], qv[kMaxSeg + 1];
+  double gu[kMaxSeg], gv[kMaxSeg];        // unit chord directions q_j -> q_j+1
+  double e0u, e0v, e1u, e1v;              // unit end chords c_1 -> c_0 and c_S-2 -> c_S-1
+};
+
+__device__ __forceinline__ void frame_of(const PolyState& P, double x, double y, double* u, double* v) {
+  const double dx = __dsub_rn(x, P.ox), dy = __dsub_rn(y, P.oy);
+  *u = __dadd_rn(__dmul_rn(dx, P.eux), __dmul_rn(dy, P.euy));
+  *v = __dadd_rn(__dmul_rn(dx, P.evx), __dmul_rn(dy, P.evy));
+}
+
+__device__ __forceinline__ int band_of(const PolyState& P, double u) {
+  const double f = floor(__ddiv_rn(__dmul_rn(static_cast<double>(P.S), u), P.W));
+  return f < 0.0 ? 0 : (f > P.S - 1 ? P.S - 1 : static_cast<int>(f));
+}
+
+// (du, dv) / |(du, dv)|; false for a zero vector
+__device__ __forceinline__ bool unit2(double du, double dv, double* ou, double* ov) {
+  const double len = sqrt(__dadd_rn(__dmul_rn(du, du), __dmul_rn(dv, dv)));
+  if (!(len > 0.0)) return false;
+  *ou = __ddiv_rn(du, len);
+  *ov = __ddiv_rn(dv, len);
+  return true;
+}
+
+// f(x, y) for every pixel of the plane, (x, y) in score-map pixels
+template <class F>
+__device__ __forceinline__ void for_blob_pixels(const uint32_t* A, int plane_words, int stride, int sx, int sy, F f) {
+  for (int i = threadIdx.x; i < plane_words; i += blockDim.x) {
+    uint32_t v = A[i];
+    const int ry = i / stride, k = i - ry * stride;
+    while (v) {
+      const int b = __ffs(v) - 1;
+      v &= v - 1;
+      f(sx + 32 * k + b, sy + ry);
+    }
+  }
+}
+
+// Called by every thread of the block; box = the component's box in score-map pixels (tl, tr, br, bl).
+__device__ void poly_of_blob(const uint32_t* A, int plane_words, int stride, int sx, int sy, const float* box,
+                             float* __restrict__ out, int* __restrict__ points) {
+  __shared__ PolyState P;
+  if (threadIdx.x == 0) P.cnt = 0;
+  __syncthreads();
+  {
+    unsigned long long c = 0;
+    for (int i = threadIdx.x; i < plane_words; i += blockDim.x) c += __popc(A[i]);
+    if (c) atomicAdd(&P.cnt, c);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    P.S = 0;
+    P.ox = box[0]; P.oy = box[1];
+    const double ux = __dsub_rn(static_cast<double>(box[2]), P.ox), uy = __dsub_rn(static_cast<double>(box[3]), P.oy);
+    const double vx = __dsub_rn(static_cast<double>(box[6]), P.ox), vy = __dsub_rn(static_cast<double>(box[7]), P.oy);
+    P.W = sqrt(__dadd_rn(__dmul_rn(ux, ux), __dmul_rn(uy, uy)));
+    if (P.cnt > 0 && unit2(ux, uy, &P.eux, &P.euy) && unit2(vx, vy, &P.evx, &P.evy)) {
+      P.t = __ddiv_rn(static_cast<double>(P.cnt), P.W);                   // mean thickness
+      const double r = __ddiv_rn(P.W, P.t);
+      const int S = r >= kMaxSeg ? kMaxSeg : static_cast<int>(floor(r));
+      if (S >= 3) P.S = S;
+    }
+    for (int j = 0; j < kMaxSeg; ++j) { P.bx[j] = P.by[j] = P.bn[j] = 0; P.rho[j] = 0; }
+    P.ext[0] = P.ext[1] = 0;
+  }
+  __syncthreads();
+  if (P.S) {
+    long long lx[kMaxSeg], ly[kMaxSeg], ln[kMaxSeg];
+    for (int j = 0; j < kMaxSeg; ++j) lx[j] = ly[j] = ln[j] = 0;
+    for_blob_pixels(A, plane_words, stride, sx, sy, [&](int x, int y) {
+      double u, v;
+      frame_of(P, x, y, &u, &v);
+      const int j = band_of(P, u);
+      lx[j] += x; ly[j] += y; ln[j] += 1;
+    });
+    for (int j = 0; j < P.S; ++j)
+      if (ln[j]) {
+        atomicAdd(reinterpret_cast<unsigned long long*>(&P.bx[j]), static_cast<unsigned long long>(lx[j]));
+        atomicAdd(reinterpret_cast<unsigned long long*>(&P.by[j]), static_cast<unsigned long long>(ly[j]));
+        atomicAdd(reinterpret_cast<unsigned long long*>(&P.bn[j]), static_cast<unsigned long long>(ln[j]));
+      }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && P.S) {
+    const int S = P.S;
+    bool ok = true;
+    double vsum = 0.0;
+    for (int j = 0; j < S; ++j) {
+      if (P.bn[j] == 0) { ok = false; break; }
+      const double n = static_cast<double>(P.bn[j]);
+      frame_of(P, __ddiv_rn(static_cast<double>(P.bx[j]), n), __ddiv_rn(static_cast<double>(P.by[j]), n), &P.cu[j],
+               &P.cv[j]);
+      vsum = __dadd_rn(vsum, P.cv[j]);
+    }
+    if (ok) {
+      const double vbar = __ddiv_rn(vsum, static_cast<double>(S));
+      double dev = 0.0;
+      for (int j = 0; j < S; ++j) dev = fmax(dev, fabs(__dsub_rn(P.cv[j], vbar)));
+      ok = dev > __dmul_rn(kStraightness, P.t);
+    }
+    if (ok) {
+      for (int j = 1; j < S; ++j) {
+        P.qu[j] = __dmul_rn(__dadd_rn(P.cu[j - 1], P.cu[j]), 0.5);
+        P.qv[j] = __dmul_rn(__dadd_rn(P.cv[j - 1], P.cv[j]), 0.5);
+      }
+      ok = unit2(__dsub_rn(P.cu[0], P.cu[1]), __dsub_rn(P.cv[0], P.cv[1]), &P.e0u, &P.e0v) &&
+           unit2(__dsub_rn(P.cu[S - 1], P.cu[S - 2]), __dsub_rn(P.cv[S - 1], P.cv[S - 2]), &P.e1u, &P.e1v);
+    }
+    if (!ok) P.S = 0;
+  }
+  __syncthreads();
+  if (P.S) {
+    // end chords: extend from c_0 (c_S-1) until the end band's farthest pixel along the chord is covered
+    double m0 = 0.0, m1 = 0.0;
+    const int last = P.S - 1;
+    for_blob_pixels(A, plane_words, stride, sx, sy, [&](int x, int y) {
+      double u, v;
+      frame_of(P, x, y, &u, &v);
+      const int j = band_of(P, u);
+      if (j == 0)
+        m0 = fmax(m0, __dadd_rn(__dmul_rn(__dsub_rn(u, P.cu[0]), P.e0u), __dmul_rn(__dsub_rn(v, P.cv[0]), P.e0v)));
+      if (j == last)
+        m1 = fmax(m1, __dadd_rn(__dmul_rn(__dsub_rn(u, P.cu[last]), P.e1u),
+                                __dmul_rn(__dsub_rn(v, P.cv[last]), P.e1v)));
+    });
+    if (m0 > 0.0) atomicMax(&P.ext[0], static_cast<unsigned long long>(__double_as_longlong(m0)));
+    if (m1 > 0.0) atomicMax(&P.ext[1], static_cast<unsigned long long>(__double_as_longlong(m1)));
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && P.S) {
+    const int S = P.S;
+    const double x0 = __longlong_as_double(static_cast<long long>(P.ext[0]));
+    const double x1 = __longlong_as_double(static_cast<long long>(P.ext[1]));
+    P.qu[0] = __dadd_rn(P.cu[0], __dmul_rn(x0, P.e0u));
+    P.qv[0] = __dadd_rn(P.cv[0], __dmul_rn(x0, P.e0v));
+    P.qu[S] = __dadd_rn(P.cu[S - 1], __dmul_rn(x1, P.e1u));
+    P.qv[S] = __dadd_rn(P.cv[S - 1], __dmul_rn(x1, P.e1v));
+    bool ok = true;
+    for (int j = 0; j < S && ok; ++j)
+      ok = unit2(__dsub_rn(P.qu[j + 1], P.qu[j]), __dsub_rn(P.qv[j + 1], P.qv[j]), &P.gu[j], &P.gv[j]);
+    if (!ok) P.S = 0;
+  }
+  __syncthreads();
+  if (P.S) {
+    double lr[kMaxSeg];
+    for (int j = 0; j < kMaxSeg; ++j) lr[j] = 0.0;
+    for_blob_pixels(A, plane_words, stride, sx, sy, [&](int x, int y) {
+      double u, v;
+      frame_of(P, x, y, &u, &v);
+      const int j = band_of(P, u);
+      const double d = fabs(__dsub_rn(__dmul_rn(__dsub_rn(u, P.qu[j]), P.gv[j]), __dmul_rn(__dsub_rn(v, P.qv[j]), P.gu[j])));
+      lr[j] = fmax(lr[j], d);
+    });
+    for (int j = 0; j < P.S; ++j)
+      if (lr[j] > 0.0) atomicMax(&P.rho[j], static_cast<unsigned long long>(__double_as_longlong(lr[j])));
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  const int S = P.S;
+  if (!S) {                                                 // the rectangle: the box itself
+    for (int i = 0; i < 8; ++i) out[i] = 2.f * box[i];
+    for (int i = 8; i < 2 * kPolyPoints; ++i) out[i] = nanf("");
+    *points = 4;
+    return;
+  }
+  for (int j = 0; j <= S; ++j) {
+    const int a = j == 0 ? 0 : j - 1, b = j == S ? S : j + 1;
+    double tu, tv;
+    unit2(__dsub_rn(P.qu[b], P.qu[a]), __dsub_rn(P.qv[b], P.qv[a]), &tu, &tv);
+    const double nu = -tv, nv = tu;                         // towards +v: from the top edge to the bottom edge
+    double rho = 0.0;
+    if (j > 0) rho = fmax(rho, __longlong_as_double(static_cast<long long>(P.rho[j - 1])));
+    if (j < S) rho = fmax(rho, __longlong_as_double(static_cast<long long>(P.rho[j])));
+    const double side[2] = {-rho, rho};
+    for (int e = 0; e < 2; ++e) {
+      const double u = __dadd_rn(P.qu[j], __dmul_rn(side[e], nu)), v = __dadd_rn(P.qv[j], __dmul_rn(side[e], nv));
+      const double X = __dadd_rn(__dadd_rn(P.ox, __dmul_rn(u, P.eux)), __dmul_rn(v, P.evx));
+      const double Y = __dadd_rn(__dadd_rn(P.oy, __dmul_rn(u, P.euy)), __dmul_rn(v, P.evy));
+      const int slot = e == 0 ? j : 2 * S + 1 - j;
+      out[2 * slot] = 2.f * static_cast<float>(X);
+      out[2 * slot + 1] = 2.f * static_cast<float>(Y);
+    }
+  }
+  for (int i = 4 * (S + 1); i < 2 * kPolyPoints; ++i) out[i] = nanf("");
+  *points = 2 * (S + 1);
+}
+
+// ROI border seeds of the outside-background flood: the first / last row and column, where the plane is background
+__device__ __forceinline__ uint32_t roi_edge(int ry, int k, int rh, int stride, uint32_t last_valid) {
+  const uint32_t valid = k == stride - 1 ? last_valid : ~0u;
+  uint32_t edge = (ry == 0 || ry == rh - 1) ? valid : 0u;
+  if (k == 0) edge |= 1u;
+  if (k == stride - 1) edge |= (valid >> 1) + 1u;            // the ROI's last column
+  return edge;
+}
+
+// One component -> one quad (POLY: and its polygon, poly_of_blob).  `dyn_smem` holds two planes of `smem_plane_words` words; a component whose planes
 // do not fit works on the per-image global scratch planes instead (serialised by a per-image lock).
+template <bool POLY>
 __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* __restrict__ label, int hs, int ws,
                                   const Component c, int img, float* __restrict__ out,
                                   uint32_t* __restrict__ big_planes, int* __restrict__ big_locks,
-                                  uint32_t* dyn_smem, int smem_plane_words) {
+                                  uint32_t* dyn_smem, int smem_plane_words, float* __restrict__ poly_out,
+                                  int* __restrict__ points_out) {
   __shared__ int row_min[kMaxHullRows / 2], row_max[kMaxHullRows / 2];   // per blob row (<= 1024 rows)
   __shared__ int first_word;
+  __shared__ float pbox[8];                  // the box in score-map pixels, for the polygon stage
   const int hw = hs * ws;
   const uint8_t* M = mask + static_cast<size_t>(img) * hw;
   const int* L = label + static_cast<size_t>(img) * hw;
@@ -546,11 +762,7 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
       __syncthreads();
       for (int i = threadIdx.x; i < plane_words; i += blockDim.x) {
         const int ry = i / stride, k = i - ry * stride;
-        const uint32_t valid = k == stride - 1 ? last_valid : ~0u;
-        uint32_t edge = (ry == 0 || ry == rh - 1) ? valid : 0u;
-        if (k == 0) edge |= 1u;
-        if (k == stride - 1) edge |= (valid >> 1) + 1u;            // the ROI's last column
-        A[i] = edge & ~B[i];
+        A[i] = roi_edge(ry, k, rh, stride, last_valid) & ~B[i];
       }
       __syncthreads();
       if (threadIdx.x < 32) close_fill<true>(A, B, rh, stride, last_valid);
@@ -575,8 +787,26 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
   if (!have_blob) {
     // The reference raises IndexError here (contours[0] of an empty list); we emit a NaN box.
     if (threadIdx.x < 8) out[threadIdx.x] = nanf("");
+    if constexpr (POLY) {
+      for (int i = threadIdx.x; i < 2 * kPolyPoints; i += blockDim.x) poly_out[i] = nanf("");
+      if (threadIdx.x == 0) *points_out = 4;
+    }
     if (big) { __syncthreads(); if (threadIdx.x == 0) atomicExch(big_locks + img, 0); }
     return;
+  }
+  if (POLY && !filled) {
+    // the polygon stage reads the blob with its holes filled (drawContours(contours[0], thickness=-1)): flood the
+    // outside background into the free plane B and take its complement, as the two-blob branch above does
+    for (int i = threadIdx.x; i < plane_words; i += blockDim.x) {
+      const int ry = i / stride, k = i - ry * stride;
+      B[i] = roi_edge(ry, k, rh, stride, last_valid) & ~A[i];
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) close_fill<true>(B, A, rh, stride, last_valid);
+    __syncthreads();
+    for (int i = threadIdx.x; i < plane_words; i += blockDim.x)
+      A[i] = ~B[i] & ((i % stride) == stride - 1 ? last_valid : ~0u);
+    __syncthreads();
   }
   // per-row extents of the blob (ROI coordinates) ---------------------------------------------
   for (int r = threadIdx.x; r < rh; r += blockDim.x) {
@@ -591,7 +821,7 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
     row_min[r] = lo; row_max[r] = hi;
   }
   __syncthreads();
-  if (big) { if (threadIdx.x == 0) atomicExch(big_locks + img, 0); }
+  if (big && !POLY) { if (threadIdx.x == 0) atomicExch(big_locks + img, 0); }   // the polygon stage still reads A
 
   if (threadIdx.x == 0) {
     // hull stack lives in the (now free) plane B / dynamic smem: 2*rh points + 3*2*rh floats
@@ -670,16 +900,25 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
       for (int i = 0; i < 4; ++i) res[i] = box[(first + i) & 3];
     }
     for (int i = 0; i < 4; ++i) { out[2 * i] = 2.f * res[i].x; out[2 * i + 1] = 2.f * res[i].y; }
+    if constexpr (POLY)
+      for (int i = 0; i < 4; ++i) { pbox[2 * i] = res[i].x; pbox[2 * i + 1] = res[i].y; }
+  }
+  if constexpr (POLY) {
+    __syncthreads();
+    poly_of_blob(A, plane_words, stride, sx, sy, pbox, poly_out, points_out);
+    if (big) { __syncthreads(); if (threadIdx.x == 0) atomicExch(big_locks + img, 0); }
   }
 }
 
 // Pass 1, one block of 128 threads per (box slot, image) with SMALL planes: eight blocks per SM instead of the two
 // that 96 KB planes allow (the work is a chain of short latency-bound phases, which wants many resident blocks).  Components that do not fit are queued for pass 2.
+template <bool POLY>
 __global__ void __launch_bounds__(256)
 quads_kernel(const uint8_t* __restrict__ mask, const int* __restrict__ label, int hs, int ws,
              const Component* __restrict__ comps, const int* __restrict__ counts, int max_boxes,
              float* __restrict__ boxes, uint32_t* __restrict__ big_planes, int* __restrict__ big_locks,
-             int smem_plane_words, int* __restrict__ queue, int* __restrict__ queue_len) {
+             int smem_plane_words, int* __restrict__ queue, int* __restrict__ queue_len, float* __restrict__ polys,
+             int* __restrict__ points) {
   extern __shared__ uint32_t dyn_smem[];
   const int img = blockIdx.y, slot = blockIdx.x;
   int cnt = counts[img];
@@ -691,21 +930,25 @@ quads_kernel(const uint8_t* __restrict__ mask, const int* __restrict__ label, in
     if (threadIdx.x == 0) queue[atomicAdd(queue_len, 1)] = static_cast<int>(id);
     return;
   }
-  quad_of_component(mask, label, hs, ws, c, img, boxes + id * 8, big_planes, big_locks, dyn_smem, smem_plane_words);
+  quad_of_component<POLY>(mask, label, hs, ws, c, img, boxes + id * 8, big_planes, big_locks, dyn_smem, smem_plane_words,
+                    polys ? polys + id * 2 * kPolyPoints : nullptr, points ? points + id : nullptr);
 }
 
 // Pass 2, a few blocks with the large planes walking the queue of pass 1 (normally empty).
+template <bool POLY>
 __global__ void __launch_bounds__(256)
 quads_queue_kernel(const uint8_t* __restrict__ mask, const int* __restrict__ label, int hs, int ws,
                    const Component* __restrict__ comps, int max_boxes, float* __restrict__ boxes,
                    uint32_t* __restrict__ big_planes, int* __restrict__ big_locks, int smem_plane_words,
-                   const int* __restrict__ queue, const int* __restrict__ queue_len) {
+                   const int* __restrict__ queue, const int* __restrict__ queue_len, float* __restrict__ polys,
+                   int* __restrict__ points) {
   extern __shared__ uint32_t dyn_smem[];
   const int len = *queue_len;
   for (int i = blockIdx.x; i < len; i += gridDim.x) {
     const int id = queue[i];
-    quad_of_component(mask, label, hs, ws, comps[id], id / max_boxes, boxes + static_cast<size_t>(id) * 8, big_planes,
-                      big_locks, dyn_smem, smem_plane_words);
+    quad_of_component<POLY>(mask, label, hs, ws, comps[id], id / max_boxes, boxes + static_cast<size_t>(id) * 8, big_planes,
+                      big_locks, dyn_smem, smem_plane_words,
+                      polys ? polys + static_cast<size_t>(id) * 2 * kPolyPoints : nullptr, points ? points + id : nullptr);
     __syncthreads();       // thread 0 builds the hull in the planes' shared memory after the others have left
   }
 }
@@ -758,10 +1001,12 @@ extern "C" int b2o_get_boxes(b2o_ctx* ctx, const float* scores, int n, int hs, i
                               size_threshold, boxes, counts, nullptr, max_boxes, ws_dev, ws_bytes, stream);
 }
 
-extern "C" int b2o_get_boxes_scored(b2o_ctx* ctx, const float* scores, int n, int hs, int ws,
-                                    float detection_threshold, float text_threshold, float link_threshold,
-                                    int size_threshold, float* boxes, int32_t* counts, float* box_scores,
-                                    int max_boxes, void* ws_dev, size_t ws_bytes, void* stream) {
+namespace {
+
+// b2o_get_boxes_scored; polys / points non-NULL: also the polygon stage (b2o_get_boxes_poly)
+int get_boxes(b2o_ctx* ctx, const float* scores, int n, int hs, int ws, float detection_threshold, float text_threshold,
+              float link_threshold, int size_threshold, float* boxes, int32_t* counts, float* box_scores, float* polys,
+              int32_t* points, int max_boxes, void* ws_dev, size_t ws_bytes, void* stream) {
   if (!ctx) return B2O_ERR_ARG;
   DeviceGuard guard(ctx->device);
   if (!scores || !boxes || !counts || !ws_dev || n <= 0 || hs <= 0 || ws <= 0 || max_boxes <= 0) {
@@ -799,19 +1044,43 @@ extern "C" int b2o_get_boxes_scored(b2o_ctx* ctx, const float* scores, int n, in
   B2O_LAUNCH_CHECK(ctx);
   const int dyn = 2 * kQuadSmemPlaneWords * 4, dyn_small = 2 * kQuadSmallPlaneWords * 4;
   if (!ctx->quads_configured) {        // a per-device attribute, hence per context (one context per device)
-    B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(quads_queue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
+    B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(quads_queue_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
+    B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(quads_queue_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
     ctx->quads_configured = true;
   }
-  quads_kernel<<<dim3(max_boxes, n), 128, dyn_small, st>>>(w.mask, w.label, hs, ws, w.comps, counts, max_boxes, boxes,
-                                                           w.big_planes, w.big_locks, kQuadSmallPlaneWords, w.queue,
-                                                           w.queue_len);
+  // the polygon stage is a separate instance, so the plain getBoxes kernels keep their registers and occupancy
+  auto quads = polys ? quads_kernel<true> : quads_kernel<false>;
+  auto queue = polys ? quads_queue_kernel<true> : quads_queue_kernel<false>;
+  quads<<<dim3(max_boxes, n), 128, dyn_small, st>>>(w.mask, w.label, hs, ws, w.comps, counts, max_boxes, boxes,
+                                                    w.big_planes, w.big_locks, kQuadSmallPlaneWords, w.queue,
+                                                    w.queue_len, polys, points);
   B2O_LAUNCH_CHECK(ctx);
   const long long slots = static_cast<long long>(n) * max_boxes;
-  quads_queue_kernel<<<static_cast<unsigned>(std::min<long long>(slots, 2 * ctx->sm_count)), 256, dyn, st>>>(
+  queue<<<static_cast<unsigned>(std::min<long long>(slots, 2 * ctx->sm_count)), 256, dyn, st>>>(
       w.mask, w.label, hs, ws, w.comps, max_boxes, boxes, w.big_planes, w.big_locks, kQuadSmemPlaneWords, w.queue,
-      w.queue_len);
+      w.queue_len, polys, points);
   B2O_LAUNCH_CHECK(ctx);
   return B2O_OK;
+}
+
+}  // namespace
+
+extern "C" int b2o_get_boxes_scored(b2o_ctx* ctx, const float* scores, int n, int hs, int ws,
+                                    float detection_threshold, float text_threshold, float link_threshold,
+                                    int size_threshold, float* boxes, int32_t* counts, float* box_scores,
+                                    int max_boxes, void* ws_dev, size_t ws_bytes, void* stream) {
+  return get_boxes(ctx, scores, n, hs, ws, detection_threshold, text_threshold, link_threshold, size_threshold, boxes,
+                   counts, box_scores, nullptr, nullptr, max_boxes, ws_dev, ws_bytes, stream);
+}
+
+extern "C" int b2o_get_boxes_poly(b2o_ctx* ctx, const float* scores, int n, int hs, int ws, float detection_threshold,
+                                  float text_threshold, float link_threshold, int size_threshold, float* boxes,
+                                  int32_t* counts, float* box_scores, float* polys, int32_t* points, int max_boxes,
+                                  void* ws_dev, size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!polys || !points) { ctx->set_error("b2o_get_boxes_poly: bad argument"); return B2O_ERR_ARG; }
+  return get_boxes(ctx, scores, n, hs, ws, detection_threshold, text_threshold, link_threshold, size_threshold, boxes,
+                   counts, box_scores, polys, points, max_boxes, ws_dev, ws_bytes, stream);
 }
 
 namespace {
@@ -885,6 +1154,23 @@ compact_boxes_kernel(const float* __restrict__ boxes, const int32_t* __restrict_
   for (int t = threadIdx.x; t < c; t += blockDim.x) image_index[off + t] = i;
 }
 
+__global__ void __launch_bounds__(128)
+compact_polys_kernel(const float* __restrict__ polys, const int32_t* __restrict__ points,
+                     const int32_t* __restrict__ counts, int max_boxes, float* __restrict__ flat,
+                     int32_t* __restrict__ flat_points, int32_t* __restrict__ image_index) {
+  const int i = blockIdx.x;
+  const int off = boxes_before(counts, i, max_boxes);
+  const int c = min(max(counts[i], 0), max_boxes);
+  constexpr int kFloats = 2 * kPolyPoints;                 // 36 floats = 9 float4 per entry
+  const float4* src = reinterpret_cast<const float4*>(polys + static_cast<size_t>(i) * max_boxes * kFloats);
+  float4* dst = reinterpret_cast<float4*>(flat + static_cast<size_t>(off) * kFloats);
+  for (int t = threadIdx.x; t < c * (kFloats / 4); t += blockDim.x) dst[t] = src[t];
+  for (int t = threadIdx.x; t < c; t += blockDim.x) {
+    flat_points[off + t] = points[static_cast<size_t>(i) * max_boxes + t];
+    image_index[off + t] = i;
+  }
+}
+
 constexpr int kSteps = 48;                         // label steps per word (recognition.py:20: 50 - 2 discarded)
 
 // SCORES: the record goes on with rec_boxes detection scores (box_scores, (n, max_boxes) as b2o_get_boxes_scored writes
@@ -940,6 +1226,21 @@ extern "C" int b2o_compact_boxes(b2o_ctx* ctx, const float* boxes, const int32_t
   }
   compact_boxes_kernel<<<n, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(boxes, counts, max_boxes, flat,
                                                                             image_index);
+  B2O_LAUNCH_CHECK(ctx);
+  return B2O_OK;
+}
+
+extern "C" int b2o_compact_polys(b2o_ctx* ctx, const float* polys, const int32_t* points, const int32_t* counts, int n,
+                                 int max_boxes, float* flat_polys, int32_t* flat_points, int32_t* image_index,
+                                 void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  DeviceGuard guard(ctx->device);
+  if (!polys || !points || !counts || !flat_polys || !flat_points || !image_index || n <= 0 || max_boxes <= 0) {
+    ctx->set_error("b2o_compact_polys: bad argument");
+    return B2O_ERR_ARG;
+  }
+  compact_polys_kernel<<<n, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(polys, points, counts, max_boxes,
+                                                                             flat_polys, flat_points, image_index);
   B2O_LAUNCH_CHECK(ctx);
   return B2O_OK;
 }

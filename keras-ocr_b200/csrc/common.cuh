@@ -222,21 +222,12 @@ static __device__ inline bool warp_extent(const float* q /*4x2*/, int turn, int 
   return true;
 }
 
-// b2o_warp_plan (include/b2ocr.h): m[9] = inverse homography (destination -> source), fp64 like cv2; dw, dh = dsize
-// of warpPerspective; valid = 0 where warpBox raises ZeroDivisionError (or the system is singular).
-static __device__ inline void plan_warp(const float* q /*4x2*/, int turn, int target_w, int target_h, b2o_warp_plan* plan) {
-  plan->valid = 0;
-  float box[8];
-  double sw, sh;
-  if (!warp_extent(q, turn, target_w, target_h, box, &sw, &sh)) return;
-  const float dst[8] = {0.f, 0.f, static_cast<float>(sw), 0.f, static_cast<float>(sw), static_cast<float>(sh),
-                        0.f, static_cast<float>(sh)};
-  plan->dw = static_cast<int>(sw);
-  plan->dh = static_cast<int>(sh);
-  // --- cv2.getPerspectiveTransform: 8x8 system, LU with partial pivoting in fp64 -----------------
+// cv2.getPerspectiveTransform(src, dst) (8x8 system, LU with partial pivoting, fp64) followed by cv::invert of the
+// 3x3 (closed form): m[9] = the inverse homography, destination -> source.  False where the system is singular.
+static __device__ inline bool persp_inverse(const float* src /*4x2*/, const float* dst /*4x2*/, double m[9]) {
   double A[8][8], b[8];
   for (int i = 0; i < 4; ++i) {
-    const double sxx = box[2 * i], syy = box[2 * i + 1], dx = dst[2 * i], dy = dst[2 * i + 1];
+    const double sxx = src[2 * i], syy = src[2 * i + 1], dx = dst[2 * i], dy = dst[2 * i + 1];
     for (int k = 0; k < 8; ++k) { A[i][k] = 0.0; A[i + 4][k] = 0.0; }
     A[i][0] = A[i + 4][3] = sxx;
     A[i][1] = A[i + 4][4] = syy;
@@ -252,7 +243,7 @@ static __device__ inline void plan_warp(const float* q /*4x2*/, int turn, int ta
     int k = i;
     for (int j = i + 1; j < 8; ++j)
       if (fabs(A[j][i]) > fabs(A[k][i])) k = j;
-    if (fabs(A[k][i]) < 2.220446049250313e-14) return;     // DBL_EPSILON*100: singular
+    if (fabs(A[k][i]) < 2.220446049250313e-14) return false;     // DBL_EPSILON*100: singular
     if (k != i) {
       for (int j = i; j < 8; ++j) { const double t = A[i][j]; A[i][j] = A[k][j]; A[k][j] = t; }
       const double t = b[i]; b[i] = b[k]; b[k] = t;
@@ -270,27 +261,40 @@ static __device__ inline void plan_warp(const float* q /*4x2*/, int turn, int ta
     b[i] = s / A[i][i];
   }
   const double M[9] = {b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7], 1.0};
-  // --- cv::invert of a 3x3 (closed form) -----------------------------------------------------------
 #define MM(r, c) M[(r) * 3 + (c)]
 #define DET2(a, b, c, d) __dsub_rn(__dmul_rn(a, b), __dmul_rn(c, d))
   const double det = __dadd_rn(
       __dsub_rn(__dmul_rn(MM(0, 0), DET2(MM(1, 1), MM(2, 2), MM(1, 2), MM(2, 1))),
                 __dmul_rn(MM(0, 1), DET2(MM(1, 0), MM(2, 2), MM(1, 2), MM(2, 0)))),
       __dmul_rn(MM(0, 2), DET2(MM(1, 0), MM(2, 1), MM(1, 1), MM(2, 0))));
-  if (det == 0.0) return;
+  if (det == 0.0) return false;
   const double id = 1.0 / det;
-  plan->m[0] = __dmul_rn(DET2(MM(1, 1), MM(2, 2), MM(1, 2), MM(2, 1)), id);
-  plan->m[1] = __dmul_rn(DET2(MM(0, 2), MM(2, 1), MM(0, 1), MM(2, 2)), id);
-  plan->m[2] = __dmul_rn(DET2(MM(0, 1), MM(1, 2), MM(0, 2), MM(1, 1)), id);
-  plan->m[3] = __dmul_rn(DET2(MM(1, 2), MM(2, 0), MM(1, 0), MM(2, 2)), id);
-  plan->m[4] = __dmul_rn(DET2(MM(0, 0), MM(2, 2), MM(0, 2), MM(2, 0)), id);
-  plan->m[5] = __dmul_rn(DET2(MM(0, 2), MM(1, 0), MM(0, 0), MM(1, 2)), id);
-  plan->m[6] = __dmul_rn(DET2(MM(1, 0), MM(2, 1), MM(1, 1), MM(2, 0)), id);
-  plan->m[7] = __dmul_rn(DET2(MM(0, 1), MM(2, 0), MM(0, 0), MM(2, 1)), id);
-  plan->m[8] = __dmul_rn(DET2(MM(0, 0), MM(1, 1), MM(0, 1), MM(1, 0)), id);
+  m[0] = __dmul_rn(DET2(MM(1, 1), MM(2, 2), MM(1, 2), MM(2, 1)), id);
+  m[1] = __dmul_rn(DET2(MM(0, 2), MM(2, 1), MM(0, 1), MM(2, 2)), id);
+  m[2] = __dmul_rn(DET2(MM(0, 1), MM(1, 2), MM(0, 2), MM(1, 1)), id);
+  m[3] = __dmul_rn(DET2(MM(1, 2), MM(2, 0), MM(1, 0), MM(2, 2)), id);
+  m[4] = __dmul_rn(DET2(MM(0, 0), MM(2, 2), MM(0, 2), MM(2, 0)), id);
+  m[5] = __dmul_rn(DET2(MM(0, 2), MM(1, 0), MM(0, 0), MM(1, 2)), id);
+  m[6] = __dmul_rn(DET2(MM(1, 0), MM(2, 1), MM(1, 1), MM(2, 0)), id);
+  m[7] = __dmul_rn(DET2(MM(0, 1), MM(2, 0), MM(0, 0), MM(2, 1)), id);
+  m[8] = __dmul_rn(DET2(MM(0, 0), MM(1, 1), MM(0, 1), MM(1, 0)), id);
 #undef MM
 #undef DET2
-  plan->valid = 1;
+  return true;
+}
+
+// b2o_warp_plan (include/b2ocr.h): m[9] = inverse homography (destination -> source), fp64 like cv2; dw, dh = dsize
+// of warpPerspective; valid = 0 where warpBox raises ZeroDivisionError (or the system is singular).
+static __device__ inline void plan_warp(const float* q /*4x2*/, int turn, int target_w, int target_h, b2o_warp_plan* plan) {
+  plan->valid = 0;
+  float box[8];
+  double sw, sh;
+  if (!warp_extent(q, turn, target_w, target_h, box, &sw, &sh)) return;
+  const float dst[8] = {0.f, 0.f, static_cast<float>(sw), 0.f, static_cast<float>(sw), static_cast<float>(sh),
+                        0.f, static_cast<float>(sh)};
+  plan->dw = static_cast<int>(sw);
+  plan->dh = static_cast<int>(sh);
+  if (persp_inverse(box, dst, plan->m)) plan->valid = 1;
 }
 
 static inline TensorView make_view(void* base, int n, int h, int w, int c, int ld = 0, int coff = 0) {

@@ -80,6 +80,51 @@ __global__ void gray_kernel(const uint8_t* __restrict__ img, long long total, ui
 using WarpPlan = b2o_warp_plan;
 
 constexpr int kCropH = 31, kCropW = 200;
+constexpr int kMaxPolySegments = B2O_MAX_POLY_SEGMENTS;
+
+// cv2.warpPerspective INTER_LINEAR (BORDER_CONSTANT 0) of one crop pixel (x, y) through the inverse map m, with
+// cv::WarpPerspectiveInvoker's block width bw0 (x is re-based at multiples of it): 1/32-pixel coordinates, 15-bit
+// weights.  Shared by warp_kernel and warp_polys_kernel.
+template <int CH>
+__device__ __forceinline__ void warp_sample(const uint8_t* __restrict__ g, int H, int W, const double* m, int x, int y,
+                                            int bw0, int v[CH]) {
+  const int bx = (x / bw0) * bw0, x1 = x - bx;
+  const double X0 = __dadd_rn(__dadd_rn(__dmul_rn(m[0], bx), __dmul_rn(m[1], y)), m[2]);
+  const double Y0 = __dadd_rn(__dadd_rn(__dmul_rn(m[3], bx), __dmul_rn(m[4], y)), m[5]);
+  const double W0 = __dadd_rn(__dadd_rn(__dmul_rn(m[6], bx), __dmul_rn(m[7], y)), m[8]);
+  double Wv = __dadd_rn(W0, __dmul_rn(m[6], x1));
+  Wv = Wv != 0.0 ? 32.0 / Wv : 0.0;
+  const double fX = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(__dadd_rn(X0, __dmul_rn(m[0], x1)), Wv)));
+  const double fY = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(__dadd_rn(Y0, __dmul_rn(m[3], x1)), Wv)));
+  const int X = __double2int_rn(fX), Y = __double2int_rn(fY);
+  const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);
+  const int ax = X & 31, ay = Y & 31;
+  const bool x0ok = sx >= 0 && sx < W, x1ok = sx + 1 >= 0 && sx + 1 < W;
+  const bool y0ok = sy >= 0 && sy < H, y1ok = sy + 1 >= 0 && sy + 1 < H;
+  // BilinearTab_i: (1-fx)(1-fy) ... scaled to 2^15; exact for 1/32 steps
+  const int w00 = (32 - ax) * (32 - ay) * 32, w01 = ax * (32 - ay) * 32;
+  const int w10 = (32 - ax) * ay * 32, w11 = ax * ay * 32;
+#pragma unroll
+  for (int c = 0; c < CH; ++c) {
+    const int p00 = (x0ok && y0ok) ? g[(static_cast<size_t>(sy) * W + sx) * CH + c] : 0;
+    const int p01 = (x1ok && y0ok) ? g[(static_cast<size_t>(sy) * W + sx + 1) * CH + c] : 0;
+    const int p10 = (x0ok && y1ok) ? g[(static_cast<size_t>(sy + 1) * W + sx) * CH + c] : 0;
+    const int p11 = (x1ok && y1ok) ? g[(static_cast<size_t>(sy + 1) * W + sx + 1) * CH + c] : 0;
+    v[c] = (p00 * w00 + p01 * w01 + p10 * w10 + p11 * w11 + 16384) >> 15;
+  }
+}
+
+// The crop tile of one word -> crops (optional) and the CRNN input (optional).  Layout (recognition.py:215-216):
+// x[t][j] = crop[30-j][t] / 255.  Called by all threads after the tile and crops are written.
+template <int CH>
+__device__ __forceinline__ void store_crnn_in(const uint8_t* tile, int k, __half* __restrict__ crnn_in) {
+  __half* o = crnn_in + static_cast<size_t>(k) * kCropH * kCropW * CH;
+  for (int i = threadIdx.x; i < kCropH * kCropW * CH; i += blockDim.x) {
+    const int c = i % CH, q = i / CH;
+    const int t = q / kCropH, j = q - t * kCropH;
+    o[i] = __float2half_rn(static_cast<float>(tile[((kCropH - 1 - j) * kCropW + t) * CH + c]) / 255.0f);
+  }
+}
 
 // CH = 1: gray image (n,H,W), crops (k,31,200), CRNN input (k,200,31).  CH = 3 (build_model(color=True),
 // recognition.py:214, 508-510: no gray conversion): RGB image (n,H,W,3), crops (k,31,200,3), CRNN input (k,200,31,3);
@@ -105,32 +150,102 @@ warp_kernel(const uint8_t* __restrict__ gray, int n, int H, int W, const float* 
     int v[CH];
 #pragma unroll
     for (int c = 0; c < CH; ++c) v[c] = 0;
-    if (x < dw && y < dh) {
-      const double* m = plan.m;
-      const int bx = (x / bw0) * bw0, x1 = x - bx;
-      const double X0 = __dadd_rn(__dadd_rn(__dmul_rn(m[0], bx), __dmul_rn(m[1], y)), m[2]);
-      const double Y0 = __dadd_rn(__dadd_rn(__dmul_rn(m[3], bx), __dmul_rn(m[4], y)), m[5]);
-      const double W0 = __dadd_rn(__dadd_rn(__dmul_rn(m[6], bx), __dmul_rn(m[7], y)), m[8]);
-      double Wv = __dadd_rn(W0, __dmul_rn(m[6], x1));
-      Wv = Wv != 0.0 ? 32.0 / Wv : 0.0;
-      const double fX = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(__dadd_rn(X0, __dmul_rn(m[0], x1)), Wv)));
-      const double fY = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(__dadd_rn(Y0, __dmul_rn(m[3], x1)), Wv)));
-      const int X = __double2int_rn(fX), Y = __double2int_rn(fY);
-      const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);
-      const int ax = X & 31, ay = Y & 31;
-      const bool x0ok = sx >= 0 && sx < W, x1ok = sx + 1 >= 0 && sx + 1 < W;
-      const bool y0ok = sy >= 0 && sy < H, y1ok = sy + 1 >= 0 && sy + 1 < H;
-      // BilinearTab_i: (1-fx)(1-fy) ... scaled to 2^15; exact for 1/32 steps
-      const int w00 = (32 - ax) * (32 - ay) * 32, w01 = ax * (32 - ay) * 32;
-      const int w10 = (32 - ax) * ay * 32, w11 = ax * ay * 32;
+    if (x < dw && y < dh) warp_sample<CH>(g, H, W, plan.m, x, y, bw0, v);
 #pragma unroll
-      for (int c = 0; c < CH; ++c) {
-        const int p00 = (x0ok && y0ok) ? g[(static_cast<size_t>(sy) * W + sx) * CH + c] : 0;
-        const int p01 = (x1ok && y0ok) ? g[(static_cast<size_t>(sy) * W + sx + 1) * CH + c] : 0;
-        const int p10 = (x0ok && y1ok) ? g[(static_cast<size_t>(sy + 1) * W + sx) * CH + c] : 0;
-        const int p11 = (x1ok && y1ok) ? g[(static_cast<size_t>(sy + 1) * W + sx + 1) * CH + c] : 0;
-        v[c] = (p00 * w00 + p01 * w01 + p10 * w10 + p11 * w11 + 16384) >> 15;
-      }
+    for (int c = 0; c < CH; ++c) {
+      tile[i * CH + c] = static_cast<uint8_t>(v[c]);
+      if (crops) crops[(static_cast<size_t>(k) * kCropH * kCropW + i) * CH + c] = static_cast<uint8_t>(v[c]);
+    }
+  }
+  if (crnn_in == nullptr) return;
+  __syncthreads();
+  store_crnn_in<CH>(tile, k, crnn_in);
+}
+
+// ------------------------------------------------------------------------------------ piecewise warpBox
+// One polygon of s segments (b2o_warp_polys): top edge t_0..t_s = poly[0..s], bottom edge b_i = poly[2s+1-i].
+// w = int(sum_i (|t_i t_i+1| + |b_i b_i+1|) / 2), h = int(mean_j |t_j b_j|), scale = min(200 / w, 31 / h), dsize =
+// (int(scale w), int(scale h)); segment i maps onto x in [X_i, X_i+1], X_i = float32(scale w * cum_i / cum_s) with cum
+// the running edge-mean length, y in [0, float32(scale h)].  A 4-point entry is warpBox itself (plan_warp).
+struct PolyPlan {
+  double m[kMaxPolySegments][9];
+  float X[kMaxPolySegments + 1];
+  int seg_ok[kMaxPolySegments];
+  int s, dw, dh, valid;
+};
+
+__device__ void plan_poly(const float* poly, int points, PolyPlan* p) {
+  p->valid = 0;
+  p->s = 1;
+  if (points == 4) {
+    b2o_warp_plan wp;
+    wp.dw = wp.dh = 0;
+    plan_warp(poly, 0, kCropW, kCropH, &wp);
+    if (!wp.valid) return;
+    for (int i = 0; i < 9; ++i) p->m[0][i] = wp.m[i];
+    p->seg_ok[0] = 1;
+    p->dw = wp.dw; p->dh = wp.dh; p->valid = 1;
+    return;
+  }
+  if (points < 6 || points > 2 * (kMaxPolySegments + 1) || (points & 1)) return;
+  const int s = points / 2 - 1;
+  const float* t = poly;
+  double cum[kMaxPolySegments + 1];
+  cum[0] = 0.0;
+  for (int i = 0; i < s; ++i) {
+    const double dt = corner_dist(t + 2 * i, t + 2 * (i + 1));
+    const double db = corner_dist(poly + 2 * (points - 1 - i), poly + 2 * (points - 2 - i));
+    cum[i + 1] = __dadd_rn(cum[i], __dadd_rn(dt, db) / 2);
+  }
+  double hs = 0.0;
+  for (int j = 0; j <= s; ++j) hs = __dadd_rn(hs, corner_dist(t + 2 * j, poly + 2 * (points - 1 - j)));
+  const int w = static_cast<int>(cum[s]);
+  const int h = static_cast<int>(hs / (s + 1));
+  if (w <= 0 || h <= 0) return;
+  const double sa = static_cast<double>(kCropW) / w, sb = static_cast<double>(kCropH) / h;
+  const double scale = sa < sb ? sa : sb;
+  const double sw = __dmul_rn(scale, w), sh = __dmul_rn(scale, h);
+  for (int i = 0; i <= s; ++i) p->X[i] = static_cast<float>(__dmul_rn(sw, cum[i] / cum[s]));
+  const float fsh = static_cast<float>(sh);
+  for (int i = 0; i < s; ++i) {
+    const float* ti = t + 2 * i;
+    const float* bi = poly + 2 * (points - 1 - i);
+    const float src[8] = {ti[0], ti[1], ti[2], ti[3], bi[-2], bi[-1], bi[0], bi[1]};
+    const float dst[8] = {p->X[i], 0.f, p->X[i + 1], 0.f, p->X[i + 1], fsh, p->X[i], fsh};
+    p->seg_ok[i] = persp_inverse(src, dst, p->m[i]) ? 1 : 0;
+  }
+  p->s = s;
+  p->dw = static_cast<int>(sw);
+  p->dh = static_cast<int>(sh);
+  p->valid = 1;
+}
+
+template <int CH>
+__global__ void __launch_bounds__(256)
+warp_polys_kernel(const uint8_t* __restrict__ img_all, int n, int H, int W, const float* __restrict__ polys,
+                  const int* __restrict__ points, const int* __restrict__ image_index, uint8_t* __restrict__ crops,
+                  __half* __restrict__ crnn_in) {
+  __shared__ PolyPlan plan;
+  __shared__ uint8_t tile[kCropH * kCropW * CH];
+  const int k = blockIdx.x;
+  if (threadIdx.x == 0) plan_poly(polys + static_cast<size_t>(k) * 4 * (kMaxPolySegments + 1), points[k], &plan);
+  __syncthreads();
+  int img = image_index[k];
+  img = min(max(img, 0), n - 1);
+  const uint8_t* g = img_all + static_cast<size_t>(img) * H * W * CH;
+  const int dw = plan.valid ? min(plan.dw, kCropW) : 0, dh = plan.valid ? min(plan.dh, kCropH) : 0;
+  int bh0 = min(16, max(dh, 1));
+  const int bw0 = min(1024 / bh0, max(dw, 1));
+  for (int i = threadIdx.x; i < kCropH * kCropW; i += blockDim.x) {
+    const int y = i / kCropW, x = i - y * kCropW;
+    int v[CH];
+#pragma unroll
+    for (int c = 0; c < CH; ++c) v[c] = 0;
+    if (x < dw && y < dh) {
+      int seg = 0;
+      const float fx = static_cast<float>(x);
+      for (int j = 1; j < plan.s; ++j) if (plan.X[j] <= fx) seg = j;
+      if (plan.seg_ok[seg]) warp_sample<CH>(g, H, W, plan.m[seg], x, y, bw0, v);
     }
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
@@ -140,13 +255,7 @@ warp_kernel(const uint8_t* __restrict__ gray, int n, int H, int W, const float* 
   }
   if (crnn_in == nullptr) return;
   __syncthreads();
-  // CRNN input layout (recognition.py:215-216): x[t][j] = crop[30-j][t] / 255
-  __half* o = crnn_in + static_cast<size_t>(k) * kCropH * kCropW * CH;
-  for (int i = threadIdx.x; i < kCropH * kCropW * CH; i += blockDim.x) {
-    const int c = i % CH, q = i / CH;
-    const int t = q / kCropH, j = q - t * kCropH;
-    o[i] = __float2half_rn(static_cast<float>(tile[((kCropH - 1 - j) * kCropW + t) * CH + c]) / 255.0f);
-  }
+  store_crnn_in<CH>(tile, k, crnn_in);
 }
 
 // b2o_warp_plan_test: plan_warp alone, one thread per box.  A degenerate box leaves m, dw and dh zero.
@@ -246,6 +355,28 @@ extern "C" int b2o_warp_boxes_turned(b2o_ctx* ctx, const uint8_t* img, int chann
                                      const float* boxes, const int32_t* image_index, int n_boxes, int turn,
                                      uint8_t* crops, void* crnn_in, void* stream) {
   return warp_boxes_impl(ctx, img, channels, n, h, w, boxes, image_index, n_boxes, turn, crops, crnn_in, stream);
+}
+
+extern "C" int b2o_warp_polys(b2o_ctx* ctx, const uint8_t* img, int channels, int n, int h, int w, const float* polys,
+                              const int32_t* points, const int32_t* image_index, int n_polys, uint8_t* crops,
+                              void* crnn_in, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  DeviceGuard guard(ctx->device);
+  if (channels != 1 && channels != 3) { ctx->set_error("b2o_warp_polys: channels must be 1 or 3"); return B2O_ERR_ARG; }
+  if (n_polys == 0) return B2O_OK;
+  if (!img || !polys || !points || !image_index || n <= 0 || h <= 0 || w <= 0 || n_polys < 0 || (!crops && !crnn_in)) {
+    ctx->set_error("b2o_warp_polys: bad argument");
+    return B2O_ERR_ARG;
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (channels == 3)
+    warp_polys_kernel<3><<<n_polys, 256, 0, st>>>(img, n, h, w, polys, points, image_index, crops,
+                                                  reinterpret_cast<__half*>(crnn_in));
+  else
+    warp_polys_kernel<1><<<n_polys, 256, 0, st>>>(img, n, h, w, polys, points, image_index, crops,
+                                                  reinterpret_cast<__half*>(crnn_in));
+  B2O_LAUNCH_CHECK(ctx);
+  return B2O_OK;
 }
 
 extern "C" int b2o_warp_plan_test(b2o_ctx* ctx, const float* boxes, int n, b2o_warp_plan* plans, void* stream) {

@@ -85,11 +85,14 @@ class Detector:
         return scores
 
     def boxes_enqueue(self, scores, detection_threshold=0.7, text_threshold=0.4, link_threshold=0.4,
-                      size_threshold=10, with_scores=False):
+                      size_threshold=10, with_scores=False, with_polygons=False):
         """getBoxes on the device, asynchronously: launches the kernels and the copy of the per-image counts into
         pinned memory, records an event and returns at once (``boxes_finish`` waits for that event only, so work
         enqueued afterwards keeps the GPU busy while the host reads the counts).  ``with_scores``: the state also
-        holds ``box_scores`` (N,M) float32 CUDA, each box's detection score (``b2o_get_boxes_scored``)."""
+        holds ``box_scores`` (N,M) float32 CUDA, each box's detection score (``b2o_get_boxes_scored``).
+        ``with_polygons``: the state also holds every box's polygon (``b2o_get_boxes_poly``), ``polys`` (N,M,18,2)
+        float32 and ``points`` (N,M) int32 CUDA, and their dense lists ``flat_polys`` / ``flat_points`` in the order
+        of ``flat``; boxes and scores are those of the call without polygons."""
         n, hs, ws_, _ = scores.shape
         stream = torch.cuda.current_stream(self.device)
         scores = scores.contiguous()
@@ -102,9 +105,16 @@ class Detector:
             self._box_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         wsp = self._box_ws
         thr = (float(detection_threshold), float(text_threshold), float(link_threshold), int(size_threshold))
-        box_scores = None
+        box_scores = polys = points = None
         if with_scores:
             box_scores = torch.empty((n, m), dtype=torch.float32, device=self.device)
+        if with_polygons:
+            polys = torch.empty((n, m, _lib.POLY_POINTS, 2), dtype=torch.float32, device=self.device)
+            points = torch.empty((n, m), dtype=torch.int32, device=self.device)
+            self.ctx.get_boxes_poly(scores.data_ptr(), n, hs, ws_, *thr, boxes.data_ptr(), counts.data_ptr(),
+                                    box_scores.data_ptr() if with_scores else None, polys.data_ptr(), points.data_ptr(),
+                                    m, wsp.data_ptr(), nbytes, stream.cuda_stream)
+        elif with_scores:
             self.ctx.get_boxes_scored(scores.data_ptr(), n, hs, ws_, *thr, boxes.data_ptr(), counts.data_ptr(),
                                       box_scores.data_ptr(), m, wsp.data_ptr(), nbytes, stream.cuda_stream)
         else:
@@ -120,19 +130,27 @@ class Detector:
         image_index = torch.empty((n * m,), dtype=torch.int32, device=self.device)
         self.ctx.compact_boxes(boxes.data_ptr(), counts.data_ptr(), n, m, flat.data_ptr(), image_index.data_ptr(),
                                stream.cuda_stream)
+        flat_polys = flat_points = None
+        if with_polygons:
+            flat_polys = torch.empty((n * m, _lib.POLY_POINTS, 2), dtype=torch.float32, device=self.device)
+            flat_points = torch.empty((n * m,), dtype=torch.int32, device=self.device)
+            self.ctx.compact_polys(polys.data_ptr(), points.data_ptr(), counts.data_ptr(), n, m, flat_polys.data_ptr(),
+                                   flat_points.data_ptr(), image_index.data_ptr(), stream.cuda_stream)
         return {"scores": scores, "boxes": boxes, "counts": counts, "counts_pin": counts_pin, "event": event, "m": m,
-                "thr": thr, "flat": flat, "image_index": image_index, "box_scores": box_scores}
+                "thr": thr, "flat": flat, "image_index": image_index, "box_scores": box_scores, "polys": polys,
+                "points": points, "flat_polys": flat_polys, "flat_points": flat_points}
 
     def boxes_finish(self, state):
         """Wait for ``boxes_enqueue``.  Returns (boxes (N,M,4,2) float32 CUDA, counts ndarray (N,)); re-runs
         getBoxes with a larger box table in the (rare) case an image had more boxes than the table holds (the state's
-        ``box_scores``, when asked for, then come from that run too)."""
+        ``box_scores`` and polygons, when asked for, then come from that run too)."""
         state["event"].synchronize()                     # the one synchronisation of the detector half
         counts_host = state["counts_pin"].numpy().copy()
         while counts_host.size and int(counts_host.max()) > state["boxes"].shape[1]:
             self.max_boxes = int(2 ** np.ceil(np.log2(int(counts_host.max()))))
             d, t, l, s = state["thr"]
-            again = self.boxes_enqueue(state["scores"], d, t, l, s, with_scores=state["box_scores"] is not None)
+            again = self.boxes_enqueue(state["scores"], d, t, l, s, with_scores=state["box_scores"] is not None,
+                                       with_polygons=state.get("polys") is not None)
             again["event"].synchronize()
             state.update(again)
             counts_host = state["counts_pin"].numpy().copy()
@@ -149,21 +167,34 @@ class Detector:
 
     # ------------------------------------------------------------------ reference API
     def detect(self, images: typing.List[typing.Union[np.ndarray, str]], detection_threshold=0.7,
-               text_threshold=0.4, link_threshold=0.4, size_threshold=10, return_scores=False, **kwargs):
+               text_threshold=0.4, link_threshold=0.4, size_threshold=10, return_scores=False, return_polygons=False,
+               **kwargs):
         """Same contract as reference detection.py:745-785: a list with one array of boxes
         ``(n_i, 4, 2)`` float32 per image (``np.array([])`` when there is none).  ``kwargs`` are the
         keras ``predict`` arguments of the reference (batch_size, verbose, ...) and are ignored.
 
         ``return_scores=True``: one ``(boxes, scores)`` pair per image instead, ``scores`` (n_i,) float32 the
         detection score of each box -- the largest text score over its connected component, the value compared
-        with ``detection_threshold`` (so every score is >= it)."""
+        with ``detection_threshold`` (so every score is >= it).
+
+        ``return_polygons=True``: every image also gives the polygon of each box, last in its tuple -- ``(boxes,
+        polygons)`` or ``(boxes, scores, polygons)`` -- a list of (p,2) float32 arrays in detector-input pixels: the box
+        itself (p = 4) for a straight word, otherwise 2 (s + 1) points along a curved word's centre line, the top edge
+        left to right then the bottom edge right to left, clockwise from the top-left (``b2o_get_boxes_poly``).  Boxes
+        and scores are those of the default call."""
         images_t = _as_device_images(images, self.device)
         state = self.boxes_enqueue(self.predict_device(images_t), detection_threshold, text_threshold, link_threshold,
-                                   size_threshold, with_scores=return_scores)
+                                   size_threshold, with_scores=return_scores, with_polygons=return_polygons)
         boxes, counts = self.boxes_finish(state)
         boxes_host = boxes.cpu().numpy()
         groups = [boxes_host[i, :c].copy() if c else np.array([]) for i, c in enumerate(counts)]
-        if not return_scores:
+        if not (return_scores or return_polygons):
             return groups
-        scores_host = state["box_scores"].cpu().numpy()
-        return [(g, scores_host[i, :c].copy()) for i, (g, c) in enumerate(zip(groups, counts))]
+        out = [(g,) for g in groups]
+        if return_scores:
+            scores_host = state["box_scores"].cpu().numpy()
+            out = [o + (scores_host[i, :c].copy(),) for i, (o, c) in enumerate(zip(out, counts))]
+        if return_polygons:
+            polys, points = state["polys"].cpu().numpy(), state["points"].cpu().numpy()
+            out = [o + ([polys[i, k, :points[i, k]].copy() for k in range(c)],) for i, (o, c) in enumerate(zip(out, counts))]
+        return out

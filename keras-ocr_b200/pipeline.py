@@ -124,11 +124,12 @@ class Pipeline:
         return (batch, scales, gray) if want_gray else (batch, scales)
 
     # ---------------------------------------------------------------- the three stages of one sub-batch
-    def _stage_detect(self, images, pad_to, thresholds, with_scores=False):
+    def _stage_detect(self, images, pad_to, thresholds, with_scores=False, with_polygons=False):
         batch, scales, gray = self.prepare_device(images, pad_to, want_gray=True)
         scores = self.detector.predict_device(batch)
         return {"batch": batch, "scales": scales, "gray": gray,
-                "boxes_state": self.detector.boxes_enqueue(scores, **thresholds, with_scores=with_scores)}
+                "boxes_state": self.detector.boxes_enqueue(scores, **thresholds, with_scores=with_scores,
+                                                           **({"with_polygons": True} if with_polygons else {}))}
 
     @staticmethod
     def _to_host(st, key, t):
@@ -140,9 +141,13 @@ class Pipeline:
         bst = st.pop("boxes_state")
         boxes, counts = det.boxes_finish(bst)
         box_scores, logp, cells = bst["box_scores"], None, None
+        polys = bst.get("polys")
+        extra = {"char_boxes": True} if char_boxes else {}
+        if polys is not None:
+            extra = {"polys": bst["flat_polys"], "points": bst["flat_points"]}
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
                                                  image_index=bst["image_index"], with_scores=box_scores is not None,
-                                                 **beam, **({"char_boxes": True} if char_boxes else {}))
+                                                 **beam, **extra)
         if char_boxes:                                   # (..., spans, cells): keep the cells
             cells, labels = labels[-1], labels[:-2]
             labels = labels if len(labels) > 1 else labels[0]
@@ -153,6 +158,9 @@ class Pipeline:
             self._to_host(st, "box_scores_host", box_scores)
         st["counts"] = counts
         self._to_host(st, "boxes_host", boxes)
+        if polys is not None:
+            self._to_host(st, "polys_host", bst["polys"])
+            self._to_host(st, "points_host", bst["points"])
         if labels is not None:
             self._to_host(st, "labels_host", labels)
         if logp is not None:
@@ -161,7 +169,7 @@ class Pipeline:
             st["char_boxes"] = True
             if cells is not None:
                 self._to_host(st, "cells_host", cells)
-        st["keep"] = (boxes, labels, box_scores, logp, cells)   # alive until the copies have run
+        st["keep"] = (boxes, labels, box_scores, logp, cells, polys)   # alive until the copies have run
         st["done"] = torch.cuda.Event()
         st["done"].record(torch.cuda.current_stream(det.device))
 
@@ -182,6 +190,10 @@ class Pipeline:
         if scored:
             box_scores = st["box_scores_host"].numpy()
             d2h += box_scores.nbytes
+        polys = None
+        if "polys_host" in st:
+            polys, points = st["polys_host"].numpy(), st["points_host"].numpy()
+            d2h += polys.nbytes + points.nbytes
         cells = None
         if "cells_host" in st:
             cells_host = st["cells_host"].numpy()
@@ -202,12 +214,16 @@ class Pipeline:
                 adjust = lambda q: tools.adjust_boxes(boxes=q, boxes_format="boxes", scale=1 / scale)  # noqa: E731
                 words = [w + ((adjust(q) if not isinstance(q, list) else [adjust(a) for a in q]),)
                          for w, q in zip(words, cells[start:start + c])]
+            if polys is not None:                        # each word's polygon, scaled as its box is
+                words = [w + (tools.adjust_boxes(boxes=polys[i, k, :points[i, k]].copy(), boxes_format="boxes",
+                                                 scale=1 / scale),)
+                         for k, w in enumerate(words)]
             out.append(words)
             start += c
         return out
 
     def recognize(self, images, detection_kwargs=None, recognition_kwargs=None, return_scores=False,
-                  return_char_boxes=False):
+                  return_char_boxes=False, return_polygons=False):
         """Run the pipeline on one or multiple images (reference pipeline.py:28-75).
 
         Returns a list (one entry per image) of lists of (text, box) tuples, boxes (4,2) float32 in
@@ -227,7 +243,14 @@ class Pipeline:
         in the input image's pixels for a text of n characters (a list of P arrays with ``top_paths = P > 1``), cell
         corner 0 the character's top-left in reading order, clockwise (``Recognizer.recognize_from_boxes_device``):
         (text, box, cells), or (text, box, detection_score, confidence, cells) with ``return_scores``.
+        ``return_polygons=True``: every word is read along its polygon (``Detector.detect(return_polygons=True)``: the
+        box itself for a straight word, points along the centre line of a curved one) and its tuple ends with that
+        polygon, a (p,2) float32 array in the input image's pixels: (text, box, polygon), or (text, box,
+        detection_score, confidence, polygon) with ``return_scores``.  It combines with ``beam_width`` / ``top_paths`` /
+        ``lexicon`` and ``inflight``; with ``rotations`` or ``return_char_boxes`` it raises ``ValueError``.
         """
+        if return_polygons and (return_char_boxes or (recognition_kwargs or {}).get("rotations") is not None):
+            raise ValueError("return_polygons does not combine with rotations or return_char_boxes")
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
                 images = [tools.read_device(image, self.detector.ctx, self.detector.device) for image in images]
@@ -253,6 +276,9 @@ class Pipeline:
             if return_char_boxes:
                 raise NotImplementedError("return_char_boxes=True needs this package's Detector and Recognizer; "
                                           "injected detectors / recognizers do not report character positions")
+            if return_polygons:
+                raise NotImplementedError("return_polygons=True needs this package's Detector and Recognizer; "
+                                          "injected detectors / recognizers do not report polygons")
             return self._recognize_generic(images, detection_kwargs, recognition_kwargs)
         thresholds = {k: detection_kwargs[k] for k in ("detection_threshold", "text_threshold", "link_threshold",
                                                         "size_threshold") if k in detection_kwargs}
@@ -268,7 +294,7 @@ class Pipeline:
         for step in range(k + 2):                        # detect(i) | recognize(i-1) | finish(i-2)
             if step < k:
                 states.append(self._stage_detect(images[bounds[step]:bounds[step + 1]], pad_to, thresholds,
-                                                 with_scores=return_scores))
+                                                 with_scores=return_scores, with_polygons=return_polygons))
             if 1 <= step <= k:
                 self._stage_recognize(states[step - 1], beam, char_boxes=return_char_boxes)
             if step >= 2:

@@ -194,6 +194,41 @@ def check_rotations(rotations=None, rotation_vote="word"):
     return turns
 
 
+def check_polygons(entries):
+    """Validates the words of a box group on the host, before anything is launched, and returns them as the dense table
+    ``b2o_warp_polys`` reads: (polys (B,18,2) float32, points (B,) int32), unused points NaN.  An entry is a (2m,2)
+    array: a box (m = 2, four corners) or a polygon of m - 1 segments, 3 <= m <= 9 -- the top edge t_0 .. t_{m-1}
+    left to right, then the bottom edge b_{m-1} .. b_0, as ``Detector.detect(return_polygons=True)`` returns them.
+    ``ValueError`` names the first entry with an odd point count, too few or too many points, a non-finite value, or
+    a degenerate segment (a quad t_i, t_i+1, b_i+1, b_i with coinciding corners or zero area)."""
+    n = len(entries)
+    polys = np.full((n, _lib.POLY_POINTS, 2), np.nan, np.float32)
+    points = np.zeros(n, np.int32)
+    for i, e in enumerate(entries):
+        a = np.asarray(e, dtype=np.float32)
+        if a.ndim != 2 or a.shape[1] != 2:
+            raise ValueError(f"entry {i} has shape {a.shape}: a word is a (points, 2) array")
+        p = a.shape[0]
+        if p % 2:
+            raise ValueError(f"entry {i} has an odd number of points ({p})")
+        if p < 4 or p > _lib.POLY_POINTS:
+            raise ValueError(f"entry {i} has {p} points: a word has 4 (a box) or 6 to {_lib.POLY_POINTS} (a polygon)")
+        if not np.isfinite(a).all():
+            raise ValueError(f"entry {i} has a non-finite coordinate")
+        if p > 4:
+            s = p // 2 - 1
+            for j in range(s):
+                q = a[[j, j + 1, p - 2 - j, p - 1 - j]].astype(np.float64)
+                x, y = q[:, 0], q[:, 1]
+                area = 0.5 * (np.dot(x, np.roll(y, -1)) - np.dot(y, np.roll(x, -1)))
+                same = (np.abs(q[:, None] - q[None]).max(-1) == 0).sum() > 4
+                if same or area == 0:
+                    raise ValueError(f"entry {i} has a degenerate segment {j}")
+        polys[i, :p] = a
+        points[i] = p
+    return polys, points
+
+
 def decode_paths(labels, alphabet=DEFAULT_ALPHABET, logp=None):
     """Host labels -> texts, and logp -> confidences (None without logp).  (B,48) labels / (B,) logp give B strings and
     a float32 array, as the greedy decoder returns them; (B,P,48) / (B,P) -- ``top_paths = P > 1`` -- give B lists of P
@@ -334,6 +369,22 @@ class Recognizer:
                                        crnn_in.data_ptr(), stream)
         return crnn_in, crops
 
+    def warp_polys_device(self, gray, polys, points, image_index, want_crops=False):
+        """warpBox along every polygon (``b2o_warp_polys``): polys (B,18,2) float32 and points (B,) int32 CUDA as
+        ``check_polygons`` / ``b2o_compact_polys`` lay them out; a 4-point entry is cut as ``warp_device`` cuts it.
+        Returns (crnn_in, crops or None) as ``warp_device`` does."""
+        n, h, w = gray.shape[:3]
+        color = gray.dim() == 4
+        assert color == self.color, "a color recognizer warps the RGB batch, a gray one the gray batch"
+        tail = (3,) if color else ()
+        b = polys.shape[0]
+        crnn_in = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + tail, dtype=torch.float16, device=self.device)
+        crops = torch.empty((b, TARGET_HEIGHT, TARGET_WIDTH) + tail, dtype=torch.uint8, device=self.device) if want_crops else None
+        self.ctx.warp_polys(gray.data_ptr(), 3 if color else 1, n, h, w, polys.data_ptr(), points.data_ptr(),
+                            image_index.data_ptr(), b, crops.data_ptr() if want_crops else None, crnn_in.data_ptr(),
+                            torch.cuda.current_stream(self.device).cuda_stream)
+        return crnn_in, crops
+
     def _decoder(self, beam_width, top_paths, lexicon):
         """``check_decoder`` for this recognizer's alphabet."""
         return check_decoder(beam_width, top_paths, lexicon, DEFAULT_ALPHABET if lexicon is None else self.alphabet)
@@ -469,7 +520,7 @@ class Recognizer:
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
                                     with_scores=False, beam_width=None, top_paths=1, lexicon=None, rotations=None,
-                                    rotation_vote="word", char_boxes=False):
+                                    rotation_vote="word", char_boxes=False, polys=None, points=None):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
         (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon``: see
         ``predict_device``).
@@ -487,9 +538,15 @@ class Recognizer:
 
         Optional device-side by-products of the earlier stages, so that nothing but the kernel launches is
         left to do once the host knows the counts: ``gray`` (N,H,W) u8 from ``b2o_resize_pad_batch``;
-        ``flat`` (>=B,4,2) / ``image_index`` (>=B,) from ``b2o_compact_boxes``."""
+        ``flat`` (>=B,4,2) / ``image_index`` (>=B,) from ``b2o_compact_boxes``.
+
+        ``polys`` (>=B,18,2) float32 / ``points`` (>=B,) int32 CUDA, the dense polygons of ``b2o_compact_polys`` in the
+        order of ``flat`` (with ``image_index``): every word is read along its polygon (``b2o_warp_polys``); a 4-point
+        entry reads as its box.  Rotations and character cells do not combine with polygons (``ValueError``)."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
         turns = check_rotations(rotations, rotation_vote)
+        if polys is not None and (turns is not None or char_boxes):
+            raise ValueError("polygons do not combine with rotations or character boxes")
         counts = np.asarray(counts)
         m = boxes.shape[1]
         total = int(np.minimum(counts, m).sum())
@@ -507,6 +564,10 @@ class Recognizer:
             counts_dev = torch.from_numpy(counts.astype(np.int32)).to(self.device)
             self.ctx.compact_boxes(boxes.data_ptr(), counts_dev.data_ptr(), n, m, flat.data_ptr(),
                                    image_index.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
+        if polys is not None:
+            crnn_in, _ = self.warp_polys_device(gray, polys[:total], points[:total], image_index[:total])
+            return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
+                                       lexicon=lexicon)
         if turns is not None:
             return self._recognize_turns(gray, flat[:total], image_index[:total], len(counts), boxes, turns,
                                          rotation_vote, with_scores, beam_width, top_paths, lexicon, char_boxes)
@@ -574,12 +635,21 @@ class Recognizer:
         most probable reading kept, per word or per image (one box group), see ``check_rotations``.
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells, an (n,4,2) float32 array
         of quads in the image's pixels for a text of n characters (a list of P arrays with ``top_paths = P > 1``):
-        (text, cells) or (text, confidence, cells); see ``recognize_from_boxes_device``."""
+        (text, cells) or (text, confidence, cells); see ``recognize_from_boxes_device``.
+
+        A box group may also hold polygons, (2m,2) arrays with 3 <= m <= 9 as ``Detector.detect(return_polygons=True)``
+        returns them (``check_polygons``): such a word is read along its polygon (``b2o_warp_polys``), a 4-point entry
+        of the same group exactly as without polygons.  Rotations and character boxes do not combine with polygons
+        (``ValueError``)."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
         turns = check_rotations(rotations, rotation_vote)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
 
+        entries = [e for g in box_groups for e in g]
+        if any(np.ndim(e) == 2 and np.shape(e)[0] != 4 for e in entries):
+            return self._recognize_polygons(images, box_groups, entries, return_scores, turns, return_char_boxes,
+                                            beam_width, top_paths, lexicon)
         images_t = _as_device_images(images, self.device)
         counts = np.array([len(b) for b in box_groups], dtype=np.int64)
         if counts.sum() == 0:
@@ -613,6 +683,33 @@ class Recognizer:
             predictions = list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
         else:
             crnn_in, _ = self.warp_device(gray, flat_t, idx)
+            predictions = decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
+        ends = np.cumsum(counts)
+        return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]
+
+    def _recognize_polygons(self, images, box_groups, entries, return_scores, turns, char_boxes, beam_width, top_paths,
+                            lexicon):
+        """``recognize_from_boxes`` for box groups that hold polygons: 4-point entries are rectified as
+        ``tools.rectify_boxes`` does and cut as boxes, the others along their polygon, all in one ``b2o_warp_polys``."""
+        if turns is not None or char_boxes:
+            raise ValueError("polygons do not combine with rotations or return_char_boxes")
+        polys, points = check_polygons(entries)
+        four = points == 4
+        if four.any():
+            polys[four, :4] = tools.rectify_boxes(polys[four, :4])
+        from .detection import _as_device_images
+
+        images_t = _as_device_images(images, self.device)
+        counts = np.array([len(b) for b in box_groups], dtype=np.int64)
+        idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
+        gray = images_t if self.color else self.gray_device(images_t)
+        crnn_in, _ = self.warp_polys_device(gray, torch.from_numpy(polys).to(self.device),
+                                            torch.from_numpy(points).to(self.device), idx)
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
+        if return_scores:
+            labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
+            predictions = list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
+        else:
             predictions = decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
         ends = np.cumsum(counts)
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]
