@@ -63,6 +63,9 @@ const char* b2o_last_error(const b2o_ctx* ctx);
 int b2o_set_conv_engine(b2o_ctx* ctx, int engine);
 /* number of kernels this library has launched since creation (bench.py's gpu_launches) */
 int64_t b2o_launch_count(const b2o_ctx* ctx);
+/* number of tensor-core conv launches since creation that ran channels by pixels on 16 x 16-pixel tiles (the streamed
+ * 128-channel 3x3 layers; B2O_TC_SWAP=0 turns that body off): lets tests see which body computed a result */
+int64_t b2o_tc_tile256_launches(const b2o_ctx* ctx);
 
 /* Measurement hook (bench.py's roofline leg): when enabled, every launch of the tensor-core conv
  * kernel is bracketed by CUDA events on its stream; b2o_profile_read sums the kernel time (ms), the

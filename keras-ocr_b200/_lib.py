@@ -57,6 +57,7 @@ SIGNATURES = {
     "b2o_last_error": (_c.c_char_p, [_vp]),
     "b2o_set_conv_engine": (_i, [_vp, _i]),
     "b2o_launch_count": (_c.c_int64, [_vp]),
+    "b2o_tc_tile256_launches": (_c.c_int64, [_vp]),
     "b2o_profile_enable": (_i, [_vp, _i]),
     "b2o_profile_read": (_i, [_vp, _c.POINTER(_c.c_double), _c.POINTER(_c.c_double), _c.POINTER(_c.c_int64)]),
     "b2o_load_craft": (_i, [_vp, _c.POINTER(_Tensor), _i]),
@@ -195,6 +196,10 @@ class Context:
 
     def launch_count(self):
         return int(self.lib.b2o_launch_count(self.handle))
+
+    def tile256_launches(self):
+        """Tensor-core conv launches so far that ran channels by pixels on 16 x 16-pixel tiles."""
+        return int(self.lib.b2o_tc_tile256_launches(self.handle))
 
     def profile_enable(self, on):
         self._check(self.lib.b2o_profile_enable(self.handle, int(on)), "b2o_profile_enable")

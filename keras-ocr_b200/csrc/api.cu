@@ -354,7 +354,7 @@ extern "C" int b2o_create(int device, b2o_ctx** out) {
   if (const char* e = getenv("B2O_TC_AFF")) ctx->tc_aff_const = std::string(e) != "smem";
   if (const char* e = getenv("B2O_GLUE")) ctx->glue_v1 = std::string(e) == "v1";
   if (const char* e = getenv("B2O_FUSED_TAIL")) ctx->no_fused_tail = atoi(e) == 0;      // 0: separate head_tail_kernel (A/B, tests)
-  if (const char* e = getenv("B2O_TC_SWAP")) ctx->tc_swap = atoi(e) != 0;               // 0: 64-channel layers as pixels x channels (A/B, tests)
+  if (const char* e = getenv("B2O_TC_SWAP")) ctx->tc_swap = atoi(e) != 0;               // 0: 64-channel and streamed 128-channel layers as pixels x channels (A/B, tests)
   if (const char* e = getenv("B2O_TC_PAIR")) {        // default 0 = single-CTA tiles; 1 = pairs on halo tiles; 2 = generic tiles too
     ctx->tc_pair = atoi(e) != 0;
     ctx->tc_pair_generic = atoi(e) == 2;
@@ -376,6 +376,7 @@ extern "C" void b2o_destroy(b2o_ctx* ctx) {
 
 extern "C" const char* b2o_last_error(const b2o_ctx* ctx) { return ctx ? ctx->error.c_str() : "null context"; }
 extern "C" int64_t b2o_launch_count(const b2o_ctx* ctx) { return ctx ? ctx->launches : 0; }
+extern "C" int64_t b2o_tc_tile256_launches(const b2o_ctx* ctx) { return ctx ? ctx->tc_tile256_launches : 0; }
 
 extern "C" int b2o_profile_enable(b2o_ctx* ctx, int on) {
   if (!ctx) return B2O_ERR_ARG;

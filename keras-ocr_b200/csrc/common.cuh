@@ -100,7 +100,9 @@ struct b2o_ctx {
   bool no_commute = true;
   bool glue_v1 = false;        // B2O_GLUE=v1: the round-1 upsample2x kernel (64-bit index chain, unshared blends) for A/B runs and the bit-identity test
   bool no_fused_tail = false;  // B2O_FUSED_TAIL=0: conv_cls.6/.8 as the separate head_tail_kernel instead of conv_cls.4's epilogue
-  bool tc_swap = true;         // 64-channel fp16 layers as channels x pixels GEMMs (bit-identical); B2O_TC_SWAP=0: pixels x channels
+  bool tc_swap = true;         // 64-channel fp16 layers, and the streamed 128-channel halo layers on 16 x 16 tiles, as channels x
+                               // pixels GEMMs (bit-identical); B2O_TC_SWAP=0: pixels x channels
+  int64_t tc_tile256_launches = 0;   // conv launches that took the 16 x 16-tile channels-by-pixels body (b2o_tc_tile256_launches)
   std::set<const void*> configured;   // kernels whose per-device launch attributes are set on this device
   int64_t launches = 0;
   std::string error;

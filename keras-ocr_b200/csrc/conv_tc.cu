@@ -22,7 +22,9 @@
 //   registers: scale/shift/ReLU/affine -> fp16|fp32 NHWC stores (possibly into a channel slice of a concat buffer) and,
 //   optionally, the fused 2x2 max-pool output or CRAFT tail.  The two warpgroups take turns on the main loop, so one
 //   runs its epilogue while the other keeps the tensor cores busy.  64-channel fp16 layers run transposed (p.ct,
-//   see conv_tc_body): one m64 (channels) x n128 (pixels) x k16 wgmma per k step and TMA-stored outputs.
+//   see conv_tc_body): one m64 (channels) x n128 (pixels) x k16 wgmma per k step and TMA-stored outputs;
+//   the streamed 128-channel halo layers run transposed on 16 x 16-pixel tiles (p.tile256): both warpgroups read every
+//   stage, one m64 (their 64 channels) x n256 (pixels) x k16 wgmma each per k step.
 // * persistent: grid = min(#tiles, #SMs); n-tiles of one pixel tile run back to back.
 #include <stdlib.h>
 #include <string.h>
@@ -53,7 +55,8 @@ struct TcParams {
   int stage_bytes, stage_tx;              // bytes between stages / bytes a stage's barrier expects
   int off_res, off_bar;                   // shared-memory offsets: resident filter bank, barriers
   int ct;                                 // channels by pixels (64-channel fp16 layers, see conv_tc_body)
-  int off_out;                            // ct: the two warpgroups' output tiles (+ pooled tiles)
+  int tile256;                            // channels by pixels on 16 x 16-pixel tiles (streamed 128-channel halo layers)
+  int off_out;                            // ct, tile256: the two warpgroups' output tiles (+ pooled tiles)
   int aff_smem;                           // epilogue constants staged in shared memory behind the barriers (B2O_TC_AFF=smem)
   int aff_const;                          // epilogue constants read from the AffConst kernel parameter (default)
   const float *s1, *t1, *s2, *t2;
@@ -242,6 +245,14 @@ __device__ __forceinline__ void wgmma_f16<128>(float* d, uint64_t adesc, uint64_
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+template <>
+__device__ __forceinline__ void wgmma_f16<256>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 
 // Walks the tiles first, first + step, ... keeping the mixed-radix coordinate (n_tile, tile_w, tile_h, tile_n)
 // incrementally: no integer divisions in the per-tile path.  The radices are read from the kernel parameters rather
@@ -291,10 +302,22 @@ struct AffConst {
 //       body.  A thread then holds 2 channels x 32 pixels, so the epilogue goes through a 16 KB shared-memory
 //       tile per warpgroup (stmatrix .trans) and TMA stores (omap, and pmap for the fused pool), which clip at the
 //       image edges.
-template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD, bool CT>
+// WIDE: channels by pixels on 16 (w) x 16 (h)-pixel halo tiles (p.tile256), for the 128-channel layers whose filter bank
+//       streams through the ring.  A stage is one (64, 16, 18) activation box plus the three dy taps' 128 filter rows,
+//       so each filter stage serves 256 pixels: a third less L2 -> shared-memory traffic per MMA than on 8 x 16 tiles.
+//       The two consumer warpgroups work cooperatively (no ping-pong): both read every stage, warpgroup wg computes
+//       output channels 64 wg .. 64 wg + 63 of all 256 pixels with one m64 x n256 x k16 per (dy, k step), A = its 64
+//       filter rows of the tap, B = pixel rows 16 dy .. 16 dy + 255 of the stage.  The sums are those of the 8 x 16
+//       tiles, in the same order: bit-identical results.  The epilogue is the CT one, once per 128-pixel half of the
+//       tile (tile rows 0-7, then 8-15), each a (64, 16, 8) TMA store at the warpgroup's channels.  Only two 84 KB stages
+//       fit, so a slot lands in three parts (halo box + dy = 0's rows on full[s], dy = 1, 2 on tap_full) and the MMAs
+//       of each dy start as soon as their part is in.
+template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD, bool CT, bool WIDE = false>
 __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUtensorMap& bmap, const CUtensorMap& omap,
                                              const CUtensorMap& pmap, const TcParams& p, const AffConst& ac) {
-  static_assert(!CT || (BLOCK_N == 64 && !PAIR && !UPADD), "channels by pixels: 64-channel single-CTA tiles");
+  static_assert(!CT || (!PAIR && !UPADD && (WIDE ? (BLOCK_N == 128 && KCH == 64 && MODE == 1) : BLOCK_N == 64)),
+                "channels by pixels: 64-channel single-CTA tiles, or 128-channel streamed halo tiles (WIDE)");
+  static_assert(!WIDE || CT, "the 16 x 16 tiles run channels by pixels");
   constexpr bool HALO = MODE >= 1, RESIDENT = MODE == 2;
   constexpr int TAPS_PER_A = HALO ? 3 : 1;                 // dy taps served by one A stage
   constexpr int B_BYTES = BLOCK_N * KCH * 2;
@@ -310,6 +333,7 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.off_bar);
   uint64_t* empty = full + MAX_RING;
   uint64_t* res_full = empty + MAX_RING;
+  uint64_t* tap_full = res_full + 1;                       // WIDE: filter rows of tap dy = 1, 2 of slot s at [(dy - 1) MAX_RING + s]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -331,9 +355,12 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
   if (threadIdx.x == 0) {
     for (int s = 0; s < MAX_RING; ++s) {
       mbar_init(&full[s], 1);                              // the producer's expect_tx arrival + the TMA bytes
-      mbar_init(&empty[s], (PAIR ? 2 : 1) * TILE_WARPS);   // one arrival per warp of the stage's consumer warpgroup (of both CTAs of a pair) once its MMAs read it
+      // one arrival per warp of the stage's consumer warpgroup (of both CTAs of a pair; of both warpgroups on 16 x 16
+      // tiles) once its MMAs read it
+      mbar_init(&empty[s], (PAIR ? 2 : 1) * (p.tile256 ? 2 : 1) * TILE_WARPS);
     }
     mbar_init(res_full, 1);
+    for (int i = 0; i < 2 * MAX_RING; ++i) mbar_init(&tap_full[i], 1);
     fence_barrier_init();
   }
   if (PAIR) cluster_sync_all();                            // the peer's barriers exist before anything signals them
@@ -370,18 +397,22 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
           for (int kc = 0; kc < kchunks; ++kc) {
             mbar_wait(&empty[s], ph ^ 1);
             uint8_t* const st = smem + s * p.stage_bytes;
-            mbar_expect_tx(&full[s], static_cast<uint32_t>(p.stage_tx));
+            // WIDE: full[s] covers the halo box and tap dy = 0's filter rows, taps 1 and 2 land on their own barriers, so
+            // the consumers start on dy = 0 before the whole 84 KB slot is in
+            mbar_expect_tx(&full[s], static_cast<uint32_t>(WIDE ? p.a_bytes + B_BYTES : p.stage_tx));
             tma_load_4d(&amap, &full[s], st, kc * KCH, ax, ay, tn0);
             if (!RESIDENT) {
 #pragma unroll
               for (int t = 0; t < TAPS_PER_A; ++t) {
                 const int tap = HALO ? (t * 3 + g) : g;
                 uint8_t* const dst = st + p.a_stride + t * B_BYTES;
+                uint64_t* const bar = (WIDE && t > 0) ? &tap_full[(t - 1) * MAX_RING + s] : &full[s];
+                if (WIDE && t > 0) mbar_expect_tx(bar, static_cast<uint32_t>(B_BYTES));
                 if (PAIR)
-                  tma_load_2d_multicast(&bmap, &full[s], dst + rank * B_HALF, tap * p.cin + kc * KCH,
+                  tma_load_2d_multicast(&bmap, bar, dst + rank * B_HALF, tap * p.cin + kc * KCH,
                                         ti.c0 * BLOCK_N + static_cast<int>(rank) * (BLOCK_N / 2));
                 else
-                  tma_load_2d(&bmap, &full[s], dst, tap * p.cin + kc * KCH, ti.c0 * BLOCK_N);
+                  tma_load_2d(&bmap, bar, dst, tap * p.cin + kc * KCH, ti.c0 * BLOCK_N);
               }
             }
             if (++s == p.ns) { s = 0; ph ^= 1; }
@@ -402,7 +433,7 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
     const int q = lane & 3;
     // accumulator layout of wgmma m64: this thread holds rows r0 and r0 + 8 of each 64-row half, columns 8i + 2q, 8i + 2q + 1
     const int r0 = (warp & 3) * 16 + (lane >> 2);
-    constexpr uint32_t TAP_BYTES = 8 * KCH * 2;              // halo: one dy tap = 8 pixel rows further into the stage
+    constexpr uint32_t TAP_BYTES = (WIDE ? 16 : 8) * KCH * 2;   // halo: one dy tap = one tile row (8 | 16 pixels) further
     constexpr uint32_t HALF_BYTES = WG_M * KCH * 2;          // tile rows 64-127: 64 rows (whole 8-row atoms) further
     const uint64_t desc_a0 = gmma_desc<KCH>(smem_u32(smem));
     const uint64_t desc_b0 = gmma_desc<KCH>(smem_u32(smem) + static_cast<uint32_t>(RESIDENT ? p.off_res : p.a_stride));
@@ -427,13 +458,14 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
       s -= laps * p.ns;
       ph ^= static_cast<uint32_t>(laps & 1);
     };
-    TileIter ti(p, cta + wg * ncta, 2 * ncta);              // the CTA's tiles wg, wg + 2, ...
-    if (wg == 1) skip_tile();
+    // the CTA's tiles wg, wg + 2, ... (WIDE: both warpgroups take every tile)
+    TileIter ti(p, cta + (WIDE ? 0 : wg * ncta), (WIDE ? 1 : 2) * ncta);
+    if (!WIDE && wg == 1) skip_tile();
     if (RESIDENT && ti.valid(p)) mbar_wait(res_full, 0);
-    float acc[2 * NACC];                                     // [rows 0-63 | rows 64-127]
+    float acc[2 * NACC];                                     // [rows 0-63 | rows 64-127] (WIDE: pixels 0-127 | 128-255)
   #pragma unroll
     for (int i = 0; i < 2 * NACC; ++i) acc[i] = 0.0f;
-    for (bool after_other = wg == 1; ti.valid(p); ti.next(p), after_other = true) {
+    for (bool after_other = !WIDE && wg == 1; ti.valid(p); ti.next(p), after_other = !WIDE) {
       if (after_other) named_bar_sync(1 + wg, 2 * 128);      // the other warpgroup has issued the previous tile
       // ---- main loop: every stage of the tile, MMAs in (dx | tap, chunk, dy, k) order, both halves per k step
       int prev = -1;
@@ -447,12 +479,19 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
           wgmma_fence();
   #pragma unroll
           for (int t = 0; t < TAPS_PER_A; ++t) {
+            if (WIDE && t > 0) {                             // this tap's filter rows (full[s]: halo box + dy = 0)
+              mbar_wait(&tap_full[(t - 1) * MAX_RING + s], ph);
+              wgmma_fence();
+            }
             const uint32_t boff = RESIDENT ? static_cast<uint32_t>(((t * 3 + g) * kchunks + kc) * B_BYTES)
                                            : static_cast<uint32_t>(s * p.stage_bytes + t * B_BYTES);
             const uint64_t bdesc = desc_b0 + static_cast<uint64_t>(boff >> 4);
   #pragma unroll
             for (int k = 0; k < KSTEPS; ++k) {
-              if constexpr (CT) {
+              if constexpr (WIDE) {
+                wgmma_f16<256>(acc, bdesc + static_cast<uint64_t>((wg * HALF_BYTES + k * 32) >> 4),
+                               adesc + static_cast<uint64_t>((t * TAP_BYTES + k * 32) >> 4), accumulate);
+              } else if constexpr (CT) {
                 wgmma_f16<128>(acc, bdesc + static_cast<uint64_t>((k * 32) >> 4),
                                adesc + static_cast<uint64_t>((t * TAP_BYTES + k * 32) >> 4), accumulate);
               } else {
@@ -463,19 +502,35 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
               }
               accumulate = 1;
             }
+            if (WIDE) {
+              // one commit group per tap: once dy = 0's MMAs are issued, the previous stage's are waited for and
+              // the stage released, before this stage's dy = 1, 2 rows have to be in
+              wgmma_commit();
+              if (t == 0) {
+                wgmma_wait<1>();
+                if (prev >= 0) {
+                  __syncwarp();
+                  if (lane == 0) release(prev);
+                }
+              }
+            }
           }
-          wgmma_commit();
-          wgmma_wait<1>();                                   // the previous stage's MMAs are done: release it
-          if (prev >= 0) {
-            __syncwarp();
-            if (lane == 0) release(prev);
+          if (!WIDE) {
+            wgmma_commit();
+            wgmma_wait<1>();                                 // the previous stage's MMAs are done: release it
+            if (prev >= 0) {
+              __syncwarp();
+              if (lane == 0) release(prev);
+            }
           }
           prev = s;
           if (++s == p.ns) { s = 0; ph ^= 1; }
         }
       }
-      if (ti.tile + ncta < p.total_tiles) named_bar_arrive(1 + (wg ^ 1), 2 * 128);   // the CTA's next tile may start
-      skip_tile();
+      if (!WIDE) {
+        if (ti.tile + ncta < p.total_tiles) named_bar_arrive(1 + (wg ^ 1), 2 * 128);   // the CTA's next tile may start
+        skip_tile();
+      }
       wgmma_wait<0>();
   #pragma unroll
       for (int i = 0; i < 2 * NACC; ++i) reg_fence(acc[i]);
@@ -485,67 +540,93 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
       // ---- epilogue from the registers, one 64-row half after the other
       const int c_base = ti.c0 * BLOCK_N;
       if constexpr (CT) {
-        // this thread holds channels r0, r0 + 8 (hh = 0, 1) x pixels 8i + 2q, 8i + 2q + 1 (i < 16) in acc[4i + 2hh + 0, 1]:
-        // the same per-element fmaf / ReLU / fmaf and fp16 rounding as below, with per-channel scalars
-        uint32_t hv[16][2];
-  #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int c = r0 + 8 * hh;
-          const float a1 = e_s1[c], b1 = e_t1[c];
-          const float a2 = p.s2 != nullptr ? e_s2[c] : 0.0f, b2 = p.s2 != nullptr ? e_t2[c] : 0.0f;
-  #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float y0 = fmaf(acc[4 * i + 2 * hh], a1, b1);
-            float y1 = fmaf(acc[4 * i + 2 * hh + 1], a1, b1);
-            if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
-            if (p.s2 != nullptr) { y0 = fmaf(y0, a2, b2); y1 = fmaf(y1, a2, b2); }
-            const __half2 h2 = __floats2half2_rn(y0, y1);
-            hv[i][hh] = *reinterpret_cast<const uint32_t*>(&h2);
-          }
-        }
-        // NHWC tile [128 pixel rows][64 channels] with the 128B swizzle of omap / pmap: 16-byte chunk j of row r sits at
-        // chunk j ^ (r & 7).  An 8x8 block (8 channels x 8 pixels) stored transposed = 8 pixel rows of one chunk.
+        // this thread holds channels r0, r0 + 8 (hh = 0, 1) x pixels 8i + 2q, 8i + 2q + 1 in acc[4i + 2hh + 0, 1]
+        // (i < 16; WIDE: i < 32, two 128-pixel halves = tile rows 0-7 and 8-15, each stored on its own): the same
+        // per-element fmaf / ReLU / fmaf and fp16 rounding as below, with per-channel scalars
+        constexpr int BW = WIDE ? 16 : 8;                      // halo tile width (the fused pool runs on halo tiles only)
         constexpr int OUT_TILE = 128 * 64 * 2, POOL_TILE = 32 * 64 * 2;
         uint8_t* const otile = smem + p.off_out + wg * OUT_TILE;
         uint8_t* const ptile = smem + p.off_out + 2 * OUT_TILE + wg * POOL_TILE;
         const int et = threadIdx.x & 127;
-        if (et == 0) bulk_wait_read_all();                   // the previous tile's stores have read the tile
-        named_bar_sync(3 + wg, 128);
-        {
-          const int m = lane >> 3, r = lane & 7;               // this lane addresses row r of matrix m = (i & 1, hh)
-          const uint32_t row = smem_u32(otile) + static_cast<uint32_t>(r * 128 + (((2 * (warp & 3) + (m & 1)) ^ r) << 4));
+        const int c_wg = c_base + (WIDE ? WG_M * wg : 0);      // WIDE: this warpgroup's 64 of the tile's 128 channels
   #pragma unroll
-          for (int i0 = 0; i0 < 16; i0 += 2)
-            stmatrix_x4_trans(row + static_cast<uint32_t>((8 * (i0 + (m >> 1))) * 128), hv[i0][0], hv[i0][1],
-                              hv[i0 + 1][0], hv[i0 + 1][1]);
-        }
-        fence_proxy_async_smem();
-        named_bar_sync(3 + wg, 128);
-        if (p.pool_out != nullptr) {                           // halo tile 8 x 16 -> pooled 4 x 8, max(max(v00, v10), max(v01, v11))
+        for (int half = 0; half < (WIDE ? 2 : 1); ++half) {
+          // keeps the second half's arithmetic behind the first half's stores (registers: 128 accumulators live)
   #pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const int item = et + 128 * j, pr = item >> 3, ch = item & 7;
-            const int r00 = 2 * (pr & 3) + 16 * (pr >> 2);   // (2 pw, 2 ph) in the 8-wide tile
-            auto ld = [&](int rr) { return *reinterpret_cast<const uint4*>(otile + rr * 128 + ((ch ^ (rr & 7)) << 4)); };
-            const uint4 v00 = ld(r00), v10 = ld(r00 + 8), v01 = ld(r00 + 1), v11 = ld(r00 + 9);
-            uint4 o;
-            const __half2* a = reinterpret_cast<const __half2*>(&v00);
-            const __half2* b = reinterpret_cast<const __half2*>(&v10);
-            const __half2* c = reinterpret_cast<const __half2*>(&v01);
-            const __half2* d = reinterpret_cast<const __half2*>(&v11);
-            __half2* op = reinterpret_cast<__half2*>(&o);
+          for (int i = 64 * half; i < 64 * half + 64; ++i) reg_fence(acc[i]);
+          float a1[2], b1[2], a2[2], b2[2];
   #pragma unroll
-            for (int e = 0; e < 4; ++e) op[e] = __hmax2(__hmax2(a[e], b[e]), __hmax2(c[e], d[e]));
-            *reinterpret_cast<uint4*>(ptile + pr * 128 + ((ch ^ (pr & 7)) << 4)) = o;
+          for (int hh = 0; hh < 2; ++hh) {
+            const int c = c_wg + r0 + 8 * hh;
+            if constexpr (WIDE) {                            // read from p here: no pointers held across the main loop
+              a1[hh] = p.aff_const ? ac.s1[c] : p.s1[c]; b1[hh] = p.aff_const ? ac.t1[c] : p.t1[c];
+              a2[hh] = p.s2 == nullptr ? 0.0f : (p.aff_const ? ac.s2[c] : p.s2[c]);
+              b2[hh] = p.s2 == nullptr ? 0.0f : (p.aff_const ? ac.t2[c] : p.t2[c]);
+            } else {
+              a1[hh] = e_s1[c]; b1[hh] = e_t1[c];
+              a2[hh] = p.s2 != nullptr ? e_s2[c] : 0.0f; b2[hh] = p.s2 != nullptr ? e_t2[c] : 0.0f;
+            }
+          }
+          // pixels 8i + 2q, 8i + 2q + 1 of channel r0 + 8hh, as fp16.  The 64-channel body converts all 32 pairs before
+          // the stores; WIDE converts each right before its stmatrix, so only four are live beside the other half's
+          // 64 accumulators
+          auto h2 = [&](int i, int hh) {
+            float y0 = fmaf(acc[64 * half + 4 * i + 2 * hh], a1[hh], b1[hh]);
+            float y1 = fmaf(acc[64 * half + 4 * i + 2 * hh + 1], a1[hh], b1[hh]);
+            if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
+            if (p.s2 != nullptr) { y0 = fmaf(y0, a2[hh], b2[hh]); y1 = fmaf(y1, a2[hh], b2[hh]); }
+            const __half2 h = __floats2half2_rn(y0, y1);
+            return *reinterpret_cast<const uint32_t*>(&h);
+          };
+          uint32_t hv[16][2];
+          if constexpr (!WIDE) {
+  #pragma unroll
+            for (int i = 0; i < 16; ++i) { hv[i][0] = h2(i, 0); hv[i][1] = h2(i, 1); }
+          }
+          auto hval = [&](int i, int hh) {
+            if constexpr (WIDE) return h2(i, hh);
+            else return hv[i][hh];
+          };
+          // NHWC tile [128 pixel rows][64 channels] with the 128B swizzle of omap / pmap: 16-byte chunk j of row r sits
+          // at chunk j ^ (r & 7).  An 8x8 block (8 channels x 8 pixels) stored transposed = 8 pixel rows of one chunk.
+          if (et == 0) bulk_wait_read_all();                 // the previous half's / tile's stores have read the tile
+          named_bar_sync(3 + wg, 128);
+          {
+            const int m = lane >> 3, r = lane & 7;             // this lane addresses row r of matrix m = (i & 1, hh)
+            const uint32_t row = smem_u32(otile) + static_cast<uint32_t>(r * 128 + (((2 * (warp & 3) + (m & 1)) ^ r) << 4));
+  #pragma unroll
+            for (int i0 = 0; i0 < 16; i0 += 2)
+              stmatrix_x4_trans(row + static_cast<uint32_t>((8 * (i0 + (m >> 1))) * 128), hval(i0, 0), hval(i0, 1),
+                                hval(i0 + 1, 0), hval(i0 + 1, 1));
           }
           fence_proxy_async_smem();
           named_bar_sync(3 + wg, 128);
-        }
-        if (et == 0) {
-          const int tw0 = ti.c1 << p.bw_log2, th0 = ti.c2 << p.bh_log2, tn0 = ti.c3 << p.bn_log2;
-          if (p.write_full) tma_store_4d(&omap, otile, 0, tw0, th0, tn0);
-          if (p.pool_out != nullptr) tma_store_4d(&pmap, ptile, 0, tw0 >> 1, th0 >> 1, tn0);
-          bulk_commit();
+          if (p.pool_out != nullptr) {   // halo half-tile BW x 128/BW -> pooled BW/2 x 64/BW, max(max(v00, v10), max(v01, v11))
+  #pragma unroll (WIDE ? 1 : 2)                            // WIDE: rolled, for registers
+            for (int j = 0; j < 2; ++j) {
+              const int item = et + 128 * j, pr = item >> 3, ch = item & 7;
+              const int r00 = 2 * (pr % (BW / 2)) + 2 * BW * (pr / (BW / 2));   // (2 pw, 2 ph) in the BW-wide tile
+              auto ld = [&](int rr) { return *reinterpret_cast<const uint4*>(otile + rr * 128 + ((ch ^ (rr & 7)) << 4)); };
+              const uint4 v00 = ld(r00), v10 = ld(r00 + BW), v01 = ld(r00 + 1), v11 = ld(r00 + BW + 1);
+              uint4 o;
+              const __half2* a = reinterpret_cast<const __half2*>(&v00);
+              const __half2* b = reinterpret_cast<const __half2*>(&v10);
+              const __half2* c = reinterpret_cast<const __half2*>(&v01);
+              const __half2* d = reinterpret_cast<const __half2*>(&v11);
+              __half2* op = reinterpret_cast<__half2*>(&o);
+  #pragma unroll
+              for (int e = 0; e < 4; ++e) op[e] = __hmax2(__hmax2(a[e], b[e]), __hmax2(c[e], d[e]));
+              *reinterpret_cast<uint4*>(ptile + pr * 128 + ((ch ^ (pr & 7)) << 4)) = o;
+            }
+            fence_proxy_async_smem();
+            named_bar_sync(3 + wg, 128);
+          }
+          if (et == 0) {
+            const int tw0 = ti.c1 << p.bw_log2, th0 = (ti.c2 << p.bh_log2) + 8 * half, tn0 = ti.c3 << p.bn_log2;
+            if (p.write_full) tma_store_4d(&omap, otile, c_wg, tw0, th0, tn0);
+            if (p.pool_out != nullptr) tma_store_4d(&pmap, ptile, c_wg, tw0 >> 1, th0 >> 1, tn0);
+            bulk_commit();
+          }
         }
       }
   #pragma unroll
@@ -695,7 +776,8 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
   if (PAIR) cluster_sync_all();
 }
 
-// The 64-channel single-CTA instances carry both bodies and take the channels-by-pixels one when p.ct is set.
+// The 64-channel single-CTA instances carry both bodies and take the channels-by-pixels one when p.ct is set; the
+// streamed 128-channel halo instance takes the 16 x 16-tile channels-by-pixels body when p.tile256 is set.
 template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
@@ -704,6 +786,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
   if constexpr (BLOCK_N == 64 && !PAIR && !UPADD) {
     if (p.ct) {
       conv_tc_body<BLOCK_N, KCH, MODE, PAIR, UPADD, true>(amap, bmap, omap, pmap, p, ac);
+      return;
+    }
+  }
+  if constexpr (BLOCK_N == 128 && KCH == 64 && MODE == 1 && !PAIR && !UPADD) {
+    if (p.tile256) {
+      conv_tc_body<BLOCK_N, KCH, MODE, PAIR, UPADD, true, true>(amap, bmap, omap, pmap, p, ac);
       return;
     }
   }
@@ -916,13 +1004,29 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   p.aff_const = (ctx->tc_aff_const && L.cout <= 256 && static_cast<int>(L.h_s1.size()) == L.cout) ? 1 : 0;
   p.aff_smem = (!p.aff_const && L.cout <= 256) ? 1 : 0;
   const int aff_bytes = (p.aff_smem ? 4 * L.cout * 4 : 0) + (tail ? TAIL_FLOATS * 4 : 0);
-  const int out_tiles = ct ? 2 * 128 * 64 * 2 + (want_pool ? 2 * 32 * 64 * 2 : 0) : 0;   // per warpgroup: 16 KB (+ 4 KB pooled)
-  const int budget = SMEM_TOTAL - 1024 /*alignment slack*/ - 512 /*barriers*/ - aff_bytes - out_tiles;
+  const int tma_out_tiles = 2 * 128 * 64 * 2 + (want_pool ? 2 * 32 * 64 * 2 : 0);   // per warpgroup: 16 KB (+ 4 KB pooled)
+  int out_tiles = ct ? tma_out_tiles : 0;
+  int budget = SMEM_TOTAL - 1024 /*alignment slack*/ - 512 /*barriers*/ - aff_bytes - out_tiles;
   p.a_bytes = p.halo ? 18 * 8 * kch * 2 : 128 * kch * 2;
   p.a_stride = (p.a_bytes + 1023) / 1024 * 1024;
   const long long res_bytes = static_cast<long long>(taps) * kchunks * b_bytes;
   // (the mbarrier tx-count holds 2^20 - 1 bytes)
   p.resident = (p.halo && p.n_tiles == 1 && res_bytes + 2LL * p.a_stride <= budget && res_bytes <= (1 << 20) - 1) ? 1 : 0;
+  // channels by pixels on 16 x 16 tiles for the streamed 128-channel fp16 halo layers (conv_tc_body, WIDE): one filter
+  // stage serves 256 pixels.  Only where the 16-wide tile covers the same columns of an image as the 8-wide one, so the
+  // choice depends on the layer and the image shape alone, never on the batch.
+  const bool tile256 = ctx->tc_swap && p.halo && !p.resident && kch == 64 && bn == 128 && !pair && !out_f32 &&
+                       up_add == nullptr && tail == nullptr && (in.w + 15) / 16 * 16 == (in.w + 7) / 8 * 8 &&
+                       (!want_pool || (in.h >= 2 && in.w >= 2));
+  if (tile256) {
+    p.tile256 = 1;
+    p.bw_log2 = 4;
+    p.tiles_w = (in.w + 15) >> 4;
+    p.total_tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles;     // half of the 8 x 16 tiles' count
+    p.a_bytes = p.a_stride = 18 * 16 * kch * 2;                          // 36 KB: (64, 16, 18, 1)
+    out_tiles = tma_out_tiles;
+    budget -= out_tiles;
+  }
   const int b_per_stage = p.resident ? 0 : (p.halo ? 3 : 1);
   p.stage_bytes = p.a_stride + b_per_stage * b_bytes;
   p.stage_tx = p.a_bytes + b_per_stage * b_bytes;
@@ -965,7 +1069,7 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   cuuint64_t strides[3] = {static_cast<cuuint64_t>(in.ld) * 2, static_cast<cuuint64_t>(in.ld) * 2 * in.w,
                            static_cast<cuuint64_t>(in.ld) * 2 * in.w * in.h};
   cuuint32_t box[4] = {static_cast<cuuint32_t>(kch), 1u << p.bw_log2, 1u << p.bh_log2, 1u << p.bn_log2};
-  if (p.halo) { box[1] = 8; box[2] = 18; box[3] = 1; }
+  if (p.halo) { box[1] = 1u << p.bw_log2; box[2] = 18; box[3] = 1; }   // 8 (tile256: 16) x 18 rows
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = enc(&amap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, in.ptr, dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(kch), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -975,23 +1079,26 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
                    std::to_string(static_cast<int>(r)));
     return B2O_ERR_CUDA;
   }
-  // channels-by-pixels output maps: 4-D (c, w, h, n) over the 64-channel view (a channel slice: base pointer + ld), boxes of one tile
+  // channels-by-pixels output maps: 4-D (c, w, h, n) over the layer's cout-channel view (a channel slice: base pointer +
+  // ld), boxes of 64 channels x one tile (tile256: one 16 x 8 half-tile)
   CUtensorMap omap, pmap;
   memset(&omap, 0, sizeof(omap));
   memset(&pmap, 0, sizeof(pmap));
   auto encode_out = [&](CUtensorMap* m, void* ptr, int ld, int n, int h, int w, const cuuint32_t* obox) {
-    cuuint64_t odims[4] = {64, static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h), static_cast<cuuint64_t>(n)};
+    cuuint64_t odims[4] = {static_cast<cuuint64_t>(L.cout), static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h),
+                           static_cast<cuuint64_t>(n)};
     cuuint64_t ostr[3] = {static_cast<cuuint64_t>(ld) * 2, static_cast<cuuint64_t>(ld) * 2 * w,
                           static_cast<cuuint64_t>(ld) * 2 * w * h};
     return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, ptr, odims, ostr, obox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   };
-  if (ct && write_full) {
-    const cuuint32_t obox[4] = {64, 1u << p.bw_log2, 1u << p.bh_log2, 1u << p.bn_log2};
+  if ((ct || tile256) && write_full) {
+    const cuuint32_t obox[4] = {64, 1u << p.bw_log2, tile256 ? 8u : 1u << p.bh_log2, 1u << p.bn_log2};
     r = encode_out(&omap, out.ptr, out.ld, in.n, in.h, in.w, obox);
   }
-  if (ct && want_pool && r == CUDA_SUCCESS) {
-    const cuuint32_t pbox[4] = {64, 4, 8, 1};              // the 2x2 max of one 8 x 16 halo tile
+  if ((ct || tile256) && want_pool && r == CUDA_SUCCESS) {
+    // the 2x2 max of one 8 x 16 halo tile, or of one 16 x 8 half of a 16 x 16 tile
+    const cuuint32_t pbox[4] = {64, tile256 ? 8u : 4u, tile256 ? 4u : 8u, 1};
     r = encode_out(&pmap, pool_out->ptr, pool_out->ld, in.n, p.PH, p.PW, pbox);
   }
   if (r != CUDA_SUCCESS) {
@@ -1010,6 +1117,7 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   }
   B2O_TC_PAIR_CASE(64); B2O_TC_PAIR_CASE(128);
 #undef B2O_TC_PAIR_CASE
+  if (tile256) ++ctx->tc_tile256_launches;
 #define B2O_TC_CASE(BN, KC)                                                                                            \
   if (bn == BN && kch == KC) {                                                                                         \
     if (p.resident) return launch<BN, KC, 2, false>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                      \

@@ -7,7 +7,8 @@ steps, one step under ``torch.profiler`` with CUDA activity (its trace goes to O
 profiler for the step time.  The trace's ``conv_tc_kernel`` launches, in launch order, are matched to the layer
 sequence of ``b2o_craft_forward`` and ``b2o_crnn_forward``; for each layer the script prints its shape, the kernel
 instance, the time, the algorithmic FLOPs (2 * pixels * taps * cin * cout with the reference's channel counts, as
-``launch()`` in csrc/conv_tc.cu counts them) and the rate, then totals for CRAFT, the CRNN and the step, and the share of
+``launch()`` in csrc/conv_tc.cu counts them) and the rate, the bytes its TMA loads bring into shared memory (from the
+plan ``conv_tc_run`` makes for that shape and instance, see ``tma_fill_bytes``) and that fill rate, then totals for CRAFT, the CRNN and the step, and the share of
 the step spent outside ``conv_tc_kernel``.  The same data goes to OUT_DIR/conv_layer_profile.json, with the card's name,
 power limit and clocks (read-only nvidia-smi query).  Only the public Python API is used.
 """
@@ -97,6 +98,54 @@ def instance(name):
     return m.group(1).replace(" ", "") if m else name
 
 
+def pick_box(n, h, w):
+    """pick_box() of csrc/conv_tc.cu: the (bw, bh, bn) power-of-two 128-pixel box that wastes the fewest pixels."""
+    best, box = 1e30, (128, 1, 1)
+    for lw in range(8):
+        for lh in range(8 - lw):
+            ln = 7 - lw - lh
+            bw, bh, bn = 1 << lw, 1 << lh, 1 << ln
+            if ln > 0 and bn > 2 * n:
+                continue
+            cover = float(-(-w // bw) * bw) * float(-(-h // bh) * bh) * float(-(-n // bn) * bn)
+            score = cover * (1.0 + 0.001 * (7 - lw)) * (1.05 if (bw < 8 and w >= 8) else 1.0)
+            if score < best:
+                best, box = score, (bw, bh, bn)
+    return box
+
+
+def tile256_selected(inst, w, wide_body):
+    """conv_tc_run's choice of the 16 x 16-pixel channels-by-pixels body of conv_tc_kernel<128,64,1,false,false>: the
+    build has it, B2O_TC_SWAP is not 0, and the 16-wide tile covers the same columns as the 8-wide one."""
+    return (wide_body and os.environ.get("B2O_TC_SWAP", "1") != "0" and inst == "128,64,1,false,false" and
+            (w + 15) // 16 * 16 == (w + 7) // 8 * 8)
+
+
+def tma_fill_bytes(inst, n, h, w, k, cin, cout, sm_count, wide_body):
+    """Bytes the launch's TMA loads bring into shared memory, from conv_tc_run's plan: every tile takes one stage per
+    (dx | tap, 64/32/16-channel chunk) holding its activation box (halo: 18 rows of the tile's width) and, unless the
+    filter bank is resident, the stage's filter rows (3 taps on halo tiles); a resident bank is loaded once per CTA.
+    Returns (bytes, tile description); None for CTA pairs (not in the default plan)."""
+    bn, kch, mode, pair = [int(v) if v.isdigit() else v for v in inst.split(",")[:4]]
+    if pair == "true":
+        return None
+    b_bytes = bn * kch * 2
+    kchunks = cin // kch
+    if mode >= 1:
+        bw, bh, bnn = (16, 16, 1) if tile256_selected(inst, w, wide_body) else (8, 16, 1)
+        groups, a_bytes = 3, (bh + 2) * bw * kch * 2
+    else:
+        bw, bh, bnn = pick_box(n, h, w)
+        groups, a_bytes = k * k, 128 * kch * 2
+    tiles = (-(-w // bw)) * (-(-h // bh)) * (-(-n // bnn)) * (cout // bn)
+    taps_per_stage = 0 if mode == 2 else (3 if mode == 1 else 1)
+    stage_tx = a_bytes + taps_per_stage * b_bytes
+    total = tiles * groups * kchunks * stage_tx
+    if mode == 2:
+        total += min(tiles, sm_count) * k * k * kchunks * b_bytes
+    return total, f"{bw}x{bh}x{bnn} stage {stage_tx} B"
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("out_dir")
@@ -134,10 +183,15 @@ def main():
     _, flop_r, n_r = rec.ctx.profile_read()
     det.ctx.profile_enable(0); rec.ctx.profile_enable(0)
 
+    def tile256_count():
+        return sum(c.tile256_launches() for c in (det.ctx, rec.ctx)) if hasattr(det.ctx.lib, "b2o_tc_tile256_launches") else 0
+
     from torch.profiler import ProfilerActivity, profile
+    tile256_in_step = -tile256_count()
     with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
         pipe.recognize(pages)
         torch.cuda.synchronize()
+    tile256_in_step += tile256_count()
     trace_path = os.path.join(args.out_dir, "step.pt.trace.json")
     prof.export_chrome_trace(trace_path)
 
@@ -158,6 +212,8 @@ def main():
     n_craft = len(table)
     table += crnn_layers(crops)
     matched = len(conv) == len(table) and n_d == n_craft and n_r == len(table) - n_craft
+    sm_count = torch.cuda.get_device_properties(device).multi_processor_count
+    wide_body = hasattr(det.ctx.lib, "b2o_tc_tile256_launches")
     rows = []
     for i, (kname, _, dur) in enumerate(conv):
         row = {"launch": i, "instance": instance(kname), "ms": dur / 1e3}
@@ -166,7 +222,13 @@ def main():
             flop = 2.0 * n * h * w * k * k * cin * cout
             row.update({"net": "craft" if i < n_craft else "crnn", "layer": name, "shape": [n, h, w, cin, cout],
                         "ksize": k, "flop": flop, "tflops": flop / (dur * 1e-6) / 1e12})
+            fill = tma_fill_bytes(row["instance"], n, h, w, k, cin, cout, sm_count, wide_body)
+            if fill is not None:
+                row.update({"fill_bytes": fill[0], "fill_tbps": fill[0] / (dur * 1e-6) / 1e12, "tile": fill[1]})
         rows.append(row)
+    if wide_body and matched:      # the plan reproduced above must agree with the launches the library counted
+        predicted = sum(tile256_selected(r["instance"], r["shape"][2], True) for r in rows)
+        assert tile256_in_step == predicted, (tile256_in_step, predicted)
 
     def total(sel):
         ms = sum(r["ms"] for r in sel)
@@ -177,7 +239,7 @@ def main():
     step = statistics.median(step_ms)
     out = {
         "card": card, "workload": bench.workload_config(1)["workload"], "detector_input": [n_pages, hp, wp],
-        "crops": crops, "matched_to_layers": matched,
+        "crops": crops, "matched_to_layers": matched, "tile256_launches_in_step": tile256_in_step,
         "layer_flop_sum": sum(r.get("flop", 0.0) for r in rows), "kernel_flop_count": flop_d + flop_r,
         "layers": rows,
         "craft": total([r for r in rows if r.get("net") == "craft"]),
@@ -197,11 +259,13 @@ def main():
     if not matched:
         print(f"WARNING: {len(conv)} conv_tc_kernel launches, {len(table)} layers in the table "
               f"(kernel counts craft {n_d}, crnn {n_r}): layers not named")
-    print(f"{'#':>3} {'layer':<28} {'n x h x w x cin -> cout':<28} {'k':>1} {'instance':<26} {'ms':>8} {'GFLOP':>9} {'TFLOP/s':>8}")
+    print(f"{'#':>3} {'layer':<28} {'n x h x w x cin -> cout':<28} {'k':>1} {'instance':<26} {'ms':>8} {'GFLOP':>9} {'TFLOP/s':>8}"
+          f" {'fill GB':>8} {'fill TB/s':>9}  tile")
     for r in rows:
         shape = "x".join(str(v) for v in r["shape"][:4]) + f"->{r['shape'][4]}" if "shape" in r else ""
         print(f"{r['launch']:>3} {r.get('layer', '?'):<28} {shape:<28} {r.get('ksize', ''):>1} {r['instance']:<26} "
-              f"{r['ms']:8.3f} {r.get('flop', 0) / 1e9:9.1f} {r.get('tflops') or 0:8.1f}")
+              f"{r['ms']:8.3f} {r.get('flop', 0) / 1e9:9.1f} {r.get('tflops') or 0:8.1f} "
+              f"{r.get('fill_bytes', 0) / 1e9:8.2f} {r.get('fill_tbps') or 0:9.2f}  {r.get('tile', '')}")
     for key in ("craft", "crnn", "conv_total"):
         t = out[key]
         print(f"{key:<10} {t['launches']:>3} launches {t['ms']:9.3f} ms {t['flop'] / 1e12:8.3f} TFLOP "
