@@ -510,6 +510,29 @@ typedef struct {
 } b2o_conv_test_desc;
 int b2o_conv_test(b2o_ctx* ctx, const b2o_conv_test_desc* desc, void* stream);
 
+/* The plan of one tensor-core convolution (test hook, not on the product path; host only, no context and no GPU): the
+ * choices the library makes before it launches a layer of (cin -> cout, ksize x ksize, dilation) over an (n, h, w, cin)
+ * input, writing fp32 when out_f32, with the fused 2x2 max pool, the fused CRAFT tail or the decoder's upsample-add of a
+ * (n, h/2, w/2, cout) tensor when pool, tail or up_add is set, on engine B2O_CONV_AUTO or B2O_CONV_TC_GENERIC, with the
+ * channels-by-pixels bodies allowed (swap = 1, the default) or not (B2O_TC_SWAP=0), on a GPU of sm_count SMs; the other
+ * switches at their defaults.  B2O_ERR_ARG where the library would refuse the launch (or the tensor cores do not run the
+ * layer).  Otherwise *plan: the conv_tc_kernel<block_n, kch, mode, pair, upadd> instance (mode 0 generic tiles, 1 halo
+ * tiles, 2 halo tiles with the filter bank resident in shared memory); body 0 pixels by channels, 1 channels by pixels,
+ * 2 channels by pixels on 16 x 16-pixel tiles; the tile_w x tile_h x tile_n pixel tile and the number of tiles (pixel
+ * tiles x output-channel tiles); the ring's stages, the bytes between stages and the bytes one stage's barrier expects;
+ * the resident filter bank's bytes (0: streamed with the stages); dynamic shared memory and grid of the launch.      */
+typedef struct {
+  int n, h, w, cin, cout, ksize, dilation;
+  int out_f32, pool, tail, up_add;
+  int engine, swap, sm_count;
+} b2o_conv_plan_desc;
+typedef struct {
+  int32_t block_n, kch, mode, pair, upadd, body;
+  int32_t tile_w, tile_h, tile_n, tiles;
+  int32_t stages, stage_bytes, stage_tx, resident_bytes, smem_bytes, grid;
+} b2o_conv_plan;
+int b2o_conv_plan_test(const b2o_conv_plan_desc* desc, b2o_conv_plan* plan);
+
 /* The plan b2o_warp_boxes derives from each box (test hook, not on the product path): get_rotated_box ordering,
  * get_rotated_width_height, the fp64 cv2.getPerspectiveTransform solve and the closed-form 3x3 inverse.  boxes: (n,4,2)
  * float32; plans: n records of 88 bytes.  m = inverse homography (destination -> source, row major), dw, dh = dsize of

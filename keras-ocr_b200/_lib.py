@@ -49,6 +49,19 @@ class _ConvTestDesc(ctypes.Structure):
                 ("w6_host", _fp), ("b6_host", _fp), ("w8_host", _fp), ("b8_host", _fp), ("scores_dev", _vp),
                 ("engine", _i)]
 
+
+class _ConvPlanDesc(ctypes.Structure):
+    """b2o_conv_plan_desc (include/b2ocr.h), field for field."""
+    _fields_ = [(name, _i) for name in ("n", "h", "w", "cin", "cout", "ksize", "dilation", "out_f32", "pool", "tail",
+                                        "up_add", "engine", "swap", "sm_count")]
+
+
+class _ConvPlan(ctypes.Structure):
+    """b2o_conv_plan (include/b2ocr.h), field for field."""
+    _fields_ = [(name, _c.c_int32) for name in ("block_n", "kch", "mode", "pair", "upadd", "body", "tile_w", "tile_h",
+                                                "tile_n", "tiles", "stages", "stage_bytes", "stage_tx", "resident_bytes",
+                                                "smem_bytes", "grid")]
+
 # name -> (restype, argtypes); mirrors include/b2ocr.h one to one
 SIGNATURES = {
     "b2o_version": (_i, []),
@@ -117,6 +130,7 @@ SIGNATURES = {
                              _c.POINTER(_c.c_float), _c.POINTER(_c.c_float), _i,
                              _c.POINTER(_c.c_float), _c.POINTER(_c.c_float), _vp, _i, _vp]),
     "b2o_conv_test": (_i, [_vp, _c.POINTER(_ConvTestDesc), _vp]),
+    "b2o_conv_plan_test": (_i, [_c.POINTER(_ConvPlanDesc), _c.POINTER(_ConvPlan)]),
     "b2o_warp_plan_test": (_i, [_vp, _vp, _i, _vp, _vp]),
     "b2o_get_boxes_test": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp, _i, _vp, _sz, _vp, _vp, _vp]),
 }
@@ -142,6 +156,18 @@ def load_library():
         fn.argtypes = args
     _lib = lib
     return lib
+
+
+def conv_plan(n, h, w, cin, cout, ksize, dilation=1, out_f32=False, pool=False, tail=False, up_add=False,
+              engine=CONV_AUTO, swap=True, sm_count=132):
+    """b2o_conv_plan_test (no GPU needed): the plan of one tensor-core convolution as a dict of b2o_conv_plan's fields,
+    or None where the library refuses the launch."""
+    desc = _ConvPlanDesc(n, h, w, cin, cout, ksize, dilation, int(out_f32), int(pool), int(tail), int(up_add), engine,
+                         int(swap), sm_count)
+    plan = _ConvPlan()
+    if load_library().b2o_conv_plan_test(ctypes.byref(desc), ctypes.byref(plan)) != 0:
+        return None
+    return {name: getattr(plan, name) for name, _ in _ConvPlan._fields_}
 
 
 def _tensor_array(weights):

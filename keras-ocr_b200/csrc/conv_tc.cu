@@ -838,40 +838,79 @@ double pick_box(int N, int H, int W, int* bw_l, int* bh_l, int* bn_l) {
   return best_cover;
 }
 
-thread_local const float* g_tail_host = nullptr;     // the fused tail's constants in AffConst::tail order (set by conv_tc_run)
+// The tensor-core tiling of a layer: K chunk kch (channels per stage) and N tile block_n; block_n = 0 leaves the layer to
+// the SIMT engine.  pair_ok: CTA pairs can run it (each CTA fetches block_n / 2 filter rows of a 64-channel chunk).
+struct TcTiling {
+  int kch, block_n;
+  bool pair_ok;
+};
+TcTiling plan_tc_tiling(int cin, int cout) {
+  TcTiling t = {cin % 64 == 0 ? 64 : (cin % 32 == 0 ? 32 : (cin % 16 == 0 ? 16 : 0)), 0, false};
+  if (t.kch == 0 || cout % 16 != 0) return t;
+  // N tile <= 128: a consumer thread holds BLOCK_N / 2 fp32 accumulators in registers
+  int bn = 128;
+  while (bn > 16 && (cout % bn != 0)) bn >>= 1;
+  if (cout % bn != 0) return t;
+  if (t.kch == 32 && bn > 32) return t;                    // instantiated combinations only
+  if (t.kch == 16 && bn != 32 && bn != 64) return t;
+  t.block_n = bn;
+  t.pair_ok = t.kch == 64 && bn >= 64;
+  return t;
+}
 
-template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD = false>
-int launch(b2o_ctx* ctx, const CUtensorMap& amap, const CUtensorMap& omap, const CUtensorMap& pmap, const ConvLayer& L,
-           const TcParams& p, int smem_bytes, cudaStream_t st) {
-  static thread_local AffConst ac;                         // 16 KB: filled per launch from the layer's host copies
-  if (p.aff_const) {
-    const size_t nb = static_cast<size_t>(L.cout) * sizeof(float);
-    memcpy(ac.s1, L.h_s1.data(), nb);
-    memcpy(ac.t1, L.h_t1.data(), nb);
-    if (!L.h_s2.empty()) { memcpy(ac.s2, L.h_s2.data(), nb); memcpy(ac.t2, L.h_t2.data(), nb); }
-    if (p.tail_out != nullptr && g_tail_host != nullptr) memcpy(ac.tail, g_tail_host, TAIL_FLOATS * sizeof(float));
-  }
+// The context's switches a plan depends on (the b2o_ctx fields of the same names).
+struct TcOptions {
+  int conv_engine;
+  bool tc_swap, tc_pair, tc_pair_generic, tc_aff_const;
+  int sm_count;
+};
+
+// What a plan reads of a layer (the ConvLayer fields of the same names).  host_aff: the epilogue constants, and the
+// fused tail's when there is one, have host copies, so they can travel in the AffConst kernel parameter.
+struct TcLayerShape {
+  const char* name;
+  int cin, cout, ksize, dil, kch, block_n;
+  bool pair_ok, host_aff;
+};
+
+// A conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD> instance.
+struct TcInstance {
+  int block_n, kch, mode;
+  bool pair, upadd;
+};
+
+// How one convolution runs: the kernel's parameters without the pointer fields and the strides and epilogue switches
+// that go with them, the instance, the launch shape and the TMA boxes of the activation map, the channels-by-pixels
+// output map and its pooled map.
+struct TcPlan {
+  TcParams p;
+  TcInstance inst;
+  int smem_bytes, grid;
+  cuuint32_t abox[4], obox[4], pbox[4];
+};
+
+template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD>
+int launch(b2o_ctx* ctx, const ConvLayer& L, const TcPlan& plan, const CUtensorMap& amap, const CUtensorMap& omap,
+           const CUtensorMap& pmap, const AffConst& ac, cudaStream_t st) {
   const void* fn = reinterpret_cast<const void*>(&conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD>);
   if (!ctx->configured.count(fn)) {                        // a per-device attribute: remembered per context
     B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD>,
                                              cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
     ctx->configured.insert(fn);
   }
-  // persistent: one CTA per SM; pairs: one cluster of two CTAs per two SMs
-  const int units = PAIR ? ctx->sm_count / 2 : ctx->sm_count;
-  const int grid = (p.total_tiles < units ? p.total_tiles : units) * (PAIR ? 2 : 1);
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (ctx->profile) {
     B2O_CUDA_CHECK(ctx, cudaEventCreate(&e0));
     B2O_CUDA_CHECK(ctx, cudaEventCreate(&e1));
     B2O_CUDA_CHECK(ctx, cudaEventRecord(e0, st));
   }
+  const TcParams& p = plan.p;
   if (PAIR) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
+    cfg.gridDim = dim3(plan.grid);
     cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = static_cast<size_t>(smem_bytes);
+    cfg.dynamicSmemBytes = static_cast<size_t>(plan.smem_bytes);
     cfg.stream = st;
     cudaLaunchAttribute attr;
     attr.id = cudaLaunchAttributeClusterDimension;
@@ -880,7 +919,7 @@ int launch(b2o_ctx* ctx, const CUtensorMap& amap, const CUtensorMap& omap, const
     cfg.numAttrs = 1;
     B2O_CUDA_CHECK(ctx, cudaLaunchKernelEx(&cfg, conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD>, amap, L.wmap_pair, omap, pmap, p, ac));
   } else {
-    conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD><<<grid, NUM_THREADS, smem_bytes, st>>>(amap, L.wmap, omap, pmap, p, ac);
+    conv_tc_kernel<BLOCK_N, KCH, MODE, PAIR, UPADD><<<plan.grid, NUM_THREADS, plan.smem_bytes, st>>>(amap, L.wmap, omap, pmap, p, ac);
   }
   B2O_LAUNCH_CHECK(ctx);
   if (ctx->profile) {
@@ -895,81 +934,63 @@ int launch(b2o_ctx* ctx, const CUtensorMap& amap, const CUtensorMap& omap, const
   return B2O_OK;
 }
 
-}  // namespace
+// Every compiled instance: MODE 0 = generic tiles, 1 = halo tiles (3x3, dilation 1), 2 = halo tiles + resident filter
+// bank; CTA pairs for 64-channel chunks with BLOCK_N >= 64; the decoder's upsample-add on generic 1x1 tiles.
+typedef int (*LaunchFn)(b2o_ctx*, const ConvLayer&, const TcPlan&, const CUtensorMap&, const CUtensorMap&,
+                        const CUtensorMap&, const AffConst&, cudaStream_t);
+struct TcKernel {
+  TcInstance inst;
+  LaunchFn launch;
+};
+const TcKernel kTcKernels[] = {
+    {{16, 64, 0, false, false}, launch<16, 64, 0, false, false>},   {{16, 64, 1, false, false}, launch<16, 64, 1, false, false>},
+    {{16, 64, 2, false, false}, launch<16, 64, 2, false, false>},   {{32, 64, 0, false, false}, launch<32, 64, 0, false, false>},
+    {{32, 64, 1, false, false}, launch<32, 64, 1, false, false>},   {{32, 64, 2, false, false}, launch<32, 64, 2, false, false>},
+    {{64, 64, 0, false, false}, launch<64, 64, 0, false, false>},   {{64, 64, 1, false, false}, launch<64, 64, 1, false, false>},
+    {{64, 64, 2, false, false}, launch<64, 64, 2, false, false>},   {{128, 64, 0, false, false}, launch<128, 64, 0, false, false>},
+    {{128, 64, 1, false, false}, launch<128, 64, 1, false, false>}, {{128, 64, 2, false, false}, launch<128, 64, 2, false, false>},
+    {{16, 32, 0, false, false}, launch<16, 32, 0, false, false>},   {{16, 32, 1, false, false}, launch<16, 32, 1, false, false>},
+    {{16, 32, 2, false, false}, launch<16, 32, 2, false, false>},   {{32, 32, 0, false, false}, launch<32, 32, 0, false, false>},
+    {{32, 32, 1, false, false}, launch<32, 32, 1, false, false>},   {{32, 32, 2, false, false}, launch<32, 32, 2, false, false>},
+    {{32, 16, 0, false, false}, launch<32, 16, 0, false, false>},   {{32, 16, 1, false, false}, launch<32, 16, 1, false, false>},
+    {{32, 16, 2, false, false}, launch<32, 16, 2, false, false>},   {{64, 16, 0, false, false}, launch<64, 16, 0, false, false>},
+    {{64, 16, 1, false, false}, launch<64, 16, 1, false, false>},   {{64, 16, 2, false, false}, launch<64, 16, 2, false, false>},
+    {{64, 64, 0, true, false}, launch<64, 64, 0, true, false>},     {{64, 64, 1, true, false}, launch<64, 64, 1, true, false>},
+    {{64, 64, 2, true, false}, launch<64, 64, 2, true, false>},     {{128, 64, 0, true, false}, launch<128, 64, 0, true, false>},
+    {{128, 64, 1, true, false}, launch<128, 64, 1, true, false>},   {{128, 64, 2, true, false}, launch<128, 64, 2, true, false>},
+    {{64, 64, 0, false, true}, launch<64, 64, 0, false, true>},     {{128, 64, 0, false, true}, launch<128, 64, 0, false, true>},
+};
 
-int conv_tc_prepare(b2o_ctx* ctx, ConvLayer& L) {
-  L.block_n = 0;
-  L.kch = L.cin % 64 == 0 ? 64 : (L.cin % 32 == 0 ? 32 : (L.cin % 16 == 0 ? 16 : 0));
-  if (L.kch == 0 || L.cout % 16 != 0) return B2O_OK;      // handled by the SIMT engine
-  // N tile <= 128: a consumer thread holds BLOCK_N / 2 fp32 accumulators in registers
-  int bn = 128;
-  while (bn > 16 && (L.cout % bn != 0)) bn >>= 1;
-  if (L.cout % bn != 0) return B2O_OK;
-  if (L.kch == 32 && bn > 32) return B2O_OK;               // instantiated combinations only
-  if (L.kch == 16 && bn != 32 && bn != 64) return B2O_OK;
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { ctx->set_error("cuTensorMapEncodeTiled entry point not available"); return B2O_ERR_CUDA; }
-  const cuuint64_t ktot = static_cast<cuuint64_t>(L.ksize) * L.ksize * L.cin;
-  cuuint64_t dims[2] = {ktot, static_cast<cuuint64_t>(L.cout)};
-  cuuint64_t strides[1] = {ktot * 2};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(L.kch), static_cast<cuuint32_t>(bn)};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(&L.wmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L.w_kmajor, dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(L.kch), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    ctx->set_error("cuTensorMapEncodeTiled(weights " + L.name + ") failed: " + std::to_string(static_cast<int>(r)));
-    return B2O_ERR_CUDA;
-  }
-  L.block_n = bn;
-  // CTA pairs: each CTA fetches bn / 2 filter rows of an n-tile (instantiated for 64-channel chunks, bn >= 64)
-  L.pair_ok = false;
-  if (L.kch == 64 && bn >= 64) {
-    cuuint32_t half_box[2] = {static_cast<cuuint32_t>(L.kch), static_cast<cuuint32_t>(bn / 2)};
-    r = enc(&L.wmap_pair, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L.w_kmajor, dims, strides, half_box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(L.kch), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      ctx->set_error("cuTensorMapEncodeTiled(pair weights " + L.name + ") failed: " + std::to_string(static_cast<int>(r)));
-      return B2O_ERR_CUDA;
-    }
-    L.pair_ok = true;
-  }
-  return B2O_OK;
+LaunchFn find_kernel(const TcInstance& k) {
+  for (const TcKernel& e : kTcKernels)
+    if (e.inst.block_n == k.block_n && e.inst.kch == k.kch && e.inst.mode == k.mode && e.inst.pair == k.pair &&
+        e.inst.upadd == k.upadd)
+      return e.launch;
+  return nullptr;
 }
 
-int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const TensorView& out, int out_f32,
-                cudaStream_t st, const TensorView* pool_out, int write_full, const ConvTail* tail, const TensorView* up_add) {
-  if (up_add != nullptr && (L.ksize != 1 || L.kch != 64 || L.block_n < 64 || out_f32 || pool_out != nullptr || tail != nullptr ||
+// Every decision about how a convolution of L over `in` runs on the tensor cores, with no CUDA call: an empty string
+// and *plan, or the reason the engine cannot run it.  pool_out and up_add are only read for their shapes (and up_add
+// for its alignment).
+std::string plan_conv_tc(const TcOptions& o, const TcLayerShape& L, const TensorView& in, int out_f32,
+                         const TensorView* pool_out, bool tail, const TensorView* up_add, TcPlan* plan) {
+  auto refuse = [&](const char* what, const char* after) { return std::string(what) + L.name + after; };
+  if (up_add != nullptr && (L.ksize != 1 || L.kch != 64 || L.block_n < 64 || out_f32 || pool_out != nullptr || tail ||
                             up_add->c != L.cout || up_add->n != in.n || 2 * up_add->h != in.h || 2 * up_add->w != in.w ||
-                            (up_add->ld % 8) || (reinterpret_cast<uintptr_t>(up_add->ptr) & 15))) {
-    ctx->set_error("conv_tc_run: up_add needs a 1x1 layer with 64-channel chunks and an exactly half-size fp16 tensor (" + L.name + ")");
-    return B2O_ERR_ARG;
-  }
-  if (tail != nullptr && (L.block_n != 16 || L.cout != 16 || pool_out != nullptr)) {
-    ctx->set_error("conv_tc_run: the fused tail needs a 16-channel layer (" + L.name + ")");
-    return B2O_ERR_ARG;
-  }
-  if (L.block_n == 0) { ctx->set_error("conv_tc_run: layer " + L.name + " not eligible"); return B2O_ERR_ARG; }
-  if (in.c != L.cin || out.c != L.cout || in.n != out.n || in.h != out.h || in.w != out.w) {
-    ctx->set_error("conv_tc_run: shape mismatch in " + L.name);
-    return B2O_ERR_ARG;
-  }
-  if ((reinterpret_cast<uintptr_t>(in.ptr) & 15) || (in.ld % 8) || (reinterpret_cast<uintptr_t>(out.ptr) & 15) ||
-      (out.ld % (out_f32 ? 4 : 8))) {
-    ctx->set_error("conv_tc_run: misaligned view in " + L.name);
-    return B2O_ERR_ARG;
-  }
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { ctx->set_error("cuTensorMapEncodeTiled entry point not available"); return B2O_ERR_CUDA; }
+                            (up_add->ld % 8) || (reinterpret_cast<uintptr_t>(up_add->ptr) & 15)))
+    return refuse("conv_tc_run: up_add needs a 1x1 layer with 64-channel chunks and an exactly half-size fp16 tensor (", ")");
+  if (tail && (L.block_n != 16 || L.cout != 16 || pool_out != nullptr))
+    return refuse("conv_tc_run: the fused tail needs a 16-channel layer (", ")");
+  if (L.block_n == 0) return refuse("conv_tc_run: layer ", " not eligible");
   const int kch = L.kch, bn = L.block_n;
   const int taps = L.ksize * L.ksize, kchunks = L.cin / kch;
   const int b_bytes = bn * kch * 2;
 
-  TcParams p;
-  memset(&p, 0, sizeof(p));
+  memset(plan, 0, sizeof(*plan));
+  TcParams& p = plan->p;
   p.N = in.n; p.H = in.h; p.W = in.w;
   p.cin = L.cin; p.cout = L.cout; p.ksize = L.ksize; p.dil = L.dil;
+  p.out_f32 = out_f32;
   pick_box(in.n, in.h, in.w, &p.bw_log2, &p.bh_log2, &p.bn_log2);
   // halo mode: 3x3, dilation 1, fixed 8 x 16 tile; skip it when that tile wastes >15 % more pixels.  The two
   // modes add the taps in different orders, so the choice must not depend on the batch size (a crop's result
@@ -979,13 +1000,19 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   const double generic_cover = pick_box(1 << 20, in.h, in.w, &dw, &dh, &dn) / big_n;
   const double halo_cover = double((in.w + 7) / 8 * 8) * double((in.h + 15) / 16 * 16);
   const bool want_pool = pool_out != nullptr;
-  p.halo = (L.ksize == 3 && L.dil == 1 && ctx->conv_engine != B2O_CONV_TC_GENERIC &&
+  p.halo = (L.ksize == 3 && L.dil == 1 && o.conv_engine != B2O_CONV_TC_GENERIC &&
             (halo_cover <= 1.15 * generic_cover || want_pool)) ? 1 : 0;
-  if (want_pool && !p.halo) { ctx->set_error("conv_tc_run: fused pool needs the halo tile (" + L.name + ")"); return B2O_ERR_ARG; }
+  if (want_pool && !p.halo) return refuse("conv_tc_run: fused pool needs the halo tile (", ")");
+  if (want_pool) {
+    if (out_f32 || pool_out->c != L.cout || pool_out->h != in.h / 2 || pool_out->w != in.w / 2 || (pool_out->ld % 8))
+      return refuse("conv_tc_run: bad pool view for ", "");
+    p.PH = pool_out->h; p.PW = pool_out->w;
+  }
+  if (up_add) { p.UH = up_add->h; p.UW = up_add->w; }
   if (p.halo) { p.bw_log2 = 3; p.bh_log2 = 4; p.bn_log2 = 0; }
   // CTA pairs (opt-in): halo tiles with B2O_TC_PAIR=1, generic tiles too with B2O_TC_PAIR=2; a pair covers
   // two horizontally adjacent tiles.  Same MMAs in the same order per output: bit-identical results.
-  const bool pair = ctx->tc_pair && (p.halo || ctx->tc_pair_generic) && L.pair_ok && ctx->conv_engine == B2O_CONV_AUTO &&
+  const bool pair = o.tc_pair && (p.halo || o.tc_pair_generic) && L.pair_ok && o.conv_engine == B2O_CONV_AUTO &&
                     up_add == nullptr;
   p.tiles_w = (in.w + (1 << p.bw_log2) - 1) >> p.bw_log2;
   if (pair) p.tiles_w = (p.tiles_w + 1) / 2;                // pair columns
@@ -993,15 +1020,15 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   p.tiles_n = (in.n + (1 << p.bn_log2) - 1) >> p.bn_log2;
   p.n_tiles = L.cout / bn;
   const long long total = static_cast<long long>(p.tiles_w) * p.tiles_h * p.tiles_n * p.n_tiles;
-  if (total > 0x7fffffffLL) { ctx->set_error("conv_tc_run: too many tiles"); return B2O_ERR_ARG; }
+  if (total > 0x7fffffffLL) return "conv_tc_run: too many tiles";
   p.total_tiles = static_cast<int>(total);
   // channels by pixels for the 64-channel fp16 layers; a pool whose output has no pixel keeps the old path
-  const bool ct = ctx->tc_swap && L.cout == 64 && bn == 64 && !out_f32 && up_add == nullptr && tail == nullptr && !pair &&
+  const bool ct = o.tc_swap && L.cout == 64 && bn == 64 && !out_f32 && up_add == nullptr && !tail && !pair &&
                   (!want_pool || (in.h >= 2 && in.w >= 2));
   p.ct = ct ? 1 : 0;
 
   // shared-memory plan: [ring of stages: A box | B boxes][resident filter bank][ct output tiles][barriers][epilogue constants]
-  p.aff_const = (ctx->tc_aff_const && L.cout <= 256 && static_cast<int>(L.h_s1.size()) == L.cout) ? 1 : 0;
+  p.aff_const = (o.tc_aff_const && L.cout <= 256 && L.host_aff) ? 1 : 0;
   p.aff_smem = (!p.aff_const && L.cout <= 256) ? 1 : 0;
   const int aff_bytes = (p.aff_smem ? 4 * L.cout * 4 : 0) + (tail ? TAIL_FLOATS * 4 : 0);
   const int tma_out_tiles = 2 * 128 * 64 * 2 + (want_pool ? 2 * 32 * 64 * 2 : 0);   // per warpgroup: 16 KB (+ 4 KB pooled)
@@ -1015,8 +1042,8 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   // channels by pixels on 16 x 16 tiles for the streamed 128-channel fp16 halo layers (conv_tc_body, WIDE): one filter
   // stage serves 256 pixels.  Only where the 16-wide tile covers the same columns of an image as the 8-wide one, so the
   // choice depends on the layer and the image shape alone, never on the batch.
-  const bool tile256 = ctx->tc_swap && p.halo && !p.resident && kch == 64 && bn == 128 && !pair && !out_f32 &&
-                       up_add == nullptr && tail == nullptr && (in.w + 15) / 16 * 16 == (in.w + 7) / 8 * 8 &&
+  const bool tile256 = o.tc_swap && p.halo && !p.resident && kch == 64 && bn == 128 && !pair && !out_f32 &&
+                       up_add == nullptr && !tail && (in.w + 15) / 16 * 16 == (in.w + 7) / 8 * 8 &&
                        (!want_pool || (in.h >= 2 && in.w >= 2));
   if (tile256) {
     p.tile256 = 1;
@@ -1032,47 +1059,122 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
   p.stage_tx = p.a_bytes + b_per_stage * b_bytes;
   p.ns = static_cast<int>((budget - (p.resident ? res_bytes : 0)) / p.stage_bytes);
   if (p.ns > MAX_RING) p.ns = MAX_RING;
-  if (p.ns < 2) { ctx->set_error("conv_tc_run: shared-memory plan failed for " + L.name); return B2O_ERR_ARG; }
+  if (p.ns < 2) return refuse("conv_tc_run: shared-memory plan failed for ", "");
   p.off_res = p.ns * p.stage_bytes;
   p.off_out = p.off_res + (p.resident ? static_cast<int>((res_bytes + 1023) / 1024 * 1024) : 0);
   p.off_bar = p.off_out + out_tiles;
-  int smem_bytes = p.off_bar + 512 + aff_bytes + 1024;
+  plan->smem_bytes = p.off_bar + 512 + aff_bytes + 1024;
   // the grid is one persistent CTA per SM: a request above half of the SM's 228 KB keeps a second CTA of a small layer
   // from landing on an SM that already runs one while other SMs sit idle
-  if (smem_bytes < 116 * 1024) smem_bytes = 116 * 1024;
+  if (plan->smem_bytes < 116 * 1024) plan->smem_bytes = 116 * 1024;
+  // persistent: one CTA per SM; pairs: one cluster of two CTAs per two SMs
+  const int units = pair ? o.sm_count / 2 : o.sm_count;
+  plan->grid = (p.total_tiles < units ? p.total_tiles : units) * (pair ? 2 : 1);
 
-  p.s1 = L.s1; p.t1 = L.t1; p.s2 = L.s2; p.t2 = L.t2; p.relu = L.relu;
-  if (up_add) { p.up_src = up_add->ptr; p.up_ld = up_add->ld; p.UH = up_add->h; p.UW = up_add->w; }
-  float tail_host[TAIL_FLOATS];
-  g_tail_host = nullptr;
-  if (tail && tail->h_w6 != nullptr) {                      // [w6 transposed | b6 | w8 | b8]
-    for (int j = 0; j < 16; ++j)
-      for (int c = 0; c < 16; ++c) tail_host[j * 16 + c] = tail->h_w6[c * 16 + j];
-    memcpy(tail_host + 256, tail->h_b6, 16 * sizeof(float));
-    memcpy(tail_host + 272, tail->h_w8, 32 * sizeof(float));
-    memcpy(tail_host + 304, tail->h_b8, 2 * sizeof(float));
-    g_tail_host = tail_host;
+  // the activation box: one tile, or on halo tiles 8 (tile256: 16) x 18 rows; channels-by-pixels output boxes: 64
+  // channels x one tile (tile256: one 16 x 8 half-tile), pooled: the 2x2 max of one 8 x 16 tile or 16 x 8 half-tile
+  const cuuint32_t bw = 1u << p.bw_log2, bh = 1u << p.bh_log2, bnn = 1u << p.bn_log2;
+  const cuuint32_t abox[4] = {static_cast<cuuint32_t>(kch), bw, p.halo ? 18u : bh, p.halo ? 1u : bnn};
+  const cuuint32_t obox[4] = {64, bw, tile256 ? 8u : bh, bnn};
+  const cuuint32_t pbox[4] = {64, tile256 ? 8u : 4u, tile256 ? 4u : 8u, 1};
+  memcpy(plan->abox, abox, sizeof(abox));
+  memcpy(plan->obox, obox, sizeof(obox));
+  memcpy(plan->pbox, pbox, sizeof(pbox));
+  plan->inst = {bn, kch, p.resident ? 2 : (p.halo ? 1 : 0), pair, up_add != nullptr};
+  if (find_kernel(plan->inst) == nullptr) return refuse("conv_tc_run: no kernel instance for ", "");
+  return std::string();
+}
+
+}  // namespace
+
+int conv_tc_prepare(b2o_ctx* ctx, ConvLayer& L) {
+  const TcTiling t = plan_tc_tiling(L.cin, L.cout);
+  L.kch = t.kch;
+  L.block_n = 0;
+  L.pair_ok = false;
+  if (t.block_n == 0) return B2O_OK;                       // handled by the SIMT engine
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { ctx->set_error("cuTensorMapEncodeTiled entry point not available"); return B2O_ERR_CUDA; }
+  const cuuint64_t ktot = static_cast<cuuint64_t>(L.ksize) * L.ksize * L.cin;
+  cuuint64_t dims[2] = {ktot, static_cast<cuuint64_t>(L.cout)};
+  cuuint64_t strides[1] = {ktot * 2};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(L.kch), static_cast<cuuint32_t>(t.block_n)};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(&L.wmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L.w_kmajor, dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(L.kch), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    ctx->set_error("cuTensorMapEncodeTiled(weights " + L.name + ") failed: " + std::to_string(static_cast<int>(r)));
+    return B2O_ERR_CUDA;
   }
-  if (tail) { p.tail_w6 = tail->w6; p.tail_b6 = tail->b6; p.tail_w8 = tail->w8; p.tail_b8 = tail->b8; p.tail_out = tail->scores; }
-  p.out = out.ptr; p.out_ld = out.ld; p.out_f32 = out_f32; p.write_full = write_full;
-  if (want_pool) {
-    if (out_f32 || pool_out->c != L.cout || pool_out->h != in.h / 2 || pool_out->w != in.w / 2 || (pool_out->ld % 8)) {
-      ctx->set_error("conv_tc_run: bad pool view for " + L.name);
-      return B2O_ERR_ARG;
+  L.block_n = t.block_n;
+  if (t.pair_ok) {
+    cuuint32_t half_box[2] = {static_cast<cuuint32_t>(L.kch), static_cast<cuuint32_t>(t.block_n / 2)};
+    r = enc(&L.wmap_pair, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, L.w_kmajor, dims, strides, half_box, estr,
+            CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(L.kch), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      ctx->set_error("cuTensorMapEncodeTiled(pair weights " + L.name + ") failed: " + std::to_string(static_cast<int>(r)));
+      return B2O_ERR_CUDA;
     }
-    p.pool_out = pool_out->ptr; p.pool_ld = pool_out->ld; p.PH = pool_out->h; p.PW = pool_out->w;
+    L.pair_ok = true;
+  }
+  return B2O_OK;
+}
+
+int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const TensorView& out, int out_f32,
+                cudaStream_t st, const TensorView* pool_out, int write_full, const ConvTail* tail, const TensorView* up_add) {
+  if (in.c != L.cin || out.c != L.cout || in.n != out.n || in.h != out.h || in.w != out.w) {
+    ctx->set_error("conv_tc_run: shape mismatch in " + L.name);
+    return B2O_ERR_ARG;
+  }
+  if ((reinterpret_cast<uintptr_t>(in.ptr) & 15) || (in.ld % 8) || (reinterpret_cast<uintptr_t>(out.ptr) & 15) ||
+      (out.ld % (out_f32 ? 4 : 8))) {
+    ctx->set_error("conv_tc_run: misaligned view in " + L.name);
+    return B2O_ERR_ARG;
+  }
+  const TcOptions opt = {ctx->conv_engine, ctx->tc_swap, ctx->tc_pair, ctx->tc_pair_generic, ctx->tc_aff_const,
+                         ctx->sm_count};
+  const int cout = L.cout;
+  const bool host_aff = static_cast<int>(L.h_s1.size()) == cout &&
+                        (L.s2 == nullptr || static_cast<int>(L.h_s2.size()) == cout) &&
+                        (tail == nullptr || tail->h_w6 != nullptr);
+  const TcLayerShape shape = {L.name.c_str(), L.cin, cout, L.ksize, L.dil, L.kch, L.block_n, L.pair_ok, host_aff};
+  TcPlan plan;
+  const std::string err = plan_conv_tc(opt, shape, in, out_f32, pool_out, tail != nullptr, up_add, &plan);
+  if (!err.empty()) { ctx->set_error(err); return B2O_ERR_ARG; }
+
+  TcParams& p = plan.p;
+  p.s1 = L.s1; p.t1 = L.t1; p.s2 = L.s2; p.t2 = L.t2; p.relu = L.relu;
+  p.out = out.ptr; p.out_ld = out.ld; p.write_full = write_full;
+  if (pool_out) { p.pool_out = pool_out->ptr; p.pool_ld = pool_out->ld; }
+  if (up_add) { p.up_src = up_add->ptr; p.up_ld = up_add->ld; }
+  if (tail) { p.tail_w6 = tail->w6; p.tail_b6 = tail->b6; p.tail_w8 = tail->w8; p.tail_b8 = tail->b8; p.tail_out = tail->scores; }
+  AffConst ac;                                             // the epilogue constants as a kernel parameter (16 KB)
+  if (p.aff_const) {
+    const size_t nb = static_cast<size_t>(cout) * sizeof(float);
+    memcpy(ac.s1, L.h_s1.data(), nb);
+    memcpy(ac.t1, L.h_t1.data(), nb);
+    if (L.s2 != nullptr) { memcpy(ac.s2, L.h_s2.data(), nb); memcpy(ac.t2, L.h_t2.data(), nb); }
+    if (tail) {                                            // [w6 transposed | b6 | w8 | b8]
+      for (int j = 0; j < 16; ++j)
+        for (int c = 0; c < 16; ++c) ac.tail[j * 16 + c] = tail->h_w6[c * 16 + j];
+      memcpy(ac.tail + 256, tail->h_b6, 16 * sizeof(float));
+      memcpy(ac.tail + 272, tail->h_w8, 32 * sizeof(float));
+      memcpy(ac.tail + 304, tail->h_b8, 2 * sizeof(float));
+    }
   }
 
+  EncodeTiledFn enc = get_encode();
+  if (!enc) { ctx->set_error("cuTensorMapEncodeTiled entry point not available"); return B2O_ERR_CUDA; }
   CUtensorMap amap;
   cuuint64_t dims[4] = {static_cast<cuuint64_t>(in.c), static_cast<cuuint64_t>(in.w), static_cast<cuuint64_t>(in.h),
                         static_cast<cuuint64_t>(in.n)};
   cuuint64_t strides[3] = {static_cast<cuuint64_t>(in.ld) * 2, static_cast<cuuint64_t>(in.ld) * 2 * in.w,
                            static_cast<cuuint64_t>(in.ld) * 2 * in.w * in.h};
-  cuuint32_t box[4] = {static_cast<cuuint32_t>(kch), 1u << p.bw_log2, 1u << p.bh_log2, 1u << p.bn_log2};
-  if (p.halo) { box[1] = 1u << p.bw_log2; box[2] = 18; box[3] = 1; }   // 8 (tile256: 16) x 18 rows
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(&amap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, in.ptr, dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(kch), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  CUresult r = enc(&amap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, in.ptr, dims, strides, plan.abox, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(L.kch), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     ctx->set_error("cuTensorMapEncodeTiled(activation for " + L.name + ") failed: " +
@@ -1080,54 +1182,49 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
     return B2O_ERR_CUDA;
   }
   // channels-by-pixels output maps: 4-D (c, w, h, n) over the layer's cout-channel view (a channel slice: base pointer +
-  // ld), boxes of 64 channels x one tile (tile256: one 16 x 8 half-tile)
+  // ld)
   CUtensorMap omap, pmap;
   memset(&omap, 0, sizeof(omap));
   memset(&pmap, 0, sizeof(pmap));
   auto encode_out = [&](CUtensorMap* m, void* ptr, int ld, int n, int h, int w, const cuuint32_t* obox) {
-    cuuint64_t odims[4] = {static_cast<cuuint64_t>(L.cout), static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h),
+    cuuint64_t odims[4] = {static_cast<cuuint64_t>(cout), static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h),
                            static_cast<cuuint64_t>(n)};
     cuuint64_t ostr[3] = {static_cast<cuuint64_t>(ld) * 2, static_cast<cuuint64_t>(ld) * 2 * w,
                           static_cast<cuuint64_t>(ld) * 2 * w * h};
     return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, ptr, odims, ostr, obox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   };
-  if ((ct || tile256) && write_full) {
-    const cuuint32_t obox[4] = {64, 1u << p.bw_log2, tile256 ? 8u : 1u << p.bh_log2, 1u << p.bn_log2};
-    r = encode_out(&omap, out.ptr, out.ld, in.n, in.h, in.w, obox);
-  }
-  if ((ct || tile256) && want_pool && r == CUDA_SUCCESS) {
-    // the 2x2 max of one 8 x 16 halo tile, or of one 16 x 8 half of a 16 x 16 tile
-    const cuuint32_t pbox[4] = {64, tile256 ? 8u : 4u, tile256 ? 4u : 8u, 1};
-    r = encode_out(&pmap, pool_out->ptr, pool_out->ld, in.n, p.PH, p.PW, pbox);
-  }
+  const bool tma_out = p.ct || p.tile256;
+  if (tma_out && write_full) r = encode_out(&omap, out.ptr, out.ld, in.n, in.h, in.w, plan.obox);
+  if (tma_out && pool_out && r == CUDA_SUCCESS) r = encode_out(&pmap, pool_out->ptr, pool_out->ld, in.n, p.PH, p.PW, plan.pbox);
   if (r != CUDA_SUCCESS) {
     ctx->set_error("cuTensorMapEncodeTiled(output of " + L.name + ") failed: " + std::to_string(static_cast<int>(r)));
     return B2O_ERR_CUDA;
   }
-  if (up_add != nullptr) {                                 // generic 1x1 tiles
-    if (bn == 64) return launch<64, 64, 0, false, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);
-    if (bn == 128) return launch<128, 64, 0, false, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);
-  }
-#define B2O_TC_PAIR_CASE(BN)                                                                                           \
-  if (pair && bn == BN) {                                                                                              \
-    if (p.resident) return launch<BN, 64, 2, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                       \
-    if (p.halo) return launch<BN, 64, 1, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                           \
-    return launch<BN, 64, 0, true>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                                       \
-  }
-  B2O_TC_PAIR_CASE(64); B2O_TC_PAIR_CASE(128);
-#undef B2O_TC_PAIR_CASE
-  if (tile256) ++ctx->tc_tile256_launches;
-#define B2O_TC_CASE(BN, KC)                                                                                            \
-  if (bn == BN && kch == KC) {                                                                                         \
-    if (p.resident) return launch<BN, KC, 2, false>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                      \
-    if (p.halo) return launch<BN, KC, 1, false>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                          \
-    return launch<BN, KC, 0, false>(ctx, amap, omap, pmap, L, p, smem_bytes, st);                                      \
-  }
-  B2O_TC_CASE(16, 64); B2O_TC_CASE(32, 64); B2O_TC_CASE(64, 64); B2O_TC_CASE(128, 64);
-  B2O_TC_CASE(16, 32); B2O_TC_CASE(32, 32);
-  B2O_TC_CASE(32, 16); B2O_TC_CASE(64, 16);
-#undef B2O_TC_CASE
-  ctx->set_error("conv_tc_run: no kernel instance for " + L.name);
-  return B2O_ERR_ARG;
+  if (p.tile256) ++ctx->tc_tile256_launches;
+  return find_kernel(plan.inst)(ctx, L, plan, amap, omap, pmap, ac, st);
+}
+
+extern "C" int b2o_conv_plan_test(const b2o_conv_plan_desc* d, b2o_conv_plan* out) {
+  if (!d || !out || d->n <= 0 || d->h <= 0 || d->w <= 0 || d->cin <= 0 || d->cout <= 0 || d->ksize <= 0 ||
+      d->dilation <= 0 || d->sm_count <= 0 || (d->engine != B2O_CONV_AUTO && d->engine != B2O_CONV_TC_GENERIC))
+    return B2O_ERR_ARG;
+  const TcOptions opt = {d->engine, d->swap != 0, false, false, true, d->sm_count};
+  const TcTiling t = plan_tc_tiling(d->cin, d->cout);
+  const TcLayerShape L = {"test", d->cin, d->cout, d->ksize, d->dilation, t.kch, t.block_n, t.pair_ok, true};
+  const TensorView in = make_view(nullptr, d->n, d->h, d->w, d->cin);
+  const TensorView half = make_view(nullptr, d->n, d->h / 2, d->w / 2, d->cout);     // pooled output, low-res summand
+  TcPlan plan;
+  if (!plan_conv_tc(opt, L, in, d->out_f32, d->pool ? &half : nullptr, d->tail != 0, d->up_add ? &half : nullptr, &plan).empty())
+    return B2O_ERR_ARG;
+  const TcParams& p = plan.p;
+  out->block_n = plan.inst.block_n; out->kch = plan.inst.kch; out->mode = plan.inst.mode;
+  out->pair = plan.inst.pair; out->upadd = plan.inst.upadd;
+  out->body = p.tile256 ? 2 : p.ct;
+  out->tile_w = 1 << p.bw_log2; out->tile_h = 1 << p.bh_log2; out->tile_n = 1 << p.bn_log2;
+  out->tiles = p.total_tiles;
+  out->stages = p.ns; out->stage_bytes = p.stage_bytes; out->stage_tx = p.stage_tx;
+  out->resident_bytes = p.resident ? d->ksize * d->ksize * d->cin * plan.inst.block_n * 2 : 0;
+  out->smem_bytes = plan.smem_bytes; out->grid = plan.grid;
+  return B2O_OK;
 }

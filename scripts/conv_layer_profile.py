@@ -8,7 +8,7 @@ profiler for the step time.  The trace's ``conv_tc_kernel`` launches, in launch 
 sequence of ``b2o_craft_forward`` and ``b2o_crnn_forward``; for each layer the script prints its shape, the kernel
 instance, the time, the algorithmic FLOPs (2 * pixels * taps * cin * cout with the reference's channel counts, as
 ``launch()`` in csrc/conv_tc.cu counts them) and the rate, the bytes its TMA loads bring into shared memory (from the
-plan ``conv_tc_run`` makes for that shape and instance, see ``tma_fill_bytes``) and that fill rate, then totals for CRAFT, the CRNN and the step, and the share of
+library's plan of that launch, see ``tma_fill_bytes``) and that fill rate, then totals for CRAFT, the CRNN and the step, and the share of
 the step spent outside ``conv_tc_kernel``.  The same data goes to OUT_DIR/conv_layer_profile.json, with the card's name,
 power limit and clocks (read-only nvidia-smi query).  Only the public Python API is used.
 """
@@ -98,52 +98,25 @@ def instance(name):
     return m.group(1).replace(" ", "") if m else name
 
 
-def pick_box(n, h, w):
-    """pick_box() of csrc/conv_tc.cu: the (bw, bh, bn) power-of-two 128-pixel box that wastes the fewest pixels."""
-    best, box = 1e30, (128, 1, 1)
-    for lw in range(8):
-        for lh in range(8 - lw):
-            ln = 7 - lw - lh
-            bw, bh, bn = 1 << lw, 1 << lh, 1 << ln
-            if ln > 0 and bn > 2 * n:
-                continue
-            cover = float(-(-w // bw) * bw) * float(-(-h // bh) * bh) * float(-(-n // bn) * bn)
-            score = cover * (1.0 + 0.001 * (7 - lw)) * (1.05 if (bw < 8 and w >= 8) else 1.0)
-            if score < best:
-                best, box = score, (bw, bh, bn)
-    return box
+# layers whose kernel runs more channels than the reference layer has (the FLOP count keeps the reference's): the stem's
+# 3 input channels padded to 16, the STN's 400 GEMM columns padded to 512
+RUN_CHANNELS = {"stem16 (basenet.slice1.0)": (16, 64), "stn.conv_a (as 1x1 GEMM)": (512, 512)}
+DILATION = {"basenet.slice5.1 (dil 6)": 6}
 
 
-def tile256_selected(inst, w, wide_body):
-    """conv_tc_run's choice of the 16 x 16-pixel channels-by-pixels body of conv_tc_kernel<128,64,1,false,false>: the
-    build has it, B2O_TC_SWAP is not 0, and the 16-wide tile covers the same columns as the 8-wide one."""
-    return (wide_body and os.environ.get("B2O_TC_SWAP", "1") != "0" and inst == "128,64,1,false,false" and
-            (w + 15) // 16 * 16 == (w + 7) // 8 * 8)
-
-
-def tma_fill_bytes(inst, n, h, w, k, cin, cout, sm_count, wide_body):
-    """Bytes the launch's TMA loads bring into shared memory, from conv_tc_run's plan: every tile takes one stage per
-    (dx | tap, 64/32/16-channel chunk) holding its activation box (halo: 18 rows of the tile's width) and, unless the
-    filter bank is resident, the stage's filter rows (3 taps on halo tiles); a resident bank is loaded once per CTA.
-    Returns (bytes, tile description); None for CTA pairs (not in the default plan)."""
-    bn, kch, mode, pair = [int(v) if v.isdigit() else v for v in inst.split(",")[:4]]
-    if pair == "true":
-        return None
-    b_bytes = bn * kch * 2
-    kchunks = cin // kch
-    if mode >= 1:
-        bw, bh, bnn = (16, 16, 1) if tile256_selected(inst, w, wide_body) else (8, 16, 1)
-        groups, a_bytes = 3, (bh + 2) * bw * kch * 2
-    else:
-        bw, bh, bnn = pick_box(n, h, w)
-        groups, a_bytes = k * k, 128 * kch * 2
-    tiles = (-(-w // bw)) * (-(-h // bh)) * (-(-n // bnn)) * (cout // bn)
-    taps_per_stage = 0 if mode == 2 else (3 if mode == 1 else 1)
-    stage_tx = a_bytes + taps_per_stage * b_bytes
-    total = tiles * groups * kchunks * stage_tx
-    if mode == 2:
-        total += min(tiles, sm_count) * k * k * kchunks * b_bytes
-    return total, f"{bw}x{bh}x{bnn} stage {stage_tx} B"
+def tma_fill_bytes(layer, n, h, w, k, cin, cout, sm_count):
+    """Bytes the launch's TMA loads bring into shared memory, from the library's plan of the launch
+    (``b2o_conv_plan_test``): every tile takes one stage per (dx | tap, 64/32/16-channel chunk) holding its activation
+    box and, unless the filter bank is resident, the stage's filter rows; a resident bank is loaded once per CTA.
+    Returns (bytes, tile description, planned instance, whether it runs the 16 x 16 body)."""
+    from keras_ocr_b200 import _lib
+    cin, cout = RUN_CHANNELS.get(layer, (cin, cout))
+    plan = _lib.conv_plan(n, h, w, cin, cout, k, DILATION.get(layer, 1), pool="+pool" in layer, tail="+tail" in layer,
+                          out_f32="fp32 out" in layer, swap=os.environ.get("B2O_TC_SWAP", "1") != "0", sm_count=sm_count)
+    groups = 3 if plan["mode"] else k * k
+    total = plan["tiles"] * groups * (cin // plan["kch"]) * plan["stage_tx"] + plan["grid"] * plan["resident_bytes"]
+    inst = ",".join(str(plan[f]) for f in ("block_n", "kch", "mode")) + ",false," + ("true" if plan["upadd"] else "false")
+    return total, f"{plan['tile_w']}x{plan['tile_h']}x{plan['tile_n']} stage {plan['stage_tx']} B", inst, plan["body"] == 2
 
 
 def main():
@@ -184,7 +157,7 @@ def main():
     det.ctx.profile_enable(0); rec.ctx.profile_enable(0)
 
     def tile256_count():
-        return sum(c.tile256_launches() for c in (det.ctx, rec.ctx)) if hasattr(det.ctx.lib, "b2o_tc_tile256_launches") else 0
+        return sum(c.tile256_launches() for c in (det.ctx, rec.ctx))
 
     from torch.profiler import ProfilerActivity, profile
     tile256_in_step = -tile256_count()
@@ -213,7 +186,6 @@ def main():
     table += crnn_layers(crops)
     matched = len(conv) == len(table) and n_d == n_craft and n_r == len(table) - n_craft
     sm_count = torch.cuda.get_device_properties(device).multi_processor_count
-    wide_body = hasattr(det.ctx.lib, "b2o_tc_tile256_launches")
     rows = []
     for i, (kname, _, dur) in enumerate(conv):
         row = {"launch": i, "instance": instance(kname), "ms": dur / 1e3}
@@ -222,12 +194,13 @@ def main():
             flop = 2.0 * n * h * w * k * k * cin * cout
             row.update({"net": "craft" if i < n_craft else "crnn", "layer": name, "shape": [n, h, w, cin, cout],
                         "ksize": k, "flop": flop, "tflops": flop / (dur * 1e-6) / 1e12})
-            fill = tma_fill_bytes(row["instance"], n, h, w, k, cin, cout, sm_count, wide_body)
-            if fill is not None:
-                row.update({"fill_bytes": fill[0], "fill_tbps": fill[0] / (dur * 1e-6) / 1e12, "tile": fill[1]})
+            if ",true," not in row["instance"]:           # CTA pairs (B2O_TC_PAIR) are not in the default plan
+                fill, tile, planned, wide = tma_fill_bytes(name, n, h, w, k, cin, cout, sm_count)
+                assert planned == row["instance"], (name, planned, row["instance"])
+                row.update({"fill_bytes": fill, "fill_tbps": fill / (dur * 1e-6) / 1e12, "tile": tile, "tile256": wide})
         rows.append(row)
-    if wide_body and matched:      # the plan reproduced above must agree with the launches the library counted
-        predicted = sum(tile256_selected(r["instance"], r["shape"][2], True) for r in rows)
+    if matched:      # the plans above must agree with the launches the library counted
+        predicted = sum(r.get("tile256", False) for r in rows)
         assert tile256_in_step == predicted, (tile256_in_step, predicted)
 
     def total(sel):

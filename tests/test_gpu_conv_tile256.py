@@ -22,6 +22,7 @@ import torch
 
 from keras_ocr_b200 import _lib
 from tests import stage_refs as R
+from tests import test_conv_plans as P
 from tests.test_gpu_conv_transposed import SENT16, Slab, _make_ctx, _untouched
 
 pytestmark = pytest.mark.gpu
@@ -44,24 +45,10 @@ LAYERS = [
 SHAPES = [(1, 16, 16), (2, 31, 47), (1, 200, 31), (2, 100, 15), (1, 32, 40), (1, 17, 24)]
 
 
-def _generic_cover(h, w):
-    """Pixels per image that conv_tc_run's best generic 128-pixel box covers (pick_box with an unbounded batch)."""
-    best, cover = 1e30, 0.0
-    for lw in range(8):
-        for lh in range(8 - lw):
-            bw, bh = 1 << lw, 1 << lh
-            c = float(-(-w // bw) * bw) * float(-(-h // bh) * bh)
-            score = c * (1.0 + 0.001 * (7 - lw)) * (1.05 if (bw < 8 and w >= 8) else 1.0)
-            if score < best:
-                best, cover = score, c
-    return cover
-
-
-def _selected(h, w, pool):
-    """conv_tc_run's choice for these layers: halo tiles (forced by the fused pool, else when they waste at most 15 %
-    more pixels than the generic box), and a 16-wide tile covering the same columns as the 8-wide one."""
-    halo = pool or (w + 7) // 8 * 8 * ((h + 15) // 16 * 16) <= 1.15 * _generic_cover(h, w)
-    return halo and (w + 15) // 16 * 16 == (w + 7) // 8 * 8
+def _selected(cin, cout, shape, pool):
+    """The plan's choice of the 16 x 16 body for this layer and shape, as tests/test_conv_plans.py restates it (and
+    checks the restatement against the library's plan)."""
+    return P.restate(*shape, cin, cout, 3, pool=pool)["body"] == P.TILE256
 
 
 def _inputs(name, n, h, w, cin, cout, aff2):
@@ -109,7 +96,7 @@ def test_tile256_bit_identical(ctxs, layer, shape):
     x, *params = _inputs(name, *shape, cin, cout, aff2)
     a_out, a_pool, a_ran = _run(ctxs["swap"], layer, x, params)
     b_out, b_pool, b_ran = _run(ctxs["noswap"], layer, x, params)
-    assert a_ran == (1 if _selected(shape[1], shape[2], pool) else 0), f"{name} {shape}: 16 x 16 body launches {a_ran}"
+    assert a_ran == (1 if _selected(cin, cout, shape, pool) else 0), f"{name} {shape}: 16 x 16 body launches {a_ran}"
     assert b_ran == 0, "B2O_TC_SWAP=0 ran the 16 x 16 body"
     assert torch.equal(a_out.raw, b_out.raw), f"{name} {shape}: out differs (or a store outside the view)"
     if write_full:
