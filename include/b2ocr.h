@@ -183,6 +183,23 @@ int b2o_compact_polys(b2o_ctx* ctx, const float* polys_dev, const int32_t* point
 int b2o_compact_boxes(b2o_ctx* ctx, const float* boxes_dev, const int32_t* counts_dev, int n, int max_boxes,
                       float* flat_dev, int32_t* image_index_dev, void* stream);
 
+/* Text lines in reading order (DESIGN.md section 1, "Text lines").  boxes (n, max_boxes, 4, 2) float32 as b2o_get_boxes
+ * writes them (box[0] -> box[1] the reading direction), c_i = min(counts[i], max_boxes) words in image i; only those
+ * are read.  Words are linked when their directions agree within cos_tol (= cos(angle tolerance), computed by the
+ * caller), their heights within height_ratio, their centres lie within offset_ratio * the smaller height of each
+ * other's centre line and the gap between them is at most gap_ratio * the larger height; lines are the connected
+ * components.  Outputs, a CSR table per image: line_counts[i] = L_i lines; the words of line l in reading order are
+ * word_order[i, line_start[i, l] : line_start[i, l + 1]] (word indices into boxes[i]); line_boxes[i, l] the line's
+ * (4, 2) box, box[0] -> box[1] its reading direction; lines in page order.  Written: line_counts (n) all,
+ * word_order[i, :c_i], line_start[i, :L_i + 1], line_boxes[i, :L_i]; every other slot is left as it was.
+ * word_order is (n, max_boxes), line_start (n, max_boxes + 1), line_boxes (n, max_boxes, 4, 2).  Every value is fp64
+ * with a fixed operation order: bit-identical in any batch and on every run.  n = 0 does nothing.             */
+size_t b2o_lines_workspace_bytes(int n, int max_boxes);
+int b2o_group_lines(b2o_ctx* ctx, const float* boxes_dev, const int32_t* counts_dev, int n, int max_boxes,
+                    double cos_tol, double height_ratio, double offset_ratio, double gap_ratio,
+                    int32_t* line_counts_dev, int32_t* word_order_dev, int32_t* line_start_dev,
+                    float* line_boxes_dev, void* ws_dev, size_t ws_bytes, void* stream);
+
 /* tools.warpBox over box groups (recognition.py:506-519; tools.py:61-117).  boxes: (n_boxes,4,2)
  * float32; image_index[k] selects the gray image of box k.  crops: (n_boxes,31,200) uint8
  * (exactly warpBox's output) and, when crnn_in != NULL, the CRNN input (n_boxes,200,31) fp16 =

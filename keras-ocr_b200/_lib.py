@@ -91,6 +91,9 @@ SIGNATURES = {
     "b2o_get_boxes_poly": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _sz, _vp]),
     "b2o_compact_polys": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "b2o_warp_polys": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "b2o_lines_workspace_bytes": (_sz, [_i, _i]),
+    "b2o_group_lines": (_i, [_vp, _vp, _vp, _i, _i, _c.c_double, _c.c_double, _c.c_double, _c.c_double, _vp, _vp, _vp,
+                             _vp, _vp, _sz, _vp]),
     "b2o_record_floats": (_sz, [_i]),
     "b2o_record_floats_scored": (_sz, [_i]),
     "b2o_pack_records": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
@@ -310,6 +313,16 @@ class Context:
     def warp_polys(self, img, channels, n, h, w, polys, points, image_index, n_polys, crops, crnn_in, stream):
         self._check(self.lib.b2o_warp_polys(self.handle, img, channels, n, h, w, polys, points, image_index, n_polys,
                                             crops, crnn_in, stream), "b2o_warp_polys")
+
+    def lines_workspace_bytes(self, n, max_boxes):
+        return int(self.lib.b2o_lines_workspace_bytes(n, max_boxes))
+
+    def group_lines(self, boxes, counts, n, max_boxes, cos_tol, height_ratio, offset_ratio, gap_ratio, line_counts,
+                    word_order, line_start, line_boxes, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_group_lines(self.handle, boxes, counts, n, max_boxes, float(cos_tol),
+                                             float(height_ratio), float(offset_ratio), float(gap_ratio), line_counts,
+                                             word_order, line_start, line_boxes, ws, ws_bytes, stream),
+                    "b2o_group_lines")
 
     def record_floats(self, rec_boxes):
         return int(self.lib.b2o_record_floats(rec_boxes))

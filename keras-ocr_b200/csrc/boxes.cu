@@ -57,25 +57,6 @@ __global__ void binarize_kernel(const float* __restrict__ scores, long long tota
   label[p] = lab;
 }
 
-__device__ __forceinline__ int uf_find(const int* L, int a) {
-  while (true) {
-    const int p = *reinterpret_cast<const volatile int*>(L + a);
-    if (p == a) return a;
-    a = p;
-  }
-}
-__device__ __forceinline__ void uf_unite(int* L, int a, int b) {
-  while (true) {
-    a = uf_find(L, a);
-    b = uf_find(L, b);
-    if (a == b) return;
-    if (a < b) { const int t = a; a = b; b = t; }
-    const int old = atomicMin(L + a, b);     // hang the larger root under the smaller one
-    if (old == a) return;
-    a = old;
-  }
-}
-
 __global__ void merge_kernel(const uint8_t* __restrict__ mask, int* __restrict__ label, long long total, int hs,
                              int ws) {
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;

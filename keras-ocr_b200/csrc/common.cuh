@@ -170,6 +170,28 @@ int upsample_run(b2o_ctx* ctx, const TensorView& in, const TensorView& out, cuda
 int head_tail_run(b2o_ctx* ctx, const ConvLayer& L6, const ConvLayer& L8, const TensorView& in,
                   float* scores, cudaStream_t st);
 
+// ---- atomic union-find (boxes.cu's connected components, lines.cu's text lines) ----------------------------
+// L[a] is a's parent; a root is its own parent.  uf_unite hangs the larger root under the smaller one, so every root is
+// the smallest index of its set, whatever order the unions run in.
+static __device__ __forceinline__ int uf_find(const int* L, int a) {
+  while (true) {
+    const int p = *reinterpret_cast<const volatile int*>(L + a);
+    if (p == a) return a;
+    a = p;
+  }
+}
+static __device__ __forceinline__ void uf_unite(int* L, int a, int b) {
+  while (true) {
+    a = uf_find(L, a);
+    b = uf_find(L, b);
+    if (a == b) return;
+    if (a < b) { const int t = a; a = b; b = t; }
+    const int old = atomicMin(L + a, b);     // hang the larger root under the smaller one
+    if (old == a) return;
+    a = old;
+  }
+}
+
 // ---- box corner order (image.cu's warp, rotation.cu's box roll, ctc_align.cu's cells) ------------
 // fp64 Euclidean distance of two float32 points, as scipy's cdist computes it (tools.py:41-57)
 static __device__ inline double corner_dist(const float* a, const float* b) {

@@ -3,6 +3,8 @@
 ``detect`` keeps the reference signature and return type; the work is done by the CUDA library:
 compute_input + CRAFT forward (``b2o_craft_forward``) and getBoxes (``b2o_get_boxes``).
 """
+import math
+import numbers
 import typing
 
 import numpy as np
@@ -16,6 +18,37 @@ PRETRAINED_WEIGHTS = {   # same files as reference detection.py:647-658
         "sha256": "4a5efbfb48b4081100544e75e1e2b57f8de3d84f213004b14b85fd4b3748db17",
     },
 }
+
+
+LINE_DEFAULTS = {"angle_tolerance": 15.0, "height_ratio": 0.5, "offset_ratio": 0.5, "gap_ratio": 1.5}
+
+
+def check_lines(**kw):
+    """Validate the text-line parameters (DESIGN.md section 1, "Text lines") and return all four as floats, defaults
+    filled in.  ``angle_tolerance`` in (0, 90] degrees, ``height_ratio`` in (0, 1], ``offset_ratio`` > 0,
+    ``gap_ratio`` >= 0; unknown keys and values that are not finite real numbers raise ``ValueError``."""
+    unknown = sorted(set(kw) - set(LINE_DEFAULTS))
+    if unknown:
+        raise ValueError(f"unknown line parameters {unknown}; expected some of {sorted(LINE_DEFAULTS)}")
+    out = dict(LINE_DEFAULTS)
+    for k, v in kw.items():
+        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(float(v)):
+            raise ValueError(f"{k} must be a finite number, got {v!r}")
+        out[k] = float(v)
+    if not 0 < out["angle_tolerance"] <= 90:
+        raise ValueError(f"angle_tolerance must be in (0, 90] degrees, got {out['angle_tolerance']}")
+    if not 0 < out["height_ratio"] <= 1:
+        raise ValueError(f"height_ratio must be in (0, 1], got {out['height_ratio']}")
+    if not out["offset_ratio"] > 0:
+        raise ValueError(f"offset_ratio must be > 0, got {out['offset_ratio']}")
+    if not out["gap_ratio"] >= 0:
+        raise ValueError(f"gap_ratio must be >= 0, got {out['gap_ratio']}")
+    return out
+
+
+def lines_from_csr(line_count, word_order, line_start, line_boxes):
+    """One image's rows of b2o_group_lines (host arrays) -> [(line_box (4,2) float32, word indices int32), ...]."""
+    return [(line_boxes[l].copy(), word_order[line_start[l]:line_start[l + 1]].copy()) for l in range(int(line_count))]
 
 
 def _as_device_images(images, device):
@@ -68,6 +101,7 @@ class Detector:
         self.max_boxes = 256
         self._ws = None                  # reusable CRAFT workspace (grown on demand)
         self._box_ws = None
+        self._line_ws = None
 
     # ------------------------------------------------------------------ device-resident API
     def predict_device(self, images_t):
@@ -161,6 +195,53 @@ class Detector:
         """getBoxes on the device.  Returns (boxes (N,M,4,2) float32 CUDA, counts ndarray (N,))."""
         return self.boxes_finish(self.boxes_enqueue(scores, detection_threshold, text_threshold, link_threshold,
                                                     size_threshold))
+
+    def group_lines_device(self, boxes, counts_dev, **line_kwargs):
+        """Text lines in reading order on the device (``b2o_group_lines``), queued on the current stream.
+        ``boxes`` (N,M,4,2) float32 CUDA and ``counts_dev`` (N,) int32 CUDA as ``boxes_enqueue`` makes them (box[0] ->
+        box[1] the reading direction); ``line_kwargs`` as ``check_lines`` takes them.  Returns (line_counts (N,),
+        word_order (N,M), line_start (N,M+1) int32, line_boxes (N,M,4,2) float32), all CUDA: the words of line l of
+        image i are ``word_order[i, line_start[i, l]:line_start[i, l + 1]]``, lines in page order.  Slots past an
+        image's word / line count are not written."""
+        p = check_lines(**line_kwargs)
+        n, m = int(boxes.shape[0]), int(boxes.shape[1])
+        assert boxes.is_cuda and boxes.dtype == torch.float32 and tuple(boxes.shape[2:]) == (4, 2)
+        assert counts_dev.is_cuda and counts_dev.dtype == torch.int32 and tuple(counts_dev.shape) == (n,)
+        boxes = boxes.contiguous()
+        dev = boxes.device
+        line_counts = torch.empty((n,), dtype=torch.int32, device=dev)
+        word_order = torch.empty((n, m), dtype=torch.int32, device=dev)
+        line_start = torch.empty((n, m + 1), dtype=torch.int32, device=dev)
+        line_boxes = torch.empty((n, m, 4, 2), dtype=torch.float32, device=dev)
+        if n == 0:
+            return line_counts, word_order, line_start, line_boxes
+        nbytes = self.ctx.lines_workspace_bytes(n, m)
+        if self._line_ws is None or self._line_ws.numel() < nbytes:
+            self._line_ws = None
+            self._line_ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        self.ctx.group_lines(boxes.data_ptr(), counts_dev.data_ptr(), n, m, math.cos(math.radians(p["angle_tolerance"])),
+                             p["height_ratio"], p["offset_ratio"], p["gap_ratio"], line_counts.data_ptr(),
+                             word_order.data_ptr(), line_start.data_ptr(), line_boxes.data_ptr(),
+                             self._line_ws.data_ptr(), nbytes, torch.cuda.current_stream(dev).cuda_stream)
+        return line_counts, word_order, line_start, line_boxes
+
+    def group_lines(self, box_groups, **line_kwargs):
+        """Text lines of host box groups, as ``detect`` returns them (``np.array([])`` for an image without boxes) or
+        from any other detector: per image a list of (line_box (4,2) float32, word_indices int32) in reading order,
+        the indices into that image's boxes.  box[0] -> box[1] of every box must be its reading direction."""
+        check_lines(**line_kwargs)
+        groups = [np.asarray(g, np.float32).reshape(-1, 4, 2) for g in box_groups]
+        if not groups:
+            return []
+        counts = np.array([len(g) for g in groups], np.int32)
+        m = max(1, int(counts.max()))
+        table = np.zeros((len(groups), m, 4, 2), np.float32)
+        for i, g in enumerate(groups):
+            table[i, :len(g)] = g
+        out = self.group_lines_device(torch.from_numpy(table).to(self.device), torch.from_numpy(counts).to(self.device),
+                                      **line_kwargs)
+        lc, wo, ls, lb = (t.cpu().numpy() for t in out)
+        return [lines_from_csr(lc[i], wo[i], ls[i], lb[i]) for i in range(len(groups))]
 
     def detect_device(self, images_t, **thresholds):
         return self.boxes_device(self.predict_device(images_t), **thresholds)

@@ -136,7 +136,7 @@ class Pipeline:
         st[key] = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
         st[key].copy_(t, non_blocking=True)
 
-    def _stage_recognize(self, st, beam, char_boxes=False):
+    def _stage_recognize(self, st, beam, char_boxes=False, lines=None):
         det, rec = self.detector, self.recognizer
         bst = st.pop("boxes_state")
         boxes, counts = det.boxes_finish(bst)
@@ -157,6 +157,11 @@ class Pipeline:
             labels, logp = labels
             self._to_host(st, "box_scores_host", box_scores)
         st["counts"] = counts
+        line_tables = ()
+        if lines is not None:                            # grouped on the boxes as returned: rolled under rotations
+            line_tables = det.group_lines_device(boxes, bst["counts"], **lines)
+            for key, t in zip(("line_counts_host", "word_order_host", "line_start_host", "line_boxes_host"), line_tables):
+                self._to_host(st, key, t)
         self._to_host(st, "boxes_host", boxes)
         if polys is not None:
             self._to_host(st, "polys_host", bst["polys"])
@@ -169,7 +174,7 @@ class Pipeline:
             st["char_boxes"] = True
             if cells is not None:
                 self._to_host(st, "cells_host", cells)
-        st["keep"] = (boxes, labels, box_scores, logp, cells, polys)   # alive until the copies have run
+        st["keep"] = (boxes, labels, box_scores, logp, cells, polys) + tuple(line_tables)   # alive until the copies ran
         st["done"] = torch.cuda.Event()
         st["done"].record(torch.cuda.current_stream(det.device))
 
@@ -199,6 +204,10 @@ class Pipeline:
             cells_host = st["cells_host"].numpy()
             d2h += cells_host.nbytes
             cells = recognition.char_boxes_host(cells_host, texts)
+        lines = None
+        if "line_counts_host" in st:
+            lines = [st[k].numpy() for k in ("line_counts_host", "word_order_host", "line_start_host", "line_boxes_host")]
+            d2h += sum(a.nbytes for a in lines)
         self.last_stats["d2h_bytes"] += int(d2h)
         out, start = [], 0
         for i, (c, scale) in enumerate(zip(counts, st["scales"])):
@@ -218,12 +227,26 @@ class Pipeline:
                 words = [w + (tools.adjust_boxes(boxes=polys[i, k, :points[i, k]].copy(), boxes_format="boxes",
                                                  scale=1 / scale),)
                          for k, w in enumerate(words)]
+            if lines is not None:
+                words = self._lines(words, detection.lines_from_csr(*(a[i] for a in lines)), scale)
             out.append(words)
             start += c
         return out
 
+    @staticmethod
+    def _lines(words, lines, scale):
+        """One image's word tuples regrouped as (text, box, words) lines, the box scaled as the word boxes are."""
+        out = []
+        for box, idx in lines:
+            members = [words[k] for k in idx]
+            text = " ".join(w[0][0] if isinstance(w[0], list) else w[0] for w in members)
+            if scale != 1:
+                box = tools.adjust_boxes(boxes=box, boxes_format="boxes", scale=1 / scale)
+            out.append((text, box, members))
+        return out
+
     def recognize(self, images, detection_kwargs=None, recognition_kwargs=None, return_scores=False,
-                  return_char_boxes=False, return_polygons=False):
+                  return_char_boxes=False, return_polygons=False, return_lines=False, line_kwargs=None):
         """Run the pipeline on one or multiple images (reference pipeline.py:28-75).
 
         Returns a list (one entry per image) of lists of (text, box) tuples, boxes (4,2) float32 in
@@ -248,9 +271,16 @@ class Pipeline:
         polygon, a (p,2) float32 array in the input image's pixels: (text, box, polygon), or (text, box,
         detection_score, confidence, polygon) with ``return_scores``.  It combines with ``beam_width`` / ``top_paths`` /
         ``lexicon`` and ``inflight``; with ``rotations`` or ``return_char_boxes`` it raises ``ValueError``.
+        ``return_lines=True``: every image is a list of text lines in reading order instead, each ``(text, box,
+        words)``: ``words`` the word tuples this call returns without ``return_lines`` (with whatever the other options
+        add), in reading order; ``text`` their texts joined by single spaces (each word's best reading with
+        ``top_paths > 1``); ``box`` the line's (4,2) float32 box in the input image's pixels, box[0] -> box[1] its
+        reading direction.  The words are grouped on the device (``Detector.group_lines_device``) from their boxes --
+        after ``rotations`` has rolled them, never from polygons -- with ``line_kwargs`` (``detection.check_lines``).
         """
         if return_polygons and (return_char_boxes or (recognition_kwargs or {}).get("rotations") is not None):
             raise ValueError("return_polygons does not combine with rotations or return_char_boxes")
+        lines = detection.check_lines(**(line_kwargs or {})) if return_lines or line_kwargs is not None else None
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
                 images = [tools.read_device(image, self.detector.ctx, self.detector.device) for image in images]
@@ -279,6 +309,9 @@ class Pipeline:
             if return_polygons:
                 raise NotImplementedError("return_polygons=True needs this package's Detector and Recognizer; "
                                           "injected detectors / recognizers do not report polygons")
+            if return_lines:
+                raise NotImplementedError("return_lines=True needs this package's Detector and Recognizer; injected "
+                                          "detectors / recognizers are grouped with Detector.group_lines")
             return self._recognize_generic(images, detection_kwargs, recognition_kwargs)
         thresholds = {k: detection_kwargs[k] for k in ("detection_threshold", "text_threshold", "link_threshold",
                                                         "size_threshold") if k in detection_kwargs}
@@ -296,7 +329,8 @@ class Pipeline:
                 states.append(self._stage_detect(images[bounds[step]:bounds[step + 1]], pad_to, thresholds,
                                                  with_scores=return_scores, with_polygons=return_polygons))
             if 1 <= step <= k:
-                self._stage_recognize(states[step - 1], beam, char_boxes=return_char_boxes)
+                self._stage_recognize(states[step - 1], beam, char_boxes=return_char_boxes,
+                                      lines=lines if return_lines else None)
             if step >= 2:
                 out.extend(self._stage_finish(states[step - 2]))
                 states[step - 2] = None
