@@ -200,6 +200,25 @@ int b2o_group_lines(b2o_ctx* ctx, const float* boxes_dev, const int32_t* counts_
                     int32_t* line_counts_dev, int32_t* word_order_dev, int32_t* line_start_dev,
                     float* line_boxes_dev, void* ws_dev, size_t ws_bytes, void* stream);
 
+/* Text blocks in reading order (DESIGN.md section 1, "Text blocks"): recursive XY-cut over the lines of each image.
+ * Inputs are b2o_group_lines' outputs (or any lines in that layout): L_i = min(line_counts[i], max_boxes) lines of
+ * image i, line l's word count line_start[i, l + 1] - line_start[i, l] (line_start nondecreasing) and its (4, 2) box
+ * line_boxes[i, l] (finite corners); only those are read.  The page frame D is box[1] - box[0] of the line with the
+ * most words; a node of lines is cut into rows wherever the gap along N between a line and the running max of those
+ * before it reaches row_gap * s, else into columns along D with col_gap * s (s the lower median of the lines'
+ * heights), recursively; a node that cuts neither way is a block.  Outputs, a CSR table per image: block_counts[i] =
+ * B_i blocks in depth-first order; the lines of block b in ascending line index are
+ * line_order[i, block_start[i, b] : block_start[i, b + 1]]; block_boxes[i, b] the block's (4, 2) box aligned to D,
+ * box[0] -> box[1] the page's reading direction.  Written: block_counts (n) all, line_order[i, :L_i],
+ * block_start[i, :B_i + 1], block_boxes[i, :B_i]; every other slot is left as it was.  line_order is (n, max_boxes),
+ * block_start (n, max_boxes + 1), block_boxes (n, max_boxes, 4, 2).  row_gap and col_gap must be finite and > 0.
+ * Every value is fp64 with a fixed operation order: bit-identical in any batch and on every run.  n = 0 does nothing. */
+size_t b2o_blocks_workspace_bytes(int n, int max_boxes);
+int b2o_group_blocks(b2o_ctx* ctx, const int32_t* line_counts_dev, const int32_t* line_start_dev,
+                     const float* line_boxes_dev, int n, int max_boxes, double row_gap, double col_gap,
+                     int32_t* block_counts_dev, int32_t* line_order_dev, int32_t* block_start_dev,
+                     float* block_boxes_dev, void* ws_dev, size_t ws_bytes, void* stream);
+
 /* tools.warpBox over box groups (recognition.py:506-519; tools.py:61-117).  boxes: (n_boxes,4,2)
  * float32; image_index[k] selects the gray image of box k.  crops: (n_boxes,31,200) uint8
  * (exactly warpBox's output) and, when crnn_in != NULL, the CRNN input (n_boxes,200,31) fp16 =

@@ -94,6 +94,8 @@ SIGNATURES = {
     "b2o_lines_workspace_bytes": (_sz, [_i, _i]),
     "b2o_group_lines": (_i, [_vp, _vp, _vp, _i, _i, _c.c_double, _c.c_double, _c.c_double, _c.c_double, _vp, _vp, _vp,
                              _vp, _vp, _sz, _vp]),
+    "b2o_blocks_workspace_bytes": (_sz, [_i, _i]),
+    "b2o_group_blocks": (_i, [_vp, _vp, _vp, _vp, _i, _i, _c.c_double, _c.c_double, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2o_record_floats": (_sz, [_i]),
     "b2o_record_floats_scored": (_sz, [_i]),
     "b2o_pack_records": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
@@ -323,6 +325,15 @@ class Context:
                                              float(height_ratio), float(offset_ratio), float(gap_ratio), line_counts,
                                              word_order, line_start, line_boxes, ws, ws_bytes, stream),
                     "b2o_group_lines")
+
+    def blocks_workspace_bytes(self, n, max_boxes):
+        return int(self.lib.b2o_blocks_workspace_bytes(n, max_boxes))
+
+    def group_blocks(self, line_counts, line_start, line_boxes, n, max_boxes, row_gap, col_gap, block_counts,
+                     line_order, block_start, block_boxes, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_group_blocks(self.handle, line_counts, line_start, line_boxes, n, max_boxes,
+                                              float(row_gap), float(col_gap), block_counts, line_order, block_start,
+                                              block_boxes, ws, ws_bytes, stream), "b2o_group_blocks")
 
     def record_floats(self, rec_boxes):
         return int(self.lib.b2o_record_floats(rec_boxes))

@@ -192,6 +192,82 @@ static __device__ __forceinline__ void uf_unite(int* L, int a, int b) {
   }
 }
 
+// ---- one-CTA sorts and scans on total-order keys (lines.cu's text lines, blocks.cu's text blocks) ----------------
+struct SortKey {                     // lexicographic (a, b, c); p travels with the key
+  unsigned long long a, b;
+  unsigned c, p;
+};
+
+static __device__ __forceinline__ bool key_less(const SortKey& x, const SortKey& y) {
+  if (x.a != y.a) return x.a < y.a;
+  if (x.b != y.b) return x.b < y.b;
+  return x.c < y.c;
+}
+
+// order-preserving map of a double onto uint64; -0.0 and +0.0 map to the same key (an exact tie)
+static __device__ __forceinline__ unsigned long long dkey(double x) {
+  if (x == 0.0) x = 0.0;
+  const unsigned long long b = static_cast<unsigned long long>(__double_as_longlong(x));
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+
+// a . b = a.x b.x + a.y b.y in fp64, in that order, without contraction
+static __device__ __forceinline__ double dot2(double ax, double ay, double bx, double by) {
+  return __dadd_rn(__dmul_rn(ax, bx), __dmul_rn(ay, by));
+}
+
+// exclusive block-wide scan of v; returns the prefix and leaves the block total in *total (smem scratch: 32 ints + 1)
+static __device__ int block_exclusive_scan(int v, int* scratch, int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  int x = v;
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) scratch[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    int s = lane < nw ? scratch[lane] : 0;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += y;
+    }
+    if (lane < nw) scratch[lane] = s;
+    if (lane == nw - 1) scratch[32] = s;
+  }
+  __syncthreads();
+  const int r = x - v + (warp ? scratch[warp - 1] : 0);
+  *total = scratch[32];
+  __syncthreads();
+  return r;
+}
+
+// ascending bitonic sort of keys[0, p) (p a power of two) by the whole CTA, in global memory
+static __device__ void block_sort(SortKey* keys, int p) {
+  for (int k = 2; k <= p; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int t = threadIdx.x; t < (p >> 1); t += blockDim.x) {
+        const int lo = 2 * t - (t & (j - 1));          // index whose bit j is clear
+        const int hi = lo + j;
+        const bool up = (lo & k) == 0;
+        const SortKey x = keys[lo], y = keys[hi];
+        if (key_less(y, x) == up) { keys[lo] = y; keys[hi] = x; }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// keys[from, p) = the largest key, so that padding sorts last
+static __device__ __forceinline__ void pad_keys(SortKey* keys, int from, int p) {
+  for (int t = from + threadIdx.x; t < p; t += blockDim.x) {
+    SortKey s;
+    s.a = s.b = ~0ull;
+    s.c = s.p = ~0u;
+    keys[t] = s;
+  }
+}
+
 // ---- box corner order (image.cu's warp, rotation.cu's box roll, ctc_align.cu's cells) ------------
 // fp64 Euclidean distance of two float32 points, as scipy's cdist computes it (tools.py:41-57)
 static __device__ inline double corner_dist(const float* a, const float* b) {

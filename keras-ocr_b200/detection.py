@@ -51,6 +51,32 @@ def lines_from_csr(line_count, word_order, line_start, line_boxes):
     return [(line_boxes[l].copy(), word_order[line_start[l]:line_start[l + 1]].copy()) for l in range(int(line_count))]
 
 
+BLOCK_DEFAULTS = {"row_gap": 1.5, "col_gap": 1.0}
+
+
+def check_blocks(**kw):
+    """Validate the text-block parameters (DESIGN.md section 1, "Text blocks") and return both as floats, defaults
+    filled in.  ``row_gap`` and ``col_gap`` > 0, in units of the median line height; unknown keys and values that are
+    not finite real numbers raise ``ValueError``."""
+    unknown = sorted(set(kw) - set(BLOCK_DEFAULTS))
+    if unknown:
+        raise ValueError(f"unknown block parameters {unknown}; expected some of {sorted(BLOCK_DEFAULTS)}")
+    out = dict(BLOCK_DEFAULTS)
+    for k, v in kw.items():
+        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(float(v)):
+            raise ValueError(f"{k} must be a finite number, got {v!r}")
+        if not float(v) > 0:
+            raise ValueError(f"{k} must be > 0, got {v!r}")
+        out[k] = float(v)
+    return out
+
+
+def blocks_from_csr(block_count, line_order, block_start, block_boxes):
+    """One image's rows of b2o_group_blocks (host arrays) -> [(block_box (4,2) float32, line indices int32), ...]."""
+    return [(block_boxes[b].copy(), line_order[block_start[b]:block_start[b + 1]].copy())
+            for b in range(int(block_count))]
+
+
 def _as_device_images(images, device):
     """list / ndarray / tensor of HxWx3 uint8 -> (N,H,W,3) uint8 CUDA tensor."""
     if isinstance(images, torch.Tensor):
@@ -102,6 +128,7 @@ class Detector:
         self._ws = None                  # reusable CRAFT workspace (grown on demand)
         self._box_ws = None
         self._line_ws = None
+        self._block_ws = None
 
     # ------------------------------------------------------------------ device-resident API
     def predict_device(self, images_t):
@@ -242,6 +269,59 @@ class Detector:
                                       **line_kwargs)
         lc, wo, ls, lb = (t.cpu().numpy() for t in out)
         return [lines_from_csr(lc[i], wo[i], ls[i], lb[i]) for i in range(len(groups))]
+
+    def group_blocks_device(self, line_counts, line_start, line_boxes, **block_kwargs):
+        """Text blocks in reading order on the device (``b2o_group_blocks``), queued on the current stream: recursive
+        XY-cut over the lines ``group_lines_device`` returns (``line_counts`` (N,), ``line_start`` (N,M+1) int32,
+        ``line_boxes`` (N,M,4,2) float32, all CUDA); ``block_kwargs`` as ``check_blocks`` takes them.  Returns
+        (block_counts (N,), line_order (N,M), block_start (N,M+1) int32, block_boxes (N,M,4,2) float32), all CUDA: the
+        lines of block b of image i, in page order, are ``line_order[i, block_start[i, b]:block_start[i, b + 1]]``,
+        blocks in reading order.  Slots past an image's line / block count are not written."""
+        p = check_blocks(**block_kwargs)
+        n, m = int(line_boxes.shape[0]), int(line_boxes.shape[1])
+        assert line_boxes.is_cuda and line_boxes.dtype == torch.float32 and tuple(line_boxes.shape[2:]) == (4, 2)
+        assert line_counts.is_cuda and line_counts.dtype == torch.int32 and tuple(line_counts.shape) == (n,)
+        assert line_start.is_cuda and line_start.dtype == torch.int32 and tuple(line_start.shape) == (n, m + 1)
+        line_counts, line_start, line_boxes = line_counts.contiguous(), line_start.contiguous(), line_boxes.contiguous()
+        dev = line_boxes.device
+        block_counts = torch.empty((n,), dtype=torch.int32, device=dev)
+        line_order = torch.empty((n, m), dtype=torch.int32, device=dev)
+        block_start = torch.empty((n, m + 1), dtype=torch.int32, device=dev)
+        block_boxes = torch.empty((n, m, 4, 2), dtype=torch.float32, device=dev)
+        if n == 0:
+            return block_counts, line_order, block_start, block_boxes
+        nbytes = self.ctx.blocks_workspace_bytes(n, m)
+        if self._block_ws is None or self._block_ws.numel() < nbytes:
+            self._block_ws = None
+            self._block_ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        self.ctx.group_blocks(line_counts.data_ptr(), line_start.data_ptr(), line_boxes.data_ptr(), n, m, p["row_gap"],
+                              p["col_gap"], block_counts.data_ptr(), line_order.data_ptr(), block_start.data_ptr(),
+                              block_boxes.data_ptr(), self._block_ws.data_ptr(), nbytes,
+                              torch.cuda.current_stream(dev).cuda_stream)
+        return block_counts, line_order, block_start, block_boxes
+
+    def group_blocks(self, line_groups, **block_kwargs):
+        """Text blocks of host lines, as ``group_lines`` returns them (per image a list of (line_box (4,2),
+        word_indices)) or from any other source in page order: per image a list of (block_box (4,2) float32,
+        line_indices int32) in reading order, the indices into that image's lines.  box[0] -> box[1] of every line box
+        must be its reading direction."""
+        check_blocks(**block_kwargs)
+        if not line_groups:
+            return []
+        n = len(line_groups)
+        counts = np.array([len(g) for g in line_groups], np.int32)
+        m = max(1, int(counts.max()))
+        boxes = np.zeros((n, m, 4, 2), np.float32)
+        starts = np.zeros((n, m + 1), np.int32)
+        for i, g in enumerate(line_groups):
+            if len(g):
+                boxes[i, :len(g)] = np.stack([np.asarray(b, np.float32).reshape(4, 2) for b, _ in g])
+                starts[i, 1:len(g) + 1] = np.cumsum([len(w) for _, w in g])
+        dev = self.device
+        out = self.group_blocks_device(torch.from_numpy(counts).to(dev), torch.from_numpy(starts).to(dev),
+                                       torch.from_numpy(boxes).to(dev), **block_kwargs)
+        bc, lo, bs, bb = (t.cpu().numpy() for t in out)
+        return [blocks_from_csr(bc[i], lo[i], bs[i], bb[i]) for i in range(n)]
 
     def detect_device(self, images_t, **thresholds):
         return self.boxes_device(self.predict_device(images_t), **thresholds)

@@ -70,6 +70,8 @@ def unpack_blocks(blocks, max_boxes, strict=True, scores=False):
     float32, labels (total,48) int8) with the words of image i at [sum(counts[:i]), +counts[i]).  Only the used
     prefix of every record is touched (two concatenations of per-image views), not the 75 % padding.
     ``scores=True`` reads the scored layout and also returns (box_scores (total,), logp (total,)) float32.
+    "Blocks" here are the gathered record blocks of the ranks, unrelated to the text blocks of
+    ``Pipeline.recognize(return_blocks=True)``.
 
     A record's count field is the number of words its image HAS; a record holds ``max_boxes`` of them.  The
     single-GPU ``Pipeline.recognize`` grows its box table on demand (as the reference returns every box), so a

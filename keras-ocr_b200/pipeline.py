@@ -136,7 +136,7 @@ class Pipeline:
         st[key] = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
         st[key].copy_(t, non_blocking=True)
 
-    def _stage_recognize(self, st, beam, char_boxes=False, lines=None):
+    def _stage_recognize(self, st, beam, char_boxes=False, lines=None, blocks=None):
         det, rec = self.detector, self.recognizer
         bst = st.pop("boxes_state")
         boxes, counts = det.boxes_finish(bst)
@@ -160,7 +160,12 @@ class Pipeline:
         line_tables = ()
         if lines is not None:                            # grouped on the boxes as returned: rolled under rotations
             line_tables = det.group_lines_device(boxes, bst["counts"], **lines)
-            for key, t in zip(("line_counts_host", "word_order_host", "line_start_host", "line_boxes_host"), line_tables):
+            if blocks is not None:                       # cut on the device tables, copied back with them
+                lc, _, ls, lb = line_tables
+                line_tables = line_tables + det.group_blocks_device(lc, ls, lb, **blocks)
+            for key, t in zip(("line_counts_host", "word_order_host", "line_start_host", "line_boxes_host",
+                               "block_counts_host", "line_order_host", "block_start_host", "block_boxes_host"),
+                              line_tables):
                 self._to_host(st, key, t)
         self._to_host(st, "boxes_host", boxes)
         if polys is not None:
@@ -208,6 +213,11 @@ class Pipeline:
         if "line_counts_host" in st:
             lines = [st[k].numpy() for k in ("line_counts_host", "word_order_host", "line_start_host", "line_boxes_host")]
             d2h += sum(a.nbytes for a in lines)
+        blocks = None
+        if "block_counts_host" in st:
+            blocks = [st[k].numpy() for k in ("block_counts_host", "line_order_host", "block_start_host",
+                                              "block_boxes_host")]
+            d2h += sum(a.nbytes for a in blocks)
         self.last_stats["d2h_bytes"] += int(d2h)
         out, start = [], 0
         for i, (c, scale) in enumerate(zip(counts, st["scales"])):
@@ -229,6 +239,8 @@ class Pipeline:
                          for k, w in enumerate(words)]
             if lines is not None:
                 words = self._lines(words, detection.lines_from_csr(*(a[i] for a in lines)), scale)
+            if blocks is not None:
+                words = self._blocks(words, detection.blocks_from_csr(*(a[i] for a in blocks)), scale)
             out.append(words)
             start += c
         return out
@@ -245,8 +257,20 @@ class Pipeline:
             out.append((text, box, members))
         return out
 
+    @staticmethod
+    def _blocks(lines, blocks, scale):
+        """One image's line tuples regrouped as (text, box, lines) blocks, the box scaled as the line boxes are."""
+        out = []
+        for box, idx in blocks:
+            members = [lines[k] for k in idx]
+            if scale != 1:
+                box = tools.adjust_boxes(boxes=box, boxes_format="boxes", scale=1 / scale)
+            out.append(("\n".join(l[0] for l in members), box, members))
+        return out
+
     def recognize(self, images, detection_kwargs=None, recognition_kwargs=None, return_scores=False,
-                  return_char_boxes=False, return_polygons=False, return_lines=False, line_kwargs=None):
+                  return_char_boxes=False, return_polygons=False, return_lines=False, line_kwargs=None,
+                  return_blocks=False, block_kwargs=None):
         """Run the pipeline on one or multiple images (reference pipeline.py:28-75).
 
         Returns a list (one entry per image) of lists of (text, box) tuples, boxes (4,2) float32 in
@@ -277,10 +301,19 @@ class Pipeline:
         ``top_paths > 1``); ``box`` the line's (4,2) float32 box in the input image's pixels, box[0] -> box[1] its
         reading direction.  The words are grouped on the device (``Detector.group_lines_device``) from their boxes --
         after ``rotations`` has rolled them, never from polygons -- with ``line_kwargs`` (``detection.check_lines``).
+        ``return_blocks=True``: every image is a list of text blocks in reading order instead, each ``(text, box,
+        lines)``: ``lines`` the ``(text, box, words)`` tuples ``return_lines=True`` returns for the same call and
+        ``line_kwargs``, split among the blocks, in page order inside each; ``text`` their texts joined by newlines;
+        ``box`` the block's (4,2) float32 box in the input image's pixels, aligned to the page's reading direction.
+        The lines are cut into blocks on the device (``Detector.group_blocks_device``, recursive XY-cut: rows first,
+        then columns) with ``block_kwargs`` (``detection.check_blocks``).  It implies ``return_lines``.
         """
         if return_polygons and (return_char_boxes or (recognition_kwargs or {}).get("rotations") is not None):
             raise ValueError("return_polygons does not combine with rotations or return_char_boxes")
         lines = detection.check_lines(**(line_kwargs or {})) if return_lines or line_kwargs is not None else None
+        blocks = detection.check_blocks(**(block_kwargs or {})) if return_blocks or block_kwargs is not None else None
+        if return_blocks and lines is None:
+            lines = detection.check_lines()
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
                 images = [tools.read_device(image, self.detector.ctx, self.detector.device) for image in images]
@@ -312,6 +345,10 @@ class Pipeline:
             if return_lines:
                 raise NotImplementedError("return_lines=True needs this package's Detector and Recognizer; injected "
                                           "detectors / recognizers are grouped with Detector.group_lines")
+            if return_blocks:
+                raise NotImplementedError("return_blocks=True needs this package's Detector and Recognizer; injected "
+                                          "detectors / recognizers are grouped with Detector.group_lines and "
+                                          "Detector.group_blocks")
             return self._recognize_generic(images, detection_kwargs, recognition_kwargs)
         thresholds = {k: detection_kwargs[k] for k in ("detection_threshold", "text_threshold", "link_threshold",
                                                         "size_threshold") if k in detection_kwargs}
@@ -330,7 +367,8 @@ class Pipeline:
                                                  with_scores=return_scores, with_polygons=return_polygons))
             if 1 <= step <= k:
                 self._stage_recognize(states[step - 1], beam, char_boxes=return_char_boxes,
-                                      lines=lines if return_lines else None)
+                                      lines=lines if return_lines or return_blocks else None,
+                                      blocks=blocks if return_blocks else None)
             if step >= 2:
                 out.extend(self._stage_finish(states[step - 2]))
                 states[step - 2] = None

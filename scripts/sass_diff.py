@@ -1,5 +1,6 @@
 """Compare the SASS of every conv_tc_kernel instance between two object files (addresses stripped): used to show that
-adding opt-in kernel variants left the GPU-validated default instances bit-identical.
+adding opt-in kernel variants left the GPU-validated default instances bit-identical, or that moving shared helpers
+into common.cuh left a file's kernels unchanged (any object file; kernels in an anonymous namespace match by name).
 
     python scripts/sass_diff.py old_conv_tc.o keras-ocr_b200/csrc/conv_tc.o [suffix-to-append-to-old-template-args]
 
@@ -18,7 +19,7 @@ def functions(path):
     for line in out.splitlines():
         m = re.search(r"Function : (\S+)", line)
         if m:
-            full = m.group(1)
+            full = re.sub(r"_GLOBAL__N__[0-9a-f]+_", "_GLOBAL__N__", m.group(1))   # anonymous namespace: per-build hash
             name = full[full.index("kernelI"):] if "kernelI" in full else full
             table[name] = []
             continue
