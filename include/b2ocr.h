@@ -219,6 +219,58 @@ int b2o_group_blocks(b2o_ctx* ctx, const int32_t* line_counts_dev, const int32_t
                      int32_t* block_counts_dev, int32_t* line_order_dev, int32_t* block_start_dev,
                      float* block_boxes_dev, void* ws_dev, size_t ws_bytes, void* stream);
 
+/* Wide words (DESIGN.md section 1, "Wide words"): a box wider than the 200 x 31 crop at full height is read in up to
+ * M = max_windows overlapping windows (1 <= M <= B2O_MAX_WINDOWS).  In warp_extent's turn-0 frame of the box (w, h
+ * from get_rotated_width_height): scale = min(T / w, 31 / h), T = 200 + (M - 1) S, S = B2O_WINDOW_STRIDE; wc = scale w,
+ * sh = scale h.  A word with wc <= 200 has K = 1 and reads as b2o_warp_boxes reads it; otherwise K = 1 + ceil((wc - 200)
+ * / S), at most M, windows start at a_k = k S (k < K - 1) and a_{K-1} = wc - 200, and window k is the homography of
+ * the ordered box onto (-a_k, 0), (wc - a_k, 0), (wc - a_k, sh), (-a_k, sh) (float32 corners), dsize (200, int(sh)).
+ * A box where warpBox raises ZeroDivisionError has K = 1.
+ *
+ * b2o_window_counts: K of every box of a table, boxes_dev (n, max_boxes, 4, 2), windows_dev (n, max_boxes) int32;
+ * counts_dev (n) int32 limits image i to its first counts[i] boxes (NULL: every slot); slots past it are not written.
+ *
+ * The wide words are then listed as words_dev (n_words) int32, indices into a dense box list boxes_dev (., 4, 2) with
+ * image_index_dev, and a CSR win_start_dev (n_words + 1) int32 of their windows: word i owns windows win_start[i] ..
+ * win_start[i+1] - 1, whose count must be its K.  b2o_warp_windows cuts windows first .. first + count - 1 into slots
+ * 0 .. count - 1 of crops_dev (count, 31, 200[, 3]) uint8 and / or crnn_in_dev (count, 200, 31[, 3]) fp16, as
+ * b2o_warp_boxes lays them out (channels 1: gray image, 3: RGB for a color recognizer).
+ *
+ * b2o_stitch_windows reads every window's fc_12 logits, logits_dev (win_start[n_words], 48, k) float32, and its STN
+ * theta, theta_dev (win_start[n_words], 6) float32 (NULL: no STN), and writes word i's reading to row words[i] of
+ * labels_dev (., 48 M) int32, -1 padded, and its log-probability S to logp_dev[words[i]] (NULL: not written); no other
+ * row is written.  Step t of window k lies at P = a_k + x in the word, x = stn_crop_x of grid row t + 2 (the map of
+ * b2o_char_cells) clamped to [0, 200] and made non-decreasing.  The cut between windows k and k+1 is the position p
+ * of a step of window k+1 inside the overlap [a_{k+1}, a_k + 200] shrunk by B2O_WINDOW_SHRINK at each end, nearest to
+ * the overlap's centre (lower step on a tie), where that step and window k's step nearest to p (lower step on a tie)
+ * both emit the blank; without such a step, the centre; a cut below the previous cut is raised to it.  Window k keeps
+ * the steps with cut_{k-1} <= P < cut_k in order; greedy CTC (first maximum, merge repeats, drop blanks) over all kept
+ * steps gives the labels, and S is the sum
+ * over them of log(max p + 1e-7), max p = 1 / sum_c exp(l_c - l_max) summed in ascending c.
+ *
+ * b2o_window_plan_test (test hook): the plan of every window slot, plans_dev (n, M): record k of box i is window k's
+ * plan, m the inverse homography, dw, dh the dsize (for K = 1, warpBox's), a = a_k; k = the box's K in every record,
+ * valid = 0 for slots k >= K and where the system is singular (b2o_warp_windows cuts an all-zero crop there).      */
+#define B2O_MAX_WINDOWS 16
+#define B2O_WINDOW_STRIDE 136
+#define B2O_WINDOW_SHRINK 8
+typedef struct {
+  double m[9];
+  double a, wc, sh;
+  int32_t k, dw, dh, valid;
+} b2o_window_plan;
+int b2o_window_counts(b2o_ctx* ctx, const float* boxes_dev, const int32_t* counts_dev, int n, int max_boxes,
+                      int max_windows, int32_t* windows_dev, void* stream);
+int b2o_warp_windows(b2o_ctx* ctx, const uint8_t* img_dev, int channels, int n, int h, int w, const float* boxes_dev,
+                     const int32_t* image_index_dev, const int32_t* words_dev, const int32_t* win_start_dev,
+                     int n_words, int max_windows, int first, int count, uint8_t* crops_dev, void* crnn_in_dev,
+                     void* stream);
+int b2o_stitch_windows(b2o_ctx* ctx, const float* logits_dev, int k, const float* theta_dev, const float* boxes_dev,
+                       const int32_t* words_dev, const int32_t* win_start_dev, int n_words, int max_windows,
+                       int32_t* labels_dev, float* logp_dev, void* stream);
+int b2o_window_plan_test(b2o_ctx* ctx, const float* boxes_dev, int n, int max_windows, b2o_window_plan* plans_dev,
+                         void* stream);
+
 /* tools.warpBox over box groups (recognition.py:506-519; tools.py:61-117).  boxes: (n_boxes,4,2)
  * float32; image_index[k] selects the gray image of box k.  crops: (n_boxes,31,200) uint8
  * (exactly warpBox's output) and, when crnn_in != NULL, the CRNN input (n_boxes,200,31) fp16 =

@@ -23,6 +23,9 @@ MAX_ALIGN_PATHS = 128         # B2O_MAX_ALIGN_PATHS
 CRAFT_LAST_STEP = 30          # B2O_CRAFT_LAST_STEP
 MAX_POLY_SEGMENTS = 8         # B2O_MAX_POLY_SEGMENTS
 POLY_POINTS = 2 * (MAX_POLY_SEGMENTS + 1)   # points per entry of a dense polygon table
+MAX_WINDOWS = 16              # B2O_MAX_WINDOWS
+WINDOW_STRIDE = 136           # B2O_WINDOW_STRIDE
+WINDOW_SHRINK = 8             # B2O_WINDOW_SHRINK
 
 
 class B2OError(RuntimeError):
@@ -96,6 +99,10 @@ SIGNATURES = {
                              _vp, _vp, _sz, _vp]),
     "b2o_blocks_workspace_bytes": (_sz, [_i, _i]),
     "b2o_group_blocks": (_i, [_vp, _vp, _vp, _vp, _i, _i, _c.c_double, _c.c_double, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_window_counts": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "b2o_warp_windows": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "b2o_stitch_windows": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "b2o_window_plan_test": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     "b2o_record_floats": (_sz, [_i]),
     "b2o_record_floats_scored": (_sz, [_i]),
     "b2o_pack_records": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
@@ -142,6 +149,10 @@ SIGNATURES = {
 
 # b2o_warp_plan (include/b2ocr.h), field for field: 9 float64, 3 int32, padded to 88 bytes
 WARP_PLAN_DTYPE = np.dtype([("m", "<f8", (9,)), ("dw", "<i4"), ("dh", "<i4"), ("valid", "<i4")], align=True)
+
+# b2o_window_plan (include/b2ocr.h), field for field: 12 float64, 4 int32 (112 bytes)
+WINDOW_PLAN_DTYPE = np.dtype([("m", "<f8", (9,)), ("a", "<f8"), ("wc", "<f8"), ("sh", "<f8"), ("k", "<i4"),
+                              ("dw", "<i4"), ("dh", "<i4"), ("valid", "<i4")], align=True)
 
 _lib = None
 
@@ -334,6 +345,25 @@ class Context:
         self._check(self.lib.b2o_group_blocks(self.handle, line_counts, line_start, line_boxes, n, max_boxes,
                                               float(row_gap), float(col_gap), block_counts, line_order, block_start,
                                               block_boxes, ws, ws_bytes, stream), "b2o_group_blocks")
+
+    def window_counts(self, boxes, counts, n, max_boxes, max_windows, windows, stream):
+        self._check(self.lib.b2o_window_counts(self.handle, boxes, counts, n, max_boxes, max_windows, windows, stream),
+                    "b2o_window_counts")
+
+    def warp_windows(self, img, channels, n, h, w, boxes, image_index, words, win_start, n_words, max_windows, first,
+                     count, crops, crnn_in, stream):
+        self._check(self.lib.b2o_warp_windows(self.handle, img, channels, n, h, w, boxes, image_index, words, win_start,
+                                              n_words, max_windows, first, count, crops, crnn_in, stream),
+                    "b2o_warp_windows")
+
+    def stitch_windows(self, logits, k, theta, boxes, words, win_start, n_words, max_windows, labels, logp, stream):
+        self._check(self.lib.b2o_stitch_windows(self.handle, logits, k, theta, boxes, words, win_start, n_words,
+                                                max_windows, labels, logp, stream), "b2o_stitch_windows")
+
+    def window_plan_test(self, boxes, n, max_windows, plans, stream):
+        """b2o_window_plan_test: ``plans`` addresses n * max_windows records of WINDOW_PLAN_DTYPE on the device."""
+        self._check(self.lib.b2o_window_plan_test(self.handle, boxes, n, max_windows, plans, stream),
+                    "b2o_window_plan_test")
 
     def record_floats(self, rec_boxes):
         return int(self.lib.b2o_record_floats(rec_boxes))

@@ -397,6 +397,96 @@ static __device__ inline void plan_warp(const float* q /*4x2*/, int turn, int ta
   if (persp_inverse(box, dst, plan->m)) plan->valid = 1;
 }
 
+// ---- warpBox sampling (image.cu's box and polygon warps, windows.cu's wide-word windows) ----------------------
+constexpr int kWarpCropH = 31, kWarpCropW = 200;
+
+// cv2.warpPerspective INTER_LINEAR (BORDER_CONSTANT 0) of one crop pixel (x, y) through the inverse map m, with
+// cv::WarpPerspectiveInvoker's block width bw0 (x is re-based at multiples of it): 1/32-pixel coordinates, 15-bit
+// weights.
+template <int CH>
+static __device__ __forceinline__ void warp_sample(const uint8_t* __restrict__ g, int H, int W, const double* m, int x,
+                                                   int y, int bw0, int v[CH]) {
+  const int bx = (x / bw0) * bw0, x1 = x - bx;
+  const double X0 = __dadd_rn(__dadd_rn(__dmul_rn(m[0], bx), __dmul_rn(m[1], y)), m[2]);
+  const double Y0 = __dadd_rn(__dadd_rn(__dmul_rn(m[3], bx), __dmul_rn(m[4], y)), m[5]);
+  const double W0 = __dadd_rn(__dadd_rn(__dmul_rn(m[6], bx), __dmul_rn(m[7], y)), m[8]);
+  double Wv = __dadd_rn(W0, __dmul_rn(m[6], x1));
+  Wv = Wv != 0.0 ? 32.0 / Wv : 0.0;
+  const double fX = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(__dadd_rn(X0, __dmul_rn(m[0], x1)), Wv)));
+  const double fY = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(__dadd_rn(Y0, __dmul_rn(m[3], x1)), Wv)));
+  const int X = __double2int_rn(fX), Y = __double2int_rn(fY);
+  const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);
+  const int ax = X & 31, ay = Y & 31;
+  const bool x0ok = sx >= 0 && sx < W, x1ok = sx + 1 >= 0 && sx + 1 < W;
+  const bool y0ok = sy >= 0 && sy < H, y1ok = sy + 1 >= 0 && sy + 1 < H;
+  // BilinearTab_i: (1-fx)(1-fy) ... scaled to 2^15; exact for 1/32 steps
+  const int w00 = (32 - ax) * (32 - ay) * 32, w01 = ax * (32 - ay) * 32;
+  const int w10 = (32 - ax) * ay * 32, w11 = ax * ay * 32;
+#pragma unroll
+  for (int c = 0; c < CH; ++c) {
+    const int p00 = (x0ok && y0ok) ? g[(static_cast<size_t>(sy) * W + sx) * CH + c] : 0;
+    const int p01 = (x1ok && y0ok) ? g[(static_cast<size_t>(sy) * W + sx + 1) * CH + c] : 0;
+    const int p10 = (x0ok && y1ok) ? g[(static_cast<size_t>(sy + 1) * W + sx) * CH + c] : 0;
+    const int p11 = (x1ok && y1ok) ? g[(static_cast<size_t>(sy + 1) * W + sx + 1) * CH + c] : 0;
+    v[c] = (p00 * w00 + p01 * w01 + p10 * w10 + p11 * w11 + 16384) >> 15;
+  }
+}
+
+// The crop tile of one word -> the CRNN input slot k.  Layout (recognition.py:215-216): x[t][j] = crop[30-j][t] / 255.
+// Called by all threads after the tile is written.
+template <int CH>
+static __device__ __forceinline__ void store_crnn_in(const uint8_t* tile, int k, __half* __restrict__ crnn_in) {
+  __half* o = crnn_in + static_cast<size_t>(k) * kWarpCropH * kWarpCropW * CH;
+  for (int i = threadIdx.x; i < kWarpCropH * kWarpCropW * CH; i += blockDim.x) {
+    const int c = i % CH, q = i / CH;
+    const int t = q / kWarpCropH, j = q - t * kWarpCropH;
+    o[i] = __float2half_rn(static_cast<float>(tile[((kWarpCropH - 1 - j) * kWarpCropW + t) * CH + c]) / 255.0f);
+  }
+}
+
+// cv::WarpPerspectiveInvoker's block width for a dsize dw x dh (clamped to the crop): x is re-based at its multiples
+static __device__ __forceinline__ int warp_block_width(int dw, int dh) {
+  const int bh0 = min(16, max(dh, 1));
+  return min(1024 / bh0, max(dw, 1));
+}
+
+// The crop of one word, shared by the box, polygon and window warps: sample(x, y, v) for x < dw, y < dh (the dsize
+// clamped to the crop, 0 where the plan is invalid) and 0 elsewhere, into tile (31 x 200 x CH, shared memory) and crop
+// slot k of crops (optional); then the CRNN input slot k (optional).
+template <int CH, typename Sample>
+static __device__ __forceinline__ void warp_crop(int dw, int dh, Sample sample, uint8_t* tile, int k,
+                                                 uint8_t* __restrict__ crops, __half* __restrict__ crnn_in) {
+  for (int i = threadIdx.x; i < kWarpCropH * kWarpCropW; i += blockDim.x) {
+    const int y = i / kWarpCropW, x = i - y * kWarpCropW;
+    int v[CH];
+#pragma unroll
+    for (int c = 0; c < CH; ++c) v[c] = 0;
+    if (x < dw && y < dh) sample(x, y, v);
+#pragma unroll
+    for (int c = 0; c < CH; ++c) {
+      tile[i * CH + c] = static_cast<uint8_t>(v[c]);
+      if (crops) crops[(static_cast<size_t>(k) * kWarpCropH * kWarpCropW + i) * CH + c] = static_cast<uint8_t>(v[c]);
+    }
+  }
+  if (crnn_in == nullptr) return;
+  __syncthreads();
+  store_crnn_in<CH>(tile, k, crnn_in);
+}
+
+// ---- the STN's time axis (ctc_align.cu's character cuts, windows.cu's stitch) -----------------------------------
+// Crop column of grid row r (r = kept step + 2 discarded steps): through the STN's time coordinate on the grid's centre
+// column, u = 0.5 (theta[4] gy + theta[5] + 1) 50 with gy = -1 + 2r/49, or u = r without an STN (th null); 4 crop
+// columns per pooled step, pixel centres at integers: x = 4u + 1.5.  fp64 without contraction.
+static __device__ __forceinline__ double stn_crop_x(double r, const float* th) {
+  double u = r;
+  if (th) {
+    const double gy = __dadd_rn(-1.0, __ddiv_rn(__dmul_rn(2.0, r), 49.0));
+    u = __dmul_rn(__dmul_rn(0.5, __dadd_rn(__dadd_rn(__dmul_rn(static_cast<double>(th[4]), gy),
+                                                     static_cast<double>(th[5])), 1.0)), 50.0);
+  }
+  return __dadd_rn(__dmul_rn(4.0, u), 1.5);
+}
+
 static inline TensorView make_view(void* base, int n, int h, int w, int c, int ld = 0, int coff = 0) {
   TensorView v;
   v.ptr = reinterpret_cast<__half*>(base) + coff;

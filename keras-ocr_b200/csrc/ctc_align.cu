@@ -131,17 +131,10 @@ ctc_align_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, const i
   }
 }
 
-// Crop x of the cut before character j (1 <= j < n): grid row r = (l_{j-1} + f_j) / 2 + 2, through the STN's time
-// coordinate on the grid's centre column, 4 crop columns per pooled step, pixel centres at integers.
+// Crop x of the cut before character j (1 <= j < n): grid row r = (l_{j-1} + f_j) / 2 + 2 (common.cuh's stn_crop_x).
 __device__ __forceinline__ double cut_x(const int32_t* sp, int j, const float* th) {
   const double r = 0.5 * static_cast<double>(sp[2 * (j - 1) + 1] + sp[2 * j]) + kDiscard;
-  double u = r;
-  if (th) {
-    const double gy = __dadd_rn(-1.0, __ddiv_rn(__dmul_rn(2.0, r), 49.0));
-    u = __dmul_rn(__dmul_rn(0.5, __dadd_rn(__dadd_rn(__dmul_rn(static_cast<double>(th[4]), gy),
-                                                     static_cast<double>(th[5])), 1.0)), 50.0);
-  }
-  return __dadd_rn(__dmul_rn(4.0, u), 1.5);
+  return stn_crop_x(r, th);
 }
 
 __global__ void __launch_bounds__(kCellThreads)

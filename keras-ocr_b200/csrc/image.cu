@@ -82,49 +82,7 @@ using WarpPlan = b2o_warp_plan;
 constexpr int kCropH = 31, kCropW = 200;
 constexpr int kMaxPolySegments = B2O_MAX_POLY_SEGMENTS;
 
-// cv2.warpPerspective INTER_LINEAR (BORDER_CONSTANT 0) of one crop pixel (x, y) through the inverse map m, with
-// cv::WarpPerspectiveInvoker's block width bw0 (x is re-based at multiples of it): 1/32-pixel coordinates, 15-bit
-// weights.  Shared by warp_kernel and warp_polys_kernel.
-template <int CH>
-__device__ __forceinline__ void warp_sample(const uint8_t* __restrict__ g, int H, int W, const double* m, int x, int y,
-                                            int bw0, int v[CH]) {
-  const int bx = (x / bw0) * bw0, x1 = x - bx;
-  const double X0 = __dadd_rn(__dadd_rn(__dmul_rn(m[0], bx), __dmul_rn(m[1], y)), m[2]);
-  const double Y0 = __dadd_rn(__dadd_rn(__dmul_rn(m[3], bx), __dmul_rn(m[4], y)), m[5]);
-  const double W0 = __dadd_rn(__dadd_rn(__dmul_rn(m[6], bx), __dmul_rn(m[7], y)), m[8]);
-  double Wv = __dadd_rn(W0, __dmul_rn(m[6], x1));
-  Wv = Wv != 0.0 ? 32.0 / Wv : 0.0;
-  const double fX = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(__dadd_rn(X0, __dmul_rn(m[0], x1)), Wv)));
-  const double fY = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(__dadd_rn(Y0, __dmul_rn(m[3], x1)), Wv)));
-  const int X = __double2int_rn(fX), Y = __double2int_rn(fY);
-  const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);
-  const int ax = X & 31, ay = Y & 31;
-  const bool x0ok = sx >= 0 && sx < W, x1ok = sx + 1 >= 0 && sx + 1 < W;
-  const bool y0ok = sy >= 0 && sy < H, y1ok = sy + 1 >= 0 && sy + 1 < H;
-  // BilinearTab_i: (1-fx)(1-fy) ... scaled to 2^15; exact for 1/32 steps
-  const int w00 = (32 - ax) * (32 - ay) * 32, w01 = ax * (32 - ay) * 32;
-  const int w10 = (32 - ax) * ay * 32, w11 = ax * ay * 32;
-#pragma unroll
-  for (int c = 0; c < CH; ++c) {
-    const int p00 = (x0ok && y0ok) ? g[(static_cast<size_t>(sy) * W + sx) * CH + c] : 0;
-    const int p01 = (x1ok && y0ok) ? g[(static_cast<size_t>(sy) * W + sx + 1) * CH + c] : 0;
-    const int p10 = (x0ok && y1ok) ? g[(static_cast<size_t>(sy + 1) * W + sx) * CH + c] : 0;
-    const int p11 = (x1ok && y1ok) ? g[(static_cast<size_t>(sy + 1) * W + sx + 1) * CH + c] : 0;
-    v[c] = (p00 * w00 + p01 * w01 + p10 * w10 + p11 * w11 + 16384) >> 15;
-  }
-}
-
-// The crop tile of one word -> crops (optional) and the CRNN input (optional).  Layout (recognition.py:215-216):
-// x[t][j] = crop[30-j][t] / 255.  Called by all threads after the tile and crops are written.
-template <int CH>
-__device__ __forceinline__ void store_crnn_in(const uint8_t* tile, int k, __half* __restrict__ crnn_in) {
-  __half* o = crnn_in + static_cast<size_t>(k) * kCropH * kCropW * CH;
-  for (int i = threadIdx.x; i < kCropH * kCropW * CH; i += blockDim.x) {
-    const int c = i % CH, q = i / CH;
-    const int t = q / kCropH, j = q - t * kCropH;
-    o[i] = __float2half_rn(static_cast<float>(tile[((kCropH - 1 - j) * kCropW + t) * CH + c]) / 255.0f);
-  }
-}
+// warp_sample, warp_block_width and warp_crop: common.cuh.
 
 // CH = 1: gray image (n,H,W), crops (k,31,200), CRNN input (k,200,31).  CH = 3 (build_model(color=True),
 // recognition.py:214, 508-510: no gray conversion): RGB image (n,H,W,3), crops (k,31,200,3), CRNN input (k,200,31,3);
@@ -142,24 +100,9 @@ warp_kernel(const uint8_t* __restrict__ gray, int n, int H, int W, const float* 
   img = min(max(img, 0), n - 1);
   const uint8_t* g = gray + static_cast<size_t>(img) * H * W * CH;
   const int dw = plan.valid ? min(plan.dw, kCropW) : 0, dh = plan.valid ? min(plan.dh, kCropH) : 0;
-  // block structure of cv::WarpPerspectiveInvoker (decides where X0/Y0/W0 are re-based)
-  int bh0 = min(16, max(dh, 1));
-  const int bw0 = min(1024 / bh0, max(dw, 1));
-  for (int i = threadIdx.x; i < kCropH * kCropW; i += blockDim.x) {
-    const int y = i / kCropW, x = i - y * kCropW;
-    int v[CH];
-#pragma unroll
-    for (int c = 0; c < CH; ++c) v[c] = 0;
-    if (x < dw && y < dh) warp_sample<CH>(g, H, W, plan.m, x, y, bw0, v);
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      tile[i * CH + c] = static_cast<uint8_t>(v[c]);
-      if (crops) crops[(static_cast<size_t>(k) * kCropH * kCropW + i) * CH + c] = static_cast<uint8_t>(v[c]);
-    }
-  }
-  if (crnn_in == nullptr) return;
-  __syncthreads();
-  store_crnn_in<CH>(tile, k, crnn_in);
+  const int bw0 = warp_block_width(dw, dh);
+  warp_crop<CH>(dw, dh, [&](int x, int y, int (&v)[CH]) { warp_sample<CH>(g, H, W, plan.m, x, y, bw0, v); },
+                tile, k, crops, crnn_in);
 }
 
 // ------------------------------------------------------------------------------------ piecewise warpBox
@@ -234,28 +177,13 @@ warp_polys_kernel(const uint8_t* __restrict__ img_all, int n, int H, int W, cons
   img = min(max(img, 0), n - 1);
   const uint8_t* g = img_all + static_cast<size_t>(img) * H * W * CH;
   const int dw = plan.valid ? min(plan.dw, kCropW) : 0, dh = plan.valid ? min(plan.dh, kCropH) : 0;
-  int bh0 = min(16, max(dh, 1));
-  const int bw0 = min(1024 / bh0, max(dw, 1));
-  for (int i = threadIdx.x; i < kCropH * kCropW; i += blockDim.x) {
-    const int y = i / kCropW, x = i - y * kCropW;
-    int v[CH];
-#pragma unroll
-    for (int c = 0; c < CH; ++c) v[c] = 0;
-    if (x < dw && y < dh) {
-      int seg = 0;
-      const float fx = static_cast<float>(x);
-      for (int j = 1; j < plan.s; ++j) if (plan.X[j] <= fx) seg = j;
-      if (plan.seg_ok[seg]) warp_sample<CH>(g, H, W, plan.m[seg], x, y, bw0, v);
-    }
-#pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      tile[i * CH + c] = static_cast<uint8_t>(v[c]);
-      if (crops) crops[(static_cast<size_t>(k) * kCropH * kCropW + i) * CH + c] = static_cast<uint8_t>(v[c]);
-    }
-  }
-  if (crnn_in == nullptr) return;
-  __syncthreads();
-  store_crnn_in<CH>(tile, k, crnn_in);
+  const int bw0 = warp_block_width(dw, dh);
+  warp_crop<CH>(dw, dh, [&](int x, int y, int (&v)[CH]) {
+    int seg = 0;
+    const float fx = static_cast<float>(x);
+    for (int j = 1; j < plan.s; ++j) if (plan.X[j] <= fx) seg = j;
+    if (plan.seg_ok[seg]) warp_sample<CH>(g, H, W, plan.m[seg], x, y, bw0, v);
+  }, tile, k, crops, crnn_in);
 }
 
 // b2o_warp_plan_test: plan_warp alone, one thread per box.  A degenerate box leaves m, dw and dh zero.

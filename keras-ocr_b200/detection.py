@@ -146,14 +146,17 @@ class Detector:
         return scores
 
     def boxes_enqueue(self, scores, detection_threshold=0.7, text_threshold=0.4, link_threshold=0.4,
-                      size_threshold=10, with_scores=False, with_polygons=False):
+                      size_threshold=10, with_scores=False, with_polygons=False, max_windows=1):
         """getBoxes on the device, asynchronously: launches the kernels and the copy of the per-image counts into
         pinned memory, records an event and returns at once (``boxes_finish`` waits for that event only, so work
         enqueued afterwards keeps the GPU busy while the host reads the counts).  ``with_scores``: the state also
         holds ``box_scores`` (N,M) float32 CUDA, each box's detection score (``b2o_get_boxes_scored``).
         ``with_polygons``: the state also holds every box's polygon (``b2o_get_boxes_poly``), ``polys`` (N,M,18,2)
         float32 and ``points`` (N,M) int32 CUDA, and their dense lists ``flat_polys`` / ``flat_points`` in the order
-        of ``flat``; boxes and scores are those of the call without polygons."""
+        of ``flat``; boxes and scores are those of the call without polygons.  ``max_windows`` > 1: the state also holds
+        ``windows_pin`` (N,M) int32 pinned, every box's window count K (``b2o_window_counts``, see
+        ``recognition.check_windows``), copied with the counts and valid once ``boxes_finish`` returns, for the first
+        count boxes of each image."""
         n, hs, ws_, _ = scores.shape
         stream = torch.cuda.current_stream(self.device)
         scores = scores.contiguous()
@@ -183,6 +186,13 @@ class Detector:
                                wsp.data_ptr(), nbytes, stream.cuda_stream)
         counts_pin = torch.empty((n,), dtype=torch.int32, pin_memory=True)
         counts_pin.copy_(counts, non_blocking=True)
+        windows_pin = None
+        if max_windows > 1:                              # read back with the counts: no synchronisation of its own
+            windows = torch.empty((n, m), dtype=torch.int32, device=self.device)
+            self.ctx.window_counts(boxes.data_ptr(), counts.data_ptr(), n, m, int(max_windows), windows.data_ptr(),
+                                   stream.cuda_stream)
+            windows_pin = torch.empty((n, m), dtype=torch.int32, pin_memory=True)
+            windows_pin.copy_(windows, non_blocking=True)
         event = torch.cuda.Event()
         event.record(stream)
         # recognize_from_boxes' bookkeeping (dense box list + image index, recognition.py:511-521) is queued
@@ -199,7 +209,8 @@ class Detector:
                                    flat_points.data_ptr(), image_index.data_ptr(), stream.cuda_stream)
         return {"scores": scores, "boxes": boxes, "counts": counts, "counts_pin": counts_pin, "event": event, "m": m,
                 "thr": thr, "flat": flat, "image_index": image_index, "box_scores": box_scores, "polys": polys,
-                "points": points, "flat_polys": flat_polys, "flat_points": flat_points}
+                "points": points, "flat_polys": flat_polys, "flat_points": flat_points, "max_windows": max_windows,
+                "windows_pin": windows_pin}
 
     def boxes_finish(self, state):
         """Wait for ``boxes_enqueue``.  Returns (boxes (N,M,4,2) float32 CUDA, counts ndarray (N,)); re-runs
@@ -211,7 +222,8 @@ class Detector:
             self.max_boxes = int(2 ** np.ceil(np.log2(int(counts_host.max()))))
             d, t, l, s = state["thr"]
             again = self.boxes_enqueue(state["scores"], d, t, l, s, with_scores=state["box_scores"] is not None,
-                                       with_polygons=state.get("polys") is not None)
+                                       with_polygons=state.get("polys") is not None,
+                                       max_windows=state.get("max_windows", 1))
             again["event"].synchronize()
             state.update(again)
             counts_host = state["counts_pin"].numpy().copy()

@@ -124,12 +124,14 @@ class Pipeline:
         return (batch, scales, gray) if want_gray else (batch, scales)
 
     # ---------------------------------------------------------------- the three stages of one sub-batch
-    def _stage_detect(self, images, pad_to, thresholds, with_scores=False, with_polygons=False):
+    def _stage_detect(self, images, pad_to, thresholds, with_scores=False, with_polygons=False, max_windows=1):
         batch, scales, gray = self.prepare_device(images, pad_to, want_gray=True)
         scores = self.detector.predict_device(batch)
+        extra = {"with_polygons": True} if with_polygons else {}
+        if max_windows > 1:
+            extra["max_windows"] = max_windows
         return {"batch": batch, "scales": scales, "gray": gray,
-                "boxes_state": self.detector.boxes_enqueue(scores, **thresholds, with_scores=with_scores,
-                                                           **({"with_polygons": True} if with_polygons else {}))}
+                "boxes_state": self.detector.boxes_enqueue(scores, **thresholds, with_scores=with_scores, **extra)}
 
     @staticmethod
     def _to_host(st, key, t):
@@ -145,6 +147,11 @@ class Pipeline:
         extra = {"char_boxes": True} if char_boxes else {}
         if polys is not None:
             extra = {"polys": bst["flat_polys"], "points": bst["flat_points"]}
+        if bst.get("windows_pin") is not None:           # every word's window count, read back with the box counts
+            windows = bst["windows_pin"].numpy()
+            m = boxes.shape[1]
+            extra = {"max_windows": bst["max_windows"],
+                     "windows": np.concatenate([windows[i, :min(int(c), m)] for i, c in enumerate(counts)])}
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
                                                  image_index=bst["image_index"], with_scores=box_scores is not None,
                                                  **beam, **extra)
@@ -307,6 +314,12 @@ class Pipeline:
         ``box`` the block's (4,2) float32 box in the input image's pixels, aligned to the page's reading direction.
         The lines are cut into blocks on the device (``Detector.group_blocks_device``, recursive XY-cut: rows first,
         then columns) with ``block_kwargs`` (``detection.check_blocks``).  It implies ``return_lines``.
+        ``recognition_kwargs`` may also hold ``max_windows`` (``recognition.check_windows``, default 1): every box wider
+        than the recognizer's 200 x 31 crop at full height is read in up to that many overlapping windows whose steps
+        are stitched into one reading; the window counts travel back with the box counts, so this adds no
+        synchronisation.  Boxes, and so lines and blocks, are unchanged.  It combines with ``return_scores``,
+        ``return_lines``, ``return_blocks`` and ``inflight``; with ``beam_width``, ``lexicon``, ``rotations``,
+        ``return_char_boxes`` or ``return_polygons`` it raises ``ValueError``.
         """
         if return_polygons and (return_char_boxes or (recognition_kwargs or {}).get("rotations") is not None):
             raise ValueError("return_polygons does not combine with rotations or return_char_boxes")
@@ -332,6 +345,8 @@ class Pipeline:
             turns = recognition.check_rotations(recognition_kwargs.get("rotations"), vote)
             if turns is not None:
                 beam["rotations"], beam["rotation_vote"] = turns, vote
+            max_windows = recognition.check_windows(recognition_kwargs.get("max_windows", 1), beam.get("beam_width"),
+                                                    beam.get("lexicon"), turns, return_char_boxes, return_polygons)
         if not self._native():
             if return_scores:
                 raise NotImplementedError("return_scores=True needs this package's Detector and Recognizer; injected "
@@ -364,7 +379,8 @@ class Pipeline:
         for step in range(k + 2):                        # detect(i) | recognize(i-1) | finish(i-2)
             if step < k:
                 states.append(self._stage_detect(images[bounds[step]:bounds[step + 1]], pad_to, thresholds,
-                                                 with_scores=return_scores, with_polygons=return_polygons))
+                                                 with_scores=return_scores, with_polygons=return_polygons,
+                                                 max_windows=max_windows))
             if 1 <= step <= k:
                 self._stage_recognize(states[step - 1], beam, char_boxes=return_char_boxes,
                                       lines=lines if return_lines or return_blocks else None,

@@ -194,6 +194,27 @@ def check_rotations(rotations=None, rotation_vote="word"):
     return turns
 
 
+def check_windows(max_windows=1, beam_width=None, lexicon=None, rotations=None, char_boxes=False, polygons=False):
+    """Validates a choice of wide-word windows before anything is launched (``ValueError`` otherwise) and returns it as
+    an int.  ``max_windows=1`` (the default) reads every box as one 200 x 31 crop, as warpBox cuts it.  An int 2 <= M <=
+    16 reads every box wider than that crop at full height in up to M overlapping 200 x 31 windows and stitches their
+    CTC steps into one reading (DESIGN.md section 1, "Wide words"); when a box of the call is wide the labels rows are
+    48 M wide, -1 padded, and every other box reads exactly as with M = 1.  The windows are decoded greedily over 48
+    steps each: with M > 1, ``beam_width``, ``lexicon``, ``rotations``, character boxes (``char_boxes``) and polygons
+    (``polygons``) raise."""
+    if (not isinstance(max_windows, (int, np.integer)) or isinstance(max_windows, (bool, np.bool_))
+            or not 1 <= max_windows <= _lib.MAX_WINDOWS):
+        raise ValueError(f"max_windows must be an int in [1, {_lib.MAX_WINDOWS}], got {max_windows!r}")
+    if max_windows > 1:
+        excluded = [name for name, on in (("beam_width", beam_width is not None), ("lexicon", lexicon is not None),
+                                          ("rotations", rotations is not None), ("return_char_boxes", char_boxes),
+                                          ("return_polygons", polygons)) if on]
+        if excluded:
+            raise ValueError(f"max_windows > 1 reads wide words by greedy decoding only; it does not combine with "
+                             f"{', '.join(excluded)}")
+    return int(max_windows)
+
+
 def check_polygons(entries):
     """Validates the words of a box group on the host, before anything is launched, and returns them as the dense table
     ``b2o_warp_polys`` reads: (polys (B,18,2) float32, points (B,) int32), unused points NaN.  An entry is a (2m,2)
@@ -385,6 +406,70 @@ class Recognizer:
                             torch.cuda.current_stream(self.device).cuda_stream)
         return crnn_in, crops
 
+    def window_counts_device(self, flat, max_windows):
+        """``b2o_window_counts`` of a dense box list: flat (B,4,2) float32 CUDA -> K (B,) int32 CUDA, the windows every
+        box is read in with ``max_windows`` (1 for a box that fits the 200 x 31 crop at full height)."""
+        b = flat.shape[0]
+        out = torch.empty((b,), dtype=torch.int32, device=self.device)
+        self.ctx.window_counts(flat.data_ptr(), None, 1, b, int(max_windows), out.data_ptr(),
+                               torch.cuda.current_stream(self.device).cuda_stream)
+        return out
+
+    def _read_windowed(self, gray, flat, image_index, max_windows, windows, with_scores):
+        """Warp + CRNN + greedy CTC of every box, then every wide box (K >= 2 in ``windows``, host ints (B,), or None:
+        computed here and read back) read again in its K windows and stitched: (labels, logp (B,) or None) CUDA, labels
+        (B,48 M) int32 -1 padded, or the default read's (B,48) when no box is wide.  The windows go through the CRNN in
+        chunks of at most B crops, so the CRNN workspace stays that of the default read; only their logits and theta are
+        kept for ``b2o_stitch_windows``.  With ``windows`` given nothing here waits for the device: the word list and the
+        CSR of window starts travel through pinned memory."""
+        b, m = flat.shape[0], int(max_windows)
+        if windows is None:
+            windows = self.window_counts_device(flat, m).cpu().numpy()
+        windows = np.asarray(windows)
+        crnn_in, _ = self.warp_device(gray, flat, image_index)
+        read = self.predict_device(crnn_in, with_scores=with_scores)
+        labels, logp = read if with_scores else (read, None)
+        del crnn_in
+        wide = np.flatnonzero(windows >= 2)
+        if wide.size == 0:
+            return labels, logp
+        out = torch.full((b, STEPS * m), -1, dtype=torch.int32, device=self.device)
+        out[:, :STEPS] = labels
+        csr = torch.empty((2 * wide.size + 1,), dtype=torch.int32, pin_memory=True)     # words, then window starts
+        host = csr.numpy()
+        host[:wide.size] = wide
+        host[wide.size] = 0
+        host[wide.size + 1:] = np.cumsum(windows[wide])
+        csr_t = csr.to(self.device, non_blocking=True)  # the pinned block is not reused before this copy has run
+        words_t, start_t = csr_t[:wide.size], csr_t[wide.size:]
+        total, k = int(host[-1]), len(self.alphabet) + 1
+        logits = torch.empty((total, STEPS, k), dtype=torch.float32, device=self.device)
+        theta = torch.empty((total, 6), dtype=torch.float32, device=self.device) if self.stn else None
+        chunk = min(b, total)
+        tail = (3,) if self.color else ()
+        x = torch.empty((chunk, TARGET_WIDTH, TARGET_HEIGHT) + tail, dtype=torch.float16, device=self.device)
+        greedy = torch.empty((chunk, STEPS), dtype=torch.int32, device=self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        n, h, w = gray.shape[:3]
+        for first in range(0, total, chunk):
+            c = min(chunk, total - first)
+            self.ctx.warp_windows(gray.data_ptr(), 3 if self.color else 1, n, h, w, flat.data_ptr(),
+                                  image_index.data_ptr(), words_t.data_ptr(), start_t.data_ptr(), wide.size, m, first, c,
+                                  None, x.data_ptr(), stream)
+            nbytes = self.ctx.crnn_workspace_bytes(c)
+            if self._ws is None or self._ws.numel() < nbytes:
+                self._ws = None
+                self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            ws = self._ws.data_ptr()
+            self.ctx.crnn_forward_logits(x.data_ptr(), c, greedy.data_ptr(), None, ws, nbytes, stream)
+            self.ctx.crnn_tap("logits", ws, c, logits[first].data_ptr(), c * STEPS * k * 4, stream)
+            if theta is not None:
+                self.ctx.crnn_tap("theta", ws, c, theta[first].data_ptr(), c * 6 * 4, stream)
+        self.ctx.stitch_windows(logits.data_ptr(), k, None if theta is None else theta.data_ptr(), flat.data_ptr(),
+                                words_t.data_ptr(), start_t.data_ptr(), wide.size, m, out.data_ptr(),
+                                None if logp is None else logp.data_ptr(), stream)
+        return out, logp
+
     def _decoder(self, beam_width, top_paths, lexicon):
         """``check_decoder`` for this recognizer's alphabet."""
         return check_decoder(beam_width, top_paths, lexicon, DEFAULT_ALPHABET if lexicon is None else self.alphabet)
@@ -520,7 +605,8 @@ class Recognizer:
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
                                     with_scores=False, beam_width=None, top_paths=1, lexicon=None, rotations=None,
-                                    rotation_vote="word", char_boxes=False, polys=None, points=None):
+                                    rotation_vote="word", char_boxes=False, polys=None, points=None, max_windows=1,
+                                    windows=None):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
         (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon``: see
         ``predict_device``).
@@ -542,14 +628,28 @@ class Recognizer:
 
         ``polys`` (>=B,18,2) float32 / ``points`` (>=B,) int32 CUDA, the dense polygons of ``b2o_compact_polys`` in the
         order of ``flat`` (with ``image_index``): every word is read along its polygon (``b2o_warp_polys``); a 4-point
-        entry reads as its box.  Rotations and character cells do not combine with polygons (``ValueError``)."""
+        entry reads as its box.  Rotations and character cells do not combine with polygons (``ValueError``).
+
+        ``max_windows`` (``check_windows``): every box wider than the crop at full height is read in up to that many
+        windows (``b2o_warp_windows``, ``b2o_stitch_windows``); labels are then (B,48 max_windows), -1 padded, or
+        (B,48) as without the option when no box is wide.  ``windows``: host ints (B,), the K of every box as
+        ``b2o_window_counts`` gives them (``Pipeline.recognize`` reads them back with the box counts; ``ValueError`` for
+        another shape or a count outside [1, max_windows]); None: computed here and read back, one more
+        synchronisation."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
         turns = check_rotations(rotations, rotation_vote)
+        max_windows = check_windows(max_windows, beam_width, lexicon, turns, char_boxes, polys is not None)
         if polys is not None and (turns is not None or char_boxes):
             raise ValueError("polygons do not combine with rotations or character boxes")
         counts = np.asarray(counts)
         m = boxes.shape[1]
         total = int(np.minimum(counts, m).sum())
+        if max_windows > 1 and windows is not None:
+            windows = np.asarray(windows)
+            if (windows.shape != (total,) or not np.issubdtype(windows.dtype, np.integer)
+                    or (total and (windows.min() < 1 or windows.max() > max_windows))):
+                raise ValueError(f"windows must hold one window count in [1, {max_windows}] per box ({total}), as "
+                                 f"b2o_window_counts gives them; got shape {windows.shape}")
         if total == 0:
             parts = 1 + bool(with_scores) + (turns is not None) + 2 * bool(char_boxes)
             return None if parts == 1 else (None,) * parts
@@ -564,6 +664,10 @@ class Recognizer:
             counts_dev = torch.from_numpy(counts.astype(np.int32)).to(self.device)
             self.ctx.compact_boxes(boxes.data_ptr(), counts_dev.data_ptr(), n, m, flat.data_ptr(),
                                    image_index.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
+        if max_windows > 1:
+            labels, logp = self._read_windowed(gray, flat[:total], image_index[:total], max_windows, windows,
+                                               with_scores)
+            return (labels, logp) if with_scores else labels
         if polys is not None:
             crnn_in, _ = self.warp_polys_device(gray, polys[:total], points[:total], image_index[:total])
             return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
@@ -627,7 +731,7 @@ class Recognizer:
 
     # ------------------------------------------------------------------ reference API
     def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                             rotations=None, rotation_vote="word", return_char_boxes=False,
+                             rotations=None, rotation_vote="word", return_char_boxes=False, max_windows=1,
                              **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
         (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon``: as
@@ -640,14 +744,18 @@ class Recognizer:
         A box group may also hold polygons, (2m,2) arrays with 3 <= m <= 9 as ``Detector.detect(return_polygons=True)``
         returns them (``check_polygons``): such a word is read along its polygon (``b2o_warp_polys``), a 4-point entry
         of the same group exactly as without polygons.  Rotations and character boxes do not combine with polygons
-        (``ValueError``)."""
+        (``ValueError``).
+        ``max_windows``: every box wider than the 200 x 31 crop at full height is read in up to that many overlapping
+        windows and their steps stitched into one reading (``check_windows``; greedy decoding, boxes only)."""
         lexicon = self._decoder(beam_width, top_paths, lexicon)
         turns = check_rotations(rotations, rotation_vote)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
 
         entries = [e for g in box_groups for e in g]
-        if any(np.ndim(e) == 2 and np.shape(e)[0] != 4 for e in entries):
+        polygons = any(np.ndim(e) == 2 and np.shape(e)[0] != 4 for e in entries)
+        max_windows = check_windows(max_windows, beam_width, lexicon, turns, return_char_boxes, polygons)
+        if polygons:
             return self._recognize_polygons(images, box_groups, entries, return_scores, turns, return_char_boxes,
                                             beam_width, top_paths, lexicon)
         images_t = _as_device_images(images, self.device)
@@ -675,6 +783,10 @@ class Recognizer:
         elif turns is not None:
             labels, logp, _ = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns, rotation_vote, True,
                                                     **beam)
+            texts, conf = decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())
+            predictions = list(zip(texts, conf)) if return_scores else texts
+        elif max_windows > 1:
+            labels, logp = self._read_windowed(gray, flat_t, idx, max_windows, None, True)
             texts, conf = decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())
             predictions = list(zip(texts, conf)) if return_scores else texts
         elif return_scores:
