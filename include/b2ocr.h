@@ -66,6 +66,9 @@ int64_t b2o_launch_count(const b2o_ctx* ctx);
 /* number of tensor-core conv launches since creation that ran channels by pixels on 16 x 16-pixel tiles (the streamed
  * 128-channel 3x3 layers; B2O_TC_SWAP=0 turns that body off): lets tests see which body computed a result */
 int64_t b2o_tc_tile256_launches(const b2o_ctx* ctx);
+/* number of tensor-core conv launches since creation that ran paired n-tiles (generic 128-channel tiles of layers with
+ * cout % 256 == 0: both consumer warpgroups share every activation box) */
+int64_t b2o_tc_coop_n_launches(const b2o_ctx* ctx);
 
 /* Measurement hook (bench.py's roofline leg): when enabled, every launch of the tensor-core conv
  * kernel is bracketed by CUDA events on its stream; b2o_profile_read sums the kernel time (ms), the
@@ -608,7 +611,9 @@ int b2o_conv_test(b2o_ctx* ctx, const b2o_conv_test_desc* desc, void* stream);
  * tiles, 2 halo tiles with the filter bank resident in shared memory); body 0 pixels by channels, 1 channels by pixels,
  * 2 channels by pixels on 16 x 16-pixel tiles; the tile_w x tile_h x tile_n pixel tile and the number of tiles (pixel
  * tiles x output-channel tiles); the ring's stages, the bytes between stages and the bytes one stage's barrier expects;
- * the resident filter bank's bytes (0: streamed with the stages); dynamic shared memory and grid of the launch.      */
+ * the resident filter bank's bytes (0: streamed with the stages); dynamic shared memory and grid of the launch; coop_n
+ * 1 where the two consumer warpgroups run paired n-tiles (tiles 2u and 2u + 1 share each activation box: a (tap,
+ * chunk) step then fills one stage_tx slot and one slot of the filter rows alone).                                    */
 typedef struct {
   int n, h, w, cin, cout, ksize, dilation;
   int out_f32, pool, tail, up_add;
@@ -618,6 +623,7 @@ typedef struct {
   int32_t block_n, kch, mode, pair, upadd, body;
   int32_t tile_w, tile_h, tile_n, tiles;
   int32_t stages, stage_bytes, stage_tx, resident_bytes, smem_bytes, grid;
+  int32_t coop_n;
 } b2o_conv_plan;
 int b2o_conv_plan_test(const b2o_conv_plan_desc* desc, b2o_conv_plan* plan);
 

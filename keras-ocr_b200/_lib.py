@@ -63,7 +63,7 @@ class _ConvPlan(ctypes.Structure):
     """b2o_conv_plan (include/b2ocr.h), field for field."""
     _fields_ = [(name, _c.c_int32) for name in ("block_n", "kch", "mode", "pair", "upadd", "body", "tile_w", "tile_h",
                                                 "tile_n", "tiles", "stages", "stage_bytes", "stage_tx", "resident_bytes",
-                                                "smem_bytes", "grid")]
+                                                "smem_bytes", "grid", "coop_n")]
 
 # name -> (restype, argtypes); mirrors include/b2ocr.h one to one
 SIGNATURES = {
@@ -74,6 +74,7 @@ SIGNATURES = {
     "b2o_set_conv_engine": (_i, [_vp, _i]),
     "b2o_launch_count": (_c.c_int64, [_vp]),
     "b2o_tc_tile256_launches": (_c.c_int64, [_vp]),
+    "b2o_tc_coop_n_launches": (_c.c_int64, [_vp]),
     "b2o_profile_enable": (_i, [_vp, _i]),
     "b2o_profile_read": (_i, [_vp, _c.POINTER(_c.c_double), _c.POINTER(_c.c_double), _c.POINTER(_c.c_int64)]),
     "b2o_load_craft": (_i, [_vp, _c.POINTER(_Tensor), _i]),
@@ -242,6 +243,10 @@ class Context:
     def tile256_launches(self):
         """Tensor-core conv launches so far that ran channels by pixels on 16 x 16-pixel tiles."""
         return int(self.lib.b2o_tc_tile256_launches(self.handle))
+
+    def coop_n_launches(self):
+        """Tensor-core conv launches so far that ran paired n-tiles (both warpgroups sharing every activation box)."""
+        return int(self.lib.b2o_tc_coop_n_launches(self.handle))
 
     def profile_enable(self, on):
         self._check(self.lib.b2o_profile_enable(self.handle, int(on)), "b2o_profile_enable")

@@ -377,6 +377,7 @@ extern "C" void b2o_destroy(b2o_ctx* ctx) {
 extern "C" const char* b2o_last_error(const b2o_ctx* ctx) { return ctx ? ctx->error.c_str() : "null context"; }
 extern "C" int64_t b2o_launch_count(const b2o_ctx* ctx) { return ctx ? ctx->launches : 0; }
 extern "C" int64_t b2o_tc_tile256_launches(const b2o_ctx* ctx) { return ctx ? ctx->tc_tile256_launches : 0; }
+extern "C" int64_t b2o_tc_coop_n_launches(const b2o_ctx* ctx) { return ctx ? ctx->tc_coop_n_launches : 0; }
 
 extern "C" int b2o_profile_enable(b2o_ctx* ctx, int on) {
   if (!ctx) return B2O_ERR_ARG;

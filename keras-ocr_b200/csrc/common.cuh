@@ -103,6 +103,7 @@ struct b2o_ctx {
   bool tc_swap = true;         // 64-channel fp16 layers, and the streamed 128-channel halo layers on 16 x 16 tiles, as channels x
                                // pixels GEMMs (bit-identical); B2O_TC_SWAP=0: pixels x channels
   int64_t tc_tile256_launches = 0;   // conv launches that took the 16 x 16-tile channels-by-pixels body (b2o_tc_tile256_launches)
+  int64_t tc_coop_n_launches = 0;    // conv launches that ran paired n-tiles (b2o_tc_coop_n_launches)
   std::set<const void*> configured;   // kernels whose per-device launch attributes are set on this device
   int64_t launches = 0;
   std::string error;

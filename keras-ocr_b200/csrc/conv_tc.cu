@@ -24,7 +24,8 @@
 //   runs its epilogue while the other keeps the tensor cores busy.  64-channel fp16 layers run transposed (p.ct,
 //   see conv_tc_body): one m64 (channels) x n128 (pixels) x k16 wgmma per k step and TMA-stored outputs;
 //   the streamed 128-channel halo layers run transposed on 16 x 16-pixel tiles (p.tile256): both warpgroups read every
-//   stage, one m64 (their 64 channels) x n256 (pixels) x k16 wgmma each per k step.
+//   stage, one m64 (their 64 channels) x n256 (pixels) x k16 wgmma each per k step; the generic 128-channel tiles of
+//   layers with cout % 256 == 0 run paired n-tiles (p.coop_n): both warpgroups share each activation box, one n-tile each.
 // * persistent: grid = min(#tiles, #SMs); n-tiles of one pixel tile run back to back.
 #include <stdlib.h>
 #include <string.h>
@@ -59,6 +60,7 @@ struct TcParams {
   int off_out;                            // ct, tile256: the two warpgroups' output tiles (+ pooled tiles)
   int aff_smem;                           // epilogue constants staged in shared memory behind the barriers (B2O_TC_AFF=smem)
   int aff_const;                          // epilogue constants read from the AffConst kernel parameter (default)
+  int coop_n;                             // paired n-tiles: both warpgroups share every activation box (generic tiles)
   const float *s1, *t1, *s2, *t2;
   int relu;
   void* out;
@@ -312,13 +314,23 @@ struct AffConst {
 //       tile (tile rows 0-7, then 8-15), each a (64, 16, 8) TMA store at the warpgroup's channels.  Only two 84 KB stages
 //       fit, so a slot lands in three parts (halo box + dy = 0's rows on full[s], dy = 1, 2 on tap_full) and the MMAs
 //       of each dy start as soon as their part is in.
-template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD, bool CT, bool WIDE = false>
+// COOP: paired n-tiles (p.coop_n) on generic 128-channel tiles: a work unit is tiles 2u and 2u + 1, i.e. n-tiles 2j and
+//       2j + 1 of one pixel tile, and warpgroup wg computes n-tile 2j + wg.  Per (tap, chunk) the producer fills a pair
+//       of ring slots: slot s gets the activation box and n-tile 2j's filter rows, slot s + 1 only n-tile 2j + 1's
+//       filter rows (in its B part), so the activation box is fetched once for both n-tiles: 24 instead of 32 KB per
+//       128 x 128 x 64 block.  Both warpgroups wait on both slots and release both (no ping-pong); each issues the
+//       two m64 x n128 x k16 of the pixels-by-channels body per k step, A from slot s, B from slot s + wg, and runs the
+//       same epilogue at its n-tile: every output gets the same products in the same order, bit-identical results.
+template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD, bool CT, bool WIDE = false, bool COOP = false>
 __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUtensorMap& bmap, const CUtensorMap& omap,
                                              const CUtensorMap& pmap, const TcParams& p, const AffConst& ac) {
   static_assert(!CT || (!PAIR && !UPADD && (WIDE ? (BLOCK_N == 128 && KCH == 64 && MODE == 1) : BLOCK_N == 64)),
                 "channels by pixels: 64-channel single-CTA tiles, or 128-channel streamed halo tiles (WIDE)");
   static_assert(!WIDE || CT, "the 16 x 16 tiles run channels by pixels");
+  static_assert(!COOP || (BLOCK_N == 128 && KCH == 64 && MODE == 0 && !PAIR && !UPADD && !CT),
+                "paired n-tiles: generic single-CTA 128-channel tiles, pixels by channels");
   constexpr bool HALO = MODE >= 1, RESIDENT = MODE == 2;
+  constexpr bool SHARED = WIDE || COOP;                    // both consumer warpgroups read every stage (no ping-pong)
   constexpr int TAPS_PER_A = HALO ? 3 : 1;                 // dy taps served by one A stage
   constexpr int B_BYTES = BLOCK_N * KCH * 2;
   constexpr int B_HALF = B_BYTES / 2;                      // pair: the B rows one CTA fetches and multicasts
@@ -356,8 +368,8 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
     for (int s = 0; s < MAX_RING; ++s) {
       mbar_init(&full[s], 1);                              // the producer's expect_tx arrival + the TMA bytes
       // one arrival per warp of the stage's consumer warpgroup (of both CTAs of a pair; of both warpgroups on 16 x 16
-      // tiles) once its MMAs read it
-      mbar_init(&empty[s], (PAIR ? 2 : 1) * (p.tile256 ? 2 : 1) * TILE_WARPS);
+      // tiles and paired n-tiles) once its MMAs read it
+      mbar_init(&empty[s], (PAIR ? 2 : 1) * ((COOP || p.tile256) ? 2 : 1) * TILE_WARPS);
     }
     mbar_init(res_full, 1);
     for (int i = 0; i < 2 * MAX_RING; ++i) mbar_init(&tap_full[i], 1);
@@ -388,7 +400,8 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
       }
       int s = 0;
       uint32_t ph = 0;
-      for (TileIter ti(p, cta, ncta); ti.valid(p); ti.next(p)) {
+      // COOP: the CTA's units u = cta, cta + ncta, ... as their first tiles 2u (n-tile c0 = 2j, n_tiles being even)
+      for (TileIter ti(p, COOP ? 2 * cta : cta, COOP ? 2 * ncta : ncta); ti.valid(p); ti.next(p)) {
         const int tw0 = ((ti.c1 << pair_shift) + static_cast<int>(rank)) << p.bw_log2, th0 = ti.c2 << p.bh_log2, tn0 = ti.c3 << p.bn_log2;
         int ky = 0, kx = 0;
         for (int g = 0; g < groups; ++g) {
@@ -415,7 +428,13 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
                   tma_load_2d(&bmap, bar, dst, tap * p.cin + kc * KCH, ti.c0 * BLOCK_N);
               }
             }
-            if (++s == p.ns) { s = 0; ph ^= 1; }
+            if (COOP) {                                    // slot s + 1: the second n-tile's filter rows only
+              mbar_wait(&empty[s + 1], ph ^ 1);
+              mbar_expect_tx(&full[s + 1], static_cast<uint32_t>(B_BYTES));
+              tma_load_2d(&bmap, &full[s + 1], st + p.stage_bytes + p.a_stride, g * p.cin + kc * KCH,
+                          (ti.c0 + 1) * BLOCK_N);
+            }
+            if (COOP ? (s += 2) == (p.ns & ~1) : ++s == p.ns) { s = 0; ph ^= 1; }   // COOP: the ring as slot pairs
           }
           if (++kx == p.ksize) { kx = 0; ++ky; }
         }
@@ -458,14 +477,14 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
       s -= laps * p.ns;
       ph ^= static_cast<uint32_t>(laps & 1);
     };
-    // the CTA's tiles wg, wg + 2, ... (WIDE: both warpgroups take every tile)
-    TileIter ti(p, cta + (WIDE ? 0 : wg * ncta), (WIDE ? 1 : 2) * ncta);
-    if (!WIDE && wg == 1) skip_tile();
+    // the CTA's tiles wg, wg + 2, ... (WIDE: both warpgroups take every tile; COOP: every unit, n-tile c0 + wg of it)
+    TileIter ti(p, COOP ? 2 * cta : cta + (WIDE ? 0 : wg * ncta), (COOP ? 2 : (WIDE ? 1 : 2)) * ncta);
+    if (!SHARED && wg == 1) skip_tile();
     if (RESIDENT && ti.valid(p)) mbar_wait(res_full, 0);
     float acc[2 * NACC];                                     // [rows 0-63 | rows 64-127] (WIDE: pixels 0-127 | 128-255)
   #pragma unroll
     for (int i = 0; i < 2 * NACC; ++i) acc[i] = 0.0f;
-    for (bool after_other = !WIDE && wg == 1; ti.valid(p); ti.next(p), after_other = !WIDE) {
+    for (bool after_other = !SHARED && wg == 1; ti.valid(p); ti.next(p), after_other = !SHARED) {
       if (after_other) named_bar_sync(1 + wg, 2 * 128);      // the other warpgroup has issued the previous tile
       // ---- main loop: every stage of the tile, MMAs in (dx | tap, chunk, dy, k) order, both halves per k step
       int prev = -1;
@@ -473,7 +492,9 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
       for (int g = 0; g < groups; ++g) {
         for (int kc = 0; kc < kchunks; ++kc) {
           mbar_wait(&full[s], ph);
+          if (COOP) mbar_wait(&full[s + 1], ph);
           const uint64_t adesc = desc_a0 + static_cast<uint64_t>(static_cast<uint32_t>(s * p.stage_bytes) >> 4);
+          const int bs = COOP ? s + wg : s;                  // the slot holding this warpgroup's filter rows
   #pragma unroll
           for (int i = 0; i < 2 * NACC; ++i) reg_fence(acc[i]);
           wgmma_fence();
@@ -484,7 +505,7 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
               wgmma_fence();
             }
             const uint32_t boff = RESIDENT ? static_cast<uint32_t>(((t * 3 + g) * kchunks + kc) * B_BYTES)
-                                           : static_cast<uint32_t>(s * p.stage_bytes + t * B_BYTES);
+                                           : static_cast<uint32_t>(bs * p.stage_bytes + t * B_BYTES);
             const uint64_t bdesc = desc_b0 + static_cast<uint64_t>(boff >> 4);
   #pragma unroll
             for (int k = 0; k < KSTEPS; ++k) {
@@ -520,14 +541,17 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
             wgmma_wait<1>();                                 // the previous stage's MMAs are done: release it
             if (prev >= 0) {
               __syncwarp();
-              if (lane == 0) release(prev);
+              if (lane == 0) {
+                release(prev);
+                if (COOP) release(prev + 1);
+              }
             }
           }
           prev = s;
-          if (++s == p.ns) { s = 0; ph ^= 1; }
+          if (COOP ? (s += 2) == (p.ns & ~1) : ++s == p.ns) { s = 0; ph ^= 1; }
         }
       }
-      if (!WIDE) {
+      if (!SHARED) {
         if (ti.tile + ncta < p.total_tiles) named_bar_arrive(1 + (wg ^ 1), 2 * 128);   // the CTA's next tile may start
         skip_tile();
       }
@@ -535,10 +559,13 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
   #pragma unroll
       for (int i = 0; i < 2 * NACC; ++i) reg_fence(acc[i]);
       __syncwarp();
-      if (lane == 0) release(prev);
+      if (lane == 0) {
+        release(prev);
+        if (COOP) release(prev + 1);
+      }
 
       // ---- epilogue from the registers, one 64-row half after the other
-      const int c_base = ti.c0 * BLOCK_N;
+      const int c_base = (COOP ? ti.c0 + wg : ti.c0) * BLOCK_N;
       if constexpr (CT) {
         // this thread holds channels r0, r0 + 8 (hh = 0, 1) x pixels 8i + 2q, 8i + 2q + 1 in acc[4i + 2hh + 0, 1]
         // (i < 16; WIDE: i < 32, two 128-pixel halves = tile rows 0-7 and 8-15, each stored on its own): the same
@@ -777,7 +804,8 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& amap, const CUte
 }
 
 // The 64-channel single-CTA instances carry both bodies and take the channels-by-pixels one when p.ct is set; the
-// streamed 128-channel halo instance takes the 16 x 16-tile channels-by-pixels body when p.tile256 is set.
+// streamed 128-channel halo instance takes the 16 x 16-tile channels-by-pixels body when p.tile256 is set, and the
+// generic 128-channel instance the paired n-tiles when p.coop_n is set.
 template <int BLOCK_N, int KCH, int MODE, bool PAIR, bool UPADD = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
@@ -792,6 +820,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
   if constexpr (BLOCK_N == 128 && KCH == 64 && MODE == 1 && !PAIR && !UPADD) {
     if (p.tile256) {
       conv_tc_body<BLOCK_N, KCH, MODE, PAIR, UPADD, true, true>(amap, bmap, omap, pmap, p, ac);
+      return;
+    }
+  }
+  if constexpr (BLOCK_N == 128 && KCH == 64 && MODE == 0 && !PAIR && !UPADD) {
+    if (p.coop_n) {
+      conv_tc_body<BLOCK_N, KCH, MODE, PAIR, UPADD, false, false, true>(amap, bmap, omap, pmap, p, ac);
       return;
     }
   }
@@ -1060,6 +1094,13 @@ std::string plan_conv_tc(const TcOptions& o, const TcLayerShape& L, const Tensor
   p.ns = static_cast<int>((budget - (p.resident ? res_bytes : 0)) / p.stage_bytes);
   if (p.ns > MAX_RING) p.ns = MAX_RING;
   if (p.ns < 2) return refuse("conv_tc_run: shared-memory plan failed for ", "");
+  // paired n-tiles (conv_tc_body, COOP) on the generic 128-channel tiles of layers with an even number of n-tiles: one
+  // activation box per two n-tiles.  Tiles, boxes, stages and grid stay as above; the rule reads the shapes, never the
+  // batch.  Short-K layers (down to lstm_in's 2 stages per tile) measured no slower than on the ping-pong schedule,
+  // whose epilogue overlap they give up, so there is no threshold on the stage count.  The ring needs two slot pairs
+  // (a pair is released once the next pair's MMAs are issued); these 32 KB stages always leave room for three.
+  p.coop_n = (!p.halo && kch == 64 && bn == 128 && L.cout % 256 == 0 && !pair && up_add == nullptr && !tail &&
+              p.ns >= 4) ? 1 : 0;
   p.off_res = p.ns * p.stage_bytes;
   p.off_out = p.off_res + (p.resident ? static_cast<int>((res_bytes + 1023) / 1024 * 1024) : 0);
   p.off_bar = p.off_out + out_tiles;
@@ -1202,6 +1243,7 @@ int conv_tc_run(b2o_ctx* ctx, const ConvLayer& L, const TensorView& in, const Te
     return B2O_ERR_CUDA;
   }
   if (p.tile256) ++ctx->tc_tile256_launches;
+  if (p.coop_n) ++ctx->tc_coop_n_launches;
   return find_kernel(plan.inst)(ctx, L, plan, amap, omap, pmap, ac, st);
 }
 
@@ -1226,5 +1268,6 @@ extern "C" int b2o_conv_plan_test(const b2o_conv_plan_desc* d, b2o_conv_plan* ou
   out->stages = p.ns; out->stage_bytes = p.stage_bytes; out->stage_tx = p.stage_tx;
   out->resident_bytes = p.resident ? d->ksize * d->ksize * d->cin * plan.inst.block_n * 2 : 0;
   out->smem_bytes = plan.smem_bytes; out->grid = plan.grid;
+  out->coop_n = p.coop_n;
   return B2O_OK;
 }

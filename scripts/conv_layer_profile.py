@@ -107,16 +107,22 @@ DILATION = {"basenet.slice5.1 (dil 6)": 6}
 def tma_fill_bytes(layer, n, h, w, k, cin, cout, sm_count):
     """Bytes the launch's TMA loads bring into shared memory, from the library's plan of the launch
     (``b2o_conv_plan_test``): every tile takes one stage per (dx | tap, 64/32/16-channel chunk) holding its activation
-    box and, unless the filter bank is resident, the stage's filter rows; a resident bank is loaded once per CTA.
-    Returns (bytes, tile description, planned instance, whether it runs the 16 x 16 body)."""
+    box and, unless the filter bank is resident, the stage's filter rows; a resident bank is loaded once per CTA.  With
+    paired n-tiles (``coop_n``) a unit of two tiles takes per stage one activation box and both tiles' filter rows.
+    Returns (bytes, tile description, planned instance, whether it runs the 16 x 16 body, whether it pairs n-tiles)."""
     from keras_ocr_b200 import _lib
     cin, cout = RUN_CHANNELS.get(layer, (cin, cout))
     plan = _lib.conv_plan(n, h, w, cin, cout, k, DILATION.get(layer, 1), pool="+pool" in layer, tail="+tail" in layer,
                           out_f32="fp32 out" in layer, swap=os.environ.get("B2O_TC_SWAP", "1") != "0", sm_count=sm_count)
     groups = 3 if plan["mode"] else k * k
-    total = plan["tiles"] * groups * (cin // plan["kch"]) * plan["stage_tx"] + plan["grid"] * plan["resident_bytes"]
+    stages = groups * (cin // plan["kch"])
+    if plan["coop_n"]:
+        total = plan["tiles"] // 2 * stages * (plan["stage_tx"] + plan["block_n"] * plan["kch"] * 2)
+    else:
+        total = plan["tiles"] * stages * plan["stage_tx"] + plan["grid"] * plan["resident_bytes"]
     inst = ",".join(str(plan[f]) for f in ("block_n", "kch", "mode")) + ",false," + ("true" if plan["upadd"] else "false")
-    return total, f"{plan['tile_w']}x{plan['tile_h']}x{plan['tile_n']} stage {plan['stage_tx']} B", inst, plan["body"] == 2
+    tile = f"{plan['tile_w']}x{plan['tile_h']}x{plan['tile_n']} stage {plan['stage_tx']} B" + (" coop_n" if plan["coop_n"] else "")
+    return total, tile, inst, plan["body"] == 2, bool(plan["coop_n"])
 
 
 def main():
@@ -156,15 +162,15 @@ def main():
     _, flop_r, n_r = rec.ctx.profile_read()
     det.ctx.profile_enable(0); rec.ctx.profile_enable(0)
 
-    def tile256_count():
-        return sum(c.tile256_launches() for c in (det.ctx, rec.ctx))
+    def counts():
+        return (sum(c.tile256_launches() for c in (det.ctx, rec.ctx)), sum(c.coop_n_launches() for c in (det.ctx, rec.ctx)))
 
     from torch.profiler import ProfilerActivity, profile
-    tile256_in_step = -tile256_count()
+    before = counts()
     with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
         pipe.recognize(pages)
         torch.cuda.synchronize()
-    tile256_in_step += tile256_count()
+    tile256_in_step, coop_n_in_step = (a - b for a, b in zip(counts(), before))
     trace_path = os.path.join(args.out_dir, "step.pt.trace.json")
     prof.export_chrome_trace(trace_path)
 
@@ -195,13 +201,16 @@ def main():
             row.update({"net": "craft" if i < n_craft else "crnn", "layer": name, "shape": [n, h, w, cin, cout],
                         "ksize": k, "flop": flop, "tflops": flop / (dur * 1e-6) / 1e12})
             if ",true," not in row["instance"]:           # CTA pairs (B2O_TC_PAIR) are not in the default plan
-                fill, tile, planned, wide = tma_fill_bytes(name, n, h, w, k, cin, cout, sm_count)
+                fill, tile, planned, wide, coop = tma_fill_bytes(name, n, h, w, k, cin, cout, sm_count)
                 assert planned == row["instance"], (name, planned, row["instance"])
-                row.update({"fill_bytes": fill, "fill_tbps": fill / (dur * 1e-6) / 1e12, "tile": tile, "tile256": wide})
+                row.update({"fill_bytes": fill, "fill_tbps": fill / (dur * 1e-6) / 1e12, "tile": tile, "tile256": wide,
+                            "coop_n": coop})
         rows.append(row)
     if matched:      # the plans above must agree with the launches the library counted
         predicted = sum(r.get("tile256", False) for r in rows)
         assert tile256_in_step == predicted, (tile256_in_step, predicted)
+        predicted = sum(r.get("coop_n", False) for r in rows)
+        assert coop_n_in_step == predicted, (coop_n_in_step, predicted)
 
     def total(sel):
         ms = sum(r["ms"] for r in sel)
@@ -213,6 +222,7 @@ def main():
     out = {
         "card": card, "workload": bench.workload_config(1)["workload"], "detector_input": [n_pages, hp, wp],
         "crops": crops, "matched_to_layers": matched, "tile256_launches_in_step": tile256_in_step,
+        "coop_n_launches_in_step": coop_n_in_step,
         "layer_flop_sum": sum(r.get("flop", 0.0) for r in rows), "kernel_flop_count": flop_d + flop_r,
         "layers": rows,
         "craft": total([r for r in rows if r.get("net") == "craft"]),
