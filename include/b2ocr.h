@@ -374,6 +374,40 @@ int b2o_ctc_beam_decode(b2o_ctx* ctx, const float* logits_dev, int b, int k, int
 int b2o_crnn_forward_beam(b2o_ctx* ctx, const void* crnn_in_dev, int b, int beam_width, int top_paths,
                           int32_t* labels_dev, float* logp_dev, void* ws_dev, size_t ws_bytes, void* stream);
 
+/* CTC prefix beam search ranked by a character n-gram language model (DESIGN.md section 1, "Language model").
+ * The device model, built on the host (recognition.CharLM.device_arrays): n_histories listed histories, each of
+ * length 0 .. order-1, as a sorted uint64 key array keys_dev, key = (length << 56) | the symbols packed 8 bits each,
+ * oldest in the highest byte, a label c as c and <s> as 127 (keys_dev[0] = 0, the empty history); rows_dev
+ * (n_histories, k) float32: column c < k-1 is log P(c | h) with the backoff folded in, column k-1 log P(</s> | h).
+ * A beam also carries G in float32: G(empty) = 0, G(a + c) = G(a) + (alpha * l(c | hist(a)) + beta), l the row value
+ * of the longest listed suffix of hist(a), the last order-1 symbols of "<s> a".  Candidates rank by F = A + G (one
+ * float32 rounding), A = the acoustic beam score of b2o_ctc_beam_decode; equal F by label sequence as there.  Each
+ * step a beam extends by its own shortlist, the min(beam_width + 1, k - 1) labels with the largest
+ * lp[t,c] + alpha * l(c | hist) (ties: smaller label).  The top_paths readings rank by F_end = F + alpha * l(</s> | hist).
+ * labels_dev (b, top_paths, 48) as b2o_ctc_beam_decode writes them; logp_dev (b, top_paths) float32 the acoustic A of
+ * each reading and fused_dev (b, top_paths) float32 its F_end (either NULL: not written).  With alpha = beta = 0 labels
+ * and logp equal b2o_ctc_beam_decode's bit for bit.  A crop's result is a function of its logits and the model alone.
+ * 2 <= order <= B2O_MAX_LM_ORDER, 1 <= n_histories <= B2O_MAX_LM_HISTORIES, finite alpha and beta, keys and rows not
+ * NULL, 2 <= k <= B2O_MAX_LM_CLASSES and the beam_width / top_paths rules of beam search, otherwise B2O_ERR_ARG.
+ * b2o_ctc_beam_lm_decode: the search alone on caller-supplied (b, 48, k) float32 logits.
+ * b2o_crnn_forward_beam_lm: the CRNN of b2o_crnn_forward, its fc_12 logits into the workspace, then the search.    */
+#define B2O_MAX_LM_ORDER 8
+#define B2O_MAX_LM_HISTORIES (1 << 20)
+#define B2O_MAX_LM_CLASSES 127
+typedef struct {
+  int order;
+  int n_histories;
+  const uint64_t* keys_dev;
+  const float* rows_dev;
+  float alpha;
+  float beta;
+} b2o_char_lm;
+int b2o_ctc_beam_lm_decode(b2o_ctx* ctx, const float* logits_dev, int b, int k, int beam_width, int top_paths,
+                           const b2o_char_lm* lm, int32_t* labels_dev, float* logp_dev, float* fused_dev, void* stream);
+int b2o_crnn_forward_beam_lm(b2o_ctx* ctx, const void* crnn_in_dev, int b, int beam_width, int top_paths,
+                             const b2o_char_lm* lm, int32_t* labels_dev, float* logp_dev, float* fused_dev, void* ws_dev,
+                             size_t ws_bytes, void* stream);
+
 /* Lexicon-constrained CTC decoding: the top_paths most probable entries of a caller's word list, per crop.
  * Inputs: the beam decoder's lp[t,c] = log(softmax(logits_t)_c + 1e-7) over the 48 kept steps, blank = k-1.
  * Lexicon: n_words entries in CSR form, offsets_dev (n_words + 1) int32 and the concatenated labels_dev int16; entry i

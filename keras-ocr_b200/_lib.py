@@ -18,6 +18,9 @@ MAX_BEAM_WIDTH = 128          # B2O_MAX_BEAM_WIDTH in include/b2ocr.h
 MAX_LEXICON_WORDS = 1 << 20   # B2O_MAX_LEXICON_WORDS
 MAX_LEXICON_LABELS = 1 << 24  # B2O_MAX_LEXICON_LABELS
 MAX_LEXICON_TOP_PATHS = 128   # B2O_MAX_LEXICON_TOP_PATHS
+MAX_LM_ORDER = 8              # B2O_MAX_LM_ORDER
+MAX_LM_HISTORIES = 1 << 20    # B2O_MAX_LM_HISTORIES
+MAX_LM_CLASSES = 127          # B2O_MAX_LM_CLASSES
 ROTATION_VOTE_WORD, ROTATION_VOTE_PAGE = 0, 1   # B2O_ROTATION_VOTE_WORD / _PAGE
 MAX_ALIGN_PATHS = 128         # B2O_MAX_ALIGN_PATHS
 CRAFT_LAST_STEP = 30          # B2O_CRAFT_LAST_STEP
@@ -64,6 +67,13 @@ class _ConvPlan(ctypes.Structure):
     _fields_ = [(name, _c.c_int32) for name in ("block_n", "kch", "mode", "pair", "upadd", "body", "tile_w", "tile_h",
                                                 "tile_n", "tiles", "stages", "stage_bytes", "stage_tx", "resident_bytes",
                                                 "smem_bytes", "grid", "coop_n")]
+
+class CharLMDesc(ctypes.Structure):
+    """b2o_char_lm (include/b2ocr.h), field for field."""
+    _fields_ = [("order", _i), ("n_histories", _i), ("keys_dev", _vp), ("rows_dev", _vp), ("alpha", _f), ("beta", _f)]
+
+
+_lmp = _c.POINTER(CharLMDesc)
 
 # name -> (restype, argtypes); mirrors include/b2ocr.h one to one
 SIGNATURES = {
@@ -120,6 +130,8 @@ SIGNATURES = {
     "b2o_crnn_forward_scored": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_ctc_beam_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "b2o_crnn_forward_beam": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_ctc_beam_lm_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _lmp, _vp, _vp, _vp, _vp]),
+    "b2o_crnn_forward_beam_lm": (_i, [_vp, _vp, _i, _i, _i, _lmp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2o_lexicon_workspace_bytes": (_sz, [_i, _i, _i]),
     "b2o_ctc_lexicon_decode": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_crnn_forward_lexicon": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
@@ -423,6 +435,16 @@ class Context:
     def crnn_forward_beam(self, crnn_in, b, beam_width, top_paths, labels, logp, ws, ws_bytes, stream):
         self._check(self.lib.b2o_crnn_forward_beam(self.handle, crnn_in, b, beam_width, top_paths, labels, logp, ws,
                                                    ws_bytes, stream), "b2o_crnn_forward_beam")
+
+    def ctc_beam_lm_decode(self, logits, b, k, beam_width, top_paths, lm, labels, logp, fused, stream):
+        """``lm``: a ``CharLMDesc``."""
+        self._check(self.lib.b2o_ctc_beam_lm_decode(self.handle, logits, b, k, beam_width, top_paths, ctypes.byref(lm),
+                                                    labels, logp, fused, stream), "b2o_ctc_beam_lm_decode")
+
+    def crnn_forward_beam_lm(self, crnn_in, b, beam_width, top_paths, lm, labels, logp, fused, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_crnn_forward_beam_lm(self.handle, crnn_in, b, beam_width, top_paths, ctypes.byref(lm),
+                                                      labels, logp, fused, ws, ws_bytes, stream),
+                    "b2o_crnn_forward_beam_lm")
 
     def lexicon_workspace_bytes(self, b, n_words, top_paths):
         return int(self.lib.b2o_lexicon_workspace_bytes(b, n_words, top_paths))

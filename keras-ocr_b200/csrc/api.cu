@@ -4,6 +4,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <functional>
 
 #include "common.cuh"
@@ -17,6 +18,8 @@ int add_run(b2o_ctx* ctx, const __half* a, const __half* b, __half* o, long long
 int fc_ctc_run(b2o_ctx* ctx, const __half* l2, int B, float* logits, int* labels, float* logp, cudaStream_t st);
 int ctc_beam_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths, int* labels, float* logp,
                  cudaStream_t st);
+int ctc_beam_lm_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
+                    const b2o_char_lm* lm, int* labels, float* logp, float* fused, cudaStream_t st);
 size_t ctc_lexicon_workspace_bytes(int B, int n_words);
 int ctc_lexicon_run(b2o_ctx* ctx, const float* logits, int B, int K, const int* offsets, const short* labels,
                     int n_words, int top_paths, int* labels_out, float* logp, void* ws, cudaStream_t st);
@@ -862,6 +865,56 @@ extern "C" int b2o_ctc_beam_decode(b2o_ctx* ctx, const float* logits, int b, int
   if (b < 0 || (b > 0 && (!logits || !labels))) { ctx->set_error("b2o_ctc_beam_decode: bad argument"); return B2O_ERR_ARG; }
   DeviceGuard guard(ctx->device);
   return ctc_beam_run(ctx, logits, b, k, beam_width, top_paths, labels, logp, reinterpret_cast<cudaStream_t>(stream));
+}
+
+namespace {
+
+bool lm_args_ok(b2o_ctx* ctx, const char* fn, int k, int beam_width, int top_paths, const b2o_char_lm* lm) {
+  if (!beam_args_ok(ctx, fn, k, beam_width, top_paths)) return false;
+  if (k > B2O_MAX_LM_CLASSES) { ctx->set_error(std::string(fn) + ": k must be in [2, 127]"); return false; }
+  if (!lm || !lm->keys_dev || !lm->rows_dev) { ctx->set_error(std::string(fn) + ": no language model"); return false; }
+  if (lm->order < 2 || lm->order > B2O_MAX_LM_ORDER) {
+    ctx->set_error(std::string(fn) + ": order must be in [2, 8]");
+    return false;
+  }
+  if (lm->n_histories < 1 || lm->n_histories > B2O_MAX_LM_HISTORIES) {
+    ctx->set_error(std::string(fn) + ": n_histories must be in [1, 2^20]");
+    return false;
+  }
+  if (!std::isfinite(lm->alpha) || !std::isfinite(lm->beta)) {
+    ctx->set_error(std::string(fn) + ": alpha and beta must be finite");
+    return false;
+  }
+  return true;
+}
+
+}  // namespace
+
+extern "C" int b2o_crnn_forward_beam_lm(b2o_ctx* ctx, const void* crnn_in, int b, int beam_width, int top_paths,
+                                        const b2o_char_lm* lm, int32_t* labels, float* logp, float* fused, void* ws,
+                                        size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_forward_beam_lm: CRNN weights not loaded"); return B2O_ERR_STATE; }
+  if (!lm_args_ok(ctx, "b2o_crnn_forward_beam_lm", ctx->n_classes, beam_width, top_paths, lm)) return B2O_ERR_ARG;
+  if (b == 0) return B2O_OK;
+  B2O_RETURN_IF(crnn_forward(ctx, crnn_in, b, labels, nullptr, true, ws, ws_bytes, stream));
+  DeviceGuard guard(ctx->device);
+  const float* logits = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(ws) + plan_crnn(b).off[rb::logits]);
+  return ctc_beam_lm_run(ctx, logits, b, ctx->n_classes, beam_width, top_paths, lm, labels, logp, fused,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2o_ctc_beam_lm_decode(b2o_ctx* ctx, const float* logits, int b, int k, int beam_width, int top_paths,
+                                      const b2o_char_lm* lm, int32_t* labels, float* logp, float* fused, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!lm_args_ok(ctx, "b2o_ctc_beam_lm_decode", k, beam_width, top_paths, lm)) return B2O_ERR_ARG;
+  if (b < 0 || (b > 0 && (!logits || !labels))) {
+    ctx->set_error("b2o_ctc_beam_lm_decode: bad argument");
+    return B2O_ERR_ARG;
+  }
+  DeviceGuard guard(ctx->device);
+  return ctc_beam_lm_run(ctx, logits, b, k, beam_width, top_paths, lm, labels, logp, fused,
+                         reinterpret_cast<cudaStream_t>(stream));
 }
 
 namespace {

@@ -403,7 +403,359 @@ ctc_beam_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W, i
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// ctc_beam_lm_kernel: the same search ranked by a character language model (DESIGN.md section 1, "Language model").
+//   A beam also carries G(a) in fp32: G(empty) = 0, G(a + c) = G(a) + (alpha * l(c | hist(a)) + beta), hist(a) the last
+//   order-1 symbols of "<s> a" and l the fp32 row value of its longest listed suffix.  Candidates are ranked by
+//   F = A + G (rounded once), A = logaddexp(p_b, p_nb) the acoustic score; G is a function of the prefix, so merging
+//   equal prefixes is unchanged.  After the last step F_end = F + alpha * l(</s> | hist) ranks the returned paths.
+// Per step, besides steps 1-6 above:
+//   2'. the shortlist is per beam: the S = min(W+1, K-1) labels with the largest lp[c] + alpha * l(c | hist(a)) (ties:
+//       smaller label first), one warp per beam (a 32-round bitwise radix select over the order-preserving keys);
+//   6'. a beam whose history changed (an extension) looks up its row once: the longest listed suffix of its history by
+//       binary search over the sorted keys (at most order-1 searches), then reads K floats of that row per use from
+//       global memory (L2-resident).  A beam kept via blank or its last label keeps its parent's row.
+// Why the per-beam shortlist loses nothing: let c be outside a's shortlist and a+c not a beam.  The only candidate that
+// yields a+c is a's extension by c: F(a+c) = (c == last(a) ? p_b(a) : A(a)) + lp[c] + G(a) + alpha l(c | hist(a)) + beta.
+// S = W+1 labels c' rank above c in lp[c'] + alpha l(c' | hist(a)); at most one of them is last(a), so at least W of
+// them give a+c' an F >= A(a) + lp[c'] + G(a) + alpha l(c' | hist(a)) + beta >= F(a+c) (p_b <= A, merging only adds,
+// and F is monotone in A), and each of those W prefixes beats a+c or ties and precedes it.  In fp32 the three sums are
+// split differently from the shortlist key, so two candidates within a few ulps of F can be ordered differently from
+// exact arithmetic: a near-tie, which tests/test_gpu_lm.py counts and bounds.
+// With alpha = beta = 0 every alpha * l is +-0, so the shortlist key is lp, G = +0, F = A and F_end = A bit for bit: the
+// per-beam shortlists equal the global one and the search returns ctc_beam_kernel's labels and scores exactly.
+constexpr unsigned kLmBos = 127u;                 // the code of <s> in a packed history (labels are < 126)
+
+struct SmemLm {
+  short* shl;                      // [W][S] per-beam shortlist, ascending labels
+  float *g[2], *f[2];              // [W] G and F of each beam
+  int* row[2];                     // [W] the beam's LM row
+  unsigned char* chg;              // [W] the beam's history changed this step
+};
+
+__host__ __device__ inline size_t smem_plan_lm(int W, int K, unsigned char* base, Smem* s, SmemLm* l) {
+  size_t off = smem_plan(W, K, base, s);
+  const int S = shortlist_size(W, K);
+  SmemLm d;
+  SmemLm* p = l ? l : &d;
+#define B2O_TAKE(ptr, type, count)                                                    \
+  do {                                                                                \
+    if (base) (ptr) = reinterpret_cast<type*>(base + off);                            \
+    off += (static_cast<size_t>(count) * sizeof(type) + 15) / 16 * 16;                \
+  } while (0)
+  B2O_TAKE(p->shl, short, W * S);
+  for (int i = 0; i < 2; ++i) {
+    B2O_TAKE(p->g[i], float, W);
+    B2O_TAKE(p->f[i], float, W);
+    B2O_TAKE(p->row[i], int, W);
+  }
+  B2O_TAKE(p->chg, unsigned char, W);
+#undef B2O_TAKE
+  return off;
+}
+
+// The row of the longest listed suffix of the history of "<s> pre[0..L)": keys sorted ascending, (n << 56) | the n
+// symbols packed 8 bits each, oldest highest; keys[0] = 0 is the empty history.
+__device__ int lm_row(const unsigned long long* __restrict__ keys, int H, int order, const short* pre, int L) {
+  const int top = min(order - 1, L + 1);
+  for (int n = top; n >= 1; --n) {
+    unsigned long long k = static_cast<unsigned long long>(n) << 56;
+    for (int i = 0; i < n; ++i) {
+      const int p = L + 1 - n + i;                // position in "<s> a"
+      const unsigned sym = p == 0 ? kLmBos : static_cast<unsigned>(pre[p - 1]);
+      k |= static_cast<unsigned long long>(sym) << (8 * (n - 1 - i));
+    }
+    int lo = 0, hi = H;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (__ldg(keys + mid) < k) lo = mid + 1; else hi = mid;
+    }
+    if (lo < H && __ldg(keys + lo) == k) return lo;
+  }
+  return 0;
+}
+
+// One warp: the S labels c < n with the largest lp[c] + alpha * lrow[c] (ties: smaller label), ascending, into out[S].
+__device__ void lm_shortlist(const float* lp, const float* __restrict__ lrow, float alpha, int n, int S, short* out) {
+  const int lane = threadIdx.x & 31;
+  const unsigned lt = (1u << lane) - 1u;
+  unsigned kv[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int c = lane + 32 * i;
+    kv[i] = c < n ? okey(__fadd_rn(lp[c], __fmul_rn(alpha, __ldg(lrow + c)))) : 0u;
+  }
+  unsigned theta = 0;
+  int take = 0;
+  if (S < n) {
+    for (int bit = 31; bit >= 0; --bit) {         // the largest theta with at least S keys >= theta: the S-th key
+      const unsigned t = theta | (1u << bit);
+      int cnt = 0;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) cnt += kv[i] >= t;
+      if (__reduce_add_sync(0xffffffffu, cnt) >= S) theta = t;
+    }
+    int gt = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) gt += kv[i] > theta;
+    take = S - __reduce_add_sync(0xffffffffu, gt);
+  }
+  int at = 0, eq_before = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int c = lane + 32 * i;
+    const bool eq = S < n && kv[i] == theta && c < n;
+    const unsigned eqm = __ballot_sync(0xffffffffu, eq);
+    const bool in = c < n && (S == n || kv[i] > theta || (eq && eq_before + __popc(eqm & lt) < take));
+    const unsigned m = __ballot_sync(0xffffffffu, in);
+    if (in) out[at + __popc(m & lt)] = static_cast<short>(c);
+    at += __popc(m);
+    eq_before += __popc(eqm);
+  }
+}
+
+struct LmOrder {                                  // candidate label sequences with per-beam shortlists
+  const Smem& s;
+  const short* shl;
+  int cur, S, S1;
+  __device__ int at(int i, int t) const {
+    const int a = i / S1, x = i - a * S1;
+    return t < s.len[cur][a] ? s.pre[cur][a * kT + t] : shl[a * S + x - 1];
+  }
+  __device__ int clen(int i) const { const int a = i / S1; return s.len[cur][a] + (i - a * S1 > 0); }
+  __device__ bool lex_less(int i, int j) const {
+    const int li = clen(i), lj = clen(j), n = li < lj ? li : lj;
+    for (int t = 0; t < n; ++t) {
+      const int u = at(i, t), v = at(j, t);
+      if (u != v) return u < v;
+    }
+    return li < lj;
+  }
+};
+
+__global__ void __launch_bounds__(kThreads)
+ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W, int P,
+                   const unsigned long long* __restrict__ lm_keys /*[H]*/, const float* __restrict__ lm_rows /*[H][K]*/,
+                   int H, int order, float alpha, float beta, int* __restrict__ labels /*[B][P][48]*/,
+                   float* __restrict__ logp /*[B][P] or null*/, float* __restrict__ fused /*[B][P] or null*/) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  Smem s;
+  SmemLm l;
+  smem_plan_lm(W, K, smem_raw, &s, &l);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int blank = K - 1, S = shortlist_size(W, K), S1 = S + 1;
+  int cur = 0, nb = 1;
+  if (tid == 0) {
+    s.len[0][0] = 0; s.pb[0][0] = 0.f; s.pnb[0][0] = -INFINITY; s.sc[0][0] = 0.f;
+    s.h[0][0] = kHashRoot; s.ph[0][0] = 0;
+    l.g[0][0] = 0.f; l.f[0][0] = 0.f;
+    l.row[0][0] = lm_row(lm_keys, H, order, s.pre[0], 0);
+  }
+  for (int t = 0; t < kT; ++t) {
+    // ---- 1. lp of step t (as ctc_beam_kernel)
+    const float* row = logits + (static_cast<size_t>(blockIdx.x) * kT + t) * K;
+    float m = -INFINITY;
+    for (int c = tid; c < K; c += kThreads) { const float v = row[c]; s.lp[c] = v; m = fmaxf(m, v); }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float* redf = reinterpret_cast<float*>(s.red);
+    if (lane == 0) redf[warp] = m;
+    __syncthreads();
+    m = redf[0];
+    for (int w = 1; w < kWarps; ++w) m = fmaxf(m, redf[w]);
+    float se = 0.f;
+    for (int c = tid; c < K; c += kThreads) se = __fadd_rn(se, expf(__fsub_rn(s.lp[c], m)));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) se = __fadd_rn(se, __shfl_xor_sync(0xffffffffu, se, o));
+    __syncthreads();
+    if (lane == 0) redf[warp] = se;
+    __syncthreads();
+    se = redf[0];
+    for (int w = 1; w < kWarps; ++w) se = __fadd_rn(se, redf[w]);
+    for (int c = tid; c < K; c += kThreads)
+      s.lp[c] = logf(__fadd_rn(__fdiv_rn(expf(__fsub_rn(s.lp[c], m)), se), 1e-7f));
+    __syncthreads();
+
+    // ---- 2'. per-beam shortlists, one warp per beam
+    for (int a = warp; a < nb; a += kWarps)
+      lm_shortlist(s.lp, lm_rows + static_cast<size_t>(l.row[cur][a]) * K, alpha, K - 1, S, l.shl + a * S);
+
+    // ---- 3. parent links and the extensions that are already beams
+    const Beams bm{s, cur, S1};
+    const LmOrder ord{s, l.shl, cur, S, S1};
+    for (int i = tid; i < nb * S; i += kThreads) s.excl[i] = 0;
+    if (tid < nb) {
+      int par = -1;
+      const int len = s.len[cur][tid];
+      if (len > 0)
+        for (int a = 0; a < nb && par < 0; ++a) {
+          if (s.len[cur][a] != len - 1 || s.h[cur][a] != s.ph[cur][tid]) continue;
+          bool same = true;
+          for (int u = 0; u < len - 1 && same; ++u) same = s.pre[cur][a * kT + u] == s.pre[cur][tid * kT + u];
+          if (same) par = a;
+        }
+      s.parent[tid] = par;
+    }
+    __syncthreads();
+    if (tid < nb && s.parent[tid] >= 0) {          // last(tid) in its parent's shortlist (ascending): binary search
+      const short* sl = l.shl + s.parent[tid] * S;
+      const int c = bm.last(tid);
+      int lo = 0, hi = S;
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (sl[mid] < c) lo = mid + 1; else hi = mid; }
+      if (lo < S && sl[lo] == c) s.excl[s.parent[tid] * S + lo] = 1;
+    }
+    __syncthreads();
+
+    // ---- 4. candidate keys: F = A + G
+    auto candidate = [&](int i, float* pb, float* pnb, float* g) {
+      const int a = i / S1, x = i - a * S1;
+      if (x == 0) {
+        bm.eval(i, blank, pb, pnb);
+        *g = l.g[cur][a];
+      } else {
+        const int c = l.shl[a * S + x - 1];
+        *pb = -INFINITY;
+        *pnb = bm.ext(a, c);
+        const float lv = __ldg(lm_rows + static_cast<size_t>(l.row[cur][a]) * K + c);
+        *g = __fadd_rn(l.g[cur][a], __fadd_rn(__fmul_rn(alpha, lv), beta));
+      }
+    };
+    const int n = nb * S1;
+    int valid = 0;
+    for (int i = tid; i < n; i += kThreads) {
+      const int a = i / S1, x = i - a * S1;
+      unsigned k = 0;
+      if (x == 0 || !s.excl[a * S + x - 1]) {
+        float pb, pnb, g;
+        candidate(i, &pb, &pnb, &g);
+        k = okey(__fadd_rn(lae(pb, pnb), g));
+        ++valid;
+      }
+      s.key[i] = k;
+      s.sel[i] = 0;
+    }
+    int nvalid;
+    block_scan(valid, s.red, &nvalid);
+
+    // ---- 5. the W best (as ctc_beam_kernel, the tie order over per-beam shortlists)
+    if (nvalid <= W) {
+      for (int i = tid; i < n; i += kThreads) s.sel[i] = s.key[i] != 0;
+    } else {
+      int take, equal;
+      const unsigned theta = radix_select(n, W, [&](int i) { return s.key[i]; }, s.hist, s.red, &take, &equal);
+      for (int i = tid; i < n; i += kThreads) s.sel[i] = s.key[i] > theta || (take == equal && s.key[i] == theta);
+      __syncthreads();
+      for (int r = 0; r < take && take < equal; ++r) {
+        int best = -1;
+        for (int i = tid; i < n; i += kThreads)
+          if (s.key[i] == theta && !s.sel[i] && (best < 0 || ord.lex_less(i, best))) best = i;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const int other = __shfl_xor_sync(0xffffffffu, best, o);
+          if (other >= 0 && (best < 0 || ord.lex_less(other, best))) best = other;
+        }
+        if (lane == 0) s.red[warp] = best;
+        __syncthreads();
+        if (tid == 0) {
+          int b = -1;
+          for (int w = 0; w < kWarps; ++w) {
+            const int o = s.red[w];
+            if (o >= 0 && (b < 0 || ord.lex_less(o, b))) b = o;
+          }
+          s.sel[b] = 1;
+        }
+        __syncthreads();
+      }
+    }
+    __syncthreads();
+
+    // ---- 6. compaction in candidate order into the other buffer; 6'. new histories look up their row
+    {
+      const int chunk = (n + kThreads - 1) / kThreads, i0 = min(n, tid * chunk), i1 = min(n, i0 + chunk);
+      int cnt = 0;
+      for (int i = i0; i < i1; ++i) cnt += s.sel[i];
+      int total;
+      int slot = block_scan(cnt, s.red, &total);
+      const int nx = cur ^ 1;
+      for (int i = i0; i < i1; ++i) {
+        if (!s.sel[i]) continue;
+        const int a = i / S1, x = i - a * S1, len = s.len[cur][a];
+        float pb, pnb, g;
+        candidate(i, &pb, &pnb, &g);
+        for (int u = 0; u < len; ++u) s.pre[nx][slot * kT + u] = s.pre[cur][a * kT + u];
+        if (x > 0) {
+          const int c = l.shl[a * S + x - 1];
+          s.pre[nx][slot * kT + len] = static_cast<short>(c);
+          s.h[nx][slot] = s.h[cur][a] * kHashMul + static_cast<unsigned long long>(c + 1);
+          s.ph[nx][slot] = s.h[cur][a];
+        } else {
+          s.h[nx][slot] = s.h[cur][a];
+          s.ph[nx][slot] = s.ph[cur][a];
+          l.row[nx][slot] = l.row[cur][a];
+        }
+        l.chg[slot] = x > 0;
+        s.len[nx][slot] = len + (x > 0);
+        s.pb[nx][slot] = pb;
+        s.pnb[nx][slot] = pnb;
+        s.sc[nx][slot] = lae(pb, pnb);
+        l.g[nx][slot] = g;
+        l.f[nx][slot] = unokey(s.key[i]);         // the selection key's F, bit for bit
+        ++slot;
+      }
+      nb = total;
+      cur = nx;
+      __syncthreads();
+      if (tid < nb && l.chg[tid]) l.row[cur][tid] = lm_row(lm_keys, H, order, s.pre[cur] + tid * kT, s.len[cur][tid]);
+      __syncthreads();
+    }
+  }
+
+  // ---- the P best of the final beams by F_end, best first
+  const Beams fin{s, cur, 1};
+  const int b = blockIdx.x;
+  float* fend = l.g[cur ^ 1];                      // free: the other buffer's G
+  if (tid < nb)
+    fend[tid] = __fadd_rn(l.f[cur][tid],
+                          __fmul_rn(alpha, __ldg(lm_rows + static_cast<size_t>(l.row[cur][tid]) * K + blank)));
+  __syncthreads();
+  if (tid < nb) {
+    const unsigned k = okey(fend[tid]);
+    int rank = 0;
+    for (int a = 0; a < nb; ++a) {
+      const unsigned ka = okey(fend[a]);
+      rank += ka > k || (ka == k && a != tid && fin.lex_less(a, tid));
+    }
+    if (rank < P) {
+      int* o = labels + (static_cast<size_t>(b) * P + rank) * kT;
+      const int len = s.len[cur][tid];
+      for (int u = 0; u < kT; ++u) o[u] = u < len ? s.pre[cur][tid * kT + u] : -1;
+      if (logp) logp[static_cast<size_t>(b) * P + rank] = s.sc[cur][tid];
+      if (fused) fused[static_cast<size_t>(b) * P + rank] = fend[tid];
+    }
+  }
+  for (int r = nb + tid; r < P; r += kThreads) {
+    int* o = labels + (static_cast<size_t>(b) * P + r) * kT;
+    for (int u = 0; u < kT; ++u) o[u] = -1;
+    if (logp) logp[static_cast<size_t>(b) * P + r] = -INFINITY;
+    if (fused) fused[static_cast<size_t>(b) * P + r] = -INFINITY;
+  }
+}
+
 }  // namespace
+
+int ctc_beam_lm_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
+                    const b2o_char_lm* lm, int* labels, float* logp, float* fused, cudaStream_t st) {
+  if (B <= 0) return B2O_OK;
+  const size_t bytes = smem_plan_lm(beam_width, K, nullptr, nullptr, nullptr);
+  B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(ctc_beam_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           static_cast<int>(bytes)));
+  ctc_beam_lm_kernel<<<B, kThreads, bytes, st>>>(logits, K, beam_width, top_paths,
+                                                 reinterpret_cast<const unsigned long long*>(lm->keys_dev),
+                                                 lm->rows_dev, lm->n_histories, lm->order, lm->alpha, lm->beta, labels,
+                                                 logp, fused);
+  B2O_LAUNCH_CHECK(ctx);
+  return B2O_OK;
+}
 
 int ctc_beam_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths, int* labels, float* logp,
                  cudaStream_t st) {

@@ -132,7 +132,7 @@ def _host_records(pipeline, local, per_rank, max_boxes):
 
 
 def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_scores=False, beam_width=None,
-                      top_paths=1, lexicon=None, rotations=None, rotation_vote="word"):
+                      top_paths=1, lexicon=None, rotations=None, rotation_vote="word", language_model=None):
     """Run ``pipeline.recognize`` on this rank's shard of ``images`` and gather to rank 0.
 
     ``images`` is the global batch (every rank passes the same list and takes its contiguous slice) or, with
@@ -149,13 +149,16 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
     (``recognition.check_beam``); records carry the best path only, so ``top_paths`` > 1 raises ``ValueError``.
     ``lexicon``: every word reads as the most probable entry of that word list (``recognition.check_decoder``); a
     ``recognition.Lexicon`` is compiled once and uploaded once per device, a plain list is compiled here.
+    ``language_model``: a ``recognition.CharLM`` that ranks the beam search (with ``beam_width``); uploaded once per
+    device.
     ``rotations`` / ``rotation_vote``: every word is read in each listed quarter turn and the most probable reading kept
     (``recognition.check_rotations``); boxes start at the chosen turn's corner, as ``Pipeline.recognize`` returns them.
     """
     from .pipeline import check_records_decoder
     from .recognition import check_rotations
     lexicon = check_records_decoder(beam_width, top_paths, lexicon,
-                                    None if lexicon is None else pipeline.recognizer.alphabet)
+                                    None if lexicon is None and language_model is None else pipeline.recognizer.alphabet,
+                                    language_model)
     rotations = check_rotations(rotations, rotation_vote)
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
@@ -176,6 +179,8 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
         sk["beam_width"] = beam_width
     if lexicon is not None:
         sk["lexicon"] = lexicon
+    if language_model is not None:
+        sk["language_model"] = language_model
     if rotations is not None:
         sk["rotations"], sk["rotation_vote"] = rotations, rotation_vote
     if native:
@@ -271,14 +276,15 @@ class ShardedStream:
     ``max_boxes``: words a record holds (an image with more raises ``RecordOverflow`` on rank 0 when its batch is
     decoded) or ``"auto"`` (sized per batch by ``agree_max_boxes``).  ``return_scores=True``: words as
     ``recognize_sharded(return_scores=True)`` returns them (device records only).  ``beam_width`` / ``lexicon`` /
-    ``rotations`` / ``rotation_vote``: as ``recognize_sharded``."""
+    ``rotations`` / ``rotation_vote`` / ``language_model``: as ``recognize_sharded``."""
 
     def __init__(self, pipeline, max_boxes=128, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                 rotations=None, rotation_vote="word"):
+                 rotations=None, rotation_vote="word", language_model=None):
         from .pipeline import check_records_decoder
         from .recognition import check_rotations
+        plain = lexicon is None and language_model is None
         lexicon = check_records_decoder(beam_width, top_paths, lexicon,
-                                        None if lexicon is None else pipeline.recognizer.alphabet)
+                                        None if plain else pipeline.recognizer.alphabet, language_model)
         rotations = check_rotations(rotations, rotation_vote)
         self.pipeline, self.max_boxes = pipeline, max_boxes
         self.world = dist.get_world_size() if dist.is_initialized() else 1
@@ -294,7 +300,7 @@ class ShardedStream:
         self._sk = {"scores": True} if return_scores else {}
         self._rk = {}
         rot = (("rotations", rotations), ("rotation_vote", rotation_vote)) if rotations is not None else ()
-        for k, v in (("beam_width", beam_width), ("lexicon", lexicon)) + rot:
+        for k, v in (("beam_width", beam_width), ("lexicon", lexicon), ("language_model", language_model)) + rot:
             if v is not None:
                 self._sk[k] = v
                 self._rk.setdefault("recognition_kwargs", {})[k] = v

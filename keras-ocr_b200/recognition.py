@@ -1,4 +1,5 @@
 """Recognizer: drop-in for ``keras_ocr.recognition.Recognizer`` (reference recognition.py:353-537)."""
+import math
 import string
 import typing
 
@@ -149,10 +150,337 @@ class Lexicon:
         return self._device[device]
 
 
-def check_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET):
+LM_BOS = 127                  # the code of <s> in a history (labels are < 126); </s> is label len(alphabet), the blank's
+_LN10 = math.log(10.0)
+
+
+class CharLM:
+    """A character n-gram language model for CTC beam search (``b2o_crnn_forward_beam_lm``; DESIGN.md section 1,
+    "Language model").  Symbols are the alphabet's labels, ``</s>`` (end of word) and ``<s>`` (start of word, only in
+    histories); a word is the sentence ``<s> w </s>``.  A backoff model of order 2 <= N <= 8 with ARPA semantics:
+    log P(w | h) = log P*(w | h) when (h, w) is listed, otherwise bo(h) + log P(w | h without its oldest symbol), bo(h) =
+    0 for an unlisted h.  The tables are kept as ARPA stores them, in log10 (``logp10``, ``backoff10``: {tuple of
+    symbols: value}, ``<s>`` = ``LM_BOS``, ``</s>`` = len(alphabet)), so ``to_arpa`` / ``from_arpa`` round-trip exactly;
+    every score the package computes from them is a natural log.
+
+    ``alpha`` (the weight of the model's log-probabilities) and ``beta`` (a bonus per character) are fixed at
+    construction; ``weighted`` returns a copy with others that shares the tables.  The device form is uploaded lazily,
+    once per CUDA device (``device_arrays``)."""
+
+    ALPHA, BETA = 1.0, 2.0       # picked by scripts/bench_lm.py's sweep on its tuning pages (DESIGN.md section 5)
+
+    def __init__(self, alphabet, order, logp10, backoff10, alpha=ALPHA, beta=BETA):
+        if len(alphabet) > _lib.MAX_LM_CLASSES - 1:
+            raise ValueError(f"a language model takes at most {_lib.MAX_LM_CLASSES - 1} alphabet characters, "
+                             f"got {len(alphabet)}")
+        if len(set(alphabet)) != len(alphabet):
+            raise ValueError("the alphabet has repeated characters")
+        if not 2 <= order <= _lib.MAX_LM_ORDER:
+            raise ValueError(f"the order must be in [2, {_lib.MAX_LM_ORDER}], got {order}")
+        eos = len(alphabet)
+        missing = [s for s in range(eos + 1) if (s,) not in logp10]
+        if missing:
+            raise ValueError(f"no unigram for {self._token(alphabet, missing[0])!r}")
+        self.alphabet, self.order = alphabet, int(order)
+        self.logp10, self.backoff10 = logp10, backoff10
+        self._histories = sorted(g for g in logp10 if len(g) < order and eos not in g)
+        if len(self._histories) + 1 > _lib.MAX_LM_HISTORIES:
+            raise ValueError(f"the model lists {len(self._histories) + 1} histories; at most {_lib.MAX_LM_HISTORIES} "
+                             "are supported")
+        self._check_weights(alpha, beta)
+        self.alpha, self.beta = float(alpha), float(beta)
+        self._tables = {}                 # shared by weighted copies: the host device form and its uploads per device
+
+    @staticmethod
+    def _check_weights(alpha, beta):
+        for name, v in (("alpha", alpha), ("beta", beta)):
+            ok = not isinstance(v, (bool, np.bool_)) and isinstance(v, (int, float, np.integer, np.floating))
+            if ok:
+                with np.errstate(over="ignore"):
+                    ok = math.isfinite(float(np.float32(v)))         # the device takes them as float32
+            if not ok:
+                raise ValueError(f"{name} must be a number finite in float32, got {v!r}")
+
+    @staticmethod
+    def _token(alphabet, s):
+        return "<s>" if s == LM_BOS else "</s>" if s == len(alphabet) else alphabet[s]
+
+    def weighted(self, alpha=ALPHA, beta=BETA):
+        """A copy with weights ``alpha`` and ``beta`` that shares this model's tables and device uploads."""
+        self._check_weights(alpha, beta)
+        other = object.__new__(CharLM)
+        other.__dict__.update(self.__dict__)
+        other.alpha, other.beta = float(alpha), float(beta)
+        return other
+
+    # ------------------------------------------------------------------ fitting
+    @classmethod
+    def fit(cls, words, alphabet=DEFAULT_ALPHABET, order=5, counts=None):
+        """Interpolated Kneser-Ney of order ``order`` on ``words`` (checked as lexicon entries are; ``counts``: an
+        optional positive int per word, its multiplicity).  One discount per order, D_n = n1 / (n1 + 2 n2) over that
+        order's adjusted counts (0.5 when n1 or n2 is 0); the highest order and n-grams that begin with <s> count
+        occurrences, the other orders continuation counts (distinct left neighbours); the unigrams interpolate with the
+        uniform distribution over the alphabet and </s>.  Written in backoff form: P* = (c - D) / c(h) + gamma(h)
+        P(w | h'), bo(h) = gamma(h).  fp64 with sorted iteration: the same input gives the same tables bit for bit."""
+        if isinstance(words, str) or not isinstance(words, (list, tuple)):
+            raise ValueError("words must be a list or tuple of strings")
+        if not words:
+            raise ValueError("there are no words")
+        if not isinstance(order, (int, np.integer)) or isinstance(order, (bool, np.bool_)) \
+                or not 2 <= order <= _lib.MAX_LM_ORDER:
+            raise ValueError(f"the order must be an int in [2, {_lib.MAX_LM_ORDER}], got {order!r}")
+        if len(alphabet) > _lib.MAX_LM_CLASSES - 1:
+            raise ValueError(f"a language model takes at most {_lib.MAX_LM_CLASSES - 1} alphabet characters, "
+                             f"got {len(alphabet)}")
+        if counts is None:
+            counts = [1] * len(words)
+        if len(counts) != len(words) or any(isinstance(c, (bool, np.bool_)) or not isinstance(c, (int, np.integer))
+                                            or c < 1 for c in counts):
+            raise ValueError("counts must hold one positive int per word")
+        index = {ch: i for i, ch in enumerate(alphabet)}
+        for i, w in enumerate(words):
+            _check_word(i, w, index, "word")
+        n, eos = int(order), len(alphabet)
+        raw = [None] + [dict() for _ in range(n)]          # raw[m][gram]: occurrences of the m-gram
+        for w, c in zip(words, counts):
+            seq = (LM_BOS,) + tuple(index[ch] for ch in w) + (eos,)
+            for m in range(1, n + 1):
+                table = raw[m]
+                for i in range(len(seq) - m + 1):
+                    g = seq[i:i + m]
+                    table[g] = table.get(g, 0) + int(c)
+        adj = [None] * (n + 1)                             # adjusted counts
+        adj[n] = raw[n]
+        for m in range(n - 1, 0, -1):
+            left = {}
+            for g in raw[m + 1]:
+                left[g[1:]] = left.get(g[1:], 0) + 1
+            adj[m] = {g: (c if g[0] == LM_BOS else left[g]) for g, c in raw[m].items()}
+        adj[1].pop((LM_BOS,), None)                         # <s> is never predicted
+        logp10, backoff10 = {}, {}
+        prob = {}                                           # interpolated P(w | h) of listed (h, w), fp64
+        vocab = eos + 1
+
+        def lower(g):                                       # P(g[-1] | g[:-1]) by the backoff recursion, fp64
+            if g in prob:
+                return prob[g]
+            return gamma.get(g[:-1], 1.0) * lower(g[1:])
+
+        gamma = {}
+        for m in range(1, n + 1):
+            values = list(adj[m].values())
+            n1, n2 = values.count(1), values.count(2)
+            d = n1 / (n1 + 2.0 * n2) if n1 and n2 else 0.5
+            by_h = {}
+            for g in sorted(adj[m]):
+                by_h.setdefault(g[:-1], []).append(g)
+            for h in sorted(by_h):
+                grams = by_h[h]
+                total = float(sum(adj[m][g] for g in grams))
+                gam = d * len(grams) / total
+                if m == 1:
+                    for s in range(vocab):
+                        a = adj[1].get((s,), 0)
+                        prob[(s,)] = max(a - d, 0.0) / total + gam / vocab
+                else:
+                    gamma[h] = gam
+                    for g in grams:
+                        prob[g] = (adj[m][g] - d) / total + gam * lower(g[1:])
+        for g in sorted(prob):
+            logp10[g] = math.log10(prob[g])
+        logp10[(LM_BOS,)] = -99.0
+        for h in sorted(gamma):
+            backoff10[h] = math.log10(gamma[h])
+        return cls(alphabet, n, logp10, backoff10)
+
+    # ------------------------------------------------------------------ ARPA
+    @classmethod
+    def from_arpa(cls, path_or_text, alphabet=DEFAULT_ALPHABET):
+        """A model from an ARPA file (a path, or the file's text): n-grams with <unk> are dropped; any other token
+        outside the alphabet, <s> and </s>, a missing unigram, an order outside [2, 8], an n-gram whose history is not
+        listed or a malformed line raise ``ValueError`` naming the line; so does a file whose sections do not hold the
+        n-gram counts its header declares (<unk> lines included), or that lacks \\end\\, as a truncated file does.
+        The alphabet may not contain whitespace (ARPA tokens are whitespace-separated).  Character-split text through KenLM's ``lmplz`` loads unchanged."""
+        if any(ch.isspace() for ch in alphabet):
+            raise ValueError("an alphabet with whitespace cannot be read from ARPA (its tokens are whitespace-separated)")
+        text = path_or_text
+        if "\n" not in path_or_text and not path_or_text.lstrip().startswith("\\data\\"):
+            with open(path_or_text, encoding="utf-8") as f:
+                text = f.read()
+        index = {ch: i for i, ch in enumerate(alphabet)}
+        index["<s>"], index["</s>"] = LM_BOS, len(alphabet)
+        logp10, backoff10, declared, found = {}, {}, {}, {}
+        m, seen_data, ended = 0, False, False
+        for no, line in enumerate(text.splitlines(), 1):
+            s = line.strip()
+            if not s or ended:
+                continue
+            if s == "\\data\\":
+                seen_data = True
+                continue
+            if s == "\\end\\":
+                ended = True
+                continue
+            if not seen_data:
+                continue
+            if s.startswith("ngram ") and m == 0:
+                try:
+                    k, v = s[6:].split("=")
+                    declared[int(k)] = int(v)
+                except ValueError:
+                    raise ValueError(f"line {no}: malformed count line {line!r}") from None
+                continue
+            if s.startswith("\\") and s.endswith("-grams:"):
+                try:
+                    m = int(s[1:-7])
+                except ValueError:
+                    raise ValueError(f"line {no}: malformed section header {line!r}") from None
+                continue
+            if m == 0:
+                raise ValueError(f"line {no}: unexpected line {line!r}")
+            f = s.split()
+            found[m] = found.get(m, 0) + 1
+            if len(f) not in (m + 1, m + 2):
+                raise ValueError(f"line {no}: a {m}-gram line has {m + 1} or {m + 2} fields, got {line!r}")
+            toks = f[1:m + 1]
+            if "<unk>" in toks:
+                continue
+            try:
+                vals = [float(f[0])] + ([float(f[m + 1])] if len(f) == m + 2 else [])
+            except ValueError:
+                raise ValueError(f"line {no}: malformed number in {line!r}") from None
+            if not all(math.isfinite(v) for v in vals):
+                raise ValueError(f"line {no}: non-finite value in {line!r}")
+            bad = next((t for t in toks if t not in index), None)
+            if bad is not None:
+                raise ValueError(f"line {no}: token {bad!r} is not in the alphabet, <s> or </s>")
+            g = tuple(index[t] for t in toks)
+            if LM_BOS in g[1:] or len(alphabet) in g[:-1]:
+                raise ValueError(f"line {no}: <s> may only open and </s> only close an n-gram: {line!r}")
+            if m > 1 and g[:-1] not in logp10:
+                raise ValueError(f"line {no}: the history of {line!r} is not listed")
+            logp10[g] = vals[0]
+            if len(vals) == 2 and vals[1] != 0.0:
+                backoff10[g] = vals[1]
+        if not seen_data:
+            raise ValueError("no \\data\\ section")
+        for k in sorted(set(declared) | set(found)):
+            if declared.get(k, 0) != found.get(k, 0):
+                raise ValueError(f"the header declares {declared.get(k, 0)} {k}-grams, the file holds {found.get(k, 0)}")
+        if not ended:
+            raise ValueError("no \\end\\ line: the file is truncated")
+        order = max((len(g) for g in logp10), default=0)
+        if not 2 <= order <= _lib.MAX_LM_ORDER:
+            raise ValueError(f"the order must be in [2, {_lib.MAX_LM_ORDER}], got {order}")
+        return cls(alphabet, order, logp10, backoff10)
+
+    def to_arpa(self, path):
+        """Writes the model as an ARPA file, 17 significant digits: ``from_arpa`` reads back the same tables."""
+        grams = sorted(self.logp10, key=lambda g: (len(g), g))
+        out = ["\\data\\"] + [f"ngram {m}={sum(len(g) == m for g in grams)}" for m in range(1, self.order + 1)]
+        for m in range(1, self.order + 1):
+            out += ["", f"\\{m}-grams:"]
+            for g in grams:
+                if len(g) == m:
+                    toks = " ".join(self._token(self.alphabet, s) for s in g)
+                    line = f"{self.logp10[g]:.17g}\t{toks}"
+                    if g in self.backoff10:
+                        line += f"\t{self.backoff10[g]:.17g}"
+                    out.append(line)
+        out += ["", "\\end\\", ""]
+        with open(path, "w", encoding="utf-8") as f:
+            f.write("\n".join(out))
+
+    # ------------------------------------------------------------------ scores
+    def log_prob(self, text):
+        """The fp64 natural-log probability of the word ``text``, </s> included."""
+        index = {ch: i for i, ch in enumerate(self.alphabet)}
+        _check_word(0, text, index, "text")
+        seq = (LM_BOS,) + tuple(index[ch] for ch in text) + (len(self.alphabet),)
+        total = 0.0
+        for i in range(1, len(seq)):
+            total += self.logp_symbol(seq[i], seq[max(0, i - self.order + 1):i])
+        return total
+
+    def logp_symbol(self, w, h):
+        """log P(w | h) (natural log, fp64) by the backoff recursion; ``h`` a tuple of symbols."""
+        bo = 0.0
+        h = tuple(h)[-(self.order - 1):] if self.order > 1 else ()
+        while h + (w,) not in self.logp10:
+            bo += self.backoff10.get(h, 0.0)
+            h = h[1:]
+        return (bo + self.logp10[h + (w,)]) * _LN10
+
+    # ------------------------------------------------------------------ device form
+    @staticmethod
+    def history_key(h):
+        """The uint64 key of history ``h``: (len << 56) | its symbols 8 bits each, oldest highest."""
+        k = len(h) << 56
+        for i, s in enumerate(h):
+            k |= int(s) << (8 * (len(h) - 1 - i))
+        return k
+
+    def host_tables(self):
+        """(keys (H,) uint64 sorted, rows (H, K) float32): every listed history, keys[0] = 0 the empty one; column
+        c < K-1 log P(c | h) with the backoff folded in (fp64, rounded once), column K-1 log P(</s> | h)."""
+        if "host" not in self._tables:
+            k = len(self.alphabet) + 1
+            hist = [()] + self._histories
+            keys = np.array([self.history_key(h) for h in hist], np.uint64)
+            order = np.argsort(keys, kind="stable")
+            hist = [hist[i] for i in order]
+            at = {h: i for i, h in enumerate(hist)}
+            children = {}
+            for g in self.logp10:
+                children.setdefault(g[:-1], []).append(g)
+            rows = np.empty((len(hist), k), np.float64)
+            for h in sorted(hist, key=len):
+                i = at[h]
+                if not h:
+                    rows[i] = -np.inf
+                else:
+                    t = h[1:]
+                    while t not in at:
+                        t = t[1:]
+                    rows[i] = rows[at[t]] + self.backoff10.get(h, 0.0)
+                for g in children.get(h, ()):
+                    if g[-1] != LM_BOS:
+                        rows[i, g[-1]] = self.logp10[g]
+            self._tables["host"] = (keys[order], (rows * _LN10).astype(np.float32))
+        return self._tables["host"]
+
+    def device_arrays(self, device):
+        """(keys (H,) int64 -- the uint64 keys' bits --, rows (H, K) float32) CUDA tensors on ``device``, uploaded on
+        first use."""
+        device = torch.device(device)
+        if device not in self._tables:
+            keys, rows = self.host_tables()
+            self._tables[device] = (torch.from_numpy(keys.view(np.int64)).to(device), torch.from_numpy(rows).to(device))
+        return self._tables[device]
+
+    def descriptor(self, device):
+        """The ``b2o_char_lm`` of this model on ``device`` (``_lib.CharLMDesc``)."""
+        keys, rows = self.device_arrays(device)
+        return _lib.CharLMDesc(self.order, keys.shape[0], keys.data_ptr(), rows.data_ptr(), self.alpha, self.beta)
+
+
+def check_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET, language_model=None):
     """Validates a decoder choice before anything is launched (``ValueError`` otherwise) and returns the ``Lexicon`` to
     decode with, or None.  Without a lexicon this is ``check_beam``.  With one (a ``Lexicon`` over ``alphabet``, or a
-    list / tuple of strings, compiled here): ``beam_width`` must be None and 1 <= ``top_paths`` <= 128."""
+    list / tuple of strings, compiled here): ``beam_width`` must be None and 1 <= ``top_paths`` <= 128.
+    ``language_model`` (a ``CharLM`` over ``alphabet``) ranks the beam search by that model
+    (``b2o_crnn_forward_beam_lm``): it needs ``beam_width`` and does not combine with a lexicon."""
+    if language_model is not None:
+        if not isinstance(language_model, CharLM):
+            raise ValueError(f"language_model must be a CharLM, got {type(language_model).__name__}")
+        if lexicon is not None:
+            raise ValueError("lexicon and language_model are mutually exclusive")
+        if beam_width is None:
+            raise ValueError("a language model needs beam search: pass beam_width")
+        check_beam(beam_width, top_paths)
+        if language_model.alphabet != alphabet:
+            raise ValueError("the language model was built for another alphabet than the recognizer's")
+        return None
     if lexicon is None:
         check_beam(beam_width, top_paths)
         return None
@@ -470,28 +798,35 @@ class Recognizer:
                                 None if logp is None else logp.data_ptr(), stream)
         return out, logp
 
-    def _decoder(self, beam_width, top_paths, lexicon):
+    def _decoder(self, beam_width, top_paths, lexicon, language_model=None):
         """``check_decoder`` for this recognizer's alphabet."""
-        return check_decoder(beam_width, top_paths, lexicon, DEFAULT_ALPHABET if lexicon is None else self.alphabet)
+        plain = lexicon is None and language_model is None
+        return check_decoder(beam_width, top_paths, lexicon, DEFAULT_ALPHABET if plain else self.alphabet,
+                             language_model)
 
-    def predict_device(self, crnn_in, with_scores=False, beam_width=None, top_paths=1, lexicon=None):
+    def predict_device(self, crnn_in, with_scores=False, beam_width=None, top_paths=1, lexicon=None,
+                       language_model=None):
         """CRNN + greedy CTC.  crnn_in: (B,200,31) fp16 -> labels (B,48) int32 (-1 padded).  ``with_scores``: returns
         (labels, logp) with logp (B,) float32 the greedy path's log-probability (``b2o_crnn_forward_scored``).
         ``beam_width``: CTC prefix beam search instead (``b2o_crnn_forward_beam``, see ``check_beam``), logp = the beam
         scores; ``top_paths > 1`` gives labels (B,P,48) and logp (B,P), best first.  ``lexicon`` (a ``Lexicon`` or a
         list of strings, see ``check_decoder``): the ``top_paths`` most probable entries instead
-        (``b2o_crnn_forward_lexicon``), logp = their CTC forward log-probabilities, in the same shapes."""
-        lexicon = self._decoder(beam_width, top_paths, lexicon)
+        (``b2o_crnn_forward_lexicon``), logp = their CTC forward log-probabilities, in the same shapes.
+        ``language_model`` (a ``CharLM``, with ``beam_width``): the beam search ranked by that model
+        (``b2o_crnn_forward_beam_lm``); logp stays the acoustic beam score of each reading."""
+        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
         b = crnn_in.shape[0]
         lead = (b,) if top_paths == 1 else (b, top_paths)
         labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
         logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
-        self._forward(crnn_in, labels, logp, beam_width, top_paths, lexicon)
+        self._forward(crnn_in, labels, logp, beam_width, top_paths, lexicon, language_model=language_model)
         return (labels, logp) if with_scores else labels
 
-    def _forward(self, crnn_in, labels, logp, beam_width, top_paths, lexicon, spans=None, theta=None):
+    def _forward(self, crnn_in, labels, logp, beam_width, top_paths, lexicon, spans=None, theta=None,
+                 language_model=None, fused=None):
         """The CRNN and the decoder of ``predict_device`` into caller-allocated ``labels`` / ``logp`` (None: greedy
-        without scores, or scores not written); ``lexicon`` is already compiled.  ``spans`` (B,P,48,2) int32: also the
+        without scores, or scores not written); ``lexicon`` is already compiled.  With ``language_model``, ``fused``
+        (B,P) float32 or None receives every reading's F_end.  ``spans`` (B,P,48,2) int32: also the
         characters' emission spans of every reading (``b2o_crnn_align``) and, with an STN, its ``theta`` (B,6) float32;
         the greedy forward then keeps its logits (``b2o_crnn_forward_logits``)."""
         b = crnn_in.shape[0]
@@ -508,6 +843,11 @@ class Recognizer:
             offsets, lex_labels = lexicon.device_arrays(self.device)
             self.ctx.crnn_forward_lexicon(crnn_in.data_ptr(), b, offsets.data_ptr(), lex_labels.data_ptr(), len(lexicon),
                                           int(top_paths), labels.data_ptr(), logp_ptr, ws.data_ptr(), nbytes, stream)
+        elif language_model is not None:
+            self.ctx.crnn_forward_beam_lm(crnn_in.data_ptr(), b, int(beam_width), int(top_paths),
+                                          language_model.descriptor(self.device), labels.data_ptr(), logp_ptr,
+                                          fused.data_ptr() if fused is not None else None, ws.data_ptr(), nbytes,
+                                          stream)
         elif beam_width is not None:
             self.ctx.crnn_forward_beam(crnn_in.data_ptr(), b, int(beam_width), int(top_paths), labels.data_ptr(),
                                        logp_ptr, ws.data_ptr(), nbytes, stream)
@@ -524,7 +864,7 @@ class Recognizer:
                                 theta.data_ptr() if theta is not None else None, ws.data_ptr(), nbytes, stream)
         self._last_ws = (ws, b) if self.keep_workspace else None
 
-    def _predict_aligned(self, crnn_in, beam_width, top_paths, lexicon):
+    def _predict_aligned(self, crnn_in, beam_width, top_paths, lexicon, language_model=None):
         """``predict_device(with_scores=True)`` plus every reading's spans: (labels (B,P,48), logp (B,P), spans
         (B,P,48,2) int32, theta (B,6) float32 or None without an STN)."""
         b, p = crnn_in.shape[0], int(top_paths)
@@ -532,7 +872,7 @@ class Recognizer:
         logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
         spans = torch.empty((b, p, STEPS, 2), dtype=torch.int32, device=self.device)
         theta = torch.empty((b, 6), dtype=torch.float32, device=self.device) if self.stn else None
-        self._forward(crnn_in, labels, logp, beam_width, p, lexicon, spans, theta)
+        self._forward(crnn_in, labels, logp, beam_width, p, lexicon, spans, theta, language_model)
         return labels, logp, spans, theta
 
     def char_cells_device(self, spans, theta, boxes=None, turns=None):
@@ -554,16 +894,18 @@ class Recognizer:
         return out
 
     def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                        return_char_boxes=False):
+                        return_char_boxes=False, language_model=None):
         """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str].
         ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``.  ``beam_width``: beam search
         decoding (``check_beam``); with ``top_paths = P > 1`` each text is a list of P strings and each confidence a
         list of P floats, best first (``decode_paths``).  ``lexicon``: the most probable entries of a word list instead
         (``check_decoder``), in the same shapes; a confidence is exp(the entry's CTC log-probability), clipped to 1.
+        ``language_model`` (a ``CharLM``, with ``beam_width``): the beam search ranked by that character model; the
+        confidences stay exp(the acoustic beam score).
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells (``b2o_char_cells``), an
         (n,4,2) float32 array for a text of n characters (a list of P arrays with ``top_paths = P > 1``), in the crop's
         200 x 31 frame: (text, cells) or (text, confidence, cells)."""
-        lexicon = self._decoder(beam_width, top_paths, lexicon)
+        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
         t = crops if isinstance(crops, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(crops))
         t = t.to(self.device).contiguous()
         b = t.shape[0]
@@ -573,7 +915,7 @@ class Recognizer:
         crnn_in = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + ((3,) if self.color else ()), dtype=torch.float16, device=self.device)
         self.ctx.crops_to_input(t.data_ptr(), b, crnn_in.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream,
                                 color=self.color)
-        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model}
         if return_char_boxes:
             labels, logp, spans, theta = self._predict_aligned(crnn_in, **beam)
             return self._with_cells(labels, logp, self.char_cells_device(spans, theta), top_paths, return_scores)
@@ -590,26 +932,27 @@ class Recognizer:
         boxes = char_boxes_host(cells.cpu().numpy(), texts)
         return list(zip(texts, conf, boxes)) if return_scores else list(zip(texts, boxes))
 
-    def recognize(self, image, beam_width=None, top_paths=1, lexicon=None):
+    def recognize(self, image, beam_width=None, top_paths=1, lexicon=None, language_model=None):
         """Recognize text from a single pre-cropped image (reference recognition.py:467-489): fit to
         200x31 with zero fill (host, as upstream), gray conversion, then the CUDA CRNN.  ``beam_width`` / ``top_paths`` /
-        ``lexicon``: as ``recognize_crops``."""
+        ``lexicon`` / ``language_model``: as ``recognize_crops``."""
         import cv2
 
-        lexicon = self._decoder(beam_width, top_paths, lexicon)
+        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
         image = tools.read_and_fit(filepath_or_array=image, width=TARGET_WIDTH, height=TARGET_HEIGHT, cval=0)
         if not self.color and image.ndim == 3 and image.shape[-1] == 3:      # recognition.py:481-483
             image = cv2.cvtColor(image, code=cv2.COLOR_RGB2GRAY)
         return self.recognize_crops(np.ascontiguousarray(image.reshape((1, TARGET_HEIGHT, TARGET_WIDTH) + ((3,) if self.color else ()))),
-                                    beam_width=beam_width, top_paths=top_paths, lexicon=lexicon)[0]
+                                    beam_width=beam_width, top_paths=top_paths, lexicon=lexicon,
+                                    language_model=language_model)[0]
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
                                     with_scores=False, beam_width=None, top_paths=1, lexicon=None, rotations=None,
                                     rotation_vote="word", char_boxes=False, polys=None, points=None, max_windows=1,
-                                    windows=None):
+                                    windows=None, language_model=None):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
-        (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon``: see
-        ``predict_device``).
+        (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon`` /
+        ``language_model``: see ``predict_device``).
 
         ``rotations`` / ``rotation_vote`` (``check_rotations``): every box is cut and decoded once per listed turn, one
         turn after another (the CRNN workspace stays that of B crops), and ``b2o_select_rotation`` keeps one reading per
@@ -636,7 +979,7 @@ class Recognizer:
         ``b2o_window_counts`` gives them (``Pipeline.recognize`` reads them back with the box counts; ``ValueError`` for
         another shape or a count outside [1, max_windows]); None: computed here and read back, one more
         synchronisation."""
-        lexicon = self._decoder(beam_width, top_paths, lexicon)
+        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
         turns = check_rotations(rotations, rotation_vote)
         max_windows = check_windows(max_windows, beam_width, lexicon, turns, char_boxes, polys is not None)
         if polys is not None and (turns is not None or char_boxes):
@@ -671,36 +1014,40 @@ class Recognizer:
         if polys is not None:
             crnn_in, _ = self.warp_polys_device(gray, polys[:total], points[:total], image_index[:total])
             return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
-                                       lexicon=lexicon)
+                                       lexicon=lexicon, language_model=language_model)
         if turns is not None:
             return self._recognize_turns(gray, flat[:total], image_index[:total], len(counts), boxes, turns,
-                                         rotation_vote, with_scores, beam_width, top_paths, lexicon, char_boxes)
+                                         rotation_vote, with_scores, beam_width, top_paths, lexicon, char_boxes,
+                                         language_model)
         if char_boxes:
             labels, logp, spans, cells = self._read_cells(gray, flat[:total], image_index[:total], beam_width,
-                                                          top_paths, lexicon)
+                                                          top_paths, lexicon, language_model)
             return (labels, logp, spans, cells) if with_scores else (labels, spans, cells)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
         return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
-                                   lexicon=lexicon)
+                                   lexicon=lexicon, language_model=language_model)
 
-    def _read_cells(self, gray, flat, image_index, beam_width, top_paths, lexicon):
+    def _read_cells(self, gray, flat, image_index, beam_width, top_paths, lexicon, language_model=None):
         """Warp + CRNN + decoder + alignment + cells of one pass: (labels, logp, spans, cells) in the shapes of
         ``recognize_from_boxes_device``."""
         crnn_in, _ = self.warp_device(gray, flat, image_index)
-        labels, logp, spans, theta = self._predict_aligned(crnn_in, beam_width, top_paths, lexicon)
+        labels, logp, spans, theta = self._predict_aligned(crnn_in, beam_width, top_paths, lexicon, language_model)
         cells = self.char_cells_device(spans, theta, flat)
         if top_paths == 1:
             labels, logp, spans, cells = labels[:, 0], logp[:, 0], spans[:, 0], cells[:, 0]
         return labels, logp, spans, cells
 
     def _recognize_turns(self, gray, flat, image_index, n_images, table, turns, vote, with_scores, beam_width,
-                         top_paths, lexicon, char_boxes=False):
+                         top_paths, lexicon, char_boxes=False, language_model=None):
         """Warp + CRNN + decoder for each turn into its slot of one (R,B,P,48) / (R,B,P) stack, then
         ``b2o_select_rotation``, which also rolls ``flat`` and ``table`` (None: no table) in place.  ``char_boxes``: each
-        turn's spans and theta are stacked alike, and the chosen turn's cells are built from the boxes as they were cut."""
+        turn's spans and theta are stacked alike, and the chosen turn's cells are built from the boxes as they were cut.
+        With ``language_model`` the vote compares the readings' F_end, and the chosen turn's acoustic logp is gathered
+        on the device."""
         b, p, r = flat.shape[0], int(top_paths), len(turns)
         labels_all = torch.empty((r, b, p, STEPS), dtype=torch.int32, device=self.device)
         logp_all = torch.empty((r, b, p), dtype=torch.float32, device=self.device)
+        fused_all = torch.empty((r, b, p), dtype=torch.float32, device=self.device) if language_model is not None else None
         spans_all = theta_all = cut = None
         if char_boxes:
             spans_all = torch.empty((r, b, p, STEPS, 2), dtype=torch.int32, device=self.device)
@@ -709,19 +1056,24 @@ class Recognizer:
         for j, turn in enumerate(turns):
             crnn_in, _ = self.warp_device(gray, flat, image_index, turn=turn)
             self._forward(crnn_in, labels_all[j], logp_all[j], beam_width, p, lexicon,
-                          None if spans_all is None else spans_all[j], None if theta_all is None else theta_all[j])
+                          None if spans_all is None else spans_all[j], None if theta_all is None else theta_all[j],
+                          language_model, None if fused_all is None else fused_all[j])
         labels = torch.empty((b, p, STEPS), dtype=torch.int32, device=self.device)
         logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
         chosen = torch.empty((b,), dtype=torch.int32, device=self.device)
-        self.ctx.select_rotation(labels_all.data_ptr(), logp_all.data_ptr(), image_index.data_ptr(), n_images, b, p,
+        vote_logp = logp_all if fused_all is None else fused_all
+        self.ctx.select_rotation(labels_all.data_ptr(), vote_logp.data_ptr(), image_index.data_ptr(), n_images, b, p,
                                  turns, ROTATION_VOTES[vote], labels.data_ptr(), logp.data_ptr(), chosen.data_ptr(),
                                  flat.data_ptr(), None if table is None else table.data_ptr(),
                                  0 if table is None else table.shape[1], torch.cuda.current_stream(self.device).cuda_stream)
         extra = ()
-        if char_boxes:
+        if char_boxes or fused_all is not None:
             slot = torch.zeros(4, dtype=torch.int64, device=self.device)
             slot[list(turns)] = torch.arange(r, device=self.device)
             pick, rows = slot[chosen.long()], torch.arange(b, device=self.device)
+        if fused_all is not None:
+            logp = logp_all[pick, rows]                  # the vote ran on F_end; the readings keep their acoustic logp
+        if char_boxes:
             spans = spans_all[pick, rows]
             cells = self.char_cells_device(spans, None if theta_all is None else theta_all[pick, rows], cut, chosen)
             extra = (spans[:, 0], cells[:, 0]) if p == 1 else (spans, cells)
@@ -732,10 +1084,10 @@ class Recognizer:
     # ------------------------------------------------------------------ reference API
     def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
                              rotations=None, rotation_vote="word", return_char_boxes=False, max_windows=1,
-                             **kwargs) -> typing.List[typing.List[str]]:
+                             language_model=None, **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
-        (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon``: as
-        ``recognize_crops``.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
+        (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon`` /
+        ``language_model``: as ``recognize_crops``; with rotations the vote compares the language model's fused scores.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
         most probable reading kept, per word or per image (one box group), see ``check_rotations``.
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells, an (n,4,2) float32 array
         of quads in the image's pixels for a text of n characters (a list of P arrays with ``top_paths = P > 1``):
@@ -747,7 +1099,7 @@ class Recognizer:
         (``ValueError``).
         ``max_windows``: every box wider than the 200 x 31 crop at full height is read in up to that many overlapping
         windows and their steps stitched into one reading (``check_windows``; greedy decoding, boxes only)."""
-        lexicon = self._decoder(beam_width, top_paths, lexicon)
+        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
         turns = check_rotations(rotations, rotation_vote)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
@@ -757,7 +1109,7 @@ class Recognizer:
         max_windows = check_windows(max_windows, beam_width, lexicon, turns, return_char_boxes, polygons)
         if polygons:
             return self._recognize_polygons(images, box_groups, entries, return_scores, turns, return_char_boxes,
-                                            beam_width, top_paths, lexicon)
+                                            beam_width, top_paths, lexicon, language_model)
         images_t = _as_device_images(images, self.device)
         counts = np.array([len(b) for b in box_groups], dtype=np.int64)
         if counts.sum() == 0:
@@ -770,7 +1122,7 @@ class Recognizer:
         flat_t = torch.from_numpy(np.ascontiguousarray(flat)).to(self.device)
         idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
         gray = images_t if self.color else self.gray_device(images_t)
-        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model}
         if return_char_boxes:
             if turns is not None:
                 labels, logp, _, _, cells = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns,
@@ -800,7 +1152,7 @@ class Recognizer:
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]
 
     def _recognize_polygons(self, images, box_groups, entries, return_scores, turns, char_boxes, beam_width, top_paths,
-                            lexicon):
+                            lexicon, language_model=None):
         """``recognize_from_boxes`` for box groups that hold polygons: 4-point entries are rectified as
         ``tools.rectify_boxes`` does and cut as boxes, the others along their polygon, all in one ``b2o_warp_polys``."""
         if turns is not None or char_boxes:
@@ -817,7 +1169,7 @@ class Recognizer:
         gray = images_t if self.color else self.gray_device(images_t)
         crnn_in, _ = self.warp_polys_device(gray, torch.from_numpy(polys).to(self.device),
                                             torch.from_numpy(points).to(self.device), idx)
-        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon}
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model}
         if return_scores:
             labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
             predictions = list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))

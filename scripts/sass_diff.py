@@ -20,6 +20,7 @@ def functions(path):
         m = re.search(r"Function : (\S+)", line)
         if m:
             full = re.sub(r"_GLOBAL__N__[0-9a-f]+_", "_GLOBAL__N__", m.group(1))   # anonymous namespace: per-build hash
+            full = re.sub(r"(_GLOBAL__N__\d+_\w+?_cu)_[0-9a-f]{8}", r"\1_", full)  # and the hash of the file's contents
             name = full[full.index("kernelI"):] if "kernelI" in full else full
             table[name] = []
             continue
