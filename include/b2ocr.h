@@ -408,6 +408,38 @@ int b2o_crnn_forward_beam_lm(b2o_ctx* ctx, const void* crnn_in_dev, int b, int b
                              const b2o_char_lm* lm, int32_t* labels_dev, float* logp_dev, float* fused_dev, void* ws_dev,
                              size_t ws_bytes, void* stream);
 
+/* CTC prefix beam search constrained to a pattern: a deterministic automaton over the labels (DESIGN.md section 1,
+ * "Patterns"), built on the host (recognition.Pattern.device_arrays).  n_states states, trans_dev (n_states, k-1) int16:
+ * trans[q][c] the state after label c in state q, -1 for none; dist_dev (n_states) uint8: the fewest labels from q to an
+ * accepting state, 0 when q accepts (saturated at 255); start the state of the empty reading.  The tables are sized
+ * for the k of the call.  A beam also carries its state; after step t (0 .. 47) a beam kept via blank or its last label
+ * and an extension alike survive only in a state q with dist[q] <= 47 - t, so every returned reading is accepted.  Each
+ * step a beam extends by its own shortlist, the min(beam_width + 1, its count) allowed labels (successor defined and
+ * feasible) with the largest lp[t,c] (ties: smaller label).  Scores, merging and ranking are b2o_ctc_beam_decode's;
+ * labels_dev (b, top_paths, 48) and logp_dev (b, top_paths) (NULL: not written) as it writes them, and a crop with
+ * fewer than top_paths surviving readings (none: the pattern cannot be met in 48 steps) has the remaining slots -1 with
+ * logp -inf; a reading of probability 0 (score -inf) is never returned.  A one-state automaton that accepts
+ * everything gives b2o_ctc_beam_decode's labels and logp bit for bit, except slots that b2o_ctc_beam_decode fills
+ * with -inf readings (fewer finite ones than top_paths, at tiny k), which are -1 here.
+ * 1 <= n_states <= B2O_MAX_PATTERN_STATES, 0 <= start < n_states, trans and dist not NULL, 2 <= k <=
+ * B2O_MAX_PATTERN_CLASSES and the beam_width / top_paths rules of beam search, otherwise B2O_ERR_ARG.
+ * b2o_ctc_beam_pattern_decode: the search alone on caller-supplied (b, 48, k) float32 logits.
+ * b2o_crnn_forward_beam_pattern: the CRNN of b2o_crnn_forward, its fc_12 logits into the workspace (so b2o_crnn_align
+ * works after it), then the search.                                                                                  */
+#define B2O_MAX_PATTERN_STATES 4096
+#define B2O_MAX_PATTERN_CLASSES 127
+typedef struct {
+  int n_states;
+  int start;
+  const int16_t* trans_dev;
+  const uint8_t* dist_dev;
+} b2o_pattern;
+int b2o_ctc_beam_pattern_decode(b2o_ctx* ctx, const float* logits_dev, int b, int k, int beam_width, int top_paths,
+                                const b2o_pattern* pattern, int32_t* labels_dev, float* logp_dev, void* stream);
+int b2o_crnn_forward_beam_pattern(b2o_ctx* ctx, const void* crnn_in_dev, int b, int beam_width, int top_paths,
+                                  const b2o_pattern* pattern, int32_t* labels_dev, float* logp_dev, void* ws_dev,
+                                  size_t ws_bytes, void* stream);
+
 /* Lexicon-constrained CTC decoding: the top_paths most probable entries of a caller's word list, per crop.
  * Inputs: the beam decoder's lp[t,c] = log(softmax(logits_t)_c + 1e-7) over the 48 kept steps, blank = k-1.
  * Lexicon: n_words entries in CSR form, offsets_dev (n_words + 1) int32 and the concatenated labels_dev int16; entry i

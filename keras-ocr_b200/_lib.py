@@ -21,6 +21,8 @@ MAX_LEXICON_TOP_PATHS = 128   # B2O_MAX_LEXICON_TOP_PATHS
 MAX_LM_ORDER = 8              # B2O_MAX_LM_ORDER
 MAX_LM_HISTORIES = 1 << 20    # B2O_MAX_LM_HISTORIES
 MAX_LM_CLASSES = 127          # B2O_MAX_LM_CLASSES
+MAX_PATTERN_STATES = 4096     # B2O_MAX_PATTERN_STATES
+MAX_PATTERN_CLASSES = 127     # B2O_MAX_PATTERN_CLASSES
 ROTATION_VOTE_WORD, ROTATION_VOTE_PAGE = 0, 1   # B2O_ROTATION_VOTE_WORD / _PAGE
 MAX_ALIGN_PATHS = 128         # B2O_MAX_ALIGN_PATHS
 CRAFT_LAST_STEP = 30          # B2O_CRAFT_LAST_STEP
@@ -74,6 +76,14 @@ class CharLMDesc(ctypes.Structure):
 
 
 _lmp = _c.POINTER(CharLMDesc)
+
+
+class PatternDesc(ctypes.Structure):
+    """b2o_pattern (include/b2ocr.h), field for field."""
+    _fields_ = [("n_states", _i), ("start", _i), ("trans_dev", _vp), ("dist_dev", _vp)]
+
+
+_patp = _c.POINTER(PatternDesc)
 
 # name -> (restype, argtypes); mirrors include/b2ocr.h one to one
 SIGNATURES = {
@@ -132,6 +142,8 @@ SIGNATURES = {
     "b2o_crnn_forward_beam": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_ctc_beam_lm_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _lmp, _vp, _vp, _vp, _vp]),
     "b2o_crnn_forward_beam_lm": (_i, [_vp, _vp, _i, _i, _i, _lmp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_ctc_beam_pattern_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _patp, _vp, _vp, _vp]),
+    "b2o_crnn_forward_beam_pattern": (_i, [_vp, _vp, _i, _i, _i, _patp, _vp, _vp, _vp, _sz, _vp]),
     "b2o_lexicon_workspace_bytes": (_sz, [_i, _i, _i]),
     "b2o_ctc_lexicon_decode": (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_crnn_forward_lexicon": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
@@ -445,6 +457,17 @@ class Context:
         self._check(self.lib.b2o_crnn_forward_beam_lm(self.handle, crnn_in, b, beam_width, top_paths, ctypes.byref(lm),
                                                       labels, logp, fused, ws, ws_bytes, stream),
                     "b2o_crnn_forward_beam_lm")
+
+    def ctc_beam_pattern_decode(self, logits, b, k, beam_width, top_paths, pattern, labels, logp, stream):
+        """``pattern``: a ``PatternDesc``."""
+        self._check(self.lib.b2o_ctc_beam_pattern_decode(self.handle, logits, b, k, beam_width, top_paths,
+                                                         ctypes.byref(pattern), labels, logp, stream),
+                    "b2o_ctc_beam_pattern_decode")
+
+    def crnn_forward_beam_pattern(self, crnn_in, b, beam_width, top_paths, pattern, labels, logp, ws, ws_bytes, stream):
+        self._check(self.lib.b2o_crnn_forward_beam_pattern(self.handle, crnn_in, b, beam_width, top_paths,
+                                                           ctypes.byref(pattern), labels, logp, ws, ws_bytes, stream),
+                    "b2o_crnn_forward_beam_pattern")
 
     def lexicon_workspace_bytes(self, b, n_words, top_paths):
         return int(self.lib.b2o_lexicon_workspace_bytes(b, n_words, top_paths))

@@ -20,6 +20,8 @@ int ctc_beam_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width
                  cudaStream_t st);
 int ctc_beam_lm_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
                     const b2o_char_lm* lm, int* labels, float* logp, float* fused, cudaStream_t st);
+int ctc_beam_pattern_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
+                         const b2o_pattern* pat, int* labels, float* logp, cudaStream_t st);
 size_t ctc_lexicon_workspace_bytes(int B, int n_words);
 int ctc_lexicon_run(b2o_ctx* ctx, const float* logits, int B, int K, const int* offsets, const short* labels,
                     int n_words, int top_paths, int* labels_out, float* logp, void* ws, cudaStream_t st);
@@ -915,6 +917,57 @@ extern "C" int b2o_ctc_beam_lm_decode(b2o_ctx* ctx, const float* logits, int b, 
   DeviceGuard guard(ctx->device);
   return ctc_beam_lm_run(ctx, logits, b, k, beam_width, top_paths, lm, labels, logp, fused,
                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+namespace {
+
+bool pattern_args_ok(b2o_ctx* ctx, const char* fn, int k, int beam_width, int top_paths, const b2o_pattern* pat) {
+  if (!beam_args_ok(ctx, fn, k, beam_width, top_paths)) return false;
+  if (k > B2O_MAX_PATTERN_CLASSES) { ctx->set_error(std::string(fn) + ": k must be in [2, 127]"); return false; }
+  if (!pat || !pat->trans_dev || !pat->dist_dev) { ctx->set_error(std::string(fn) + ": no pattern"); return false; }
+  if (pat->n_states < 1 || pat->n_states > B2O_MAX_PATTERN_STATES) {
+    ctx->set_error(std::string(fn) + ": n_states must be in [1, 4096]");
+    return false;
+  }
+  if (pat->start < 0 || pat->start >= pat->n_states) {
+    ctx->set_error(std::string(fn) + ": start must be in [0, n_states)");
+    return false;
+  }
+  return true;
+}
+
+}  // namespace
+
+extern "C" int b2o_crnn_forward_beam_pattern(b2o_ctx* ctx, const void* crnn_in, int b, int beam_width, int top_paths,
+                                             const b2o_pattern* pattern, int32_t* labels, float* logp, void* ws,
+                                             size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!ctx->crnn_loaded) {
+    ctx->set_error("b2o_crnn_forward_beam_pattern: CRNN weights not loaded");
+    return B2O_ERR_STATE;
+  }
+  if (!pattern_args_ok(ctx, "b2o_crnn_forward_beam_pattern", ctx->n_classes, beam_width, top_paths, pattern))
+    return B2O_ERR_ARG;
+  if (b == 0) return B2O_OK;
+  B2O_RETURN_IF(crnn_forward(ctx, crnn_in, b, labels, nullptr, true, ws, ws_bytes, stream));
+  DeviceGuard guard(ctx->device);
+  const float* logits = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(ws) + plan_crnn(b).off[rb::logits]);
+  return ctc_beam_pattern_run(ctx, logits, b, ctx->n_classes, beam_width, top_paths, pattern, labels, logp,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2o_ctc_beam_pattern_decode(b2o_ctx* ctx, const float* logits, int b, int k, int beam_width,
+                                           int top_paths, const b2o_pattern* pattern, int32_t* labels, float* logp,
+                                           void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!pattern_args_ok(ctx, "b2o_ctc_beam_pattern_decode", k, beam_width, top_paths, pattern)) return B2O_ERR_ARG;
+  if (b < 0 || (b > 0 && (!logits || !labels))) {
+    ctx->set_error("b2o_ctc_beam_pattern_decode: bad argument");
+    return B2O_ERR_ARG;
+  }
+  DeviceGuard guard(ctx->device);
+  return ctc_beam_pattern_run(ctx, logits, b, k, beam_width, top_paths, pattern, labels, logp,
+                              reinterpret_cast<cudaStream_t>(stream));
 }
 
 namespace {

@@ -741,7 +741,322 @@ ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// ctc_beam_pattern_kernel: the same search constrained to the readings a DFA accepts (DESIGN.md section 1, "Patterns").
+//   The DFA: states 0 .. n-1, trans[q][c] the successor of q by label c (-1: none), dist[q] the fewest labels from q to
+//   an accepting state (0: q accepts).  A beam also carries its state q(a) = delta*(start, a); the empty beam starts in
+//   start.  Equal prefixes have equal states, so merging is unchanged.  After step t a candidate in state q is kept only
+//   if dist[q] <= 47 - t -- a beam kept via blank or its last label and an extension alike -- so after the last step
+//   every survivor accepts.  Ranking, merging, the tie order and the returned scores are those of ctc_beam_kernel.
+// Per step, besides steps 1-6 above:
+//   2'. the shortlist is per beam: of the labels c with delta(q(a), c) defined and dist[delta(q(a), c)] <= 47 - t (the
+//       beam's allowed labels), the min(S, their count) with the largest lp[c] (ties: smaller label), ascending, one
+//       warp per beam; slots past the count are not candidates;
+//   6'. an extension's state is read from trans; trans and dist are read from global memory (L2-resident).
+// Why the per-beam shortlist loses nothing: a label outside the allowed set yields a prefix that either the DFA rejects
+// or that cannot reach acceptance in the steps left, so it is never a candidate.  Let c be allowed, outside a's
+// shortlist and a+c not a beam.  The shortlist then holds S = W+1 allowed labels c' ranked above c (lp[c'] > lp[c], or
+// equal with c' < c); at most one of them is last(a), so at least W of them give a+c' a contribution score(a) + lp[c']
+// >= the score of a+c.  Each a+c' is a candidate in the same step: as a's extension, or, if a+c' is already a beam, as
+// that beam kept -- whose state is delta(q(a), c') too, so it is feasible, and whose score includes the extension's
+// contribution.  So W candidates beat a+c or tie and precede it, and a+c is not among the W best.  The fp32 argument of
+// ctc_beam_kernel carries over unchanged.
+// A candidate of score -inf (an extension by the last label of a beam whose p_b is -inf) is no candidate here: its
+// prefix has probability 0, and left in, it would walk the DFA without the blanks a repeated label needs (a{30} would
+// "survive" in 30 steps).  ctc_beam_kernel keeps such candidates while there is room, which only ever fills places no
+// finite candidate wants; a -inf beam later becomes finite only through its parent's extension, whose contribution
+// lae(-inf, x) = x is bit for bit the score that extension gets here as a new beam.  So with a one-state DFA that
+// accepts everything (".*") every label is allowed at every step, the per-beam shortlists equal the global one, and
+// the search returns ctc_beam_kernel's readings and scores bit for bit; only slots that ctc_beam_kernel fills with
+// -inf readings (fewer finite ones than paths asked for, at tiny K) are -1 with -inf here.
+struct SmemPat {
+  short* shl;                      // [W][S] per-beam shortlist, ascending labels
+  int* cnt;                        // [W] its length
+  int* q[2];                       // [W] the beam's DFA state
+};
+
+__host__ __device__ inline size_t smem_plan_pattern(int W, int K, unsigned char* base, Smem* s, SmemPat* l) {
+  size_t off = smem_plan(W, K, base, s);
+  const int S = shortlist_size(W, K);
+  SmemPat d;
+  SmemPat* p = l ? l : &d;
+#define B2O_TAKE(ptr, type, count)                                                    \
+  do {                                                                                \
+    if (base) (ptr) = reinterpret_cast<type*>(base + off);                            \
+    off += (static_cast<size_t>(count) * sizeof(type) + 15) / 16 * 16;                \
+  } while (0)
+  B2O_TAKE(p->shl, short, W * S);
+  B2O_TAKE(p->cnt, int, W);
+  for (int i = 0; i < 2; ++i) B2O_TAKE(p->q[i], int, W);
+#undef B2O_TAKE
+  return off;
+}
+
+// One warp: of the labels c < n with trow[c] >= 0 and dist[trow[c]] <= limit, the min(S, their count) with the largest
+// lp[c] (ties: smaller label), ascending, into out; returns how many.  Not inlined: inlined, the kernel spills.
+__device__ __noinline__ int pattern_shortlist(const float* lp, const short* __restrict__ trow, const unsigned char* __restrict__ dist,
+                                 int limit, int n, int S, short* out) {
+  const int lane = threadIdx.x & 31;
+  const unsigned lt = (1u << lane) - 1u;
+  unsigned kv[4];
+  int allowed = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int c = lane + 32 * i;
+    bool ok = false;
+    if (c < n) {
+      const int q = __ldg(trow + c);
+      ok = q >= 0 && static_cast<int>(__ldg(dist + q)) <= limit;
+    }
+    kv[i] = ok ? okey(lp[c]) : 0u;                 // okey of a finite lp is never 0
+    allowed += ok;
+  }
+  const int m = __reduce_add_sync(0xffffffffu, allowed), Sa = S < m ? S : m;
+  unsigned theta = 0;
+  int take = 0;
+  if (Sa < m) {
+    for (int bit = 31; bit >= 0; --bit) {         // the largest theta with at least Sa keys >= theta: the Sa-th key
+      const unsigned t = theta | (1u << bit);
+      int cnt = 0;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) cnt += kv[i] >= t;
+      if (__reduce_add_sync(0xffffffffu, cnt) >= Sa) theta = t;
+    }
+    int gt = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) gt += kv[i] > theta;
+    take = Sa - __reduce_add_sync(0xffffffffu, gt);
+  }
+  int at = 0, eq_before = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const bool eq = Sa < m && kv[i] == theta;
+    const unsigned eqm = __ballot_sync(0xffffffffu, eq);
+    const bool in = kv[i] != 0u && (Sa == m || kv[i] > theta || (eq && eq_before + __popc(eqm & lt) < take));
+    const unsigned msk = __ballot_sync(0xffffffffu, in);
+    if (in) out[at + __popc(msk & lt)] = static_cast<short>(lane + 32 * i);
+    at += __popc(msk);
+    eq_before += __popc(eqm);
+  }
+  return Sa;
+}
+
+__global__ void __launch_bounds__(kThreads)
+ctc_beam_pattern_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W, int P,
+                        const short* __restrict__ trans /*[n][K-1]*/, const unsigned char* __restrict__ dist /*[n]*/,
+                        int start, int* __restrict__ labels /*[B][P][48]*/, float* __restrict__ logp /*[B][P] or null*/) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  Smem s;
+  SmemPat l;
+  smem_plan_pattern(W, K, smem_raw, &s, &l);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int blank = K - 1, S = shortlist_size(W, K), S1 = S + 1;
+  int cur = 0, nb = 1;
+  if (tid == 0) {
+    s.len[0][0] = 0; s.pb[0][0] = 0.f; s.pnb[0][0] = -INFINITY; s.sc[0][0] = 0.f;
+    s.h[0][0] = kHashRoot; s.ph[0][0] = 0;
+    l.q[0][0] = start;
+  }
+  for (int t = 0; t < kT; ++t) {
+    const int limit = kT - 1 - t;                  // labels that can still follow after this step
+    // ---- 1. lp of step t (as ctc_beam_kernel)
+    const float* row = logits + (static_cast<size_t>(blockIdx.x) * kT + t) * K;
+    float m = -INFINITY;
+    for (int c = tid; c < K; c += kThreads) { const float v = row[c]; s.lp[c] = v; m = fmaxf(m, v); }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float* redf = reinterpret_cast<float*>(s.red);
+    if (lane == 0) redf[warp] = m;
+    __syncthreads();
+    m = redf[0];
+    for (int w = 1; w < kWarps; ++w) m = fmaxf(m, redf[w]);
+    float se = 0.f;
+    for (int c = tid; c < K; c += kThreads) se = __fadd_rn(se, expf(__fsub_rn(s.lp[c], m)));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) se = __fadd_rn(se, __shfl_xor_sync(0xffffffffu, se, o));
+    __syncthreads();
+    if (lane == 0) redf[warp] = se;
+    __syncthreads();
+    se = redf[0];
+    for (int w = 1; w < kWarps; ++w) se = __fadd_rn(se, redf[w]);
+    for (int c = tid; c < K; c += kThreads)
+      s.lp[c] = logf(__fadd_rn(__fdiv_rn(expf(__fsub_rn(s.lp[c], m)), se), 1e-7f));
+    __syncthreads();
+
+    // ---- 2'. per-beam shortlists over the allowed labels, one warp per beam
+    for (int a = warp; a < nb; a += kWarps) {
+      const int c = pattern_shortlist(s.lp, trans + static_cast<size_t>(l.q[cur][a]) * (K - 1), dist, limit, K - 1, S,
+                                      l.shl + a * S);
+      if (lane == 0) l.cnt[a] = c;
+    }
+
+    // ---- 3. parent links and the extensions that are already beams
+    const Beams bm{s, cur, S1};
+    const LmOrder ord{s, l.shl, cur, S, S1};
+    for (int i = tid; i < nb * S; i += kThreads) s.excl[i] = 0;
+    if (tid < nb) {
+      int par = -1;
+      const int len = s.len[cur][tid];
+      if (len > 0)
+        for (int a = 0; a < nb && par < 0; ++a) {
+          if (s.len[cur][a] != len - 1 || s.h[cur][a] != s.ph[cur][tid]) continue;
+          bool same = true;
+          for (int u = 0; u < len - 1 && same; ++u) same = s.pre[cur][a * kT + u] == s.pre[cur][tid * kT + u];
+          if (same) par = a;
+        }
+      s.parent[tid] = par;
+    }
+    __syncthreads();
+    if (tid < nb && s.parent[tid] >= 0) {          // last(tid) in its parent's shortlist (ascending): binary search
+      const int pa = s.parent[tid], n_sl = l.cnt[pa];
+      const short* sl = l.shl + pa * S;
+      const int c = bm.last(tid);
+      int lo = 0, hi = n_sl;
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (sl[mid] < c) lo = mid + 1; else hi = mid; }
+      if (lo < n_sl && sl[lo] == c) s.excl[pa * S + lo] = 1;
+    }
+    __syncthreads();
+
+    // ---- 4. candidate keys: a beam kept only while it can still reach acceptance, extensions by its shortlist
+    const int n = nb * S1;
+    int valid = 0;
+    for (int i = tid; i < n; i += kThreads) {
+      const int a = i / S1, x = i - a * S1;
+      const bool cand = x == 0 ? static_cast<int>(__ldg(dist + l.q[cur][a])) <= limit
+                               : x - 1 < l.cnt[a] && !s.excl[a * S + x - 1];
+      unsigned k = 0;
+      if (cand) {
+        float pb, pnb;
+        if (x == 0) {
+          bm.eval(i, blank, &pb, &pnb);
+        } else {
+          pb = -INFINITY;
+          pnb = bm.ext(a, l.shl[a * S + x - 1]);
+        }
+        const float a_i = lae(pb, pnb);
+        if (a_i > -INFINITY) {                     // a zero-probability prefix (a repeat without a blank) is none
+          k = okey(a_i);
+          ++valid;
+        }
+      }
+      s.key[i] = k;
+      s.sel[i] = 0;
+    }
+    int nvalid;
+    block_scan(valid, s.red, &nvalid);
+
+    // ---- 5. the W best (as ctc_beam_kernel, the tie order over per-beam shortlists)
+    if (nvalid <= W) {
+      for (int i = tid; i < n; i += kThreads) s.sel[i] = s.key[i] != 0;
+    } else {
+      int take, equal;
+      const unsigned theta = radix_select(n, W, [&](int i) { return s.key[i]; }, s.hist, s.red, &take, &equal);
+      for (int i = tid; i < n; i += kThreads) s.sel[i] = s.key[i] > theta || (take == equal && s.key[i] == theta);
+      __syncthreads();
+      for (int r = 0; r < take && take < equal; ++r) {
+        int best = -1;
+        for (int i = tid; i < n; i += kThreads)
+          if (s.key[i] == theta && !s.sel[i] && (best < 0 || ord.lex_less(i, best))) best = i;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const int other = __shfl_xor_sync(0xffffffffu, best, o);
+          if (other >= 0 && (best < 0 || ord.lex_less(other, best))) best = other;
+        }
+        if (lane == 0) s.red[warp] = best;
+        __syncthreads();
+        if (tid == 0) {
+          int b = -1;
+          for (int w = 0; w < kWarps; ++w) {
+            const int o = s.red[w];
+            if (o >= 0 && (b < 0 || ord.lex_less(o, b))) b = o;
+          }
+          s.sel[b] = 1;
+        }
+        __syncthreads();
+      }
+    }
+    __syncthreads();
+
+    // ---- 6. compaction in candidate order into the other buffer; 6'. an extension steps its DFA state
+    {
+      const int chunk = (n + kThreads - 1) / kThreads, i0 = min(n, tid * chunk), i1 = min(n, i0 + chunk);
+      int cnt = 0;
+      for (int i = i0; i < i1; ++i) cnt += s.sel[i];
+      int total;
+      int slot = block_scan(cnt, s.red, &total);
+      const int nx = cur ^ 1;
+      for (int i = i0; i < i1; ++i) {
+        if (!s.sel[i]) continue;
+        const int a = i / S1, x = i - a * S1, len = s.len[cur][a];
+        float pb, pnb;
+        if (x == 0) {
+          bm.eval(i, blank, &pb, &pnb);
+        } else {
+          pb = -INFINITY;
+          pnb = bm.ext(a, l.shl[a * S + x - 1]);
+        }
+        for (int u = 0; u < len; ++u) s.pre[nx][slot * kT + u] = s.pre[cur][a * kT + u];
+        if (x > 0) {
+          const int c = l.shl[a * S + x - 1];
+          s.pre[nx][slot * kT + len] = static_cast<short>(c);
+          s.h[nx][slot] = s.h[cur][a] * kHashMul + static_cast<unsigned long long>(c + 1);
+          s.ph[nx][slot] = s.h[cur][a];
+          l.q[nx][slot] = __ldg(trans + static_cast<size_t>(l.q[cur][a]) * (K - 1) + c);
+        } else {
+          s.h[nx][slot] = s.h[cur][a];
+          s.ph[nx][slot] = s.ph[cur][a];
+          l.q[nx][slot] = l.q[cur][a];
+        }
+        s.len[nx][slot] = len + (x > 0);
+        s.pb[nx][slot] = pb;
+        s.pnb[nx][slot] = pnb;
+        s.sc[nx][slot] = unokey(s.key[i]);        // the selection key's score, bit for bit
+        ++slot;
+      }
+      nb = total;
+      cur = nx;
+      __syncthreads();
+    }
+  }
+
+  // ---- the P best of the final beams (every one accepts), best first; -1 labels and -inf past the survivors
+  const Beams fin{s, cur, 1};
+  const int b = blockIdx.x;
+  if (tid < nb) {
+    const unsigned k = okey(s.sc[cur][tid]);
+    int rank = 0;
+    for (int a = 0; a < nb; ++a) {
+      const unsigned ka = okey(s.sc[cur][a]);
+      rank += ka > k || (ka == k && a != tid && fin.lex_less(a, tid));
+    }
+    if (rank < P) {
+      int* o = labels + (static_cast<size_t>(b) * P + rank) * kT;
+      const int len = s.len[cur][tid];
+      for (int u = 0; u < kT; ++u) o[u] = u < len ? s.pre[cur][tid * kT + u] : -1;
+      if (logp) logp[static_cast<size_t>(b) * P + rank] = s.sc[cur][tid];
+    }
+  }
+  for (int r = nb + tid; r < P; r += kThreads) {
+    int* o = labels + (static_cast<size_t>(b) * P + r) * kT;
+    for (int u = 0; u < kT; ++u) o[u] = -1;
+    if (logp) logp[static_cast<size_t>(b) * P + r] = -INFINITY;
+  }
+}
+
 }  // namespace
+
+int ctc_beam_pattern_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
+                         const b2o_pattern* pat, int* labels, float* logp, cudaStream_t st) {
+  if (B <= 0) return B2O_OK;
+  const size_t bytes = smem_plan_pattern(beam_width, K, nullptr, nullptr, nullptr);
+  B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(ctc_beam_pattern_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           static_cast<int>(bytes)));
+  ctc_beam_pattern_kernel<<<B, kThreads, bytes, st>>>(logits, K, beam_width, top_paths,
+                                                      reinterpret_cast<const short*>(pat->trans_dev), pat->dist_dev,
+                                                      pat->start, labels, logp);
+  B2O_LAUNCH_CHECK(ctx);
+  return B2O_OK;
+}
 
 int ctc_beam_lm_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
                     const b2o_char_lm* lm, int* labels, float* logp, float* fused, cudaStream_t st) {

@@ -6,10 +6,10 @@ from . import detection, recognition, tools
 
 
 def check_records_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=recognition.DEFAULT_ALPHABET,
-                          language_model=None):
+                          language_model=None, pattern=None):
     """``recognition.check_decoder`` for the records path, whose fixed-size records carry one reading per word; returns
     the compiled lexicon or None."""
-    lexicon = recognition.check_decoder(beam_width, top_paths, lexicon, alphabet, language_model)
+    lexicon = recognition.check_decoder(beam_width, top_paths, lexicon, alphabet, language_model, pattern)
     if top_paths != 1:
         raise ValueError("records carry the best path only: top_paths must be 1")
     return lexicon
@@ -290,8 +290,9 @@ class Pipeline:
         readings and its confidence a list of P floats, best first.  Or ``lexicon`` (a ``recognition.Lexicon`` or a
         list of strings) / ``top_paths``: every word reads as the most probable entries of that list, in the same
         shapes (``recognition.check_decoder``).  Or ``language_model`` (a ``recognition.CharLM``) with ``beam_width``:
-        the beam search ranked by that character model, confidences still from the acoustic score.  With any of these
-        decoders, ``rotations`` / ``rotation_vote``
+        the beam search ranked by that character model, confidences still from the acoustic score.  Or ``pattern`` (a
+        ``recognition.Pattern`` or a str) with ``beam_width``: only readings that match that regular expression in full,
+        a word without one reading "" with confidence 0.  With any of these decoders, ``rotations`` / ``rotation_vote``
         (``recognition.check_rotations``) read every word in each listed quarter turn and keep the most probable
         reading, per word or per image; every returned box then starts at the chosen turn's corner, so box[0] is the
         text's own top-left corner (the same corners, still clockwise).  Injected recognizers get
@@ -340,12 +341,15 @@ class Pipeline:
         if recognition_kwargs is None:
             recognition_kwargs = {}
         if self._native():
-            beam = {k: recognition_kwargs[k] for k in ("beam_width", "top_paths", "lexicon", "language_model")
+            beam = {k: recognition_kwargs[k] for k in ("beam_width", "top_paths", "lexicon", "language_model", "pattern")
                     if k in recognition_kwargs}
-            lexicon = self.recognizer._decoder(beam.get("beam_width"), beam.get("top_paths", 1), beam.get("lexicon"),
-                                               beam.get("language_model"))
+            lexicon, pattern = self.recognizer._decoder(beam.get("beam_width"), beam.get("top_paths", 1),
+                                                        beam.get("lexicon"), beam.get("language_model"),
+                                                        beam.get("pattern"))
             if lexicon is not None:
                 beam["lexicon"] = lexicon                 # compiled once for every sub-batch
+            if pattern is not None:
+                beam["pattern"] = pattern
             vote = recognition_kwargs.get("rotation_vote", "word")
             turns = recognition.check_rotations(recognition_kwargs.get("rotations"), vote)
             if turns is not None:
@@ -396,7 +400,8 @@ class Pipeline:
         return out
 
     def recognize_records(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
-                          top_paths=1, lexicon=None, rotations=None, rotation_vote="word", language_model=None):
+                          top_paths=1, lexicon=None, rotations=None, rotation_vote="word", language_model=None,
+                          pattern=None):
         """``recognize`` without the trip to the host: returns the results as a CUDA float32 tensor of fixed-size
         per-image records, ``(rows, b2o_record_floats(rec_boxes))`` = [count | rec_boxes x (4,2) boxes in source
         pixels | rec_boxes x 48 int8 labels] (``distributed.unpack_blocks`` decodes it; rows beyond ``len(images)``
@@ -407,21 +412,28 @@ class Pipeline:
         (``recognition.check_beam``); a record carries the best path only, so ``top_paths`` > 1 raises ``ValueError``.
         ``lexicon``: every word reads as the most probable entry of that word list (``recognition.check_decoder``), its
         log-probability in the scored layout.  ``language_model`` (a ``recognition.CharLM``, with ``beam_width``): the
-        beam search ranked by that model, the acoustic score in the scored layout.  ``rotations`` / ``rotation_vote``: every word is read in each listed
+        beam search ranked by that model, the acoustic score in the scored layout.  ``pattern`` (a
+        ``recognition.Pattern`` or a str, with ``beam_width``): the best reading that matches it in full, a word without
+        one carrying no labels and -inf in the scored layout.  ``rotations`` / ``rotation_vote``: every word is read in each listed
         quarter turn and the most probable reading kept (``recognition.check_rotations``); the records' boxes start at
         the chosen turn's corner, as ``recognize`` returns them."""
         return self.records_end(self.records_begin(images, rows, rec_boxes, detection_kwargs, scores, beam_width,
-                                                   top_paths, lexicon, rotations, rotation_vote, language_model))
+                                                   top_paths, lexicon, rotations, rotation_vote, language_model,
+                                                   pattern))
 
     def records_begin(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
-                      top_paths=1, lexicon=None, rotations=None, rotation_vote="word", language_model=None):
+                      top_paths=1, lexicon=None, rotations=None, rotation_vote="word", language_model=None,
+                      pattern=None):
         """First half of ``recognize_records``: queues resize/pad, CRAFT and getBoxes and returns at once (no
         synchronisation), so the caller can use the host while the GPU works (``distributed.ShardedStream`` decodes the
         previous batch's words here).  Pass the returned state to ``records_end``."""
-        plain = lexicon is None and language_model is None
+        if pattern is not None:
+            pattern = recognition.check_pattern(pattern, beam_width, top_paths, lexicon, self.recognizer.alphabet,
+                                                language_model)
+        plain = lexicon is None and language_model is None and pattern is None
         lexicon = check_records_decoder(beam_width, top_paths, lexicon,
                                         recognition.DEFAULT_ALPHABET if plain else self.recognizer.alphabet,
-                                        language_model)
+                                        language_model, pattern)
         turns = recognition.check_rotations(rotations, rotation_vote)
         assert self._native(), "recognize_records needs this package's Detector and Recognizer"
         assert len(self.recognizer.alphabet) + 1 <= 127, "record labels travel as int8: alphabets up to 126 characters"
@@ -438,7 +450,7 @@ class Pipeline:
         self.last_stats = {"h2d_bytes": 0, "d2h_bytes": 0}
         state = {"n": n, "rows": rows, "rec_boxes": rec_boxes, "scores": bool(scores), "beam_width": beam_width,
                  "lexicon": lexicon, "rotations": turns, "rotation_vote": rotation_vote,
-                 "language_model": language_model}
+                 "language_model": language_model, "pattern": pattern}
         if n:
             plans = self._plans(images)
             state["st"] = self._stage_detect(images, (max(p[1] for p in plans), max(p[2] for p in plans)), thresholds,
@@ -479,6 +491,7 @@ class Pipeline:
                                                  image_index=bst["image_index"], with_scores=scored,
                                                  beam_width=state.get("beam_width"), lexicon=state.get("lexicon"),
                                                  language_model=state.get("language_model"),
+                                                 pattern=state.get("pattern"),
                                                  rotations=state.get("rotations"),
                                                  rotation_vote=state.get("rotation_vote", "word"))
         if state.get("rotations") is not None:           # the turns are in the rolled boxes the records carry

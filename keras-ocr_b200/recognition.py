@@ -464,12 +464,97 @@ class CharLM:
         return _lib.CharLMDesc(self.order, keys.shape[0], keys.data_ptr(), rows.data_ptr(), self.alpha, self.beta)
 
 
-def check_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET, language_model=None):
+class Pattern:
+    """A regular expression every reading must match in full, enforced inside the CTC prefix beam search
+    (``b2o_crnn_forward_beam_pattern``; DESIGN.md section 1, "Patterns"): a reading is returned only if
+    ``re.fullmatch(regex, reading)`` accepts it.  The syntax is a strict subset of Python's ``re`` -- literals, ``\\``
+    escapes of punctuation, ``.``, ``\\d``, classes with ranges and ``^``, groups, ``|`` and the quantifiers ``?``, ``*``,
+    ``+``, ``{m}``, ``{m,}``, ``{m,n}`` with n <= 48 -- over ``alphabet``; everything else raises ``ValueError`` naming
+    its position (``patterns``).  So do an automaton past 4096 states and a pattern whose shortest reading is longer
+    than 48 characters.
+
+    The pattern is compiled once on the host to its minimal trimmed DFA and uploaded lazily, once per CUDA device, so
+    one object serves every rank of a sharded run.  A plain ``str`` is accepted wherever a ``Pattern`` is and is
+    compiled for that call."""
+
+    def __init__(self, regex, alphabet=DEFAULT_ALPHABET):
+        from . import patterns
+        self.regex, self.alphabet = regex, alphabet
+        self.trans, self.dist, self.start = patterns.compile_pattern(regex, alphabet)
+        self._index = {ch: i for i, ch in enumerate(alphabet)}
+        self._device = {}
+
+    @property
+    def n_states(self):
+        return int(self.trans.shape[0])
+
+    def __repr__(self):
+        return f"Pattern({self.regex!r}, {self.n_states} states)"
+
+    def fullmatch(self, text):
+        """Whether the DFA accepts ``text`` (a str), run on the host."""
+        q = self.start
+        for ch in text:
+            c = self._index.get(ch)
+            if c is None:
+                return False
+            q = int(self.trans[q, c])
+            if q < 0:
+                return False
+        return bool(self.dist[q] == 0)
+
+    def host_tables(self):
+        """(trans (n, K-1) int16, -1 where there is no transition; dist (n,) uint8, the fewest labels to an accepting
+        state, 0 for an accepting one, saturated at 255; start)."""
+        return self.trans, self.dist, self.start
+
+    def device_arrays(self, device):
+        """(trans, dist) CUDA tensors on ``device``, uploaded on first use."""
+        device = torch.device(device)
+        if device not in self._device:
+            self._device[device] = (torch.from_numpy(self.trans).to(device), torch.from_numpy(self.dist).to(device))
+        return self._device[device]
+
+    def descriptor(self, device):
+        """The ``b2o_pattern`` of this pattern on ``device`` (``_lib.PatternDesc``)."""
+        trans, dist = self.device_arrays(device)
+        return _lib.PatternDesc(self.n_states, self.start, trans.data_ptr(), dist.data_ptr())
+
+
+def check_pattern(pattern, beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET, language_model=None):
+    """Validates a pattern choice before anything is launched (``ValueError`` otherwise) and returns the ``Pattern`` to
+    decode with, or None for ``pattern=None``.  A ``Pattern`` over ``alphabet`` or a ``str`` (compiled here) constrains
+    the beam search: it needs ``beam_width`` and does not combine with a lexicon or a language model."""
+    if pattern is None:
+        return None
+    if not isinstance(pattern, (Pattern, str)):
+        raise ValueError(f"pattern must be a Pattern or a str, got {type(pattern).__name__}")
+    if beam_width is None:
+        raise ValueError("a pattern needs beam search: pass beam_width")
+    if lexicon is not None:
+        raise ValueError("lexicon and pattern are mutually exclusive")
+    if language_model is not None:
+        raise ValueError("language_model and pattern do not combine in one search")
+    check_beam(beam_width, top_paths)
+    if isinstance(pattern, str):
+        return Pattern(pattern, alphabet)
+    if pattern.alphabet != alphabet:
+        raise ValueError("the pattern was compiled for another alphabet than the recognizer's")
+    return pattern
+
+
+def check_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET, language_model=None,
+                  pattern=None):
     """Validates a decoder choice before anything is launched (``ValueError`` otherwise) and returns the ``Lexicon`` to
     decode with, or None.  Without a lexicon this is ``check_beam``.  With one (a ``Lexicon`` over ``alphabet``, or a
     list / tuple of strings, compiled here): ``beam_width`` must be None and 1 <= ``top_paths`` <= 128.
     ``language_model`` (a ``CharLM`` over ``alphabet``) ranks the beam search by that model
-    (``b2o_crnn_forward_beam_lm``): it needs ``beam_width`` and does not combine with a lexicon."""
+    (``b2o_crnn_forward_beam_lm``): it needs ``beam_width`` and does not combine with a lexicon.
+    ``pattern`` (a ``Pattern`` over ``alphabet`` or a str): the rules of ``check_pattern``, which returns the compiled
+    pattern."""
+    if pattern is not None:
+        check_pattern(pattern, beam_width, top_paths, lexicon, alphabet, language_model)
+        return None
     if language_model is not None:
         if not isinstance(language_model, CharLM):
             raise ValueError(f"language_model must be a CharLM, got {type(language_model).__name__}")
@@ -798,14 +883,17 @@ class Recognizer:
                                 None if logp is None else logp.data_ptr(), stream)
         return out, logp
 
-    def _decoder(self, beam_width, top_paths, lexicon, language_model=None):
-        """``check_decoder`` for this recognizer's alphabet."""
+    def _decoder(self, beam_width, top_paths, lexicon, language_model=None, pattern=None):
+        """``check_decoder`` for this recognizer's alphabet: (the compiled lexicon or None, the compiled pattern or
+        None)."""
+        if pattern is not None:
+            return None, check_pattern(pattern, beam_width, top_paths, lexicon, self.alphabet, language_model)
         plain = lexicon is None and language_model is None
         return check_decoder(beam_width, top_paths, lexicon, DEFAULT_ALPHABET if plain else self.alphabet,
-                             language_model)
+                             language_model), None
 
     def predict_device(self, crnn_in, with_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                       language_model=None):
+                       language_model=None, pattern=None):
         """CRNN + greedy CTC.  crnn_in: (B,200,31) fp16 -> labels (B,48) int32 (-1 padded).  ``with_scores``: returns
         (labels, logp) with logp (B,) float32 the greedy path's log-probability (``b2o_crnn_forward_scored``).
         ``beam_width``: CTC prefix beam search instead (``b2o_crnn_forward_beam``, see ``check_beam``), logp = the beam
@@ -813,20 +901,23 @@ class Recognizer:
         list of strings, see ``check_decoder``): the ``top_paths`` most probable entries instead
         (``b2o_crnn_forward_lexicon``), logp = their CTC forward log-probabilities, in the same shapes.
         ``language_model`` (a ``CharLM``, with ``beam_width``): the beam search ranked by that model
-        (``b2o_crnn_forward_beam_lm``); logp stays the acoustic beam score of each reading."""
-        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
+        (``b2o_crnn_forward_beam_lm``); logp stays the acoustic beam score of each reading.  ``pattern`` (a
+        ``Pattern`` or a str, with ``beam_width``): only readings that match it in full (``b2o_crnn_forward_beam_pattern``),
+        logp their beam scores; slots past a crop's matching readings are -1 with logp -inf."""
+        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
         b = crnn_in.shape[0]
         lead = (b,) if top_paths == 1 else (b, top_paths)
         labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
         logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
-        self._forward(crnn_in, labels, logp, beam_width, top_paths, lexicon, language_model=language_model)
+        self._forward(crnn_in, labels, logp, beam_width, top_paths, lexicon, language_model=language_model,
+                      pattern=pattern)
         return (labels, logp) if with_scores else labels
 
     def _forward(self, crnn_in, labels, logp, beam_width, top_paths, lexicon, spans=None, theta=None,
-                 language_model=None, fused=None):
+                 language_model=None, fused=None, pattern=None):
         """The CRNN and the decoder of ``predict_device`` into caller-allocated ``labels`` / ``logp`` (None: greedy
         without scores, or scores not written); ``lexicon`` is already compiled.  With ``language_model``, ``fused``
-        (B,P) float32 or None receives every reading's F_end.  ``spans`` (B,P,48,2) int32: also the
+        (B,P) float32 or None receives every reading's F_end.  ``pattern`` is already compiled.  ``spans`` (B,P,48,2) int32: also the
         characters' emission spans of every reading (``b2o_crnn_align``) and, with an STN, its ``theta`` (B,6) float32;
         the greedy forward then keeps its logits (``b2o_crnn_forward_logits``)."""
         b = crnn_in.shape[0]
@@ -848,6 +939,10 @@ class Recognizer:
                                           language_model.descriptor(self.device), labels.data_ptr(), logp_ptr,
                                           fused.data_ptr() if fused is not None else None, ws.data_ptr(), nbytes,
                                           stream)
+        elif pattern is not None:
+            self.ctx.crnn_forward_beam_pattern(crnn_in.data_ptr(), b, int(beam_width), int(top_paths),
+                                               pattern.descriptor(self.device), labels.data_ptr(), logp_ptr,
+                                               ws.data_ptr(), nbytes, stream)
         elif beam_width is not None:
             self.ctx.crnn_forward_beam(crnn_in.data_ptr(), b, int(beam_width), int(top_paths), labels.data_ptr(),
                                        logp_ptr, ws.data_ptr(), nbytes, stream)
@@ -864,7 +959,7 @@ class Recognizer:
                                 theta.data_ptr() if theta is not None else None, ws.data_ptr(), nbytes, stream)
         self._last_ws = (ws, b) if self.keep_workspace else None
 
-    def _predict_aligned(self, crnn_in, beam_width, top_paths, lexicon, language_model=None):
+    def _predict_aligned(self, crnn_in, beam_width, top_paths, lexicon, language_model=None, pattern=None):
         """``predict_device(with_scores=True)`` plus every reading's spans: (labels (B,P,48), logp (B,P), spans
         (B,P,48,2) int32, theta (B,6) float32 or None without an STN)."""
         b, p = crnn_in.shape[0], int(top_paths)
@@ -872,7 +967,7 @@ class Recognizer:
         logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
         spans = torch.empty((b, p, STEPS, 2), dtype=torch.int32, device=self.device)
         theta = torch.empty((b, 6), dtype=torch.float32, device=self.device) if self.stn else None
-        self._forward(crnn_in, labels, logp, beam_width, p, lexicon, spans, theta, language_model)
+        self._forward(crnn_in, labels, logp, beam_width, p, lexicon, spans, theta, language_model, pattern=pattern)
         return labels, logp, spans, theta
 
     def char_cells_device(self, spans, theta, boxes=None, turns=None):
@@ -894,18 +989,19 @@ class Recognizer:
         return out
 
     def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                        return_char_boxes=False, language_model=None):
+                        return_char_boxes=False, language_model=None, pattern=None):
         """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str].
         ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``.  ``beam_width``: beam search
         decoding (``check_beam``); with ``top_paths = P > 1`` each text is a list of P strings and each confidence a
         list of P floats, best first (``decode_paths``).  ``lexicon``: the most probable entries of a word list instead
         (``check_decoder``), in the same shapes; a confidence is exp(the entry's CTC log-probability), clipped to 1.
         ``language_model`` (a ``CharLM``, with ``beam_width``): the beam search ranked by that character model; the
-        confidences stay exp(the acoustic beam score).
+        confidences stay exp(the acoustic beam score).  ``pattern`` (a ``Pattern`` or a str, with ``beam_width``): only
+        readings that match it in full; a word with no matching reading reads "" with confidence 0.
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells (``b2o_char_cells``), an
         (n,4,2) float32 array for a text of n characters (a list of P arrays with ``top_paths = P > 1``), in the crop's
         200 x 31 frame: (text, cells) or (text, confidence, cells)."""
-        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
+        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
         t = crops if isinstance(crops, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(crops))
         t = t.to(self.device).contiguous()
         b = t.shape[0]
@@ -915,7 +1011,8 @@ class Recognizer:
         crnn_in = torch.empty((b, TARGET_WIDTH, TARGET_HEIGHT) + ((3,) if self.color else ()), dtype=torch.float16, device=self.device)
         self.ctx.crops_to_input(t.data_ptr(), b, crnn_in.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream,
                                 color=self.color)
-        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model}
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
+                "pattern": pattern}
         if return_char_boxes:
             labels, logp, spans, theta = self._predict_aligned(crnn_in, **beam)
             return self._with_cells(labels, logp, self.char_cells_device(spans, theta), top_paths, return_scores)
@@ -932,27 +1029,27 @@ class Recognizer:
         boxes = char_boxes_host(cells.cpu().numpy(), texts)
         return list(zip(texts, conf, boxes)) if return_scores else list(zip(texts, boxes))
 
-    def recognize(self, image, beam_width=None, top_paths=1, lexicon=None, language_model=None):
+    def recognize(self, image, beam_width=None, top_paths=1, lexicon=None, language_model=None, pattern=None):
         """Recognize text from a single pre-cropped image (reference recognition.py:467-489): fit to
         200x31 with zero fill (host, as upstream), gray conversion, then the CUDA CRNN.  ``beam_width`` / ``top_paths`` /
-        ``lexicon`` / ``language_model``: as ``recognize_crops``."""
+        ``lexicon`` / ``language_model`` / ``pattern``: as ``recognize_crops``."""
         import cv2
 
-        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
+        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
         image = tools.read_and_fit(filepath_or_array=image, width=TARGET_WIDTH, height=TARGET_HEIGHT, cval=0)
         if not self.color and image.ndim == 3 and image.shape[-1] == 3:      # recognition.py:481-483
             image = cv2.cvtColor(image, code=cv2.COLOR_RGB2GRAY)
         return self.recognize_crops(np.ascontiguousarray(image.reshape((1, TARGET_HEIGHT, TARGET_WIDTH) + ((3,) if self.color else ()))),
                                     beam_width=beam_width, top_paths=top_paths, lexicon=lexicon,
-                                    language_model=language_model)[0]
+                                    language_model=language_model, pattern=pattern)[0]
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
                                     with_scores=False, beam_width=None, top_paths=1, lexicon=None, rotations=None,
                                     rotation_vote="word", char_boxes=False, polys=None, points=None, max_windows=1,
-                                    windows=None, language_model=None):
+                                    windows=None, language_model=None, pattern=None):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
         (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon`` /
-        ``language_model``: see ``predict_device``).
+        ``language_model`` / ``pattern``: see ``predict_device``).
 
         ``rotations`` / ``rotation_vote`` (``check_rotations``): every box is cut and decoded once per listed turn, one
         turn after another (the CRNN workspace stays that of B crops), and ``b2o_select_rotation`` keeps one reading per
@@ -979,7 +1076,7 @@ class Recognizer:
         ``b2o_window_counts`` gives them (``Pipeline.recognize`` reads them back with the box counts; ``ValueError`` for
         another shape or a count outside [1, max_windows]); None: computed here and read back, one more
         synchronisation."""
-        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
+        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
         turns = check_rotations(rotations, rotation_vote)
         max_windows = check_windows(max_windows, beam_width, lexicon, turns, char_boxes, polys is not None)
         if polys is not None and (turns is not None or char_boxes):
@@ -1014,31 +1111,32 @@ class Recognizer:
         if polys is not None:
             crnn_in, _ = self.warp_polys_device(gray, polys[:total], points[:total], image_index[:total])
             return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
-                                       lexicon=lexicon, language_model=language_model)
+                                       lexicon=lexicon, language_model=language_model, pattern=pattern)
         if turns is not None:
             return self._recognize_turns(gray, flat[:total], image_index[:total], len(counts), boxes, turns,
                                          rotation_vote, with_scores, beam_width, top_paths, lexicon, char_boxes,
-                                         language_model)
+                                         language_model, pattern)
         if char_boxes:
             labels, logp, spans, cells = self._read_cells(gray, flat[:total], image_index[:total], beam_width,
-                                                          top_paths, lexicon, language_model)
+                                                          top_paths, lexicon, language_model, pattern)
             return (labels, logp, spans, cells) if with_scores else (labels, spans, cells)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
         return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
-                                   lexicon=lexicon, language_model=language_model)
+                                   lexicon=lexicon, language_model=language_model, pattern=pattern)
 
-    def _read_cells(self, gray, flat, image_index, beam_width, top_paths, lexicon, language_model=None):
+    def _read_cells(self, gray, flat, image_index, beam_width, top_paths, lexicon, language_model=None, pattern=None):
         """Warp + CRNN + decoder + alignment + cells of one pass: (labels, logp, spans, cells) in the shapes of
         ``recognize_from_boxes_device``."""
         crnn_in, _ = self.warp_device(gray, flat, image_index)
-        labels, logp, spans, theta = self._predict_aligned(crnn_in, beam_width, top_paths, lexicon, language_model)
+        labels, logp, spans, theta = self._predict_aligned(crnn_in, beam_width, top_paths, lexicon, language_model,
+                                                           pattern)
         cells = self.char_cells_device(spans, theta, flat)
         if top_paths == 1:
             labels, logp, spans, cells = labels[:, 0], logp[:, 0], spans[:, 0], cells[:, 0]
         return labels, logp, spans, cells
 
     def _recognize_turns(self, gray, flat, image_index, n_images, table, turns, vote, with_scores, beam_width,
-                         top_paths, lexicon, char_boxes=False, language_model=None):
+                         top_paths, lexicon, char_boxes=False, language_model=None, pattern=None):
         """Warp + CRNN + decoder for each turn into its slot of one (R,B,P,48) / (R,B,P) stack, then
         ``b2o_select_rotation``, which also rolls ``flat`` and ``table`` (None: no table) in place.  ``char_boxes``: each
         turn's spans and theta are stacked alike, and the chosen turn's cells are built from the boxes as they were cut.
@@ -1057,7 +1155,7 @@ class Recognizer:
             crnn_in, _ = self.warp_device(gray, flat, image_index, turn=turn)
             self._forward(crnn_in, labels_all[j], logp_all[j], beam_width, p, lexicon,
                           None if spans_all is None else spans_all[j], None if theta_all is None else theta_all[j],
-                          language_model, None if fused_all is None else fused_all[j])
+                          language_model, None if fused_all is None else fused_all[j], pattern)
         labels = torch.empty((b, p, STEPS), dtype=torch.int32, device=self.device)
         logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
         chosen = torch.empty((b,), dtype=torch.int32, device=self.device)
@@ -1084,10 +1182,10 @@ class Recognizer:
     # ------------------------------------------------------------------ reference API
     def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
                              rotations=None, rotation_vote="word", return_char_boxes=False, max_windows=1,
-                             language_model=None, **kwargs) -> typing.List[typing.List[str]]:
+                             language_model=None, pattern=None, **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
         (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon`` /
-        ``language_model``: as ``recognize_crops``; with rotations the vote compares the language model's fused scores.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
+        ``language_model`` / ``pattern``: as ``recognize_crops``; with rotations the vote compares the language model's fused scores.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
         most probable reading kept, per word or per image (one box group), see ``check_rotations``.
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells, an (n,4,2) float32 array
         of quads in the image's pixels for a text of n characters (a list of P arrays with ``top_paths = P > 1``):
@@ -1099,7 +1197,7 @@ class Recognizer:
         (``ValueError``).
         ``max_windows``: every box wider than the 200 x 31 crop at full height is read in up to that many overlapping
         windows and their steps stitched into one reading (``check_windows``; greedy decoding, boxes only)."""
-        lexicon = self._decoder(beam_width, top_paths, lexicon, language_model)
+        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
         turns = check_rotations(rotations, rotation_vote)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
@@ -1109,7 +1207,7 @@ class Recognizer:
         max_windows = check_windows(max_windows, beam_width, lexicon, turns, return_char_boxes, polygons)
         if polygons:
             return self._recognize_polygons(images, box_groups, entries, return_scores, turns, return_char_boxes,
-                                            beam_width, top_paths, lexicon, language_model)
+                                            beam_width, top_paths, lexicon, language_model, pattern)
         images_t = _as_device_images(images, self.device)
         counts = np.array([len(b) for b in box_groups], dtype=np.int64)
         if counts.sum() == 0:
@@ -1122,7 +1220,8 @@ class Recognizer:
         flat_t = torch.from_numpy(np.ascontiguousarray(flat)).to(self.device)
         idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
         gray = images_t if self.color else self.gray_device(images_t)
-        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model}
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
+                "pattern": pattern}
         if return_char_boxes:
             if turns is not None:
                 labels, logp, _, _, cells = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns,
@@ -1152,7 +1251,7 @@ class Recognizer:
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]
 
     def _recognize_polygons(self, images, box_groups, entries, return_scores, turns, char_boxes, beam_width, top_paths,
-                            lexicon, language_model=None):
+                            lexicon, language_model=None, pattern=None):
         """``recognize_from_boxes`` for box groups that hold polygons: 4-point entries are rectified as
         ``tools.rectify_boxes`` does and cut as boxes, the others along their polygon, all in one ``b2o_warp_polys``."""
         if turns is not None or char_boxes:
@@ -1169,7 +1268,8 @@ class Recognizer:
         gray = images_t if self.color else self.gray_device(images_t)
         crnn_in, _ = self.warp_polys_device(gray, torch.from_numpy(polys).to(self.device),
                                             torch.from_numpy(points).to(self.device), idx)
-        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model}
+        beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
+                "pattern": pattern}
         if return_scores:
             labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
             predictions = list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
