@@ -136,6 +136,35 @@ int b2o_craft_forward_until(b2o_ctx* ctx, const uint8_t* img_dev, int n, int h, 
                             void* ws_dev, size_t ws_bytes, int last_step, void* stream);
 int b2o_craft_tap(b2o_ctx* ctx, const char* name, const void* ws_dev, int n, int h, int w, void* out_dev,
                   size_t out_bytes, void* stream);
+/* b2o_craft_forward refuses (B2O_ERR_ARG) an image of more than B2O_CRAFT_MAX_PIXELS pixels (h * w): its 64-channel
+ * full-resolution maps would pass 2^31 elements per image.  Larger pages run over tiles (below).               */
+#define B2O_CRAFT_MAX_PIXELS (1 << 25)
+
+/* Tiled detection (DESIGN.md section 1, "Tiles"): CRAFT over overlapping square tiles of a padded (n, hp, wp, 3)
+ * batch, whose cores are stitched into one (n, hp/2, wp/2, 2) score map.  One grid serves every image; per axis of
+ * length L: tile extent t = min(tile_size, L), stride s = t - 2 margin, origins o_k = k s (multiples of 32), the fewest
+ * tiles that cover L.  The core of tile k is [o_k + margin, o_k + t - margin), except that the first starts at 0 and
+ * the last ends at L: the cores partition [0, L).  In the score map every range is halved (floor).
+ * b2o_tile_plan: pure host function (no context, no GPU).  tile_size a multiple of 32 with 4 margin <= tile_size <= 2048,
+ * margin >= 0 a multiple of 16, hp, wp >= 32, otherwise B2O_ERR_ARG and *plan is not written.                  */
+typedef struct {
+  int hp, wp, tile_size, margin;
+  int t_h, t_w;            /* tile extent per axis: min(tile_size, hp), min(tile_size, wp) */
+  int s_h, s_w;            /* stride per axis: t - 2 margin */
+  int n_h, n_w;            /* tiles per axis; tiles per image = n_h * n_w */
+} b2o_tiles;
+int b2o_tile_plan(int hp, int wp, int tile_size, int margin, b2o_tiles* plan);
+/* b2o_cut_tiles: tiles [first_tile, first_tile + n_tiles) of img_dev (n, plan->hp, plan->wp, 3) uint8, numbered image by
+ * image, then tile row, then tile column, into tiles_dev (n_tiles, t_h, t_w, 3) uint8 (16-byte aligned); pixels past the
+ * page are 255, as b2o_resize_pad pads.  b2o_stitch_tiles: the cores of those tiles' scores, tile_scores_dev (n_tiles,
+ * t_h/2, t_w/2, 2) float32, copied bit for bit into scores_dev (n, hp/2, wp/2, 2) float32; over the chunks of one batch
+ * every score is written exactly once and nothing else is.  Both: plan must be b2o_tile_plan's for its own hp, wp,
+ * tile_size, margin, and 0 <= first_tile, n_tiles >= 1, first_tile + n_tiles <= n * n_h * n_w, otherwise B2O_ERR_ARG
+ * and nothing is enqueued.                                                                                     */
+int b2o_cut_tiles(b2o_ctx* ctx, const uint8_t* img_dev, int n, const b2o_tiles* plan, int first_tile, int n_tiles,
+                  uint8_t* tiles_dev, void* stream);
+int b2o_stitch_tiles(b2o_ctx* ctx, const float* tile_scores_dev, int n, const b2o_tiles* plan, int first_tile,
+                     int n_tiles, float* scores_dev, void* stream);
 
 /* getBoxes (detection.py:207-287).  scores: (n,hs,ws,2) float32.  Writes, per image i,
  * counts[i] = number of boxes found (may exceed max_boxes: then only the first max_boxes are

@@ -31,6 +31,7 @@ POLY_POINTS = 2 * (MAX_POLY_SEGMENTS + 1)   # points per entry of a dense polygo
 MAX_WINDOWS = 16              # B2O_MAX_WINDOWS
 WINDOW_STRIDE = 136           # B2O_WINDOW_STRIDE
 WINDOW_SHRINK = 8             # B2O_WINDOW_SHRINK
+CRAFT_MAX_PIXELS = 1 << 25    # B2O_CRAFT_MAX_PIXELS
 
 
 class B2OError(RuntimeError):
@@ -85,6 +86,14 @@ class PatternDesc(ctypes.Structure):
 
 _patp = _c.POINTER(PatternDesc)
 
+
+class TilePlan(ctypes.Structure):
+    """b2o_tiles (include/b2ocr.h), field for field."""
+    _fields_ = [(name, _i) for name in ("hp", "wp", "tile_size", "margin", "t_h", "t_w", "s_h", "s_w", "n_h", "n_w")]
+
+
+_tilep = _c.POINTER(TilePlan)
+
 # name -> (restype, argtypes); mirrors include/b2ocr.h one to one
 SIGNATURES = {
     "b2o_version": (_i, []),
@@ -108,6 +117,9 @@ SIGNATURES = {
     "b2o_craft_forward": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "b2o_craft_forward_until": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _i, _vp]),
     "b2o_craft_tap": (_i, [_vp, _c.c_char_p, _vp, _i, _i, _i, _vp, _sz, _vp]),
+    "b2o_tile_plan": (_i, [_i, _i, _i, _i, _tilep]),
+    "b2o_cut_tiles": (_i, [_vp, _vp, _i, _tilep, _i, _i, _vp, _vp]),
+    "b2o_stitch_tiles": (_i, [_vp, _vp, _i, _tilep, _i, _i, _vp, _vp]),
     "b2o_boxes_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "b2o_get_boxes": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _i, _vp, _sz, _vp]),
     "b2o_get_boxes_scored": (_i, [_vp, _vp, _i, _i, _i, _f, _f, _f, _i, _vp, _vp, _vp, _i, _vp, _sz, _vp]),
@@ -209,6 +221,15 @@ def conv_plan(n, h, w, cin, cout, ksize, dilation=1, out_f32=False, pool=False, 
     if load_library().b2o_conv_plan_test(ctypes.byref(desc), ctypes.byref(plan)) != 0:
         return None
     return {name: getattr(plan, name) for name, _ in _ConvPlan._fields_}
+
+
+def tile_plan(hp, wp, tile_size, margin):
+    """b2o_tile_plan (no GPU needed): the tile grid of a padded (hp, wp) batch as a ``TilePlan``, or None where the
+    library refuses the parameters."""
+    plan = TilePlan()
+    if load_library().b2o_tile_plan(int(hp), int(wp), int(tile_size), int(margin), ctypes.byref(plan)) != 0:
+        return None
+    return plan
 
 
 def _tensor_array(weights):
@@ -325,6 +346,14 @@ class Context:
         message."""
         self._check(self.lib.b2o_craft_tap(self.handle, name.encode(), ws, n, h, w, out, out_bytes, stream),
                     "b2o_craft_tap")
+
+    def cut_tiles(self, img, n, plan, first_tile, n_tiles, tiles, stream):
+        self._check(self.lib.b2o_cut_tiles(self.handle, img, n, ctypes.byref(plan), first_tile, n_tiles, tiles, stream),
+                    "b2o_cut_tiles")
+
+    def stitch_tiles(self, tile_scores, n, plan, first_tile, n_tiles, scores, stream):
+        self._check(self.lib.b2o_stitch_tiles(self.handle, tile_scores, n, ctypes.byref(plan), first_tile, n_tiles,
+                                              scores, stream), "b2o_stitch_tiles")
 
     def boxes_workspace_bytes(self, n, hs, ws, max_boxes):
         return int(self.lib.b2o_boxes_workspace_bytes(n, hs, ws, max_boxes))

@@ -620,6 +620,13 @@ extern "C" int b2o_craft_forward_until(b2o_ctx* ctx, const uint8_t* img, int n, 
     ctx->set_error("b2o_craft_forward: bad argument");
     return B2O_ERR_ARG;
   }
+  // the glue kernels and the conv engine index inside one image's maps with 32-bit integers in places; the largest
+  // per-image map is a full-resolution 64-channel one, h * w * 64 elements, which stays below 2^31 up to this bound
+  if (static_cast<long long>(h) * w > B2O_CRAFT_MAX_PIXELS) {
+    ctx->set_error("b2o_craft_forward: more than 2^25 pixels per image (h * w = " +
+                   std::to_string(static_cast<long long>(h) * w) + "); detect a page this large over tiles (tile_size)");
+    return B2O_ERR_ARG;
+  }
   const CraftPlan p = plan_craft(n, h, w);
   if (ws_bytes < p.bytes) { ctx->set_error("b2o_craft_forward: workspace too small"); return B2O_ERR_WORKSPACE; }
   ctx->craft_step = -1;

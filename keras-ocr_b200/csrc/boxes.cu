@@ -19,7 +19,7 @@
 
 namespace {
 
-constexpr int kMaxHullRows = 2048;      // score maps are at most 1024 rows (max_size 2048 / 2)
+constexpr int kRowTable = 1024;         // ROI rows of the shared per-row blob extents; taller ROIs use global scratch
 
 struct Component {                       // one kept connected component
   int root, x, y, w, h, area;
@@ -415,8 +415,18 @@ __device__ __forceinline__ Roi roi_of(const Component& c, int hs, int ws) {
 // Whether a component can be handled by the small-tile launch: both bit planes and the hull scratch that later
 // reuses plane B (worst case 2*rh hull points: 56 bytes per row + the padding of the index arrays) fit `words` words.
 __device__ __forceinline__ bool fits_words(const Roi& r, int words) {
-  return r.plane_words <= words && 56 * r.rh + 64 <= 4 * words;
+  return r.plane_words <= words && 56 * r.rh + 64 <= 4 * words;      // rh <= hs <= 2^24 (get_boxes)
 }
+
+// Whether a component's row tables (over kRowTable ROI rows) or hull stack (56 bytes per ROI row, see fits_words) do not
+// fit shared memory: it then keeps both in its image's tall scratch, under the image's lock with the global planes.
+// Never true on a map of at most kRowTable rows (56 * 1024 + 64 bytes fit the 96 KB of pass 2).
+__device__ __forceinline__ bool tall_roi(const Roi& r, int smem_plane_words) {
+  return r.rh > kRowTable || 56LL * r.rh + 64 > 8LL * smem_plane_words;
+}
+
+// Per-image tall scratch in 32-bit words: row_min and row_max (hs each), then the hull stack (56 bytes per row + 64).
+__host__ __device__ __forceinline__ size_t tall_words(int hs) { return 2 * static_cast<size_t>(hs) + 14 * static_cast<size_t>(hs) + 16; }
 
 // --------------------------------------------------------------------------- polygon stage (b2o_get_boxes_poly)
 // Per kept component, after its box: a polygon along the centre line of its filled blob B (DESIGN.md section 1).
@@ -632,14 +642,15 @@ __device__ __forceinline__ uint32_t roi_edge(int ry, int k, int rh, int stride, 
 }
 
 // One component -> one quad (POLY: and its polygon, poly_of_blob).  `dyn_smem` holds two planes of `smem_plane_words` words; a component whose planes
-// do not fit works on the per-image global scratch planes instead (serialised by a per-image lock).
-template <bool POLY>
+// do not fit works on the per-image global scratch planes instead (serialised by a per-image lock).  TALL: the component
+// may need the tall scratch (pass 2 only: pass 1 takes components whose ROI has at most 145 rows).
+template <bool POLY, bool TALL>
 __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* __restrict__ label, int hs, int ws,
                                   const Component c, int img, float* __restrict__ out,
                                   uint32_t* __restrict__ big_planes, int* __restrict__ big_locks,
-                                  uint32_t* dyn_smem, int smem_plane_words, float* __restrict__ poly_out,
-                                  int* __restrict__ points_out) {
-  __shared__ int row_min[kMaxHullRows / 2], row_max[kMaxHullRows / 2];   // per blob row (<= 1024 rows)
+                                  uint32_t* __restrict__ tall_scratch, uint32_t* dyn_smem, int smem_plane_words,
+                                  float* __restrict__ poly_out, int* __restrict__ points_out) {
+  __shared__ int row_min_s[kRowTable], row_max_s[kRowTable];   // per blob row (ROIs of at most kRowTable rows)
   __shared__ int first_word;
   __shared__ float pbox[8];                  // the box in score-map pixels, for the polygon stage
   const int hw = hs * ws;
@@ -653,7 +664,17 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
   const int ksz = 1 + niter, grow_hi = ksz / 2, grow_lo = ksz - 1 - grow_hi;
 
   uint32_t *A, *B;
-  bool big = plane_words > smem_plane_words;
+  // a tall ROI keeps its row tables and hull stack in global scratch, taken with the big planes under the image's lock
+  const bool tall = TALL && tall_roi(roi, smem_plane_words);
+  bool big = plane_words > smem_plane_words || tall;
+  int *row_min = row_min_s, *row_max = row_max_s;
+  uint32_t* tall_hull = nullptr;
+  if (tall) {
+    uint32_t* t = tall_scratch + static_cast<size_t>(img) * tall_words(hs);
+    row_min = reinterpret_cast<int*>(t);
+    row_max = row_min + hs;
+    tall_hull = t + 2 * static_cast<size_t>(hs);
+  }
   if (!big) {
     A = dyn_smem; B = dyn_smem + smem_plane_words;
   } else {
@@ -802,13 +823,13 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
     row_min[r] = lo; row_max[r] = hi;
   }
   __syncthreads();
-  if (big && !POLY) { if (threadIdx.x == 0) atomicExch(big_locks + img, 0); }   // the polygon stage still reads A
+  if (big && !POLY && !tall) { if (threadIdx.x == 0) atomicExch(big_locks + img, 0); }   // the polygon stage still reads A
 
   if (threadIdx.x == 0) {
     // hull stack lives in the (now free) plane B / dynamic smem: 2*rh points + 3*2*rh floats
     // Convex hull in cv2.convexHull(clockwise=False) order of the contour: right side top->bottom,
     // then left side bottom->top, ending at the blob's first raster pixel.
-    int* hx = reinterpret_cast<int*>(big ? reinterpret_cast<uint32_t*>(dyn_smem) : B);
+    int* hx = reinterpret_cast<int*>(tall ? tall_hull : big ? reinterpret_cast<uint32_t*>(dyn_smem) : B);
     int* hy = hx + 2 * rh + 4;
     int n = 0, r_first = -1, r_last = -1;
     for (int r = 0; r < rh; ++r) if (row_min[r] >= 0) { if (r_first < 0) r_first = r; r_last = r; }
@@ -888,6 +909,9 @@ __device__ void quad_of_component(const uint8_t* __restrict__ mask, const int* _
     __syncthreads();
     poly_of_blob(A, plane_words, stride, sx, sy, pbox, poly_out, points_out);
     if (big) { __syncthreads(); if (threadIdx.x == 0) atomicExch(big_locks + img, 0); }
+  } else if (tall) {
+    __syncthreads();                         // thread 0's hull walk over the tall scratch is done
+    if (threadIdx.x == 0) atomicExch(big_locks + img, 0);
   }
 }
 
@@ -898,8 +922,8 @@ __global__ void __launch_bounds__(256)
 quads_kernel(const uint8_t* __restrict__ mask, const int* __restrict__ label, int hs, int ws,
              const Component* __restrict__ comps, const int* __restrict__ counts, int max_boxes,
              float* __restrict__ boxes, uint32_t* __restrict__ big_planes, int* __restrict__ big_locks,
-             int smem_plane_words, int* __restrict__ queue, int* __restrict__ queue_len, float* __restrict__ polys,
-             int* __restrict__ points) {
+             uint32_t* __restrict__ tall_scratch, int smem_plane_words, int* __restrict__ queue,
+             int* __restrict__ queue_len, float* __restrict__ polys, int* __restrict__ points) {
   extern __shared__ uint32_t dyn_smem[];
   const int img = blockIdx.y, slot = blockIdx.x;
   int cnt = counts[img];
@@ -911,8 +935,8 @@ quads_kernel(const uint8_t* __restrict__ mask, const int* __restrict__ label, in
     if (threadIdx.x == 0) queue[atomicAdd(queue_len, 1)] = static_cast<int>(id);
     return;
   }
-  quad_of_component<POLY>(mask, label, hs, ws, c, img, boxes + id * 8, big_planes, big_locks, dyn_smem, smem_plane_words,
-                    polys ? polys + id * 2 * kPolyPoints : nullptr, points ? points + id : nullptr);
+  quad_of_component<POLY, false>(mask, label, hs, ws, c, img, boxes + id * 8, big_planes, big_locks, tall_scratch, dyn_smem,
+                          smem_plane_words, polys ? polys + id * 2 * kPolyPoints : nullptr, points ? points + id : nullptr);
 }
 
 // Pass 2, a few blocks with the large planes walking the queue of pass 1 (normally empty).
@@ -920,15 +944,15 @@ template <bool POLY>
 __global__ void __launch_bounds__(256)
 quads_queue_kernel(const uint8_t* __restrict__ mask, const int* __restrict__ label, int hs, int ws,
                    const Component* __restrict__ comps, int max_boxes, float* __restrict__ boxes,
-                   uint32_t* __restrict__ big_planes, int* __restrict__ big_locks, int smem_plane_words,
-                   const int* __restrict__ queue, const int* __restrict__ queue_len, float* __restrict__ polys,
-                   int* __restrict__ points) {
+                   uint32_t* __restrict__ big_planes, int* __restrict__ big_locks, uint32_t* __restrict__ tall_scratch,
+                   int smem_plane_words, const int* __restrict__ queue, const int* __restrict__ queue_len,
+                   float* __restrict__ polys, int* __restrict__ points) {
   extern __shared__ uint32_t dyn_smem[];
   const int len = *queue_len;
   for (int i = blockIdx.x; i < len; i += gridDim.x) {
     const int id = queue[i];
-    quad_of_component<POLY>(mask, label, hs, ws, comps[id], id / max_boxes, boxes + static_cast<size_t>(id) * 8, big_planes,
-                      big_locks, dyn_smem, smem_plane_words,
+    quad_of_component<POLY, true>(mask, label, hs, ws, comps[id], id / max_boxes, boxes + static_cast<size_t>(id) * 8, big_planes,
+                      big_locks, tall_scratch, dyn_smem, smem_plane_words,
                       polys ? polys + static_cast<size_t>(id) * 2 * kPolyPoints : nullptr, points ? points + id : nullptr);
     __syncthreads();       // thread 0 builds the hull in the planes' shared memory after the others have left
   }
@@ -942,6 +966,7 @@ constexpr int kQuadSmallPlaneWords = 2 * 1024;     // pass 1: 2 planes x 8 KB, R
 
 struct BoxWorkspace {
   uint8_t* mask; int* label; Stats st; Component* comps; uint32_t* big_planes; int* big_locks;
+  uint32_t* tall_scratch;           // per image tall_words(hs), on maps of more than kRowTable rows only
   int* queue; int* queue_len;       // components that pass 1 of the quads leaves to pass 2
   size_t bytes;
 };
@@ -965,6 +990,8 @@ BoxWorkspace carve(void* ws, int n, int hs, int ws_w, int max_boxes) {
   w.big_locks = reinterpret_cast<int*>(take(static_cast<size_t>(n) * 4));
   w.queue = reinterpret_cast<int*>(take(static_cast<size_t>(n) * max_boxes * 4));
   w.queue_len = reinterpret_cast<int*>(take(4));
+  w.tall_scratch = nullptr;
+  if (hs > kRowTable) w.tall_scratch = reinterpret_cast<uint32_t*>(take(static_cast<size_t>(n) * tall_words(hs) * 4));
   w.bytes = off;
   return w;
 }
@@ -994,8 +1021,8 @@ int get_boxes(b2o_ctx* ctx, const float* scores, int n, int hs, int ws, float de
     ctx->set_error("b2o_get_boxes: bad argument");
     return B2O_ERR_ARG;
   }
-  if (hs > kMaxHullRows / 2 || static_cast<long long>(hs) * ws >= (1LL << 30)) {
-    ctx->set_error("b2o_get_boxes: score map larger than 1024 rows is not supported");
+  if (hs > (1 << 24) || static_cast<long long>(hs) * ws >= (1LL << 30)) {
+    ctx->set_error("b2o_get_boxes: score map of more than 2^24 rows or 2^30 pixels per image is not supported");
     return B2O_ERR_ARG;
   }
   BoxWorkspace w = carve(ws_dev, n, hs, ws, max_boxes);
@@ -1033,13 +1060,13 @@ int get_boxes(b2o_ctx* ctx, const float* scores, int n, int hs, int ws, float de
   auto quads = polys ? quads_kernel<true> : quads_kernel<false>;
   auto queue = polys ? quads_queue_kernel<true> : quads_queue_kernel<false>;
   quads<<<dim3(max_boxes, n), 128, dyn_small, st>>>(w.mask, w.label, hs, ws, w.comps, counts, max_boxes, boxes,
-                                                    w.big_planes, w.big_locks, kQuadSmallPlaneWords, w.queue,
-                                                    w.queue_len, polys, points);
+                                                    w.big_planes, w.big_locks, w.tall_scratch, kQuadSmallPlaneWords,
+                                                    w.queue, w.queue_len, polys, points);
   B2O_LAUNCH_CHECK(ctx);
   const long long slots = static_cast<long long>(n) * max_boxes;
   queue<<<static_cast<unsigned>(std::min<long long>(slots, 2 * ctx->sm_count)), 256, dyn, st>>>(
-      w.mask, w.label, hs, ws, w.comps, max_boxes, boxes, w.big_planes, w.big_locks, kQuadSmemPlaneWords, w.queue,
-      w.queue_len, polys, points);
+      w.mask, w.label, hs, ws, w.comps, max_boxes, boxes, w.big_planes, w.big_locks, w.tall_scratch, kQuadSmemPlaneWords,
+      w.queue, w.queue_len, polys, points);
   B2O_LAUNCH_CHECK(ctx);
   return B2O_OK;
 }

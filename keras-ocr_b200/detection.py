@@ -20,6 +20,40 @@ PRETRAINED_WEIGHTS = {   # same files as reference detection.py:647-658
 }
 
 
+# Tiled detection (DESIGN.md section 1, "Tiles").  TILE_MARGIN: detector pixels of context kept on each inner side of a
+# tile's core, the smallest margin at which the tiled forward's boxes and texts matched the whole page's (DESIGN.md
+# section 5).  DEFAULT_TILE_SIZE: tile_size=None tiles a batch whose padded height is over it -- the batches the
+# whole-page forward cannot take, as getBoxes once refused their score maps.  TILE_CHUNK_PIXELS: tiles per CRAFT launch
+# are as many as fit this pixel count, which bounds the forward's workspace whatever the page size.
+TILE_MARGIN = 64
+DEFAULT_TILE_SIZE = 2048
+MAX_TILE_SIZE = 2048
+TILE_CHUNK_PIXELS = 8 * 2048 * 2048
+
+
+def check_tiles(tile_size=None):
+    """Validate ``tile_size`` (DESIGN.md section 1, "Tiles") and return it as an int, or None for the default rule: a
+    multiple of 32 with 4 * TILE_MARGIN <= tile_size <= 2048.  Bools, non-integers and other values raise
+    ``ValueError``."""
+    if tile_size is None:
+        return None
+    if isinstance(tile_size, bool) or not isinstance(tile_size, numbers.Integral):
+        raise ValueError(f"tile_size must be an integer or None, got {tile_size!r}")
+    t = int(tile_size)
+    if t % 32 or not 4 * TILE_MARGIN <= t <= MAX_TILE_SIZE:
+        raise ValueError(f"tile_size must be a multiple of 32 in [{4 * TILE_MARGIN}, {MAX_TILE_SIZE}], got {t}")
+    return t
+
+
+def tile_size_for(hp, wp, tile_size=None):
+    """The tile size a padded (hp, wp) batch is detected with, or None for the whole-page forward.  ``tile_size`` as
+    ``check_tiles`` returns it: None tiles at DEFAULT_TILE_SIZE only a batch taller than that; a size tiles a batch
+    larger than it in either dimension."""
+    if tile_size is None:
+        return DEFAULT_TILE_SIZE if hp > DEFAULT_TILE_SIZE else None
+    return tile_size if hp > tile_size or wp > tile_size else None
+
+
 LINE_DEFAULTS = {"angle_tolerance": 15.0, "height_ratio": 0.5, "offset_ratio": 0.5, "gap_ratio": 1.5}
 
 
@@ -131,18 +165,48 @@ class Detector:
         self._block_ws = None
 
     # ------------------------------------------------------------------ device-resident API
-    def predict_device(self, images_t):
-        """CRAFT forward.  images_t: (N,H,W,3) uint8 CUDA tensor -> (N,H/2,W/2,2) float32 scores."""
-        n, h, w, _ = images_t.shape
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        scores = torch.empty((n, h // 2, w // 2, 2), dtype=torch.float32, device=self.device)
+    def _workspace(self, n, h, w):
         nbytes = self.ctx.craft_workspace_bytes(n, h, w)
         assert nbytes > 0, "image too small for CRAFT (needs H, W >= 32)"
         if self._ws is None or self._ws.numel() < nbytes:
             self._ws = None
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        ws = self._ws
-        self.ctx.craft_forward(images_t.data_ptr(), n, h, w, scores.data_ptr(), ws.data_ptr(), nbytes, stream)
+        return self._ws, nbytes
+
+    def predict_device(self, images_t, tile_size=None, margin=TILE_MARGIN):
+        """CRAFT forward.  images_t: (N,H,W,3) uint8 CUDA tensor -> (N,H/2,W/2,2) float32 scores.
+
+        ``tile_size`` None: the whole page in one forward.  Otherwise (``check_tiles``) a batch larger than one tile
+        runs over overlapping tiles (DESIGN.md section 1, "Tiles"): cut (``b2o_cut_tiles``), CRAFT on chunks of at
+        most TILE_CHUNK_PIXELS pixels of tiles, each tile's core stitched into the page map (``b2o_stitch_tiles``),
+        all queued on the current stream without a host wait; a batch that fits one tile takes the whole-page
+        forward.  ``margin`` (a multiple of 16) is the context around each core; other values than TILE_MARGIN are
+        for measuring the seams."""
+        n, h, w, _ = images_t.shape
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        scores = torch.empty((n, h // 2, w // 2, 2), dtype=torch.float32, device=self.device)
+        plan = None
+        if tile_size is not None:
+            tile_size = check_tiles(tile_size)
+            plan = _lib.tile_plan(h, w, tile_size, margin)
+            if plan is None:
+                raise ValueError(f"no tile grid for a ({h}, {w}) batch with tile_size={tile_size}, margin={margin}")
+        if plan is None or plan.n_h * plan.n_w == 1:
+            ws, nbytes = self._workspace(n, h, w)
+            self.ctx.craft_forward(images_t.data_ptr(), n, h, w, scores.data_ptr(), ws.data_ptr(), nbytes, stream)
+            return scores
+        images_t = images_t.contiguous()
+        total = n * plan.n_h * plan.n_w
+        per = min(total, max(1, TILE_CHUNK_PIXELS // (plan.t_h * plan.t_w)))
+        tiles = torch.empty((per, plan.t_h, plan.t_w, 3), dtype=torch.uint8, device=self.device)
+        tile_scores = torch.empty((per, plan.t_h // 2, plan.t_w // 2, 2), dtype=torch.float32, device=self.device)
+        ws, nbytes = self._workspace(per, plan.t_h, plan.t_w)
+        for first in range(0, total, per):
+            k = min(per, total - first)
+            self.ctx.cut_tiles(images_t.data_ptr(), n, plan, first, k, tiles.data_ptr(), stream)
+            self.ctx.craft_forward(tiles.data_ptr(), k, plan.t_h, plan.t_w, tile_scores.data_ptr(), ws.data_ptr(), nbytes,
+                                   stream)
+            self.ctx.stitch_tiles(tile_scores.data_ptr(), n, plan, first, k, scores.data_ptr(), stream)
         return scores
 
     def boxes_enqueue(self, scores, detection_threshold=0.7, text_threshold=0.4, link_threshold=0.4,
@@ -335,13 +399,15 @@ class Detector:
         bc, lo, bs, bb = (t.cpu().numpy() for t in out)
         return [blocks_from_csr(bc[i], lo[i], bs[i], bb[i]) for i in range(n)]
 
-    def detect_device(self, images_t, **thresholds):
-        return self.boxes_device(self.predict_device(images_t), **thresholds)
+    def detect_device(self, images_t, tile_size=None, **thresholds):
+        tile_size = check_tiles(tile_size)
+        return self.boxes_device(self.predict_device(images_t, tile_size_for(images_t.shape[1], images_t.shape[2],
+                                                                             tile_size)), **thresholds)
 
     # ------------------------------------------------------------------ reference API
     def detect(self, images: typing.List[typing.Union[np.ndarray, str]], detection_threshold=0.7,
                text_threshold=0.4, link_threshold=0.4, size_threshold=10, return_scores=False, return_polygons=False,
-               **kwargs):
+               tile_size=None, **kwargs):
         """Same contract as reference detection.py:745-785: a list with one array of boxes
         ``(n_i, 4, 2)`` float32 per image (``np.array([])`` when there is none).  ``kwargs`` are the
         keras ``predict`` arguments of the reference (batch_size, verbose, ...) and are ignored.
@@ -354,9 +420,15 @@ class Detector:
         polygons)`` or ``(boxes, scores, polygons)`` -- a list of (p,2) float32 arrays in detector-input pixels: the box
         itself (p = 4) for a straight word, otherwise 2 (s + 1) points along a curved word's centre line, the top edge
         left to right then the bottom edge right to left, clockwise from the top-left (``b2o_get_boxes_poly``).  Boxes
-        and scores are those of the default call."""
+        and scores are those of the default call.
+
+        ``tile_size`` (``check_tiles``): the batch runs CRAFT over overlapping tiles of that size when it is larger than
+        one in either dimension; None (the default) tiles at 2048 a batch taller than 2048 only (``tile_size_for``).
+        Everything after the score map is unchanged."""
+        tile_size = check_tiles(tile_size)
         images_t = _as_device_images(images, self.device)
-        state = self.boxes_enqueue(self.predict_device(images_t), detection_threshold, text_threshold, link_threshold,
+        scores = self.predict_device(images_t, tile_size_for(images_t.shape[1], images_t.shape[2], tile_size))
+        state = self.boxes_enqueue(scores, detection_threshold, text_threshold, link_threshold,
                                    size_threshold, with_scores=return_scores, with_polygons=return_polygons)
         boxes, counts = self.boxes_finish(state)
         boxes_host = boxes.cpu().numpy()

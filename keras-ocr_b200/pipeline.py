@@ -125,9 +125,11 @@ class Pipeline:
         return (batch, scales, gray) if want_gray else (batch, scales)
 
     # ---------------------------------------------------------------- the three stages of one sub-batch
-    def _stage_detect(self, images, pad_to, thresholds, with_scores=False, with_polygons=False, max_windows=1):
+    def _stage_detect(self, images, pad_to, thresholds, with_scores=False, with_polygons=False, max_windows=1,
+                      tile_size=None):
         batch, scales, gray = self.prepare_device(images, pad_to, want_gray=True)
-        scores = self.detector.predict_device(batch)
+        scores = self.detector.predict_device(batch, tile_size=detection.tile_size_for(batch.shape[1], batch.shape[2],
+                                                                                      tile_size))
         extra = {"with_polygons": True} if with_polygons else {}
         if max_windows > 1:
             extra["max_windows"] = max_windows
@@ -324,6 +326,11 @@ class Pipeline:
         synchronisation.  Boxes, and so lines and blocks, are unchanged.  It combines with ``return_scores``,
         ``return_lines``, ``return_blocks`` and ``inflight``; with ``beam_width``, ``lexicon``, ``rotations``,
         ``return_char_boxes`` or ``return_polygons`` it raises ``ValueError``.
+        ``detection_kwargs`` may hold ``tile_size`` (``detection.check_tiles``): a batch whose padded pages are larger
+        than that in either dimension runs CRAFT over overlapping tiles stitched into one score map on the device;
+        the default, None, tiles at 2048 a batch padded taller than 2048 only, so ``Pipeline(max_size=8192)`` reads
+        large pages as they are.  Everything after the score map is unchanged.  Injected detectors get
+        ``detection_kwargs`` as they are.
         """
         if return_polygons and (return_char_boxes or (recognition_kwargs or {}).get("rotations") is not None):
             raise ValueError("return_polygons does not combine with rotations or return_char_boxes")
@@ -331,6 +338,8 @@ class Pipeline:
         blocks = detection.check_blocks(**(block_kwargs or {})) if return_blocks or block_kwargs is not None else None
         if return_blocks and lines is None:
             lines = detection.check_lines()
+        # validated before anything is decoded or launched; injected detectors get detection_kwargs as they are
+        tile_size = detection.check_tiles((detection_kwargs or {}).get("tile_size")) if self._native() else None
         if not isinstance(images, (np.ndarray, torch.Tensor)):
             if self.gpu_decode and self._native():
                 images = [tools.read_device(image, self.detector.ctx, self.detector.device) for image in images]
@@ -389,7 +398,7 @@ class Pipeline:
             if step < k:
                 states.append(self._stage_detect(images[bounds[step]:bounds[step + 1]], pad_to, thresholds,
                                                  with_scores=return_scores, with_polygons=return_polygons,
-                                                 max_windows=max_windows))
+                                                 max_windows=max_windows, tile_size=tile_size))
             if 1 <= step <= k:
                 self._stage_recognize(states[step - 1], beam, char_boxes=return_char_boxes,
                                       lines=lines if return_lines or return_blocks else None,
@@ -435,6 +444,7 @@ class Pipeline:
                                         recognition.DEFAULT_ALPHABET if plain else self.recognizer.alphabet,
                                         language_model, pattern)
         turns = recognition.check_rotations(rotations, rotation_vote)
+        tile_size = detection.check_tiles((detection_kwargs or {}).get("tile_size"))
         assert self._native(), "recognize_records needs this package's Detector and Recognizer"
         assert len(self.recognizer.alphabet) + 1 <= 127, "record labels travel as int8: alphabets up to 126 characters"
         if not isinstance(images, (np.ndarray, torch.Tensor)):
@@ -454,7 +464,7 @@ class Pipeline:
         if n:
             plans = self._plans(images)
             state["st"] = self._stage_detect(images, (max(p[1] for p in plans), max(p[2] for p in plans)), thresholds,
-                                             with_scores=bool(scores))
+                                             with_scores=bool(scores), tile_size=tile_size)
         return state
 
     def records_counts(self, state):
