@@ -546,6 +546,36 @@ int b2o_crnn_forward_logits(b2o_ctx* ctx, const void* crnn_in_dev, int b, int32_
 int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths, int32_t* spans_dev, float* logp_dev,
                    float* theta_dev, const void* ws_dev, size_t ws_bytes, void* stream);
 
+/* Character scores: how sure the model is of each character of a reading, and what it would read there instead
+ * (DESIGN.md section 1, "Character scores").  On lp[t,c] = log(softmax(l_t)_c + 1e-7) over the 48 kept steps (blank =
+ * k-1), F(z) is the CTC forward log-probability of a label sequence z (b2o_ctc_lexicon_decode's entry score; -inf when
+ * z cannot be aligned).  For a reading y_0..y_{n-1} and a position j the k one-character edits at j are the
+ * substitutions y[j->c], c = 0..k-2 (c = y_j is y itself), and the deletion y[j->nothing], labelled k-1.  The posterior
+ * of edit e is pi_j(e) = exp(F(y[j->e]) - L_j), L_j = logsumexp_e F(y[j->e]); the character's confidence is
+ * pi_j(y_j); its alternatives are the A edits of largest posterior, best first, equal values by smaller label (the
+ * reading's own character appears where it ranks).  Insertions are not scored.  The scores are acoustic: they do not
+ * depend on the decoder that produced y.
+ * Inputs: logits_dev (b, 48, k) float32 and labels_dev (b, top_paths, 48) int32, each reading's labels followed by -1
+ * (what the decoders write).  Outputs: conf_dev (b, top_paths, 48) float32; alt_labels_dev (b, top_paths, 48, A) int32
+ * and alt_post_dev (b, top_paths, 48, A) float32, A = alternatives (both may be NULL when A = 0); logp_dev (b, top_paths)
+ * float32 = F(y) (NULL: not written).  Where L_j = -inf (and at every position of a reading with a label outside
+ * [0, k-2]) the confidence and the posteriors are 0 and the labels -1; with A > k the slots past the k edits are -1
+ * with posterior 0; positions past the reading's end are NaN, -1 and NaN.  A reading with a label outside [0, k-2] has
+ * logp -inf.  The posteriors at a position sum to 1 up to fp32 rounding.  A crop's result is a function of its logits
+ * and labels alone: bit-identical alone, in any batch and on every run.  No workspace.
+ * 2 <= k <= B2O_MAX_CLASSES, 1 <= top_paths <= B2O_MAX_ALIGN_PATHS, 0 <= alternatives <= B2O_MAX_CHAR_ALTERNATIVES,
+ * otherwise B2O_ERR_ARG.
+ * b2o_crnn_char_scores: the same on the logits of the preceding forward in ws_dev, under b2o_crnn_align's rule (the
+ * context's last successful CRNN forward, same ws_dev and b, and it kept its logits: otherwise B2O_ERR_STATE and
+ * nothing is written).                                                                                             */
+#define B2O_MAX_CHAR_ALTERNATIVES 8
+int b2o_ctc_char_scores(b2o_ctx* ctx, const float* logits_dev, int b, int k, const int32_t* labels_dev, int top_paths,
+                        int alternatives, float* conf_dev, int32_t* alt_labels_dev, float* alt_post_dev,
+                        float* logp_dev, void* stream);
+int b2o_crnn_char_scores(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths, int alternatives,
+                         float* conf_dev, int32_t* alt_labels_dev, float* alt_post_dev, float* logp_dev,
+                         const void* ws_dev, size_t ws_bytes, void* stream);
+
 /* Training the output layer for a custom alphabet: Recognizer.compile() + training_model with ctc_batch_cost
  * (recognition.py:321-349, 539-545; docs/examples/fine_tuning_recognizer.rst) restricted to fc_12 (Dense 256 -> k plus
  * bias), the rest of the CRNN frozen.

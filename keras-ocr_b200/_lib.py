@@ -25,6 +25,7 @@ MAX_PATTERN_STATES = 4096     # B2O_MAX_PATTERN_STATES
 MAX_PATTERN_CLASSES = 127     # B2O_MAX_PATTERN_CLASSES
 ROTATION_VOTE_WORD, ROTATION_VOTE_PAGE = 0, 1   # B2O_ROTATION_VOTE_WORD / _PAGE
 MAX_ALIGN_PATHS = 128         # B2O_MAX_ALIGN_PATHS
+MAX_CHAR_ALTERNATIVES = 8     # B2O_MAX_CHAR_ALTERNATIVES
 CRAFT_LAST_STEP = 30          # B2O_CRAFT_LAST_STEP
 MAX_POLY_SEGMENTS = 8         # B2O_MAX_POLY_SEGMENTS
 POLY_POINTS = 2 * (MAX_POLY_SEGMENTS + 1)   # points per entry of a dense polygon table
@@ -163,6 +164,8 @@ SIGNATURES = {
     "b2o_char_cells": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "b2o_crnn_forward_logits": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_crnn_align": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_ctc_char_scores": (_i, [_vp, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "b2o_crnn_char_scores": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2o_crnn_features": (_i, [_vp, _vp, _i, _vp, _vp, _sz, _vp]),
     "b2o_ctc_train_workspace_bytes": (_sz, [_i, _i]),
     "b2o_ctc_loss_grad": (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _c.c_uint64, _c.c_uint64, _vp, _vp,
@@ -526,6 +529,15 @@ class Context:
     def crnn_align(self, b, labels, top_paths, spans, logp, theta, ws, ws_bytes, stream):
         self._check(self.lib.b2o_crnn_align(self.handle, b, labels, top_paths, spans, logp, theta, ws, ws_bytes, stream),
                     "b2o_crnn_align")
+
+    def ctc_char_scores(self, logits, b, k, labels, top_paths, alternatives, conf, alt_labels, alt_post, logp, stream):
+        self._check(self.lib.b2o_ctc_char_scores(self.handle, logits, b, k, labels, top_paths, alternatives, conf,
+                                                 alt_labels, alt_post, logp, stream), "b2o_ctc_char_scores")
+
+    def crnn_char_scores(self, b, labels, top_paths, alternatives, conf, alt_labels, alt_post, logp, ws, ws_bytes,
+                         stream):
+        self._check(self.lib.b2o_crnn_char_scores(self.handle, b, labels, top_paths, alternatives, conf, alt_labels,
+                                                  alt_post, logp, ws, ws_bytes, stream), "b2o_crnn_char_scores")
 
     def crnn_features(self, crnn_in, b, features, ws, ws_bytes, stream):
         self._check(self.lib.b2o_crnn_features(self.handle, crnn_in, b, features, ws, ws_bytes, stream),

@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb2ocr.so")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "boxes.cu", "image.cu", "crnn_tail.cu", "ctc_beam.cu", "ctc_lexicon.cu",
            "jpeg.cu", "rotation.cu", "ctc_align.cu", "ctc_train.cu", "rnn_train.cu", "lines.cu",
-           "blocks.cu", "windows.cu", "tiles.cu"]
+           "blocks.cu", "windows.cu", "tiles.cu", "ctc_char_scores.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]

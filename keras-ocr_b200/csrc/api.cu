@@ -27,6 +27,9 @@ int ctc_lexicon_run(b2o_ctx* ctx, const float* logits, int B, int K, const int* 
                     int n_words, int top_paths, int* labels_out, float* logp, void* ws, cudaStream_t st);
 int ctc_align_run(b2o_ctx* ctx, const float* logits, int B, int K, const int32_t* labels, int P, int32_t* spans,
                   float* logp, cudaStream_t st);
+int ctc_char_scores_run(b2o_ctx* ctx, const float* logits, int B, int K, const int32_t* labels, int P, int A, float* conf,
+                        int32_t* alt_labels, float* alt_post, float* logp, cudaStream_t st);
+bool ctc_char_scores_args(int k, int top_paths, int alternatives);
 size_t ctc_train_workspace_bytes(int B, int K);
 int ctc_loss_grad_run(b2o_ctx* ctx, const __half* features, long long feat_stride, bool feat_by_batch, int n_rows,
                       const int* index, int B, int K, const float* w, const float* bias, const int* offsets,
@@ -1170,6 +1173,31 @@ extern "C" int b2o_crnn_align(b2o_ctx* ctx, int b, const int32_t* labels_dev, in
                                         cudaMemcpyDeviceToDevice, st));
   return ctc_align_run(ctx, reinterpret_cast<const float*>(base + p.off[rb::logits]), b, ctx->n_classes, labels_dev, top_paths,
                        spans_dev, logp_dev, st);
+}
+
+extern "C" int b2o_crnn_char_scores(b2o_ctx* ctx, int b, const int32_t* labels_dev, int top_paths, int alternatives,
+                                    float* conf_dev, int32_t* alt_labels_dev, float* alt_post_dev, float* logp_dev,
+                                    const void* ws, size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!ctx->crnn_loaded) { ctx->set_error("b2o_crnn_char_scores: CRNN weights not loaded"); return B2O_ERR_STATE; }
+  if (!ctc_char_scores_args(ctx->n_classes, top_paths, alternatives) || b < 0 ||
+      (b > 0 && (!labels_dev || !conf_dev || !ws || (alternatives > 0 && (!alt_labels_dev || !alt_post_dev))))) {
+    ctx->set_error("b2o_crnn_char_scores: bad argument");
+    return B2O_ERR_ARG;
+  }
+  if (b == 0) return B2O_OK;
+  const CrnnPlan p = plan_crnn(b);
+  if (ws_bytes < p.bytes) { ctx->set_error("b2o_crnn_char_scores: workspace too small"); return B2O_ERR_WORKSPACE; }
+  if (!crnn_wrote(ctx, rb::logits, ws, b)) {
+    ctx->set_error("b2o_crnn_char_scores: the last successful CRNN forward of this context did not keep its logits in "
+                   "this ws with this b");
+    return B2O_ERR_STATE;
+  }
+  DeviceGuard guard(ctx->device);
+  const uint8_t* base = reinterpret_cast<const uint8_t*>(ws);
+  return ctc_char_scores_run(ctx, reinterpret_cast<const float*>(base + p.off[rb::logits]), b, ctx->n_classes, labels_dev,
+                             top_paths, alternatives, conf_dev, alternatives > 0 ? alt_labels_dev : nullptr,
+                             alternatives > 0 ? alt_post_dev : nullptr, logp_dev, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int b2o_set_debug_taps(b2o_ctx* ctx, int on) {

@@ -141,7 +141,7 @@ class Pipeline:
         st[key] = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
         st[key].copy_(t, non_blocking=True)
 
-    def _stage_recognize(self, st, beam, char_boxes=False, lines=None, blocks=None):
+    def _stage_recognize(self, st, beam, char_boxes=False, lines=None, blocks=None, char_scores=None):
         det, rec = self.detector, self.recognizer
         bst = st.pop("boxes_state")
         boxes, counts = det.boxes_finish(bst)
@@ -150,6 +150,8 @@ class Pipeline:
         extra = {"char_boxes": True} if char_boxes else {}
         if polys is not None:
             extra = {"polys": bst["flat_polys"], "points": bst["flat_points"]}
+        if char_scores is not None:
+            extra = dict(extra, char_scores=True, char_alternatives=char_scores)
         if bst.get("windows_pin") is not None:           # every word's window count, read back with the box counts
             windows = bst["windows_pin"].numpy()
             m = boxes.shape[1]
@@ -158,6 +160,11 @@ class Pipeline:
         labels = rec.recognize_from_boxes_device(st["batch"], boxes, counts, gray=st["gray"], flat=bst["flat"],
                                                  image_index=bst["image_index"], with_scores=box_scores is not None,
                                                  **beam, **extra)
+        scores = ()
+        if char_scores is not None:                      # (..., conf[, alternative labels, posteriors])
+            k = 1 + 2 * bool(char_scores)
+            scores, labels = labels[-k:], labels[:-k]
+            labels = labels if len(labels) > 1 else labels[0]
         if char_boxes:                                   # (..., spans, cells): keep the cells
             cells, labels = labels[-1], labels[:-2]
             labels = labels if len(labels) > 1 else labels[0]
@@ -189,7 +196,11 @@ class Pipeline:
             st["char_boxes"] = True
             if cells is not None:
                 self._to_host(st, "cells_host", cells)
-        st["keep"] = (boxes, labels, box_scores, logp, cells, polys) + tuple(line_tables)   # alive until the copies ran
+        for i, t in enumerate(scores):
+            if t is not None:
+                self._to_host(st, f"char_scores{i}_host", t)
+        st["keep"] = ((boxes, labels, box_scores, logp, cells, polys) + tuple(line_tables)    # alive until the copies ran
+                      + tuple(scores))
         st["done"] = torch.cuda.Event()
         st["done"].record(torch.cuda.current_stream(det.device))
 
@@ -219,6 +230,11 @@ class Pipeline:
             cells_host = st["cells_host"].numpy()
             d2h += cells_host.nbytes
             cells = recognition.char_boxes_host(cells_host, texts)
+        char_scores = None
+        if "char_scores0_host" in st:
+            host = [st[k].numpy() for k in ("char_scores0_host", "char_scores1_host", "char_scores2_host") if k in st]
+            d2h += sum(a.nbytes for a in host)
+            char_scores = recognition.char_scores_host(host[0], texts, self.recognizer.alphabet, *host[1:])
         lines = None
         if "line_counts_host" in st:
             lines = [st[k].numpy() for k in ("line_counts_host", "word_order_host", "line_start_host", "line_boxes_host")]
@@ -247,6 +263,8 @@ class Pipeline:
                 words = [w + (tools.adjust_boxes(boxes=polys[i, k, :points[i, k]].copy(), boxes_format="boxes",
                                                  scale=1 / scale),)
                          for k, w in enumerate(words)]
+            if char_scores is not None:                  # the character scores end every word's tuple
+                words = [w + (q,) for w, q in zip(words, char_scores[start:start + c])]
             if lines is not None:
                 words = self._lines(words, detection.lines_from_csr(*(a[i] for a in lines)), scale)
             if blocks is not None:
@@ -280,7 +298,7 @@ class Pipeline:
 
     def recognize(self, images, detection_kwargs=None, recognition_kwargs=None, return_scores=False,
                   return_char_boxes=False, return_polygons=False, return_lines=False, line_kwargs=None,
-                  return_blocks=False, block_kwargs=None):
+                  return_blocks=False, block_kwargs=None, return_char_scores=False, char_alternatives=0):
         """Run the pipeline on one or multiple images (reference pipeline.py:28-75).
 
         Returns a list (one entry per image) of lists of (text, box) tuples, boxes (4,2) float32 in
@@ -331,7 +349,16 @@ class Pipeline:
         the default, None, tiles at 2048 a batch padded taller than 2048 only, so ``Pipeline(max_size=8192)`` reads
         large pages as they are.  Everything after the score map is unchanged.  Injected detectors get
         ``detection_kwargs`` as they are.
+        ``return_char_scores=True``: every word's tuple ends with its character scores, after the cells or the polygon
+        when those are asked for: an (n,) float32 array, the confidence of each of the n characters of the text, or
+        with ``char_alternatives = A > 0`` (0 .. 8) that array and n lists of A (character, posterior) pairs, best
+        first, ``''`` for the deletion (``recognition.char_scores_host``); a list of P of these with ``top_paths = P >
+        1``.  The scores are acoustic -- the same whichever decoder produced the reading -- and change nothing else.
+        They combine with every decoder, ``top_paths``, ``rotations``, ``return_scores``, ``return_char_boxes``,
+        ``return_polygons``, ``return_lines`` / ``return_blocks`` and ``inflight``; with ``max_windows > 1`` they raise
+        ``ValueError``.
         """
+        char_scores = recognition.check_char_scores(return_char_scores, char_alternatives)
         if return_polygons and (return_char_boxes or (recognition_kwargs or {}).get("rotations") is not None):
             raise ValueError("return_polygons does not combine with rotations or return_char_boxes")
         lines = detection.check_lines(**(line_kwargs or {})) if return_lines or line_kwargs is not None else None
@@ -364,7 +391,8 @@ class Pipeline:
             if turns is not None:
                 beam["rotations"], beam["rotation_vote"] = turns, vote
             max_windows = recognition.check_windows(recognition_kwargs.get("max_windows", 1), beam.get("beam_width"),
-                                                    beam.get("lexicon"), turns, return_char_boxes, return_polygons)
+                                                    beam.get("lexicon"), turns, return_char_boxes, return_polygons,
+                                                    char_scores is not None)
         if not self._native():
             if return_scores:
                 raise NotImplementedError("return_scores=True needs this package's Detector and Recognizer; injected "
@@ -372,6 +400,9 @@ class Pipeline:
             if return_char_boxes:
                 raise NotImplementedError("return_char_boxes=True needs this package's Detector and Recognizer; "
                                           "injected detectors / recognizers do not report character positions")
+            if char_scores is not None:
+                raise NotImplementedError("return_char_scores=True needs this package's Detector and Recognizer; "
+                                          "injected recognizers do not report character scores")
             if return_polygons:
                 raise NotImplementedError("return_polygons=True needs this package's Detector and Recognizer; "
                                           "injected detectors / recognizers do not report polygons")
@@ -402,7 +433,7 @@ class Pipeline:
             if 1 <= step <= k:
                 self._stage_recognize(states[step - 1], beam, char_boxes=return_char_boxes,
                                       lines=lines if return_lines or return_blocks else None,
-                                      blocks=blocks if return_blocks else None)
+                                      blocks=blocks if return_blocks else None, char_scores=char_scores)
             if step >= 2:
                 out.extend(self._stage_finish(states[step - 2]))
                 states[step - 2] = None

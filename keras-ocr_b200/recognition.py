@@ -607,25 +607,42 @@ def check_rotations(rotations=None, rotation_vote="word"):
     return turns
 
 
-def check_windows(max_windows=1, beam_width=None, lexicon=None, rotations=None, char_boxes=False, polygons=False):
+def check_windows(max_windows=1, beam_width=None, lexicon=None, rotations=None, char_boxes=False, polygons=False,
+                  char_scores=False):
     """Validates a choice of wide-word windows before anything is launched (``ValueError`` otherwise) and returns it as
     an int.  ``max_windows=1`` (the default) reads every box as one 200 x 31 crop, as warpBox cuts it.  An int 2 <= M <=
     16 reads every box wider than that crop at full height in up to M overlapping 200 x 31 windows and stitches their
     CTC steps into one reading (DESIGN.md section 1, "Wide words"); when a box of the call is wide the labels rows are
     48 M wide, -1 padded, and every other box reads exactly as with M = 1.  The windows are decoded greedily over 48
-    steps each: with M > 1, ``beam_width``, ``lexicon``, ``rotations``, character boxes (``char_boxes``) and polygons
-    (``polygons``) raise."""
+    steps each: with M > 1, ``beam_width``, ``lexicon``, ``rotations``, character boxes (``char_boxes``), polygons
+    (``polygons``) and character scores (``char_scores``) raise: a stitched reading spans more than 48 steps."""
     if (not isinstance(max_windows, (int, np.integer)) or isinstance(max_windows, (bool, np.bool_))
             or not 1 <= max_windows <= _lib.MAX_WINDOWS):
         raise ValueError(f"max_windows must be an int in [1, {_lib.MAX_WINDOWS}], got {max_windows!r}")
     if max_windows > 1:
         excluded = [name for name, on in (("beam_width", beam_width is not None), ("lexicon", lexicon is not None),
                                           ("rotations", rotations is not None), ("return_char_boxes", char_boxes),
-                                          ("return_polygons", polygons)) if on]
+                                          ("return_polygons", polygons), ("return_char_scores", char_scores)) if on]
         if excluded:
             raise ValueError(f"max_windows > 1 reads wide words by greedy decoding only; it does not combine with "
                              f"{', '.join(excluded)}")
     return int(max_windows)
+
+
+def check_char_scores(return_char_scores=False, char_alternatives=0):
+    """Validates a request for character scores before anything is launched (``ValueError`` otherwise).  Returns None
+    when ``return_char_scores`` is off, else A = ``char_alternatives``, an int in [0, 8]: every character of a reading
+    gets its confidence and, with A > 0, the A most probable one-character edits at its position (``b2o_ctc_char_scores``,
+    DESIGN.md section 1, "Character scores").  ``char_alternatives > 0`` without ``return_char_scores`` raises."""
+    a = char_alternatives
+    if (not isinstance(a, (int, np.integer)) or isinstance(a, (bool, np.bool_))
+            or not 0 <= a <= _lib.MAX_CHAR_ALTERNATIVES):
+        raise ValueError(f"char_alternatives must be an int in [0, {_lib.MAX_CHAR_ALTERNATIVES}], got {a!r}")
+    if not return_char_scores:
+        if a:
+            raise ValueError("char_alternatives needs return_char_scores=True")
+        return None
+    return int(a)
 
 
 def check_polygons(entries):
@@ -683,6 +700,30 @@ def char_boxes_host(cells, texts):
     if cells.ndim == 4:
         return [cells[i, :len(t)] for i, t in enumerate(texts)]
     return [[cells[i, j, :len(t)] for j, t in enumerate(row)] for i, row in enumerate(texts)]
+
+
+def char_scores_host(conf, texts, alphabet=DEFAULT_ALPHABET, alt_labels=None, alt_post=None):
+    """Host character scores (``b2o_ctc_char_scores``) -> one entry per word, n = len(text): conf (B,48) or (B,P,48)
+    float32 gives an (n,) float32 array of the characters' confidences; with alt_labels / alt_post (B[,P],48,A) the
+    entry is (that array, n lists of A (character, posterior) pairs, best first), the character ``''`` for the deletion
+    and None for a slot without an edit (posterior 0).  With ``top_paths = P > 1`` (texts are lists of P strings) a list
+    of P entries per word."""
+    conf = np.asarray(conf)
+    chars = list(alphabet) + [""]                                  # label K-1: the deletion
+
+    def one(c, text, lab, post):
+        n = len(text)
+        if lab is None:
+            return c[:n]
+        alts = [[(chars[e] if e >= 0 else None, q) for e, q in zip(le, pe)]
+                for le, pe in zip(lab[:n].tolist(), post[:n].tolist())]
+        return c[:n], alts
+
+    pick = (lambda a, *i: None if a is None else a[i])             # noqa: E731
+    if conf.ndim == 2:
+        return [one(conf[i], t, pick(alt_labels, i), pick(alt_post, i)) for i, t in enumerate(texts)]
+    return [[one(conf[i, j], t, pick(alt_labels, i, j), pick(alt_post, i, j)) for j, t in enumerate(row)]
+            for i, row in enumerate(texts)]
 
 
 class Recognizer:
@@ -893,7 +934,7 @@ class Recognizer:
                              language_model), None
 
     def predict_device(self, crnn_in, with_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                       language_model=None, pattern=None):
+                       language_model=None, pattern=None, char_scores=None):
         """CRNN + greedy CTC.  crnn_in: (B,200,31) fp16 -> labels (B,48) int32 (-1 padded).  ``with_scores``: returns
         (labels, logp) with logp (B,) float32 the greedy path's log-probability (``b2o_crnn_forward_scored``).
         ``beam_width``: CTC prefix beam search instead (``b2o_crnn_forward_beam``, see ``check_beam``), logp = the beam
@@ -903,23 +944,40 @@ class Recognizer:
         ``language_model`` (a ``CharLM``, with ``beam_width``): the beam search ranked by that model
         (``b2o_crnn_forward_beam_lm``); logp stays the acoustic beam score of each reading.  ``pattern`` (a
         ``Pattern`` or a str, with ``beam_width``): only readings that match it in full (``b2o_crnn_forward_beam_pattern``),
-        logp their beam scores; slots past a crop's matching readings are -1 with logp -inf."""
+        logp their beam scores; slots past a crop's matching readings are -1 with logp -inf.
+        ``char_scores`` = A (``check_char_scores``): the result also ends with every reading's character confidences
+        (B,48) float32 and, with A > 0, its alternatives' labels (B,48,A) int32 and posteriors (B,48,A) float32
+        (``b2o_crnn_char_scores``); (B,P,48) / (B,P,48,A) with ``top_paths = P > 1``."""
         lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
         b = crnn_in.shape[0]
         lead = (b,) if top_paths == 1 else (b, top_paths)
         labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
         logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
+        scores = None if char_scores is None else self._score_buffers(lead, char_scores)
         self._forward(crnn_in, labels, logp, beam_width, top_paths, lexicon, language_model=language_model,
-                      pattern=pattern)
+                      pattern=pattern, char_scores=scores)
+        if scores is not None:
+            return ((labels, logp) if with_scores else (labels,)) + tuple(t for t in scores if t is not None)
         return (labels, logp) if with_scores else labels
 
+    def _score_buffers(self, lead, alternatives):
+        """Device outputs of ``b2o_crnn_char_scores`` for readings of shape ``lead``: (conf, alternative labels,
+        posteriors), the last two None when ``alternatives`` is 0."""
+        conf = torch.empty(lead + (STEPS,), dtype=torch.float32, device=self.device)
+        if not alternatives:
+            return conf, None, None
+        return (conf, torch.empty(lead + (STEPS, alternatives), dtype=torch.int32, device=self.device),
+                torch.empty(lead + (STEPS, alternatives), dtype=torch.float32, device=self.device))
+
     def _forward(self, crnn_in, labels, logp, beam_width, top_paths, lexicon, spans=None, theta=None,
-                 language_model=None, fused=None, pattern=None):
+                 language_model=None, fused=None, pattern=None, char_scores=None):
         """The CRNN and the decoder of ``predict_device`` into caller-allocated ``labels`` / ``logp`` (None: greedy
         without scores, or scores not written); ``lexicon`` is already compiled.  With ``language_model``, ``fused``
         (B,P) float32 or None receives every reading's F_end.  ``pattern`` is already compiled.  ``spans`` (B,P,48,2) int32: also the
         characters' emission spans of every reading (``b2o_crnn_align``) and, with an STN, its ``theta`` (B,6) float32;
-        the greedy forward then keeps its logits (``b2o_crnn_forward_logits``)."""
+        the greedy forward then keeps its logits (``b2o_crnn_forward_logits``).  ``char_scores``: (conf, alternative
+        labels or None, posteriors or None) of ``_score_buffers``, filled by ``b2o_crnn_char_scores`` after the decoder
+        (the greedy forward then keeps its logits too)."""
         b = crnn_in.shape[0]
         nbytes = self.ctx.crnn_workspace_bytes(b)
         if lexicon is not None:
@@ -946,7 +1004,7 @@ class Recognizer:
         elif beam_width is not None:
             self.ctx.crnn_forward_beam(crnn_in.data_ptr(), b, int(beam_width), int(top_paths), labels.data_ptr(),
                                        logp_ptr, ws.data_ptr(), nbytes, stream)
-        elif spans is not None:
+        elif spans is not None or char_scores is not None:
             self.ctx.crnn_forward_logits(crnn_in.data_ptr(), b, labels.data_ptr(), logp_ptr, ws.data_ptr(), nbytes,
                                          stream)
         elif logp is not None:
@@ -957,18 +1015,27 @@ class Recognizer:
         if spans is not None:
             self.ctx.crnn_align(b, labels.data_ptr(), int(top_paths), spans.data_ptr(), None,
                                 theta.data_ptr() if theta is not None else None, ws.data_ptr(), nbytes, stream)
+        if char_scores is not None:
+            conf, alt_labels, alt_post = char_scores
+            ptr = lambda t: t.data_ptr() if t is not None else None      # noqa: E731
+            self.ctx.crnn_char_scores(b, labels.data_ptr(), int(top_paths), 0 if alt_labels is None else alt_labels.shape[-1],
+                                      conf.data_ptr(), ptr(alt_labels), ptr(alt_post), None, ws.data_ptr(), nbytes, stream)
         self._last_ws = (ws, b) if self.keep_workspace else None
 
-    def _predict_aligned(self, crnn_in, beam_width, top_paths, lexicon, language_model=None, pattern=None):
+    def _predict_aligned(self, crnn_in, beam_width, top_paths, lexicon, language_model=None, pattern=None,
+                         char_scores=None):
         """``predict_device(with_scores=True)`` plus every reading's spans: (labels (B,P,48), logp (B,P), spans
-        (B,P,48,2) int32, theta (B,6) float32 or None without an STN)."""
+        (B,P,48,2) int32, theta (B,6) float32 or None without an STN), followed by the ``_score_buffers`` of
+        ``char_scores`` = A when it is given."""
         b, p = crnn_in.shape[0], int(top_paths)
         labels = torch.empty((b, p, STEPS), dtype=torch.int32, device=self.device)
         logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
         spans = torch.empty((b, p, STEPS, 2), dtype=torch.int32, device=self.device)
         theta = torch.empty((b, 6), dtype=torch.float32, device=self.device) if self.stn else None
-        self._forward(crnn_in, labels, logp, beam_width, p, lexicon, spans, theta, language_model, pattern=pattern)
-        return labels, logp, spans, theta
+        scores = None if char_scores is None else self._score_buffers((b, p), char_scores)
+        self._forward(crnn_in, labels, logp, beam_width, p, lexicon, spans, theta, language_model, pattern=pattern,
+                      char_scores=scores)
+        return (labels, logp, spans, theta) + (() if scores is None else (scores,))
 
     def char_cells_device(self, spans, theta, boxes=None, turns=None):
         """``b2o_char_cells``: spans (B,P,48,2) int32, theta (B,6) or None, boxes (B,4,2) float32 as they were cut (None:
@@ -989,7 +1056,8 @@ class Recognizer:
         return out
 
     def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                        return_char_boxes=False, language_model=None, pattern=None):
+                        return_char_boxes=False, language_model=None, pattern=None, return_char_scores=False,
+                        char_alternatives=0):
         """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str].
         ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``.  ``beam_width``: beam search
         decoding (``check_beam``); with ``top_paths = P > 1`` each text is a list of P strings and each confidence a
@@ -1000,8 +1068,13 @@ class Recognizer:
         readings that match it in full; a word with no matching reading reads "" with confidence 0.
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells (``b2o_char_cells``), an
         (n,4,2) float32 array for a text of n characters (a list of P arrays with ``top_paths = P > 1``), in the crop's
-        200 x 31 frame: (text, cells) or (text, confidence, cells)."""
+        200 x 31 frame: (text, cells) or (text, confidence, cells).
+        ``return_char_scores=True``: every word's tuple ends with its character scores (``check_char_scores``,
+        ``char_scores_host``), after the cells when both are asked for: an (n,) float32 array of the characters'
+        confidences, or with ``char_alternatives = A > 0`` that array and n lists of A (character, posterior) pairs;
+        a list of P of these with ``top_paths = P > 1``.  They are acoustic: they do not depend on the decoder."""
         lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
+        char_scores = check_char_scores(return_char_scores, char_alternatives)
         t = crops if isinstance(crops, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(crops))
         t = t.to(self.device).contiguous()
         b = t.shape[0]
@@ -1014,20 +1087,34 @@ class Recognizer:
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
                 "pattern": pattern}
         if return_char_boxes:
-            labels, logp, spans, theta = self._predict_aligned(crnn_in, **beam)
-            return self._with_cells(labels, logp, self.char_cells_device(spans, theta), top_paths, return_scores)
+            labels, logp, spans, theta, *scores = self._predict_aligned(crnn_in, char_scores=char_scores, **beam)
+            return self._host_words(labels, logp, top_paths, return_scores, self.char_cells_device(spans, theta),
+                                    scores[0] if scores else None)
+        if char_scores is not None:
+            labels, logp, *scores = self.predict_device(crnn_in, with_scores=True, char_scores=char_scores, **beam)
+            return self._host_words(labels, logp, top_paths, return_scores, None, scores)
         if not return_scores:
             return decode_paths(self.predict_device(crnn_in, **beam).cpu().numpy(), self.alphabet)[0]
         labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
         return list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
 
-    def _with_cells(self, labels, logp, cells, top_paths, return_scores):
-        """Host words of ``recognize_crops`` / ``recognize_from_boxes`` with cells: (text[, confidence], cells)."""
-        if top_paths == 1:
-            labels, logp, cells = labels[:, 0], logp[:, 0], cells[:, 0]
+    def _host_words(self, labels, logp, top_paths, return_scores, cells=None, scores=None):
+        """Host words of ``recognize_crops`` / ``recognize_from_boxes`` with cells and / or character scores:
+        (text[, confidence][, cells][, character scores]).  ``scores``: the device tensors of ``_score_buffers``
+        (None entries are skipped), or None."""
+        scores = None if scores is None else [t for t in scores if t is not None]
+        if top_paths == 1 and labels.dim() == 3:
+            labels, logp = labels[:, 0], logp[:, 0]
+            cells = None if cells is None else cells[:, 0]
+            scores = None if scores is None else [t[:, 0] for t in scores]
         texts, conf = decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())
-        boxes = char_boxes_host(cells.cpu().numpy(), texts)
-        return list(zip(texts, conf, boxes)) if return_scores else list(zip(texts, boxes))
+        cols = [texts] + ([conf] if return_scores else [])
+        if cells is not None:
+            cols.append(char_boxes_host(cells.cpu().numpy(), texts))
+        if scores is not None:
+            host = [t.cpu().numpy() for t in scores]
+            cols.append(char_scores_host(host[0], texts, self.alphabet, *host[1:]))
+        return list(zip(*cols))
 
     def recognize(self, image, beam_width=None, top_paths=1, lexicon=None, language_model=None, pattern=None):
         """Recognize text from a single pre-cropped image (reference recognition.py:467-489): fit to
@@ -1046,7 +1133,8 @@ class Recognizer:
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
                                     with_scores=False, beam_width=None, top_paths=1, lexicon=None, rotations=None,
                                     rotation_vote="word", char_boxes=False, polys=None, points=None, max_windows=1,
-                                    windows=None, language_model=None, pattern=None):
+                                    windows=None, language_model=None, pattern=None, char_scores=False,
+                                    char_alternatives=0):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
         (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon`` /
         ``language_model`` / ``pattern``: see ``predict_device``).
@@ -1061,6 +1149,12 @@ class Recognizer:
         character's first and last emitting step (``b2o_ctc_align``), -1 past the last -- and cells (B,48,4,2) float32,
         its quad in detector-input pixels (``b2o_char_cells``), NaN past the last character; (B,P,48,2) / (B,P,48,4,2)
         with ``top_paths = P > 1``.
+
+        ``char_scores=True`` (``check_char_scores``, with ``char_alternatives``): the result ends with every reading's
+        character confidences (B,48) float32 (``b2o_crnn_char_scores``) and, with ``char_alternatives = A > 0``, its
+        alternatives' labels (B,48,A) int32 and posteriors (B,48,A) float32, after the spans and cells when both are
+        asked for; (B,P,48) / (B,P,48,A) with ``top_paths = P > 1``.  It combines with every decoder, rotations and
+        polygons.
 
         Optional device-side by-products of the earlier stages, so that nothing but the kernel launches is
         left to do once the host knows the counts: ``gray`` (N,H,W) u8 from ``b2o_resize_pad_batch``;
@@ -1078,7 +1172,9 @@ class Recognizer:
         synchronisation."""
         lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
         turns = check_rotations(rotations, rotation_vote)
-        max_windows = check_windows(max_windows, beam_width, lexicon, turns, char_boxes, polys is not None)
+        scores = check_char_scores(char_scores, char_alternatives)
+        max_windows = check_windows(max_windows, beam_width, lexicon, turns, char_boxes, polys is not None,
+                                    scores is not None)
         if polys is not None and (turns is not None or char_boxes):
             raise ValueError("polygons do not combine with rotations or character boxes")
         counts = np.asarray(counts)
@@ -1091,7 +1187,8 @@ class Recognizer:
                 raise ValueError(f"windows must hold one window count in [1, {max_windows}] per box ({total}), as "
                                  f"b2o_window_counts gives them; got shape {windows.shape}")
         if total == 0:
-            parts = 1 + bool(with_scores) + (turns is not None) + 2 * bool(char_boxes)
+            parts = (1 + bool(with_scores) + (turns is not None) + 2 * bool(char_boxes)
+                     + (0 if scores is None else 1 + 2 * bool(scores)))
             return None if parts == 1 else (None,) * parts
         if self.color:
             gray = images_t                                       # color recognizer: crops come straight from the RGB batch
@@ -1111,37 +1208,39 @@ class Recognizer:
         if polys is not None:
             crnn_in, _ = self.warp_polys_device(gray, polys[:total], points[:total], image_index[:total])
             return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
-                                       lexicon=lexicon, language_model=language_model, pattern=pattern)
+                                       lexicon=lexicon, language_model=language_model, pattern=pattern,
+                                       char_scores=scores)
         if turns is not None:
             return self._recognize_turns(gray, flat[:total], image_index[:total], len(counts), boxes, turns,
                                          rotation_vote, with_scores, beam_width, top_paths, lexicon, char_boxes,
-                                         language_model, pattern)
+                                         language_model, pattern, scores)
         if char_boxes:
-            labels, logp, spans, cells = self._read_cells(gray, flat[:total], image_index[:total], beam_width,
-                                                          top_paths, lexicon, language_model, pattern)
-            return (labels, logp, spans, cells) if with_scores else (labels, spans, cells)
+            labels, logp, spans, cells, *extra = self._read_cells(gray, flat[:total], image_index[:total], beam_width,
+                                                                  top_paths, lexicon, language_model, pattern, scores)
+            return ((labels, logp, spans, cells) if with_scores else (labels, spans, cells)) + tuple(extra)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
         return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
-                                   lexicon=lexicon, language_model=language_model, pattern=pattern)
+                                   lexicon=lexicon, language_model=language_model, pattern=pattern, char_scores=scores)
 
-    def _read_cells(self, gray, flat, image_index, beam_width, top_paths, lexicon, language_model=None, pattern=None):
+    def _read_cells(self, gray, flat, image_index, beam_width, top_paths, lexicon, language_model=None, pattern=None,
+                    char_scores=None):
         """Warp + CRNN + decoder + alignment + cells of one pass: (labels, logp, spans, cells) in the shapes of
-        ``recognize_from_boxes_device``."""
+        ``recognize_from_boxes_device``, followed by the character scores with ``char_scores`` = A."""
         crnn_in, _ = self.warp_device(gray, flat, image_index)
-        labels, logp, spans, theta = self._predict_aligned(crnn_in, beam_width, top_paths, lexicon, language_model,
-                                                           pattern)
+        labels, logp, spans, theta, *scores = self._predict_aligned(crnn_in, beam_width, top_paths, lexicon,
+                                                                    language_model, pattern, char_scores)
         cells = self.char_cells_device(spans, theta, flat)
-        if top_paths == 1:
-            labels, logp, spans, cells = labels[:, 0], logp[:, 0], spans[:, 0], cells[:, 0]
-        return labels, logp, spans, cells
+        out = (labels, logp, spans, cells) + (tuple(t for t in scores[0] if t is not None) if scores else ())
+        return tuple(t[:, 0] for t in out) if top_paths == 1 else out
 
     def _recognize_turns(self, gray, flat, image_index, n_images, table, turns, vote, with_scores, beam_width,
-                         top_paths, lexicon, char_boxes=False, language_model=None, pattern=None):
+                         top_paths, lexicon, char_boxes=False, language_model=None, pattern=None, char_scores=None):
         """Warp + CRNN + decoder for each turn into its slot of one (R,B,P,48) / (R,B,P) stack, then
         ``b2o_select_rotation``, which also rolls ``flat`` and ``table`` (None: no table) in place.  ``char_boxes``: each
         turn's spans and theta are stacked alike, and the chosen turn's cells are built from the boxes as they were cut.
         With ``language_model`` the vote compares the readings' F_end, and the chosen turn's acoustic logp is gathered
-        on the device."""
+        on the device.  ``char_scores`` = A: each turn's character scores are stacked alike and the chosen turn's
+        gathered; they end the result."""
         b, p, r = flat.shape[0], int(top_paths), len(turns)
         labels_all = torch.empty((r, b, p, STEPS), dtype=torch.int32, device=self.device)
         logp_all = torch.empty((r, b, p), dtype=torch.float32, device=self.device)
@@ -1151,11 +1250,13 @@ class Recognizer:
             spans_all = torch.empty((r, b, p, STEPS, 2), dtype=torch.int32, device=self.device)
             theta_all = torch.empty((r, b, 6), dtype=torch.float32, device=self.device) if self.stn else None
             cut = flat.clone()                           # b2o_select_rotation rolls flat in place
+        scores_all = None if char_scores is None else self._score_buffers((r, b, p), char_scores)
         for j, turn in enumerate(turns):
             crnn_in, _ = self.warp_device(gray, flat, image_index, turn=turn)
             self._forward(crnn_in, labels_all[j], logp_all[j], beam_width, p, lexicon,
                           None if spans_all is None else spans_all[j], None if theta_all is None else theta_all[j],
-                          language_model, None if fused_all is None else fused_all[j], pattern)
+                          language_model, None if fused_all is None else fused_all[j], pattern,
+                          None if scores_all is None else tuple(None if t is None else t[j] for t in scores_all))
         labels = torch.empty((b, p, STEPS), dtype=torch.int32, device=self.device)
         logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
         chosen = torch.empty((b,), dtype=torch.int32, device=self.device)
@@ -1165,7 +1266,7 @@ class Recognizer:
                                  flat.data_ptr(), None if table is None else table.data_ptr(),
                                  0 if table is None else table.shape[1], torch.cuda.current_stream(self.device).cuda_stream)
         extra = ()
-        if char_boxes or fused_all is not None:
+        if char_boxes or fused_all is not None or scores_all is not None:
             slot = torch.zeros(4, dtype=torch.int64, device=self.device)
             slot[list(turns)] = torch.arange(r, device=self.device)
             pick, rows = slot[chosen.long()], torch.arange(b, device=self.device)
@@ -1175,6 +1276,9 @@ class Recognizer:
             spans = spans_all[pick, rows]
             cells = self.char_cells_device(spans, None if theta_all is None else theta_all[pick, rows], cut, chosen)
             extra = (spans[:, 0], cells[:, 0]) if p == 1 else (spans, cells)
+        if scores_all is not None:
+            picked = tuple(t[pick, rows] for t in scores_all if t is not None)
+            extra = extra + (tuple(t[:, 0] for t in picked) if p == 1 else picked)
         if p == 1:
             labels, logp = labels.view(b, STEPS), logp.view(b)
         return ((labels, logp, chosen) if with_scores else (labels, chosen)) + extra
@@ -1182,7 +1286,8 @@ class Recognizer:
     # ------------------------------------------------------------------ reference API
     def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
                              rotations=None, rotation_vote="word", return_char_boxes=False, max_windows=1,
-                             language_model=None, pattern=None, **kwargs) -> typing.List[typing.List[str]]:
+                             language_model=None, pattern=None, return_char_scores=False, char_alternatives=0,
+                             **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
         (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon`` /
         ``language_model`` / ``pattern``: as ``recognize_crops``; with rotations the vote compares the language model's fused scores.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
@@ -1190,6 +1295,8 @@ class Recognizer:
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells, an (n,4,2) float32 array
         of quads in the image's pixels for a text of n characters (a list of P arrays with ``top_paths = P > 1``):
         (text, cells) or (text, confidence, cells); see ``recognize_from_boxes_device``.
+        ``return_char_scores=True`` / ``char_alternatives``: every word's tuple ends with its character scores, after
+        the cells when both are asked for, as ``recognize_crops`` returns them.
 
         A box group may also hold polygons, (2m,2) arrays with 3 <= m <= 9 as ``Detector.detect(return_polygons=True)``
         returns them (``check_polygons``): such a word is read along its polygon (``b2o_warp_polys``), a 4-point entry
@@ -1204,10 +1311,12 @@ class Recognizer:
 
         entries = [e for g in box_groups for e in g]
         polygons = any(np.ndim(e) == 2 and np.shape(e)[0] != 4 for e in entries)
-        max_windows = check_windows(max_windows, beam_width, lexicon, turns, return_char_boxes, polygons)
+        char_scores = check_char_scores(return_char_scores, char_alternatives)
+        max_windows = check_windows(max_windows, beam_width, lexicon, turns, return_char_boxes, polygons,
+                                    char_scores is not None)
         if polygons:
             return self._recognize_polygons(images, box_groups, entries, return_scores, turns, return_char_boxes,
-                                            beam_width, top_paths, lexicon, language_model, pattern)
+                                            beam_width, top_paths, lexicon, language_model, pattern, char_scores)
         images_t = _as_device_images(images, self.device)
         counts = np.array([len(b) for b in box_groups], dtype=np.int64)
         if counts.sum() == 0:
@@ -1222,15 +1331,21 @@ class Recognizer:
         gray = images_t if self.color else self.gray_device(images_t)
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
                 "pattern": pattern}
-        if return_char_boxes:
+        if return_char_boxes or char_scores is not None:
+            cells = None
             if turns is not None:
-                labels, logp, _, _, cells = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns,
-                                                                  rotation_vote, True, char_boxes=True, **beam)
+                labels, logp, _, *rest = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns,
+                                                               rotation_vote, True, char_boxes=return_char_boxes,
+                                                               char_scores=char_scores, **beam)
+                if return_char_boxes:
+                    cells, rest = rest[1], rest[2:]
+            elif return_char_boxes:
+                labels, logp, _, cells, *rest = self._read_cells(gray, flat_t, idx, char_scores=char_scores, **beam)
             else:
-                labels, logp, _, cells = self._read_cells(gray, flat_t, idx, **beam)
-            texts, conf = decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())
-            cells = char_boxes_host(cells.cpu().numpy(), texts)
-            predictions = list(zip(texts, conf, cells)) if return_scores else list(zip(texts, cells))
+                crnn_in, _ = self.warp_device(gray, flat_t, idx)
+                labels, logp, *rest = self.predict_device(crnn_in, with_scores=True, char_scores=char_scores, **beam)
+            predictions = self._host_words(labels, logp, top_paths, return_scores, cells,
+                                           rest if char_scores is not None else None)
         elif turns is not None:
             labels, logp, _ = self._recognize_turns(gray, flat_t, idx, len(counts), None, turns, rotation_vote, True,
                                                     **beam)
@@ -1251,7 +1366,7 @@ class Recognizer:
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]
 
     def _recognize_polygons(self, images, box_groups, entries, return_scores, turns, char_boxes, beam_width, top_paths,
-                            lexicon, language_model=None, pattern=None):
+                            lexicon, language_model=None, pattern=None, char_scores=None):
         """``recognize_from_boxes`` for box groups that hold polygons: 4-point entries are rectified as
         ``tools.rectify_boxes`` does and cut as boxes, the others along their polygon, all in one ``b2o_warp_polys``."""
         if turns is not None or char_boxes:
@@ -1270,7 +1385,10 @@ class Recognizer:
                                             torch.from_numpy(points).to(self.device), idx)
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
                 "pattern": pattern}
-        if return_scores:
+        if char_scores is not None:
+            labels, logp, *scores = self.predict_device(crnn_in, with_scores=True, char_scores=char_scores, **beam)
+            predictions = self._host_words(labels, logp, top_paths, return_scores, None, scores)
+        elif return_scores:
             labels, logp = self.predict_device(crnn_in, with_scores=True, **beam)
             predictions = list(zip(*decode_paths(labels.cpu().numpy(), self.alphabet, logp.cpu().numpy())))
         else:
