@@ -437,6 +437,42 @@ int b2o_crnn_forward_beam_lm(b2o_ctx* ctx, const void* crnn_in_dev, int b, int b
                              const b2o_char_lm* lm, int32_t* labels_dev, float* logp_dev, float* fused_dev, void* ws_dev,
                              size_t ws_bytes, void* stream);
 
+/* CTC prefix beam search with a bonus for a caller's word list, with or without a language model (DESIGN.md section 1,
+ * "Hotwords").  The trie of the list, built on the host (recognition.Hotwords.device_arrays): n_nodes nodes numbered
+ * breadth-first by (depth, parent, label), the root 0 the empty prefix; n_edges = n_nodes - 1 edges as ascending uint64
+ * keys keys_dev, key = (parent << 8) | label, with child_dev (n_edges) int32 the child of each edge, so the children of
+ * a node are contiguous; final_dev (n_nodes) uint8, 1 where the node's prefix is a listed word.  A prefix is live when
+ * it is a node (a prefix of a listed word).  Bonus H(a) = weight * |a| for a live a, else 0; H_end(a) = weight * |a|
+ * for a listed word, else 0.  Candidates rank by F = (A + G) + H and the top_paths readings by
+ * F_end = ((A + G) + alpha * l(</s> | hist)) + H_end, in float32 in that order, each addition of H or H_end skipped
+ * when it is 0; A and G are those of b2o_ctc_beam_lm_decode, and lm = NULL is a model of zeros (G = 0, alpha = 0).
+ * Each step a beam extends by its own shortlist, the min(beam_width + 1, k - 1) labels with the largest
+ * (lp[t,c] + alpha * l(c | hist)) + H(a + c) (ties: smaller label).  labels_dev, logp_dev (the acoustic A) and
+ * fused_dev (F_end) as b2o_ctc_beam_lm_decode writes them.  weight = 0, or a trie of the root alone, gives
+ * b2o_ctc_beam_lm_decode's labels, logp and fused bit for bit, and without a model b2o_ctc_beam_decode's labels and
+ * logp.  A crop's result is a function of its logits, the model and the list alone.
+ * 1 <= n_nodes <= B2O_MAX_HOTWORD_NODES, n_edges = n_nodes - 1, keys and child not NULL when n_edges > 0, final not
+ * NULL, weight finite and >= 0, a valid lm (as b2o_ctc_beam_lm_decode takes it) or NULL, 2 <= k <=
+ * B2O_MAX_LM_CLASSES and the beam_width / top_paths rules of beam search, otherwise B2O_ERR_ARG.
+ * b2o_ctc_beam_hotword_decode: the search alone on caller-supplied (b, 48, k) float32 logits.
+ * b2o_crnn_forward_beam_hotword: the CRNN of b2o_crnn_forward, its fc_12 logits into the workspace (so b2o_crnn_align
+ * and b2o_crnn_char_scores work after it), then the search.                                                         */
+#define B2O_MAX_HOTWORD_NODES ((1 << 24) + 1)
+typedef struct {
+  int n_nodes;
+  int n_edges;
+  const uint64_t* keys_dev;
+  const int32_t* child_dev;
+  const uint8_t* final_dev;
+  float weight;
+} b2o_hotwords;
+int b2o_ctc_beam_hotword_decode(b2o_ctx* ctx, const float* logits_dev, int b, int k, int beam_width, int top_paths,
+                                const b2o_char_lm* lm, const b2o_hotwords* hw, int32_t* labels_dev, float* logp_dev,
+                                float* fused_dev, void* stream);
+int b2o_crnn_forward_beam_hotword(b2o_ctx* ctx, const void* crnn_in_dev, int b, int beam_width, int top_paths,
+                                  const b2o_char_lm* lm, const b2o_hotwords* hw, int32_t* labels_dev, float* logp_dev,
+                                  float* fused_dev, void* ws_dev, size_t ws_bytes, void* stream);
+
 /* CTC prefix beam search constrained to a pattern: a deterministic automaton over the labels (DESIGN.md section 1,
  * "Patterns"), built on the host (recognition.Pattern.device_arrays).  n_states states, trans_dev (n_states, k-1) int16:
  * trans[q][c] the state after label c in state q, -1 for none; dist_dev (n_states) uint8: the fewest labels from q to an

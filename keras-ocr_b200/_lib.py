@@ -21,6 +21,7 @@ MAX_LEXICON_TOP_PATHS = 128   # B2O_MAX_LEXICON_TOP_PATHS
 MAX_LM_ORDER = 8              # B2O_MAX_LM_ORDER
 MAX_LM_HISTORIES = 1 << 20    # B2O_MAX_LM_HISTORIES
 MAX_LM_CLASSES = 127          # B2O_MAX_LM_CLASSES
+MAX_HOTWORD_NODES = (1 << 24) + 1   # B2O_MAX_HOTWORD_NODES
 MAX_PATTERN_STATES = 4096     # B2O_MAX_PATTERN_STATES
 MAX_PATTERN_CLASSES = 127     # B2O_MAX_PATTERN_CLASSES
 ROTATION_VOTE_WORD, ROTATION_VOTE_PAGE = 0, 1   # B2O_ROTATION_VOTE_WORD / _PAGE
@@ -78,6 +79,15 @@ class CharLMDesc(ctypes.Structure):
 
 
 _lmp = _c.POINTER(CharLMDesc)
+
+
+class HotwordsDesc(ctypes.Structure):
+    """b2o_hotwords (include/b2ocr.h), field for field."""
+    _fields_ = [("n_nodes", _i), ("n_edges", _i), ("keys_dev", _vp), ("child_dev", _vp), ("final_dev", _vp),
+                ("weight", _f)]
+
+
+_hwp = _c.POINTER(HotwordsDesc)
 
 
 class PatternDesc(ctypes.Structure):
@@ -155,6 +165,8 @@ SIGNATURES = {
     "b2o_crnn_forward_beam": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "b2o_ctc_beam_lm_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _lmp, _vp, _vp, _vp, _vp]),
     "b2o_crnn_forward_beam_lm": (_i, [_vp, _vp, _i, _i, _i, _lmp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2o_ctc_beam_hotword_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _lmp, _hwp, _vp, _vp, _vp, _vp]),
+    "b2o_crnn_forward_beam_hotword": (_i, [_vp, _vp, _i, _i, _i, _lmp, _hwp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2o_ctc_beam_pattern_decode": (_i, [_vp, _vp, _i, _i, _i, _i, _patp, _vp, _vp, _vp]),
     "b2o_crnn_forward_beam_pattern": (_i, [_vp, _vp, _i, _i, _i, _patp, _vp, _vp, _vp, _sz, _vp]),
     "b2o_lexicon_workspace_bytes": (_sz, [_i, _i, _i]),
@@ -489,6 +501,19 @@ class Context:
         self._check(self.lib.b2o_crnn_forward_beam_lm(self.handle, crnn_in, b, beam_width, top_paths, ctypes.byref(lm),
                                                       labels, logp, fused, ws, ws_bytes, stream),
                     "b2o_crnn_forward_beam_lm")
+
+    def ctc_beam_hotword_decode(self, logits, b, k, beam_width, top_paths, lm, hw, labels, logp, fused, stream):
+        """``lm``: a ``CharLMDesc`` or None (no model); ``hw``: a ``HotwordsDesc``."""
+        self._check(self.lib.b2o_ctc_beam_hotword_decode(self.handle, logits, b, k, beam_width, top_paths,
+                                                         None if lm is None else ctypes.byref(lm), ctypes.byref(hw),
+                                                         labels, logp, fused, stream), "b2o_ctc_beam_hotword_decode")
+
+    def crnn_forward_beam_hotword(self, crnn_in, b, beam_width, top_paths, lm, hw, labels, logp, fused, ws, ws_bytes,
+                                  stream):
+        self._check(self.lib.b2o_crnn_forward_beam_hotword(self.handle, crnn_in, b, beam_width, top_paths,
+                                                           None if lm is None else ctypes.byref(lm), ctypes.byref(hw),
+                                                           labels, logp, fused, ws, ws_bytes, stream),
+                    "b2o_crnn_forward_beam_hotword")
 
     def ctc_beam_pattern_decode(self, logits, b, k, beam_width, top_paths, pattern, labels, logp, stream):
         """``pattern``: a ``PatternDesc``."""

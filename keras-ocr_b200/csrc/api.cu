@@ -20,6 +20,9 @@ int ctc_beam_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width
                  cudaStream_t st);
 int ctc_beam_lm_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
                     const b2o_char_lm* lm, int* labels, float* logp, float* fused, cudaStream_t st);
+int ctc_beam_hotword_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
+                         const b2o_char_lm* lm, const b2o_hotwords* hw, int* labels, float* logp, float* fused,
+                         cudaStream_t st);
 int ctc_beam_pattern_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
                          const b2o_pattern* pat, int* labels, float* logp, cudaStream_t st);
 size_t ctc_lexicon_workspace_bytes(int B, int n_words);
@@ -927,6 +930,83 @@ extern "C" int b2o_ctc_beam_lm_decode(b2o_ctx* ctx, const float* logits, int b, 
   DeviceGuard guard(ctx->device);
   return ctc_beam_lm_run(ctx, logits, b, k, beam_width, top_paths, lm, labels, logp, fused,
                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+namespace {
+
+bool hotword_args_ok(b2o_ctx* ctx, const char* fn, int k, int beam_width, int top_paths, const b2o_char_lm* lm,
+                     const b2o_hotwords* hw) {
+  if (lm) {
+    if (!lm_args_ok(ctx, fn, k, beam_width, top_paths, lm)) return false;
+  } else {
+    if (!beam_args_ok(ctx, fn, k, beam_width, top_paths)) return false;
+    if (k > B2O_MAX_LM_CLASSES) { ctx->set_error(std::string(fn) + ": k must be in [2, 127]"); return false; }
+  }
+  if (!hw) { ctx->set_error(std::string(fn) + ": no hotwords"); return false; }
+  if (hw->n_nodes < 1 || hw->n_nodes > B2O_MAX_HOTWORD_NODES || hw->n_edges != hw->n_nodes - 1) {
+    ctx->set_error(std::string(fn) + ": n_nodes must be in [1, 2^24 + 1] and n_edges = n_nodes - 1");
+    return false;
+  }
+  if (!hw->final_dev || (hw->n_edges > 0 && (!hw->keys_dev || !hw->child_dev))) {
+    ctx->set_error(std::string(fn) + ": missing trie arrays");
+    return false;
+  }
+  if (!std::isfinite(hw->weight) || hw->weight < 0.f) {
+    ctx->set_error(std::string(fn) + ": weight must be finite and >= 0");
+    return false;
+  }
+  return true;
+}
+
+// The model of b2o_ctc_beam_hotword_decode without one: order 2, one empty-history row of zeros, alpha = beta = 0,
+// which makes the language-model search plain beam search bit for bit.  Uploaded once per context.
+const b2o_char_lm* zero_lm(b2o_ctx* ctx) {
+  if (!ctx->zero_lm.keys_dev) {
+    const uint64_t* keys = dev_upload(ctx, std::vector<uint64_t>(1, 0));
+    const float* rows = keys ? dev_upload(ctx, std::vector<float>(B2O_MAX_LM_CLASSES, 0.f)) : nullptr;
+    if (!rows) return nullptr;
+    ctx->zero_lm = b2o_char_lm{2, 1, keys, rows, 0.f, 0.f};
+  }
+  return &ctx->zero_lm;
+}
+
+}  // namespace
+
+extern "C" int b2o_crnn_forward_beam_hotword(b2o_ctx* ctx, const void* crnn_in, int b, int beam_width, int top_paths,
+                                             const b2o_char_lm* lm, const b2o_hotwords* hw, int32_t* labels,
+                                             float* logp, float* fused, void* ws, size_t ws_bytes, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!ctx->crnn_loaded) {
+    ctx->set_error("b2o_crnn_forward_beam_hotword: CRNN weights not loaded");
+    return B2O_ERR_STATE;
+  }
+  if (!hotword_args_ok(ctx, "b2o_crnn_forward_beam_hotword", ctx->n_classes, beam_width, top_paths, lm, hw))
+    return B2O_ERR_ARG;
+  if (b == 0) return B2O_OK;
+  DeviceGuard guard(ctx->device);
+  const b2o_char_lm* model = lm ? lm : zero_lm(ctx);
+  if (!model) return B2O_ERR_CUDA;
+  B2O_RETURN_IF(crnn_forward(ctx, crnn_in, b, labels, nullptr, true, ws, ws_bytes, stream));
+  const float* logits = reinterpret_cast<const float*>(reinterpret_cast<uint8_t*>(ws) + plan_crnn(b).off[rb::logits]);
+  return ctc_beam_hotword_run(ctx, logits, b, ctx->n_classes, beam_width, top_paths, model, hw, labels, logp, fused,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2o_ctc_beam_hotword_decode(b2o_ctx* ctx, const float* logits, int b, int k, int beam_width,
+                                           int top_paths, const b2o_char_lm* lm, const b2o_hotwords* hw,
+                                           int32_t* labels, float* logp, float* fused, void* stream) {
+  if (!ctx) return B2O_ERR_ARG;
+  if (!hotword_args_ok(ctx, "b2o_ctc_beam_hotword_decode", k, beam_width, top_paths, lm, hw)) return B2O_ERR_ARG;
+  if (b < 0 || (b > 0 && (!logits || !labels))) {
+    ctx->set_error("b2o_ctc_beam_hotword_decode: bad argument");
+    return B2O_ERR_ARG;
+  }
+  if (b == 0) return B2O_OK;
+  DeviceGuard guard(ctx->device);
+  const b2o_char_lm* model = lm ? lm : zero_lm(ctx);
+  if (!model) return B2O_ERR_CUDA;
+  return ctc_beam_hotword_run(ctx, logits, b, k, beam_width, top_paths, model, hw, labels, logp, fused,
+                              reinterpret_cast<cudaStream_t>(stream));
 }
 
 namespace {

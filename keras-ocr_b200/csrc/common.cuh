@@ -118,6 +118,7 @@ struct b2o_ctx {
   float *fc12_w = nullptr, *fc12_b = nullptr;                  // [256][K], [K] fp32, K = len(alphabet) + 1
   int n_classes = 37;                                          // K (last index = CTC blank), <= B2O_MAX_CLASSES
   std::vector<void*> owned;    // device allocations freed in b2o_destroy
+  b2o_char_lm zero_lm{};       // hotwords without a model: order 2, one empty-history row of zeros (uploaded on first use)
   // optional per-launch timing of the tensor-core conv kernel (bench.py's roofline leg)
   bool debug_taps = false;     // b2o_set_debug_taps: the CRNN forward also writes its fp32 logits (tests only)
   int craft_step = -1;         // last step of the most recent successful CRAFT forward (b2o_craft_tap), -1: none

@@ -424,7 +424,50 @@ ctc_beam_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W, i
 // exact arithmetic: a near-tie, which tests/test_gpu_lm.py counts and bounds.
 // With alpha = beta = 0 every alpha * l is +-0, so the shortlist key is lp, G = +0, F = A and F_end = A bit for bit: the
 // per-beam shortlists equal the global one and the search returns ctc_beam_kernel's labels and scores exactly.
+//
+// Hotwords (kHot, DESIGN.md section 1, "Hotwords"): the same kernel also ranks by a bonus for a caller's word list.
+//   A prefix is live when it is a prefix of a listed word (the empty prefix is); H(a) = gamma |a| when a is live, else 0,
+//   and H_end(a) = gamma |a| when a is a listed word, else 0.  Candidates rank by F = (A + G) + H and the returned paths
+//   by F_end = ((A + G) + alpha l(</s> | hist)) + H_end, each addition of H or H_end skipped when it is 0 (so gamma = 0,
+//   or an empty list, gives the kernel without kHot bit for bit).  H is a function of the prefix: merging is unchanged.
+//   A beam also carries its trie node (-1 once it is not live): a beam kept via blank or its last label keeps its
+//   parent's node, an extension a+c looks up the child of a's node by c once, by binary search over the sorted edge
+//   keys (parent << 8) | label, whose children of one node are contiguous.
+//   2''. the shortlist key of c is lp[c] + alpha l(c | hist(a)) + H(a+c) (the addition skipped when H(a+c) = 0): F(a+c)
+//       less the per-beam terms A(a) or p_b(a), G(a) and beta.  A live a finds its children's range once, and each lane
+//       its labels in that range; the shortlist records which of its labels keep a+c live.
+// Why the per-beam shortlist still loses nothing: F(a+c) = (c == last(a) ? p_b(a) : A(a)) + G(a) + beta + key(c) in
+// exact arithmetic.  S = W+1 labels c' rank above c by key; at most one of them is last(a), so at least W of them give
+// a+c' an F >= A(a) + G(a) + beta + key(c') >= F(a+c) (H(a+c') enters F(a+c') exactly as it enters key(c'), merging
+// only adds to A, and F is monotone in A), and each of those W prefixes beats a+c or ties and precedes it.  In fp32
+// the key and F group the sums differently, so candidates within a few ulps of F can be ordered differently from exact
+// arithmetic: a near-tie, which tests/test_gpu_hotwords.py counts and bounds.
 constexpr unsigned kLmBos = 127u;                 // the code of <s> in a packed history (labels are < 126)
+
+struct Trie {                                     // b2o_hotwords on the device (kHot only)
+  const unsigned long long* keys;                 // [n_edges] (parent << 8) | label, ascending
+  const int* child;                               // [n_edges] the child node of each edge
+  const unsigned char* fin;                       // [n_nodes] 1: the node's prefix is a listed word
+  int n_edges;
+  float gamma;
+};
+
+// The first index in [lo, hi) whose key is >= k.
+__device__ __forceinline__ int lower_key(const unsigned long long* __restrict__ keys, int lo, int hi,
+                                         unsigned long long k) {
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(keys + mid) < k) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// The child of live node u by label c, or -1.
+__device__ int trie_child(const Trie& tr, int u, int c) {
+  const unsigned long long k = (static_cast<unsigned long long>(u) << 8) | static_cast<unsigned>(c);
+  const int j = lower_key(tr.keys, 0, tr.n_edges, k);
+  return j < tr.n_edges && __ldg(tr.keys + j) == k ? __ldg(tr.child + j) : -1;
+}
 
 struct SmemLm {
   short* shl;                      // [W][S] per-beam shortlist, ascending labels
@@ -454,6 +497,27 @@ __host__ __device__ inline size_t smem_plan_lm(int W, int K, unsigned char* base
   return off;
 }
 
+struct SmemHot {
+  int* node[2];                    // [W] the beam's trie node, -1 once its prefix is not live
+  unsigned char* kid;              // [W][S] shl[x] keeps the beam's prefix live
+};
+
+__host__ __device__ inline size_t smem_plan_hot(int W, int K, unsigned char* base, Smem* s, SmemLm* l, SmemHot* h) {
+  size_t off = smem_plan_lm(W, K, base, s, l);
+  const int S = shortlist_size(W, K);
+  SmemHot d;
+  SmemHot* p = h ? h : &d;
+#define B2O_TAKE(ptr, type, count)                                                    \
+  do {                                                                                \
+    if (base) (ptr) = reinterpret_cast<type*>(base + off);                            \
+    off += (static_cast<size_t>(count) * sizeof(type) + 15) / 16 * 16;                \
+  } while (0)
+  for (int i = 0; i < 2; ++i) B2O_TAKE(p->node[i], int, W);
+  B2O_TAKE(p->kid, unsigned char, W * S);
+#undef B2O_TAKE
+  return off;
+}
+
 // The row of the longest listed suffix of the history of "<s> pre[0..L)": keys sorted ascending, (n << 56) | the n
 // symbols packed 8 bits each, oldest highest; keys[0] = 0 is the empty history.
 __device__ int lm_row(const unsigned long long* __restrict__ keys, int H, int order, const short* pre, int L) {
@@ -476,14 +540,44 @@ __device__ int lm_row(const unsigned long long* __restrict__ keys, int H, int or
 }
 
 // One warp: the S labels c < n with the largest lp[c] + alpha * lrow[c] (ties: smaller label), ascending, into out[S].
-__device__ void lm_shortlist(const float* lp, const float* __restrict__ lrow, float alpha, int n, int S, short* out) {
+// kHot: plus hb = H(a+c) for the labels that keep the beam's prefix live (node >= 0: its trie node); kid[S] then flags
+// those labels of out.
+template <bool kHot>
+__device__ void lm_shortlist(const float* lp, const float* __restrict__ lrow, float alpha, int n, int S, short* out,
+                             const Trie& tr, int node, float hb, unsigned char* kid) {
   const int lane = threadIdx.x & 31;
   const unsigned lt = (1u << lane) - 1u;
   unsigned kv[4];
+  unsigned live = 0;                              // kHot: bit i set when lane + 32 i keeps the prefix live
+  if constexpr (kHot) {
+    int lo = 0, hi = 0;
+    const unsigned long long base = static_cast<unsigned long long>(node) << 8;
+    if (node >= 0) {                              // the node's children: one contiguous key range
+      lo = lower_key(tr.keys, 0, tr.n_edges, base);
+      hi = lower_key(tr.keys, lo, tr.n_edges, base + 256);
+    }
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int c = lane + 32 * i;
-    kv[i] = c < n ? okey(__fadd_rn(lp[c], __fmul_rn(alpha, __ldg(lrow + c)))) : 0u;
+    for (int i = 0; i < 4; ++i) {
+      const int c = lane + 32 * i;
+      float v = 0.f;
+      if (c < n) {
+        v = __fadd_rn(lp[c], __fmul_rn(alpha, __ldg(lrow + c)));
+        if (lo < hi) {
+          const int j = lower_key(tr.keys, lo, hi, base | static_cast<unsigned>(c));
+          if (j < hi && __ldg(tr.keys + j) == (base | static_cast<unsigned>(c))) {
+            live |= 1u << i;
+            if (hb != 0.f) v = __fadd_rn(v, hb);
+          }
+        }
+      }
+      kv[i] = c < n ? okey(v) : 0u;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = lane + 32 * i;
+      kv[i] = c < n ? okey(__fadd_rn(lp[c], __fmul_rn(alpha, __ldg(lrow + c)))) : 0u;
+    }
   }
   unsigned theta = 0;
   int take = 0;
@@ -509,6 +603,9 @@ __device__ void lm_shortlist(const float* lp, const float* __restrict__ lrow, fl
     const bool in = c < n && (S == n || kv[i] > theta || (eq && eq_before + __popc(eqm & lt) < take));
     const unsigned m = __ballot_sync(0xffffffffu, in);
     if (in) out[at + __popc(m & lt)] = static_cast<short>(c);
+    if constexpr (kHot) {
+      if (in) kid[at + __popc(m & lt)] = static_cast<unsigned char>((live >> i) & 1u);
+    }
     at += __popc(m);
     eq_before += __popc(eqm);
   }
@@ -533,15 +630,19 @@ struct LmOrder {                                  // candidate label sequences w
   }
 };
 
+template <bool kHot>
 __global__ void __launch_bounds__(kThreads)
 ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W, int P,
                    const unsigned long long* __restrict__ lm_keys /*[H]*/, const float* __restrict__ lm_rows /*[H][K]*/,
                    int H, int order, float alpha, float beta, int* __restrict__ labels /*[B][P][48]*/,
-                   float* __restrict__ logp /*[B][P] or null*/, float* __restrict__ fused /*[B][P] or null*/) {
+                   float* __restrict__ logp /*[B][P] or null*/, float* __restrict__ fused /*[B][P] or null*/,
+                   Trie tr /*kHot only*/) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   Smem s;
   SmemLm l;
-  smem_plan_lm(W, K, smem_raw, &s, &l);
+  SmemHot hw;
+  if constexpr (kHot) smem_plan_hot(W, K, smem_raw, &s, &l, &hw);
+  else smem_plan_lm(W, K, smem_raw, &s, &l);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int blank = K - 1, S = shortlist_size(W, K), S1 = S + 1;
   int cur = 0, nb = 1;
@@ -550,6 +651,7 @@ ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W
     s.h[0][0] = kHashRoot; s.ph[0][0] = 0;
     l.g[0][0] = 0.f; l.f[0][0] = 0.f;
     l.row[0][0] = lm_row(lm_keys, H, order, s.pre[0], 0);
+    if constexpr (kHot) hw.node[0][0] = 0;         // the trie's root: the empty prefix is live
   }
   for (int t = 0; t < kT; ++t) {
     // ---- 1. lp of step t (as ctc_beam_kernel)
@@ -577,8 +679,14 @@ ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W
     __syncthreads();
 
     // ---- 2'. per-beam shortlists, one warp per beam
-    for (int a = warp; a < nb; a += kWarps)
-      lm_shortlist(s.lp, lm_rows + static_cast<size_t>(l.row[cur][a]) * K, alpha, K - 1, S, l.shl + a * S);
+    for (int a = warp; a < nb; a += kWarps) {
+      if constexpr (kHot)
+        lm_shortlist<true>(s.lp, lm_rows + static_cast<size_t>(l.row[cur][a]) * K, alpha, K - 1, S, l.shl + a * S, tr,
+                           hw.node[cur][a], __fmul_rn(tr.gamma, static_cast<float>(s.len[cur][a] + 1)), hw.kid + a * S);
+      else
+        lm_shortlist<false>(s.lp, lm_rows + static_cast<size_t>(l.row[cur][a]) * K, alpha, K - 1, S, l.shl + a * S,
+                            tr, -1, 0.f, nullptr);
+    }
 
     // ---- 3. parent links and the extensions that are already beams
     const Beams bm{s, cur, S1};
@@ -606,7 +714,7 @@ ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W
     }
     __syncthreads();
 
-    // ---- 4. candidate keys: F = A + G
+    // ---- 4. candidate keys: F = A + G (kHot: F = (A + G) + H)
     auto candidate = [&](int i, float* pb, float* pnb, float* g) {
       const int a = i / S1, x = i - a * S1;
       if (x == 0) {
@@ -628,7 +736,16 @@ ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W
       if (x == 0 || !s.excl[a * S + x - 1]) {
         float pb, pnb, g;
         candidate(i, &pb, &pnb, &g);
-        k = okey(__fadd_rn(lae(pb, pnb), g));
+        if constexpr (kHot) {
+          float f = __fadd_rn(lae(pb, pnb), g);
+          const int len = s.len[cur][a];
+          const bool live = x == 0 ? hw.node[cur][a] >= 0 : hw.kid[a * S + x - 1] != 0;
+          const float h = live ? __fmul_rn(tr.gamma, static_cast<float>(len + (x > 0))) : 0.f;
+          if (h != 0.f) f = __fadd_rn(f, h);
+          k = okey(f);
+        } else {
+          k = okey(__fadd_rn(lae(pb, pnb), g));
+        }
         ++valid;
       }
       s.key[i] = k;
@@ -699,13 +816,25 @@ ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W
         s.pnb[nx][slot] = pnb;
         s.sc[nx][slot] = lae(pb, pnb);
         l.g[nx][slot] = g;
-        l.f[nx][slot] = unokey(s.key[i]);         // the selection key's F, bit for bit
+        if constexpr (kHot) {
+          l.f[nx][slot] = __fadd_rn(lae(pb, pnb), g);   // A + G: F_end adds H_end, not H
+          // the parent's node for now; an extension that stays live steps to its child in 6'
+          hw.node[nx][slot] = x == 0 || hw.kid[a * S + x - 1] ? hw.node[cur][a] : -1;
+        } else {
+          l.f[nx][slot] = unokey(s.key[i]);         // the selection key's F, bit for bit
+        }
         ++slot;
       }
       nb = total;
       cur = nx;
       __syncthreads();
-      if (tid < nb && l.chg[tid]) l.row[cur][tid] = lm_row(lm_keys, H, order, s.pre[cur] + tid * kT, s.len[cur][tid]);
+      if (tid < nb && l.chg[tid]) {
+        l.row[cur][tid] = lm_row(lm_keys, H, order, s.pre[cur] + tid * kT, s.len[cur][tid]);
+        if constexpr (kHot) {
+          const int u = hw.node[cur][tid];
+          if (u >= 0) hw.node[cur][tid] = trie_child(tr, u, s.pre[cur][tid * kT + s.len[cur][tid] - 1]);
+        }
+      }
       __syncthreads();
     }
   }
@@ -714,9 +843,16 @@ ctc_beam_lm_kernel(const float* __restrict__ logits /*[B][48][K]*/, int K, int W
   const Beams fin{s, cur, 1};
   const int b = blockIdx.x;
   float* fend = l.g[cur ^ 1];                      // free: the other buffer's G
-  if (tid < nb)
-    fend[tid] = __fadd_rn(l.f[cur][tid],
-                          __fmul_rn(alpha, __ldg(lm_rows + static_cast<size_t>(l.row[cur][tid]) * K + blank)));
+  if (tid < nb) {
+    float fe = __fadd_rn(l.f[cur][tid],
+                         __fmul_rn(alpha, __ldg(lm_rows + static_cast<size_t>(l.row[cur][tid]) * K + blank)));
+    if constexpr (kHot) {                          // + H_end: the bonus stays only on a listed word
+      const int u = hw.node[cur][tid];
+      const float he = u >= 0 && __ldg(tr.fin + u) ? __fmul_rn(tr.gamma, static_cast<float>(s.len[cur][tid])) : 0.f;
+      if (he != 0.f) fe = __fadd_rn(fe, he);
+    }
+    fend[tid] = fe;
+  }
   __syncthreads();
   if (tid < nb) {
     const unsigned k = okey(fend[tid]);
@@ -1062,12 +1198,29 @@ int ctc_beam_lm_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_wi
                     const b2o_char_lm* lm, int* labels, float* logp, float* fused, cudaStream_t st) {
   if (B <= 0) return B2O_OK;
   const size_t bytes = smem_plan_lm(beam_width, K, nullptr, nullptr, nullptr);
-  B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(ctc_beam_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(ctc_beam_lm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            static_cast<int>(bytes)));
-  ctc_beam_lm_kernel<<<B, kThreads, bytes, st>>>(logits, K, beam_width, top_paths,
-                                                 reinterpret_cast<const unsigned long long*>(lm->keys_dev),
-                                                 lm->rows_dev, lm->n_histories, lm->order, lm->alpha, lm->beta, labels,
-                                                 logp, fused);
+  ctc_beam_lm_kernel<false><<<B, kThreads, bytes, st>>>(logits, K, beam_width, top_paths,
+                                                        reinterpret_cast<const unsigned long long*>(lm->keys_dev),
+                                                        lm->rows_dev, lm->n_histories, lm->order, lm->alpha, lm->beta,
+                                                        labels, logp, fused, Trie{});
+  B2O_LAUNCH_CHECK(ctx);
+  return B2O_OK;
+}
+
+int ctc_beam_hotword_run(b2o_ctx* ctx, const float* logits, int B, int K, int beam_width, int top_paths,
+                         const b2o_char_lm* lm, const b2o_hotwords* hw, int* labels, float* logp, float* fused,
+                         cudaStream_t st) {
+  if (B <= 0) return B2O_OK;
+  const size_t bytes = smem_plan_hot(beam_width, K, nullptr, nullptr, nullptr, nullptr);
+  B2O_CUDA_CHECK(ctx, cudaFuncSetAttribute(ctc_beam_lm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           static_cast<int>(bytes)));
+  const Trie tr{reinterpret_cast<const unsigned long long*>(hw->keys_dev), hw->child_dev, hw->final_dev, hw->n_edges,
+                hw->weight};
+  ctc_beam_lm_kernel<true><<<B, kThreads, bytes, st>>>(logits, K, beam_width, top_paths,
+                                                       reinterpret_cast<const unsigned long long*>(lm->keys_dev),
+                                                       lm->rows_dev, lm->n_histories, lm->order, lm->alpha, lm->beta,
+                                                       labels, logp, fused, tr);
   B2O_LAUNCH_CHECK(ctx);
   return B2O_OK;
 }

@@ -133,7 +133,7 @@ def _host_records(pipeline, local, per_rank, max_boxes):
 
 def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_scores=False, beam_width=None,
                       top_paths=1, lexicon=None, rotations=None, rotation_vote="word", language_model=None,
-                      pattern=None):
+                      pattern=None, hotwords=None):
     """Run ``pipeline.recognize`` on this rank's shard of ``images`` and gather to rank 0.
 
     ``images`` is the global batch (every rank passes the same list and takes its contiguous slice) or, with
@@ -154,16 +154,21 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
     device.
     ``pattern``: a ``recognition.Pattern`` or a str (compiled here) every reading must match in full (with
     ``beam_width``); uploaded once per device.
+    ``hotwords``: a ``recognition.Hotwords`` or a list of strings (compiled here) whose words the beam search favours
+    (with ``beam_width``, alone or with ``language_model``); uploaded once per device.
     ``rotations`` / ``rotation_vote``: every word is read in each listed quarter turn and the most probable reading kept
     (``recognition.check_rotations``); boxes start at the chosen turn's corner, as ``Pipeline.recognize`` returns them.
     """
     from .pipeline import check_records_decoder
-    from .recognition import check_pattern, check_rotations
+    from .recognition import check_hotwords, check_pattern, check_rotations
     if pattern is not None:
-        pattern = check_pattern(pattern, beam_width, top_paths, lexicon, pipeline.recognizer.alphabet, language_model)
-    plain = lexicon is None and language_model is None and pattern is None
+        pattern = check_pattern(pattern, beam_width, top_paths, lexicon, pipeline.recognizer.alphabet, language_model,
+                                hotwords)
+    if hotwords is not None:
+        hotwords = check_hotwords(hotwords, beam_width, top_paths, lexicon, pipeline.recognizer.alphabet)
+    plain = lexicon is None and language_model is None and pattern is None and hotwords is None
     lexicon = check_records_decoder(beam_width, top_paths, lexicon, None if plain else pipeline.recognizer.alphabet,
-                                    language_model, pattern)
+                                    language_model, pattern, hotwords)
     rotations = check_rotations(rotations, rotation_vote)
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
@@ -188,6 +193,8 @@ def recognize_sharded(pipeline, images, max_boxes=128, presharded=False, return_
         sk["language_model"] = language_model
     if pattern is not None:
         sk["pattern"] = pattern
+    if hotwords is not None:
+        sk["hotwords"] = hotwords
     if rotations is not None:
         sk["rotations"], sk["rotation_vote"] = rotations, rotation_vote
     if native:
@@ -283,18 +290,21 @@ class ShardedStream:
     ``max_boxes``: words a record holds (an image with more raises ``RecordOverflow`` on rank 0 when its batch is
     decoded) or ``"auto"`` (sized per batch by ``agree_max_boxes``).  ``return_scores=True``: words as
     ``recognize_sharded(return_scores=True)`` returns them (device records only).  ``beam_width`` / ``lexicon`` /
-    ``rotations`` / ``rotation_vote`` / ``language_model`` / ``pattern``: as ``recognize_sharded``."""
+    ``rotations`` / ``rotation_vote`` / ``language_model`` / ``pattern`` / ``hotwords``: as ``recognize_sharded``."""
 
     def __init__(self, pipeline, max_boxes=128, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                 rotations=None, rotation_vote="word", language_model=None, pattern=None):
+                 rotations=None, rotation_vote="word", language_model=None, pattern=None, hotwords=None):
         from .pipeline import check_records_decoder
-        from .recognition import check_pattern, check_rotations
+        from .recognition import check_hotwords, check_pattern, check_rotations
         if pattern is not None:
             pattern = check_pattern(pattern, beam_width, top_paths, lexicon, pipeline.recognizer.alphabet,
-                                    language_model)
-        plain = lexicon is None and language_model is None and pattern is None
+                                    language_model, hotwords)
+        if hotwords is not None:
+            hotwords = check_hotwords(hotwords, beam_width, top_paths, lexicon, pipeline.recognizer.alphabet)
+        plain = lexicon is None and language_model is None and pattern is None and hotwords is None
         lexicon = check_records_decoder(beam_width, top_paths, lexicon,
-                                        None if plain else pipeline.recognizer.alphabet, language_model, pattern)
+                                        None if plain else pipeline.recognizer.alphabet, language_model, pattern,
+                                        hotwords)
         rotations = check_rotations(rotations, rotation_vote)
         self.pipeline, self.max_boxes = pipeline, max_boxes
         self.world = dist.get_world_size() if dist.is_initialized() else 1
@@ -311,7 +321,7 @@ class ShardedStream:
         self._rk = {}
         rot = (("rotations", rotations), ("rotation_vote", rotation_vote)) if rotations is not None else ()
         for k, v in (("beam_width", beam_width), ("lexicon", lexicon), ("language_model", language_model),
-                     ("pattern", pattern)) + rot:
+                     ("pattern", pattern), ("hotwords", hotwords)) + rot:
             if v is not None:
                 self._sk[k] = v
                 self._rk.setdefault("recognition_kwargs", {})[k] = v

@@ -6,10 +6,10 @@ from . import detection, recognition, tools
 
 
 def check_records_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=recognition.DEFAULT_ALPHABET,
-                          language_model=None, pattern=None):
+                          language_model=None, pattern=None, hotwords=None):
     """``recognition.check_decoder`` for the records path, whose fixed-size records carry one reading per word; returns
     the compiled lexicon or None."""
-    lexicon = recognition.check_decoder(beam_width, top_paths, lexicon, alphabet, language_model, pattern)
+    lexicon = recognition.check_decoder(beam_width, top_paths, lexicon, alphabet, language_model, pattern, hotwords)
     if top_paths != 1:
         raise ValueError("records carry the best path only: top_paths must be 1")
     return lexicon
@@ -312,7 +312,9 @@ class Pipeline:
         shapes (``recognition.check_decoder``).  Or ``language_model`` (a ``recognition.CharLM``) with ``beam_width``:
         the beam search ranked by that character model, confidences still from the acoustic score.  Or ``pattern`` (a
         ``recognition.Pattern`` or a str) with ``beam_width``: only readings that match that regular expression in full,
-        a word without one reading "" with confidence 0.  With any of these decoders, ``rotations`` / ``rotation_vote``
+        a word without one reading "" with confidence 0.  Or ``hotwords`` (a ``recognition.Hotwords`` or a list of
+        strings) with ``beam_width``, alone or with ``language_model``: listed words win where the image is ambiguous,
+        everything else reads as without them.  With any of these decoders, ``rotations`` / ``rotation_vote``
         (``recognition.check_rotations``) read every word in each listed quarter turn and keep the most probable
         reading, per word or per image; every returned box then starts at the chosen turn's corner, so box[0] is the
         text's own top-left corner (the same corners, still clockwise).  Injected recognizers get
@@ -377,15 +379,17 @@ class Pipeline:
         if recognition_kwargs is None:
             recognition_kwargs = {}
         if self._native():
-            beam = {k: recognition_kwargs[k] for k in ("beam_width", "top_paths", "lexicon", "language_model", "pattern")
-                    if k in recognition_kwargs}
-            lexicon, pattern = self.recognizer._decoder(beam.get("beam_width"), beam.get("top_paths", 1),
-                                                        beam.get("lexicon"), beam.get("language_model"),
-                                                        beam.get("pattern"))
+            beam = {k: recognition_kwargs[k] for k in ("beam_width", "top_paths", "lexicon", "language_model", "pattern",
+                                                       "hotwords") if k in recognition_kwargs}
+            lexicon, pattern, hotwords = self.recognizer._decoder(beam.get("beam_width"), beam.get("top_paths", 1),
+                                                                  beam.get("lexicon"), beam.get("language_model"),
+                                                                  beam.get("pattern"), beam.get("hotwords"))
             if lexicon is not None:
                 beam["lexicon"] = lexicon                 # compiled once for every sub-batch
             if pattern is not None:
                 beam["pattern"] = pattern
+            if hotwords is not None:
+                beam["hotwords"] = hotwords
             vote = recognition_kwargs.get("rotation_vote", "word")
             turns = recognition.check_rotations(recognition_kwargs.get("rotations"), vote)
             if turns is not None:
@@ -441,7 +445,7 @@ class Pipeline:
 
     def recognize_records(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
                           top_paths=1, lexicon=None, rotations=None, rotation_vote="word", language_model=None,
-                          pattern=None):
+                          pattern=None, hotwords=None):
         """``recognize`` without the trip to the host: returns the results as a CUDA float32 tensor of fixed-size
         per-image records, ``(rows, b2o_record_floats(rec_boxes))`` = [count | rec_boxes x (4,2) boxes in source
         pixels | rec_boxes x 48 int8 labels] (``distributed.unpack_blocks`` decodes it; rows beyond ``len(images)``
@@ -454,26 +458,30 @@ class Pipeline:
         log-probability in the scored layout.  ``language_model`` (a ``recognition.CharLM``, with ``beam_width``): the
         beam search ranked by that model, the acoustic score in the scored layout.  ``pattern`` (a
         ``recognition.Pattern`` or a str, with ``beam_width``): the best reading that matches it in full, a word without
-        one carrying no labels and -inf in the scored layout.  ``rotations`` / ``rotation_vote``: every word is read in each listed
+        one carrying no labels and -inf in the scored layout.  ``hotwords`` (a ``recognition.Hotwords`` or a list of
+        strings, with ``beam_width``): the beam search with a bonus for the listed words, the acoustic score in the
+        scored layout.  ``rotations`` / ``rotation_vote``: every word is read in each listed
         quarter turn and the most probable reading kept (``recognition.check_rotations``); the records' boxes start at
         the chosen turn's corner, as ``recognize`` returns them."""
         return self.records_end(self.records_begin(images, rows, rec_boxes, detection_kwargs, scores, beam_width,
                                                    top_paths, lexicon, rotations, rotation_vote, language_model,
-                                                   pattern))
+                                                   pattern, hotwords))
 
     def records_begin(self, images, rows=None, rec_boxes=128, detection_kwargs=None, scores=False, beam_width=None,
                       top_paths=1, lexicon=None, rotations=None, rotation_vote="word", language_model=None,
-                      pattern=None):
+                      pattern=None, hotwords=None):
         """First half of ``recognize_records``: queues resize/pad, CRAFT and getBoxes and returns at once (no
         synchronisation), so the caller can use the host while the GPU works (``distributed.ShardedStream`` decodes the
         previous batch's words here).  Pass the returned state to ``records_end``."""
         if pattern is not None:
             pattern = recognition.check_pattern(pattern, beam_width, top_paths, lexicon, self.recognizer.alphabet,
-                                                language_model)
-        plain = lexicon is None and language_model is None and pattern is None
+                                                language_model, hotwords)
+        if hotwords is not None:
+            hotwords = recognition.check_hotwords(hotwords, beam_width, top_paths, lexicon, self.recognizer.alphabet)
+        plain = lexicon is None and language_model is None and pattern is None and hotwords is None
         lexicon = check_records_decoder(beam_width, top_paths, lexicon,
                                         recognition.DEFAULT_ALPHABET if plain else self.recognizer.alphabet,
-                                        language_model, pattern)
+                                        language_model, pattern, hotwords)
         turns = recognition.check_rotations(rotations, rotation_vote)
         tile_size = detection.check_tiles((detection_kwargs or {}).get("tile_size"))
         assert self._native(), "recognize_records needs this package's Detector and Recognizer"
@@ -491,7 +499,7 @@ class Pipeline:
         self.last_stats = {"h2d_bytes": 0, "d2h_bytes": 0}
         state = {"n": n, "rows": rows, "rec_boxes": rec_boxes, "scores": bool(scores), "beam_width": beam_width,
                  "lexicon": lexicon, "rotations": turns, "rotation_vote": rotation_vote,
-                 "language_model": language_model, "pattern": pattern}
+                 "language_model": language_model, "pattern": pattern, "hotwords": hotwords}
         if n:
             plans = self._plans(images)
             state["st"] = self._stage_detect(images, (max(p[1] for p in plans), max(p[2] for p in plans)), thresholds,
@@ -532,7 +540,7 @@ class Pipeline:
                                                  image_index=bst["image_index"], with_scores=scored,
                                                  beam_width=state.get("beam_width"), lexicon=state.get("lexicon"),
                                                  language_model=state.get("language_model"),
-                                                 pattern=state.get("pattern"),
+                                                 pattern=state.get("pattern"), hotwords=state.get("hotwords"),
                                                  rotations=state.get("rotations"),
                                                  rotation_vote=state.get("rotation_vote", "word"))
         if state.get("rotations") is not None:           # the turns are in the rolled boxes the records carry

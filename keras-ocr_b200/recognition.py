@@ -464,6 +464,128 @@ class CharLM:
         return _lib.CharLMDesc(self.order, keys.shape[0], keys.data_ptr(), rows.data_ptr(), self.alpha, self.beta)
 
 
+class Hotwords:
+    """Words to boost without requiring them, fused into the CTC prefix beam search (``b2o_crnn_forward_beam_hotword``;
+    DESIGN.md section 1, "Hotwords").  A prefix is live when it is a prefix of a listed word (the empty prefix is).
+    During the search a prefix a earns H(a) = ``weight`` * |a| while it is live and nothing once it leaves the list's
+    trie; a returned reading keeps weight * |a| only if it is a listed word.  Readings rank by the acoustic score plus
+    the language model's (if any) plus that bonus; the confidences stay acoustic.  Text outside the list reads as it
+    does without hotwords, except where the bonus decides an ambiguous image.
+
+    Entries are non-empty strings over ``alphabet`` of at most 48 characters, distinct, at most 2^20 of them and 2^24
+    characters in all; the alphabet has at most 126 characters (the language-model kernel's class bound) and
+    ``weight`` is a number >= 0, finite in float32.  Anything else raises ``ValueError`` naming the first offending entry
+    or value.  An empty list is valid and changes nothing.
+
+    The trie is compiled once on the host (``host_tables``) and uploaded lazily, once per CUDA device, so one object
+    serves every rank of a sharded run.  A plain list or tuple of strings is accepted wherever a ``Hotwords`` is and is
+    compiled for that call with the default weight."""
+
+    WEIGHT = 1.5       # picked by scripts/bench_hotwords.py's sweep on its tuning pages (DESIGN.md section 5)
+
+    def __init__(self, words, weight=WEIGHT, alphabet=DEFAULT_ALPHABET):
+        if isinstance(words, str) or not isinstance(words, (list, tuple)):
+            raise ValueError("hotwords are a list or tuple of strings")
+        if len(alphabet) > _lib.MAX_LM_CLASSES - 1:
+            raise ValueError(f"hotwords take an alphabet of at most {_lib.MAX_LM_CLASSES - 1} characters, "
+                             f"got {len(alphabet)}")
+        if len(words) > _lib.MAX_LEXICON_WORDS:
+            raise ValueError(f"there are {len(words)} hotwords; at most {_lib.MAX_LEXICON_WORDS} are supported")
+        index = {ch: i for i, ch in enumerate(alphabet)}
+        seen = set()
+        total = 0
+        for i, w in enumerate(words):
+            _check_word(i, w, index, "hotword")
+            if w in seen:
+                raise ValueError(f"hotword {i} ({w!r}) is a duplicate")
+            seen.add(w)
+            total += len(w)
+            if total > _lib.MAX_LEXICON_LABELS:
+                raise ValueError(f"hotword {i} ({w!r}) takes the list past {_lib.MAX_LEXICON_LABELS} characters in all")
+        self._check_weight(weight)
+        self.words, self.alphabet, self.weight = tuple(words), alphabet, float(weight)
+        self._tables = {"host": compile_trie(self.words, index)}   # shared by weighted copies, with the uploads
+
+    @staticmethod
+    def _check_weight(weight):
+        ok = not isinstance(weight, (bool, np.bool_)) and isinstance(weight, (int, float, np.integer, np.floating))
+        if ok:
+            with np.errstate(over="ignore"):
+                ok = math.isfinite(float(np.float32(weight))) and float(weight) >= 0
+        if not ok:
+            raise ValueError(f"weight must be a number >= 0, finite in float32, got {weight!r}")
+
+    def __len__(self):
+        return len(self.words)
+
+    def __repr__(self):
+        return f"Hotwords({len(self.words)} words, weight={self.weight})"
+
+    def weighted(self, weight=WEIGHT):
+        """A copy with weight ``weight`` that shares this list's trie and device uploads."""
+        self._check_weight(weight)
+        other = object.__new__(Hotwords)
+        other.__dict__.update(self.__dict__)
+        other.weight = float(weight)
+        return other
+
+    def host_tables(self):
+        """The trie (``compile_trie``): (keys (E,) uint64, child (E,) int32, final (N,) uint8), E = N - 1."""
+        return self._tables["host"]
+
+    def device_arrays(self, device):
+        """(keys (E,) int64 -- the uint64 keys' bits --, child (E,) int32, final (N,) uint8) CUDA tensors on
+        ``device``, uploaded on first use."""
+        device = torch.device(device)
+        if device not in self._tables:
+            keys, child, final = self.host_tables()
+            self._tables[device] = tuple(torch.from_numpy(a).to(device) for a in (keys.view(np.int64), child, final))
+        return self._tables[device]
+
+    def descriptor(self, device):
+        """The ``b2o_hotwords`` of this list on ``device`` (``_lib.HotwordsDesc``)."""
+        keys, child, final = self.device_arrays(device)
+        ptr = lambda t: t.data_ptr() if t.numel() else None      # noqa: E731
+        return _lib.HotwordsDesc(final.numel(), keys.numel(), ptr(keys), ptr(child), final.data_ptr(), self.weight)
+
+
+def compile_trie(words, index):
+    """The trie of checked, distinct ``words`` (``index``: character -> label), deterministic: nodes numbered
+    breadth-first by (depth, parent, label), the root 0 the empty prefix.  Returns (keys (E,) uint64 ascending, key =
+    (parent << 8) | label, child (E,) int32 the child of each edge -- so a node's children are contiguous --, final
+    (N,) uint8, 1 where the node's prefix is a listed word), E = N - 1 edges."""
+    nested = [{}]                                 # build ids -> {label: build id}
+    ends = [False]
+    for w in words:
+        u = 0
+        for ch in w:
+            c = index[ch]
+            v = nested[u].get(c)
+            if v is None:
+                v = nested[u][c] = len(nested)
+                nested.append({})
+                ends.append(False)
+            u = v
+        ends[u] = True
+    n = len(nested)
+    new = np.zeros(n, np.int64)                   # build id -> node
+    parent = np.zeros(n, np.int64)                # node -> its parent and label
+    label = np.zeros(n, np.int64)
+    order = [0]                                   # build ids in node order; grows while it is walked
+    for pos in range(n):
+        u = order[pos]
+        for c in sorted(nested[u]):
+            v = nested[u][c]
+            new[v], parent[len(order)], label[len(order)] = len(order), pos, c
+            order.append(v)
+    final = np.zeros(n, np.uint8)
+    final[new[np.flatnonzero(np.asarray(ends))]] = 1
+    # parents are non-decreasing in node order and a parent's children follow in label order: the keys ascend, and
+    # the child of edge j is node j + 1
+    keys = (parent[1:].astype(np.uint64) << np.uint64(8)) | label[1:].astype(np.uint64)
+    return keys, np.arange(1, n, dtype=np.int32), final
+
+
 class Pattern:
     """A regular expression every reading must match in full, enforced inside the CTC prefix beam search
     (``b2o_crnn_forward_beam_pattern``; DESIGN.md section 1, "Patterns"): a reading is returned only if
@@ -521,10 +643,34 @@ class Pattern:
         return _lib.PatternDesc(self.n_states, self.start, trans.data_ptr(), dist.data_ptr())
 
 
-def check_pattern(pattern, beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET, language_model=None):
+def check_hotwords(hotwords, beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET, pattern=None):
+    """Validates a hotword choice before anything is launched (``ValueError`` otherwise) and returns the ``Hotwords`` to
+    decode with, or None for ``hotwords=None``.  A ``Hotwords`` over ``alphabet`` or a list / tuple of strings
+    (compiled here with the default weight) boosts its words in the beam search: it needs ``beam_width`` and does not
+    combine with a lexicon or a pattern; it combines with a language model."""
+    if hotwords is None:
+        return None
+    if not isinstance(hotwords, (Hotwords, list, tuple)):
+        raise ValueError(f"hotwords must be a Hotwords or a list of strings, got {type(hotwords).__name__}")
+    if beam_width is None:
+        raise ValueError("hotwords need beam search: pass beam_width")
+    if lexicon is not None:
+        raise ValueError("lexicon and hotwords are mutually exclusive")
+    if pattern is not None:
+        raise ValueError("pattern and hotwords do not combine in one search")
+    check_beam(beam_width, top_paths)
+    if not isinstance(hotwords, Hotwords):
+        return Hotwords(hotwords, alphabet=alphabet)
+    if hotwords.alphabet != alphabet:
+        raise ValueError("the hotwords were compiled for another alphabet than the recognizer's")
+    return hotwords
+
+
+def check_pattern(pattern, beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET, language_model=None,
+                  hotwords=None):
     """Validates a pattern choice before anything is launched (``ValueError`` otherwise) and returns the ``Pattern`` to
     decode with, or None for ``pattern=None``.  A ``Pattern`` over ``alphabet`` or a ``str`` (compiled here) constrains
-    the beam search: it needs ``beam_width`` and does not combine with a lexicon or a language model."""
+    the beam search: it needs ``beam_width`` and does not combine with a lexicon, a language model or hotwords."""
     if pattern is None:
         return None
     if not isinstance(pattern, (Pattern, str)):
@@ -535,6 +681,8 @@ def check_pattern(pattern, beam_width=None, top_paths=1, lexicon=None, alphabet=
         raise ValueError("lexicon and pattern are mutually exclusive")
     if language_model is not None:
         raise ValueError("language_model and pattern do not combine in one search")
+    if hotwords is not None:
+        raise ValueError("pattern and hotwords do not combine in one search")
     check_beam(beam_width, top_paths)
     if isinstance(pattern, str):
         return Pattern(pattern, alphabet)
@@ -544,17 +692,22 @@ def check_pattern(pattern, beam_width=None, top_paths=1, lexicon=None, alphabet=
 
 
 def check_decoder(beam_width=None, top_paths=1, lexicon=None, alphabet=DEFAULT_ALPHABET, language_model=None,
-                  pattern=None):
+                  pattern=None, hotwords=None):
     """Validates a decoder choice before anything is launched (``ValueError`` otherwise) and returns the ``Lexicon`` to
     decode with, or None.  Without a lexicon this is ``check_beam``.  With one (a ``Lexicon`` over ``alphabet``, or a
     list / tuple of strings, compiled here): ``beam_width`` must be None and 1 <= ``top_paths`` <= 128.
     ``language_model`` (a ``CharLM`` over ``alphabet``) ranks the beam search by that model
     (``b2o_crnn_forward_beam_lm``): it needs ``beam_width`` and does not combine with a lexicon.
     ``pattern`` (a ``Pattern`` over ``alphabet`` or a str): the rules of ``check_pattern``, which returns the compiled
-    pattern."""
+    pattern.  ``hotwords`` (a ``Hotwords`` over ``alphabet`` or a list of strings): the rules of ``check_hotwords``,
+    which returns the compiled list; it combines with ``language_model``."""
     if pattern is not None:
-        check_pattern(pattern, beam_width, top_paths, lexicon, alphabet, language_model)
+        check_pattern(pattern, beam_width, top_paths, lexicon, alphabet, language_model, hotwords)
         return None
+    if hotwords is not None:
+        check_hotwords(hotwords, beam_width, top_paths, lexicon, alphabet)
+        if language_model is None:
+            return None
     if language_model is not None:
         if not isinstance(language_model, CharLM):
             raise ValueError(f"language_model must be a CharLM, got {type(language_model).__name__}")
@@ -924,17 +1077,22 @@ class Recognizer:
                                 None if logp is None else logp.data_ptr(), stream)
         return out, logp
 
-    def _decoder(self, beam_width, top_paths, lexicon, language_model=None, pattern=None):
+    def _decoder(self, beam_width, top_paths, lexicon, language_model=None, pattern=None, hotwords=None):
         """``check_decoder`` for this recognizer's alphabet: (the compiled lexicon or None, the compiled pattern or
-        None)."""
+        None, the compiled hotwords or None)."""
         if pattern is not None:
-            return None, check_pattern(pattern, beam_width, top_paths, lexicon, self.alphabet, language_model)
+            return None, check_pattern(pattern, beam_width, top_paths, lexicon, self.alphabet, language_model,
+                                       hotwords), None
+        if hotwords is not None:
+            hotwords = check_hotwords(hotwords, beam_width, top_paths, lexicon, self.alphabet)
+            check_decoder(beam_width, top_paths, None, self.alphabet, language_model)
+            return None, None, hotwords
         plain = lexicon is None and language_model is None
         return check_decoder(beam_width, top_paths, lexicon, DEFAULT_ALPHABET if plain else self.alphabet,
-                             language_model), None
+                             language_model), None, None
 
     def predict_device(self, crnn_in, with_scores=False, beam_width=None, top_paths=1, lexicon=None,
-                       language_model=None, pattern=None, char_scores=None):
+                       language_model=None, pattern=None, char_scores=None, hotwords=None):
         """CRNN + greedy CTC.  crnn_in: (B,200,31) fp16 -> labels (B,48) int32 (-1 padded).  ``with_scores``: returns
         (labels, logp) with logp (B,) float32 the greedy path's log-probability (``b2o_crnn_forward_scored``).
         ``beam_width``: CTC prefix beam search instead (``b2o_crnn_forward_beam``, see ``check_beam``), logp = the beam
@@ -944,18 +1102,20 @@ class Recognizer:
         ``language_model`` (a ``CharLM``, with ``beam_width``): the beam search ranked by that model
         (``b2o_crnn_forward_beam_lm``); logp stays the acoustic beam score of each reading.  ``pattern`` (a
         ``Pattern`` or a str, with ``beam_width``): only readings that match it in full (``b2o_crnn_forward_beam_pattern``),
-        logp their beam scores; slots past a crop's matching readings are -1 with logp -inf.
+        logp their beam scores; slots past a crop's matching readings are -1 with logp -inf.  ``hotwords`` (a
+        ``Hotwords`` or a list of strings, with ``beam_width``, with or without ``language_model``): the beam search
+        with a bonus for the listed words (``b2o_crnn_forward_beam_hotword``); logp stays the acoustic beam score.
         ``char_scores`` = A (``check_char_scores``): the result also ends with every reading's character confidences
         (B,48) float32 and, with A > 0, its alternatives' labels (B,48,A) int32 and posteriors (B,48,A) float32
         (``b2o_crnn_char_scores``); (B,P,48) / (B,P,48,A) with ``top_paths = P > 1``."""
-        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
+        lexicon, pattern, hotwords = self._decoder(beam_width, top_paths, lexicon, language_model, pattern, hotwords)
         b = crnn_in.shape[0]
         lead = (b,) if top_paths == 1 else (b, top_paths)
         labels = torch.empty(lead + (STEPS,), dtype=torch.int32, device=self.device)
         logp = torch.empty(lead, dtype=torch.float32, device=self.device) if with_scores else None
         scores = None if char_scores is None else self._score_buffers(lead, char_scores)
         self._forward(crnn_in, labels, logp, beam_width, top_paths, lexicon, language_model=language_model,
-                      pattern=pattern, char_scores=scores)
+                      pattern=pattern, char_scores=scores, hotwords=hotwords)
         if scores is not None:
             return ((labels, logp) if with_scores else (labels,)) + tuple(t for t in scores if t is not None)
         return (labels, logp) if with_scores else labels
@@ -970,10 +1130,11 @@ class Recognizer:
                 torch.empty(lead + (STEPS, alternatives), dtype=torch.float32, device=self.device))
 
     def _forward(self, crnn_in, labels, logp, beam_width, top_paths, lexicon, spans=None, theta=None,
-                 language_model=None, fused=None, pattern=None, char_scores=None):
+                 language_model=None, fused=None, pattern=None, char_scores=None, hotwords=None):
         """The CRNN and the decoder of ``predict_device`` into caller-allocated ``labels`` / ``logp`` (None: greedy
         without scores, or scores not written); ``lexicon`` is already compiled.  With ``language_model``, ``fused``
-        (B,P) float32 or None receives every reading's F_end.  ``pattern`` is already compiled.  ``spans`` (B,P,48,2) int32: also the
+        (B,P) float32 or None receives every reading's F_end, and so it does with ``hotwords`` (already compiled).
+        ``pattern`` is already compiled.  ``spans`` (B,P,48,2) int32: also the
         characters' emission spans of every reading (``b2o_crnn_align``) and, with an STN, its ``theta`` (B,6) float32;
         the greedy forward then keeps its logits (``b2o_crnn_forward_logits``).  ``char_scores``: (conf, alternative
         labels or None, posteriors or None) of ``_score_buffers``, filled by ``b2o_crnn_char_scores`` after the decoder
@@ -992,6 +1153,12 @@ class Recognizer:
             offsets, lex_labels = lexicon.device_arrays(self.device)
             self.ctx.crnn_forward_lexicon(crnn_in.data_ptr(), b, offsets.data_ptr(), lex_labels.data_ptr(), len(lexicon),
                                           int(top_paths), labels.data_ptr(), logp_ptr, ws.data_ptr(), nbytes, stream)
+        elif hotwords is not None:
+            self.ctx.crnn_forward_beam_hotword(crnn_in.data_ptr(), b, int(beam_width), int(top_paths),
+                                               None if language_model is None else language_model.descriptor(self.device),
+                                               hotwords.descriptor(self.device), labels.data_ptr(), logp_ptr,
+                                               fused.data_ptr() if fused is not None else None, ws.data_ptr(), nbytes,
+                                               stream)
         elif language_model is not None:
             self.ctx.crnn_forward_beam_lm(crnn_in.data_ptr(), b, int(beam_width), int(top_paths),
                                           language_model.descriptor(self.device), labels.data_ptr(), logp_ptr,
@@ -1023,7 +1190,7 @@ class Recognizer:
         self._last_ws = (ws, b) if self.keep_workspace else None
 
     def _predict_aligned(self, crnn_in, beam_width, top_paths, lexicon, language_model=None, pattern=None,
-                         char_scores=None):
+                         char_scores=None, hotwords=None):
         """``predict_device(with_scores=True)`` plus every reading's spans: (labels (B,P,48), logp (B,P), spans
         (B,P,48,2) int32, theta (B,6) float32 or None without an STN), followed by the ``_score_buffers`` of
         ``char_scores`` = A when it is given."""
@@ -1034,7 +1201,7 @@ class Recognizer:
         theta = torch.empty((b, 6), dtype=torch.float32, device=self.device) if self.stn else None
         scores = None if char_scores is None else self._score_buffers((b, p), char_scores)
         self._forward(crnn_in, labels, logp, beam_width, p, lexicon, spans, theta, language_model, pattern=pattern,
-                      char_scores=scores)
+                      char_scores=scores, hotwords=hotwords)
         return (labels, logp, spans, theta) + (() if scores is None else (scores,))
 
     def char_cells_device(self, spans, theta, boxes=None, turns=None):
@@ -1057,7 +1224,7 @@ class Recognizer:
 
     def recognize_crops(self, crops, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
                         return_char_boxes=False, language_model=None, pattern=None, return_char_scores=False,
-                        char_alternatives=0):
+                        char_alternatives=0, hotwords=None):
         """crops: (B,31,200) uint8 -- (B,31,200,3) for a color recognizer -- i.e. what tools.warpBox returns -> list[str].
         ``return_scores=True``: a list of (text, confidence) instead, see ``confidences``.  ``beam_width``: beam search
         decoding (``check_beam``); with ``top_paths = P > 1`` each text is a list of P strings and each confidence a
@@ -1065,7 +1232,9 @@ class Recognizer:
         (``check_decoder``), in the same shapes; a confidence is exp(the entry's CTC log-probability), clipped to 1.
         ``language_model`` (a ``CharLM``, with ``beam_width``): the beam search ranked by that character model; the
         confidences stay exp(the acoustic beam score).  ``pattern`` (a ``Pattern`` or a str, with ``beam_width``): only
-        readings that match it in full; a word with no matching reading reads "" with confidence 0.
+        readings that match it in full; a word with no matching reading reads "" with confidence 0.  ``hotwords`` (a
+        ``Hotwords`` or a list of strings, with ``beam_width``, alone or with ``language_model``): listed words win
+        where the image is ambiguous, everything else reads as without them; the confidences stay acoustic.
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells (``b2o_char_cells``), an
         (n,4,2) float32 array for a text of n characters (a list of P arrays with ``top_paths = P > 1``), in the crop's
         200 x 31 frame: (text, cells) or (text, confidence, cells).
@@ -1073,7 +1242,7 @@ class Recognizer:
         ``char_scores_host``), after the cells when both are asked for: an (n,) float32 array of the characters'
         confidences, or with ``char_alternatives = A > 0`` that array and n lists of A (character, posterior) pairs;
         a list of P of these with ``top_paths = P > 1``.  They are acoustic: they do not depend on the decoder."""
-        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
+        lexicon, pattern, hotwords = self._decoder(beam_width, top_paths, lexicon, language_model, pattern, hotwords)
         char_scores = check_char_scores(return_char_scores, char_alternatives)
         t = crops if isinstance(crops, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(crops))
         t = t.to(self.device).contiguous()
@@ -1085,7 +1254,7 @@ class Recognizer:
         self.ctx.crops_to_input(t.data_ptr(), b, crnn_in.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream,
                                 color=self.color)
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
-                "pattern": pattern}
+                "pattern": pattern, "hotwords": hotwords}
         if return_char_boxes:
             labels, logp, spans, theta, *scores = self._predict_aligned(crnn_in, char_scores=char_scores, **beam)
             return self._host_words(labels, logp, top_paths, return_scores, self.char_cells_device(spans, theta),
@@ -1116,28 +1285,29 @@ class Recognizer:
             cols.append(char_scores_host(host[0], texts, self.alphabet, *host[1:]))
         return list(zip(*cols))
 
-    def recognize(self, image, beam_width=None, top_paths=1, lexicon=None, language_model=None, pattern=None):
+    def recognize(self, image, beam_width=None, top_paths=1, lexicon=None, language_model=None, pattern=None,
+                  hotwords=None):
         """Recognize text from a single pre-cropped image (reference recognition.py:467-489): fit to
         200x31 with zero fill (host, as upstream), gray conversion, then the CUDA CRNN.  ``beam_width`` / ``top_paths`` /
-        ``lexicon`` / ``language_model`` / ``pattern``: as ``recognize_crops``."""
+        ``lexicon`` / ``language_model`` / ``pattern`` / ``hotwords``: as ``recognize_crops``."""
         import cv2
 
-        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
+        lexicon, pattern, hotwords = self._decoder(beam_width, top_paths, lexicon, language_model, pattern, hotwords)
         image = tools.read_and_fit(filepath_or_array=image, width=TARGET_WIDTH, height=TARGET_HEIGHT, cval=0)
         if not self.color and image.ndim == 3 and image.shape[-1] == 3:      # recognition.py:481-483
             image = cv2.cvtColor(image, code=cv2.COLOR_RGB2GRAY)
         return self.recognize_crops(np.ascontiguousarray(image.reshape((1, TARGET_HEIGHT, TARGET_WIDTH) + ((3,) if self.color else ()))),
                                     beam_width=beam_width, top_paths=top_paths, lexicon=lexicon,
-                                    language_model=language_model, pattern=pattern)[0]
+                                    language_model=language_model, pattern=pattern, hotwords=hotwords)[0]
 
     def recognize_from_boxes_device(self, images_t, boxes, counts, gray=None, flat=None, image_index=None,
                                     with_scores=False, beam_width=None, top_paths=1, lexicon=None, rotations=None,
                                     rotation_vote="word", char_boxes=False, polys=None, points=None, max_windows=1,
                                     windows=None, language_model=None, pattern=None, char_scores=False,
-                                    char_alternatives=0):
+                                    char_alternatives=0, hotwords=None):
         """images_t (N,H,W,3) u8 CUDA; boxes (N,M,4,2) f32 CUDA; counts host ndarray -> labels (B,48) i32 CUDA
         (``with_scores``: (labels, logp (B,) f32 CUDA); ``beam_width`` / ``top_paths`` / ``lexicon`` /
-        ``language_model`` / ``pattern``: see ``predict_device``).
+        ``language_model`` / ``pattern`` / ``hotwords``: see ``predict_device``).
 
         ``rotations`` / ``rotation_vote`` (``check_rotations``): every box is cut and decoded once per listed turn, one
         turn after another (the CRNN workspace stays that of B crops), and ``b2o_select_rotation`` keeps one reading per
@@ -1170,7 +1340,7 @@ class Recognizer:
         ``b2o_window_counts`` gives them (``Pipeline.recognize`` reads them back with the box counts; ``ValueError`` for
         another shape or a count outside [1, max_windows]); None: computed here and read back, one more
         synchronisation."""
-        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
+        lexicon, pattern, hotwords = self._decoder(beam_width, top_paths, lexicon, language_model, pattern, hotwords)
         turns = check_rotations(rotations, rotation_vote)
         scores = check_char_scores(char_scores, char_alternatives)
         max_windows = check_windows(max_windows, beam_width, lexicon, turns, char_boxes, polys is not None,
@@ -1209,42 +1379,46 @@ class Recognizer:
             crnn_in, _ = self.warp_polys_device(gray, polys[:total], points[:total], image_index[:total])
             return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
                                        lexicon=lexicon, language_model=language_model, pattern=pattern,
-                                       char_scores=scores)
+                                       char_scores=scores, hotwords=hotwords)
         if turns is not None:
             return self._recognize_turns(gray, flat[:total], image_index[:total], len(counts), boxes, turns,
                                          rotation_vote, with_scores, beam_width, top_paths, lexicon, char_boxes,
-                                         language_model, pattern, scores)
+                                         language_model, pattern, scores, hotwords)
         if char_boxes:
             labels, logp, spans, cells, *extra = self._read_cells(gray, flat[:total], image_index[:total], beam_width,
-                                                                  top_paths, lexicon, language_model, pattern, scores)
+                                                                  top_paths, lexicon, language_model, pattern, scores,
+                                                                  hotwords)
             return ((labels, logp, spans, cells) if with_scores else (labels, spans, cells)) + tuple(extra)
         crnn_in, _ = self.warp_device(gray, flat[:total], image_index[:total])
         return self.predict_device(crnn_in, with_scores=with_scores, beam_width=beam_width, top_paths=top_paths,
-                                   lexicon=lexicon, language_model=language_model, pattern=pattern, char_scores=scores)
+                                   lexicon=lexicon, language_model=language_model, pattern=pattern, char_scores=scores,
+                                   hotwords=hotwords)
 
     def _read_cells(self, gray, flat, image_index, beam_width, top_paths, lexicon, language_model=None, pattern=None,
-                    char_scores=None):
+                    char_scores=None, hotwords=None):
         """Warp + CRNN + decoder + alignment + cells of one pass: (labels, logp, spans, cells) in the shapes of
         ``recognize_from_boxes_device``, followed by the character scores with ``char_scores`` = A."""
         crnn_in, _ = self.warp_device(gray, flat, image_index)
         labels, logp, spans, theta, *scores = self._predict_aligned(crnn_in, beam_width, top_paths, lexicon,
-                                                                    language_model, pattern, char_scores)
+                                                                    language_model, pattern, char_scores, hotwords)
         cells = self.char_cells_device(spans, theta, flat)
         out = (labels, logp, spans, cells) + (tuple(t for t in scores[0] if t is not None) if scores else ())
         return tuple(t[:, 0] for t in out) if top_paths == 1 else out
 
     def _recognize_turns(self, gray, flat, image_index, n_images, table, turns, vote, with_scores, beam_width,
-                         top_paths, lexicon, char_boxes=False, language_model=None, pattern=None, char_scores=None):
+                         top_paths, lexicon, char_boxes=False, language_model=None, pattern=None, char_scores=None,
+                         hotwords=None):
         """Warp + CRNN + decoder for each turn into its slot of one (R,B,P,48) / (R,B,P) stack, then
         ``b2o_select_rotation``, which also rolls ``flat`` and ``table`` (None: no table) in place.  ``char_boxes``: each
         turn's spans and theta are stacked alike, and the chosen turn's cells are built from the boxes as they were cut.
-        With ``language_model`` the vote compares the readings' F_end, and the chosen turn's acoustic logp is gathered
-        on the device.  ``char_scores`` = A: each turn's character scores are stacked alike and the chosen turn's
+        With ``language_model`` or ``hotwords`` the vote compares the readings' F_end, and the chosen turn's acoustic
+        logp is gathered on the device.  ``char_scores`` = A: each turn's character scores are stacked alike and the chosen turn's
         gathered; they end the result."""
         b, p, r = flat.shape[0], int(top_paths), len(turns)
         labels_all = torch.empty((r, b, p, STEPS), dtype=torch.int32, device=self.device)
         logp_all = torch.empty((r, b, p), dtype=torch.float32, device=self.device)
-        fused_all = torch.empty((r, b, p), dtype=torch.float32, device=self.device) if language_model is not None else None
+        fused = language_model is not None or hotwords is not None
+        fused_all = torch.empty((r, b, p), dtype=torch.float32, device=self.device) if fused else None
         spans_all = theta_all = cut = None
         if char_boxes:
             spans_all = torch.empty((r, b, p, STEPS, 2), dtype=torch.int32, device=self.device)
@@ -1256,7 +1430,8 @@ class Recognizer:
             self._forward(crnn_in, labels_all[j], logp_all[j], beam_width, p, lexicon,
                           None if spans_all is None else spans_all[j], None if theta_all is None else theta_all[j],
                           language_model, None if fused_all is None else fused_all[j], pattern,
-                          None if scores_all is None else tuple(None if t is None else t[j] for t in scores_all))
+                          None if scores_all is None else tuple(None if t is None else t[j] for t in scores_all),
+                          hotwords)
         labels = torch.empty((b, p, STEPS), dtype=torch.int32, device=self.device)
         logp = torch.empty((b, p), dtype=torch.float32, device=self.device)
         chosen = torch.empty((b,), dtype=torch.int32, device=self.device)
@@ -1287,10 +1462,10 @@ class Recognizer:
     def recognize_from_boxes(self, images, box_groups, return_scores=False, beam_width=None, top_paths=1, lexicon=None,
                              rotations=None, rotation_vote="word", return_char_boxes=False, max_windows=1,
                              language_model=None, pattern=None, return_char_scores=False, char_alternatives=0,
-                             **kwargs) -> typing.List[typing.List[str]]:
+                             hotwords=None, **kwargs) -> typing.List[typing.List[str]]:
         """Same contract as reference recognition.py:491-537.  ``return_scores=True``: every word is a
         (text, confidence) pair instead, see ``confidences``.  ``beam_width`` / ``top_paths`` / ``lexicon`` /
-        ``language_model`` / ``pattern``: as ``recognize_crops``; with rotations the vote compares the language model's fused scores.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
+        ``language_model`` / ``pattern`` / ``hotwords``: as ``recognize_crops``; with rotations the vote compares the fused scores F_end of a language model or hotwords.  ``rotations`` / ``rotation_vote``: every box is read in each listed quarter turn and the
         most probable reading kept, per word or per image (one box group), see ``check_rotations``.
         ``return_char_boxes=True``: every word is a tuple that ends with its character cells, an (n,4,2) float32 array
         of quads in the image's pixels for a text of n characters (a list of P arrays with ``top_paths = P > 1``):
@@ -1304,7 +1479,7 @@ class Recognizer:
         (``ValueError``).
         ``max_windows``: every box wider than the 200 x 31 crop at full height is read in up to that many overlapping
         windows and their steps stitched into one reading (``check_windows``; greedy decoding, boxes only)."""
-        lexicon, pattern = self._decoder(beam_width, top_paths, lexicon, language_model, pattern)
+        lexicon, pattern, hotwords = self._decoder(beam_width, top_paths, lexicon, language_model, pattern, hotwords)
         turns = check_rotations(rotations, rotation_vote)
         assert len(box_groups) == len(images), "You must provide the same number of box groups as images."
         from .detection import _as_device_images
@@ -1316,7 +1491,8 @@ class Recognizer:
                                     char_scores is not None)
         if polygons:
             return self._recognize_polygons(images, box_groups, entries, return_scores, turns, return_char_boxes,
-                                            beam_width, top_paths, lexicon, language_model, pattern, char_scores)
+                                            beam_width, top_paths, lexicon, language_model, pattern, char_scores,
+                                            hotwords)
         images_t = _as_device_images(images, self.device)
         counts = np.array([len(b) for b in box_groups], dtype=np.int64)
         if counts.sum() == 0:
@@ -1330,7 +1506,7 @@ class Recognizer:
         idx = torch.from_numpy(np.repeat(np.arange(len(counts), dtype=np.int32), counts)).to(self.device)
         gray = images_t if self.color else self.gray_device(images_t)
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
-                "pattern": pattern}
+                "pattern": pattern, "hotwords": hotwords}
         if return_char_boxes or char_scores is not None:
             cells = None
             if turns is not None:
@@ -1366,7 +1542,7 @@ class Recognizer:
         return [predictions[int(e - c):int(e)] for c, e in zip(counts, ends)]
 
     def _recognize_polygons(self, images, box_groups, entries, return_scores, turns, char_boxes, beam_width, top_paths,
-                            lexicon, language_model=None, pattern=None, char_scores=None):
+                            lexicon, language_model=None, pattern=None, char_scores=None, hotwords=None):
         """``recognize_from_boxes`` for box groups that hold polygons: 4-point entries are rectified as
         ``tools.rectify_boxes`` does and cut as boxes, the others along their polygon, all in one ``b2o_warp_polys``."""
         if turns is not None or char_boxes:
@@ -1384,7 +1560,7 @@ class Recognizer:
         crnn_in, _ = self.warp_polys_device(gray, torch.from_numpy(polys).to(self.device),
                                             torch.from_numpy(points).to(self.device), idx)
         beam = {"beam_width": beam_width, "top_paths": top_paths, "lexicon": lexicon, "language_model": language_model,
-                "pattern": pattern}
+                "pattern": pattern, "hotwords": hotwords}
         if char_scores is not None:
             labels, logp, *scores = self.predict_device(crnn_in, with_scores=True, char_scores=char_scores, **beam)
             predictions = self._host_words(labels, logp, top_paths, return_scores, None, scores)

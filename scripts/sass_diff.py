@@ -5,7 +5,11 @@ into common.cuh left a file's kernels unchanged (any object file; kernels in an 
     python scripts/sass_diff.py old_conv_tc.o keras-ocr_b200/csrc/conv_tc.o [suffix-to-append-to-old-template-args]
 
 e.g. after a new trailing template parameter `bool BOX16 = false` pass `ELb0` so that old `<64,64,3,true>` is compared
-with new `<64,64,3,true,false>`.
+with new `<64,64,3,true,false>`.  A kernel that became a template, or gained parameters, is matched by an argument
+OLD=NEW that renames it (substrings of the mangled names), e.g.
+
+    python scripts/sass_diff.py old_ctc_beam.o new_ctc_beam.o \
+        ctc_beam_lm_kernelEPKfiiiPKyS1_iiffPiPfS5_=ctc_beam_lm_kernelILb0EEEvPKfiiiPKyS2_iiffPiPfS6_NS_4TrieE
 """
 import collections
 import re
@@ -21,10 +25,11 @@ def functions(path):
         if m:
             full = re.sub(r"_GLOBAL__N__[0-9a-f]+_", "_GLOBAL__N__", m.group(1))   # anonymous namespace: per-build hash
             full = re.sub(r"(_GLOBAL__N__\d+_\w+?_cu)_[0-9a-f]{8}", r"\1_", full)  # and the hash of the file's contents
-            name = full[full.index("kernelI"):] if "kernelI" in full else full
+            # conv_tc_kernel instances are named by their template arguments; other templates keep their full name
+            name = full[full.index("kernelI"):] if "conv_tc_kernelI" in full else full
             table[name] = []
             continue
-        m = re.match(r"\s+/\*[0-9a-f]{4}\*/\s+(.*?);", line)
+        m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?);", line)
         if m and name:
             table[name].append(re.sub(r"\s+", " ", m.group(1)))
     return table
@@ -32,10 +37,14 @@ def functions(path):
 
 def main():
     old, new = functions(sys.argv[1]), functions(sys.argv[2])
-    suffix = sys.argv[3] if len(sys.argv) > 3 else ""
+    extra = sys.argv[3:]
+    renames = [tuple(a.split("=", 1)) for a in extra if "=" in a]
+    suffix = next((a for a in extra if "=" not in a), "")
     same = 0
     for name, body in old.items():
         other = name.replace("EEEv14CUtensorMap", suffix + "EEEv14CUtensorMap") if suffix else name
+        for a, b in renames:
+            other = other.replace(a, b)
         if body == new.get(other):
             same += 1
         else:
